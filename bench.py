@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""bench.py — 802.11a 54 Mbps RX PHY throughput (IQ in, bits out) on B200, BASELINE.json's metric.
+"""bench.py — 802.11a 54 Mbps RX PHY throughput (IQ in, bits out) on H100, BASELINE.json's metric.
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--frames F] [--impl reference]
 
@@ -37,7 +37,7 @@ def load_peaks():
         with open(os.path.join(ROOT, "MEASURED_PEAKS.json")) as f:
             return float(json.load(f)["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
     except Exception:
-        return 6650.0, "fallback (B200_PROFILING.md 6.65 TB/s)"
+        return 3350.0, "fallback (H100 SXM data sheet, 3.35 TB/s HBM3)"
 
 # ---- host description: what this process may really use ------------------------------------------------------------------------------------
 def effective_cpus():
@@ -82,7 +82,7 @@ def numa_bind(local):
         return f"not bound ({type(e).__name__})"
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled every 100 ms (B200_PROFILING.md recipe).  The process is started before the warm-up
+    """nvidia-smi clocks / throttle reasons sampled every 100 ms.  The process is started before the warm-up
     (nvidia-smi needs up to a second before its first line) and every line is stamped on arrival; stop() keeps the lines that arrived
     between mark() and stop(), i.e. under the load of the timed steps."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -231,6 +231,23 @@ def oracle_gate(eng, torch, iq_u, ps_u, U, res_dev, out_dev, ncores, rank):
     oracle_gate.rerun = int(len(idx))
     return U
 
+DUMP_ROWS = 4096
+
+def dump_outputs(d, res_dev, out_dev):
+    """What the last timed step returned, for comparing two builds output for output: every field of every slot's sb200_frame_result as
+    result_<field>.npy (float64, which holds each 32-bit value exactly) and the decoded bytes of a fixed, seeded sample of DUMP_ROWS slots
+    (float32), with the sampled slot indices.  About 29 MB at the default 65536 slots."""
+    import torch
+    from sora_b200 import api
+    os.makedirs(d, exist_ok=True)
+    F = out_dev.shape[0]
+    rows = np.sort(np.random.default_rng(0).choice(F, min(F, DUMP_ROWS), replace=False))
+    res = res_dev.cpu().numpy().view(api.RESULT_DTYPE).reshape(-1)
+    for name in api.RESULT_DTYPE.names:
+        np.save(os.path.join(d, f"result_{name}.npy"), res[name].astype(np.float64))
+    np.save(os.path.join(d, "psdu_sample.npy"), out_dev[torch.from_numpy(rows).to(out_dev.device)].cpu().numpy().astype(np.float32))
+    np.save(os.path.join(d, "psdu_sample_rows.npy"), rows.astype(np.float64))
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--gpus", type=int, default=1)
@@ -251,9 +268,11 @@ def main():
     ap.add_argument("--vl-hist-block", type=int, default=0, help="experiment: columns per history block of the lane kernel (6 | 8); 0 = library default")
     ap.add_argument("--vl-l2-hints", type=int, default=-1, help="experiment: L2 eviction hints of the lane kernel (bit 0 ring evict_last, bit 1 soft values evict_first); -1 = library default")
     ap.add_argument("--lane-min", type=int, default=-1, help="experiment: option viterbi_lane_min (smallest launch, in code blocks, the one-lane-per-code-block Viterbi takes); -1 = library default")
+    ap.add_argument("--lane-max", type=int, default=-1, help="experiment: option viterbi_lane_max (largest launch the one-lane-per-code-block Viterbi takes); -1 = library default")
     ap.add_argument("--no-e2e", action="store_true")
     ap.add_argument("--no-cpu", action="store_true")
     ap.add_argument("--no-mgpu", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write what the last timed step computed to DIR/*.npy (dump_outputs)")
     args = ap.parse_args()
     if args.warmup < 3: args.warmup = 3
     if args.impl == "reference":
@@ -286,12 +305,13 @@ def main():
     if args.vq_pad_smem: eng.set_option("vq_pad_smem", args.vq_pad_smem)
     if args.front_stage >= 0: eng.set_option("front_stage", args.front_stage)
     if args.lane_min >= 0: eng.set_option("viterbi_lane_min", args.lane_min)
+    if args.lane_max >= 0: eng.set_option("viterbi_lane_max", args.lane_max)
     if args.vl_pad_smem: eng.set_option("vl_pad_smem", args.vl_pad_smem)
     if args.vl_hist_block: eng.set_option("vl_hist_block", args.vl_hist_block)
     if args.vl_defer >= 0: eng.set_option("vl_defer_walk", args.vl_defer)
     if args.vl_l2_hints >= 0: eng.set_option("vl_l2_hints", args.vl_l2_hints)
     stream = torch.cuda.current_stream()
-    # ---- HBM-resident input: U unique slots tiled to F (distinct addresses: 2.6 GB at F=65536 >> 126 MB L2) ----
+    # ---- HBM-resident input: U unique slots tiled to F (distinct addresses: 2.6 GB at F=65536 >> 50 MB L2) ----
     iq_unique_dev = torch.from_numpy(iq_u.reshape(U, -1)).to(dev)
     reps = (F + U - 1) // U
     iq_dev = iq_unique_dev.repeat(reps, 1)[:F].contiguous()
@@ -318,6 +338,8 @@ def main():
     for _ in range(args.steps):
         step_dev()
     e1.record(stream); torch.cuda.synchronize()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res_dev, out_dev)
     if dist: dist.barrier()
     ms_total = e0.elapsed_time(e1)
     launches = eng.launches - l0
@@ -465,7 +487,7 @@ def main():
             "config": {"workload": WORKLOAD,
                        "slots_per_step_per_gpu": F, "unique_slots": U, "samples_per_slot": SLOT, "psdu_bytes": PSDU,
                        "parallelism": f"independent slots, {world} GPU(s), no data-path collective",
-                       "l2_policy": "input 2.6 GB per step >> 126 MB L2 (no flush needed)" if F * SLOT * 4 > 4e8 else "input smaller than L2: increase --frames",
+                       "l2_policy": "input 2.6 GB per step >> 50 MB L2 (no flush needed)" if F * SLOT * 4 > 4e8 else "input smaller than L2: increase --frames",
                        "oracle_gate": f"{gated} unique slots compared field by field and byte by byte with the CPU oracle before timing"
                                       + (f" ({oracle_gate.rerun} slots where the threaded oracle run disagreed were settled by a single-threaded oracle run)" if getattr(oracle_gate, "rerun", 0) else ""),
                        "numa": numa},

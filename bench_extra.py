@@ -172,7 +172,7 @@ def bench_11n(args):
                 "roofline": {"bound": "hbm", "achieved": alg / (ms * 1e-3) / 1e9, "peak": peaks(), "unit": "GB/s", "frac": alg / (ms * 1e-3) / 1e9 / peaks(), "note": "per GPU"},
                 "parity": "bytes and verdicts identical to the oracle on the %d unique slots" % U}
         if dist:
-            # "frames sharded across 2/4/8 B200" (BASELINE config #4): both antenna captures of all world*F slots sit on rank 0; NCCL scatters the two
+            # "frames sharded across 2/4/8 H100" (BASELINE config #4): both antenna captures of all world*F slots sit on rank 0; NCCL scatters the two
             # slabs per rank, every rank decodes its share, NCCL gathers bytes + verdicts on rank 0; everything inside the timed region
             P = 4; Fp = F // P; assert Fp * P == F
             s0 = torch.empty_like(d0); s1 = torch.empty_like(d1); v0 = s0.view(torch.int32); v1 = s1.view(torch.int32)   # NCCL has no 16-bit integer type

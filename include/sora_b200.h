@@ -1,4 +1,4 @@
-/* sora_b200 — C ABI of the Blackwell (sm_100a) 802.11 receive baseband.
+/* sora_b200 — C ABI of the Hopper (sm_90a) 802.11 receive baseband.
  *
  * This is the drop-in boundary for Sora's dot11 RX hot path.  Every entry point states which reference
  * interface it stands behind (paths relative to the reference tree):
@@ -100,9 +100,11 @@ int sb200_last_kernel_times(sb200_handle* h, float* ms4);
  * "host_decimate_mix" (default 1): with host_decimate on, 1 = per chunk the call either gathers on the host threads or — when the copies
  *   already queued would run out before a gather could finish — sends the chunk as it is, so that the link and the host cores are both kept
  *   busy (link rate and gather cost are estimated from the call's own events); 0 = every chunk is gathered; 2 = alternate (tests).
- * "viterbi_lane_min": launches of at least this many code blocks are decoded by the one-lane-per-code-block Viterbi kernel (32 code blocks per
- *   warp, history ring in global memory: the fewest instructions, but it needs a large batch to fill the machine), smaller ones by the
- *   four-lanes-per-code-block kernel (ring in shared memory).  Results are identical.  0 = always, 0xFFFFFFFF = never.
+ * "viterbi_lane_min" (default 16384), "viterbi_lane_max" (default 49152): launches of lane_min .. lane_max code blocks are decoded by the
+ *   one-lane-per-code-block Viterbi kernel (32 code blocks per warp, history ring in global memory: the fewest instructions, but it needs a
+ *   large batch to fill the machine, and its ring traffic costs more than it saves on the largest ones), the others by the
+ *   four-lanes-per-code-block kernel (ring in shared memory).  Results are identical.  lane_min 0 and lane_max 0xFFFFFFFF = always,
+ *   lane_min 0xFFFFFFFF = never.
  * Slot tables (frame_off/frame_len) are bounds-checked against iq_total_samples on EVERY call, host- or device-resident (a device table costs one
  * small reduction kernel and an 8-byte read-back).  "slot_table_immutable" (default 0): set to 1 to promise that a device-resident table is not
  * rewritten while the same pointers, count and total are passed again; only then is the check (and the host copy the chunked path needs) cached. */

@@ -1,4 +1,4 @@
-// sora_b200 — anti-alias FIR decimator 2:1 for COMPLEX16 captures (sm_100a).
+// sora_b200 — anti-alias FIR decimator 2:1 for COMPLEX16 captures (sm_90a).
 //
 // BASELINE.json's north_star lists "FIR decimation / channel-select" as the first stage of the chain.  The reference's 802.11a graph has no
 // filter there: TDownSample2 (Brick11/src/samples.hpp:27-49) just keeps every other sample, which aliases whatever sits between 10 and

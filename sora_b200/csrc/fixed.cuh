@@ -1,4 +1,4 @@
-// sora_b200 — lane-exact fixed-point primitives for sm_100a device code.
+// sora_b200 — lane-exact fixed-point primitives for sm_90a device code.
 //
 // Scalar (one complex int16 sample per call) definitions of the arithmetic the reference performs with
 // SSE vectors.  Each function cites the reference primitive whose per-lane result it reproduces

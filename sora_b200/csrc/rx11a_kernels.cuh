@@ -1,4 +1,4 @@
-// sora_b200 — 802.11a receive kernels (sm_100a).
+// sora_b200 — 802.11a receive kernels (sm_90a).
 //
 //   k_sync11a    one thread per capture slot: 2:1 decimation, DC removal/estimation and the STS carrier-sense
 //                state machine, up to the vector where the reference switches to the demod branch.
@@ -238,13 +238,13 @@ __device__ __forceinline__ int data_index(int bin) {   // demapper11a.hpp:22-36 
 
 #define SB_FRONT_WARPS 4
 #ifndef SB_FRONT_MINB
-#define SB_FRONT_MINB 6           // resident CTAs per SM the register allocation aims at
+#define SB_FRONT_MINB 5           // resident CTAs per SM the register allocation aims at: 6 spills on sm_90a and measured 5 % slower (tools/front_sweep.sh)
 #endif
 // Two OFDM symbols are transformed at once: lanes 0-15 run the three radix stages of symbol A, lanes 16-31 those of
 // symbol B (16 butterflies per stage = 16 lanes, so every lane is busy); the first stage consumes the freq-compensated
 // time samples straight from registers.  Only the part behind the FFT (phase compensation from the pilot recurrence)
 // is serial across symbols, and there every lane owns two subcarriers.
-// STAGE: how the time samples of the DATA symbols reach the FFT (A/B of the staging experiment, profiles/README.md):
+// STAGE: how the time samples of the DATA symbols reach the FFT (A/B of the staging experiment, DESIGN.md §4):
 //   0  loaded straight into registers right before the transform (round 1);
 //   1  the next symbol pair's samples are loaded into registers while the current pair is processed (register double buffer);
 //   2  one lane starts a 1-D bulk asynchronous copy (cp.async.bulk, the TMA unit; SASS UBLKCP) of the next pair's span into a shared-memory

@@ -1,4 +1,4 @@
-// sora_b200 — 802.11b (DSSS / CCK) receive kernel for sm_100a.
+// sora_b200 — 802.11b (DSSS / CCK) receive kernel for sm_90a.
 //
 // One thread decodes one capture slot (44 Msps COMPLEX16, 4 samples per chip) from a fresh context up to its first
 // frame event, like MAC11b_Receive drives CreateDemodGraph (kernel/bb/demod11/fb11b_demod.cpp:26-79,

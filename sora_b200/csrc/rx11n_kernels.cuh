@@ -1,4 +1,4 @@
-// sora_b200 — 802.11n 2x2 (HT mixed format, 20 MHz, 2 spatial streams, MCS 8..10) receive kernels (sm_100a).
+// sora_b200 — 802.11n 2x2 (HT mixed format, 20 MHz, 2 spatial streams, MCS 8..10) receive kernels (sm_90a).
 //
 //   k_sync11n    one thread per slot (a slot = the same sample range of both antenna captures): 2:1 decimation and the
 //                joint two-antenna carrier sense — 32-lag autocorrelation^2 against energy^2 in int64, energy step against
@@ -329,7 +329,7 @@ __device__ __noinline__ void demap_qam11n(uint8_t* sb, const uint16_t* __restric
 }
 
 #ifndef SB_FRONT11N_MINB
-#define SB_FRONT11N_MINB 6         // resident CTAs per SM the register allocation aims at (profiles/README.md, front-end sweep)
+#define SB_FRONT11N_MINB 6         // resident CTAs per SM the register allocation aims at (tools/front_sweep.sh: 4 and 5 are no faster)
 #endif
 __global__ void __launch_bounds__(32 * SB_FRONT11N_WARPS, SB_FRONT11N_MINB) k_front11n(const uint32_t* __restrict__ iq0, const uint32_t* __restrict__ iq1,
         const uint64_t* __restrict__ off, const uint32_t* __restrict__ len, uint32_t nframes, DevTables T, DevTables11n N, const uint16_t* __restrict__ inv_deint48,

@@ -146,7 +146,8 @@ struct DecimPool {
     ~DecimPool() { shutdown(); }
 };
 
-#define SB200_LANE_MIN_DEFAULT 16384u                 // measured (profiles/r2j_vit_crossover.jsonl): the lane kernel wins from 16 384 code blocks per launch on (0.85x at 16 384, 0.70x at 65 536)
+#define SB200_LANE_MIN_DEFAULT 16384u                 // the lane kernel for launches of 16 384 .. 49 152 code blocks, the four-lane kernel outside
+#define SB200_LANE_MAX_DEFAULT 49152u                 // (tools/vit_crossover.py on an H100 SXM at 400 W: lane/four-lane time 1.46 at 8 192, 0.96 at 16 384, 0.85-0.93 up to 49 152, 1.03 at 65 536)
 
 struct sb200_handle {
     int device = 0;
@@ -193,8 +194,9 @@ struct sb200_handle {
     uint32_t vl_pad_smem = 0;                          // experiment knob: the same for the lane kernel (fewer resident warps = a smaller history-ring working set in L2)
     uint32_t vq_pad_smem = 0;                          // experiment knob: extra dynamic shared memory per Viterbi CTA (lowers occupancy)
     // viterbi_k7_lane.cuh (one lane per code block, 32 per warp) needs a large batch to fill the machine: it decodes launches of at least
-    // lane_min code blocks, the four-lanes-per-code-block kernel the smaller ones.  Option "viterbi_lane_min"; SB200_VITERBI=v8 forces it (0), v3 forbids it.
-    uint32_t lane_min = SB200_LANE_MIN_DEFAULT;
+    // lane_min and at most lane_max code blocks, the four-lanes-per-code-block kernel the others.  Options "viterbi_lane_min" / "viterbi_lane_max";
+    // SB200_VITERBI=v8 forces it (0 .. 0xFFFFFFFF), v3 forbids it.
+    uint32_t lane_min = SB200_LANE_MIN_DEFAULT, lane_max = SB200_LANE_MAX_DEFAULT;
     const char* last_vit = "";                         // name of the Viterbi kernel the last launch used (sb200_last_viterbi_kernel)
     DevBuf vring;
     bool use_pair = false;                             // SB200_VITERBI=v4: two lanes per code block, 16 code blocks per warp (A/B against four lanes)
@@ -260,7 +262,7 @@ extern "C" int sb200_create(int device, const sb200_cfg* cfg, sb200_handle** out
     if (!h) return SB200_E_NOMEM;
     h->device = device;
     if (cfg && cfg->cca_pwr_threshold) h->cca_thr = cfg->cca_pwr_threshold;
-    { const char* e = getenv("SB200_VITERBI"); h->use_v2 = e && e[0] == 'v' && e[1] == '2'; h->use_pair = e && e[0] == 'v' && e[1] == '4'; if (e && e[0] == 'v' && e[1] == '8') h->lane_min = 0; else if (e && e[0] == 'v') h->lane_min = 0xFFFFFFFFu; }
+    { const char* e = getenv("SB200_VITERBI"); h->use_v2 = e && e[0] == 'v' && e[1] == '2'; h->use_pair = e && e[0] == 'v' && e[1] == '4'; if (e && e[0] == 'v' && e[1] == '8') { h->lane_min = 0; h->lane_max = 0xFFFFFFFFu; } else if (e && e[0] == 'v') h->lane_min = 0xFFFFFFFFu; }
     if (cudaSetDevice(device) != cudaSuccess) { delete h; return SB200_E_CUDA; }
     int rc = upload_tables(h);
     if (rc == SB200_OK && (cudaEventCreate(&h->ev0) != cudaSuccess || cudaEventCreate(&h->ev1) != cudaSuccess)) rc = SB200_E_CUDA;
@@ -363,11 +365,12 @@ static int slot_table(sb200_handle* h, const uint64_t* frame_off, const uint32_t
     return SB200_OK;
 }
 
-// One launch of the Viterbi for code rate CR: the lane kernel (viterbi_k7_lane.cuh) for launches of at least lane_min code blocks, in the
+// One launch of the Viterbi for code rate CR: the lane kernel (viterbi_k7_lane.cuh) for launches of lane_min .. lane_max code blocks, in the
 // rendering the options select (8-column history blocks with the deferred walk unless told otherwise); below that the four-lanes-per-code-
 // block kernel (SB200_VITERBI=v4: two lanes, for A/B).  vring_need() sizes the lane kernel's history rings for n code blocks first.
+static bool use_lane(const sb200_handle* h, uint32_t n) { return n >= h->lane_min && n <= h->lane_max; }
 static cudaError_t vring_need(sb200_handle* h, uint32_t n) {
-    if (n >= h->lane_min) return h->vring.need((size_t)((n + SB_VL_FR - 1) / SB_VL_FR) * SB_VL_NB8D * SB_VL_ENTRY * 16);   // the largest ring of the lane kernel's renderings
+    if (use_lane(h, n)) return h->vring.need((size_t)((n + SB_VL_FR - 1) / SB_VL_FR) * SB_VL_NB8D * SB_VL_ENTRY * 16);   // the largest ring of the lane kernel's renderings
     return cudaSuccess;                                // the four- / two-lane kernels keep their ring in shared memory
 }
 template <int CR>
@@ -375,10 +378,10 @@ static void launch_viterbi_re(sb200_handle* h, uint32_t n, cudaStream_t s, const
                               const FrameInfo* info, const VitJob& job, uint8_t* out, uint64_t out_stride, uint32_t raw_off, uint32_t* nraw) {
     const unsigned g = (n + SB_VR_FR - 1) / SB_VR_FR, gp = (n + 15) / 16;
     uint4* const ring = (uint4*)h->vring.p;             // the lane kernel's history rings
-    h->last_vit = n >= h->lane_min ? "k_viterbi_lane" : "k_viterbi_re";
-    if (n >= h->lane_min && h->vl_hb == 8 && h->vl_defer) k_viterbi_lane<CR, 8, true><<<(n + SB_VL_FR - 1) / SB_VL_FR, 32, h->vl_pad_smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, ring, h->vl_flags);
-    else if (n >= h->lane_min && h->vl_hb == 8) k_viterbi_lane<CR, 8><<<(n + SB_VL_FR - 1) / SB_VL_FR, 32, h->vl_pad_smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, ring, h->vl_flags);
-    else if (n >= h->lane_min)       k_viterbi_lane<CR, 6><<<(n + SB_VL_FR - 1) / SB_VL_FR, 32, h->vl_pad_smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, ring, h->vl_flags);
+    h->last_vit = use_lane(h, n) ? "k_viterbi_lane" : "k_viterbi_re";
+    if (use_lane(h, n) && h->vl_hb == 8 && h->vl_defer) k_viterbi_lane<CR, 8, true><<<(n + SB_VL_FR - 1) / SB_VL_FR, 32, h->vl_pad_smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, ring, h->vl_flags);
+    else if (use_lane(h, n) && h->vl_hb == 8) k_viterbi_lane<CR, 8><<<(n + SB_VL_FR - 1) / SB_VL_FR, 32, h->vl_pad_smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, ring, h->vl_flags);
+    else if (use_lane(h, n))         k_viterbi_lane<CR, 6><<<(n + SB_VL_FR - 1) / SB_VL_FR, 32, h->vl_pad_smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, ring, h->vl_flags);
     else if (h->use_pair)            k_viterbi_re<CR, 1><<<gp, 32, 0, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw);
     else                             k_viterbi_re<CR, 2><<<g, 32, 0, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw);
 }
@@ -453,7 +456,7 @@ static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
     CK(h->status.need(nframes * 4ull)); CK(h->crc.need(nframes * 4ull)); CK(h->res.need(nframes * sizeof(sb200_frame_result)));
     CK(h->vlist.need(nframes * 12ull));
     const bool tapping = taps.freq_coeffs || taps.fft_out || soft_host || dc_init;
-    // device-resident IQ gains nothing from chunking (a chunk's Viterbi grid no longer fills 148 SMs x 5 CTAs); host IQ does:
+    // device-resident IQ gains nothing from chunking (a chunk's Viterbi grid no longer fills 132 SMs x 5 CTAs); host IQ does:
     // the PCIe copy of chunk k+1 hides behind the kernels of chunk k.  chunk_frames_device lets a caller force it anyway.
     const uint32_t want = (no_chunk || rate20) ? 0u : iq_dev ? h->chunk_frames_device : h->chunk_frames;
     const uint32_t chunk = (want == 0 || tapping || nframes <= want || (!iq_dev && !tab_on_host)) ? nframes : want;
@@ -1445,6 +1448,7 @@ extern "C" int sb200_set_option(sb200_handle* h, const char* name, uint64_t valu
     if (!strcmp(name, "vl_l2_hints")) { h->vl_flags = (uint32_t)value & 3u; return SB200_OK; }   // bit 0 ring traffic evict_last, bit 1 soft values evict_first
     if (!strcmp(name, "vl_pad_smem")) { if (value > 48 * 1024) return h->fail(SB200_E_INVALID, "vl_pad_smem <= 49152"); h->vl_pad_smem = (uint32_t)value; return SB200_OK; }
     if (!strcmp(name, "viterbi_lane_min")) { h->lane_min = value > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)value; return SB200_OK; }
+    if (!strcmp(name, "viterbi_lane_max")) { h->lane_max = value > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)value; return SB200_OK; }
     if (!strcmp(name, "host_stage_wc")) { h->hstage_wc = value != 0; return SB200_OK; }
     if (!strcmp(name, "host_decimate_mix")) { if (value > 2) return h->fail(SB200_E_INVALID, "host_decimate_mix: 0, 1 or 2"); h->host_mix = (uint32_t)value; h->gather_ms_per_sample = 0.0; return SB200_OK; }
     if (!strcmp(name, "slot_table_immutable")) { h->tab_immutable = value != 0; h->tab_off = nullptr; return SB200_OK; }

@@ -1,4 +1,4 @@
-// sora_b200 — 802.11a transmit kernels (sm_100a): SURVEY.md §8(f) rank 2, the reference's brick modulator on the device.
+// sora_b200 — 802.11a transmit kernels (sm_90a): SURVEY.md §8(f) rank 2, the reference's brick modulator on the device.
 //
 //   k_tx11a_preamble   one warp, once per handle: the 640-sample short/long training waveform exactly as TTS11aSrc builds it
 //                      (Brick11/src/preamble11a.hpp:22-104: two fixed-point IFFT<128>, >> 4, periodic extension, GI2, window).

@@ -1,4 +1,4 @@
-// 802.11b transmit on sm_100a: the brick modulator graph of kernel/bb/demod11/fb11bmod_config.hpp:19-45
+// 802.11b transmit on sm_90a: the brick modulator graph of kernel/bb/demod11/fb11bmod_config.hpp:19-45
 //   TBB11bSrc -> TSc741 -> TBB11bMRSelect -> {TBB11bDBPSKSpread, TBB11bDQPSKSpread, TCCK5Encode, TCCK11Encode}
 //             -> TQuickPulseShaper -> TPackSample16to8 -> TModSink
 // split where the data dependence allows it:

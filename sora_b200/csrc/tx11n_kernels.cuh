@@ -1,4 +1,4 @@
-// 802.11n two-stream HT-mixed-format transmit on sm_100a: the modulator graphs of kernel/bb/demod11/fb11nmod_config.hpp:74-171
+// 802.11n two-stream HT-mixed-format transmit on sm_90a: the modulator graphs of kernel/bb/demod11/fb11nmod_config.hpp:74-171
 // (CreatePreambleGraph11n, CreateSigGraph11n, CreateModGraph11n) driven like kernel/bb/demod11/fb11n_mod.cpp:44-70.
 //   k_tx11n   one warp per (OFDM symbol, stream): symbols 0..2 are L-SIG / HT-SIG 1 / HT-SIG 2 (one spectrum, stream 2 delayed by
 //             TCSD<2>), symbols 3.. are DATA.  As in k_tx11a nothing is carried from symbol to symbol: the scrambler is read as a

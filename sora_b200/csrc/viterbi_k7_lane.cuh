@@ -1,10 +1,10 @@
-// sora_b200 — batched K=7 (133,171) soft Viterbi, "lane" kernel for sm_100a: ONE LANE PER CODE BLOCK, six-column history blocks.
+// sora_b200 — batched K=7 (133,171) soft Viterbi, "lane" kernel for sm_90a: ONE LANE PER CODE BLOCK, six-column history blocks.
 //
 // Arithmetic contract: the same as viterbi_k7_re.cuh (bit-exact with kernel/bb/Brick11/src/viterbicore.h:269-556 driven like
 // kernel/bb/Brick11/src/viterbi.hpp:104-237); the add-compare-select is that file's vr_step — one fused VIADDMNMX.U16x2 and one
 // VIADD.16x2 per register and trellis step, the survivor history riding in the low byte of every 16-bit metric.
 //
-// What is different, and why (profiles/r2c_viterbi_v5_ncu.txt, r2c_viterbi_v7_ncu.txt, r2b_final_viterbi_ncu.txt):
+// What is different, and why (DESIGN.md §4):
 //   * A lane owns all 64 states of a code block (32 registers); a warp decodes 32 code blocks.  No lane ever needs another lane's
 //     metrics: no shuffle, no quad mask, no per-lane selector — every PRMT selector and pairing distance is a compile-time constant.
 //     The per-warp overhead of a step (branch-metric construction, fetch, loop) is spread over 32 code blocks instead of 8:

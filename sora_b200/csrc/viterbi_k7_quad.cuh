@@ -1,10 +1,10 @@
-// sora_b200 — batched K=7 (133,171) soft Viterbi, v2 "quad" mapping for sm_100a.
+// sora_b200 — batched K=7 (133,171) soft Viterbi, v2 "quad" mapping for sm_90a.
 //
 // Arithmetic contract: bit-exact with kernel/bb/Brick11/src/viterbicore.h:269-556 driven like
 // kernel/bb/Brick11/src/viterbi.hpp:104-237), different machine mapping:
 //
 //   * 4 lanes decode one code block; each lane keeps 16 of the 64 path metrics in 8 registers, two per register as
-//     16-bit halves, so compare-select is Blackwell's native 16x2 SIMD (VIMNMX.U16x2).
+//     16-bit halves, so compare-select is the native 16x2 SIMD of sm_90 (VIMNMX.U16x2).
 //   * Metrics sit in the HIGH byte of each half: the reference's uint8 wrap is the natural carry-out of the half (a plain
 //     32-bit IMAD.IADD on the FMA pipe is a 16x2 add; the carry of the low half only lands in a dead byte), and the
 //     survivor mark costs one LOP3 per *input* register (even role: & 0xFE00FE00, odd role: (& 0xFF00FF00) | 0x01000100).
@@ -49,7 +49,7 @@ struct VqLane {
 // one trellis step at compile-time phase T.  Cbase byte (cA<<1|cB) = metric of the even candidate for a predecessor of
 // that class; the complement class (3 - index) is the odd candidate's.
 // Two renderings of the same arithmetic; which one is faster depends on how often the per-group bookkeeping runs, i.e. on the
-// code rate (measured, profiles/README.md): style A keeps the ALU pipe lighter (R = 1/2), style B issues fewer instructions (R = 2/3, 3/4).
+// code rate: style A keeps the ALU pipe lighter (R = 1/2), style B issues fewer instructions (R = 2/3, 3/4).
 //   style A: the survivor marks are taken out of the fresh metrics once per step (LOP3 + IMAD-side subtract / shifted accumulate), the
 //            even / odd roles of the next step are plain adds; address = lane | half | reg.
 //   style B: the role masks of the next step replace the stale marks (one LOP3 per input register), the 16 marks of a lane are gathered

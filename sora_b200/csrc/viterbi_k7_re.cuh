@@ -1,4 +1,4 @@
-// sora_b200 — batched K=7 (133,171) soft Viterbi, v3 "history-carrying" kernel for sm_100a.
+// sora_b200 — batched K=7 (133,171) soft Viterbi, v3 "history-carrying" kernel for sm_90a.
 //
 // Arithmetic contract (bit-exact with kernel/bb/Brick11/src/viterbicore.h:269-556 driven like
 // kernel/bb/Brick11/src/viterbi.hpp:104-237): path metrics are the reference's uint8 values, whose LSB is the survivor mark and whose upper
@@ -25,8 +25,8 @@
 //     traceback trigger run as one branch-free instruction stream, everything else goes through a 6-step path with the event checks.
 //   * The kernel emits the decoded bytes (SERVICE + PSDU, still scrambled).  Descrambler, CRC-32 and the verdict (scramble.hpp:269-355,
 //     PHY_11a.hpp:609-702) run in k_sink11a, one thread per frame, after it.
-// Measured instruction rates that shaped this (tools/microbench/pipes.cu on B200): VIADDMNMX.U16x2 + IMAD/VIADD issue together at ~1.0 per
-// cycle per sub-partition; VIMNMX + two adds (the v2 ACS) at 0.75; LOP3 and PRMT at 0.5.
+// Instruction rates that shape this (tools/microbench/pipes.cu on an H100 SXM, 400 W limit): VIADDMNMX.U16x2 + IMAD/VIADD issue together at
+// ~0.9 per cycle per sub-partition; VIMNMX + two adds (the v2 ACS) at 0.74; LOP3 and PRMT at 0.5.
 #pragma once
 #include "viterbi_k7_quad.cuh"
 #include <type_traits>

@@ -28,3 +28,13 @@ def dummy_vectors():
 
 def fsample6_psdu():
     return np.fromfile(os.path.join(GOLD, "fsample-6.psdu.bin"), np.uint8)
+
+def reference_tables():
+    """The reference's lookup tables and constants as parsed out of its headers, and SHA-256 digests of what its compiled 802.11b
+    transmit filter returns for the suites' inputs (make_reference_tables.py)."""
+    return dict(np.load(os.path.join(GOLD, "reference_tables.npz")))
+
+def digest(a):
+    """SHA-256 of an integer table as little-endian int64, the form the large tables of reference_tables.npz are kept in."""
+    import hashlib
+    return np.frombuffer(hashlib.sha256(np.asarray(a, "<i8").tobytes()).digest(), np.uint8)

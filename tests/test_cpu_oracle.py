@@ -8,7 +8,6 @@ from sora_b200.dumpfile import load_dump, write_dump
 
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 GOLD = os.path.join(ROOT, "tests", "golden")
-REF = "/root/reference"
 
 def _fs6():
     iq = load_dump(os.path.join(GOLD, "fsample-6.dmp"))
@@ -24,8 +23,8 @@ def test_fsample6_golden_frame():
     assert oracle_py.crc32(psdu[:-4]) == int(r["crc32"]) == int.from_bytes(psdu[-4:].tobytes(), "little")
     gold = np.fromfile(os.path.join(GOLD, "fsample-6.psdu.bin"), np.uint8)
     assert (psdu == gold).all()
-    if os.path.exists(os.path.join(REF, "kernel/test-data/fsample-6.dmp")):
-        assert open(os.path.join(REF, "kernel/test-data/fsample-6.dmp"), "rb").read() == open(os.path.join(GOLD, "fsample-6.dmp"), "rb").read()
+    import hashlib, golden_vectors as gv                   # the vector is the reference's capture, byte for byte
+    assert hashlib.sha256(open(os.path.join(GOLD, "fsample-6.dmp"), "rb").read()).digest() == gv.reference_tables()["fsample6_sha256"].tobytes()
 
 def _ofdm_bin():
     raw = np.fromfile(os.path.join(GOLD, "ofdm.bin"), dtype=np.int8).reshape(-1, 2)
@@ -142,37 +141,32 @@ def test_signal_field_known_answer():
     w = oracle_py.lib().sbo_viterbi_signal(soft.ctypes.data_as(ctypes.c_void_p))
     assert (w & 0xF) == 0xB and ((w >> 5) & 0xFFF) == 1392
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree only exists in the build container")
 def test_tables_vs_reference_headers():
     sys.path.insert(0, os.path.join(ROOT, "tools"))
-    import refcheck as rc
+    import refcheck as rc, golden_vectors as gv
+    R = gv.reference_tables()
     for N in (16, 64):
         for M in (1, 2, 3):
-            assert (rc.ref_twiddle(N, M)[: N // 4] == rc.gen_twiddle(N, M)).all()
-    assert (rc.ref_bitrev(64) == np.array([int(f"{i:06b}"[::-1], 2) for i in range(64)])).all()
-    s, c, a = rc.ref_trig()
-    assert (s == rc.gen_sin()).all() and (c == rc.gen_cos()).all() and (a == rc.gen_atan2()).all()
-    ra, rb = rc.ref_vit(); ga, gb = rc.gen_vit()
-    assert (ra == ga).all() and (rb == gb).all()
+            assert (R[f"twiddle{N}_{M}"] == rc.gen_twiddle(N, M)).all()
+    assert (R["bitrev64"] == np.array([int(f"{i:06b}"[::-1], 2) for i in range(64)])).all()
+    for n, gen in (("usin", rc.gen_sin), ("ucos", rc.gen_cos), ("uatan2", rc.gen_atan2)):
+        assert (gv.digest(gen()) == R[n + "_sha256"]).all(), n
+    ga, gb = rc.gen_vit()
+    assert (R["vit_ma"] == ga).all() and (R["vit_mb"] == gb).all()
     for cls, n, b in (("BPSK", 48, 1), ("QPSK", 96, 2), ("QAM16", 192, 4), ("QAM64", 288, 6)):
-        assert (rc.ref_deinterleave(cls) == rc.gen_deinterleave(n, b)).all()
+        assert (R[f"deint11a_{cls}"] == rc.gen_deinterleave(n, b)).all()
     # LTS signs and pilot polarity used by oracle/rx11a.cpp and csrc/tables.cuh
-    t = rc._read("kernel/bb/Brick11/src/channel_11a.hpp")
-    lts = np.array(rc.parse_array(t, "LTS_Sequence_11a"))
     exp = np.array([1 if (-26 <= (i if i < 32 else i - 64) <= 26 and synth._LTS[(i if i < 32 else i - 64) + 26] > 0) else 0 for i in range(64)])
-    assert (lts == exp).all()
-    t = rc._read("kernel/bb/Brick11/src/pilot.hpp")
-    pil = np.array(rc.parse_array(t, "PilotSgn"))
+    assert (R["lts_11a"] == exp).all()
     pol = synth._PILOT_POL
     exp = np.array([0 if pol[(i + 1) % 127] > 0 else -1 for i in range(127)] + [0])
-    assert (pil == exp).all()
+    assert (R["pilot_sgn_11a"] == exp).all()
     # demap tables shipped as data
-    luts = rc.ref_demap_luts()
     tb = ctypes.POINTER(ctypes.c_uint8)
     a_, b_, d_ = tb(), tb(), tb()
     oracle_py.lib().sbo_tables(ctypes.byref(a_), ctypes.byref(b_), ctypes.byref(d_))
     got = np.ctypeslib.as_array(d_, shape=(1024,))
-    assert (got == np.concatenate([luts["m_bpsk_lut"], luts["m_qam16_lut2"], luts["m_qam64_lut2"], luts["m_qam64_lut3"]])).all()
+    assert (got == np.concatenate([R["demap_m_bpsk_lut"], R["demap_m_qam16_lut2"], R["demap_m_qam64_lut2"], R["demap_m_qam64_lut3"]])).all()
 
 def test_abi_exports_every_declared_symbol():
     hdr = open(os.path.join(ROOT, "include", "sora_b200.h")).read()

@@ -3,25 +3,19 @@ import os, sys, numpy as np, pytest
 import oracle_py
 from sora_b200 import synth
 
-REF = "/root/reference"
-sys.path.insert(0, os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "tools"))
-
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree only exists in the build container")
 def test_tables_vs_reference_headers_11n():
-    import refcheck as rc
+    import golden_vectors as gv
+    R = gv.reference_tables()
     T = oracle_py.tables11n()
-    d = rc.ref_demap_11n()
-    assert (d["bpsk"] == T["demap"]).all() and (d["qpsk"] == T["demap"]).all()
-    assert (rc.ref_crc8() == T["crc8"]).all()
+    assert (R["demap11n_bpsk"] == T["demap"]).all() and (R["demap11n_qpsk"] == T["demap"]).all()
+    assert (R["crc8"] == T["crc8"]).all()
     for q, name in enumerate(("BPSK", "QPSK")):
         for s in range(2):
-            ref = rc.ref_deinterleave_11n(f"{name}_S{s}")
+            ref = R[f"deint11n_{name}_S{s}"]
             assert (ref == T["deint"][q, s, :len(ref)]).all() and len(ref) == 52 * (q + 1), (name, s)
             assert (synth.ht_interleave_map(q + 1, s) == ref).all()        # modulator and receiver agree on the permutation
-    lp, hp = rc.ref_ltf_masks()
-    assert (lp == T["lltf_sign"].astype(bool)).all() and (hp == T["htltf_sign"].astype(bool)).all()
-    nd = rc.ref_ht_ndbps()
-    assert {m: nd[m][1] for m in (8, 9, 10)} == {m: synth.HT_MCS[m][2] for m in (8, 9, 10)}
+    assert (R["lltf_plus"] == T["lltf_sign"].astype(bool)).all() and (R["htltf_plus"] == T["htltf_sign"].astype(bool)).all()
+    assert {m: int(R["ht_ndbps"][m][1]) for m in (8, 9, 10)} == {m: synth.HT_MCS[m][2] for m in (8, 9, 10)}
 
 def test_dsp_math_tables_closed_form():
     T = oracle_py.tables11n()

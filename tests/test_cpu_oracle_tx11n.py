@@ -5,8 +5,6 @@ the receive restatement bit for bit (L-SIG / HT-SIG fields, CRC-8, HT interleave
 import os, re, zlib, numpy as np, pytest
 import oracle_py
 
-REF = "/root/reference"
-
 def _rx(o0, o1, chan=((1, 0), (0, 1)), noise=0.0, seed=0, lead=400, trail=300, cfo_hz=0.0):
     a = o0.astype(np.float64); b = o1.astype(np.float64)
     rot = np.exp(2j * np.pi * cfo_hz * np.arange(len(a)) / 40e6)
@@ -66,17 +64,14 @@ def test_second_stream_is_a_cyclically_delayed_copy_in_the_legacy_part():
     assert (o0[h:h + 160] == -o0[h + 160:h + 320]).all() and (o1[h:h + 160] == o1[h + 160:h + 320]).all()
     assert (np.roll(o0[h + 32:h + 160], 16, axis=0) == o1[h + 32:h + 160]).all()
 
-@pytest.mark.skipif(not os.path.isdir(REF), reason="reference tree only exists in the build container")
 def test_preamble_and_pilot_tables_vs_reference():
-    def table(path, name):
-        s = open(os.path.join(REF, "kernel/bb/Brick11/src", path)).read(); i = s.index(name + "[] ="); j = s.index("};", i)
-        return np.array(re.findall(r"\{\s*(-?\d+)\s*,\s*(-?\d+)\s*\}", s[i:j]), dtype=np.int16)
+    import golden_vectors as gv
+    R = gv.reference_tables()
     a, b, c, d = oracle_py.tx11n_preamble_tables()
-    assert (a == table("_b_lstf.h", "L_STF::_stf")).all() and (b == table("_b_lltf.h", "L_LTF::_ltf")).all()
-    assert (c == table("_b_htstf.h", "HT_STF::_stf")).all() and (d == table("_b_htltf.h", "HT_LTF::_ltf")).all()
+    assert a.shape == R["l_stf"].shape and (a == R["l_stf"]).all() and b.shape == R["l_ltf"].shape and (b == R["l_ltf"]).all()
+    assert c.shape == R["ht_stf"].shape and (c == R["ht_stf"]).all() and d.shape == R["ht_ltf"].shape and (d == R["ht_ltf"]).all()
     # the 127-entry pilot polarity table of the HT pilot generator is the 802.11a one (entry i = p(i+1)): x^7 + x^4 + 1 from all ones
-    s = open(os.path.join(REF, "kernel/bb/Brick11/src/_b_dot11_pilot.h")).read(); i = s.index("dot11_ofdm_pilot::_pilot_sign[pilot_size] ="); j = s.index("};", i)
-    sign = np.array([int(v) for v in re.findall(r"-?\d+", s[s.index("{", i):j])])
+    sign = R["pilot_sign_11n"]
     st = 0x7F; seq = []
     for _ in range(127): o = ((st >> 6) ^ (st >> 3)) & 1; st = ((st << 1) | o) & 0x7F; seq.append(1 - 2 * o)
     assert len(sign) == 127 and (sign == np.array([seq[(k + 1) % 127] for k in range(127)])).all()

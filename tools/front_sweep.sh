@@ -2,8 +2,8 @@
 # register/occupancy sweep of the two OFDM front-end kernels on the GPU box: rebuild with -DSB_FRONT_MINB / -DSB_FRONT11N_MINB
 # (resident CTAs per SM that __launch_bounds__ asks for) and print the per-kernel times
 cd "$(dirname "$0")/.."
-F="-O3 -std=c++17 -lineinfo -gencode arch=compute_100a,code=sm_100a -Xcompiler -fPIC"
-for b in ${A_LIST:-6 7}; do
+F="-O3 -std=c++17 -lineinfo -gencode arch=compute_90a,code=sm_90a -Xcompiler -fPIC"
+for b in ${A_LIST:-4 5 6}; do
   touch sora_b200/csrc/sb200.cu; make -C sora_b200/csrc NVFLAGS="$F -DSB_FRONT_MINB=$b" >/dev/null 2>&1
   echo "11a MINB=$b"; python bench.py --steps 3 --warmup 2 2>/dev/null | python -c "import sys,json; d=json.loads(sys.stdin.read().strip().splitlines()[-1]); print(d['value'], d['ms_per_step'], d.get('kernel_ms'))"
 done

@@ -1,6 +1,6 @@
-// Pipe-rate microbenchmark for the integer SIMD instructions the Viterbi kernel is built from (sm_100a).
+// Pipe-rate microbenchmark for the integer SIMD instructions the Viterbi kernel is built from (sm_90a).
 // Each kernel runs a dependent-free stream of one instruction kind (8 independent chains per thread) so the number reported is
-// issue throughput: warp-instructions per cycle per SM sub-partition.   nvcc -arch=sm_100a -O3 -o pipes pipes.cu && ./pipes
+// issue throughput: warp-instructions per cycle per SM sub-partition.   nvcc -arch=sm_90a -O3 -o pipes pipes.cu && ./pipes
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -48,9 +48,10 @@ __global__ void k(uint32_t* out, uint32_t s, long long* cyc) {
 }
 template <int OPA, int OPB, int NA, int NB> void run(const char* name, int warps_per_smsp) {
     uint32_t* d; long long* dc; cudaMalloc(&d, 1 << 22); cudaMalloc(&dc, 8);
+    int nsm; cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, 0);     // one CTA per SM
     int threads = 32 * 4 * warps_per_smsp;
-    k<OPA, OPB, NA, NB><<<148, threads>>>(d, 12345u, dc); cudaDeviceSynchronize();
-    k<OPA, OPB, NA, NB><<<148, threads>>>(d, 12345u, dc); cudaDeviceSynchronize();
+    k<OPA, OPB, NA, NB><<<nsm, threads>>>(d, 12345u, dc); cudaDeviceSynchronize();
+    k<OPA, OPB, NA, NB><<<nsm, threads>>>(d, 12345u, dc); cudaDeviceSynchronize();
     long long c; cudaMemcpy(&c, dc, 8, cudaMemcpyDeviceToHost);
     double ninst = (double)ITER * 8 * (NA + NB) * warps_per_smsp;      // warp-instructions per SMSP
     printf("%-34s warps/SMSP %d  cycles %9lld  warp-inst/cycle/SMSP %.3f\n", name, warps_per_smsp, c, ninst / (double)c);

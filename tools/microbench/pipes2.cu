@@ -1,7 +1,7 @@
-// Second pipe-rate microbenchmark: mixes of the instructions of the v3 Viterbi step, to learn which share an issue pipe on sm_100a.
+// Second pipe-rate microbenchmark: mixes of the instructions of the v3 Viterbi step, to learn which share an issue pipe on sm_90a.
 // Every kernel interleaves up to three instruction kinds over independent register chains; the number printed is warp-instructions per
 // cycle per SM sub-partition (all kinds together).  Check the SASS of this file (cuobjdump -sass) before trusting a line: ptxas is free
-// to pick another opcode for an add.   nvcc -arch=sm_100a -O3 -o pipes2 pipes2.cu && ./pipes2
+// to pick another opcode for an add.   nvcc -arch=sm_90a -O3 -o pipes2 pipes2.cu && ./pipes2
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -51,7 +51,8 @@ __global__ void k(uint32_t* out, uint32_t s, long long* cyc) {
 }
 template <int A, int NA, int B, int NB, int C, int NC> void run(const char* name, int wps = 4) {
     uint32_t* d; long long* dc; cudaMalloc(&d, 1 << 22); cudaMalloc(&dc, 8);
-    for (int r = 0; r < 2; r++) { k<A, NA, B, NB, C, NC><<<148, 128 * wps>>>(d, 12345u, dc); cudaDeviceSynchronize(); }
+    int nsm; cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, 0);     // one CTA per SM
+    for (int r = 0; r < 2; r++) { k<A, NA, B, NB, C, NC><<<nsm, 128 * wps>>>(d, 12345u, dc); cudaDeviceSynchronize(); }
     long long c; cudaMemcpy(&c, dc, 8, cudaMemcpyDeviceToHost);
     printf("%-52s warps/SMSP %d  warp-inst/cycle/SMSP %.3f\n", name, wps, (double)ITER * 4 * (NA + NB + NC) * wps / (double)c);
     cudaFree(d); cudaFree(dc);

@@ -1,5 +1,5 @@
 #!/usr/bin/env python3
-"""Summarise an .ncu-rep (ncu --set full) into a small text file for profiles/: key throughput, occupancy, DRAM traffic,
+"""Summarise an .ncu-rep (ncu --set full) into a small text file: key throughput, occupancy, DRAM traffic,
 issue statistics and the top stall reasons.  Usage: tools/ncu_summary.py in.ncu-rep out.txt [note...]"""
 import csv, subprocess, sys, io
 KEYS = ["gpu__time_duration.sum", "dram__bytes_read.sum", "dram__bytes_write.sum", "gpu__dram_throughput.avg.pct_of_peak_sustained_elapsed",
