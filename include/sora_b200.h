@@ -262,6 +262,25 @@ void  sb200_host_free(void* p);
 int sb200_tx11b_fir37(sb200_handle* h, const int8_t* chips, uint64_t chips_total_samples, const uint64_t* frame_off, const uint32_t* frame_len,
                       uint32_t nframes, uint32_t variant, int8_t* out, void* cuda_stream);
 
+/* Legacy 802.11b transmitter, long or short preamble: BB11BPMDBufferTx4XWithLongHeader / ...WithShortHeader (kernel/bb/dot11b/bbb_tx.c:508-758,
+ * declared in kernel/inc/bb/bbb.h:204-240) — PLCP frame with CRC-16, the table scrambler (seed 0x6C long, 0x1B short) over PLCP + PSDU + FCS,
+ * Barker DBPSK preamble (long: and header), DQPSK header (short), DBPSK / DQPSK / CCK 5.5 / CCK 11 data, each chip followed by three zero
+ * samples, then TX_FIR_DEPTH zeros rounded up to a multiple of 128 samples — optionally run through the 37-tap filter as
+ * BB11BPMDPacketGenSignal (bbb_tx.c:119-150) does.  Frame i = payload[pay_off[i] .. +pay_len[i]) is the MPDU WITHOUT FCS; CRC-32 is
+ * appended, or, with flags SB200_TX11B_LEGACY_FCS_IN_PAYLOAD, the payload's last 4 bytes are sent verbatim as the FCS (PSDU 4 .. 4095 bytes).
+ * SB200_TX11B_LEGACY_PBCC is refused (SB200_E_INVALID): ModSelect PBCC only changes the LENGTH field in the reference (bbb_tx.c:51-57), the
+ * data would still be CCK.  Short preamble at 1 Mbps writes preamble and header only, as the reference does (its short-preamble switch has
+ * no 1 Mbps case, bbb_tx.c:563-605).  filter 0 = the encoder output (what BB11BPMDBufferTx4X* writes), 1 = BB11BPMDSpreadFIR4SSE over it,
+ * 2 = BB11BPMDSpreadFIR4ASM (see sb200_tx11b_fir37); the filtered stream is computed from the chips directly, never stored zero-stuffed.
+ * Slot i of `out` (out_stride_samples COMPLEX8 samples at 44 Msps, a multiple of 8; out 16-byte aligned) receives nsamples[i] samples and
+ * zeros to the end of the slot.  All pointers host or device.  The caller's payload is not modified (the reference scrambles its buffer in
+ * place; the legacy entry points of sora_b200_legacy.h reproduce that). */
+#define SB200_TX11B_LEGACY_FCS_IN_PAYLOAD 1u
+#define SB200_TX11B_LEGACY_PBCC           2u
+int sb200_tx11b_legacy_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_total, const uint64_t* pay_off, const uint32_t* pay_len,
+                             uint32_t nframes, uint32_t rate_kbps, uint32_t short_preamble, uint32_t flags, uint32_t filter, int8_t* out,
+                             uint64_t out_stride_samples, uint32_t* nsamples, void* cuda_stream);
+
 /* 802.11n transmit, two spatial streams, HT-mixed format: the modulator graphs CreatePreambleGraph11n + CreateSigGraph11n + CreateModGraph11n
  * (kernel/bb/demod11/fb11nmod_config.hpp:74-171) driven like Test11N_FB_Mod (kernel/bb/demod11/fb11n_mod.cpp:44-70).  Frame i =
  * payload[pay_off[i] .. +pay_len[i]) is the MPDU WITHOUT FCS (CF_11nTxVector::crc32 is appended); mcs 8 .. 14 (the modulator graph's own

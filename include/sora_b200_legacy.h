@@ -123,6 +123,51 @@ typedef struct _SORA_COMPLEX8 { int8_t re, im; } SORA_COMPLEX8, *PCOMPLEX8;
 HRESULT BB11BPMDSpreadFIR4SSE(const SORA_COMPLEX8* pcSrc, uint32_t uiInputSize, SORA_COMPLEX8* pcDest, ULONG* puiOutputSize);
 HRESULT BB11BPMDSpreadFIR4ASM(const SORA_COMPLEX8* pcSrc, uint32_t uiInputSize, SORA_COMPLEX8* pcDest, ULONG* puiOutputSize);
 
+/* ---- 802.11b transmitter: kernel/inc/bb/bbb.h:204-240, kernel/bb/dot11b/bbb_tx.c (encoder) + the filter above, long and short preamble.
+ * Served by sb200_tx11b_legacy_batch on the same process-wide engine.  Side effects callers see are reproduced: the encoder scrambles the
+ * caller's PSDU + FCS in place (Buffer variants: pbData[0 .. dataLength + 4); Packet variants: every MDL of the chain and Reserved1), and
+ * BB11BPMDPacketGenSignal stores the signal length in bytes into the packet's TX descriptor.  E_FAIL (SORA_E_FAIL) as in the reference
+ * (PreambleType other than 0 / 1; GenSignal buffers shorter than BB11B_MAX_SYMBOL_LENGTH) and also without a GPU, for a rate code other
+ * than 0x0A / 0x14 / 0x37 / 0x6E, for ModSelect PBCC (sb200_tx11b_legacy_batch), for a PSDU over 4095 bytes, and when an MDL chain does not
+ * add up to PacketSize.  PACKET_BASE, TX_DESC and MDL carry only the fields bbb_tx.c and the SoraPacket* helpers use. */
+#define DOT11B_PLCP_DATA_RATE_1M        0x0A
+#define DOT11B_PLCP_DATA_RATE_2M        0x14
+#define DOT11B_PLCP_DATA_RATE_5P5M      0x37
+#define DOT11B_PLCP_DATA_RATE_11M       0x6E
+#define DOT11B_PLCP_IS_LONG_PREAMBLE    0
+#define DOT11B_PLCP_IS_SHORT_PREAMBLE   1
+#define DOT11B_PLCP_IS_CCK              0
+#define DOT11B_PLCP_IS_PBCC             1
+typedef struct _DOT11B_PLCP_TXVECTOR {          /* kernel/inc/dot11_plcp.h:55-59 */
+    UCHAR DateRate;                             /* PLCP SIGNAL code */
+    UCHAR PreambleType;                         /* 0 = long, 1 = short */
+    UCHAR ModSelect;                            /* 0 = CCK, 1 = PBCC (refused) */
+} DOT11B_PLCP_TXVECTOR, *PDOT11B_PLCP_TXVECTOR;
+typedef SORA_COMPLEX8 TXSAMPLE, *PTXSAMPLE;
+typedef struct _MDL {                           /* the fields of the WDK MDL the encoder walks */
+    struct _MDL* Next; void* StartVa; ULONG ByteOffset; ULONG ByteCount;
+} MDL, *PMDL;
+typedef struct _TX_DESC {                       /* where the modulated samples go */
+    PTXSAMPLE pSampleBuffer; ULONG SampleBufferSize; ULONG SignalLength;   /* sizes in bytes */
+} TX_DESC, *PTX_DESC;
+typedef struct __PACKET_BASE {                  /* kernel/core/inc/_packet_base.h:44-56 */
+    PMDL pMdl; PTX_DESC pTxDesc; int32_t fStatus; ULONG PacketSize;
+    ULONG Reserved1;                            /* the FCS (CRC-32) the Packet variants send */
+    ULONG Reserved2, Reserved3, Reserved4; void* pReserved;
+} PACKET_BASE, *PPACKET_BASE;
+/* (MTU 1500 + long PLCP frame 24 + CRC-32 4) x 8 bits x 4 x 11 x sizeof(COMPLEX8), kernel/inc/bb/bbb.h:75-80 */
+#define BB11B_MAX_SYMBOL_LENGTH ((1500u + 24u + 4u) * 8u * 4u * 11u * 2u)
+
+void    BB11BTxVectorInit(PDOT11B_PLCP_TXVECTOR pTxVector, UCHAR cDataRate, UCHAR cModSelect, UCHAR cPreambleType);
+/* pbData = MPDU + FCS (dataLength + 4 bytes); pOutput receives *pOutputLength COMPLEX8 samples: the 4x zero-stuffed chips and zero padding */
+HRESULT BB11BPMDBufferTx4XWithShortHeader(PDOT11B_PLCP_TXVECTOR pTxVector, PUCHAR pbData, unsigned int dataLength, PUCHAR pOutput, unsigned int* pOutputLength);
+HRESULT BB11BPMDBufferTx4XWithLongHeader(PDOT11B_PLCP_TXVECTOR pTxVector, PUCHAR pbData, unsigned int dataLength, PUCHAR pOutput, unsigned int* pOutputLength);
+HRESULT BB11BPMDPacketTx4X(PDOT11B_PLCP_TXVECTOR pTxVector, PPACKET_BASE pSendSlot, PUCHAR pOutput, ULONG BufferLength, ULONG* puiOutputLength);
+/* encoder into pTempBuffer, then BB11BPMDSpreadFIR4SSE into the packet's sample buffer (bbb_tx.c:119-150) */
+HRESULT BB11BPMDPacketGenSignal(PPACKET_BASE pPacket, PDOT11B_PLCP_TXVECTOR pTxVector, PUCHAR pTempBuffer, ULONG TempBufferLength);
+void    SoraPacketGetTxSampleBuffer(PPACKET_BASE pPacket, PTXSAMPLE* ppBuffer, ULONG* pBufferSize);
+void    SoraPacketSetSignalLength(PPACKET_BASE pPacket, ULONG uLen);
+
 #ifdef __cplusplus
 }
 #endif

@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_tx11b_fir37", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -237,6 +237,27 @@ class Engine:
         out = np.zeros_like(fr)
         self.tx11b_fir37_raw(_ptr(fr), F * L, _ptr(off), _ptr(ln), F, variant, _ptr(out))
         return out.reshape(x.shape)
+
+    TX11B_LEGACY_FCS_IN_PAYLOAD = 1
+
+    def tx11b_legacy_raw(self, pay_ptr, pay_total, off_ptr, len_ptr, nframes, rate_kbps, short_preamble, flags, filt, out_ptr, out_stride, ns_ptr, stream=0):
+        self._check(self._lib.sb200_tx11b_legacy_batch(self._h, C.c_void_p(pay_ptr), C.c_uint64(pay_total), C.c_void_p(off_ptr), C.c_void_p(len_ptr), C.c_uint32(nframes),
+                                                       C.c_uint32(rate_kbps), C.c_uint32(short_preamble), C.c_uint32(flags), C.c_uint32(filt), C.c_void_p(out_ptr),
+                                                       C.c_uint64(out_stride), C.c_void_p(ns_ptr), C.c_void_p(stream)), "sb200_tx11b_legacy_batch")
+
+    def tx11b_legacy_batch(self, payloads, rate_kbps, short_preamble=False, filter=1, fcs_in_payload=False, out_stride=None):
+        """The legacy 802.11b transmitter (BB11BPMDBufferTx4X* and, filter 1 / 2, the SSE / ASM 37-tap filter).  payloads: list of uint8 arrays,
+        MPDUs without FCS (or with it, fcs_in_payload=True) -> (COMPLEX8 samples int8 [F, out_stride, 2] at 44 Msps, nsamples [F])."""
+        lens = np.array([len(p) for p in payloads], np.uint32); offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.uint64)
+        flat = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8) for p in payloads]) if lens.sum() else np.zeros(1, np.uint8))
+        if out_stride is None:
+            size = int(lens.max()) + (0 if fcs_in_payload else 4)
+            cpb = {1000: 0 if short_preamble else 88, 2000: 44, 5500: 16, 11000: 8}.get(rate_kbps, 8)     # an unknown rate is the library's error to report
+            out_stride = (4 * ((1056 if short_preamble else 2112) + size * cpb) + 37 + 127) // 128 * 128
+        out = np.zeros((len(lens), out_stride, 2), np.int8); ns = np.zeros(len(lens), np.uint32)
+        self.tx11b_legacy_raw(_ptr(flat), max(int(lens.sum()), 1), _ptr(offs), _ptr(lens), len(lens), rate_kbps, int(bool(short_preamble)),
+                              self.TX11B_LEGACY_FCS_IN_PAYLOAD if fcs_in_payload else 0, filter, _ptr(out), out_stride, _ptr(ns))
+        return out, ns
 
     def rxblocks_unpack(self, raw, left_shift=0):
         """raw: uint8 array of whole 128-byte RX_BLOCKs (a *.dmp file) -> int16 [28*nblocks, 2] via the device gather."""

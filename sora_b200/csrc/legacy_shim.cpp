@@ -200,14 +200,18 @@ extern "C" HRESULT BB11BRx(PBB11B_RX_CONTEXT c, PSORA_RADIO_RX_STREAM s) {
 // ---- BB11BPMDSpreadFIR4SSE / BB11BPMDSpreadFIR4ASM (bbb.h:188-200): context-free in the reference, so the engine is process-wide here ----
 #include <mutex>
 static std::mutex g_fir_mu; static sb200_handle* g_fir_engine = nullptr;
+static bool fir_engine() {                              // under g_fir_mu
+    if (!g_fir_engine) {
+        const char* d = getenv("SB200_DEVICE"); sb200_handle* h = nullptr;
+        if (sb200_create(d ? atoi(d) : 0, nullptr, &h) != SB200_OK) return false;                  // no CPU fallback
+        g_fir_engine = h;
+    }
+    return true;
+}
 static HRESULT spread_fir(const SORA_COMPLEX8* src, uint32_t n, SORA_COMPLEX8* dst, ULONG* out_n, uint32_t variant) {
     if (!src || !dst || (n & 7u)) return SORA_E_FAIL;
     std::lock_guard<std::mutex> lk(g_fir_mu);
-    if (!g_fir_engine) {
-        const char* d = getenv("SB200_DEVICE"); sb200_handle* h = nullptr;
-        if (sb200_create(d ? atoi(d) : 0, nullptr, &h) != SB200_OK) return SORA_E_FAIL;            // no CPU fallback
-        g_fir_engine = h;
-    }
+    if (!fir_engine()) return SORA_E_FAIL;
     const uint64_t off = 0; const uint32_t len = n;
     if (n && sb200_tx11b_fir37(g_fir_engine, (const int8_t*)src, n, &off, &len, 1, variant, (int8_t*)dst, nullptr) != SB200_OK) return SORA_E_FAIL;
     if (out_n) *out_n = n;
@@ -215,3 +219,107 @@ static HRESULT spread_fir(const SORA_COMPLEX8* src, uint32_t n, SORA_COMPLEX8* d
 }
 extern "C" HRESULT BB11BPMDSpreadFIR4SSE(const SORA_COMPLEX8* s, uint32_t n, SORA_COMPLEX8* d, ULONG* on) { return spread_fir(s, n, d, on, 0); }
 extern "C" HRESULT BB11BPMDSpreadFIR4ASM(const SORA_COMPLEX8* s, uint32_t n, SORA_COMPLEX8* d, ULONG* on) { return spread_fir(s, n, d, on, 1); }
+
+// ---- the legacy 802.11b transmitter (bbb.h:204-240, bbb_tx.c) over sb200_tx11b_legacy_batch ---------------------------------------------
+namespace {
+uint32_t kbps_of_code(UCHAR c) { return c == 0x0A ? 1000u : c == 0x14 ? 2000u : c == 0x37 ? 5500u : c == 0x6E ? 11000u : 0u; }
+// the samples BB11BPMDBufferTx4X* writes for a PSDU of `size` bytes (FCS included): 4 per chip, TX_FIR_DEPTH zeros rounded up to 128
+uint32_t legacy_nsamples(uint32_t size, UCHAR pre, uint32_t kbps) {
+    const uint32_t cpb = kbps == 1000 ? (pre ? 0u : 88u) : kbps == 2000 ? 44u : kbps == 5500 ? 16u : 8u;
+    return (4u * ((pre ? 1056u : 2112u) + size * cpb) + 37u + 127u) & ~127u;
+}
+// the scrambler's side effect on the caller's bytes: the stream runs over the PLCP frame first (bbb_tx.c:537-538, :669-670)
+void scramble_in_place(const DOT11B_PLCP_TXVECTOR* v, uint32_t kbps, uint32_t size, const std::vector<uint8_t*>& bytes) {
+    uint32_t plen, ext = 0;                                                                 // PLCPGetLength (bbb_tx.c:39-65), CCK
+    if (kbps == 1000) plen = size << 3; else if (kbps == 2000) plen = size << 2;
+    else if (kbps == 5500) plen = ((size << 4) - 1u) / 11u + 1u;
+    else { plen = ((size << 3) - 1u) / 11u + 1u; if (plen * 11u - (size << 3) >= 8u) ext = 1; }
+    uint8_t hdr[6] = {v->DateRate, (uint8_t)(ext << 7), (uint8_t)plen, (uint8_t)(plen >> 8), 0, 0};
+    unsigned c = 0xFFFFu;
+    for (int i = 0; i < 4; i++) { c ^= hdr[i]; for (int k = 0; k < 8; k++) c = (c & 1u) ? (c >> 1) ^ 0x8408u : c >> 1; }
+    c = ~c & 0xFFFFu; hdr[4] = (uint8_t)c; hdr[5] = (uint8_t)(c >> 8);
+    unsigned reg = v->PreambleType ? 0x1Bu : 0x6Cu;
+    auto scr = [&](uint8_t x) { uint8_t o = 0; for (int k = 0; k < 8; k++) { const unsigned b = (x ^ reg ^ (reg >> 3)) & 1u; reg = (reg >> 1) | (b << 6); o |= (uint8_t)(b << k); x >>= 1; } reg = o >> 1; return o; };
+    const int nsync = v->PreambleType ? 7 : 16;
+    for (int i = 0; i < nsync; i++) scr(v->PreambleType ? 0x00 : 0xFF);
+    if (v->PreambleType) { scr(0xCF); scr(0x05); } else { scr(0xA0); scr(0xF3); }
+    for (int i = 0; i < 6; i++) scr(hdr[i]);
+    for (uint8_t* b : bytes) *b = scr(*b);
+}
+// encode psdu (FCS included) with the filter selected (0 encoder output, 1 SSE filter) into dst; n = samples written
+HRESULT legacy_tx(const DOT11B_PLCP_TXVECTOR* v, const std::vector<uint8_t>& psdu, uint32_t filter, void* dst, uint32_t* n) {
+    const uint32_t kbps = kbps_of_code(v->DateRate);
+    if (!kbps || v->PreambleType > 1 || v->ModSelect != 0 || psdu.size() < 4 || psdu.size() > 4095) return SORA_E_FAIL;
+    const uint32_t ns = legacy_nsamples((uint32_t)psdu.size(), v->PreambleType, kbps);
+    void* buf = nullptr;
+    if (posix_memalign(&buf, 16, (size_t)ns * 2) != 0) return SORA_E_FAIL;
+    const uint64_t off = 0; const uint32_t len = (uint32_t)psdu.size(); uint32_t got = 0;
+    int rc;
+    {   std::lock_guard<std::mutex> lk(g_fir_mu);
+        rc = fir_engine() ? sb200_tx11b_legacy_batch(g_fir_engine, psdu.data(), len, &off, &len, 1, kbps, v->PreambleType, SB200_TX11B_LEGACY_FCS_IN_PAYLOAD, filter,
+                                                     (int8_t*)buf, ns, &got, nullptr) : SB200_E_NODEVICE; }
+    if (rc == SB200_OK && got == ns) memcpy(dst, buf, (size_t)ns * 2);
+    free(buf);
+    if (rc != SB200_OK || got != ns) return SORA_E_FAIL;
+    *n = ns;
+    return SORA_S_OK;
+}
+HRESULT buffer_tx(PDOT11B_PLCP_TXVECTOR v, PUCHAR data, unsigned int dataLength, PUCHAR out, unsigned int* n, UCHAR pre) {
+    if (!v || !data || !out || !n) return SORA_E_FAIL;
+    DOT11B_PLCP_TXVECTOR w = *v; w.PreambleType = pre;                                   // the entry point, not the vector, picks the preamble
+    std::vector<uint8_t> psdu(data, data + dataLength + 4u);
+    uint32_t ns = 0;
+    const HRESULT r = legacy_tx(&w, psdu, 0, out, &ns);
+    if (r != SORA_S_OK) return r;
+    std::vector<uint8_t*> bytes; for (unsigned int i = 0; i < dataLength + 4u; i++) bytes.push_back(data + i);
+    scramble_in_place(&w, kbps_of_code(w.DateRate), dataLength + 4u, bytes);
+    *n = ns;
+    return SORA_S_OK;
+}
+// the MDL chain and Reserved1 as one PSDU; pointers to the bytes in order (for the in-place scramble)
+bool packet_bytes(PPACKET_BASE p, std::vector<uint8_t>& psdu, std::vector<uint8_t*>& where) {
+    for (PMDL m = p->pMdl; m; m = m->Next)
+        for (ULONG i = 0; i < m->ByteCount; i++) { uint8_t* b = (uint8_t*)m->StartVa + m->ByteOffset + i; psdu.push_back(*b); where.push_back(b); }
+    if (psdu.size() != p->PacketSize) return false;
+    for (int i = 0; i < 4; i++) { uint8_t* b = (uint8_t*)&p->Reserved1 + i; psdu.push_back(*b); where.push_back(b); }   // little endian, as sizeof(ULONG) bytes are read
+    return true;
+}
+HRESULT packet_tx(PDOT11B_PLCP_TXVECTOR v, PPACKET_BASE p, PUCHAR out, ULONG* n, PTXSAMPLE filtered, ULONG* nfiltered) {
+    if (!v || !p || !out) return SORA_E_FAIL;
+    if (v->PreambleType > 1) return SORA_E_FAIL;                                            // bbb_tx.c:94-97
+    std::vector<uint8_t> psdu; std::vector<uint8_t*> where;
+    if (!packet_bytes(p, psdu, where)) return SORA_E_FAIL;
+    uint32_t ns = 0;
+    HRESULT r = legacy_tx(v, psdu, 0, out, &ns);
+    if (r == SORA_S_OK && filtered) r = legacy_tx(v, psdu, 1, filtered, &ns);
+    if (r != SORA_S_OK) return r;
+    scramble_in_place(v, kbps_of_code(v->DateRate), (uint32_t)psdu.size(), where);
+    if (n) *n = ns;
+    if (nfiltered) *nfiltered = ns;
+    return SORA_S_OK;
+}
+}
+
+extern "C" void BB11BTxVectorInit(PDOT11B_PLCP_TXVECTOR v, UCHAR rate, UCHAR mod, UCHAR pre) { v->DateRate = rate; v->ModSelect = mod; v->PreambleType = pre; }
+extern "C" HRESULT BB11BPMDBufferTx4XWithShortHeader(PDOT11B_PLCP_TXVECTOR v, PUCHAR d, unsigned int len, PUCHAR o, unsigned int* n) { return buffer_tx(v, d, len, o, n, 1); }
+extern "C" HRESULT BB11BPMDBufferTx4XWithLongHeader(PDOT11B_PLCP_TXVECTOR v, PUCHAR d, unsigned int len, PUCHAR o, unsigned int* n) { return buffer_tx(v, d, len, o, n, 0); }
+extern "C" HRESULT BB11BPMDPacketTx4X(PDOT11B_PLCP_TXVECTOR v, PPACKET_BASE p, PUCHAR o, ULONG BufferLength, ULONG* n) {
+    (void)BufferLength;                                                                      // unused by the reference too (bbb_tx.c:84)
+    return packet_tx(v, p, o, n, nullptr, nullptr);
+}
+extern "C" void SoraPacketGetTxSampleBuffer(PPACKET_BASE p, PTXSAMPLE* b, ULONG* size) {
+    *b = p && p->pTxDesc ? p->pTxDesc->pSampleBuffer : nullptr; *size = p && p->pTxDesc ? p->pTxDesc->SampleBufferSize : 0;
+}
+extern "C" void SoraPacketSetSignalLength(PPACKET_BASE p, ULONG len) { if (p && p->pTxDesc) p->pTxDesc->SignalLength = len; }
+extern "C" HRESULT BB11BPMDPacketGenSignal(PPACKET_BASE p, PDOT11B_PLCP_TXVECTOR v, PUCHAR temp, ULONG temp_len) {
+    PTXSAMPLE sb = nullptr; ULONG sb_size = 0;
+    if (!p) return SORA_E_FAIL;
+    SoraPacketGetTxSampleBuffer(p, &sb, &sb_size);
+    if (temp_len < BB11B_MAX_SYMBOL_LENGTH || sb_size < BB11B_MAX_SYMBOL_LENGTH || !sb || !temp) return SORA_E_FAIL;   // bbb_tx.c:133-137
+    ULONG n = 0, nf = 0;
+    const HRESULT r = packet_tx(v, p, temp, &n, sb, &nf);
+    if (r != SORA_S_OK) return r;
+    memset(temp + (size_t)n * 2, 0, 64);                                                     // bbb_tx.c:140
+    SoraPacketSetSignalLength(p, nf * (ULONG)sizeof(TXSAMPLE));
+    return SORA_S_OK;
+}

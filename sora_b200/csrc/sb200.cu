@@ -1311,6 +1311,75 @@ extern "C" int sb200_tx11b_fir37(sb200_handle* h, const int8_t* chips, uint64_t 
     return SB200_OK;
 }
 
+// Legacy 802.11b transmitter (tx11b_legacy_kernels.cuh): BB11BPMDBufferTx4XWith{Long,Short}Header, optionally followed by the 37-tap filter.
+extern "C" int sb200_tx11b_legacy_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_total, const uint64_t* pay_off, const uint32_t* pay_len,
+                                        uint32_t nframes, uint32_t rate_kbps, uint32_t short_preamble, uint32_t flags, uint32_t filter, int8_t* out,
+                                        uint64_t out_stride_samples, uint32_t* nsamples, void* cuda_stream) {
+    if (!h || !payload || !pay_off || !pay_len || !out) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
+    if (flags & SB200_TX11B_LEGACY_PBCC) return h->fail(SB200_E_INVALID, "PBCC is not supported: the reference only lengthens PLCPGetLength for it and still sends CCK");
+    if (flags & ~SB200_TX11B_LEGACY_FCS_IN_PAYLOAD) return h->fail(SB200_E_INVALID, "unknown flags");
+    if (filter > 2) return h->fail(SB200_E_INVALID, "filter must be 0 (encoder output), 1 (BB11BPMDSpreadFIR4SSE) or 2 (BB11BPMDSpreadFIR4ASM)");
+    if (short_preamble > 1) return h->fail(SB200_E_INVALID, "short_preamble must be 0 or 1");
+    if (out_stride_samples % 8u || ((uintptr_t)out & 15u)) return h->fail(SB200_E_INVALID, "out must be 16-byte aligned and out_stride_samples a multiple of 8");
+    if (nframes == 0) return SB200_OK;
+    Tx11bLegacyJob job{};
+    job.rate_kbps = rate_kbps; job.short_preamble = short_preamble; job.fcs_in_payload = (flags & SB200_TX11B_LEGACY_FCS_IN_PAYLOAD) ? 1u : 0u; job.filter = filter;
+    switch (rate_kbps) {                                                                // bb/bbb.h:47-50
+        case 1000: job.rate_code = 0x0A; job.data_chips_per_byte = short_preamble ? 0u : 88u; break;
+        case 2000: job.rate_code = 0x14; job.data_chips_per_byte = 44; break;
+        case 5500: job.rate_code = 0x37; job.data_chips_per_byte = 16; break;
+        case 11000: job.rate_code = 0x6E; job.data_chips_per_byte = 8; break;
+        default: return h->fail(SB200_E_INVALID, "rate_kbps is not an 802.11b rate");
+    }
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    CK(cudaSetDevice(h->device));
+    std::vector<uint64_t> offh(nframes); std::vector<uint32_t> lenh(nframes);
+    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len), pay_dev = is_device_ptr(payload), out_dev = is_device_ptr(out);
+    if (off_dev) CK(cudaMemcpyAsync(offh.data(), pay_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), pay_off, nframes * 8ull);
+    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), pay_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), pay_len, nframes * 4ull);
+    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    uint32_t max_size = 0;
+    for (uint32_t i = 0; i < nframes; i++) {
+        const uint32_t size = job.fcs_in_payload ? lenh[i] : lenh[i] + 4u;            // PSDU bytes, FCS included
+        if (job.fcs_in_payload && lenh[i] < 4u) return h->fail(SB200_E_INVALID, "with SB200_TX11B_LEGACY_FCS_IN_PAYLOAD every payload carries its 4 FCS bytes");
+        if (lenh[i] > 4095u || size > 4095u || lenh[i] > payload_total || offh[i] > payload_total - lenh[i]) return h->fail(SB200_E_INVALID, "payload slot out of range (PSDU 4 .. 4095 bytes incl. FCS)");
+        if (tx11b_legacy_nsamples(size, short_preamble, job.data_chips_per_byte) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
+        if (size > max_size) max_size = size;
+    }
+    job.desc_stride = (24u + max_size + 7u) & ~7u;
+    const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len;
+    if (pay_dev) d_pay = payload; else { CK(h->txpay.need(payload_total)); CK(cudaMemcpyAsync(h->txpay.p, payload, payload_total, cudaMemcpyHostToDevice, st)); d_pay = (const uint8_t*)h->txpay.p; }
+    if (off_dev) d_off = pay_off; else { CK(h->txoff.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->txoff.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); d_off = (const uint64_t*)h->txoff.p; }
+    if (len_dev) d_len = pay_len; else { CK(h->txlen.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->txlen.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); d_len = (const uint32_t*)h->txlen.p; }
+    const size_t out_bytes = (size_t)nframes * out_stride_samples * 2;
+    int8_t* d_out = out; if (!out_dev) { CK(h->txout.need(out_bytes)); d_out = (int8_t*)h->txout.p; }
+    uint32_t* d_ns = nullptr; const bool ns_dev = nsamples && is_device_ptr(nsamples);
+    if (nsamples) { if (ns_dev) d_ns = nsamples; else { CK(h->txns.need(nframes * 4ull)); d_ns = (uint32_t*)h->txns.p; } }
+    CK(h->txdesc.need((size_t)nframes * job.desc_stride * 2ull));
+    const uint64_t per_cta = SB_TX11B_LEGACY_THREADS * 8, ny = (out_stride_samples + per_cta - 1) / per_cta;
+    if (ny > 65535u) return h->fail(SB200_E_INVALID, "out_stride_samples too large");
+    CK(cudaEventRecord(h->ev0, st));
+    const uint32_t* d_crc = nullptr;
+    if (!job.fcs_in_payload) {
+        CK(h->crc.need(nframes * 4ull));
+        k_tx11a_crc<<<(nframes + 127) / 128, 128, 0, st>>>(d_pay, d_off, d_len, nframes, h->T, (uint32_t*)h->crc.p);
+        d_crc = (const uint32_t*)h->crc.p; h->launches += 1;
+    }
+    k_tx11b_legacy_code<<<(nframes + 127) / 128, 128, 0, st>>>(d_pay, d_off, d_len, nframes, job, d_crc, (uint16_t*)h->txdesc.p);
+    const dim3 grid(nframes, (unsigned)ny); const uint16_t* dd = (const uint16_t*)h->txdesc.p;
+    if (filter == 0) k_tx11b_legacy_spread<0><<<grid, SB_TX11B_LEGACY_THREADS, 0, st>>>(d_len, job, dd, d_out, out_stride_samples, d_ns);
+    else if (filter == 1) k_tx11b_legacy_spread<1><<<grid, SB_TX11B_LEGACY_THREADS, 0, st>>>(d_len, job, dd, d_out, out_stride_samples, d_ns);
+    else k_tx11b_legacy_spread<2><<<grid, SB_TX11B_LEGACY_THREADS, 0, st>>>(d_len, job, dd, d_out, out_stride_samples, d_ns);
+    CK(cudaEventRecord(h->ev1, st));
+    h->timed = true; h->nk = 0; h->launches += 2;
+    CK(cudaGetLastError());
+    bool sync = false;
+    if (!out_dev) { CK(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st)); sync = true; }
+    if (nsamples && !ns_dev) { CK(cudaMemcpyAsync(nsamples, d_ns, nframes * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
+    if (sync) CK(cudaStreamSynchronize(st));
+    return SB200_OK;
+}
+
 // 802.11n transmit (tx11n_kernels.cuh)
 static int upload_tables_tx11n(sb200_handle* h) {
     if (h->tabtx11n.p) return SB200_OK;
