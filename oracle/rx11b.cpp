@@ -12,6 +12,10 @@ static inline c16 csub(c16 a, c16 b) { return c16{w16(a.re - b.re), w16(a.im - b
 static inline c16 cadd(c16 a, c16 b) { return c16{w16(a.re + b.re), w16(a.im + b.im)}; }
 static inline c16 csra(c16 a, int n) { return c16{w16(a.re >> n), w16(a.im >> n)}; }
 static inline int cnorm2(c16 a) { return a.re * a.re + a.im * a.im; }
+// int32 arithmetic of the reference's scalar C and SSE code, which wraps (two's complement, paddd / pmaddwd / psubd)
+static inline int32_t wadd(int32_t a, int32_t b) { return (int32_t)((uint32_t)a + (uint32_t)b); }
+static inline int32_t wsub(int32_t a, int32_t b) { return (int32_t)((uint32_t)a - (uint32_t)b); }
+static inline int32_t wneg(int32_t a) { return (int32_t)(0u - (uint32_t)a); }
 
 static uint16_t g_crc16_lut[256];
 static bool build_crc16() {                 // CCITT CRC-16 reflected (0x8408), core/inc/CRC16.h:37-48
@@ -65,7 +69,8 @@ void Rx11b::dcest(const c16* v) {
 void Rx11b::energy_detect(const c16* v) {
     if (error_code == E_CS_TIMEOUT) return;            // `ipin.clear(); return 0`: later vectors of the block still arrive, see below
     uint32_t p = 0;
-    for (int k = 0; k < 4; k++) p += (uint32_t)((v[k].re * v[k].re + v[k].im * v[k].im) >> 5);
+    // hadd(shift_right(SquaredNorm(pi), 5)) (cca.hpp:65): pmaddwd wraps (-32768, -32768) to INT_MIN, psrad 5 keeps the sign, the hadd wraps
+    for (int k = 0; k < 4; k++) p += (uint32_t)(wadd(v[k].re * v[k].re, v[k].im * v[k].im) >> 5);
     avg_energy = avg_energy - win[win_idx] + p; win[win_idx] = p; win_idx = (win_idx + 1) & 7;
     ed_count++;
     if (ed_count >= 32) {
@@ -87,16 +92,17 @@ static Pick cck11_module(int32_t a1r, int32_t a1i, int32_t a2r, int32_t a2i, int
     b2r[1] = a4r - a3i; b2i[1] = a4i + a3r; b3r[1] = a4r + a3i; b3i[1] = a4i - a3r;
     for (int k = 0; k < 2; k++) { b0r[k] >>= 2; b0i[k] >>= 2; b1r[k] >>= 2; b1i[k] >>= 2; b2r[k] >>= 2; b2i[k] >>= 2; b3r[k] >>= 2; b3i[k] >>= 2; }
     int32_t Lr[4], Li[4];
-    Lr[0] = mul32(b0r[0], b2r[0]) + mul32(b0i[0], b2i[0]); Li[0] = mul32(b0r[0], b2i[0]) - mul32(b0i[0], b2r[0]);
-    Lr[1] = mul32(b0r[1], b2r[1]) + mul32(b0i[1], b2i[1]); Li[1] = mul32(b0r[1], b2i[1]) - mul32(b0i[1], b2r[1]);
-    Lr[2] = mul32(b1r[0], b3r[0]) + mul32(b1i[0], b3i[0]); Li[2] = mul32(b1r[0], b3i[0]) - mul32(b1i[0], b3r[0]);
-    Lr[3] = mul32(b1r[1], b3r[1]) + mul32(b1i[1], b3i[1]); Li[3] = mul32(b1r[1], b3i[1]) - mul32(b1i[1], b3r[1]);
+    // cck.hpp:300-307 and the abs / negations below are 32-bit int C: full-scale chips wrap them
+    Lr[0] = wadd(mul32(b0r[0], b2r[0]), mul32(b0i[0], b2i[0])); Li[0] = wsub(mul32(b0r[0], b2i[0]), mul32(b0i[0], b2r[0]));
+    Lr[1] = wadd(mul32(b0r[1], b2r[1]), mul32(b0i[1], b2i[1])); Li[1] = wsub(mul32(b0r[1], b2i[1]), mul32(b0i[1], b2r[1]));
+    Lr[2] = wadd(mul32(b1r[0], b3r[0]), mul32(b1i[0], b3i[0])); Li[2] = wsub(mul32(b1r[0], b3i[0]), mul32(b1i[0], b3r[0]));
+    Lr[3] = wadd(mul32(b1r[1], b3r[1]), mul32(b1i[1], b3i[1])); Li[3] = wsub(mul32(b1r[1], b3i[1]), mul32(b1i[1], b3r[1]));
     static const uint8_t base[4] = {0x00, 0x30, 0x10, 0x20};
     int32_t mx[4]; uint8_t vl[4];
     for (int k = 0; k < 4; k++) {
-        int32_t ar = Lr[k] < 0 ? -Lr[k] : Lr[k], ai = Li[k] < 0 ? -Li[k] : Li[k];
-        if (ar > ai) { if (Lr[k] > 0) { mx[k] = Lr[k]; vl[k] = base[k] | 0x00; } else { mx[k] = -Lr[k]; vl[k] = base[k] | 0x40; } }
-        else         { if (Li[k] > 0) { mx[k] = Li[k]; vl[k] = base[k] | 0xC0; } else { mx[k] = -Li[k]; vl[k] = base[k] | 0x80; } }
+        int32_t ar = Lr[k] < 0 ? wneg(Lr[k]) : Lr[k], ai = Li[k] < 0 ? wneg(Li[k]) : Li[k];
+        if (ar > ai) { if (Lr[k] > 0) { mx[k] = Lr[k]; vl[k] = base[k] | 0x00; } else { mx[k] = wneg(Lr[k]); vl[k] = base[k] | 0x40; } }
+        else         { if (Li[k] > 0) { mx[k] = Li[k]; vl[k] = base[k] | 0xC0; } else { mx[k] = wneg(Li[k]); vl[k] = base[k] | 0x80; } }
     }
     Pick p;
     if (mx[0] > mx[1]) { p.max = mx[0]; p.val = vl[0]; } else { p.max = mx[1]; p.val = vl[1]; }
@@ -105,9 +111,10 @@ static Pick cck11_module(int32_t a1r, int32_t a1i, int32_t a2r, int32_t a2i, int
     return p;
 }
 static inline void dqpsk_bits(uint8_t& r, int pos, c16 ref, c16 s) {       // barkerspread.hpp:430-437
-    int32_t re = ref.re * s.re + ref.im * s.im, im = ref.re * s.im - ref.im * s.re;
-    r |= (uint8_t)(((uint32_t)(re + im) >> 31) << pos);
-    r |= (uint8_t)(((uint32_t)(re - im) >> 31) << (pos + 1));
+    // int C: after a CCK symbol `ref` is a raw chip, and full-scale chips wrap the sums
+    int32_t re = wadd(ref.re * s.re, ref.im * s.im), im = wsub(ref.re * s.im, ref.im * s.re);
+    r |= (uint8_t)(((uint32_t)wadd(re, im) >> 31) << pos);
+    r |= (uint8_t)(((uint32_t)wsub(re, im) >> 31) << (pos + 1));
 }
 uint8_t cck11_decode(const c16* P, c16& last, int& even) {                  // cck.hpp:262-769 CCK11_DECODER
     int32_t p[8][2]; for (int i = 0; i < 8; i++) { p[i][0] = P[i].re; p[i][1] = P[i].im; }
@@ -143,7 +150,7 @@ static void cck5_half(uint8_t& out, const c16* P, c16& last, bool hi) {
         int32_t b0r = a00r + a01r, b0i = a00i + a01i, b1r = a10r + a11r, b1i = a10i + a11i;
         b0i = -b0i;
         b0r >>= 2; b0i >>= 2; b1r >>= 2; b1i >>= 2;
-        return mul32(b0r, b1r) - mul32(b0i, b1i);                          // L1.re
+        return wsub(mul32(b0r, b1r), mul32(b0i, b1i));                     // L1.re
     };
     int32_t l1 = corr(I(0) + R(1), I(1) - R(0), I(2) - R(3), -(R(2) + I(3)), I(4) + R(5), I(5) - R(4), R(7) - I(6), R(6) + I(7));
     int32_t l2 = corr(R(1) - I(0), R(0) + I(1), -(I(2) + R(3)), R(2) - I(3), R(5) - I(4), R(4) + I(5), I(6) + R(7), I(7) - R(6));
@@ -151,8 +158,8 @@ static void cck5_half(uint8_t& out, const c16* P, c16& last, bool hi) {
 #undef I
     int32_t max1, max2; uint8_t v1, v2;
     const uint8_t b3 = hi ? 0x80 : 0x08, b2 = hi ? 0x40 : 0x04;
-    if (l1 > 0) { max1 = l1; v1 = 0; } else { max1 = -l1; v1 = b3; }
-    if (l2 > 0) { max2 = l2; v2 = b2; } else { max2 = -l2; v2 = (uint8_t)(b2 | b3); }
+    if (l1 > 0) { max1 = l1; v1 = 0; } else { max1 = wneg(l1); v1 = b3; }
+    if (l2 > 0) { max2 = l2; v2 = b2; } else { max2 = wneg(l2); v2 = (uint8_t)(b2 | b3); }
     const uint8_t pick = max1 > max2 ? v1 : v2;
     if (!hi) { out = pick; dqpsk_bits(out, 0, last, P[7]); }
     else { out |= pick; dqpsk_bits(out, 4, last, P[7]); out ^= 0x30; }

@@ -74,13 +74,18 @@ bool ht_mcs_params(uint32_t mcs, HtMcs& m) {
     m = P[mcs - 8]; return true;
 }
 
-int16_t dsp_atan(int x, int y) {                        // dsp_math.h:166-212 (the short overload :90-164 agrees on its range)
+int16_t dsp_atan(int x, int y) {                        // dsp_math.h:157-212 (the short overload :90-164 agrees on its range)
+    // dsp_math::abs / imax (dsp_math.h:64-88) and the sums are 32-bit int C, which wraps: abs(INT_MIN) = INT_MIN, and
+    // tsum = |x| + |y| wraps once either argument passes 2^30
+    auto wadd = [](int a, int b) { return (int)((unsigned)a + (unsigned)b); };
+    auto wsub = [](int a, int b) { return (int)((unsigned)a - (unsigned)b); };
+    auto iabs = [&](int v) { return wsub(v ^ (v >> 31), v >> 31); };
     const int sign = (x ^ y) >> 31;                     // 0 or -1
-    const int ax = (x ^ (x >> 31)) - (x >> 31), ay = (y ^ (y >> 31)) - (y >> 31);
-    const int tsign = (ax - ay) >> 31;
-    const int tsum = ax + ay; int d = ax - ay; d = (d ^ (d >> 31)) - (d >> 31);
-    const int tmax = (tsum + d) >> 1, tmin = tsum - tmax;
-    int64_t num = (int64_t)tmin << 16, den = tmax; if (den == 0) den = 1;
+    const int ax = iabs(x), ay = iabs(y);
+    const int tsign = wsub(ax, ay) >> 31;
+    const int tsum = wadd(ax, ay), d = iabs(wsub(ax, ay));
+    const int tmax = wadd(tsum, d) >> 1, tmin = wsub(tsum, tmax);
+    int64_t num = (int64_t)tmin * 65536, den = tmax; if (den == 0) den = 1;
     int idx = (int)((num + (den >> 1)) / den); idx >>= 4;
     if (idx < 0 || idx >= 4097) return 0;
     int16_t srad = tables11n().atan_lut[idx];
@@ -140,7 +145,7 @@ void Rx11n::cca_process(const c16* a, const c16* b) {
     his_idx = (his_idx + 1) % 8;
     for (int k = 0; k < 4; k++) {
         const int32_t cr = w32((int64_t)(R[0][k].re >> 1) + (R[1][k].re >> 1)), ci = w32((int64_t)(R[0][k].im >> 1) + (R[1][k].im >> 1));
-        const int64_t acorr = (int64_t)cr * cr + (int64_t)ci * ci;
+        const int64_t acorr = (int64_t)((uint64_t)((int64_t)cr * cr) + (uint64_t)((int64_t)ci * ci));  // SquaredNorm(vci): pmuldq, paddq wraps (vector128.h:922-933)
         const int32_t es = w32((int64_t)(ve[0][k] >> 1) + (ve[1][k] >> 1));
         const int64_t energy = (int64_t)es * es;
         // his + 1 overflows for the LLONG_MAX start value (cca_11n.hpp:153): the quotient is then 0

@@ -16,6 +16,8 @@ struct cs16 { int re, im; };     // values always kept in int16 range (sign-exte
 __host__ __device__ __forceinline__ int sx16(int v) { return (int)(short)v; }                 // truncate to int16
 __host__ __device__ __forceinline__ int sat16(int v) { return v > 32767 ? 32767 : (v < -32768 ? -32768 : v); }
 __host__ __device__ __forceinline__ int wadd(int a, int b) { return (int)((unsigned)a + (unsigned)b); }   // pmaddwd / paddd wrap
+__host__ __device__ __forceinline__ int wsub(int a, int b) { return (int)((unsigned)a - (unsigned)b); }   // psubd / int C wrap
+__host__ __device__ __forceinline__ int wneg(int a) { return (int)(0u - (unsigned)a); }                  // int C negate (INT_MIN stays)
 
 __host__ __device__ __forceinline__ cs16 unpack(uint32_t w) { cs16 c; c.re = (int)(short)(w & 0xFFFF); c.im = (int)w >> 16; return c; }
 __host__ __device__ __forceinline__ uint32_t pack(cs16 c) { return ((uint32_t)c.re & 0xFFFFu) | ((uint32_t)c.im << 16); }

@@ -39,17 +39,17 @@ __device__ __forceinline__ CckPick cck11_module(int a1r, int a1i, int a2r, int a
     const int b20r = (a4r + a3r) >> 2, b20i = (a4i + a3i) >> 2, b30r = (a4r - a3r) >> 2, b30i = (a4i - a3i) >> 2;
     const int b21r = (a4r - a3i) >> 2, b21i = (a4i + a3r) >> 2, b31r = (a4r + a3i) >> 2, b31i = (a4i - a3r) >> 2;
     int Lr[4], Li[4];
-    Lr[0] = imul(b00r, b20r) + imul(b00i, b20i); Li[0] = imul(b00r, b20i) - imul(b00i, b20r);
-    Lr[1] = imul(b01r, b21r) + imul(b01i, b21i); Li[1] = imul(b01r, b21i) - imul(b01i, b21r);
-    Lr[2] = imul(b10r, b30r) + imul(b10i, b30i); Li[2] = imul(b10r, b30i) - imul(b10i, b30r);
-    Lr[3] = imul(b11r, b31r) + imul(b11i, b31i); Li[3] = imul(b11r, b31i) - imul(b11i, b31r);
+    Lr[0] = wadd(imul(b00r, b20r), imul(b00i, b20i)); Li[0] = wsub(imul(b00r, b20i), imul(b00i, b20r));     // 32-bit int C: full-scale chips wrap
+    Lr[1] = wadd(imul(b01r, b21r), imul(b01i, b21i)); Li[1] = wsub(imul(b01r, b21i), imul(b01i, b21r));
+    Lr[2] = wadd(imul(b10r, b30r), imul(b10i, b30i)); Li[2] = wsub(imul(b10r, b30i), imul(b10i, b30r));
+    Lr[3] = wadd(imul(b11r, b31r), imul(b11i, b31i)); Li[3] = wsub(imul(b11r, b31i), imul(b11i, b31r));
     int mx[4]; unsigned vl[4];
 #pragma unroll
     for (int k = 0; k < 4; k++) {
         const unsigned base = k == 0 ? 0x00u : k == 1 ? 0x30u : k == 2 ? 0x10u : 0x20u;
-        const int ar = Lr[k] < 0 ? -Lr[k] : Lr[k], ai = Li[k] < 0 ? -Li[k] : Li[k];
-        if (ar > ai) { if (Lr[k] > 0) { mx[k] = Lr[k]; vl[k] = base; } else { mx[k] = -Lr[k]; vl[k] = base | 0x40u; } }
-        else         { if (Li[k] > 0) { mx[k] = Li[k]; vl[k] = base | 0xC0u; } else { mx[k] = -Li[k]; vl[k] = base | 0x80u; } }
+        const int ar = Lr[k] < 0 ? wneg(Lr[k]) : Lr[k], ai = Li[k] < 0 ? wneg(Li[k]) : Li[k];
+        if (ar > ai) { if (Lr[k] > 0) { mx[k] = Lr[k]; vl[k] = base; } else { mx[k] = wneg(Lr[k]); vl[k] = base | 0x40u; } }
+        else         { if (Li[k] > 0) { mx[k] = Li[k]; vl[k] = base | 0xC0u; } else { mx[k] = wneg(Li[k]); vl[k] = base | 0x80u; } }
     }
     CckPick p;
     if (mx[0] > mx[1]) { p.mx = mx[0]; p.val = vl[0]; } else { p.mx = mx[1]; p.val = vl[1]; }
@@ -58,8 +58,8 @@ __device__ __forceinline__ CckPick cck11_module(int a1r, int a1i, int a2r, int a
     return p;
 }
 __device__ __forceinline__ unsigned dqpsk_bits(S16 ref, S16 s) {              // barkerspread.hpp:430-437; bit0 | bit1<<1
-    const int re = ref.re * s.re + ref.im * s.im, im = ref.re * s.im - ref.im * s.re;
-    return ((unsigned)(re + im) >> 31) | (((unsigned)(re - im) >> 31) << 1);
+    const int re = wadd(ref.re * s.re, ref.im * s.im), im = wsub(ref.re * s.im, ref.im * s.re);     // after a CCK symbol `ref` is a raw chip: wraps at full scale
+    return ((unsigned)wadd(re, im) >> 31) | (((unsigned)wsub(re, im) >> 31) << 1);
 }
 
 struct Rx11bState {
@@ -235,14 +235,14 @@ __global__ void __launch_bounds__(64) k_rx11b(const uint32_t* __restrict__ iq, c
             auto corr = [&](int a00r, int a00i, int a01r, int a01i, int a10r, int a10i, int a11r, int a11i) -> int {
                 int b0r = a00r + a01r, b0i = -(a00i + a01i), b1r = a10r + a11r, b1i = a10i + a11i;
                 b0r >>= 2; b0i >>= 2; b1r >>= 2; b1i >>= 2;
-                return imul(b0r, b1r) - imul(b0i, b1i);
+                return wsub(imul(b0r, b1r), imul(b0i, b1i));
             };
             const int l1 = corr(I[0] + R[1], I[1] - R[0], I[2] - R[3], -(R[2] + I[3]), I[4] + R[5], I[5] - R[4], R[7] - I[6], R[6] + I[7]);
             const int l2 = corr(R[1] - I[0], R[0] + I[1], -(I[2] + R[3]), R[2] - I[3], R[5] - I[4], R[4] + I[5], I[6] + R[7], I[7] - R[6]);
             const unsigned b3 = hb ? 0x80u : 0x08u, b2 = hb ? 0x40u : 0x04u;
             int max1, max2; unsigned v1, v2;
-            if (l1 > 0) { max1 = l1; v1 = 0; } else { max1 = -l1; v1 = b3; }
-            if (l2 > 0) { max2 = l2; v2 = b2; } else { max2 = -l2; v2 = b2 | b3; }
+            if (l1 > 0) { max1 = l1; v1 = 0; } else { max1 = wneg(l1); v1 = b3; }
+            if (l2 > 0) { max2 = l2; v2 = b2; } else { max2 = wneg(l2); v2 = b2 | b3; }
             b |= max1 > max2 ? v1 : v2;
             b |= dqpsk_bits(s.last_symbol, q7) << (4 * hb);
             if (hb) b ^= 0x30u;
@@ -287,7 +287,7 @@ __global__ void __launch_bounds__(64) k_rx11b(const uint32_t* __restrict__ iq, c
                     S16 xv[4]; uint32_t pw = 0;
                     uint32_t w4[4]; ld4(x + p0, w4);
 #pragma unroll
-                    for (int k = 0; k < 4; k++) { xv[k] = s_sub(s_w(w4[k]), s.DC); pw += (uint32_t)((xv[k].re * xv[k].re + xv[k].im * xv[k].im) >> 5); }
+                    for (int k = 0; k < 4; k++) { xv[k] = s_sub(s_w(w4[k]), s.DC); pw += (uint32_t)(wadd(xv[k].re * xv[k].re, xv[k].im * xv[k].im) >> 5); }   // cca.hpp:65: pmaddwd wraps, psrad, hadd
                     s.avg_energy = s.avg_energy - s.win7 + pw;
                     s.win7 = s.win6; s.win6 = s.win5; s.win5 = s.win4; s.win4 = s.win3; s.win3 = s.win2; s.win2 = s.win1; s.win1 = s.win0; s.win0 = pw;
                     s.ed_count++;

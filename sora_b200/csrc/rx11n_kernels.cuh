@@ -84,19 +84,20 @@ static inline void build_host_tables11n(HostTables11n& H) {
     }
 }
 
-// dsp_math::atan(x, y) (dsp_math.h:166-212; the short overload :90-164 agrees wherever it does not overflow)
+// dsp_math::atan(x, y) (dsp_math.h:157-212; the short overload :90-164 agrees wherever it does not overflow).  abs, imax and the sums are
+// 32-bit int C there (dsp_math.h:64-88), which wraps: abs(INT_MIN) = INT_MIN, |x| + |y| wraps past 2^31.
 // SMALL: both arguments are int16 values (the pilot carriers), so (tmin << 16) + tmax / 2 fits 32 unsigned bits and the
 // quotient is the same as the reference's 64-bit one at a fifth of the instructions.
 template <bool SMALL = false>
 __device__ __forceinline__ int d_atan11n(const DevTables11n& N, int x, int y) {
     const int sign = (x ^ y) >> 31;
-    const int ax = (x ^ (x >> 31)) - (x >> 31), ay = (y ^ (y >> 31)) - (y >> 31);
-    const int tsign = (ax - ay) >> 31;
-    const int tsum = ax + ay; int d = ax - ay; d = (d ^ (d >> 31)) - (d >> 31);
-    const int tmax = (tsum + d) >> 1, tmin = tsum - tmax;
+    const int ax = wsub(x ^ (x >> 31), x >> 31), ay = wsub(y ^ (y >> 31), y >> 31);
+    const int tsign = wsub(ax, ay) >> 31;
+    const int tsum = wadd(ax, ay); int d = wsub(ax, ay); d = wsub(d ^ (d >> 31), d >> 31);
+    const int tmax = wadd(tsum, d) >> 1, tmin = wsub(tsum, tmax);
     int idx;
     if (SMALL) { const unsigned den = tmax ? (unsigned)tmax : 1u; idx = (int)((((unsigned)tmin << 16) + (den >> 1)) / den); }
-    else { long long num = (long long)tmin << 16, den = tmax; if (den == 0) den = 1; idx = (int)((num + (den >> 1)) / den); }
+    else { long long num = (long long)tmin * 65536, den = tmax; if (den == 0) den = 1; idx = (int)((num + (den >> 1)) / den); }
     idx >>= 4;
     if (idx < 0 || idx >= 4097) return 0;
     int srad = __ldg(N.atan_lut + idx);
@@ -150,7 +151,7 @@ __global__ void __launch_bounds__(128) k_sync11n(const uint32_t* __restrict__ iq
                 es[a] = wadd(es[a], wadd(e0, -e1)); es64[a] = wadd(es64[a], wadd(e2, -e3));        // autocorr.hpp:133-146; es64 = es as it was 64 samples ago
             }
             const long long cr = wadd(Rre[0] >> 1, Rre[1] >> 1), ci = wadd(Rim[0] >> 1, Rim[1] >> 1);
-            const long long acorr = cr * cr + ci * ci;
+            const long long acorr = (long long)((unsigned long long)(cr * cr) + (unsigned long long)(ci * ci));    // SquaredNorm(vci): paddq wraps (vector128.h:922-933)
             const long long e = wadd(es[0] >> 1, es[1] >> 1), energy = e * e;
             const long long h = wadd(es64[0] >> 1, es64[1] >> 1), hise = h * h;
             // eb = energy / (his_moving_energy + 1) > 5  <=>  energy / 6 >= his + 1; the first 64 entries hold LLONG_MAX (eb = 0)
@@ -220,7 +221,7 @@ __global__ void __launch_bounds__(64) k_sync11n_stream(const uint32_t* __restric
         hidx = (hidx + 1u) & 7u;
         for (int k = 0; k < 4; k++) {                                                   // cca_11n.hpp:62-118
             const long long cr = wadd(R_re[0][k] >> 1, R_re[1][k] >> 1), ci = wadd(R_im[0][k] >> 1, R_im[1][k] >> 1);
-            const long long acorr = cr * cr + ci * ci;
+            const long long acorr = (long long)((unsigned long long)(cr * cr) + (unsigned long long)(ci * ci));    // SquaredNorm(vci): paddq wraps
             const long long e = wadd(ve[0][k] >> 1, ve[1][k] >> 1), energy = e * e;
             const bool step = written >= 64u && energy / 6 >= S.ring[rindex] + 1;       // eb = energy / (his + 1) > 5; the ring starts at LLONG_MAX (eb = 0)
             if (!peak_found) {

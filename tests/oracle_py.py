@@ -27,13 +27,19 @@ def lib():
                 try:
                     if stale(): subprocess.check_call(["make", "-C", os.path.join(ROOT, "oracle")], stdout=subprocess.DEVNULL, stderr=subprocess.DEVNULL)
                 finally: fcntl.flock(lk, fcntl.LOCK_UN)
-        _LIB = C.CDLL(so)
-        _LIB.sbo_viterbi_block.restype = C.c_uint64
-        _LIB.sbo_uatan2.restype = C.c_int16; _LIB.sbo_usin.restype = C.c_int16; _LIB.sbo_ucos.restype = C.c_int16
-        _LIB.sbo_uatan2.argtypes = [C.c_int, C.c_int]; _LIB.sbo_usin.argtypes = [C.c_int16]; _LIB.sbo_ucos.argtypes = [C.c_int16]
-        _LIB.sbo_sts_pattern.restype = C.POINTER(C.c_int16)
-        _LIB.sbo_crc32.restype = C.c_uint32
-        _LIB.sbo_viterbi_signal.restype = C.c_uint32
+        use_library(so)
+    return _LIB
+
+def use_library(so):
+    """Bind the oracle library at path `so` (a build of oracle/ with other compiler flags, for instance) instead of oracle/libsora_oracle.so."""
+    global _LIB
+    _LIB = C.CDLL(so)
+    _LIB.sbo_viterbi_block.restype = C.c_uint64
+    _LIB.sbo_uatan2.restype = C.c_int16; _LIB.sbo_usin.restype = C.c_int16; _LIB.sbo_ucos.restype = C.c_int16
+    _LIB.sbo_uatan2.argtypes = [C.c_int, C.c_int]; _LIB.sbo_usin.argtypes = [C.c_int16]; _LIB.sbo_ucos.argtypes = [C.c_int16]
+    _LIB.sbo_sts_pattern.restype = C.POINTER(C.c_int16)
+    _LIB.sbo_crc32.restype = C.c_uint32
+    _LIB.sbo_viterbi_signal.restype = C.c_uint32
     return _LIB
 
 def _p(a, t=C.c_void_p):
