@@ -9,6 +9,7 @@
   --config tx11n     the 802.11n two-stream modulator on the device, MCS 8 / 9 / 10, 1500 B frames: the input of config #4 made on the device
   --config fir37     the legacy 802.11b transmit filter (BB11BPMDSpreadFIR4SSE) on the device
   --config tx11b_legacy  the legacy 802.11b transmitter (BB11BPMDPacketGenSignal: encoder + SSE filter, fused) on the device, 11 Mbps / 1500 B
+  --config tx11a_legacy  the legacy 802.11a transmitter (BB11ATxFrameMod) on the device, 54 Mbps / 1500 B, at 40 and at 44 Msps
   --config 11n       config #4: 802.11n HT-MF 2x2 RX chain at MCS 8, 9, 10, PSDU 1500 B, 2 x 40 Msps, fixed 2x2 channel
 
 Each prints one JSON line per measurement (same timing rules as bench.py: >= 3 warm-ups, CUDA events on the launch
@@ -371,6 +372,33 @@ def bench_tx11b_legacy(args):
             "parity": "equal to the oracle (restated encoder + filter) on the %d unique frames" % U})
     c.close()
 
+def bench_tx11a_legacy(args):
+    """The legacy 802.11a transmitter on the device: payload bytes in, the RCB-padded COMPLEX8 signal of BB11ATxFrameMod out (54 Mbps,
+    1500 B MPDUs), one row per sample rate (40 and 44 Msps)."""
+    import oracle_tx11a_legacy as O
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    F = args.frames; L = 1500; rate = 54000
+    rng = np.random.default_rng(12); U = 16
+    host = rng.integers(0, 256, (U, L)).astype(np.uint8)
+    d_pay = torch.from_numpy(host).to(dev).repeat((F + U - 1) // U, 1)[:F].contiguous()
+    d_off = torch.arange(F, dtype=torch.int64, device=dev) * L; d_len = torch.full((F,), L, dtype=torch.int32, device=dev)
+    d_pre = torch.from_numpy(O.preamble().copy()).to(dev)
+    for sr in (40, 44):
+        slot = O.padded_samples(L + 4, rate, sr)
+        d_out = torch.empty((F, slot, 2), dtype=torch.int8, device=dev); d_ns = torch.zeros(F, dtype=torch.int32, device=dev)
+        def step(): eng.tx11a_legacy_raw(d_pay.data_ptr(), F * L, d_off.data_ptr(), d_len.data_ptr(), F, rate, sr, 0, d_pre.data_ptr(), d_out.data_ptr(), slot, d_ns.data_ptr(), st.cuda_stream)
+        step(); torch.cuda.synchronize()
+        got = d_out[:U].cpu().numpy()
+        for i in range(U): assert (got[i] == O.modulate(host[i], rate, sr)).all(), "legacy 802.11a transmitter output differs from the oracle"
+        ms = c.timed(step, args.steps)
+        written = F * slot * 2.0
+        c.emit({"metric": "legacy 802.11a transmitter frames/s at %d Msps (bytes in, COMPLEX8 out)" % sr, "value": c.world * F / (ms * 1e-3), "unit": "frames/s", "ms_per_step": ms, "n_gpus": c.world,
+                "gb_per_s_written": written / (ms * 1e-3) / 1e9,
+                "config": {"workload": "BB11ATxFrameMod: 54 Mbps, 1500 B MPDU, %d Msps, RCB padded" % sr, "frames_per_step_per_gpu": F, "samples_per_frame": slot},
+                "roofline": {"bound": "compute", "achieved": written / (ms * 1e-3) / 1e9, "peak": peaks(), "unit": "GB/s", "frac": written / (ms * 1e-3) / 1e9 / peaks(), "note": "2 B per output sample written; the payload read is 1 B per 8 samples"},
+                "parity": "equal to the oracle on the %d unique frames" % U})
+    c.close()
+
 def bench_fir(args):
     """The anti-alias FIR decimator on a device-resident capture: the one streaming (HBM-bound) stage of the path; 6 B per input sample."""
     c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
@@ -394,10 +422,10 @@ def bench_fir(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy}[a.config](a)

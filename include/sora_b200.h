@@ -281,6 +281,23 @@ int sb200_tx11b_legacy_batch(sb200_handle* h, const uint8_t* payload, uint64_t p
                              uint32_t nframes, uint32_t rate_kbps, uint32_t short_preamble, uint32_t flags, uint32_t filter, int8_t* out,
                              uint64_t out_stride_samples, uint32_t* nsamples, void* cuda_stream);
 
+/* Legacy 802.11a transmitter: BB11ATxFrameMod / BB11ATxBufferMod6M (kernel/bb/dot11a/dot11/atx_fe.c, atx_tpl_imp.h:5-58, declared in
+ * kernel/inc/bb/bba.h:239-247) at SampleRate 40 or 44 — the caller's 640-sample preamble, SIGNAL, the data symbols (scrambler from 0xFF,
+ * the lutst/mapa_* constellation, pilots +-10720, IFFT64x with a wrapping << 2, a window that carries three samples into the next symbol),
+ * each 160-sample chunk upsampled afresh to 176 at 44 Msps (Upsample40MTo44M_160, with its one-sample over-read), Copy_NT (>> 6, int8
+ * saturation), the 8-sample tail, then zeros to a multiple of 128 bytes (ALIGN_WITH_RCB_BUFFER_PADDING_ZERO).  Frame i =
+ * payload[pay_off[i] .. +pay_len[i]) is the MPDU WITHOUT FCS; CRC-32 is appended, or, with flags SB200_TX11A_LEGACY_FCS_IN_PAYLOAD, the
+ * payload's last 4 bytes are sent verbatim as the FCS (BB11ATxFrameMod sends PACKET_BASE::Reserved1).  MPDU + FCS may be 4096 bytes, as
+ * atx_fe.c:23 admits; GetSignal then shifts LENGTH 4096 into the parity bit, and so does this.  preamble: the 640 COMPLEX16 samples of the
+ * reference's PREAMBLE40_11A_LUT (not part of this library; host or device; exactly 640 are read).  Slot i of `out` (out_stride_samples
+ * COMPLEX8 samples, a multiple of 8; out 16-byte aligned) receives nsamples[i] samples — the RCB-padded signal length, what
+ * SoraPacketSetSignalLength stores, divided by 2 — and zeros to the end of the slot.  SB200_E_INVALID for a rate that is not an 802.11a
+ * rate, a sample rate other than 40 / 44, MPDU + FCS over 4096 bytes, or a slot too small.  All pointers host or device. */
+#define SB200_TX11A_LEGACY_FCS_IN_PAYLOAD 1u
+int sb200_tx11a_legacy_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_total, const uint64_t* pay_off, const uint32_t* pay_len,
+                             uint32_t nframes, uint32_t rate_kbps, uint32_t sample_rate_mhz, uint32_t flags, const int16_t* preamble, int8_t* out,
+                             uint64_t out_stride_samples, uint32_t* nsamples, void* cuda_stream);
+
 /* 802.11n transmit, two spatial streams, HT-mixed format: the modulator graphs CreatePreambleGraph11n + CreateSigGraph11n + CreateModGraph11n
  * (kernel/bb/demod11/fb11nmod_config.hpp:74-171) driven like Test11N_FB_Mod (kernel/bb/demod11/fb11n_mod.cpp:44-70).  Frame i =
  * payload[pay_off[i] .. +pay_len[i]) is the MPDU WITHOUT FCS (CF_11nTxVector::crc32 is appended); mcs 8 .. 14 (the modulator graph's own

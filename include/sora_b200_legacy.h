@@ -168,6 +168,37 @@ HRESULT BB11BPMDPacketGenSignal(PPACKET_BASE pPacket, PDOT11B_PLCP_TXVECTOR pTxV
 void    SoraPacketGetTxSampleBuffer(PPACKET_BASE pPacket, PTXSAMPLE* ppBuffer, ULONG* pBufferSize);
 void    SoraPacketSetSignalLength(PPACKET_BASE pPacket, ULONG uLen);
 
+/* ---- 802.11a transmitter: kernel/inc/bb/bba.h:146-186 (BB11A_TX_VECTOR, DOT11A_RATE_*), :201-206, :239-247; kernel/bb/dot11a/dot11/atx_fe.c.
+ * Served by sb200_tx11a_legacy_batch on the same process-wide engine, at SampleRate 40 or 44.  Only the public fields of BB11A_TX_VECTOR keep
+ * their names; the reference's working buffers have no counterpart.  The 640-sample preamble table PREAMBLE40_11A_LUT is not part of this
+ * library: a caller hands it in once per process with BB11ATxSetPreamble (in the Sora tree: BB11ATxSetPreamble(PREAMBLE40_11A())).
+ * BB11ATxFrameMod sends the MDL chain and Reserved1 as the FCS, writes the signal and its zero padding to a multiple of 128 bytes into the
+ * packet's sample buffer and stores that length in bytes (SoraPacketSetSignalLength).  BB11AModulateACK writes the 14-byte ACK to RA at
+ * 6 Mbps into PhyACKBuffer (sized by the caller, as in the reference) and returns the padded length in bytes.  E_FAIL (SORA_E_FAIL) as in
+ * the reference (a rate code not in DOT11A_RATE_*, PacketSize + 4 > 4096), and, without writing anything, where the reference would assert
+ * or overrun (SampleRate other than 40 / 44, a sample buffer too small), when the MDL chain does not add up to PacketSize, without a GPU, and
+ * until BB11ATxSetPreamble was called; BB11AModulateACK returns 0 in those cases. */
+#define DOT11A_RATE_6M  0xB
+#define DOT11A_RATE_9M  0xF
+#define DOT11A_RATE_12M 0xA
+#define DOT11A_RATE_18M 0xE
+#define DOT11A_RATE_24M 0x9
+#define DOT11A_RATE_36M 0xD
+#define DOT11A_RATE_48M 0x8
+#define DOT11A_RATE_54M 0xC
+typedef struct _MAC_ADDRESS { UCHAR Address[6]; } MAC_ADDRESS, *PMAC_ADDRESS;   /* kernel/inc/dot11_pkt.h:35-39 */
+typedef struct _BB11A_TX_VECTOR {
+    unsigned int SampleRate;                    /* 40 or 44 (Msps) */
+    unsigned int ti_uiDataRate;                 /* DOT11A_RATE_* */
+    unsigned int ti_uiBufferLength;
+} BB11A_TX_VECTOR, *PBB11A_TX_VECTOR;
+
+void    BB11ATxContextInit(PBB11A_TX_VECTOR info, unsigned int SampleRate);
+HRESULT BB11ATxFrameMod(PBB11A_TX_VECTOR info, PPACKET_BASE pPacket);
+ULONG   BB11AModulateACK(unsigned int SampleRate, const PMAC_ADDRESS RecvMacAddress, void* PhyACKBuffer);
+/* not in the reference: the 640 COMPLEX16 samples of PREAMBLE40_11A_LUT, copied; process-wide; NULL forgets them */
+void    BB11ATxSetPreamble(const void* preamble640);
+
 #ifdef __cplusplus
 }
 #endif

@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -257,6 +257,34 @@ class Engine:
         out = np.zeros((len(lens), out_stride, 2), np.int8); ns = np.zeros(len(lens), np.uint32)
         self.tx11b_legacy_raw(_ptr(flat), max(int(lens.sum()), 1), _ptr(offs), _ptr(lens), len(lens), rate_kbps, int(bool(short_preamble)),
                               self.TX11B_LEGACY_FCS_IN_PAYLOAD if fcs_in_payload else 0, filter, _ptr(out), out_stride, _ptr(ns))
+        return out, ns
+
+    TX11A_LEGACY_FCS_IN_PAYLOAD = 1
+
+    def tx11a_legacy_raw(self, pay_ptr, pay_total, off_ptr, len_ptr, nframes, rate_kbps, sample_rate_mhz, flags, pre_ptr, out_ptr, out_stride, ns_ptr, stream=0):
+        self._check(self._lib.sb200_tx11a_legacy_batch(self._h, C.c_void_p(pay_ptr), C.c_uint64(pay_total), C.c_void_p(off_ptr), C.c_void_p(len_ptr), C.c_uint32(nframes),
+                                                       C.c_uint32(rate_kbps), C.c_uint32(sample_rate_mhz), C.c_uint32(flags), C.c_void_p(pre_ptr), C.c_void_p(out_ptr),
+                                                       C.c_uint64(out_stride), C.c_void_p(ns_ptr), C.c_void_p(stream)), "sb200_tx11a_legacy_batch")
+
+    @staticmethod
+    def tx11a_legacy_nsamples(psdu_len, rate_kbps, sample_rate_mhz=40):
+        """Samples BB11ATxFrameMod writes for a PSDU of psdu_len bytes (FCS included): the signal rounded up to 128 bytes."""
+        ndbps = {6000: 24, 9000: 36, 12000: 48, 18000: 72, 24000: 96, 36000: 144, 48000: 192, 54000: 216}.get(rate_kbps, 24)   # an unknown rate is the library's error
+        nsym = (22 + 8 * psdu_len + ndbps - 1) // ndbps
+        return ((176 if sample_rate_mhz == 44 else 160) * (5 + nsym) + 8 + 63) // 64 * 64
+
+    def tx11a_legacy_batch(self, payloads, rate_kbps, preamble, sample_rate_mhz=40, fcs_in_payload=False, out_stride=None):
+        """The legacy 802.11a transmitter (BB11ATxFrameMod).  payloads: list of uint8 arrays, MPDUs without FCS (or with it, fcs_in_payload=True);
+        preamble: the reference's 640-sample PREAMBLE40_11A_LUT, int16 [640, 2] -> (COMPLEX8 samples int8 [F, out_stride, 2], nsamples [F])."""
+        lens = np.array([len(p) for p in payloads], np.uint32); offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.uint64)
+        flat = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8) for p in payloads]) if lens.sum() else np.zeros(1, np.uint8))
+        pre = np.ascontiguousarray(preamble, dtype=np.int16)
+        if pre.size != 1280: raise Sb200Error("preamble must be 640 COMPLEX16 samples")
+        if out_stride is None:
+            out_stride = self.tx11a_legacy_nsamples(int(lens.max()) + (0 if fcs_in_payload else 4), rate_kbps, sample_rate_mhz)
+        out = np.zeros((len(lens), out_stride, 2), np.int8); ns = np.zeros(len(lens), np.uint32)
+        self.tx11a_legacy_raw(_ptr(flat), max(int(lens.sum()), 1), _ptr(offs), _ptr(lens), len(lens), rate_kbps, sample_rate_mhz,
+                              self.TX11A_LEGACY_FCS_IN_PAYLOAD if fcs_in_payload else 0, _ptr(pre), _ptr(out), out_stride, _ptr(ns))
         return out, ns
 
     def rxblocks_unpack(self, raw, left_shift=0):

@@ -323,3 +323,75 @@ extern "C" HRESULT BB11BPMDPacketGenSignal(PPACKET_BASE p, PDOT11B_PLCP_TXVECTOR
     SoraPacketSetSignalLength(p, nf * (ULONG)sizeof(TXSAMPLE));
     return SORA_S_OK;
 }
+
+// ---- the legacy 802.11a transmitter (bba.h:201-247, atx_fe.c) over sb200_tx11a_legacy_batch ------------------------------------------------
+namespace {
+std::mutex g_pre_mu; bool g_pre_set = false; int16_t g_pre[1280];
+uint32_t kbps_of_11a(unsigned int c) {
+    switch (c) { case 0xB: return 6000; case 0xF: return 9000; case 0xA: return 12000; case 0xE: return 18000;
+                 case 0x9: return 24000; case 0xD: return 36000; case 0x8: return 48000; case 0xC: return 54000; default: return 0; }
+}
+uint32_t nsamples_11a(uint32_t size, uint32_t kbps, unsigned int sr) {   // GetSignalBytes (atx_tpl.h:69-83) / 2, rounded up to 128 bytes
+    const uint32_t ndbps = kbps / 250u, nsym = (22u + 8u * size + ndbps - 1u) / ndbps;
+    return ((sr == 44 ? 176u : 160u) * (5u + nsym) + 8u + 63u) & ~63u;
+}
+// modulate psdu (FCS included) into dst, which holds at least cap_bytes; *n = padded samples
+bool tx11a(const std::vector<uint8_t>& psdu, uint32_t kbps, unsigned int sr, void* dst, size_t cap_bytes, uint32_t* n) {
+    if (!kbps || (sr != 40 && sr != 44) || psdu.size() < 4 || psdu.size() > 4096 || !dst) return false;
+    const uint32_t ns = nsamples_11a((uint32_t)psdu.size(), kbps, sr);
+    if ((size_t)ns * 2 > cap_bytes) return false;
+    void* buf = nullptr;
+    if (posix_memalign(&buf, 16, (size_t)ns * 2) != 0) return false;
+    int16_t pre[1280];
+    {   std::lock_guard<std::mutex> lk(g_pre_mu);
+        if (!g_pre_set) { free(buf); return false; }
+        memcpy(pre, g_pre, sizeof pre); }
+    const uint64_t off = 0; const uint32_t len = (uint32_t)psdu.size(); uint32_t got = 0;
+    int rc;
+    {   std::lock_guard<std::mutex> lk(g_fir_mu);
+        rc = fir_engine() ? sb200_tx11a_legacy_batch(g_fir_engine, psdu.data(), len, &off, &len, 1, kbps, sr, SB200_TX11A_LEGACY_FCS_IN_PAYLOAD, pre,
+                                                     (int8_t*)buf, ns, &got, nullptr) : SB200_E_NODEVICE; }
+    const bool ok = rc == SB200_OK && got == ns;
+    if (ok) memcpy(dst, buf, (size_t)ns * 2);
+    free(buf);
+    if (ok) *n = ns;
+    return ok;
+}
+}
+
+extern "C" void BB11ATxSetPreamble(const void* p) {
+    std::lock_guard<std::mutex> lk(g_pre_mu);
+    g_pre_set = p != nullptr;
+    if (p) memcpy(g_pre, p, sizeof g_pre);
+}
+extern "C" void BB11ATxContextInit(PBB11A_TX_VECTOR info, unsigned int SampleRate) {   // a_init.c:61-86: the data rate is left as it is
+    if (!info) return;
+    info->SampleRate = SampleRate; info->ti_uiBufferLength = 0;
+}
+extern "C" HRESULT BB11ATxFrameMod(PBB11A_TX_VECTOR info, PPACKET_BASE p) {
+    if (!info || !p) return SORA_E_FAIL;
+    if (p->PacketSize + 4u > 4096u) return SORA_E_FAIL;                                    // atx_fe.c:23
+    const uint32_t kbps = kbps_of_11a(info->ti_uiDataRate);
+    if (!kbps) return SORA_E_FAIL;                                                          // atx_fe.c:59-62
+    std::vector<uint8_t> psdu; std::vector<uint8_t*> where;
+    if (!packet_bytes(p, psdu, where)) return SORA_E_FAIL;                                  // MDL chain + Reserved1 (atx_tpl.h:24-46)
+    PTXSAMPLE sb = nullptr; ULONG sb_size = 0;
+    SoraPacketGetTxSampleBuffer(p, &sb, &sb_size);
+    uint32_t n = 0;
+    if (!tx11a(psdu, kbps, info->SampleRate, sb, sb_size, &n)) return SORA_E_FAIL;
+    SoraPacketSetSignalLength(p, n * (ULONG)sizeof(TXSAMPLE));
+    return SORA_S_OK;
+}
+extern "C" ULONG BB11AModulateACK(unsigned int SampleRate, const PMAC_ADDRESS ra, void* out) {
+    if (!ra || !out) return 0;
+    std::vector<uint8_t> ack = {0xD4, 0x00, 0x00, 0x00};                                  // FrameControl: ACK, control; Duration 0 (atx_fe.c:181-184)
+    ack.insert(ack.end(), ra->Address, ra->Address + 6);
+    uint32_t c = 0xFFFFFFFFu;
+    for (uint8_t b : ack) { c ^= b; for (int k = 0; k < 8; k++) c = (c & 1u) ? (c >> 1) ^ 0xEDB88320u : c >> 1; }
+    c = ~c;
+    for (int i = 0; i < 4; i++) ack.push_back((uint8_t)(c >> (8 * i)));
+    // BB11ATxBufferMod6M: 6 Mbps whatever ti_uiDataRate says (the reference sets DOT11A_RATE_24M and never reads it there)
+    uint32_t n = 0;
+    if (!tx11a(ack, 6000, SampleRate, out, (size_t)nsamples_11a(14, 6000, SampleRate) * 2, &n)) return 0;
+    return n * (ULONG)sizeof(TXSAMPLE);
+}

@@ -8,6 +8,7 @@
 #include "tx11a_kernels.cuh"
 #include "tx11b_kernels.cuh"
 #include "tx11b_legacy_kernels.cuh"
+#include "tx11a_legacy_kernels.cuh"
 #include "tx11n_kernels.cuh"
 #include "fir_kernels.cuh"
 #include <stdlib.h>
@@ -168,7 +169,7 @@ struct sb200_handle {
     double gather_ms = 0.0;                            // host_decimate: time the host threads spent gathering during the last call (SB200_TRACE prints it)
     uint32_t ht_mcs_limit = 11;                        // first MCS the 802.11n HT-SIG parser refuses (PHY_11n.hpp:497); option "ht_mcs_limit"
     DevBuf soff, slen, spos, snev, sev;                // continuous-capture scout: current slot of every capture, position, event count, event list
-    DevTablesTx X{}; DevBuf tabtx, txpay, txoff, txlen, txseed, txout, txns, txdesc, cca11n, ccaidx, tabtx11n, txout1; DevTablesTx11n XN{};   // 802.11a transmit tables (built on first use) and staging
+    DevTablesTx X{}; DevBuf tabtx, txpay, txoff, txlen, txseed, txout, txns, txdesc, cca11n, ccaidx, tabtx11n, txout1, txpre; DevTablesTx11n XN{};   // 802.11a transmit tables (built on first use) and staging
     DevTables11n N{}; DevBuf tab11n, iq1;              // 802.11n tables (uploaded on first use) and the second antenna's samples
     std::vector<uint64_t> offh; std::vector<uint32_t> lenh;   // host copy of the slot table (cached for device-resident tables)
     const uint64_t* tab_off = nullptr; const uint32_t* tab_len = nullptr; uint32_t tab_n = 0, tab_max_len = 0; uint64_t tab_total = 0; bool tab_host = false;
@@ -281,7 +282,7 @@ extern "C" void sb200_destroy(sb200_handle* h) {
     DevBuf* all[] = {&h->tab, &h->iq, &h->off, &h->len, &h->info, &h->soft, &h->out, &h->status, &h->crc, &h->res,
                      &h->taps[0], &h->taps[1], &h->taps[2], &h->taps[3], &h->taps[4], &h->vlist, &h->vcnt, &h->slotchk, &h->doff};
     for (DevBuf* b : all) b->release();
-    h->iq40.release(); h->off40.release(); h->len40.release(); h->dcbuf.release(); h->vring.release(); h->soff.release(); h->slen.release(); h->spos.release(); h->snev.release(); h->sev.release(); h->tab11n.release(); h->iq1.release(); h->tabtx.release(); h->txpay.release(); h->txoff.release(); h->txlen.release(); h->txseed.release(); h->txout.release(); h->txns.release(); h->txdesc.release(); h->cca11n.release(); h->ccaidx.release(); h->tabtx11n.release(); h->txout1.release();
+    h->iq40.release(); h->off40.release(); h->len40.release(); h->dcbuf.release(); h->vring.release(); h->soff.release(); h->slen.release(); h->spos.release(); h->snev.release(); h->sev.release(); h->tab11n.release(); h->iq1.release(); h->tabtx.release(); h->txpay.release(); h->txoff.release(); h->txlen.release(); h->txseed.release(); h->txout.release(); h->txns.release(); h->txdesc.release(); h->cca11n.release(); h->ccaidx.release(); h->tabtx11n.release(); h->txout1.release(); h->txpre.release();
     if (h->ev0) cudaEventDestroy(h->ev0);
     if (h->ev1) cudaEventDestroy(h->ev1);
     for (int i = 0; i < 5; i++) if (h->evk[i]) cudaEventDestroy(h->evk[i]);
@@ -1372,6 +1373,71 @@ extern "C" int sb200_tx11b_legacy_batch(sb200_handle* h, const uint8_t* payload,
     else k_tx11b_legacy_spread<2><<<grid, SB_TX11B_LEGACY_THREADS, 0, st>>>(d_len, job, dd, d_out, out_stride_samples, d_ns);
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 0; h->launches += 2;
+    CK(cudaGetLastError());
+    bool sync = false;
+    if (!out_dev) { CK(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st)); sync = true; }
+    if (nsamples && !ns_dev) { CK(cudaMemcpyAsync(nsamples, d_ns, nframes * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
+    if (sync) CK(cudaStreamSynchronize(st));
+    return SB200_OK;
+}
+
+// Legacy 802.11a transmitter (tx11a_legacy_kernels.cuh): BB11ATxFrameMod / BB11ATxBufferMod6M at SampleRate 40 or 44.
+extern "C" int sb200_tx11a_legacy_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_total, const uint64_t* pay_off, const uint32_t* pay_len,
+                                        uint32_t nframes, uint32_t rate_kbps, uint32_t sample_rate_mhz, uint32_t flags, const int16_t* preamble, int8_t* out,
+                                        uint64_t out_stride_samples, uint32_t* nsamples, void* cuda_stream) {
+    if (!h || !payload || !pay_off || !pay_len || !out || !preamble) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
+    if (flags & ~SB200_TX11A_LEGACY_FCS_IN_PAYLOAD) return h->fail(SB200_E_INVALID, "unknown flags");
+    if (sample_rate_mhz != 40 && sample_rate_mhz != 44) return h->fail(SB200_E_INVALID, "sample_rate_mhz must be 40 or 44");
+    if (out_stride_samples % 8u || ((uintptr_t)out & 15u)) return h->fail(SB200_E_INVALID, "out must be 16-byte aligned and out_stride_samples a multiple of 8");
+    if (nframes == 0) return SB200_OK;
+    static const struct { uint32_t kbps, code, nbpsc, cr, ndbps; } R[8] = {{6000, 0xB, 1, CR_12, 24}, {9000, 0xF, 1, CR_34, 36}, {12000, 0xA, 2, CR_12, 48}, {18000, 0xE, 2, CR_34, 72},
+        {24000, 0x9, 4, CR_12, 96}, {36000, 0xD, 4, CR_34, 144}, {48000, 0x8, 6, CR_23, 192}, {54000, 0xC, 6, CR_34, 216}};          // bba.h:179-186, atx.h:20-57
+    int ri = -1; for (int i = 0; i < 8; i++) if (R[i].kbps == rate_kbps) ri = i;
+    if (ri < 0) return h->fail(SB200_E_INVALID, "rate_kbps is not an 802.11a rate");
+    Tx11aLegacyJob job{};
+    job.rate_code = R[ri].code; job.nbpsc = R[ri].nbpsc; job.code_rate = R[ri].cr; job.ndbps = R[ri].ndbps;
+    job.sr44 = sample_rate_mhz == 44; job.fcs_in_payload = (flags & SB200_TX11A_LEGACY_FCS_IN_PAYLOAD) ? 1u : 0u;
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    CK(cudaSetDevice(h->device));
+    int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
+    std::vector<uint64_t> offh(nframes); std::vector<uint32_t> lenh(nframes);
+    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len), pay_dev = is_device_ptr(payload), out_dev = is_device_ptr(out), pre_dev = is_device_ptr(preamble);
+    if (off_dev) CK(cudaMemcpyAsync(offh.data(), pay_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), pay_off, nframes * 8ull);
+    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), pay_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), pay_len, nframes * 4ull);
+    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    uint32_t max_nsym = 0;
+    for (uint32_t i = 0; i < nframes; i++) {
+        if (job.fcs_in_payload && lenh[i] < 4u) return h->fail(SB200_E_INVALID, "with SB200_TX11A_LEGACY_FCS_IN_PAYLOAD every payload carries its 4 FCS bytes");
+        const uint32_t size = job.fcs_in_payload ? lenh[i] : lenh[i] + 4u;                // PSDU bytes, FCS included
+        if (lenh[i] > 4096u || size > 4096u || lenh[i] > payload_total || offh[i] > payload_total - lenh[i]) return h->fail(SB200_E_INVALID, "payload slot out of range (MPDU + FCS at most 4096 bytes)");
+        const uint32_t ns = tx11a_legacy_nsym(size, job.ndbps);
+        if (tx11a_legacy_padded(ns, job.sr44) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
+        if (ns > max_nsym) max_nsym = ns;
+    }
+    job.runs = (1u + max_nsym + SB_TXL_RUN - 1u) / SB_TXL_RUN;
+    const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len; const uint32_t* d_pre;
+    if (pay_dev) d_pay = payload; else { CK(h->txpay.need(payload_total + 1)); CK(cudaMemcpyAsync(h->txpay.p, payload, payload_total, cudaMemcpyHostToDevice, st)); d_pay = (const uint8_t*)h->txpay.p; }
+    if (off_dev) d_off = pay_off; else { CK(h->txoff.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->txoff.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); d_off = (const uint64_t*)h->txoff.p; }
+    if (len_dev) d_len = pay_len; else { CK(h->txlen.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->txlen.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); d_len = (const uint32_t*)h->txlen.p; }
+    if (pre_dev && ((uintptr_t)preamble & 3u) == 0) d_pre = (const uint32_t*)preamble;
+    else { CK(h->txpre.need(640 * 4)); CK(cudaMemcpyAsync(h->txpre.p, preamble, 640 * 4, pre_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st)); d_pre = (const uint32_t*)h->txpre.p; }
+    const size_t out_bytes = (size_t)nframes * out_stride_samples * 2;
+    int8_t* d_out = out; if (!out_dev) { CK(h->txout.need(out_bytes)); d_out = (int8_t*)h->txout.p; }
+    uint32_t* d_ns = nullptr; const bool ns_dev = nsamples && is_device_ptr(nsamples);
+    if (nsamples) { if (ns_dev) d_ns = nsamples; else { CK(h->txns.need(nframes * 4ull)); d_ns = (uint32_t*)h->txns.p; } }
+    const unsigned helpers = 4;                          // warps per frame for the preamble and the zero fill
+    const uint64_t ny = (job.runs + helpers + SB_TXL_WARPS - 1) / SB_TXL_WARPS;
+    if (ny > 65535u) return h->fail(SB200_E_INVALID, "too many symbols per frame");
+    CK(cudaEventRecord(h->ev0, st));
+    const uint32_t* d_crc = nullptr;
+    if (!job.fcs_in_payload) {
+        CK(h->crc.need(nframes * 4ull));
+        k_tx11a_crc<<<(nframes + 127) / 128, 128, 0, st>>>(d_pay, d_off, d_len, nframes, h->T, (uint32_t*)h->crc.p);
+        d_crc = (const uint32_t*)h->crc.p; h->launches += 1;
+    }
+    k_tx11a_legacy<<<dim3(nframes, (unsigned)ny), 32 * SB_TXL_WARPS, 0, st>>>(d_pay, d_off, d_len, nframes, job, h->T, h->X, h->inv_deint, d_crc, d_pre, d_out, out_stride_samples, d_ns);
+    CK(cudaEventRecord(h->ev1, st));
+    h->timed = true; h->nk = 0; h->launches += 1;
     CK(cudaGetLastError());
     bool sync = false;
     if (!out_dev) { CK(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st)); sync = true; }
