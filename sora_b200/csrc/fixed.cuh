@@ -7,7 +7,9 @@
 // complement) and are checked bit-for-bit against the SSE oracle by tests/test_gpu_stages.py.
 #pragma once
 #include <stdint.h>
+#ifndef SB_HOST_EMU                  // tests/cpp/packed_emu.cpp compiles this header for the host with the intrinsics written out
 #include <cuda_runtime.h>
+#endif
 
 namespace sb {
 
@@ -71,6 +73,59 @@ __host__ __device__ __forceinline__ void dft4(cs16& v0, cs16& v1, cs16& v2, cs16
     cs16 s0 = adds(x0, x2), s1 = adds(x1, x3), s2 = adds(cnot(x2), x0), s3 = adds(cnot(x3), x1);
     cs16 t3 = mk(s3.im, ~s3.re);                      // lane 3 times -j (swap, then complement the new im)
     v0 = adds(s0, s1); v1 = adds(cnot(s1), s0); v2 = adds(s2, t3); v3 = adds(cnot(t3), s2);
+}
+
+// ------------------------------------------------------------------------------------------------
+// Packed forms: one complex int16 per 32-bit word, re in bits 0-15, im in bits 16-31 (the layout of pack()), on the 16x2 SIMD
+// integer instructions.  Each one states when it equals its scalar counterpart above; tests/test_cpu_packed.py checks that on the
+// host, exhaustively or on random and edge words.
+// ------------------------------------------------------------------------------------------------
+// paddw / psubw: per-half wrap-around.  Equal to adds / subs wherever the exact sum lies in [-32768, 32767].
+__device__ __forceinline__ uint32_t pk_add(uint32_t a, uint32_t b) { return __vadd2(a, b); }
+__device__ __forceinline__ uint32_t pk_sub(uint32_t a, uint32_t b) { return __vsub2(a, b); }
+// sra(a, N), any input: logical shift, clear the bits the high half pushed into the low one, sign-extend each half from bit 15 - N
+// as (t ^ s) - s, the subtraction written as the add of -s (16x2 adds take no negated operand)
+template <int N> __device__ __forceinline__ uint32_t pk_sra(uint32_t a) {
+    const uint32_t m = (0xFFFFu >> N) * 0x10001u, s = (0x8000u >> N) * 0x10001u, ns = (0x10000u - (0x8000u >> N)) * 0x10001u;
+    return __vadd2(((a >> N) & m) ^ s, ns);
+}
+__device__ __forceinline__ uint32_t pk_mulj(uint32_t a) { return __byte_perm(a, 0, 0x1032) ^ 0x0000FFFFu; }    // mulj: (~im, re), any input
+__device__ __forceinline__ uint32_t pk_mulmj(uint32_t a) { return __byte_perm(a, 0, 0x1032) ^ 0xFFFF0000u; }   // (im, ~re): dft4's t3, any input
+// Factor of a complex product a * b whose components are then taken as sx16(x >> S): b's halves pre-multiplied by 2^(16 - S), `nim` being
+// what a.im is multiplied by in the real part.  The 32-bit wrapped sum a.re * (re << (16 - S)) + a.im * (nim << (16 - S)) is
+// x << (16 - S) mod 2^32, whose high half is bits S..S+15 of x, i.e. sx16(x >> S): one PRMT repacks both components.  Exact for any input.
+struct cfac { int re, im, nim; };
+template <int S> __device__ __forceinline__ cfac mkfac(int re, int im, int nim) { return cfac{re * (1 << (16 - S)), im * (1 << (16 - S)), nim * (1 << (16 - S))}; }
+__device__ __forceinline__ cfac fac_q15(cs16 b) { return mkfac<15>(b.re, b.im, neg16(b.im)); }        // cmul_q15(a, b)
+__device__ __forceinline__ cfac fac_tw(cs16 w) { return mkfac<15>(w.re, w.im, (int)(short)~w.im); }   // cmul_tw(a, w)
+__device__ __forceinline__ cfac fac_mul8(cs16 b) { return mkfac<8>(b.re, b.im, neg16(b.im)); }        // cmul32(a, b) >> 8, sx16
+__device__ __forceinline__ uint32_t pk_cmul(int re, int im, cfac f) {
+    const uint32_t x = (uint32_t)re * (uint32_t)f.re + (uint32_t)im * (uint32_t)f.nim, y = (uint32_t)re * (uint32_t)f.im + (uint32_t)im * (uint32_t)f.re;
+    return __byte_perm(x, y, 0x7632);
+}
+__device__ __forceinline__ uint32_t pk_cmul(uint32_t a, cfac f) { return pk_cmul((int)(short)a, (int)a >> 16, f); }
+// The demapper's index byte per half, (uint8)min(max(v >> 4, -128), 127): >> 4 is monotone and maps -2048 / 2047 to -128 / 127, so
+// clamping v to [-2048, 2047] first gives the same value, and its bits 4..11 are that byte.  Any input; re's byte in bits 4..11, im's in 20..27.
+__device__ __forceinline__ uint32_t pk_demap_clamp(uint32_t a) { return __vmins2(__vmaxs2(a, 0xF800F800u), 0x07FF07FFu); }
+
+// r4_butterfly on packed words.  After the >> 2 every component lies in [-8192, 8191]: ac, bd in [-16384, 16382], a_c, b_d in
+// [-16383, 16383], jbd in [-16384, 16383]; so ac +- bd and a_c -+ jbd lie in [-32768, 32767] and every saturating add of the scalar
+// butterfly is a wrap-around one here.
+__device__ __forceinline__ void pk_r4_butterfly(uint32_t& a, uint32_t& b, uint32_t& c, uint32_t& d, const cfac& w1, const cfac& w2, const cfac& w3) {
+    a = pk_sra<2>(a); b = pk_sra<2>(b); c = pk_sra<2>(c); d = pk_sra<2>(d);
+    const uint32_t ac = pk_add(a, c), bd = pk_add(b, d), a_c = pk_sub(a, c), b_d = pk_sub(b, d), jbd = pk_mulj(b_d);
+    a = pk_add(ac, bd);
+    b = pk_cmul(pk_sub(ac, bd), w2);
+    c = pk_cmul(pk_sub(a_c, jbd), w1);
+    d = pk_cmul(pk_add(a_c, jbd), w3);
+}
+// dft4 on packed words.  x in [-8192, 8191] after the >> 2; s0, s1, s2 = x0 - x2 - 1, s3 in [-16384, 16382]; t3, ~s1, ~t3 in
+// [-16384, 16383]; every output sum lies in [-32768, 32765], so again no saturating add can clip.
+__device__ __forceinline__ void pk_dft4(uint32_t& v0, uint32_t& v1, uint32_t& v2, uint32_t& v3) {
+    const uint32_t x0 = pk_sra<2>(v0), x1 = pk_sra<2>(v1), x2 = pk_sra<2>(v2), x3 = pk_sra<2>(v3);
+    const uint32_t s0 = pk_add(x0, x2), s1 = pk_add(x1, x3), s2 = pk_add(~x2, x0), s3 = pk_add(~x3, x1);
+    const uint32_t t3 = pk_mulmj(s3);
+    v0 = pk_add(s0, s1); v1 = pk_add(~s1, s0); v2 = pk_add(s2, t3); v3 = pk_add(~t3, s2);
 }
 
 } // namespace sb
