@@ -182,7 +182,8 @@ int sb200_rx11b_streams(sb200_handle* h, const int16_t* iq, uint64_t iq_total_sa
  * I,Q), both host or both device; slot i covers samples [frame_off[i], frame_off[i]+frame_len[i]) of BOTH captures. */
 typedef struct sb200_frame_result_11n {
     uint32_t status;        /* SB200_FRAME_* */
-    uint32_t mcs;           /* CF_HTRxVector::ht_frame_mcs */
+    uint32_t mcs;           /* CF_HTRxVector::ht_frame_mcs.  It has no reset: when the L-SIG is refused before HT-SIG is parsed, a
+                             * capture of sb200_rx11n_streams reports its previous event's value (0 for the first), a batch slot 0 */
     uint32_t length;        /* CF_11aRxVector::frame_length: HT LENGTH once HT-SIG parsed, else 2 x L-SIG LENGTH, else 0 */
     uint32_t crc32;         /* received FCS */
     uint32_t nsym;          /* CF_11aRxVector::total_symbols: data symbols + 4 (PHY_11n.hpp:508) */

@@ -108,7 +108,7 @@ void Rx11n::init() {
     for (int i = 0; i < 64; i++) { his_moving_energy[i] = LLONG_MAX; his_valid[i] = false; }       // cca_11n.hpp:153
     his_index = 0;
     mem_sample_index = 0; vec20_count = 0; detect_index = 0; ds_n = 0;
-    vfo_d = 0; vfo_theta = 0; vfo_n = 0; CFO_est = 0; ht_frame_length = 0; ht_frame_mcs = 0; lsig_len2 = 0;
+    vfo_d = 0; vfo_theta = 0; vfo_n = 0; CFO_est = 0; ht_frame_length = 0; ht_frame_mcs = 0;   // CF_HTRxVector has no Reset(): carried across events
     memset(siso_ch, 0, sizeof siso_ch); memset(hinv, 0, sizeof hinv);
     reset_after_event();
 }
@@ -118,7 +118,8 @@ void Rx11n::reset_carrier_sense() {                    // BB11nDemodContext::Res
 }
 void Rx11n::reset_after_event() {                      // ssrc->Flush(); ctx.Reset(); ssrc->Reset()  (fb11n_demod.cpp:64-70)
     reset_carrier_sense();
-    frame_length = 0; total_symbols = 0; remain_symbols = 0; data_rate_kbps = 6000; code_rate = CR_12; frame_crc32 = 0;
+    frame_length = 0; total_symbols = 0; remain_symbols = 0; data_rate_kbps = 6000; code_rate = CR_12; frame_crc32 = 0;   // CF_11aRxVector::Reset()
+    lsig_len2 = 0;                                      // the L-SIG length is frame_length before the HT-SIG overwrites it: zero again when L-SIG is refused
     ds_n = 0; lltf_n = sym_n = sig_n = htltf_n = 0;
     vit.max_steps = 5000 * 8; vit.reset(); ob_count = 0; vit_in.clear(); vit_out.assign(256, 0);
     desc_count = 0; desc_reg = 0; byte_count = 0; crc_run = 0xFFFFFFFFu;

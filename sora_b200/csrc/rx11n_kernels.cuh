@@ -36,6 +36,9 @@ struct DevTables11n {
     const uint8_t*  demap64;    // [3][288] dsp_demap.h lookup_table_64qam1..3, entry 144 = value 0 (data)
     uint32_t mcs_limit;         // first MCS index the HT-SIG parser refuses: 11 as the reference ships it (PHY_11n.hpp:497), 15 with the QAM branches enabled
 };
+// FrameInfo::rate_kbps of an event whose HT-SIG was never parsed.  CF_HTRxVector has no Reset() (ieee80211facade.hpp:269-272), so the
+// reference then still holds the previous event's ht_frame_mcs: the stream driver substitutes it, a batch slot (a fresh context) reports 0.
+constexpr uint32_t MCS11N_UNPARSED = 0xFFFFFFFFu;
 struct HostTables11n {
     uint32_t sincos[65536]; int16_t atan_lut[4097]; uint8_t demap[256], crc8[256], pos[2][2][104], lltf_pos[64], htltf_pos[64];
     uint16_t pos16[2][2][312]; uint8_t demap16[2][256], demap64[3][288];
@@ -450,7 +453,7 @@ __global__ void __launch_bounds__(32 * SB_FRONT11N_WARPS, SB_FRONT11N_MINB) k_fr
         put(m0, ds0); put(m1, ds1);
         __syncwarp();
     }
-    uint32_t mcs = 0, frame_length = 0, total_symbols = 0, lsig_len2 = 0, code_rate = CR_12;
+    uint32_t mcs = MCS11N_UNPARSED, frame_length = 0, total_symbols = 0, lsig_len2 = 0, code_rate = CR_12;
     if (status == E_SUCCESS) {                         // T11nViterbiSig (viterbi.hpp:53-99) + T11nSigParser (PHY_11n.hpp:402-514)
         const uint32_t lsig = (uint32_t)warp_viterbi_sig_n<24>(sb, lane, s_dec[wib]);
         const unsigned long long ht = warp_viterbi_sig_n<48>(sb + 48, lane, s_dec[wib]);

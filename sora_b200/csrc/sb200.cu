@@ -882,13 +882,13 @@ static int upload_tables11n(sb200_handle* h) {
 }
 
 __global__ void k_pack_results11n(const FrameInfo* __restrict__ info, const uint32_t* __restrict__ status, const uint32_t* __restrict__ crc, uint32_t n,
-                                  sb200_frame_result_11n* __restrict__ res) {
+                                  bool keep_unparsed, sb200_frame_result_11n* __restrict__ res) {
     uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= n) return;
     FrameInfo fi = info[i];
     sb200_frame_result_11n r;
     const bool decoded = fi.status == E_SUCCESS;
-    r.status = decoded ? status[i] : fi.status; r.mcs = fi.rate_kbps; r.length = fi.length; r.crc32 = decoded ? crc[i] : 0u; r.nsym = fi.nsym_total;
+    r.status = decoded ? status[i] : fi.status; r.mcs = fi.rate_kbps == MCS11N_UNPARSED && !keep_unparsed ? 0u : fi.rate_kbps; r.length = fi.length; r.crc32 = decoded ? crc[i] : 0u; r.nsym = fi.nsym_total;
     r.detect_index = fi.detect_vec == 0xFFFFFFFFu ? 0u : fi.detect_vec * 4u;
     r.cfo_est = (int16_t)fi.cfo_est; r.lsig_length = (uint16_t)fi.peak_index;
     res[i] = r;
@@ -949,7 +949,7 @@ static int rx11n_run(sb200_handle* h, const int16_t* iq0, const int16_t* iq1, ui
     CK(cudaEventRecord(h->evk[3], st));
     const bool res_dev = is_device_ptr(res);
     sb200_frame_result_11n* d_res = res_dev ? res : (sb200_frame_result_11n*)h->res.p;
-    k_pack_results11n<<<(nframes + 255) / 256, 256, 0, st>>>(d_info, (const uint32_t*)h->status.p, (const uint32_t*)h->crc.p, nframes, d_res);
+    k_pack_results11n<<<(nframes + 255) / 256, 256, 0, st>>>(d_info, (const uint32_t*)h->status.p, (const uint32_t*)h->crc.p, nframes, state_idx != nullptr, d_res);
     CK(cudaEventRecord(h->evk[4], st)); CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 4; h->launches += 5;
     CK(cudaGetLastError());
@@ -986,6 +986,7 @@ extern "C" int sb200_rx11n_streams(sb200_handle* h, const int16_t* iq0, const in
     }
     CK(h->cca11n.need((size_t)nstreams * sizeof(Cca11nState))); CK(cudaMemsetAsync(h->cca11n.p, 0, (size_t)nstreams * sizeof(Cca11nState), st));   // TCCA11n / MimoAutoCorr constructors
     std::vector<uint64_t> pos(nstreams, 0);
+    std::vector<uint32_t> last_mcs(nstreams, 0);      // CF_HTRxVector::ht_frame_mcs of each capture: never reset between events
     std::vector<uint32_t> active(nstreams); for (uint32_t s = 0; s < nstreams; s++) active[s] = s;
     std::vector<uint64_t> off; std::vector<uint32_t> len, idx; std::vector<sb200_frame_result_11n> r; std::vector<uint8_t> bytes;
     const uint32_t row = out_bytes ? (out_stride < 1536u ? out_stride : 1536u) : 0u;
@@ -1011,6 +1012,8 @@ extern "C" int sb200_rx11n_streams(sb200_handle* h, const int16_t* iq0, const in
             const uint64_t v_last = e20 / 4ull - 1ull, blk = (8ull * v_last + 7ull) / 28ull;
             pos[s] += (blk + 1ull) * 28ull;                                                   // the driver sees the event after that source block
             const size_t slot = (size_t)s * max_frames + nframes_out[s];
+            if (r[j].mcs == MCS11N_UNPARSED) r[j].mcs = last_mcs[s];
+            last_mcs[s] = r[j].mcs;
             res[slot] = r[j];
             if (sample_index) sample_index[slot] = (uint32_t)pos[s];
             if (row) memcpy(out_bytes + slot * out_stride, bytes.data() + (size_t)j * row, row);

@@ -122,9 +122,15 @@ def psdu_with_fcs(payload):
     fcs = zlib.crc32(payload.tobytes()) & 0xFFFFFFFF
     return np.concatenate([payload, np.frombuffer(fcs.to_bytes(4, "little"), np.uint8)])
 
-def modulate(psdus, rate_kbps=54000, scramble_seeds=None, window=True):
-    """psdus: uint8 [F, L] (L bytes each, FCS already included).  Returns complex128 [F, nsamp] time signal in
-    int8-LSB units (i.e. what TPackSample16to8 would saturate), 640 + 160*(1+Nsym) samples at 40 Msps."""
+def signal_word_11a(rate_kbps, length):
+    """The 24-bit SIGNAL field (bit i = i-th bit on air) of a frame of `length` PSDU bytes: RATE, reserved 0, LENGTH, even parity, tail 0."""
+    w = RATES[rate_kbps][0] | (length & 0xFFF) << 5
+    return w | (bin(w).count("1") & 1) << 17
+
+def modulate(psdus, rate_kbps=54000, scramble_seeds=None, window=True, signal_word=None):
+    """psdus: uint8 [F, L] (L >= 0 bytes each, FCS already included).  Returns complex128 [F, nsamp] time signal in
+    int8-LSB units (i.e. what TPackSample16to8 would saturate), 640 + 160*(1+Nsym) samples at 40 Msps.
+    signal_word: the 24 SIGNAL bits to send instead of signal_word_11a(rate_kbps, L); the DATA field is still the PSDU at rate_kbps."""
     psdus = np.atleast_2d(np.asarray(psdus, np.uint8))
     F, L = psdus.shape
     rbits, nbpsc, cr, ndbps = RATES[rate_kbps]
@@ -145,10 +151,8 @@ def modulate(psdus, rate_kbps=54000, scramble_seeds=None, window=True):
     pol = _PILOT_POL[(np.arange(nsym) + 1) % 127]
     td_data = _ofdm_td(_place(data, pol))               # [F, nsym, 160]
     # SIGNAL
-    sig = np.zeros(24, np.uint8)
-    sig[0:4] = [(rbits >> i) & 1 for i in range(4)]
-    sig[5:17] = [(L >> i) & 1 for i in range(12)]
-    sig[17] = sig[:17].sum() & 1
+    sw = signal_word_11a(rate_kbps, L) if signal_word is None else int(signal_word)
+    sig = np.array([(sw >> i) & 1 for i in range(24)], np.uint8)
     As, Bs = conv_encode(sig)
     cs = puncture(As, Bs, (1, 2))
     j48 = interleave_map(48, 1)
@@ -219,10 +223,8 @@ def _scramble_11b(bits, state=0x1B):
 _DQPSK = {(0, 0): 0, (0, 1): 1, (1, 1): 2, (1, 0): 3}          # (d0, d1) -> quarter turns, counter-clockwise
 _QPSK = {(0, 0): 0, (0, 1): 1, (1, 0): 2, (1, 1): 3}           # CCK phi2..phi4 encoding (Table 18-?): 00,01,10,11 -> 0, pi/2, pi, 3pi/2
 
-def modulate_11b(psdu, rate_kbps=11000, amp=90.0, shape=True):
-    """psdu: uint8 [L] (FCS included).  Returns complex chips-domain waveform at 44 Msps in int8 units."""
-    psdu = np.asarray(psdu, np.uint8)
-    L = len(psdu)
+def plcp_11b(L, rate_kbps):
+    """(SIGNAL, SERVICE, LENGTH) of a long-preamble PLCP header for L PSDU bytes at rate_kbps."""
     service = 0x04                                      # locked clocks
     if rate_kbps == 11000:
         lp = L * 8 / 11.0; length = int(np.ceil(lp))
@@ -231,8 +233,16 @@ def modulate_11b(psdu, rate_kbps=11000, amp=90.0, shape=True):
         length = int(np.ceil(L * 8 / 5.5))
     else:
         length = L * 8 * 1000 // rate_kbps
-    hdr = bytes([_SIGNAL_11B[rate_kbps], service, length & 0xFF, length >> 8])
-    crc = _crc16_ccitt_reflected(hdr)
+    return _SIGNAL_11B[rate_kbps], service, length
+
+def modulate_11b(psdu, rate_kbps=11000, amp=90.0, shape=True, plcp=None):
+    """psdu: uint8 [L] (FCS included).  Returns complex chips-domain waveform at 44 Msps in int8 units.
+    plcp: (SIGNAL, SERVICE, LENGTH, CRC-16 xor mask) to send instead of plcp_11b(L, rate_kbps) with a correct CRC-16;
+    the PSDU is still modulated at rate_kbps."""
+    psdu = np.asarray(psdu, np.uint8)
+    signal, service, length, crc_xor = plcp_11b(len(psdu), rate_kbps) + (0,) if plcp is None else plcp
+    hdr = bytes([signal & 0xFF, service & 0xFF, length & 0xFF, (length >> 8) & 0xFF])
+    crc = _crc16_ccitt_reflected(hdr) ^ (crc_xor & 0xFFFF)
     hdr = hdr + bytes([crc & 0xFF, crc >> 8])
     bits = np.concatenate([np.ones(128, np.uint8),
                            np.unpackbits(np.frombuffer((0xF3A0).to_bytes(2, "little"), np.uint8), bitorder="little"),
@@ -329,8 +339,10 @@ def _td_plain(freq64, n):
     reps = -(-n // 128) + 1
     return np.tile(p, reps)[-n:]
 
-def modulate_11n(psdus, mcs=8, scramble_seeds=None):
-    """psdus uint8 [F, L] (FCS included) -> complex128 [F, 2, nsamp]: the two transmit chains at 40 Msps, int8 units."""
+def modulate_11n(psdus, mcs=8, scramble_seeds=None, lsig_word=None, htsig=None):
+    """psdus uint8 [F, L] (FCS included) -> complex128 [F, 2, nsamp]: the two transmit chains at 40 Msps, int8 units.
+    lsig_word: the 24 L-SIG bits to send instead of 6 Mbps with the spoofed length; htsig: (first 34 HT-SIG bits, CRC-8 xor mask)
+    instead of (MCS | L << 8 | 0x07 << 24, 0).  The data field is still the PSDU at `mcs`."""
     psdus = np.atleast_2d(np.asarray(psdus, np.uint8)); F, L = psdus.shape
     nbpsc, cr, ndbps = HT_MCS[mcs]
     nsym = -(-(16 + 8 * L + 6) // ndbps); ndata = nsym * ndbps
@@ -344,7 +356,8 @@ def modulate_11n(psdus, mcs=8, scramble_seeds=None):
     for k in range(-26, 27): Lf[k % 64] = _LTS[k + 26]
     nt = nsym + 5
     lsig_len = (nt * 24 - 22) // 8
-    sig = np.zeros(24, np.uint8); sig[0:4] = [1, 1, 0, 1]; sig[5:17] = [(lsig_len >> i) & 1 for i in range(12)]; sig[17] = sig[:17].sum() & 1
+    lw = signal_word_11a(6000, lsig_len) if lsig_word is None else int(lsig_word)
+    sig = np.array([(lw >> i) & 1 for i in range(24)], np.uint8)
     j48 = interleave_map(48, 1)
     def bpsk48(bits24_or_48):
         a, b = conv_encode(bits24_or_48); c = puncture(a, b, (1, 2)).reshape(-1, 48)
@@ -353,8 +366,9 @@ def modulate_11n(psdus, mcs=8, scramble_seeds=None):
     lsig_f = _place(bpsk48(sig)[None, :, :] * BPSK_MOD, _PILOT_POL[:1])[0, 0] / BPSK_MOD
     td = np.zeros((F, 2, 640 + 160 * (nt + 1)), np.complex128)
     for fidx in range(F):
-        hb = np.zeros(6, np.uint8); hb[0] = mcs; hb[1] = L & 0xFF; hb[2] = L >> 8; hb[3] = 0x07
-        c8 = _crc8_htsig(hb); hb[4] |= (c8 << 2) & 0xFF; hb[5] |= c8 >> 6
+        h34, c8x = (mcs | L << 8 | 0x07 << 24, 0) if htsig is None else htsig
+        hb = np.frombuffer((int(h34) & ((1 << 34) - 1)).to_bytes(6, "little"), np.uint8).copy()
+        c8 = _crc8_htsig(hb) ^ (c8x & 0xFF); hb[4] |= (c8 << 2) & 0xFF; hb[5] |= c8 >> 6
         hbits = np.unpackbits(hb, bitorder="little")
         hs = _place(bpsk48(hbits)[None, :, :] * BPSK_MOD, _PILOT_POL[1:3])[0] / BPSK_MOD          # [2, 64]
         hs = np.where(np.abs(hs) > 0, hs, 0); data_mask = np.ones(64, bool); data_mask[[7, 21, 57, 43]] = False
