@@ -30,6 +30,9 @@ namespace {
 
 struct DevBuf {
     void* p = nullptr; size_t cap = 0;
+    DevBuf() = default;
+    DevBuf(const DevBuf&) = delete; DevBuf& operator=(const DevBuf&) = delete;
+    ~DevBuf() { release(); }
     cudaError_t need(size_t n) {
         if (n <= cap) return cudaSuccess;
         if (p) cudaFree(p);
@@ -98,6 +101,63 @@ bool is_device_ptr(const void* p) {
     if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
     return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
+
+// [off, off + len) lies inside [0, total), without the sum that a 64-bit offset near 2^64 would wrap
+inline bool in_range(uint64_t off, uint64_t len, uint64_t total) { return len <= total && off <= total - len; }
+
+// Host copy of a slot or payload table whose parts may each live on either side: one synchronise only if a part is on the device.
+cudaError_t read_table(cudaStream_t st, const uint64_t* off, bool off_dev, const uint32_t* len, bool len_dev, uint32_t n,
+                       std::vector<uint64_t>& offh, std::vector<uint32_t>& lenh) {
+    offh.resize(n); lenh.resize(n);
+    cudaError_t e = cudaSuccess;
+    if (off_dev) e = cudaMemcpyAsync(offh.data(), off, n * 8ull, cudaMemcpyDeviceToHost, st); else memcpy(offh.data(), off, n * 8ull);
+    if (e != cudaSuccess) return e;
+    if (len_dev) e = cudaMemcpyAsync(lenh.data(), len, n * 4ull, cudaMemcpyDeviceToHost, st); else memcpy(lenh.data(), len, n * 4ull);
+    if (e == cudaSuccess && (off_dev || len_dev)) e = cudaStreamSynchronize(st);
+    return e;
+}
+
+// Device address of an input: `p` itself when it is device memory (`dev`), else workspace `b` (grown to bytes + slack) with the copy queued on `st`.
+template <class T>
+cudaError_t to_device(DevBuf& b, const T* p, bool dev, size_t bytes, cudaStream_t st, const T** d, size_t slack = 0) {
+    if (dev) { *d = p; return cudaSuccess; }
+    cudaError_t e = b.need(bytes + slack);
+    if (e == cudaSuccess) e = cudaMemcpyAsync(b.p, p, bytes, cudaMemcpyHostToDevice, st);
+    *d = (const T*)b.p;
+    return e;
+}
+
+// The results of one call.  bind() gives the device address a kernel writes: the caller's buffer when it is device memory, else workspace `b`
+// (grown to bytes + slack; a null result stays null).  bind2d() notes a strided copy of `rows` rows of `width` bytes out of a workspace into
+// the caller's buffer on either side; copy() a linear one into host memory.  finish() queues the noted copies in the order they were noted
+// and synchronises once if any of them goes to host memory.
+struct Returns {
+    struct Copy { void* dst; size_t dpitch; const void* src; size_t spitch, width, rows; bool to_host; };   // dpitch 0: one linear copy of width bytes
+    Copy c[4]; int n = 0;                              // no call returns more than four results
+    void copy(void* dst, const void* src, size_t bytes) { c[n++] = Copy{dst, 0, src, 0, bytes, 1, true}; }
+    void bind2d(void* dst, size_t dpitch, const void* src, size_t spitch, size_t width, size_t rows) {
+        c[n++] = Copy{dst, dpitch, src, spitch, width, rows, !is_device_ptr(dst)};
+    }
+    template <class T>
+    cudaError_t bind(DevBuf& b, T* p, size_t bytes, T** d, size_t slack = 0) {
+        *d = p;
+        if (!p || is_device_ptr(p)) return cudaSuccess;
+        const cudaError_t e = b.need(bytes + slack);
+        if (e != cudaSuccess) return e;
+        *d = (T*)b.p; copy(p, b.p, bytes);
+        return cudaSuccess;
+    }
+    cudaError_t finish(cudaStream_t st) {
+        bool host = false;
+        for (int i = 0; i < n; i++) {
+            const Copy& k = c[i]; const cudaMemcpyKind kind = k.to_host ? cudaMemcpyDeviceToHost : cudaMemcpyDeviceToDevice;
+            const cudaError_t e = k.dpitch ? cudaMemcpy2DAsync(k.dst, k.dpitch, k.src, k.spitch, k.width, k.rows, kind, st) : cudaMemcpyAsync(k.dst, k.src, k.width, kind, st);
+            if (e != cudaSuccess) return e;
+            host |= k.to_host;
+        }
+        return host ? cudaStreamSynchronize(st) : cudaSuccess;
+    }
+};
 
 } // namespace
 
@@ -278,16 +338,12 @@ extern "C" int sb200_create(int device, const sb200_cfg* cfg, sb200_handle** out
 
 extern "C" void sb200_destroy(sb200_handle* h) {
     if (!h) return;
-    cudaSetDevice(h->device);
-    DevBuf* all[] = {&h->tab, &h->iq, &h->off, &h->len, &h->info, &h->soft, &h->out, &h->status, &h->crc, &h->res,
-                     &h->taps[0], &h->taps[1], &h->taps[2], &h->taps[3], &h->taps[4], &h->vlist, &h->vcnt, &h->slotchk, &h->doff};
-    for (DevBuf* b : all) b->release();
-    h->iq40.release(); h->off40.release(); h->len40.release(); h->dcbuf.release(); h->vring.release(); h->soff.release(); h->slen.release(); h->spos.release(); h->snev.release(); h->sev.release(); h->tab11n.release(); h->iq1.release(); h->tabtx.release(); h->txpay.release(); h->txoff.release(); h->txlen.release(); h->txseed.release(); h->txout.release(); h->txns.release(); h->txdesc.release(); h->cca11n.release(); h->ccaidx.release(); h->tabtx11n.release(); h->txout1.release(); h->txpre.release();
+    cudaSetDevice(h->device);                          // the workspaces (DevBuf) free themselves in `delete h`
     if (h->ev0) cudaEventDestroy(h->ev0);
     if (h->ev1) cudaEventDestroy(h->ev1);
     for (int i = 0; i < 5; i++) if (h->evk[i]) cudaEventDestroy(h->evk[i]);
     if (h->ev_start) cudaEventDestroy(h->ev_start);
-    for (int i = 0; i < 2; i++) { if (h->ev_h2d[i]) cudaEventDestroy(h->ev_h2d[i]); if (h->ev_front[i]) cudaEventDestroy(h->ev_front[i]); h->stage[i].release(); }
+    for (int i = 0; i < 2; i++) { if (h->ev_h2d[i]) cudaEventDestroy(h->ev_h2d[i]); if (h->ev_front[i]) cudaEventDestroy(h->ev_front[i]); }
     for (cudaEvent_t e : h->ev_link) cudaEventDestroy(e);
     delete h->pool; for (int i = 0; i < 4; i++) { if (h->hstage[i]) cudaFreeHost(h->hstage[i]); if (h->ev_hfree[i]) cudaEventDestroy(h->ev_hfree[i]); }
     if (h->s_copy) cudaStreamDestroy(h->s_copy);
@@ -351,17 +407,14 @@ static int slot_table(sb200_handle* h, const uint64_t* frame_off, const uint32_t
         return SB200_OK;
     }
     h->tab_off = nullptr;
-    offh.resize(nframes); lenh.resize(nframes);
-    if (off_dev) CK(cudaMemcpyAsync(offh.data(), frame_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), frame_off, nframes * 8ull);
-    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), frame_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), frame_len, nframes * 4ull);
-    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    CK(read_table(st, frame_off, off_dev, frame_len, len_dev, nframes, offh, lenh));
     uint32_t mx = 0;
     for (uint32_t i = 0; i < nframes; i++) {
-        if (lenh[i] > iq_total || offh[i] > iq_total - lenh[i]) return h->fail(SB200_E_INVALID, "slot exceeds iq_total_samples");
+        if (!in_range(offh[i], lenh[i], iq_total)) return h->fail(SB200_E_INVALID, "slot exceeds iq_total_samples");
         if (lenh[i] > mx) mx = lenh[i];
     }
-    if (off_dev) *d_off = frame_off; else { CK(h->off.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->off.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); *d_off = (const uint64_t*)h->off.p; }
-    if (len_dev) *d_len = frame_len; else { CK(h->len.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->len.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); *d_len = (const uint32_t*)h->len.p; }
+    CK(to_device(h->off, off_dev ? frame_off : offh.data(), off_dev, nframes * 8ull, st, d_off));   // host parts: the copy checked above
+    CK(to_device(h->len, len_dev ? frame_len : lenh.data(), len_dev, nframes * 4ull, st, d_len));
     *max_len = mx; *host_valid = true;
     return SB200_OK;
 }
@@ -468,8 +521,8 @@ static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
     CK(cudaEventRecord(h->ev0, st));
     if (!pipelined) {
         const uint32_t* d_iq;
-        if (iq_dev) d_iq = (const uint32_t*)iq;
-        else { CK(h->iq.need(iq_total * 4ull)); CK(cudaMemcpyAsync(h->iq.p, iq, iq_total * 4ull, cudaMemcpyHostToDevice, st)); d_iq = (const uint32_t*)h->iq.p; h->last_h2d_bytes = iq_total * 4ull; h->last_gathered_chunks = 0; h->last_chunks = 1; }
+        CK(to_device(h->iq, (const uint32_t*)iq, iq_dev, iq_total * 4ull, st, &d_iq));
+        if (!iq_dev) { h->last_h2d_bytes = iq_total * 4ull; h->last_gathered_chunks = 0; h->last_chunks = 1; }
         int rc = launch_chunk(h, d_iq, d_off, d_len, 0, nframes, soft_stride, row, st, st, nullptr, taps, true, dc_init, 0, rate20 ? 0u : 1u, rate20 ? 1u : 0u);
         if (rc != SB200_OK) return rc;
         h->nk = 4;
@@ -613,31 +666,24 @@ static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
         h->nk = 0;
         if (dec && getenv("SB200_TRACE")) fprintf(stderr, "[sb200] rx11a host_decimate: %u chunks (%u gathered, %u sent as they are), host gather %.2f ms in total (%u threads), link estimate %.1f GB/s, %.1f MB copied\n", k, gk, k - gk, h->gather_ms, h->host_decimate, h->link_bpms / 1e6, h2d_bytes / 1e6);
     }
-    const bool res_dev = res_dev_all;
-    sb200_frame_result* d_res = d_res_all;
     if (!pipelined) {
-        k_pack_results<<<(nframes + 255) / 256, 256, 0, st>>>((const FrameInfo*)h->info.p, (const uint32_t*)h->status.p, (const uint32_t*)h->crc.p, nframes, d_res);
+        k_pack_results<<<(nframes + 255) / 256, 256, 0, st>>>((const FrameInfo*)h->info.p, (const uint32_t*)h->status.p, (const uint32_t*)h->crc.p, nframes, d_res_all);
         h->launches += 1;
         CK(cudaEventRecord(h->evk[4], st));
     }
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true;
     CK(cudaGetLastError());
-    bool host_out = false;
     if (pipelined) {                                    // everything that goes to the host was already queued per chunk
         if (out_bytes && out_stride && out_dev_all) { const size_t w = out_stride < row ? out_stride : row; CK(cudaMemcpy2DAsync(out_bytes, out_stride, h->out.p, row, w, nframes, cudaMemcpyDeviceToDevice, st)); }
         if ((out_bytes && out_stride && !out_dev_all) || !res_dev_all) CK(cudaStreamSynchronize(st));
         return SB200_OK;
     }
-    if (out_bytes && out_stride) {
-        const size_t w = out_stride < row ? out_stride : row;
-        const bool od = is_device_ptr(out_bytes);
-        CK(cudaMemcpy2DAsync(out_bytes, out_stride, h->out.p, row, w, nframes, od ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-        host_out |= !od;
-    }
-    if (!res_dev) { CK(cudaMemcpyAsync(res, d_res, nframes * sizeof(sb200_frame_result), cudaMemcpyDeviceToHost, st)); host_out = true; }
-    if (soft_host) { CK(cudaMemcpy2DAsync(soft_host, soft_host_stride, h->soft.p, soft_stride, soft_host_stride < soft_stride ? soft_host_stride : soft_stride, nframes, cudaMemcpyDeviceToHost, st)); host_out = true; }
-    if (host_out) CK(cudaStreamSynchronize(st));
+    Returns ret;
+    if (out_bytes && out_stride) ret.bind2d(out_bytes, out_stride, h->out.p, row, out_stride < row ? out_stride : row, nframes);
+    if (!res_dev_all) ret.copy(res, d_res_all, nframes * sizeof(sb200_frame_result));
+    if (soft_host) ret.bind2d(soft_host, soft_host_stride, h->soft.p, soft_stride, soft_host_stride < soft_stride ? soft_host_stride : soft_stride, nframes);
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -657,7 +703,7 @@ extern "C" int sb200_rx11a_streams(sb200_handle* h, const int16_t* iq, uint64_t 
     CK(cudaSetDevice(h->device));
     if (is_device_ptr(res) || (out_bytes && is_device_ptr(out_bytes)) || is_device_ptr(stream_off) || is_device_ptr(stream_len) || is_device_ptr(nframes_out))
         return h->fail(SB200_E_INVALID, "stream mode takes its tables and returns its results in host memory");
-    for (uint32_t s = 0; s < nstreams; s++) { nframes_out[s] = 0; if (stream_off[s] + stream_len[s] > iq_total) return h->fail(SB200_E_INVALID, "capture exceeds iq_total_samples"); }
+    for (uint32_t s = 0; s < nstreams; s++) { nframes_out[s] = 0; if (!in_range(stream_off[s], stream_len[s], iq_total)) return h->fail(SB200_E_INVALID, "capture exceeds iq_total_samples"); }
     if (nstreams == 0 || max_frames == 0) return SB200_OK;
     const int16_t* d_iq = iq;
     if (!is_device_ptr(iq)) {                           // host captures: only the ranges the streams name travel (they may be islands in a large arena)
@@ -749,18 +795,18 @@ extern "C" int sb200_fir_decimate2(sb200_handle* h, const int16_t* iq, uint64_t 
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
     const uint64_t n_out = (n_in + 1) / 2;
-    const bool in_dev = is_device_ptr(iq), out_dev = is_device_ptr(out);
-    const uint32_t* d_in; uint32_t* d_out;
-    if (in_dev) { if ((uintptr_t)iq & 15u) return h->fail(SB200_E_INVALID, "device input must be 16-byte aligned"); d_in = (const uint32_t*)iq; }
-    else { CK(h->iq.need(n_in * 4ull + 16)); CK(cudaMemcpyAsync(h->iq.p, iq, n_in * 4ull, cudaMemcpyHostToDevice, st)); d_in = (const uint32_t*)h->iq.p; }
-    if (out_dev) d_out = (uint32_t*)out; else { CK(h->iq40.need(n_out * 4ull + 16)); d_out = (uint32_t*)h->iq40.p; }
+    const bool in_dev = is_device_ptr(iq);
+    if (in_dev && ((uintptr_t)iq & 15u)) return h->fail(SB200_E_INVALID, "device input must be 16-byte aligned");
+    const uint32_t* d_in; uint32_t* d_out; Returns ret;
+    CK(to_device(h->iq, (const uint32_t*)iq, in_dev, n_in * 4ull, st, &d_in, 16));
+    CK(ret.bind(h->iq40, (uint32_t*)out, n_out * 4ull, &d_out, 16));
     FirTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
     CK(cudaEventRecord(h->ev0, st));
     k_fir_decimate2<<<(unsigned)((n_in + SB_FIR_TILE - 1) / SB_FIR_TILE), SB_FIR_THREADS, 0, st>>>(d_in, n_in, T, d_out, n_out);
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 0; h->launches += 1;
     CK(cudaGetLastError());
-    if (!out_dev) { CK(cudaMemcpyAsync(out, d_out, n_out * 4ull, cudaMemcpyDeviceToHost, st)); CK(cudaStreamSynchronize(st)); }
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -779,21 +825,19 @@ extern "C" int sb200_rx11a_batch_ex(sb200_handle* h, const int16_t* iq, uint64_t
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
     // slot table on the host (sizing) and on the device (kernel)
-    std::vector<uint64_t> offh(nframes); std::vector<uint32_t> lenh(nframes);
+    std::vector<uint64_t> offh; std::vector<uint32_t> lenh;
     const bool off_dev = is_device_ptr(frame_off), len_dev = is_device_ptr(frame_len), iq_dev = is_device_ptr(iq);
-    if (off_dev) CK(cudaMemcpyAsync(offh.data(), frame_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), frame_off, nframes * 8ull);
-    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), frame_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), frame_len, nframes * 4ull);
-    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    CK(read_table(st, frame_off, off_dev, frame_len, len_dev, nframes, offh, lenh));
     uint32_t max40 = 28;
     for (uint32_t i = 0; i < nframes; i++) {
-        if (lenh[i] > iq_total || offh[i] > iq_total - lenh[i]) return h->fail(SB200_E_INVALID, "slot exceeds iq_total_samples");
+        if (!in_range(offh[i], lenh[i], iq_total)) return h->fail(SB200_E_INVALID, "slot exceeds iq_total_samples");
         const uint32_t n40 = resampled_len_40(lenh[i]); if (n40 > max40) max40 = n40;
     }
     const uint64_t stride40 = ((uint64_t)max40 + 3ull) & ~3ull;
     const uint32_t* d_iq; const uint64_t* d_off; const uint32_t* d_len;
-    if (iq_dev) d_iq = (const uint32_t*)iq; else { CK(h->iq.need(iq_total * 4ull)); CK(cudaMemcpyAsync(h->iq.p, iq, iq_total * 4ull, cudaMemcpyHostToDevice, st)); d_iq = (const uint32_t*)h->iq.p; }
-    if (off_dev) d_off = frame_off; else { CK(h->off.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->off.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); d_off = (const uint64_t*)h->off.p; }
-    if (len_dev) d_len = frame_len; else { CK(h->len.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->len.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); d_len = (const uint32_t*)h->len.p; }
+    CK(to_device(h->iq, (const uint32_t*)iq, iq_dev, iq_total * 4ull, st, &d_iq));
+    CK(to_device(h->off, off_dev ? frame_off : offh.data(), off_dev, nframes * 8ull, st, &d_off));
+    CK(to_device(h->len, len_dev ? frame_len : lenh.data(), len_dev, nframes * 4ull, st, &d_len));
     CK(h->iq40.need(nframes * stride40 * 4ull)); CK(h->off40.need(nframes * 8ull)); CK(h->len40.need(nframes * 4ull));
     dim3 grid(nframes, (unsigned)((max40 + 255) / 256 > 64 ? 64 : (max40 + 255) / 256));   // slots on x: the y extent stops at 65535
     k_resample_44_40<<<grid, 256, 0, st>>>(d_iq, d_off, d_len, nframes, (uint32_t*)h->iq40.p, stride40, (uint64_t*)h->off40.p, (uint32_t*)h->len40.p);
@@ -814,28 +858,20 @@ static int rx11b_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
     const bool iq_dev = is_device_ptr(iq);
     const uint32_t* d_iq; const uint64_t* d_off; const uint32_t* d_len; uint32_t max_len = 0; bool tab_on_host = false;
     { int rc = slot_table(h, frame_off, frame_len, nframes, iq_total, false, st, &d_off, &d_len, &max_len, &tab_on_host); if (rc != SB200_OK) return rc; }
-    if (iq_dev) d_iq = (const uint32_t*)iq; else { CK(h->iq.need(iq_total * 4ull)); CK(cudaMemcpyAsync(h->iq.p, iq, iq_total * 4ull, cudaMemcpyHostToDevice, st)); d_iq = (const uint32_t*)h->iq.p; }
+    CK(to_device(h->iq, (const uint32_t*)iq, iq_dev, iq_total * 4ull, st, &d_iq));
     const uint64_t row = 4096; const size_t nres = (size_t)nframes * max_frames;
-    CK(h->out.need(nres * row)); CK(h->res.need(nres * sizeof(Result11b)));
-    const bool res_dev = is_device_ptr(res);
-    Result11b* d_res = res_dev ? (Result11b*)res : (Result11b*)h->res.p;
-    uint32_t* d_cnt = nullptr; const bool cnt_dev = counts && is_device_ptr(counts);
-    if (counts) { if (cnt_dev) d_cnt = counts; else { CK(h->txns.need(nframes * 4ull)); d_cnt = (uint32_t*)h->txns.p; } }
+    CK(h->out.need(nres * row));
+    Returns ret; Result11b* d_res; uint32_t* d_cnt;
+    if (out_bytes && out_stride) ret.bind2d(out_bytes, out_stride, h->out.p, row, out_stride < row ? out_stride : row, nres);
+    CK(ret.bind(h->res, (Result11b*)res, nres * sizeof(Result11b), &d_res));
+    CK(ret.bind(h->txns, counts, nframes * 4ull, &d_cnt));
     if (max_frames > 1) CK(cudaMemsetAsync(d_res, 0, nres * sizeof(Result11b), st));          // entries past the count read "no event"
     CK(cudaEventRecord(h->ev0, st));
     k_rx11b<<<(nframes + 63) / 64, 64, 0, st>>>(d_iq, d_off, d_len, nframes, h->cca_thr, (uint8_t*)h->out.p, row, d_res, max_frames, d_cnt);
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 0; h->launches += 1;
     CK(cudaGetLastError());
-    bool host_out = false;
-    if (out_bytes && out_stride) {
-        const size_t w = out_stride < row ? out_stride : row; const bool od = is_device_ptr(out_bytes);
-        CK(cudaMemcpy2DAsync(out_bytes, out_stride, h->out.p, row, w, nres, od ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-        host_out |= !od;
-    }
-    if (!res_dev) { CK(cudaMemcpyAsync(res, d_res, nres * sizeof(Result11b), cudaMemcpyDeviceToHost, st)); host_out = true; }
-    if (counts && !cnt_dev) { CK(cudaMemcpyAsync(counts, d_cnt, nframes * 4ull, cudaMemcpyDeviceToHost, st)); host_out = true; }
-    if (host_out) CK(cudaStreamSynchronize(st));
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -906,23 +942,23 @@ static int rx11n_run(sb200_handle* h, const int16_t* iq0, const int16_t* iq1, ui
     const uint64_t* d_off; const uint32_t* d_len; uint32_t max_len = 0; bool tab_on_host = false;
     { int rc = slot_table(h, frame_off, frame_len, nframes, iq_total, false, st, &d_off, &d_len, &max_len, &tab_on_host); if (rc != SB200_OK) return rc; }
     const uint32_t* d_iq0; const uint32_t* d_iq1;
-    if (iq_dev) { d_iq0 = (const uint32_t*)iq0; d_iq1 = (const uint32_t*)iq1; }
-    else {
-        CK(h->iq.need(iq_total * 4ull)); CK(h->iq1.need(iq_total * 4ull));
-        CK(cudaMemcpyAsync(h->iq.p, iq0, iq_total * 4ull, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(h->iq1.p, iq1, iq_total * 4ull, cudaMemcpyHostToDevice, st));
-        d_iq0 = (const uint32_t*)h->iq.p; d_iq1 = (const uint32_t*)h->iq1.p;
-    }
+    CK(to_device(h->iq, (const uint32_t*)iq0, iq_dev, iq_total * 4ull, st, &d_iq0));
+    CK(to_device(h->iq1, (const uint32_t*)iq1, iq_dev, iq_total * 4ull, st, &d_iq1));
     const uint64_t max_sym = (max_len / 2u) / 80u + 1u;
     h->N.mcs_limit = h->ht_mcs_limit;
     const uint64_t soft_stride = ((max_sym * (h->ht_mcs_limit > 11u ? 624ull : 208ull)) + 15ull) & ~15ull;   // 2 x 52 x N_BPSC soft values per symbol
     const uint64_t row = 1536;                         // >= 1500 (MTU, PHY_11n.hpp:478,505)
     CK(h->info.need(nframes * sizeof(FrameInfo))); CK(h->soft.need(nframes * soft_stride)); CK(h->out.need(nframes * row));
-    CK(h->status.need(nframes * 4ull)); CK(h->crc.need(nframes * 4ull)); CK(h->res.need(nframes * sizeof(sb200_frame_result_11n)));
+    CK(h->status.need(nframes * 4ull)); CK(h->crc.need(nframes * 4ull));
+    Returns ret; sb200_frame_result_11n* d_res;
+    if (out_bytes && out_stride) ret.bind2d(out_bytes, out_stride, h->out.p, row, out_stride < row ? out_stride : row, nframes);
+    CK(ret.bind(h->res, res, nframes * sizeof(sb200_frame_result_11n), &d_res));
+    if (soft_host) ret.bind2d(soft_host, soft_host_stride, h->soft.p, soft_stride, soft_host_stride < soft_stride ? soft_host_stride : soft_stride, nframes);
     FrameInfo* d_info = (FrameInfo*)h->info.p;
     CK(cudaEventRecord(h->ev0, st)); CK(cudaEventRecord(h->evk[0], st));
     if (state_idx) {
-        CK(h->ccaidx.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->ccaidx.p, state_idx, nframes * 4ull, cudaMemcpyHostToDevice, st));
-        k_sync11n_stream<<<(nframes + 63) / 64, 64, 0, st>>>(d_iq0, d_iq1, d_off, d_len, nframes, (const uint32_t*)h->ccaidx.p, (Cca11nState*)h->cca11n.p, d_info);
+        const uint32_t* d_idx; CK(to_device(h->ccaidx, state_idx, false, nframes * 4ull, st, &d_idx));
+        k_sync11n_stream<<<(nframes + 63) / 64, 64, 0, st>>>(d_iq0, d_iq1, d_off, d_len, nframes, d_idx, (Cca11nState*)h->cca11n.p, d_info);
     } else
     k_sync11n<<<(nframes + 127) / 128, 128, 0, st>>>(d_iq0, d_iq1, d_off, d_len, nframes, d_info);
     CK(cudaEventRecord(h->evk[1], st));
@@ -947,21 +983,11 @@ static int rx11n_run(sb200_handle* h, const int16_t* iq0, const int16_t* iq1, ui
         h->launches += 2;
     }
     CK(cudaEventRecord(h->evk[3], st));
-    const bool res_dev = is_device_ptr(res);
-    sb200_frame_result_11n* d_res = res_dev ? res : (sb200_frame_result_11n*)h->res.p;
     k_pack_results11n<<<(nframes + 255) / 256, 256, 0, st>>>(d_info, (const uint32_t*)h->status.p, (const uint32_t*)h->crc.p, nframes, state_idx != nullptr, d_res);
     CK(cudaEventRecord(h->evk[4], st)); CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 4; h->launches += 5;
     CK(cudaGetLastError());
-    bool host_out = false;
-    if (out_bytes && out_stride) {
-        const size_t w = out_stride < row ? out_stride : row; const bool od = is_device_ptr(out_bytes);
-        CK(cudaMemcpy2DAsync(out_bytes, out_stride, h->out.p, row, w, nframes, od ? cudaMemcpyDeviceToDevice : cudaMemcpyDeviceToHost, st));
-        host_out |= !od;
-    }
-    if (!res_dev) { CK(cudaMemcpyAsync(res, d_res, nframes * sizeof(sb200_frame_result_11n), cudaMemcpyDeviceToHost, st)); host_out = true; }
-    if (soft_host) { CK(cudaMemcpy2DAsync(soft_host, soft_host_stride, h->soft.p, soft_stride, soft_host_stride < soft_stride ? soft_host_stride : soft_stride, nframes, cudaMemcpyDeviceToHost, st)); host_out = true; }
-    if (host_out) CK(cudaStreamSynchronize(st));
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -975,15 +1001,13 @@ extern "C" int sb200_rx11n_streams(sb200_handle* h, const int16_t* iq0, const in
     CK(cudaSetDevice(h->device));
     if (is_device_ptr(res) || (out_bytes && is_device_ptr(out_bytes)) || is_device_ptr(stream_off) || is_device_ptr(stream_len) || is_device_ptr(nframes_out))
         return h->fail(SB200_E_INVALID, "stream mode takes its tables and returns its results in host memory");
-    if (is_device_ptr(iq0) != is_device_ptr(iq1)) return h->fail(SB200_E_INVALID, "both antenna buffers must live on the same side");
-    for (uint32_t s = 0; s < nstreams; s++) { nframes_out[s] = 0; if (stream_off[s] + stream_len[s] > iq_total) return h->fail(SB200_E_INVALID, "capture exceeds iq_total_samples"); }
+    const bool iq_dev = is_device_ptr(iq0);
+    if (iq_dev != is_device_ptr(iq1)) return h->fail(SB200_E_INVALID, "both antenna buffers must live on the same side");
+    for (uint32_t s = 0; s < nstreams; s++) { nframes_out[s] = 0; if (!in_range(stream_off[s], stream_len[s], iq_total)) return h->fail(SB200_E_INVALID, "capture exceeds iq_total_samples"); }
     if (nstreams == 0 || max_frames == 0) return SB200_OK;
-    const int16_t* d_iq0 = iq0; const int16_t* d_iq1 = iq1;
-    if (!is_device_ptr(iq0)) {
-        CK(h->iq.need(iq_total * 4ull)); CK(h->iq1.need(iq_total * 4ull));
-        CK(cudaMemcpyAsync(h->iq.p, iq0, iq_total * 4ull, cudaMemcpyHostToDevice, st)); CK(cudaMemcpyAsync(h->iq1.p, iq1, iq_total * 4ull, cudaMemcpyHostToDevice, st));
-        d_iq0 = (const int16_t*)h->iq.p; d_iq1 = (const int16_t*)h->iq1.p;
-    }
+    const int16_t* d_iq0; const int16_t* d_iq1;
+    CK(to_device(h->iq, iq0, iq_dev, iq_total * 4ull, st, &d_iq0));
+    CK(to_device(h->iq1, iq1, iq_dev, iq_total * 4ull, st, &d_iq1));
     CK(h->cca11n.need((size_t)nstreams * sizeof(Cca11nState))); CK(cudaMemsetAsync(h->cca11n.p, 0, (size_t)nstreams * sizeof(Cca11nState), st));   // TCCA11n / MimoAutoCorr constructors
     std::vector<uint64_t> pos(nstreams, 0);
     std::vector<uint32_t> last_mcs(nstreams, 0);      // CF_HTRxVector::ht_frame_mcs of each capture: never reset between events
@@ -1071,16 +1095,15 @@ extern "C" int sb200_rxblocks_unpack(sb200_handle* h, const void* blocks, uint64
     if (nblocks == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
-    const bool in_dev = is_device_ptr(blocks), out_dev = is_device_ptr(iq_out);
-    const uint4* d_in = (const uint4*)blocks; uint4* d_out = (uint4*)iq_out;
-    if (!in_dev) { CK(h->stage[0].need(nblocks * 128ull)); CK(cudaMemcpyAsync(h->stage[0].p, blocks, nblocks * 128ull, cudaMemcpyHostToDevice, st)); d_in = (const uint4*)h->stage[0].p; }
-    if (!out_dev) { CK(h->stage[1].need(nblocks * 112ull)); d_out = (uint4*)h->stage[1].p; }
+    const uint4* d_in; uint4* d_out; Returns ret;
+    CK(to_device(h->stage[0], (const uint4*)blocks, is_device_ptr(blocks), nblocks * 128ull, st, &d_in));
+    CK(ret.bind(h->stage[1], (uint4*)iq_out, nblocks * 112ull, &d_out));
     const uint64_t nunits = nblocks * 7ull;
     const unsigned grid = (unsigned)((nunits + 255) / 256 < 148ull * 16 ? (nunits + 255) / 256 : 148ull * 16);
     k_rxblocks_unpack<<<grid, 256, 0, st>>>(d_in, nunits, left_shift, d_out);
     h->launches += 1;
     CK(cudaGetLastError());
-    if (!out_dev) { CK(cudaMemcpyAsync(iq_out, d_out, nblocks * 112ull, cudaMemcpyDeviceToHost, st)); CK(cudaStreamSynchronize(st)); }
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -1097,20 +1120,15 @@ extern "C" int sb200_rxblocks_desc(sb200_handle* h, const void* blocks, uint64_t
     if (nblocks == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
-    const bool in_dev = is_device_ptr(blocks);
-    const bool v_dev = vstream_bits && is_device_ptr(vstream_bits), t_dev = timestamps && is_device_ptr(timestamps);
-    const uint4* d_in = (const uint4*)blocks;
-    if (!in_dev) { CK(h->stage[0].need(nblocks * 128ull)); CK(cudaMemcpyAsync(h->stage[0].p, blocks, nblocks * 128ull, cudaMemcpyHostToDevice, st)); d_in = (const uint4*)h->stage[0].p; }
-    uint32_t* d_v = vstream_bits; uint32_t* d_t = timestamps;
-    if ((vstream_bits && !v_dev) || (timestamps && !t_dev)) { CK(h->stage[1].need(nblocks * 8ull)); if (vstream_bits && !v_dev) d_v = (uint32_t*)h->stage[1].p; if (timestamps && !t_dev) d_t = (uint32_t*)h->stage[1].p + nblocks; }
+    const uint4* d_in; uint32_t* d_v; uint32_t* d_t; Returns ret;
+    CK(to_device(h->stage[0], (const uint4*)blocks, is_device_ptr(blocks), nblocks * 128ull, st, &d_in));
+    CK(ret.bind(h->stage[1], vstream_bits, nblocks * 4ull, &d_v));
+    CK(ret.bind(h->txns, timestamps, nblocks * 4ull, &d_t));
     const unsigned grid = (unsigned)((nblocks + 255) / 256 < 148ull * 8 ? (nblocks + 255) / 256 : 148ull * 8);
     k_rxblocks_desc<<<grid, 256, 0, st>>>(d_in, nblocks, d_v, d_t);
     h->launches += 1;
     CK(cudaGetLastError());
-    bool sync = false;
-    if (vstream_bits && !v_dev) { CK(cudaMemcpyAsync(vstream_bits, d_v, nblocks * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (timestamps && !t_dev) { CK(cudaMemcpyAsync(timestamps, d_t, nblocks * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (sync) CK(cudaStreamSynchronize(st));
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -1166,30 +1184,28 @@ extern "C" int sb200_tx11a_batch(sb200_handle* h, const uint8_t* payload, uint64
     CK(cudaSetDevice(h->device));
     int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
     // frame table on the host (sizes the grid and checks the slots)
-    std::vector<uint64_t> offh(nframes); std::vector<uint32_t> lenh(nframes);
-    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len), pay_dev = is_device_ptr(payload), out_dev = is_device_ptr(out);
-    if (off_dev) CK(cudaMemcpyAsync(offh.data(), pay_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), pay_off, nframes * 8ull);
-    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), pay_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), pay_len, nframes * 4ull);
-    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    std::vector<uint64_t> offh; std::vector<uint32_t> lenh;
+    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len);
+    CK(read_table(st, pay_off, off_dev, pay_len, len_dev, nframes, offh, lenh));
     TxJob job{}; job.rate_code = R[ri].code; job.nbpsc = R[ri].nbpsc; job.code_rate = R[ri].cr; job.ndbps = R[ri].ndbps; job.ndbps_pad = rate_kbps == 9000 ? 72 : R[ri].ndbps;
     job.lead = lead_samples; job.fmt16 = sample_bits == 16;
     uint32_t max_nsym = 0;
     for (uint32_t i = 0; i < nframes; i++) {
-        if (lenh[i] + 4u > 4095u || offh[i] + lenh[i] > payload_total) return h->fail(SB200_E_INVALID, "payload slot out of range (LENGTH is 12 bits incl. FCS)");
+        if (lenh[i] > 4091u || !in_range(offh[i], lenh[i], payload_total)) return h->fail(SB200_E_INVALID, "payload slot out of range (LENGTH is 12 bits incl. FCS)");
         const uint32_t ns = tx11a_nsym(lenh[i], job.ndbps, job.ndbps_pad);
         if ((uint64_t)lead_samples + 640u + 160ull * (1u + ns) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
         if (ns > max_nsym) max_nsym = ns;
     }
     job.max_sym = 1u + max_nsym;
     const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len; const uint8_t* d_seed = nullptr;
-    if (pay_dev) d_pay = payload; else { CK(h->txpay.need(payload_total)); CK(cudaMemcpyAsync(h->txpay.p, payload, payload_total, cudaMemcpyHostToDevice, st)); d_pay = (const uint8_t*)h->txpay.p; }
-    if (off_dev) d_off = pay_off; else { CK(h->txoff.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->txoff.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); d_off = (const uint64_t*)h->txoff.p; }
-    if (len_dev) d_len = pay_len; else { CK(h->txlen.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->txlen.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); d_len = (const uint32_t*)h->txlen.p; }
-    if (seeds) { if (is_device_ptr(seeds)) d_seed = seeds; else { CK(h->txseed.need(nframes)); CK(cudaMemcpyAsync(h->txseed.p, seeds, nframes, cudaMemcpyHostToDevice, st)); d_seed = (const uint8_t*)h->txseed.p; } }
+    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay));
+    CK(to_device(h->txoff, off_dev ? pay_off : offh.data(), off_dev, nframes * 8ull, st, &d_off));
+    CK(to_device(h->txlen, len_dev ? pay_len : lenh.data(), len_dev, nframes * 4ull, st, &d_len));
+    if (seeds) CK(to_device(h->txseed, seeds, is_device_ptr(seeds), nframes, st, &d_seed));
     const size_t bps = sample_bits == 16 ? 4 : 2, out_bytes = (size_t)nframes * out_stride_samples * bps;
-    void* d_out = out; if (!out_dev) { CK(h->txout.need(out_bytes)); d_out = h->txout.p; }
-    uint32_t* d_ns = nullptr; const bool ns_dev = nsamples && is_device_ptr(nsamples);
-    if (nsamples) { if (ns_dev) d_ns = nsamples; else { CK(h->txns.need(nframes * 4ull)); d_ns = (uint32_t*)h->txns.p; } }
+    Returns ret; void* d_out; uint32_t* d_ns;
+    CK(ret.bind(h->txout, out, out_bytes, &d_out));
+    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
     const unsigned helpers = 8;                          // warps per frame for the preamble and the zero fill
     dim3 grid(nframes, (job.max_sym + helpers + SB_TX_WARPS - 1) / SB_TX_WARPS);
     CK(cudaEventRecord(h->ev0, st));
@@ -1199,10 +1215,7 @@ extern "C" int sb200_tx11a_batch(sb200_handle* h, const uint8_t* payload, uint64
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 0; h->launches += 2;
     CK(cudaGetLastError());
-    bool sync = false;
-    if (!out_dev) { CK(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (nsamples && !ns_dev) { CK(cudaMemcpyAsync(nsamples, d_ns, nframes * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (sync) CK(cudaStreamSynchronize(st));
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -1230,28 +1243,25 @@ extern "C" int sb200_tx11b_batch(sb200_handle* h, const uint8_t* payload, uint64
         for (int k = 0; k < 20; k++) if (job.taps[k] != H[k]) return h->fail(SB200_E_INVALID, "shaper taps differ from the compiled constants"); }
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
-    std::vector<uint64_t> offh(nframes); std::vector<uint32_t> lenh(nframes);
-    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len), pay_dev = is_device_ptr(payload), out_dev = is_device_ptr(out);
-    if (off_dev) CK(cudaMemcpyAsync(offh.data(), pay_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), pay_off, nframes * 8ull);
-    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), pay_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), pay_len, nframes * 4ull);
-    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    std::vector<uint64_t> offh; std::vector<uint32_t> lenh;
+    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len);
+    CK(read_table(st, pay_off, off_dev, pay_len, len_dev, nframes, offh, lenh));
     uint32_t max_len = 0;
     for (uint32_t i = 0; i < nframes; i++) {
-        if (lenh[i] + 4u > 4095u || offh[i] + lenh[i] > payload_total) return h->fail(SB200_E_INVALID, "payload slot out of range (frame_length 1..4095 incl. FCS)");
+        if (lenh[i] > 4091u || !in_range(offh[i], lenh[i], payload_total)) return h->fail(SB200_E_INVALID, "payload slot out of range (frame_length 1..4095 incl. FCS)");
         if ((uint64_t)lead_samples + tx11b_nsamples(tx11b_nchips(lenh[i], job.chips_per_byte)) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
         if (lenh[i] > max_len) max_len = lenh[i];
     }
     job.desc_stride = (24u + max_len + 4u + 7u) & ~7u;
     const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len;
-    if (pay_dev) d_pay = payload; else { CK(h->txpay.need(payload_total)); CK(cudaMemcpyAsync(h->txpay.p, payload, payload_total, cudaMemcpyHostToDevice, st)); d_pay = (const uint8_t*)h->txpay.p; }
-    if (off_dev) d_off = pay_off; else { CK(h->txoff.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->txoff.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); d_off = (const uint64_t*)h->txoff.p; }
-    if (len_dev) d_len = pay_len; else { CK(h->txlen.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->txlen.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); d_len = (const uint32_t*)h->txlen.p; }
+    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay));
+    CK(to_device(h->txoff, off_dev ? pay_off : offh.data(), off_dev, nframes * 8ull, st, &d_off));
+    CK(to_device(h->txlen, len_dev ? pay_len : lenh.data(), len_dev, nframes * 4ull, st, &d_len));
     const size_t bps = sample_bits == 16 ? 4 : 2, out_bytes = (size_t)nframes * out_stride_samples * bps;
-    void* d_out = out; if (!out_dev) { CK(h->txout.need(out_bytes)); d_out = h->txout.p; }
-    uint32_t* d_ns = nullptr; const bool ns_dev = nsamples && is_device_ptr(nsamples);
-    if (nsamples) { if (ns_dev) d_ns = nsamples; else { CK(h->txns.need(nframes * 4ull)); d_ns = (uint32_t*)h->txns.p; } }
-    uint32_t* d_fp = nullptr; const bool fp_dev = final_phase && is_device_ptr(final_phase);
-    if (final_phase) { if (fp_dev) d_fp = final_phase; else { CK(h->txseed.need(nframes * 4ull)); d_fp = (uint32_t*)h->txseed.p; } }
+    Returns ret; void* d_out; uint32_t* d_ns; uint32_t* d_fp;
+    CK(ret.bind(h->txout, out, out_bytes, &d_out));
+    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
+    CK(ret.bind(h->txseed, final_phase, nframes * 4ull, &d_fp));
     CK(h->crc.need(nframes * 4ull)); CK(h->txdesc.need((size_t)nframes * job.desc_stride * 2ull));
     const uint64_t per_cta = (uint64_t)SB_TX11B_THREADS * SB_TX11B_SPT, ny = (out_stride_samples + per_cta - 1) / per_cta;
     if (ny > 65535u || (uint64_t)lead_samples + out_stride_samples >= (1ull << 27)) return h->fail(SB200_E_INVALID, "out_stride_samples too large");
@@ -1267,11 +1277,7 @@ extern "C" int sb200_tx11b_batch(sb200_handle* h, const uint8_t* payload, uint64
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 0; h->launches += 3;
     CK(cudaGetLastError());
-    bool sync = false;
-    if (!out_dev) { CK(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (nsamples && !ns_dev) { CK(cudaMemcpyAsync(nsamples, d_ns, nframes * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (final_phase && !fp_dev) { CK(cudaMemcpyAsync(final_phase, d_fp, nframes * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (sync) CK(cudaStreamSynchronize(st));
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -1283,23 +1289,21 @@ extern "C" int sb200_tx11b_fir37(sb200_handle* h, const int8_t* chips, uint64_t 
     if (nframes == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
-    std::vector<uint64_t> offh(nframes); std::vector<uint32_t> lenh(nframes);
+    std::vector<uint64_t> offh; std::vector<uint32_t> lenh;
     const bool off_dev = is_device_ptr(frame_off), len_dev = is_device_ptr(frame_len), in_dev = is_device_ptr(chips), out_dev = is_device_ptr(out);
-    if (off_dev) CK(cudaMemcpyAsync(offh.data(), frame_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), frame_off, nframes * 8ull);
-    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), frame_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), frame_len, nframes * 4ull);
-    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    CK(read_table(st, frame_off, off_dev, frame_len, len_dev, nframes, offh, lenh));
     uint32_t max_len = 0;
     for (uint32_t i = 0; i < nframes; i++) {
         if ((lenh[i] & 7u) || (offh[i] & 7u)) return h->fail(SB200_E_INVALID, "frame_off and frame_len must be multiples of 8 samples (the reference fails on uiInputSize & 7 and needs 16-byte aligned buffers)");
-        if (lenh[i] > chips_total || offh[i] > chips_total - lenh[i]) return h->fail(SB200_E_INVALID, "frame exceeds chips_total");
+        if (!in_range(offh[i], lenh[i], chips_total)) return h->fail(SB200_E_INVALID, "frame exceeds chips_total");
         if (lenh[i] > max_len) max_len = lenh[i];
     }
     if ((in_dev && ((uintptr_t)chips & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device buffers must be 16-byte aligned");
-    const int8_t* d_in; int8_t* d_out; const uint64_t* d_off; const uint32_t* d_len;
-    if (in_dev) d_in = chips; else { CK(h->txpay.need(chips_total * 2ull + 16)); CK(cudaMemcpyAsync(h->txpay.p, chips, chips_total * 2ull, cudaMemcpyHostToDevice, st)); d_in = (const int8_t*)h->txpay.p; }
-    if (out_dev) d_out = out; else { CK(h->txout.need(chips_total * 2ull + 16)); d_out = (int8_t*)h->txout.p; }
-    if (off_dev) d_off = frame_off; else { CK(h->txoff.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->txoff.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); d_off = (const uint64_t*)h->txoff.p; }
-    if (len_dev) d_len = frame_len; else { CK(h->txlen.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->txlen.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); d_len = (const uint32_t*)h->txlen.p; }
+    const int8_t* d_in; int8_t* d_out = out; const uint64_t* d_off; const uint32_t* d_len;
+    CK(to_device(h->txpay, chips, in_dev, chips_total * 2ull, st, &d_in, 16));
+    if (!out_dev) { CK(h->txout.need(chips_total * 2ull + 16)); d_out = (int8_t*)h->txout.p; }
+    CK(to_device(h->txoff, off_dev ? frame_off : offh.data(), off_dev, nframes * 8ull, st, &d_off));
+    CK(to_device(h->txlen, len_dev ? frame_len : lenh.data(), len_dev, nframes * 4ull, st, &d_len));
     const uint64_t groups = (uint64_t)(max_len >> 3) * 2u; uint64_t ny = (groups + SB_FIR37_THREADS - 1) / SB_FIR37_THREADS; if (ny > 4096) ny = 4096; if (ny == 0) ny = 1;
     CK(cudaEventRecord(h->ev0, st));
     const dim3 grid(nframes, (unsigned)ny);
@@ -1337,28 +1341,26 @@ extern "C" int sb200_tx11b_legacy_batch(sb200_handle* h, const uint8_t* payload,
     }
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
-    std::vector<uint64_t> offh(nframes); std::vector<uint32_t> lenh(nframes);
-    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len), pay_dev = is_device_ptr(payload), out_dev = is_device_ptr(out);
-    if (off_dev) CK(cudaMemcpyAsync(offh.data(), pay_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), pay_off, nframes * 8ull);
-    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), pay_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), pay_len, nframes * 4ull);
-    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    std::vector<uint64_t> offh; std::vector<uint32_t> lenh;
+    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len);
+    CK(read_table(st, pay_off, off_dev, pay_len, len_dev, nframes, offh, lenh));
     uint32_t max_size = 0;
     for (uint32_t i = 0; i < nframes; i++) {
         const uint32_t size = job.fcs_in_payload ? lenh[i] : lenh[i] + 4u;            // PSDU bytes, FCS included
         if (job.fcs_in_payload && lenh[i] < 4u) return h->fail(SB200_E_INVALID, "with SB200_TX11B_LEGACY_FCS_IN_PAYLOAD every payload carries its 4 FCS bytes");
-        if (lenh[i] > 4095u || size > 4095u || lenh[i] > payload_total || offh[i] > payload_total - lenh[i]) return h->fail(SB200_E_INVALID, "payload slot out of range (PSDU 4 .. 4095 bytes incl. FCS)");
+        if (lenh[i] > 4095u || size > 4095u || !in_range(offh[i], lenh[i], payload_total)) return h->fail(SB200_E_INVALID, "payload slot out of range (PSDU 4 .. 4095 bytes incl. FCS)");
         if (tx11b_legacy_nsamples(size, short_preamble, job.data_chips_per_byte) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
         if (size > max_size) max_size = size;
     }
     job.desc_stride = (24u + max_size + 7u) & ~7u;
     const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len;
-    if (pay_dev) d_pay = payload; else { CK(h->txpay.need(payload_total)); CK(cudaMemcpyAsync(h->txpay.p, payload, payload_total, cudaMemcpyHostToDevice, st)); d_pay = (const uint8_t*)h->txpay.p; }
-    if (off_dev) d_off = pay_off; else { CK(h->txoff.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->txoff.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); d_off = (const uint64_t*)h->txoff.p; }
-    if (len_dev) d_len = pay_len; else { CK(h->txlen.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->txlen.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); d_len = (const uint32_t*)h->txlen.p; }
+    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay));
+    CK(to_device(h->txoff, off_dev ? pay_off : offh.data(), off_dev, nframes * 8ull, st, &d_off));
+    CK(to_device(h->txlen, len_dev ? pay_len : lenh.data(), len_dev, nframes * 4ull, st, &d_len));
     const size_t out_bytes = (size_t)nframes * out_stride_samples * 2;
-    int8_t* d_out = out; if (!out_dev) { CK(h->txout.need(out_bytes)); d_out = (int8_t*)h->txout.p; }
-    uint32_t* d_ns = nullptr; const bool ns_dev = nsamples && is_device_ptr(nsamples);
-    if (nsamples) { if (ns_dev) d_ns = nsamples; else { CK(h->txns.need(nframes * 4ull)); d_ns = (uint32_t*)h->txns.p; } }
+    Returns ret; int8_t* d_out; uint32_t* d_ns;
+    CK(ret.bind(h->txout, out, out_bytes, &d_out));
+    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
     CK(h->txdesc.need((size_t)nframes * job.desc_stride * 2ull));
     const uint64_t per_cta = SB_TX11B_LEGACY_THREADS * 8, ny = (out_stride_samples + per_cta - 1) / per_cta;
     if (ny > 65535u) return h->fail(SB200_E_INVALID, "out_stride_samples too large");
@@ -1377,10 +1379,7 @@ extern "C" int sb200_tx11b_legacy_batch(sb200_handle* h, const uint8_t* payload,
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 0; h->launches += 2;
     CK(cudaGetLastError());
-    bool sync = false;
-    if (!out_dev) { CK(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (nsamples && !ns_dev) { CK(cudaMemcpyAsync(nsamples, d_ns, nframes * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (sync) CK(cudaStreamSynchronize(st));
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -1403,31 +1402,29 @@ extern "C" int sb200_tx11a_legacy_batch(sb200_handle* h, const uint8_t* payload,
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
     int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
-    std::vector<uint64_t> offh(nframes); std::vector<uint32_t> lenh(nframes);
-    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len), pay_dev = is_device_ptr(payload), out_dev = is_device_ptr(out), pre_dev = is_device_ptr(preamble);
-    if (off_dev) CK(cudaMemcpyAsync(offh.data(), pay_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), pay_off, nframes * 8ull);
-    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), pay_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), pay_len, nframes * 4ull);
-    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    std::vector<uint64_t> offh; std::vector<uint32_t> lenh;
+    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len), pre_dev = is_device_ptr(preamble);
+    CK(read_table(st, pay_off, off_dev, pay_len, len_dev, nframes, offh, lenh));
     uint32_t max_nsym = 0;
     for (uint32_t i = 0; i < nframes; i++) {
         if (job.fcs_in_payload && lenh[i] < 4u) return h->fail(SB200_E_INVALID, "with SB200_TX11A_LEGACY_FCS_IN_PAYLOAD every payload carries its 4 FCS bytes");
         const uint32_t size = job.fcs_in_payload ? lenh[i] : lenh[i] + 4u;                // PSDU bytes, FCS included
-        if (lenh[i] > 4096u || size > 4096u || lenh[i] > payload_total || offh[i] > payload_total - lenh[i]) return h->fail(SB200_E_INVALID, "payload slot out of range (MPDU + FCS at most 4096 bytes)");
+        if (lenh[i] > 4096u || size > 4096u || !in_range(offh[i], lenh[i], payload_total)) return h->fail(SB200_E_INVALID, "payload slot out of range (MPDU + FCS at most 4096 bytes)");
         const uint32_t ns = tx11a_legacy_nsym(size, job.ndbps);
         if (tx11a_legacy_padded(ns, job.sr44) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
         if (ns > max_nsym) max_nsym = ns;
     }
     job.runs = (1u + max_nsym + SB_TXL_RUN - 1u) / SB_TXL_RUN;
     const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len; const uint32_t* d_pre;
-    if (pay_dev) d_pay = payload; else { CK(h->txpay.need(payload_total + 1)); CK(cudaMemcpyAsync(h->txpay.p, payload, payload_total, cudaMemcpyHostToDevice, st)); d_pay = (const uint8_t*)h->txpay.p; }
-    if (off_dev) d_off = pay_off; else { CK(h->txoff.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->txoff.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); d_off = (const uint64_t*)h->txoff.p; }
-    if (len_dev) d_len = pay_len; else { CK(h->txlen.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->txlen.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); d_len = (const uint32_t*)h->txlen.p; }
+    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay, 1));
+    CK(to_device(h->txoff, off_dev ? pay_off : offh.data(), off_dev, nframes * 8ull, st, &d_off));
+    CK(to_device(h->txlen, len_dev ? pay_len : lenh.data(), len_dev, nframes * 4ull, st, &d_len));
     if (pre_dev && ((uintptr_t)preamble & 3u) == 0) d_pre = (const uint32_t*)preamble;
     else { CK(h->txpre.need(640 * 4)); CK(cudaMemcpyAsync(h->txpre.p, preamble, 640 * 4, pre_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st)); d_pre = (const uint32_t*)h->txpre.p; }
     const size_t out_bytes = (size_t)nframes * out_stride_samples * 2;
-    int8_t* d_out = out; if (!out_dev) { CK(h->txout.need(out_bytes)); d_out = (int8_t*)h->txout.p; }
-    uint32_t* d_ns = nullptr; const bool ns_dev = nsamples && is_device_ptr(nsamples);
-    if (nsamples) { if (ns_dev) d_ns = nsamples; else { CK(h->txns.need(nframes * 4ull)); d_ns = (uint32_t*)h->txns.p; } }
+    Returns ret; int8_t* d_out; uint32_t* d_ns;
+    CK(ret.bind(h->txout, out, out_bytes, &d_out));
+    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
     const unsigned helpers = 4;                          // warps per frame for the preamble and the zero fill
     const uint64_t ny = (job.runs + helpers + SB_TXL_WARPS - 1) / SB_TXL_WARPS;
     if (ny > 65535u) return h->fail(SB200_E_INVALID, "too many symbols per frame");
@@ -1442,10 +1439,7 @@ extern "C" int sb200_tx11a_legacy_batch(sb200_handle* h, const uint8_t* payload,
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 0; h->launches += 1;
     CK(cudaGetLastError());
-    bool sync = false;
-    if (!out_dev) { CK(cudaMemcpyAsync(out, d_out, out_bytes, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (nsamples && !ns_dev) { CK(cudaMemcpyAsync(nsamples, d_ns, nframes * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (sync) CK(cudaStreamSynchronize(st));
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -1534,43 +1528,38 @@ extern "C" int sb200_tx11n_batch(sb200_handle* h, const uint8_t* payload, uint64
     CK(cudaSetDevice(h->device));
     int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
     rc = upload_tables_tx11n(h); if (rc != SB200_OK) return rc;
-    std::vector<uint64_t> offh(nframes); std::vector<uint32_t> lenh(nframes);
-    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len), pay_dev = is_device_ptr(payload), out_dev = is_device_ptr(out0);
-    if (out_dev != is_device_ptr(out1)) return h->fail(SB200_E_INVALID, "both output buffers must live on the same side");
-    if (off_dev) CK(cudaMemcpyAsync(offh.data(), pay_off, nframes * 8ull, cudaMemcpyDeviceToHost, st)); else memcpy(offh.data(), pay_off, nframes * 8ull);
-    if (len_dev) CK(cudaMemcpyAsync(lenh.data(), pay_len, nframes * 4ull, cudaMemcpyDeviceToHost, st)); else memcpy(lenh.data(), pay_len, nframes * 4ull);
-    if (off_dev || len_dev) CK(cudaStreamSynchronize(st));
+    std::vector<uint64_t> offh; std::vector<uint32_t> lenh;
+    const bool off_dev = is_device_ptr(pay_off), len_dev = is_device_ptr(pay_len);
+    if (is_device_ptr(out0) != is_device_ptr(out1)) return h->fail(SB200_E_INVALID, "both output buffers must live on the same side");
+    CK(read_table(st, pay_off, off_dev, pay_len, len_dev, nframes, offh, lenh));
     uint32_t max_nsym = 0;
     for (uint32_t i = 0; i < nframes; i++) {
-        if (lenh[i] + 4u > 4095u || offh[i] + lenh[i] > payload_total) return h->fail(SB200_E_INVALID, "payload slot out of range");
+        if (lenh[i] > 4091u || !in_range(offh[i], lenh[i], payload_total)) return h->fail(SB200_E_INVALID, "payload slot out of range");
         const uint32_t ns = tx11n_nsym_emitted(lenh[i], job, nullptr, nullptr);
         if ((uint64_t)lead_samples + 1600u + 160ull * ns > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
         if (ns > max_nsym) max_nsym = ns;
     }
     job.max_sym = 3u + max_nsym;
     const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len; const uint8_t* d_seed = nullptr;
-    if (pay_dev) d_pay = payload; else { CK(h->txpay.need(payload_total)); CK(cudaMemcpyAsync(h->txpay.p, payload, payload_total, cudaMemcpyHostToDevice, st)); d_pay = (const uint8_t*)h->txpay.p; }
-    if (off_dev) d_off = pay_off; else { CK(h->txoff.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->txoff.p, offh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st)); d_off = (const uint64_t*)h->txoff.p; }
-    if (len_dev) d_len = pay_len; else { CK(h->txlen.need(nframes * 4ull)); CK(cudaMemcpyAsync(h->txlen.p, lenh.data(), nframes * 4ull, cudaMemcpyHostToDevice, st)); d_len = (const uint32_t*)h->txlen.p; }
-    if (seeds) { if (is_device_ptr(seeds)) d_seed = seeds; else { CK(h->txseed.need(nframes)); CK(cudaMemcpyAsync(h->txseed.p, seeds, nframes, cudaMemcpyHostToDevice, st)); d_seed = (const uint8_t*)h->txseed.p; } }
+    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay));
+    CK(to_device(h->txoff, off_dev ? pay_off : offh.data(), off_dev, nframes * 8ull, st, &d_off));
+    CK(to_device(h->txlen, len_dev ? pay_len : lenh.data(), len_dev, nframes * 4ull, st, &d_len));
+    if (seeds) CK(to_device(h->txseed, seeds, is_device_ptr(seeds), nframes, st, &d_seed));
     const size_t out_bytes = (size_t)nframes * out_stride_samples * 4;
-    uint32_t* d_o0 = (uint32_t*)out0; uint32_t* d_o1 = (uint32_t*)out1;
-    if (!out_dev) { CK(h->txout.need(out_bytes)); CK(h->txout1.need(out_bytes)); d_o0 = (uint32_t*)h->txout.p; d_o1 = (uint32_t*)h->txout1.p; }
-    uint32_t* d_ns = nullptr; const bool ns_dev = nsamples && is_device_ptr(nsamples);
-    if (nsamples) { if (ns_dev) d_ns = nsamples; else { CK(h->txns.need(nframes * 4ull)); d_ns = (uint32_t*)h->txns.p; } }
+    Returns ret; int16_t* d_o0; int16_t* d_o1; uint32_t* d_ns;
+    CK(ret.bind(h->txout, out0, out_bytes, &d_o0));
+    CK(ret.bind(h->txout1, out1, out_bytes, &d_o1));
+    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
     const unsigned helpers = 8;
     dim3 grid(nframes, (2u * job.max_sym + helpers + SB_TX11N_WARPS - 1) / SB_TX11N_WARPS);
     CK(cudaEventRecord(h->ev0, st));
     CK(h->crc.need(nframes * 4ull));
     k_tx11a_crc<<<(nframes + 127) / 128, 128, 0, st>>>(d_pay, d_off, d_len, nframes, h->T, (uint32_t*)h->crc.p);
-    k_tx11n<<<grid, 32 * SB_TX11N_WARPS, 0, st>>>(d_pay, d_off, d_len, d_seed, nframes, job, h->T, h->X, h->XN, h->inv_deint, (const uint32_t*)h->crc.p, d_o0, d_o1, out_stride_samples, d_ns);
+    k_tx11n<<<grid, 32 * SB_TX11N_WARPS, 0, st>>>(d_pay, d_off, d_len, d_seed, nframes, job, h->T, h->X, h->XN, h->inv_deint, (const uint32_t*)h->crc.p, (uint32_t*)d_o0, (uint32_t*)d_o1, out_stride_samples, d_ns);
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 0; h->launches += 2;
     CK(cudaGetLastError());
-    bool sync = false;
-    if (!out_dev) { CK(cudaMemcpyAsync(out0, d_o0, out_bytes, cudaMemcpyDeviceToHost, st)); CK(cudaMemcpyAsync(out1, d_o1, out_bytes, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (nsamples && !ns_dev) { CK(cudaMemcpyAsync(nsamples, d_ns, nframes * 4ull, cudaMemcpyDeviceToHost, st)); sync = true; }
-    if (sync) CK(cudaStreamSynchronize(st));
+    CK(ret.finish(st));
     return SB200_OK;
 }
 
@@ -1643,9 +1632,11 @@ extern "C" int sb200_viterbi_k7(sb200_handle* h, const uint8_t* soft, uint64_t s
         CK(cudaMemcpy2DAsync(h->soft.p, d_stride, soft, soft_stride, nsoft, nblocks, is_device_ptr(soft) ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st));
         d_soft = (const uint8_t*)h->soft.p;
     }
-    const bool od = is_device_ptr(out);
-    uint8_t* d_out = out; uint64_t d_ostride = out_stride;
-    if (!od) { d_ostride = (frame_len_bytes + 2ull + 15ull) & ~15ull; CK(h->out.need(nblocks * d_ostride)); d_out = (uint8_t*)h->out.p; }
+    uint8_t* d_out = out; uint64_t d_ostride = out_stride; Returns ret;
+    if (!is_device_ptr(out)) {
+        d_ostride = (frame_len_bytes + 2ull + 15ull) & ~15ull; CK(h->out.need(nblocks * d_ostride)); d_out = (uint8_t*)h->out.p;
+        ret.bind2d(out, out_stride, d_out, d_ostride, frame_len_bytes + 2ull, nblocks);
+    }
     CK(h->status.need(nblocks * 4ull)); CK(h->crc.need(nblocks * 4ull));
     VitJob job{}; job.code_rate = (uint32_t)code_rate; job.frame_len = frame_len_bytes; job.nsoft = nsoft; job.depth = depth; job.lookahead = lookahead; job.raw = 1;
     CK(cudaEventRecord(h->ev0, st));
@@ -1663,9 +1654,6 @@ extern "C" int sb200_viterbi_k7(sb200_handle* h, const uint8_t* soft, uint64_t s
     CK(cudaEventRecord(h->ev1, st));
     h->timed = true; h->nk = 0; h->launches += 1;
     CK(cudaGetLastError());
-    if (!od) {
-        CK(cudaMemcpy2DAsync(out, out_stride, d_out, d_ostride, frame_len_bytes + 2ull, nblocks, cudaMemcpyDeviceToHost, st));
-        CK(cudaStreamSynchronize(st));
-    }
+    CK(ret.finish(st));
     return SB200_OK;
 }
