@@ -62,6 +62,14 @@ def load_library():
         _lib = lib
     return _lib
 
+def _payload_table(payloads):
+    """List of payloads -> (flat uint8 bytes, offsets uint64, lengths uint32); one zero byte stands for an all-empty list."""
+    lens = np.array([len(p) for p in payloads], np.uint32); offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.uint64)
+    flat = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8) for p in payloads]) if lens.sum() else np.zeros(1, np.uint8))
+    return flat, offs, lens
+
+_NDBPS_11A = {6000: 24, 9000: 36, 12000: 48, 18000: 72, 24000: 96, 36000: 144, 48000: 192, 54000: 216}   # 802.11a data bits per OFDM symbol
+
 def _ptr(a):
     """numpy array -> host pointer; torch tensor / int -> raw (device or pinned) pointer."""
     if a is None:
@@ -161,15 +169,14 @@ class Engine:
 
     def tx11a_batch(self, payloads, rate_kbps, seeds=None, lead=0, sample_bits=8, out_stride=None):
         """payloads: list of uint8 arrays (MPDUs without FCS) -> (samples [F, out_stride, 2] int8 or int16, nsamples [F])."""
-        lens = np.array([len(p) for p in payloads], np.uint32); offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.uint64)
-        flat = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8) for p in payloads]) if lens.sum() else np.zeros(1, np.uint8))
+        flat, offs, lens = _payload_table(payloads)
         from math import ceil
         if out_stride is None:
-            nd = {6000: 24, 9000: 36, 12000: 48, 18000: 72, 24000: 96, 36000: 144, 48000: 192, 54000: 216}[rate_kbps]
+            nd = _NDBPS_11A[rate_kbps]
             out_stride = lead + 640 + 160 * (2 + ceil((int(lens.max()) + 7) * 8 / nd) + 1) + 32
         out = np.zeros((len(lens), out_stride, 2), np.int8 if sample_bits == 8 else np.int16); ns = np.zeros(len(lens), np.uint32)
         sd = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.uint8)
-        self.tx11a_raw(_ptr(flat), max(int(lens.sum()), 1), _ptr(offs), _ptr(lens), 0 if sd is None else _ptr(sd), len(lens), rate_kbps, lead, sample_bits, _ptr(out), out_stride, _ptr(ns))
+        self.tx11a_raw(_ptr(flat), flat.size, _ptr(offs), _ptr(lens), 0 if sd is None else _ptr(sd), len(lens), rate_kbps, lead, sample_bits, _ptr(out), out_stride, _ptr(ns))
         return out, ns
 
     def tx11n_raw(self, pay_ptr, pay_total, off_ptr, len_ptr, seed_ptr, nframes, mcs, lead, out0_ptr, out1_ptr, out_stride, ns_ptr, stream=0):
@@ -179,14 +186,13 @@ class Engine:
 
     def tx11n_batch(self, payloads, mcs, seeds=None, lead=0, out_stride=None):
         """payloads: list of uint8 arrays (MPDUs without FCS) -> (stream 0 [F, out_stride, 2] int16, stream 1, nsamples [F]) at 40 Msps."""
-        lens = np.array([len(p) for p in payloads], np.uint32); offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.uint64)
-        flat = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8) for p in payloads]) if lens.sum() else np.zeros(1, np.uint8))
+        flat, offs, lens = _payload_table(payloads)
         if out_stride is None:
             nd = {8: 52, 9: 104, 10: 156}.get(mcs, 52)
             out_stride = lead + 1600 + 160 * (-(-((int(lens.max()) + 4) * 8 + 22) // nd) + 1)
         o0 = np.zeros((len(lens), out_stride, 2), np.int16); o1 = np.zeros_like(o0); ns = np.zeros(len(lens), np.uint32)
         sd = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.uint8)
-        self.tx11n_raw(_ptr(flat), max(int(lens.sum()), 1), _ptr(offs), _ptr(lens), 0 if sd is None else _ptr(sd), len(lens), mcs, lead, _ptr(o0), _ptr(o1), out_stride, _ptr(ns))
+        self.tx11n_raw(_ptr(flat), flat.size, _ptr(offs), _ptr(lens), 0 if sd is None else _ptr(sd), len(lens), mcs, lead, _ptr(o0), _ptr(o1), out_stride, _ptr(ns))
         return o0, o1, ns
 
     def tx11b_raw(self, pay_ptr, pay_total, off_ptr, len_ptr, nframes, rate_kbps, init_phase, lead, bits, out_ptr, out_stride, ns_ptr, stream=0, fp_ptr=0):
@@ -196,14 +202,13 @@ class Engine:
 
     def tx11b_batch(self, payloads, rate_kbps, init_phase=0, lead=0, sample_bits=8, out_stride=None, return_phase=False):
         """payloads: list of uint8 arrays (MPDUs without FCS) -> (samples [F, out_stride, 2] int8 or int16 at 44 Msps, nsamples [F])."""
-        lens = np.array([len(p) for p in payloads], np.uint32); offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.uint64)
-        flat = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8) for p in payloads]) if lens.sum() else np.zeros(1, np.uint8))
+        flat, offs, lens = _payload_table(payloads)
         if out_stride is None:
             cpb = {1000: 88, 2000: 44, 5500: 16, 11000: 8}.get(rate_kbps, 8)      # an unknown rate is the library's error to report
             out_stride = (lead + (24 * 88 + (int(lens.max()) + 4) * cpb + 5) * 4 + 15) // 8 * 8
         out = np.zeros((len(lens), out_stride, 2), np.int8 if sample_bits == 8 else np.int16); ns = np.zeros(len(lens), np.uint32)
         fp = np.zeros(len(lens), np.uint32)
-        self.tx11b_raw(_ptr(flat), max(int(lens.sum()), 1), _ptr(offs), _ptr(lens), len(lens), rate_kbps, init_phase, lead, sample_bits, _ptr(out), out_stride, _ptr(ns), 0, _ptr(fp))
+        self.tx11b_raw(_ptr(flat), flat.size, _ptr(offs), _ptr(lens), len(lens), rate_kbps, init_phase, lead, sample_bits, _ptr(out), out_stride, _ptr(ns), 0, _ptr(fp))
         return (out, ns, fp) if return_phase else (out, ns)
 
     def rxblocks_desc(self, raw):
@@ -248,14 +253,13 @@ class Engine:
     def tx11b_legacy_batch(self, payloads, rate_kbps, short_preamble=False, filter=1, fcs_in_payload=False, out_stride=None):
         """The legacy 802.11b transmitter (BB11BPMDBufferTx4X* and, filter 1 / 2, the SSE / ASM 37-tap filter).  payloads: list of uint8 arrays,
         MPDUs without FCS (or with it, fcs_in_payload=True) -> (COMPLEX8 samples int8 [F, out_stride, 2] at 44 Msps, nsamples [F])."""
-        lens = np.array([len(p) for p in payloads], np.uint32); offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.uint64)
-        flat = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8) for p in payloads]) if lens.sum() else np.zeros(1, np.uint8))
+        flat, offs, lens = _payload_table(payloads)
         if out_stride is None:
             size = int(lens.max()) + (0 if fcs_in_payload else 4)
             cpb = {1000: 0 if short_preamble else 88, 2000: 44, 5500: 16, 11000: 8}.get(rate_kbps, 8)     # an unknown rate is the library's error to report
             out_stride = (4 * ((1056 if short_preamble else 2112) + size * cpb) + 37 + 127) // 128 * 128
         out = np.zeros((len(lens), out_stride, 2), np.int8); ns = np.zeros(len(lens), np.uint32)
-        self.tx11b_legacy_raw(_ptr(flat), max(int(lens.sum()), 1), _ptr(offs), _ptr(lens), len(lens), rate_kbps, int(bool(short_preamble)),
+        self.tx11b_legacy_raw(_ptr(flat), flat.size, _ptr(offs), _ptr(lens), len(lens), rate_kbps, int(bool(short_preamble)),
                               self.TX11B_LEGACY_FCS_IN_PAYLOAD if fcs_in_payload else 0, filter, _ptr(out), out_stride, _ptr(ns))
         return out, ns
 
@@ -269,21 +273,20 @@ class Engine:
     @staticmethod
     def tx11a_legacy_nsamples(psdu_len, rate_kbps, sample_rate_mhz=40):
         """Samples BB11ATxFrameMod writes for a PSDU of psdu_len bytes (FCS included): the signal rounded up to 128 bytes."""
-        ndbps = {6000: 24, 9000: 36, 12000: 48, 18000: 72, 24000: 96, 36000: 144, 48000: 192, 54000: 216}.get(rate_kbps, 24)   # an unknown rate is the library's error
+        ndbps = _NDBPS_11A.get(rate_kbps, 24)             # an unknown rate is the library's error
         nsym = (22 + 8 * psdu_len + ndbps - 1) // ndbps
         return ((176 if sample_rate_mhz == 44 else 160) * (5 + nsym) + 8 + 63) // 64 * 64
 
     def tx11a_legacy_batch(self, payloads, rate_kbps, preamble, sample_rate_mhz=40, fcs_in_payload=False, out_stride=None):
         """The legacy 802.11a transmitter (BB11ATxFrameMod).  payloads: list of uint8 arrays, MPDUs without FCS (or with it, fcs_in_payload=True);
         preamble: the reference's 640-sample PREAMBLE40_11A_LUT, int16 [640, 2] -> (COMPLEX8 samples int8 [F, out_stride, 2], nsamples [F])."""
-        lens = np.array([len(p) for p in payloads], np.uint32); offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.uint64)
-        flat = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8) for p in payloads]) if lens.sum() else np.zeros(1, np.uint8))
+        flat, offs, lens = _payload_table(payloads)
         pre = np.ascontiguousarray(preamble, dtype=np.int16)
         if pre.size != 1280: raise Sb200Error("preamble must be 640 COMPLEX16 samples")
         if out_stride is None:
             out_stride = self.tx11a_legacy_nsamples(int(lens.max()) + (0 if fcs_in_payload else 4), rate_kbps, sample_rate_mhz)
         out = np.zeros((len(lens), out_stride, 2), np.int8); ns = np.zeros(len(lens), np.uint32)
-        self.tx11a_legacy_raw(_ptr(flat), max(int(lens.sum()), 1), _ptr(offs), _ptr(lens), len(lens), rate_kbps, sample_rate_mhz,
+        self.tx11a_legacy_raw(_ptr(flat), flat.size, _ptr(offs), _ptr(lens), len(lens), rate_kbps, sample_rate_mhz,
                               self.TX11A_LEGACY_FCS_IN_PAYLOAD if fcs_in_payload else 0, _ptr(pre), _ptr(out), out_stride, _ptr(ns))
         return out, ns
 

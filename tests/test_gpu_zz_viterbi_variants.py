@@ -50,3 +50,20 @@ def test_viterbi_variants_on_mixed_batches():
     finally:
         if old is None: os.environ.pop("SB200_VITERBI", None)
         else: os.environ["SB200_VITERBI"] = old
+
+@pytest.mark.parametrize("name, launches", [("rx11a_batch", 6), ("rx11n_batch", 5), ("rx11n_batch_mcs15", 5), ("viterbi_k7", 1)])
+def test_v2_launch_counts(name, launches):
+    """sb200_launch_count delta of a warm call under SB200_VITERBI=v2 (the quad kernel, one launch per code rate): the 802.11a receiver
+    counts its three quads; the 802.11n receiver counts two, also when ht_mcs_limit 15 makes it launch the CR_23 one as well."""
+    from test_gpu_abi_residency import BOOKKEEPING
+    old = os.environ.get("SB200_VITERBI")
+    os.environ["SB200_VITERBI"] = "v2"
+    try:
+        e = api.Engine(0)
+        call = BOOKKEEPING[name][0](e)
+        call(); n0 = e.launches; call()
+        assert e.launches - n0 == launches
+        e.close()
+    finally:
+        if old is None: os.environ.pop("SB200_VITERBI", None)
+        else: os.environ["SB200_VITERBI"] = old
