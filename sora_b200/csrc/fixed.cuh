@@ -77,8 +77,8 @@ __host__ __device__ __forceinline__ void dft4(cs16& v0, cs16& v1, cs16& v2, cs16
 
 // ------------------------------------------------------------------------------------------------
 // Packed forms: one complex int16 per 32-bit word, re in bits 0-15, im in bits 16-31 (the layout of pack()), on the 16x2 SIMD
-// integer instructions.  Each one states when it equals its scalar counterpart above; tests/test_cpu_packed.py checks that on the
-// host, exhaustively or on random and edge words.
+// integer instructions.  Each one states when it equals its scalar counterpart above; tests/test_cpu_packed.py and
+// tests/test_cpu_packed_rot.py check that on the host, exhaustively or on random and edge words.
 // ------------------------------------------------------------------------------------------------
 // paddw / psubw: per-half wrap-around.  Equal to adds / subs wherever the exact sum lies in [-32768, 32767].
 __device__ __forceinline__ uint32_t pk_add(uint32_t a, uint32_t b) { return __vadd2(a, b); }
@@ -104,6 +104,21 @@ __device__ __forceinline__ uint32_t pk_cmul(int re, int im, cfac f) {
     return __byte_perm(x, y, 0x7632);
 }
 __device__ __forceinline__ uint32_t pk_cmul(uint32_t a, cfac f) { return pk_cmul((int)(short)a, (int)a >> 16, f); }
+// The two 32-bit sums of pk_cmul without the repack: (int)x >> 16 and (int)y >> 16 are the product's re and im, ready for the next product.
+__device__ __forceinline__ void pk_cmul_xy(int re, int im, const cfac& f, int& x, int& y) {
+    x = (int)((uint32_t)re * (uint32_t)f.re + (uint32_t)im * (uint32_t)f.nim); y = (int)((uint32_t)re * (uint32_t)f.im + (uint32_t)im * (uint32_t)f.re);
+}
+// cmul_q15(a, unpack(w)) for a word w of the rotation table, (round(32767 cos), -round(32767 sin)): both halves lie in [-32767, 32767],
+// where neg16 is plain negation, so the real part is a.re * re - a.im * im and the factor needs no third component.  Built straight from
+// the word: each half sign-extended and doubled (S = 15 of mkfac).
+struct rfac { int re, im; };
+__device__ __forceinline__ rfac fac_rotw(uint32_t w) { return rfac{(int)(w << 16) >> 15, (int)(w & 0xFFFF0000u) >> 15}; }
+__device__ __forceinline__ void pk_cmul_xy(int re, int im, rfac f, int& x, int& y) {
+    x = (int)((uint32_t)re * (uint32_t)f.re - (uint32_t)im * (uint32_t)f.im); y = (int)((uint32_t)re * (uint32_t)f.im + (uint32_t)im * (uint32_t)f.re);
+}
+__device__ __forceinline__ uint32_t pk_cmul(int re, int im, rfac f) { int x, y; pk_cmul_xy(re, im, f, x, y); return __byte_perm((uint32_t)x, (uint32_t)y, 0x7632); }
+// sx16(th + 0x8000) for th in [-32768, 32767] (a pilot angle turned by pi): flipping bit 15 and every bit above it.  flip = 0 leaves th.
+__host__ __device__ __forceinline__ int turn_pi(int th, bool flip) { return th ^ (flip ? (int)0xFFFF8000u : 0); }
 // The demapper's index byte per half, (uint8)min(max(v >> 4, -128), 127): >> 4 is monotone and maps -2048 / 2047 to -128 / 127, so
 // clamping v to [-2048, 2047] first gives the same value, and its bits 4..11 are that byte.  Any input; re's byte in bits 4..11, im's in 20..27.
 __device__ __forceinline__ uint32_t pk_demap_clamp(uint32_t a) { return __vmins2(__vmaxs2(a, 0xF800F800u), 0x07FF07FFu); }

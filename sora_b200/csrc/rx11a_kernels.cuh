@@ -31,7 +31,6 @@ __device__ __forceinline__ int d_uatan2(const DevTables& T, int y, int x) {     
 __device__ __forceinline__ uint32_t d_rotw(const DevTables& T, int th) {          // (ucos(th), -usin(th)), packed
     return __ldg(T.rot + ((unsigned)th & 0xFFFFu));
 }
-__device__ __forceinline__ cs16 d_rot(const DevTables& T, int th) { return unpack(d_rotw(T, th)); }
 
 // ------------------------------------------------------------------------------------------------
 // carrier sense
@@ -240,10 +239,14 @@ __device__ __forceinline__ int data_index(int bin) {   // demapper11a.hpp:22-36 
     if (bin >= 1 && bin <= 26) { if (bin == 7 || bin == 21) return -1; return 24 + bin - 1 - (bin > 7) - (bin > 21); }
     return -1;
 }
+__device__ __forceinline__ int data_bin(int d) {       // inverse of data_index, d = 0..47
+    return d < 24 ? 38 + d + (d >= 5) + (d >= 18) : d - 23 + (d >= 30) + (d >= 43);
+}
 
 #define SB_FRONT_WARPS 4
 #ifndef SB_FRONT_MINB
-#define SB_FRONT_MINB 5           // resident CTAs per SM the register allocation aims at: 6 spills on sm_90a and measured 5 % slower (tools/front_sweep.sh)
+#define SB_FRONT_MINB 5           // resident CTAs per SM the register allocation aims at; front end on the H100 (tools/front_sweep.sh, DESIGN.md §8):
+                                  // 4 -> 2.50 ms (123 registers), 5 -> 2.32 ms (96), 6 -> 2.83 ms (80 registers, 184 B of spill stores)
 #endif
 // Two OFDM symbols are transformed at once: lanes 0-15 run the three radix stages of symbol A, lanes 16-31 those of
 // symbol B (16 butterflies per stage = 16 lanes, so every lane is busy); the first stage consumes the freq-compensated
@@ -286,7 +289,14 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
     const uint32_t s0 = fi.detect_vec * 4u;            // first 20 Msps sample of the 144-sample LTS block
     if (fi.detect_vec + 36u > nvec) { if (lane == 0) info[f].status = E_NO_FRAME; return; }
     const int half = lane >> 4, hl = lane & 15;        // FFT role: which of the two symbols, which butterfly
-    const int b0 = lane, b1 = lane + 32;               // post-FFT role: this lane's two bins
+    // Post-FFT role: this lane's two bins.  Lanes 0-23 own the data subcarriers d0 = 6 (lane / 3) + lane % 3 and d1 = d0 + 3 (demapper
+    // order): at 64-QAM the 802.11a de-interleaver puts coded bit i of d0 at an even position and bit (2 0 1 5 3 4)[i] of d1 right after
+    // it, so the pair's soft bits leave as six 16-bit stores.  Lanes 24-27 own the pilots (bins 43, 57, 7, 21) in b0, the twelve zero
+    // bins (0, 27..37) fill the rest.
+    const int d0 = lane < 24 ? 6 * (lane / 3) + lane % 3 : -1, d1 = lane < 24 ? d0 + 3 : -1;
+    const int j24 = lane - 24;
+    const int b0 = lane < 24 ? data_bin(d0) : j24 < 4 ? (0x1507392B >> (8 * j24)) & 0xFF : j24 == 4 ? 0 : 22 + j24;
+    const int b1 = lane < 24 ? data_bin(d1) : 30 + j24;
     const int r0 = bitrev6(b0), r1 = bitrev6(b1);
     const cfac w64_1 = fac_tw(unpack(__ldg(T.tw64 + hl))), w64_2 = fac_tw(unpack(__ldg(T.tw64 + 16 + hl))), w64_3 = fac_tw(unpack(__ldg(T.tw64 + 32 + hl)));
     const cfac w16_1 = fac_tw(unpack(__ldg(T.tw16 + (hl & 3)))), w16_2 = fac_tw(unpack(__ldg(T.tw16 + 4 + (hl & 3)))), w16_3 = fac_tw(unpack(__ldg(T.tw16 + 8 + (hl & 3))));
@@ -308,16 +318,17 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
     };
     // ---- T11aLTS (channel_11a.hpp:34-230) -----------------------------------------------------------
     {   // FreqOffsetEstimate<16> (dspalg.hpp:227-243): sum over the 64 samples of (LTS2 * conj(LTS1 >> 1)) >> 5
-        cs16 l0 = sra(unpack(__ldg(x + ((s0 + 8u + b0) << sh))), 1), l1 = sra(unpack(__ldg(x + ((s0 + 8u + b1) << sh))), 1);
-        cs16 h0 = unpack(__ldg(x + ((s0 + 72u + b0) << sh))), h1 = unpack(__ldg(x + ((s0 + 72u + b1) << sh)));
+        const uint32_t n0 = (uint32_t)lane, n1 = n0 + 32u;
+        cs16 l0 = sra(unpack(__ldg(x + ((s0 + 8u + n0) << sh))), 1), l1 = sra(unpack(__ldg(x + ((s0 + 8u + n1) << sh))), 1);
+        cs16 h0 = unpack(__ldg(x + ((s0 + 72u + n0) << sh))), h1 = unpack(__ldg(x + ((s0 + 72u + n1) << sh)));
         int re0, im0, re1, im1; cmul_conj32(re0, im0, h0, l0); cmul_conj32(re1, im1, h1, l1);
         int sr = wadd(re0 >> 5, re1 >> 5), si = wadd(im0 >> 5, im1 >> 5);
         for (int o = 16; o; o >>= 1) { sr = wadd(sr, __shfl_xor_sync(FULL, sr, o)); si = wadd(si, __shfl_xor_sync(FULL, si, o)); }
         fi.cfo_est = (int)(short)(((uint32_t)d_uatan2(T, si, sr)) / 64u);  // short / size_t (dspalg.hpp:242)
     }
-    cfac fcv[4];                                       // FreqCoeffs of this lane's four time samples (dspalg.hpp:201-208)
+    rfac fcv[4];                                       // FreqCoeffs of this lane's four time samples (dspalg.hpp:201-208)
 #pragma unroll
-    for (int j = 0; j < 4; j++) fcv[j] = fac_q15(d_rot(T, fi.cfo_est * (hl + 16 * j)));
+    for (int j = 0; j < 4; j++) fcv[j] = fac_rotw(d_rotw(T, fi.cfo_est * (hl + 16 * j)));
     auto fcomp = [&](uint32_t w, int j) { return pk_cmul((int)(short)w >> 1, (int)w >> 17, fcv[j]); };   // cmul_q15(sra(w, 1), FreqCoeffs)
     auto load4 = [&](uint32_t first, uint32_t (&v)[4]) {  // (x >> 1) * FreqCoeffs for samples first + hl + 16 j
 #pragma unroll
@@ -337,74 +348,83 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
         ch0 = inv(unpack(xb[r0]), b0); ch1 = inv(unpack(xb[r1]), b1);
     }
     __syncwarp();
-    if (taps.freq_coeffs) { taps.freq_coeffs[(size_t)f * 64 + b0] = pack(d_rot(T, fi.cfo_est * b0)); taps.freq_coeffs[(size_t)f * 64 + b1] = pack(d_rot(T, fi.cfo_est * b1));
+    if (taps.freq_coeffs) { taps.freq_coeffs[(size_t)f * 64 + b0] = d_rotw(T, fi.cfo_est * b0); taps.freq_coeffs[(size_t)f * 64 + b1] = d_rotw(T, fi.cfo_est * b1);
                             taps.chan_coeffs[(size_t)f * 64 + b0] = pack(ch0); taps.chan_coeffs[(size_t)f * 64 + b1] = pack(ch1); }
     // ---- symbols -----------------------------------------------------------------------------------
-    const int k0 = b0, k1 = b1 - 64;                   // signed subcarrier numbers of this lane's bins
-    const bool v0 = (k0 >= 1 && k0 <= 26), v1 = (k1 >= -26 && k1 <= -1);
-    const int d0 = data_index(b0), d1 = data_index(b1);
+    const int k0 = b0 < 32 ? b0 : b0 - 64, k1 = b1 < 32 ? b1 : b1 - 64;   // signed subcarrier numbers of this lane's bins
+    const bool v0 = k0 != 0 && k0 >= -26 && k0 <= 26, v1 = k1 != 0 && k1 >= -26 && k1 <= 26;
     // bins 28..35 (SSE vectors 7,8) are forced to zero: their channel coefficient is zero, so is everything multiplied by it
     const cfac eq0 = fac_mul8(ch0), eq1 = fac_mul8(ch1);
-    cfac comp0 = fac_q15(mk(0x7fff, 0)), comp1 = comp0;
-    int CFO_comp = 0, SFO_comp = 0, CFO_tr = 0, SFO_tr = 0; unsigned symbol_count = 127;
+    rfac comp0 = fac_rotw(0x7fffu), comp1 = comp0;
+    // The tracker's accumulators only ever index the rotation table (mod 2^16) and feed each other by addition, so they wrap mod 2^32
+    // instead of being truncated with sx16 at every step: the low 16 bits are the same.
+    uint32_t CFO_comp = 0, SFO_comp = 0, CFO_tr = 0, SFO_tr = 0; unsigned symbol_count = 127;
     int plcp_data = 0; uint32_t remain = 0; uint32_t soft_bytes = 0; int nbpsc = 1;
     uint8_t* sout = soft_out + (size_t)f * soft_stride;
     uint32_t status = E_SUCCESS;
-    unsigned short pos0[6], pos1[6];                   // where this lane's soft bits go after de-interleaving
+    // Where this lane's soft bits go after de-interleaving, as byte offsets into s_soft: at 64-QAM pos[i] is the even position of bit i of
+    // d0 (the 16-bit store of the pair); at the other rates the low half of pos[i] is bit i of d0, the high half bit i of d1.
+    uint32_t pos[6];
     auto load_positions = [&](int nb) {
         const uint16_t* inv = inv_deint + (nb == 1 ? 0 : nb == 2 ? 48 : nb == 4 ? 144 : 336);
+        const uint32_t base = (uint32_t)wib * 288u;
 #pragma unroll
         for (int i = 0; i < 6; i++) {
-            pos0[i] = (d0 >= 0 && i < nb) ? __ldg(inv + d0 * nb + i) : (unsigned short)0;
-            pos1[i] = (d1 >= 0 && i < nb) ? __ldg(inv + d1 * nb + i) : (unsigned short)0;
+            if (d0 < 0 || i >= nb) pos[i] = 0;
+            else if (nb == 6) pos[i] = base + __ldg(inv + d0 * 6 + i);
+            else pos[i] = (base + __ldg(inv + d0 * nb + i)) | ((base + __ldg(inv + d1 * nb + i)) << 16);
         }
     };
     load_positions(1);
+    uint8_t* const s8 = &s_soft[0][0];
     // everything behind the FFT for one symbol whose spectrum sits in s_fft[wib][h]; returns false when the frame ended
     auto post_fft = [&](int h, uint32_t sym) -> bool {
         const uint32_t* xb = s_fft[wib][h];
         const uint32_t F0 = xb[r0], F1 = xb[r1];
-        const uint32_t E0 = pk_cmul(F0, eq0), E1 = pk_cmul(F1, eq1);                  // channel_11a.hpp:551-579
-        const uint32_t C0 = pk_cmul(E0, comp0), C1 = pk_cmul(E1, comp1);              // freqoffset.hpp:28-30
-        int th = 0;                                                                    // pilot.hpp:168-232
-        {   // one table walk for the whole warp: bins 43 (-21) and 57 (-7) sit in C1 of lanes 11 / 25, bins 7 and 21 in C0 of lanes 7 / 21
-            const bool hi = lane == 11 || lane == 25, neg = lane == 21;               // bin 21's pilot is sent negated
-            const cs16 p = unpack(hi ? C1 : C0);
-            const int py = neg ? -p.im : p.im, px = neg ? -p.re : p.re;
-            const int a = d_uatan2(T, py, px);
-            if (hi || lane == 7 || lane == 21) th = a;
-        }
-        if (s_pilot[symbol_count]) th = sx16(th + 0x8000);
-        int th1 = __shfl_sync(FULL, th, 11), th2 = __shfl_sync(FULL, th, 25), th3 = __shfl_sync(FULL, th, 7), th4 = __shfl_sync(FULL, th, 21);
+        int e0x, e0y, e1x, e1y, c0x, c0y, c1x, c1y;                                    // products as 32-bit sums, value = sum >> 16
+        pk_cmul_xy((int)(short)F0, (int)F0 >> 16, eq0, e0x, e0y);                       // channel_11a.hpp:551-579
+        pk_cmul_xy((int)(short)F1, (int)F1 >> 16, eq1, e1x, e1y);
+        pk_cmul_xy(e0x >> 16, e0y >> 16, comp0, c0x, c0y);                              // freqoffset.hpp:28-30
+        pk_cmul_xy(e1x >> 16, e1y >> 16, comp1, c1x, c1y);
+        const int C0re = c0x >> 16, C0im = c0y >> 16, C1re = c1x >> 16, C1im = c1y >> 16;
+        // pilot.hpp:168-232: one table walk for the whole warp, the pilots sit in C0 of lanes 24-27 (bins 43, 57, 7, 21; bin 21's is sent negated)
+        const bool neg = lane == 27;
+        const int th = turn_pi(d_uatan2(T, neg ? -C0im : C0im, neg ? -C0re : C0re), s_pilot[symbol_count]);
+        const int th1 = __shfl_sync(FULL, th, 24), th2 = __shfl_sync(FULL, th, 25), th3 = __shfl_sync(FULL, th, 26), th4 = __shfl_sync(FULL, th, 27);
         symbol_count++; if (symbol_count >= 127) symbol_count = 0;
-        int avg = sx16((th1 + th2 + th3 + th4) / 4);
-        int del = sx16(((th3 - th1) / 28 + (th4 - th2) / 28) >> 1);
+        // the angles are int16, so the sum / 4 lies in [-32768, 32767] and each difference / 28 in [-2340, 2340]: the sx16 of both is the identity
+        const int avg = (th1 + th2 + th3 + th4) / 4;
+        const int del = ((th3 - th1) / 28 + (th4 - th2) / 28) >> 1;
+        CFO_tr += (uint32_t)(avg >> 2); SFO_tr += (uint32_t)(del >> 2);
+        CFO_comp += (uint32_t)avg + CFO_tr; SFO_comp += (uint32_t)del + SFO_tr;
+        // next symbol's phase compensation; only the rotated bins below use it, every other bin's R is zero whatever its C
+        comp0 = fac_rotw(d_rotw(T, (int)(CFO_comp + (uint32_t)k0 * SFO_comp)));
+        comp1 = fac_rotw(d_rotw(T, (int)(CFO_comp + (uint32_t)k1 * SFO_comp)));
         // subcarriers -26..-1, 1..26 are rotated, every other bin becomes zero
-        const uint32_t R0 = pk_cmul(C0, v0 ? fac_q15(d_rot(T, avg + k0 * del)) : cfac{0, 0, 0});
-        const uint32_t R1 = pk_cmul(C1, v1 ? fac_q15(d_rot(T, avg + k1 * del)) : cfac{0, 0, 0});
-        CFO_tr = sx16(CFO_tr + (avg >> 2)); SFO_tr = sx16(SFO_tr + (del >> 2));
-        CFO_comp = sx16(CFO_comp + avg + CFO_tr); SFO_comp = sx16(SFO_comp + del + SFO_tr);
-        if (v0) comp0 = fac_q15(d_rot(T, CFO_comp + k0 * SFO_comp));
-        if (v1) comp1 = fac_q15(d_rot(T, CFO_comp + k1 * SFO_comp));
+        const uint32_t R0 = pk_cmul(C0re, C0im, fac_rotw(v0 ? d_rotw(T, avg + k0 * del) : 0u));
+        const uint32_t R1 = pk_cmul(C1re, C1im, fac_rotw(v1 ? d_rotw(T, avg + k1 * del) : 0u));
         if (taps.fft_out && sym < taps.max_sym) {
             size_t o = ((size_t)f * taps.max_sym + sym) * 64;
             taps.fft_out[o + b0] = F0; taps.fft_out[o + b1] = F1;
-            taps.equalized[o + b0] = E0; taps.equalized[o + b1] = E1;
+            taps.equalized[o + b0] = __byte_perm((uint32_t)e0x, (uint32_t)e0y, 0x7632); taps.equalized[o + b1] = __byte_perm((uint32_t)e1x, (uint32_t)e1y, 0x7632);
             taps.tracked[o + b0] = R0; taps.tracked[o + b1] = R1;
         }
         // soft demap (demapper.h:141-151 limit + LUTs) scattered through the inverse de-interleaver map
         const int ncbps = 48 * nbpsc;
-        auto demap = [&](uint32_t r, int d, const unsigned short (&pos)[6]) {
-            if (d < 0) return;
-            const uint32_t c = pk_demap_clamp(r);
-            const uint32_t wr = s_demap[(c >> 4) & 0xFF], wi = s_demap[(c >> 20) & 0xFF];
-            if (nbpsc == 1) { sb[pos[0]] = (uint8_t)wr; }
-            else if (nbpsc == 2) { sb[pos[0]] = (uint8_t)wr; sb[pos[1]] = (uint8_t)wi; }
-            else if (nbpsc == 4) { sb[pos[0]] = (uint8_t)wr; sb[pos[1]] = (uint8_t)(wr >> 8); sb[pos[2]] = (uint8_t)wi; sb[pos[3]] = (uint8_t)(wi >> 8); }
-            else { sb[pos[0]] = (uint8_t)wr; sb[pos[1]] = (uint8_t)(wr >> 16); sb[pos[2]] = (uint8_t)(wr >> 24);
-                   sb[pos[3]] = (uint8_t)wi; sb[pos[4]] = (uint8_t)(wi >> 16); sb[pos[5]] = (uint8_t)(wi >> 24); }
-        };
-        demap(R0, d0, pos0); demap(R1, d1, pos1);
+        if (d0 >= 0) {
+            const uint32_t c0 = pk_demap_clamp(R0), c1 = pk_demap_clamp(R1);
+            const uint32_t wr0 = s_demap[(c0 >> 4) & 0xFF], wi0 = s_demap[(c0 >> 20) & 0xFF], wr1 = s_demap[(c1 >> 4) & 0xFF], wi1 = s_demap[(c1 >> 20) & 0xFF];
+            if (nbpsc == 6) {                          // bits 0-2 are bytes 0, 2, 3 of wr, bits 3-5 those of wi; d0's byte low, d1's high
+                auto st16 = [&](uint32_t p, uint32_t v) { *(uint16_t*)(s8 + p) = (uint16_t)v; };
+                st16(pos[0], __byte_perm(wr0, wr1, 0x70)); st16(pos[1], __byte_perm(wr0, wr1, 0x42)); st16(pos[2], __byte_perm(wr0, wr1, 0x63));
+                st16(pos[3], __byte_perm(wi0, wi1, 0x70)); st16(pos[4], __byte_perm(wi0, wi1, 0x42)); st16(pos[5], __byte_perm(wi0, wi1, 0x63));
+            } else {
+                auto st8 = [&](uint32_t p, uint32_t v0w, uint32_t v1w) { s8[p & 0xFFFFu] = (uint8_t)v0w; s8[p >> 16] = (uint8_t)v1w; };
+                if (nbpsc == 1) { st8(pos[0], wr0, wr1); }
+                else if (nbpsc == 2) { st8(pos[0], wr0, wr1); st8(pos[1], wi0, wi1); }
+                else { st8(pos[0], wr0, wr1); st8(pos[1], wr0 >> 8, wr1 >> 8); st8(pos[2], wi0, wi1); st8(pos[3], wi0 >> 8, wi1 >> 8); }
+            }
+        }
         __syncwarp();
         if (!plcp_data) {                              // PHY_11a.hpp:520-604
             uint32_t sig = warp_viterbi_signal(sb, s_dec[wib], lane) & 0xFFFFFFu;
@@ -426,11 +446,8 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
             fi.nsym_total = (L * 8 + 16 + 6 + nd - 1) / nd + 1;
             remain = fi.nsym_total; plcp_data = 1; nbpsc = nb; fi.ncbps = 48 * nb;
             load_positions(nb);
-        } else {
-            {   uint32_t* dst = (uint32_t*)(sout + soft_bytes); const uint32_t* src = (const uint32_t*)sb; const int nw = ncbps >> 2;   // <= 72 words
-                if (lane < nw) dst[lane] = src[lane];
-                if (lane + 32 < nw) dst[lane + 32] = src[lane + 32];
-                if (lane + 64 < nw) dst[lane + 64] = src[lane + 64]; }
+        } else {                                       // N_CBPS = 48 N_BPSC bytes: 3 N_BPSC 16-byte lines (soft_out and soft_stride are 16-byte aligned)
+            if (lane < 3 * nbpsc) ((uint4*)(sout + soft_bytes))[lane] = ((const uint4*)sb)[lane];
             soft_bytes += ncbps;
         }
         __syncwarp();
