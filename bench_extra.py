@@ -10,6 +10,7 @@
   --config fir37     the legacy 802.11b transmit filter (BB11BPMDSpreadFIR4SSE) on the device
   --config tx11b_legacy  the legacy 802.11b transmitter (BB11BPMDPacketGenSignal: encoder + SSE filter, fused) on the device, 11 Mbps / 1500 B
   --config tx11a_legacy  the legacy 802.11a transmitter (BB11ATxFrameMod) on the device, 54 Mbps / 1500 B, at 40 and at 44 Msps
+  --config channelize  the wideband channelizer: four 802.11a channels of a 160 Msps capture, 127 taps, D = 4, device-resident
   --config 11n       config #4: 802.11n HT-MF 2x2 RX chain at MCS 8, 9, 10, PSDU 1500 B, 2 x 40 Msps, fixed 2x2 channel
 
 Each prints one JSON line per measurement (same timing rules as bench.py: >= 3 warm-ups, CUDA events on the launch
@@ -420,12 +421,51 @@ def bench_fir(args):
             "parity": "equal to the arithmetic of include/sora_b200.h (numpy, 64-bit) on the first 24000 outputs"})
     c.close()
 
+def _card():
+    """(name, power limit W, max SM clock MHz) of GPU 0 as nvidia-smi reports them (None where it cannot)."""
+    import subprocess
+    try:
+        s = subprocess.run(["nvidia-smi", "-i", "0", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader,nounits"], capture_output=True, text=True, timeout=30).stdout
+        name, pl, clk = [v.strip() for v in s.strip().splitlines()[0].split(",")]
+        return name, float(pl), float(clk)
+    except Exception:
+        return None, None, None
+
+def bench_channelize(args):
+    """The wideband channelizer on a device-resident 160 Msps capture: four 802.11a channels at -60 / -20 / +20 / +60 MHz, 127 taps, D = 4.
+    Work per input sample: K (4 + 2 ntaps / D) integer multiply-adds; HBM traffic 4 B read + 4 K / D B written."""
+    import wideband_inputs as W
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    n = args.frames * 9824 * 4; K, D = 4, 4
+    taps = W.lowpass(127, 0.1); ch = [(W.phase_inc(f, 160e6), 0) for f in (-60e6, -20e6, 20e6, 60e6)]
+    n_out = -(-n // D); stride = (n_out + 3) // 4 * 4
+    x = torch.randint(-20000, 20000, (n, 2), dtype=torch.int16, device=dev); y = torch.empty((K, stride, 2), dtype=torch.int16, device=dev)
+    def step(): eng.channelize_raw(x.data_ptr(), n, ch, D, taps, y.data_ptr(), stride, st.cuda_stream)
+    step(); torch.cuda.synchronize()
+    P = 20000; m = (P - len(taps)) // D                                  # outputs that a prefix of P samples determines
+    assert (W.channelize(x[:P].cpu().numpy(), ch, D, taps)[:, :m] == y[:, :m].cpu().numpy()).all(), "channelizer output differs from the stated arithmetic"
+    ms = c.timed(step, args.steps)
+    sec = ms * 1e-3
+    hbm = n * (4.0 + 4.0 * K / D); macs = n * K * (4.0 + 2.0 * len(taps) / D)
+    name, plim, clk = _card(); sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    imad_peak = sms * 64 * clk * 1e6 if clk else None                    # int32 IMAD: 64 per SM per clock on sm_90
+    f_hbm = hbm / sec / 1e9 / peaks(); f_int = (macs / sec / imad_peak) if imad_peak else None
+    c.emit({"metric": "wideband channelizer input Msamples/s (COMPLEX16 in, 4 channels, D = 4)", "value": c.world * n / sec / 1e6, "unit": "Msamples/s", "ms_per_step": ms, "n_gpus": c.world,
+            "config": {"workload": "160 Msps capture, 4 x 802.11a channels at -60/-20/+20/+60 MHz, 127 taps, D = 4, device-resident", "samples_per_step_per_gpu": n},
+            "hbm": {"achieved": hbm / sec / 1e9, "peak": peaks(), "unit": "GB/s", "frac": f_hbm, "note": "4 B read + 4 K / D B written per input sample"},
+            "int_mad": {"achieved": macs / sec / 1e9, "peak": imad_peak / 1e9 if imad_peak else None, "unit": "G multiply-adds/s", "frac": f_int,
+                        "note": "K (4 + 2 ntaps / D) per input sample; peak = SMs x 64 x max SM clock"},
+            "bound": None if f_int is None else ("integer" if f_int > f_hbm else "hbm"),
+            "card": name, "power_limit_w": plim,
+            "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs of every channel" % m})
+    c.close()
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize}[a.config](a)

@@ -136,8 +136,28 @@ int sb200_rx11a_streams(sb200_handle* h, const int16_t* iq, uint64_t iq_total_sa
 /* 2:1 anti-alias FIR decimator for a COMPLEX16 capture — the "FIR decimation / channel-select" stage; an extension: the reference's 802.11a
  * graph only drops every other sample (TDownSample2, Brick11/src/samples.hpp:27-49).  out[m] = sat16((sum_k taps[k] * x[2m + k - (ntaps-1)/2]
  * + 2^14) >> 15), x = 0 outside the buffer, re and im independently; taps Q15, ntaps odd <= 63, taps = NULL: built-in 31-tap half-band low-pass.
- * out receives (n_in + 1) / 2 samples and is what sb200_rx11a_batch_ex(sample_rate_mhz = 20) takes.  Host or device pointers (device: 16-byte aligned). */
+ * out receives (n_in + 1) / 2 samples and is what sb200_rx11a_batch_ex(sample_rate_mhz = 20) takes.  Host or device pointers (device: 16-byte aligned).
+ * It computes what sb200_channelize below computes for channel (0, 0) and decim 2, without that call's tap-sum and stride checks. */
 int sb200_fir_decimate2(sb200_handle* h, const int16_t* iq, uint64_t n_in_samples, const int16_t* taps, uint32_t ntaps, int16_t* out, void* cuda_stream);
+
+/* Wideband channelizer: several channels of one COMPLEX16 capture x[0 .. n_in) (x = 0 outside it) shifted to 0 Hz, low-pass filtered and
+ * decimated by D = decim, in one call; an extension without a reference counterpart.  For channel (phase_inc, phase0) and every output
+ * m in 0 .. n_out = ceil(n_in / D):
+ *     phi(n)  = (phase0 + (uint32)n * phase_inc) mod 2^32             n = absolute input index: stateless, no serial NCO
+ *     (C, S)  = NCO[phi(n) >> 20]                                      4096 entries, Q14: C = rint(16384 cos(2 pi i / 4096)), S = rint(16384 sin(2 pi i / 4096))
+ *     v(n).re = sat16((x.re * C + x.im * S + 2^13) >> 14)            x * e^{-j theta}: moves +f_c to 0 Hz
+ *     v(n).im = sat16((x.im * C - x.re * S + 2^13) >> 14)
+ *     y[m]    = sat16((sum_k taps[k] * v(D m + k - c) + 2^14) >> 15)   c = (ntaps - 1) / 2, int32 accumulator, re and im independently
+ * The NCO is Q14 so that phase_inc = phase0 = 0 is the identity bit for bit; with D = 2 that channel is sb200_fir_decimate2.  A channel
+ * centred at f_c in a capture at f_s takes phase_inc = round(f_c / f_s * 2^32) mod 2^32 (negative f_c wraps).
+ * Channel c goes to out[c * out_stride .. + n_out) (samples), so stream_off[c] = c * out_stride and stream_len[c] = n_out hand the rows
+ * to sb200_rx11a_streams / sb200_rx11b_streams / sb200_rx11n_streams as they are.  iq and out may be host or device pointers (device:
+ * 16-byte aligned, and the call is then asynchronous on the stream); channels and taps are host arrays.  Limits (SB200_E_INVALID):
+ * 1 <= nchannels <= 16, 1 <= decim <= 16, ntaps odd and <= 255, sum |taps| <= 65535 (the accumulator cannot wrap), out_stride >= n_out,
+ * a multiple of 4 and <= 2^40, n_in <= 2^40.  One kernel launch; sb200_last_kernel_ms times it. */
+typedef struct sb200_ddc_channel { uint32_t phase_inc; uint32_t phase0; } sb200_ddc_channel;
+int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_in_samples, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t decim,
+                     const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride_samples, void* cuda_stream);
 
 /* Same as sb200_rx11a_batch for captures at `sample_rate_mhz` = 20, 40 or 44.  20: the capture is already at the channel rate (slots counted in
  * 20 Msps samples; sample j stands where TDownSample2 would have put sample 2j of a 40 Msps capture).  44 Msps slots first pass the reference's 11:10 linear

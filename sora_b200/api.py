@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -67,6 +67,13 @@ def _payload_table(payloads):
     lens = np.array([len(p) for p in payloads], np.uint32); offs = np.concatenate([[0], np.cumsum(lens[:-1])]).astype(np.uint64)
     flat = np.ascontiguousarray(np.concatenate([np.asarray(p, np.uint8) for p in payloads]) if lens.sum() else np.zeros(1, np.uint8))
     return flat, offs, lens
+
+def phase_inc(f_hz, fs_hz):
+    """NCO increment of sb200_channelize for a channel centred at f_hz in a capture at fs_hz: round(f / fs * 2^32) mod 2^32 (negative f wraps)."""
+    return int(round(f_hz / fs_hz * 2 ** 32)) % 2 ** 32
+
+class DdcChannel(C.Structure):
+    _fields_ = [("phase_inc", C.c_uint32), ("phase0", C.c_uint32)]
 
 _NDBPS_11A = {6000: 24, 9000: 36, 12000: 48, 18000: 72, 24000: 96, 36000: 144, 48000: 192, 54000: 216}   # 802.11a data bits per OFDM symbol
 
@@ -228,6 +235,22 @@ class Engine:
         t = None if taps is None else np.ascontiguousarray(taps, dtype=np.int16)
         self.fir_decimate2_raw(_ptr(iq), len(iq), _ptr(t) if t is not None else 0, 0 if t is None else len(t), _ptr(out))
         return out
+
+    def channelize_raw(self, in_ptr, n_in, channels, decim, taps, out_ptr, out_stride, stream=0):
+        """Pointer-level sb200_channelize: in_ptr / out_ptr host or device addresses; channels a list of (phase_inc, phase0); taps int16 Q15."""
+        ch = (DdcChannel * max(len(channels), 1))(*[DdcChannel(int(a) % 2 ** 32, int(b) % 2 ** 32) for a, b in channels])
+        t = np.ascontiguousarray(taps, dtype=np.int16)
+        self._check(self._lib.sb200_channelize(self._h, C.c_void_p(in_ptr), C.c_uint64(n_in), C.cast(ch, C.c_void_p), C.c_uint32(len(channels)), C.c_uint32(decim),
+                                               C.c_void_p(_ptr(t)), C.c_uint32(len(t)), C.c_void_p(out_ptr), C.c_uint64(out_stride), C.c_void_p(stream)), "sb200_channelize")
+
+    def channelize(self, iq, channels, decim, taps):
+        """Wideband channelizer: int16 [n,2] and K channels (phase_inc, phase0) -> int16 [K, ceil(n / decim), 2], channel k shifted to 0 Hz,
+        filtered by taps (int16 Q15, odd count <= 255, sum |t| <= 65535) and decimated."""
+        iq = np.ascontiguousarray(iq, dtype=np.int16).reshape(-1, 2)
+        n_out = -(-len(iq) // decim); stride = (n_out + 3) // 4 * 4
+        out = np.zeros((len(channels), stride, 2), np.int16)
+        self.channelize_raw(_ptr(iq), len(iq), channels, decim, taps, _ptr(out), stride)
+        return out[:, :n_out]
 
     def tx11b_fir37_raw(self, in_ptr, total, off_ptr, len_ptr, nframes, variant, out_ptr, stream=0):
         self._check(self._lib.sb200_tx11b_fir37(self._h, C.c_void_p(in_ptr), C.c_uint64(total), C.c_void_p(off_ptr), C.c_void_p(len_ptr), C.c_uint32(nframes),

@@ -260,6 +260,9 @@ struct sb200_handle {
     // SB200_VITERBI=v8 forces it (0 .. 0xFFFFFFFF), v3 forbids it.
     uint32_t lane_min = SB200_LANE_MIN_DEFAULT, lane_max = SB200_LANE_MAX_DEFAULT;
     const char* last_vit = "";                         // name of the Viterbi kernel the last launch used (sb200_last_viterbi_kernel)
+    DevBuf nco;                                        // channelizer NCO table (fir_kernels.cuh), built on first use
+    uint32_t ch_smem_set = 0;                          // bit J: k_channelize<J> may use SB_CH_SMEM bytes of dynamic shared memory on this device
+    int sms = 0;                                       // multiprocessors of the device (channel groups of k_channelize)
     DevBuf vring;
     bool use_pair = false;                             // SB200_VITERBI=v4: two lanes per code block, 16 code blocks per warp (A/B against four lanes)
     bool use_v2 = false;                               // SB200_VITERBI=v2 selects the per-step-mark quad kernel (A/B against the history-carrying one)
@@ -839,8 +842,38 @@ extern "C" int sb200_rx11a_stream(sb200_handle* h, const int16_t* iq, uint64_t n
     return sb200_rx11a_streams(h, iq, nsamples, &off, &len, 1, max_frames, out_bytes, out_stride, res, sample_index, nframes_out, cuda_stream);
 }
 
-// 2:1 anti-alias FIR decimator (fir_kernels.cuh): out[m] = sat16((sum_k taps[k] x[2m + k - (ntaps-1)/2] + 2^14) >> 15), zero outside the buffer.
-// taps == NULL selects the built-in 31-tap half-band low-pass (equiripple: +-0.05 dB to 8.3 MHz of a 40 Msps capture, 50 dB down beyond 11.7 MHz).
+// One launch of k_channelize (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.  Outputs per thread from D;
+// channels split into groups (the input then read once per group) only as far as needed for four CTAs per multiprocessor.
+template <int J>
+static int channelize_launch_j(sb200_handle* h, cudaStream_t st, dim3 grid, const uint32_t* d_in, uint64_t n_in, const ChChannels& ch, uint32_t cpg,
+                               uint32_t D, const ChTaps& T, uint32_t* d_out, uint64_t stride, uint64_t n_out) {
+    if (!(h->ch_smem_set & (1u << J))) {
+        CK(cudaFuncSetAttribute(k_channelize<J>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_CH_SMEM));
+        h->ch_smem_set |= 1u << J;
+    }
+    CK(cudaEventRecord(h->ev0, st));
+    k_channelize<J><<<grid, SB_FIR_THREADS, SB_CH_SMEM, st>>>(d_in, n_in, (const uint32_t*)h->nco.p, ch, cpg, D, T, d_out, stride, n_out);
+    return SB200_OK;
+}
+static int channelize_launch(sb200_handle* h, cudaStream_t st, const uint32_t* d_in, uint64_t n_in, const ChChannels& ch, uint32_t D, const ChTaps& T,
+                             uint32_t* d_out, uint64_t stride, uint64_t n_out) {
+    if (!h->sms) CK(cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, h->device));
+    const uint64_t tiles = (n_in + SB_FIR_TILE - 1) / SB_FIR_TILE;
+    uint32_t groups = 1;
+    while (groups < ch.n && tiles * groups < 4ull * (uint64_t)h->sms) groups++;
+    const uint32_t cpg = (ch.n + groups - 1) / groups; groups = (ch.n + cpg - 1) / cpg;
+    const dim3 grid((unsigned)tiles, groups);
+    const uint32_t need = ((SB_FIR_TILE + D - 1) / D + SB_FIR_THREADS - 1) / SB_FIR_THREADS;     // outputs per thread of a tile
+    if (need <= 1) return channelize_launch_j<1>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
+    if (need <= 2) return channelize_launch_j<2>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
+    if (need <= 4) return channelize_launch_j<4>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
+    if (need <= 8) return channelize_launch_j<8>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
+    return channelize_launch_j<16>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
+}
+
+// 2:1 anti-alias FIR decimator (k_fir_decimate2): channel (0, 0) of the channelizer's arithmetic with D = 2,
+// out[m] = sat16((sum_k taps[k] x[2m + k - (ntaps-1)/2] + 2^14) >> 15), zero outside the buffer.  taps == NULL selects the built-in 31-tap half-band low-pass (equiripple: +-0.05 dB to 8.3 MHz of a 40 Msps
+// capture, 50 dB down beyond 11.7 MHz).
 static const int16_t kHalfBand31[31] = {-121, 0, 209, 0, -381, 0, 644, 0, -1056, 0, 1759, 0, -3278, 0, 10391, 16434, 10391, 0, -3278, 0, 1759, 0, -1056, 0, 644, 0, -381, 0, 209, 0, -121};   // sum 32768 (unit DC gain)
 extern "C" int sb200_fir_decimate2(sb200_handle* h, const int16_t* iq, uint64_t n_in, const int16_t* taps, uint32_t ntaps, int16_t* out, void* cuda_stream) {
     if (!h || !iq || !out) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
@@ -859,6 +892,44 @@ extern "C" int sb200_fir_decimate2(sb200_handle* h, const int16_t* iq, uint64_t 
     CK(cudaEventRecord(h->ev0, st));
     k_fir_decimate2<<<(unsigned)((n_in + SB_FIR_TILE - 1) / SB_FIR_TILE), SB_FIR_THREADS, 0, st>>>(d_in, n_in, T, d_out, n_out);
     return finish_call(h, st, ret, 0, 1);
+}
+
+// Wideband channelizer (fir_kernels.cuh): every channel shifted by its NCO, filtered and decimated by `decim`; channel c in row c of `out`.
+extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t decim,
+                                const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
+    if (!h) return SB200_E_INVALID;
+    if (!iq || !channels || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
+    if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
+    if (decim < 1 || decim > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "decim must be 1 .. 16");
+    if ((ntaps & 1u) == 0 || ntaps > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 255");
+    uint32_t asum = 0; for (uint32_t i = 0; i < ntaps; i++) asum += (uint32_t)abs((int)taps[i]);
+    if (asum > 65535u) return h->fail(SB200_E_INVALID, "sum of |taps| must be at most 65535 (the int32 accumulator must not wrap)");
+    if (n_in > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples must be at most 2^40");
+    const uint64_t n_out = (n_in + decim - 1) / decim;
+    if (out_stride < n_out || (out_stride & 3u) || out_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "out_stride must be at least ceil(n_in / decim), at most 2^40 and a multiple of 4");
+    if (n_in == 0) return SB200_OK;
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    CK(cudaSetDevice(h->device));
+    const bool in_dev = is_device_ptr(iq), out_dev = is_device_ptr(out);
+    if ((in_dev && ((uintptr_t)iq & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device input and output must be 16-byte aligned");
+    if (!h->nco.p) {                                   // (C, S) = (rint(2^14 cos 2 pi i / 4096), rint(2^14 sin 2 pi i / 4096)), packed like cs16
+        std::vector<uint32_t> t(SB_CH_NCO);
+        for (int i = 0; i < SB_CH_NCO; i++) { const double a = 2.0 * M_PI * i / 4096.0; t[i] = pack(mk((int)nearbyint(16384.0 * cos(a)), (int)nearbyint(16384.0 * sin(a)))); }
+        cudaError_t e = h->nco.need(SB_CH_NCO * 4);
+        if (e == cudaSuccess) e = cudaMemcpy(h->nco.p, t.data(), SB_CH_NCO * 4, cudaMemcpyHostToDevice);
+        if (e != cudaSuccess) { h->nco.release(); return h->fail(SB200_E_CUDA, "NCO table upload", e); }
+    }
+    const uint32_t* d_in; uint32_t* d_out = (uint32_t*)out; uint64_t d_stride = out_stride; Returns ret;
+    CK(to_device(h->iq, (const uint32_t*)iq, in_dev, n_in * 4ull, st, &d_in, 16));
+    if (!out_dev) {                                    // rows n_out (rounded to 4) apart in the workspace, copied into the caller's rows
+        d_stride = (n_out + 3u) & ~3ull; CK(h->iq40.need(nchannels * d_stride * 4ull)); d_out = (uint32_t*)h->iq40.p;
+        ret.bind2d(out, out_stride * 4ull, d_out, d_stride * 4ull, n_out * 4ull, nchannels);
+    }
+    ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
+    ChChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
+    for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; }
+    const int rc = channelize_launch(h, st, d_in, n_in, ch, decim, T, d_out, d_stride, n_out);
+    return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
 }
 
 extern "C" int sb200_rx11a_batch_ex(sb200_handle* h, const int16_t* iq, uint64_t iq_total, const uint64_t* frame_off, const uint32_t* frame_len,
