@@ -19,9 +19,17 @@
  *
  * Conventions: plain pointers and sizes only; every function returns 0 on success or a negative SB200_E_* code
  * and never throws.  Sample and result buffers may live in host or device memory (detected per pointer); host
- * buffers are staged through the handle's pinned/device workspaces on `stream`.  Calls are asynchronous on
- * `stream` when all buffers are device buffers, and synchronise the stream before returning when a result buffer
- * is host memory.  One handle may be used by one host thread at a time.
+ * buffers are staged through the handle's pinned/device workspaces on `stream`.  When a call touches memory:
+ *   - a call returns once it no longer needs any host buffer of the caller: it synchronises `stream` before
+ *     returning when a result buffer is host memory, or when an input it copies is page-locked host memory
+ *     (sb200_host_alloc, cudaHostRegister); pageable inputs are copied out before the call returns;
+ *   - with device buffers and host-resident tables a call does not wait for `stream`: its work stays queued;
+ *   - device-resident slot or payload tables cost a read-back (one stream synchronisation), except a repeated
+ *     receive call on the same slot table under the option slot_table_immutable; sb200_rx11a_batch_ex at 44 Msps
+ *     checks the slot table of its resampled captures the same way;
+ *   - calls on one handle execute in the order they were made, whatever streams they are given (a call on another
+ *     stream than the previous one waits for it on the device, not on the host).
+ * One handle may be used by one host thread at a time; separate handles may run concurrently.
  * There is NO CPU fallback: if no CUDA device is usable the create call fails.
  */
 #ifndef SORA_B200_H

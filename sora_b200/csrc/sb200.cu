@@ -103,6 +103,14 @@ bool is_device_ptr(const void* p) {
     return a.type == cudaMemoryTypeDevice || a.type == cudaMemoryTypeManaged;
 }
 
+// Page-locked host memory (cudaHostAlloc, cudaHostRegister): a queued copy out of it reads it only when the stream reaches the copy.
+// Pageable memory reports cudaMemoryTypeUnregistered; cudaMemcpyAsync copies it out before returning.
+bool is_host_locked(const void* p) {
+    cudaPointerAttributes a;
+    if (cudaPointerGetAttributes(&a, p) != cudaSuccess) { cudaGetLastError(); return false; }
+    return a.type == cudaMemoryTypeHost;
+}
+
 // [off, off + len) lies inside [0, total), without the sum that a 64-bit offset near 2^64 would wrap
 inline bool in_range(uint64_t off, uint64_t len, uint64_t total) { return len <= total && off <= total - len; }
 
@@ -218,6 +226,7 @@ struct sb200_handle {
     DevBuf tab, iq, off, len, info, soft, out, status, crc, res, taps[5], vlist, vcnt;
     uint16_t* inv_deint = nullptr;
     cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    cudaEvent_t ev_done = nullptr; cudaStream_t last_st = nullptr; bool ordered = false;   // end of the previous call and its stream (CallScope)
     cudaEvent_t evk[5] = {nullptr, nullptr, nullptr, nullptr, nullptr};   // boundaries of sync | front | viterbi | pack
     int nk = 0;
     bool timed = false;
@@ -275,6 +284,22 @@ struct sb200_handle {
 
 #define CK(call) do { cudaError_t _e = (call); if (_e != cudaSuccess) return h->fail(SB200_E_CUDA, #call, _e); } while (0)
 
+// One call of the C ABI on the caller's stream `st`.  Calls on one handle share its workspaces, so they run in the order they were made,
+// whatever streams they are given: begin() makes `st` wait for the end of the handle's previous call when that ran on another stream (an
+// event: no host synchronisation, no launch), and every call records its end on its stream.  cudaStreamPerThread names a different stream
+// in every host thread, so it always waits.  reads(p) notes an input the call copies out of caller host memory on the stream: if it is
+// page-locked, the call synchronises `st` once before it returns, so the caller may refill the buffer as soon as it has control back.
+struct CallScope {
+    sb200_handle* h; cudaStream_t st; bool locked = false;
+    CallScope(sb200_handle* h_, cudaStream_t st_) : h(h_), st(st_) {}
+    cudaError_t begin() const { return h->ordered && (h->last_st != st || st == cudaStreamPerThread) ? cudaStreamWaitEvent(st, h->ev_done, 0) : cudaSuccess; }
+    void reads(const void* p) { if (p && !locked) locked = is_host_locked(p); }
+    ~CallScope() {
+        if (cudaEventRecord(h->ev_done, st) == cudaSuccess) { h->last_st = st; h->ordered = true; } else cudaGetLastError();
+        if (locked) cudaStreamSynchronize(st);
+    }
+};
+
 // Payload or slot table of a call, each half on either side.  load() reads it to the host and runs the call's own checks, check(i, inside =
 // in_range(off, len, total)), which must refuse an entry not inside; upload() later places off and len in the call's workspaces.
 struct FrameTable {
@@ -314,6 +339,8 @@ static int run_with_taps(sb200_handle* h, const size_t (&size)[5], void* const (
 }
 
 // One allocation of 256-byte aligned tables: add() returns a part's offset (src null: a kernel fills it); upload() frees `b` on any failure.
+// A cudaMemcpy from pageable memory may return before its DMA has landed, and a kernel on a non-blocking stream is not ordered after it:
+// upload() synchronises the device once at the end (tables are uploaded once per handle).
 struct TableArena {
     struct Part { size_t off; const void* src; size_t bytes; };
     std::vector<Part> parts; size_t size = 0;
@@ -322,6 +349,7 @@ struct TableArena {
         cudaError_t e = b.need(size);
         if (e != cudaSuccess) return h->fail(SB200_E_NOMEM, alloc_what, e);
         for (const Part& p : parts) if (p.src && e == cudaSuccess) e = cudaMemcpy((char*)b.p + p.off, p.src, p.bytes, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();
         if (e != cudaSuccess) { b.release(); return h->fail(SB200_E_CUDA, copy_what, e); }
         return SB200_OK;
     }
@@ -369,7 +397,7 @@ extern "C" int sb200_create(int device, const sb200_cfg* cfg, sb200_handle** out
     if (rc == SB200_OK && (cudaEventCreate(&h->ev0) != cudaSuccess || cudaEventCreate(&h->ev1) != cudaSuccess)) rc = SB200_E_CUDA;
     for (int i = 0; i < 5 && rc == SB200_OK; i++) if (cudaEventCreate(&h->evk[i]) != cudaSuccess) rc = SB200_E_CUDA;
     if (rc == SB200_OK && (cudaStreamCreateWithFlags(&h->s_copy, cudaStreamNonBlocking) != cudaSuccess || cudaStreamCreateWithFlags(&h->s_front, cudaStreamNonBlocking) != cudaSuccess)) rc = SB200_E_CUDA;
-    if (rc == SB200_OK && cudaEventCreateWithFlags(&h->ev_start, cudaEventDisableTiming) != cudaSuccess) rc = SB200_E_CUDA;
+    if (rc == SB200_OK && (cudaEventCreateWithFlags(&h->ev_start, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&h->ev_done, cudaEventDisableTiming) != cudaSuccess)) rc = SB200_E_CUDA;
     for (int i = 0; i < 2 && rc == SB200_OK; i++) if (cudaEventCreateWithFlags(&h->ev_h2d[i], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&h->ev_front[i], cudaEventDisableTiming) != cudaSuccess) rc = SB200_E_CUDA;
     if (rc != SB200_OK) { sb200_destroy(h); return rc; }
     *out = h;
@@ -383,6 +411,7 @@ extern "C" void sb200_destroy(sb200_handle* h) {
     if (h->ev1) cudaEventDestroy(h->ev1);
     for (int i = 0; i < 5; i++) if (h->evk[i]) cudaEventDestroy(h->evk[i]);
     if (h->ev_start) cudaEventDestroy(h->ev_start);
+    if (h->ev_done) cudaEventDestroy(h->ev_done);
     for (int i = 0; i < 2; i++) { if (h->ev_h2d[i]) cudaEventDestroy(h->ev_h2d[i]); if (h->ev_front[i]) cudaEventDestroy(h->ev_front[i]); }
     for (cudaEvent_t e : h->ev_link) cudaEventDestroy(e);
     delete h->pool; for (int i = 0; i < 4; i++) { if (h->hstage[i]) cudaFreeHost(h->hstage[i]); if (h->ev_hfree[i]) cudaEventDestroy(h->ev_hfree[i]); }
@@ -547,6 +576,7 @@ static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
     if (!h || !iq || !frame_off || !frame_len || !res) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
     if (nframes == 0) return SB200_OK;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(iq);
     // slot table: checked on every call (slot_table above); the chunked host-IQ path also needs it on the host
     const bool iq_dev = is_device_ptr(iq);
     std::vector<uint64_t>& offh = h->offh; std::vector<uint32_t>& lenh = h->lenh;
@@ -608,6 +638,7 @@ static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
             if (dec) {
                 if (!h->pool || h->pool->n != (int)h->host_decimate) { delete h->pool; h->pool = new (std::nothrow) DecimPool(); if (!h->pool) return h->fail(SB200_E_NOMEM, "host thread pool"); h->pool->start((int)h->host_decimate); }
                 if (h->hstage_cap < hstage_samples * 4ull || h->hstage_wc != h->hstage_is_wc) {
+                    for (int i = 0; i < 4; i++) if (h->ev_hfree[i]) CK(cudaEventSynchronize(h->ev_hfree[i]));     // no copy out of a buffer still queued
                     for (int i = 0; i < 4; i++) { if (h->hstage[i]) cudaFreeHost(h->hstage[i]); h->hstage[i] = nullptr; }
                     h->hstage_cap = 0;
                     const size_t want_b = hstage_samples * 4ull + hstage_samples / 2 + 256;
@@ -670,7 +701,9 @@ static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
             }
             if (!gather) return SB200_OK;
             const int hb = (int)(gsub % 4u);
-            if (gsub >= 4) CK(cudaEventSynchronize(h->ev_hfree[hb]));                        // pinned buffer hb is free once the gathered chunk four back has crossed the link
+            // pinned buffer hb is free once its last copy has crossed the link: the gathered chunk four back, or one of an earlier call that
+            // returned with its copies still queued (an event never recorded counts as complete)
+            CK(cudaEventSynchronize(h->ev_hfree[hb]));
             DecimPool::Job j{(const uint32_t*)iq, offh.data(), lenh.data(), doffh.data(), f0, f1, (uint32_t*)h->hstage[hb]};
             h->pool->submit(j); inflight.on = true;
             cbuf[c] = (int8_t)hb; gsub++;
@@ -761,6 +794,7 @@ extern "C" int sb200_rx11a_streams(sb200_handle* h, const int16_t* iq, uint64_t 
     if (!h || !iq || !stream_off || !stream_len || !res || !nframes_out) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin());          // results in host memory: the call synchronises anyway
     {   const int rc = stream_table(h, stream_off, stream_len, nstreams, iq_total, res, out_bytes, nframes_out, false); if (rc != SB200_OK) return rc; }
     if (nstreams == 0 || max_frames == 0) return SB200_OK;
     const int16_t* d_iq = iq;
@@ -882,6 +916,7 @@ extern "C" int sb200_fir_decimate2(sb200_handle* h, const int16_t* iq, uint64_t 
     if (n_in == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(iq);
     const uint64_t n_out = (n_in + 1) / 2;
     const bool in_dev = is_device_ptr(iq);
     if (in_dev && ((uintptr_t)iq & 15u)) return h->fail(SB200_E_INVALID, "device input must be 16-byte aligned");
@@ -912,11 +947,13 @@ extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_i
     CK(cudaSetDevice(h->device));
     const bool in_dev = is_device_ptr(iq), out_dev = is_device_ptr(out);
     if ((in_dev && ((uintptr_t)iq & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device input and output must be 16-byte aligned");
+    CallScope call(h, st); CK(call.begin()); call.reads(iq);
     if (!h->nco.p) {                                   // (C, S) = (rint(2^14 cos 2 pi i / 4096), rint(2^14 sin 2 pi i / 4096)), packed like cs16
         std::vector<uint32_t> t(SB_CH_NCO);
         for (int i = 0; i < SB_CH_NCO; i++) { const double a = 2.0 * M_PI * i / 4096.0; t[i] = pack(mk((int)nearbyint(16384.0 * cos(a)), (int)nearbyint(16384.0 * sin(a)))); }
         cudaError_t e = h->nco.need(SB_CH_NCO * 4);
         if (e == cudaSuccess) e = cudaMemcpy(h->nco.p, t.data(), SB_CH_NCO * 4, cudaMemcpyHostToDevice);
+        if (e == cudaSuccess) e = cudaDeviceSynchronize();   // landed before a kernel on a non-blocking stream reads it (TableArena::upload)
         if (e != cudaSuccess) { h->nco.release(); return h->fail(SB200_E_CUDA, "NCO table upload", e); }
     }
     const uint32_t* d_in; uint32_t* d_out = (uint32_t*)out; uint64_t d_stride = out_stride; Returns ret;
@@ -946,6 +983,7 @@ extern "C" int sb200_rx11a_batch_ex(sb200_handle* h, const int16_t* iq, uint64_t
     if (nframes == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(iq);
     // slot table on the host (sizing) and on the device (kernel)
     FrameTable ft(frame_off, frame_len, nframes);
     const bool iq_dev = is_device_ptr(iq);
@@ -977,6 +1015,7 @@ static int rx11b_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
     if (nframes == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(iq);
     const bool iq_dev = is_device_ptr(iq);
     const uint32_t* d_iq; const uint64_t* d_off; const uint32_t* d_len; uint32_t max_len = 0; bool tab_on_host = false;
     { int rc = slot_table(h, frame_off, frame_len, nframes, iq_total, false, st, &d_off, &d_len, &max_len, &tab_on_host); if (rc != SB200_OK) return rc; }
@@ -1043,6 +1082,7 @@ static int rx11n_run(sb200_handle* h, const int16_t* iq0, const int16_t* iq1, ui
     if (!h || !iq0 || !iq1 || !frame_off || !frame_len || !res) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
     if (nframes == 0) return SB200_OK;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(iq0); call.reads(iq1);
     int rc = upload_tables11n(h); if (rc != SB200_OK) return rc;
     const bool iq_dev = is_device_ptr(iq0);
     if (iq_dev != is_device_ptr(iq1)) return h->fail(SB200_E_INVALID, "both antenna buffers must live on the same side");
@@ -1092,6 +1132,7 @@ extern "C" int sb200_rx11n_streams(sb200_handle* h, const int16_t* iq0, const in
     if (!h || !iq0 || !iq1 || !stream_off || !stream_len || !res || !nframes_out) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin());          // results in host memory: the call synchronises anyway
     const bool iq_dev = is_device_ptr(iq0);
     {   const int rc = stream_table(h, stream_off, stream_len, nstreams, iq_total, res, out_bytes, nframes_out, iq_dev != is_device_ptr(iq1)); if (rc != SB200_OK) return rc; }
     if (nstreams == 0 || max_frames == 0) return SB200_OK;
@@ -1180,6 +1221,7 @@ extern "C" int sb200_rxblocks_unpack(sb200_handle* h, const void* blocks, uint64
     if (nblocks == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(blocks);
     const uint4* d_in; uint4* d_out; Returns ret;
     CK(to_device(h->stage[0], (const uint4*)blocks, is_device_ptr(blocks), nblocks * 128ull, st, &d_in));
     CK(ret.bind(h->stage[1], (uint4*)iq_out, nblocks * 112ull, &d_out));
@@ -1205,6 +1247,7 @@ extern "C" int sb200_rxblocks_desc(sb200_handle* h, const void* blocks, uint64_t
     if (nblocks == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(blocks);
     const uint4* d_in; uint32_t* d_v; uint32_t* d_t; Returns ret;
     CK(to_device(h->stage[0], (const uint4*)blocks, is_device_ptr(blocks), nblocks * 128ull, st, &d_in));
     CK(ret.bind(h->stage[1], vstream_bits, nblocks * 4ull, &d_v));
@@ -1280,6 +1323,7 @@ extern "C" int sb200_tx11a_batch(sb200_handle* h, const uint8_t* payload, uint64
     if (!R) return h->fail(SB200_E_INVALID, "rate_kbps is not an 802.11a rate");
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(payload); call.reads(seeds);
     int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
     // frame table on the host (sizes the grid and checks the slots)
     FrameTable ft(pay_off, pay_len, nframes);
@@ -1333,6 +1377,7 @@ extern "C" int sb200_tx11b_batch(sb200_handle* h, const uint8_t* payload, uint64
         for (int k = 0; k < 20; k++) if (job.taps[k] != H[k]) return h->fail(SB200_E_INVALID, "shaper taps differ from the compiled constants"); }
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(payload);
     FrameTable ft(pay_off, pay_len, nframes);
     uint32_t max_len = 0;
     int rc = ft.load(h, st, payload_total, [&](uint32_t i, bool inside) {
@@ -1375,6 +1420,7 @@ extern "C" int sb200_tx11b_fir37(sb200_handle* h, const int8_t* chips, uint64_t 
     if (nframes == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(chips);
     FrameTable ft(frame_off, frame_len, nframes);
     const bool in_dev = is_device_ptr(chips), out_dev = is_device_ptr(out);
     uint32_t max_len = 0;
@@ -1421,6 +1467,7 @@ extern "C" int sb200_tx11b_legacy_batch(sb200_handle* h, const uint8_t* payload,
     job.rate_code = R->code; job.data_chips_per_byte = short_preamble && rate_kbps == 1000 ? 0u : R->chips_per_byte;   // the short preamble's 1 Mbps case sends no data chips
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(payload);
     FrameTable ft(pay_off, pay_len, nframes);
     uint32_t max_size = 0;
     int rc = ft.load(h, st, payload_total, [&](uint32_t i, bool inside) {
@@ -1470,6 +1517,7 @@ extern "C" int sb200_tx11a_legacy_batch(sb200_handle* h, const uint8_t* payload,
     job.sr44 = sample_rate_mhz == 44; job.fcs_in_payload = (flags & SB200_TX11A_LEGACY_FCS_IN_PAYLOAD) ? 1u : 0u;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(payload); call.reads(preamble);
     int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
     FrameTable ft(pay_off, pay_len, nframes);
     const bool pre_dev = is_device_ptr(preamble);
@@ -1584,6 +1632,7 @@ extern "C" int sb200_tx11n_batch(sb200_handle* h, const uint8_t* payload, uint64
     }
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(payload); call.reads(seeds);
     int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
     rc = upload_tables_tx11n(h); if (rc != SB200_OK) return rc;
     FrameTable ft(pay_off, pay_len, nframes);
@@ -1672,6 +1721,7 @@ extern "C" int sb200_viterbi_k7(sb200_handle* h, const uint8_t* soft, uint64_t s
     if (nblocks == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
+    CallScope call(h, st); CK(call.begin()); call.reads(soft);
     const uint8_t* d_soft; uint64_t d_stride = soft_stride;
     const bool aligned = ((uintptr_t)soft & 15) == 0 && (soft_stride & 15) == 0;
     if (is_device_ptr(soft) && aligned) d_soft = soft;
