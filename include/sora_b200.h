@@ -342,7 +342,10 @@ int sb200_tx11n_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_
 /* Standalone K=7 Viterbi over `nblocks` independent blocks of `nsoft` soft values (uint8 0..7, one per coded bit after
  * puncturing; block b starts at soft + b*soft_stride).  frame_len_bytes L sets the flush point 8L+16+6 exactly like
  * CF_11aRxVector::frame_length; each block yields L+2 bytes (SERVICE + PSDU, not descrambled) at out + b*out_stride.
- * depth/lookahead = TRELLIS_DEPTH/TRELLIS_LOOKAHEAD (256/24 for 11a, 192/36 for 11n). */
+ * depth/lookahead = TRELLIS_DEPTH/TRELLIS_LOOKAHEAD (256/24 for 11a, 192/36 for 11n).  A trailing partial puncture group (nsoft not a
+ * multiple of 2 / 3 / 4 soft values at rate 1/2 / 2/3 / 3/4) is ignored, as the reference brick keeps it buffered.  A block whose soft values
+ * end before its flush point is defined only up to its last traceback window: the bytes of the windows that fired, the rest of its row
+ * unspecified. */
 int sb200_viterbi_k7(sb200_handle* h, const uint8_t* soft, uint64_t soft_stride, uint32_t nsoft, uint32_t nblocks,
                      int code_rate, uint32_t frame_len_bytes, uint32_t depth, uint32_t lookahead,
                      uint8_t* out, uint64_t out_stride, void* cuda_stream);

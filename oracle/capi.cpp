@@ -135,18 +135,26 @@ uint64_t sbo_viterbi_block(const uint8_t* soft, uint64_t nsoft, int code_rate, u
     uint32_t ob = 0;
     return viterbi_decode_block(v, soft, (size_t)nsoft, code_rate, frame_len_bytes, depth, lookahead, out, ob);
 }
-void sbo_viterbi_blocks(const uint8_t* soft, uint64_t nsoft_per_block, uint32_t nblocks, int code_rate, uint32_t frame_len_bytes,
-                        uint32_t depth, uint32_t lookahead, uint8_t* out, uint64_t out_stride, int nthreads) {
+// nblocks blocks of one layout; nbytes (may be null): bytes each block produced.  A block whose soft values end before its flush point
+// produces only the windows that fired; the rest of its output row is left untouched.
+void sbo_viterbi_blocks_n(const uint8_t* soft, uint64_t nsoft_per_block, uint32_t nblocks, int code_rate, uint32_t frame_len_bytes,
+                          uint32_t depth, uint32_t lookahead, uint8_t* out, uint64_t out_stride, uint32_t* nbytes, int nthreads) {
     std::atomic<uint32_t> next(0);
     auto work = [&]() {
         ViterbiCore v; v.max_steps = (uint32_t)nsoft_per_block + 8;
         for (;;) { uint32_t i = next.fetch_add(1); if (i >= nblocks) break;
             v.reset(); uint32_t ob = 0;
-            viterbi_decode_block(v, soft + (size_t)i * nsoft_per_block, (size_t)nsoft_per_block, code_rate, frame_len_bytes, depth, lookahead, out + (size_t)i * out_stride, ob); }
+            const size_t n = viterbi_decode_block(v, soft + (size_t)i * nsoft_per_block, (size_t)nsoft_per_block, code_rate, frame_len_bytes, depth, lookahead,
+                                                  out + (size_t)i * out_stride, ob);
+            if (nbytes) nbytes[i] = (uint32_t)n; }
     };
     if (nthreads <= 1) { work(); return; }
     std::vector<std::thread> th; for (int t = 0; t < nthreads; t++) th.emplace_back(work);
     for (auto& t : th) t.join();
+}
+void sbo_viterbi_blocks(const uint8_t* soft, uint64_t nsoft_per_block, uint32_t nblocks, int code_rate, uint32_t frame_len_bytes,
+                        uint32_t depth, uint32_t lookahead, uint8_t* out, uint64_t out_stride, int nthreads) {
+    sbo_viterbi_blocks_n(soft, nsoft_per_block, nblocks, code_rate, frame_len_bytes, depth, lookahead, out, out_stride, nullptr, nthreads);
 }
 uint32_t sbo_viterbi_signal(const uint8_t* soft48) { return viterbi_signal(soft48); }
 

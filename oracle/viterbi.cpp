@@ -97,14 +97,16 @@ uint32_t viterbi_signal(const uint8_t soft[48]) {
 
 // Whole-block decode with the brick's cadence (viterbi.hpp:104-237): groups per code rate, normalise
 // when (steps & 7)==0 after a group, windowed traceback depth/lookahead, final flush.
-// `nsoft` need not be a multiple of 48 here; the brick's 48-byte bursts only bound the granularity.
+// `nsoft` need not be a multiple of 48 here; the brick's 48-byte bursts only bound the granularity.  A trailing partial puncture group is
+// not decoded: the brick keeps it buffered for the next burst, and the device stops at the last whole group too.
 size_t viterbi_decode_block(ViterbiCore& v, const uint8_t* soft, size_t nsoft, int code_rate,
                             uint32_t frame_len_bytes, uint32_t depth, uint32_t look, uint8_t* out, uint32_t& ob_count) {
     size_t produced = 0;
     const uint32_t prefix = 6;
     const uint32_t end = frame_len_bytes * 8 + 16 + prefix;
+    const size_t group = code_rate == CR_12 ? 2 : code_rate == CR_34 ? 4 : 3;
     size_t i = 0;
-    while (i < nsoft) {
+    while (i + group <= nsoft) {
         if (code_rate == CR_12) { v.step_ab(soft[i], soft[i + 1]); i += 2; }
         else if (code_rate == CR_34) { v.step_ab(soft[i], soft[i + 1]); v.step_one(false, soft[i + 2]); v.step_one(true, soft[i + 3]); i += 4; }
         else { v.step_ab(soft[i], soft[i + 1]); v.step_one(false, soft[i + 2]); i += 3; }

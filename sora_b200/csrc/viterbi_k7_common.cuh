@@ -1,7 +1,7 @@
 // sora_b200 — what the K=7 (133,171) Viterbi kernels share: the frame record handed from kernel to kernel, the branch-metric construction
 // and the history-carrying add-compare-select step (vr_step) with its helpers.  Device functions only — no kernel, no table, no CUDA runtime
-// call — so that tests/cpp/lane_emu.cpp can compile the one-lane-per-code-block kernel for the HOST (every intrinsic it needs is a few lines of
-// C++ there) and run the very code the GPU runs against the CPU oracle without a GPU.
+// call — so that tests/cpp/lane_emu.cpp and tests/cpp/re_emu.cpp can compile the one-lane and the four- / two-lane kernels for the HOST (every
+// intrinsic they need is a few lines of C++ in tests/cpp/warp_emu.h) and run the very code the GPU runs against the CPU oracle without a GPU.
 // Arithmetic contract and machine mapping: see viterbi_k7_re.cuh (history-carrying metrics) and viterbi_k7_quad.cuh (in-place trellis).
 #pragma once
 #include <stdint.h>

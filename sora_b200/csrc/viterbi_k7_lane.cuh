@@ -336,24 +336,11 @@ __global__ void __launch_bounds__(32, 16) k_viterbi_lane(const uint8_t* __restri
     // away and the kernel got 3 % slower — it is bound by the ALU pipe, and the parity branches cost more than the wait they removed.)
     uint32_t w0[3], w1[3];
     d.fetch(pos, w0); d.fetch(pos + D::CHUNK_BYTES, w1);
-    bool stale = false;                                 // out of input while others kept stepping (cannot happen with whole-symbol inputs)
-#pragma unroll 1
-    for (;;) {
-        const bool more = !d.done && pos + D::CHUNK_BYTES <= d.nsoft;
-        if (!__any_sync(FULL, more)) break;
-        if (!more && !d.done) stale = true;
-        uint32_t w2[3];
-        d.fetch(pos + 2u * D::CHUNK_BYTES, w2);
-        if constexpr (DEFER) d.walk_tick();                 // one look-up of the window in flight (its load was issued a chunk ago)
-        const bool quiet = d.done || (more && tb + 6u < d.next_tb);
-        if (__all_sync(FULL, quiet)) d.template chunk<0, false>(w0, tb, more);
-        else d.template chunk<0, true>(w0, tb, more);
-#pragma unroll
-        for (int i = 0; i < 3; i++) { w0[i] = w1[i]; w1[i] = w2[i]; }
-        tb += 6u; pos += D::CHUNK_BYTES;
-    }
-    // tail: whole puncture groups that do not fill a 6-step chunk (standalone API with arbitrary nsoft): per lane, phases at run time
-    if (!d.done && !stale) {
+    // tail: the whole puncture groups of a code block that do not fill a 6-step chunk, per lane, phases at run time (tb, pos: the start of
+    // the chunk the lane could not fill).  A lane runs it once, as soon as it has no whole chunk left, also while other lanes of the warp still
+    // have chunks to step (802.11n symbols of 52, 104, 208 and 416 trellis steps leave a partial chunk at the end of a frame,
+    // and the flush point may lie in it).  After it the lane is done; it keeps step on zeros without triggers, like a lane that ended in the loop.
+    auto tail = [&](uint32_t tb, uint32_t pos) {
         uint32_t k = 0;                                 // steps into the chunk at tb
         auto step_rt = [&](const uint32_t cb, const uint32_t KC) {
             const uint32_t mark = 0x00010001u << (HB == 6 ? k : ((tb + k) & 7u));
@@ -378,7 +365,26 @@ __global__ void __launch_bounds__(32, 16) k_viterbi_lane(const uint8_t* __restri
             block_end();
             if (k == 6u) { k = 0; tb += 6u; }
         }
+        d.done = true;
+    };
+#pragma unroll 1
+    for (;;) {
+        const bool more = !d.done && pos + D::CHUNK_BYTES <= d.nsoft;
+        if (!__any_sync(FULL, more)) break;
+        uint32_t w2[3];
+        d.fetch(pos + 2u * D::CHUNK_BYTES, w2);
+        if constexpr (DEFER) d.walk_tick();                 // one look-up of the window in flight (its load was issued a chunk ago)
+        const bool quiet = d.done || (more && tb + 6u < d.next_tb);
+        if (__all_sync(FULL, quiet)) d.template chunk<0, false>(w0, tb, more);
+        else {                                          // a lane out of whole chunks is never quiet: its tail runs here, once per code block
+            if (!more && !d.done) tail(tb, pos);
+            d.template chunk<0, true>(w0, tb, more);
+        }
+#pragma unroll
+        for (int i = 0; i < 3; i++) { w0[i] = w1[i]; w1[i] = w2[i]; }
+        tb += 6u; pos += D::CHUNK_BYTES;
     }
+    if (!d.done) tail(tb, pos);                         // the warp ran out together
     if constexpr (DEFER) d.walk_drain();                    // the last window's walk
     if (valid) nraw_out[f] = d.nraw;
 }

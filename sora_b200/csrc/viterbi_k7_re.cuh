@@ -28,7 +28,11 @@
 // Instruction rates that shape this (tools/microbench/pipes.cu on an H100 SXM, 400 W limit): VIADDMNMX.U16x2 + IMAD/VIADD issue together at
 // ~0.9 per cycle per sub-partition; VIMNMX + two adds (the v2 ACS) at 0.74; LOP3 and PRMT at 0.5.
 #pragma once
+#ifndef SB_HOST_EMU
 #include "viterbi_k7_quad.cuh"
+#else        // host emulation (tests/cpp/re_emu.cpp): the decoder and k_viterbi_re only, without the work lists and the frame sink
+#include "viterbi_k7_common.cuh"
+#endif
 #include <type_traits>
 
 namespace sb {
@@ -214,6 +218,7 @@ struct VrDecoder {
     }
 };
 
+#ifndef SB_HOST_EMU
 // Work lists: the frames of every code rate, densely, so that each rate's launch runs warps of eight live code blocks.
 // cnt[3] must be zero on entry; list holds 3 x nframes entries.
 __global__ void k_vit_lists(const FrameInfo* __restrict__ info, uint32_t nframes, uint32_t* __restrict__ cnt, uint32_t* __restrict__ list) {
@@ -230,6 +235,7 @@ __global__ void k_vit_lists(const FrameInfo* __restrict__ info, uint32_t nframes
         if (rate == r) list[(size_t)r * nframes + base + (uint32_t)__popc(m & ((1u << (threadIdx.x & 31)) - 1u))] = f;
     }
 }
+#endif
 
 // list / cnt: work list of this code rate (k_vit_lists) or null = frames 0 .. nframes-1 with the uniform parameters of `job`.
 template <int CODE_RATE, int LB = 2>
@@ -296,32 +302,11 @@ __global__ void __launch_bounds__(32) k_viterbi_re(const uint8_t* __restrict__ s
     uint32_t w[4][3];
 #pragma unroll
     for (int c = 0; c < 4; c++) d.fetch(pos + c * D::CHUNK_BYTES, w[c]);
-    bool stale = false;                                 // out of input while others kept stepping (cannot happen with whole-symbol inputs)
-    for (;;) {
-        const bool more = !d.done && pos + D::CHUNK_BYTES <= d.nsoft;
-        if (!__any_sync(FULL, more)) break;
-        if (!more && !d.done) stale = true;
-        const bool fast_ok = d.done || (tb + 24u < d.next_tb && pos + 4u * D::CHUNK_BYTES <= d.nsoft);
-        if (phase24 == 0u && __all_sync(FULL, fast_ok)) {
-            uint32_t n[4][3];
-#pragma unroll
-            for (int c = 0; c < 4; c++) d.fetch(pos + (4 + c) * D::CHUNK_BYTES, n[c]);
-            d.template fast<0>(w);
-#pragma unroll
-            for (int c = 0; c < 4; c++) { w[c][0] = n[c][0]; w[c][1] = n[c][1]; w[c][2] = n[c][2]; }
-            tb += 24u; pos += 4u * D::CHUNK_BYTES;
-            continue;
-        }
-        uint32_t n[3];
-        d.fetch(pos + 4u * D::CHUNK_BYTES, n);
-        d.template slow<0>(w[0], tb, more);
-#pragma unroll
-        for (int c = 0; c < 3; c++) { w[c][0] = w[c + 1][0]; w[c][1] = w[c + 1][1]; w[c][2] = w[c + 1][2]; }
-        w[3][0] = n[0]; w[3][1] = n[1]; w[3][2] = n[2];
-        tb += 6u; pos += D::CHUNK_BYTES; phase24 = (phase24 + 1u) & 3u;
-    }
-    // tail: whole puncture groups that do not fill a 6-step chunk (standalone API with arbitrary nsoft): per code block, phases at run time
-    if (!d.done && !stale) {
+    // tail: the whole puncture groups of a code block that do not fill a 6-step chunk, per code block, phases at run time (tb, pos: the start
+    // of the chunk it could not fill).  A code block runs it once, as soon as it has no whole chunk left, also while other code blocks of the
+    // warp still have chunks to step (802.11n symbols of 52, 104, 208 and 416 trellis steps leave a partial chunk at the end
+    // of a frame, and the flush point may lie in it).  After it the code block is done; it keeps step on zeros without triggers.
+    auto tail = [&](uint32_t tb, uint32_t pos) {
         uint32_t k = 0;                                 // steps into the chunk at tb
         auto step_rt = [&](const uint32_t Cbase, const uint32_t KC) {
             const uint32_t mark = 0x00010001u << ((tb + k) & 7u);
@@ -346,10 +331,42 @@ __global__ void __launch_bounds__(32) k_viterbi_re(const uint8_t* __restrict__ s
             block_end();
             if (k == 6) { k = 0; tb += 6; }
         }
+        d.done = true;
+    };
+    // The lockstep loop runs while every code block has a whole chunk left or is done; when one runs out while others go on, the loop is left,
+    // that block decodes its remaining groups (tail) and is done, and the loop resumes.  One vote per iteration decides both.  (The tail
+    // called inside the loop instead changed the register allocation of the 24-step stream: 1 % on config #2, measured.)
+    for (;;) {
+        for (;;) {
+            const bool more = !d.done && pos + D::CHUNK_BYTES <= d.nsoft;
+            if (__reduce_or_sync(FULL, more ? 1u : d.done ? 0u : 2u) != 1u) break;   // 0: all done, 2 or 3: a code block is out of whole chunks
+            const bool fast_ok = d.done || (tb + 24u < d.next_tb && pos + 4u * D::CHUNK_BYTES <= d.nsoft);
+            if (phase24 == 0u && __all_sync(FULL, fast_ok)) {
+                uint32_t n[4][3];
+#pragma unroll
+                for (int c = 0; c < 4; c++) d.fetch(pos + (4 + c) * D::CHUNK_BYTES, n[c]);
+                d.template fast<0>(w);
+#pragma unroll
+                for (int c = 0; c < 4; c++) { w[c][0] = n[c][0]; w[c][1] = n[c][1]; w[c][2] = n[c][2]; }
+                tb += 24u; pos += 4u * D::CHUNK_BYTES;
+                continue;
+            }
+            uint32_t n[3];
+            d.fetch(pos + 4u * D::CHUNK_BYTES, n);
+            d.template slow<0>(w[0], tb, more);
+#pragma unroll
+            for (int c = 0; c < 3; c++) { w[c][0] = w[c + 1][0]; w[c][1] = w[c + 1][1]; w[c][2] = w[c + 1][2]; }
+            w[3][0] = n[0]; w[3][1] = n[1]; w[3][2] = n[2];
+            tb += 6u; pos += D::CHUNK_BYTES; phase24 = (phase24 + 1u) & 3u;
+        }
+        const bool more = !d.done && pos + D::CHUNK_BYTES <= d.nsoft;
+        if (!more && !d.done) tail(tb, pos);
+        if (!__any_sync(FULL, more)) break;
     }
     if (valid && q == 0) nraw_out[f] = d.nraw;
 }
 
+#ifndef SB_HOST_EMU
 // Descrambler + frame sink after the Viterbi kernel, one thread per frame (T11aDesc, scramble.hpp:269-355; TBB11aFrameSink, PHY_11a.hpp:609-702):
 // raw bytes (SERVICE + scrambled PSDU) sit at row + 14 so that the PSDU starts 16-byte aligned at row + 16; the descrambled PSDU goes to row + 0.
 // The first SERVICE byte is dropped, the second seeds the register (byte >> 1), then out = byte ^ lut[reg], reg advances by eight bits per byte.
@@ -420,5 +437,6 @@ __global__ void __launch_bounds__(128) k_sink11a(uint8_t* __restrict__ out, uint
     }
     status_io[f] = verdict; crc_out[f] = fcs;
 }
+#endif
 
 } // namespace sb

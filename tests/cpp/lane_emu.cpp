@@ -1,51 +1,18 @@
 // Host emulation of the one-lane-per-code-block Viterbi kernel (sora_b200/csrc/viterbi_k7_lane.cuh): the DEVICE SOURCE ITSELF, compiled by g++
-// with the handful of CUDA intrinsics it uses written out in C++ below, one lane at a time.  Test infrastructure (tests/test_cpu_lane_emu.py
-// compares it with the CPU oracle); it lets the -m "not gpu" suite check the kernel's trellis, history blocks, trigger schedule, traceback and
-// bit packing where no GPU exists.  What it cannot see: anything that depends on 32 lanes really running together — the kernel is written so
-// that nothing does (a lane never reads another lane's data; the warp votes only choose between two bodies that compute the same thing).
+// with the CUDA intrinsics it uses written out in C++ (warp_emu.h).  Test infrastructure (tests/test_cpu_lane_emu.py compares it with the CPU
+// oracle); it lets the -m "not gpu" suite check the kernel's trellis, history blocks, trigger schedule, traceback and bit packing where no GPU
+// exists.  A lane never reads another lane's data, but the warp votes of the step loop decide together when the loop ends and which lanes
+// step on without input while others still have some: so the 32 lanes of a CTA run as 32 threads, and every vote is a real vote of all 32.
 //
-//   g++ -O1 -std=c++17 -shared -fPIC -DSB_HOST_EMU -I sora_b200/csrc -o lane_emu.so tests/cpp/lane_emu.cpp
-#include <algorithm>
-#include <cstdint>
-#include <cstring>
-#include <vector>
-
-#define __device__
-#define __host__
-#define __global__
-#define __forceinline__ inline
-#define __noinline__ __attribute__((noinline))
-#define __launch_bounds__(...)
-#define __restrict__
-
-struct uint2 { uint32_t x, y; };
-struct uint4 { uint32_t x, y, z, w; };
-struct Dim { unsigned x = 0, y = 0, z = 0; };
-static thread_local Dim threadIdx, blockIdx;
-
-using std::min; using std::max;
-static inline uint32_t __byte_perm(uint32_t a, uint32_t b, uint32_t s) {        // PRMT, default mode: selector nibble n picks byte n of {b, a}
-    const uint64_t v = ((uint64_t)b << 32) | a; uint32_t r = 0;
-    for (int i = 0; i < 4; i++) r |= (uint32_t)((v >> (8 * ((s >> (4 * i)) & 7u))) & 0xFFu) << (8 * i);
-    return r;
-}
-static inline uint32_t __brev(uint32_t v) { uint32_t r = 0; for (int i = 0; i < 32; i++) r |= ((v >> i) & 1u) << (31 - i); return r; }
-static inline uint32_t __vminu2(uint32_t a, uint32_t b) { return min(a & 0xFFFFu, b & 0xFFFFu) | (min(a >> 16, b >> 16) << 16); }
-static inline uint32_t __vadd2(uint32_t a, uint32_t b) { return ((a + b) & 0xFFFFu) | (((a >> 16) + (b >> 16)) << 16); }     // per-half wrap-around add
-static inline uint32_t __viaddmin_u16x2(uint32_t a, uint32_t b, uint32_t c) { return __vminu2(__vadd2(a, b), c); }           // min(a + b, c) per half, unsigned
-template <class T> static inline T __ldg(const T* p) { return *p; }
-template <class T> static inline T __ldcg(const T* p) { return *p; }
-template <class T> static inline void __stcg(T* p, const T& v) { *p = v; }
-static inline uint32_t __shfl_xor_sync(unsigned, uint32_t v, int) { return v; }   // never reached with one lane per code block
-static inline bool __any_sync(unsigned, bool p) { return p; }                    // one lane at a time: the vote is its own predicate
-static inline bool __all_sync(unsigned, bool p) { return p; }
-
+//   g++ -O1 -std=c++20 -pthread -shared -fPIC -DSB_HOST_EMU -I sora_b200/csrc -o lane_emu.so tests/cpp/lane_emu.cpp
+#include "warp_emu.h"
 #include "viterbi_k7_lane.cuh"
 
 // Decode nblocks code blocks the way sb200_viterbi_k7 launches the kernel (uniform parameters, no work list): every CTA of 32 lanes, every lane.
+// lens / nsofts: per code block (the receive chains' FrameInfo path) or null.  hb: columns per history block, 6 or 8; 9 = 8 with the deferred walk.
 extern "C" int lane_emu_viterbi(const uint8_t* soft, uint64_t soft_stride, uint32_t nsoft, uint32_t nblocks, int code_rate, uint32_t frame_len,
                                 uint32_t depth, uint32_t lookahead, uint8_t* out, uint64_t out_stride, uint32_t* nraw,
-                                const uint32_t* lens, const uint32_t* nsofts, int hb) {   // hb: columns per history block, 6 or 8; 9 = 8 with the deferred walk    // lens / nsofts: per code block (the receive chains' FrameInfo path) or null
+                                const uint32_t* lens, const uint32_t* nsofts, int hb) {
     if (code_rate < 0 || code_rate > 2 || (hb != 6 && hb != 8 && hb != 9)) return -1;
     std::vector<sb::FrameInfo> fi;
     if (lens && nsofts) { fi.resize(nblocks); for (uint32_t i = 0; i < nblocks; i++) { fi[i] = sb::FrameInfo{}; fi[i].length = lens[i]; fi[i].soft_bytes = nsofts[i]; fi[i].code_rate = (uint32_t)code_rate; } }
@@ -53,13 +20,12 @@ extern "C" int lane_emu_viterbi(const uint8_t* soft, uint64_t soft_stride, uint3
     sb::VitJob job{}; job.code_rate = (uint32_t)code_rate; job.frame_len = frame_len; job.nsoft = nsoft; job.depth = depth; job.lookahead = lookahead; job.raw = 1;
     const uint32_t ctas = (nblocks + SB_VL_FR - 1) / SB_VL_FR;
     std::vector<uint4> ring((size_t)ctas * SB_VL_NB8D * SB_VL_ENTRY);
-    for (uint32_t c = 0; c < ctas; c++) for (unsigned lane = 0; lane < 32; lane++) {
-        blockIdx.x = c; threadIdx.x = lane;
+    for (uint32_t c = 0; c < ctas; c++) warp_emu::run_cta(c, [&] {
 #define SB_EMU_RUND(CR) sb::k_viterbi_lane<CR, 8, true>(soft, soft_stride, nblocks, nullptr, nullptr, info, job, out, out_stride, 0u, nraw, ring.data(), 0u)
 #define SB_EMU_RUN(CR, HB) sb::k_viterbi_lane<CR, HB>(soft, soft_stride, nblocks, nullptr, nullptr, info, job, out, out_stride, 0u, nraw, ring.data(), 0u)
         if (hb == 6) { if (code_rate == sb::CR_12) SB_EMU_RUN(sb::CR_12, 6); else if (code_rate == sb::CR_23) SB_EMU_RUN(sb::CR_23, 6); else SB_EMU_RUN(sb::CR_34, 6); }
         else if (hb == 9) { if (code_rate == sb::CR_12) SB_EMU_RUND(sb::CR_12); else if (code_rate == sb::CR_23) SB_EMU_RUND(sb::CR_23); else SB_EMU_RUND(sb::CR_34); }
         else         { if (code_rate == sb::CR_12) SB_EMU_RUN(sb::CR_12, 8); else if (code_rate == sb::CR_23) SB_EMU_RUN(sb::CR_23, 8); else SB_EMU_RUN(sb::CR_34, 8); }
-    }
+    });
     return 0;
 }

@@ -95,6 +95,17 @@ def viterbi_blocks(soft2d, code_rate, frame_len_bytes, depth=256, lookahead=24, 
                              C.c_uint32(depth), C.c_uint32(lookahead), _p(out), C.c_uint64(stride), C.c_int(nthreads))
     return out
 
+def viterbi_blocks_n(soft2d, code_rate, frame_len_bytes, depth=256, lookahead=24, nthreads=1):
+    """viterbi_blocks, plus the bytes each block produced: fewer than L + 2 when its soft values end before the flush point
+    (only out[i, :n[i]] is defined then; the rest of the row is zero)."""
+    soft2d = np.ascontiguousarray(soft2d, dtype=np.uint8)
+    nb, ns = soft2d.shape
+    stride = frame_len_bytes + 2
+    out = np.zeros((nb, stride), dtype=np.uint8); n = np.zeros(nb, dtype=np.uint32)
+    lib().sbo_viterbi_blocks_n(_p(soft2d), C.c_uint64(ns), C.c_uint32(nb), C.c_int(code_rate), C.c_uint32(frame_len_bytes),
+                               C.c_uint32(depth), C.c_uint32(lookahead), _p(out), C.c_uint64(stride), _p(n), C.c_int(nthreads))
+    return out, n
+
 def fft64(x):
     x = np.ascontiguousarray(x, dtype=np.int16); o = np.zeros((64, 2), np.int16); lib().sbo_fft64(_p(x), _p(o)); return o
 def ifft64(x):

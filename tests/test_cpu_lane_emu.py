@@ -1,8 +1,10 @@
 """The one-lane-per-code-block Viterbi kernel (sora_b200/csrc/viterbi_k7_lane.cuh) WITHOUT a GPU: its device source is compiled for the host
-by tests/cpp/lane_emu.cpp (the few CUDA intrinsics it uses are written out in C++ there, lanes run one after another) and compared with the
-CPU oracle, bit for bit, on the cases the GPU tests use: clean and noisy code words, wrap-around garbage, block lengths that end anywhere in
-the 6-step trellis phase / 8-step normalisation period / 6-column history block, both traceback windows, and code blocks of different lengths
-side by side (the receive chains' per-frame path).  The GPU run of the same kernel is in tests/test_gpu_rx11a.py."""
+by tests/cpp/lane_emu.cpp (the CUDA intrinsics it uses are written out in C++ in tests/cpp/warp_emu.h; the 32 lanes of a CTA run as 32
+threads and every warp vote is a real vote) and compared with the CPU oracle, bit for bit, on the cases the GPU tests use: clean and noisy
+code words, wrap-around garbage, block lengths that end anywhere in the 6-step trellis phase / 8-step normalisation period / 6-column history
+block, both traceback windows, code blocks of different lengths side by side (the receive chains' per-frame path), and code blocks that run
+out of whole 6-step chunks while a neighbour in the warp still has some (802.11n symbols).  The GPU run of the same kernel is in
+tests/test_gpu_rx11a.py and tests/test_gpu_zz_viterbi_ragged.py."""
 import ctypes as C, os, shutil, subprocess
 import numpy as np, pytest
 import oracle_py
@@ -16,7 +18,7 @@ pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="no host com
 @pytest.fixture(scope="module")
 def emu(tmp_path_factory):
     so = str(tmp_path_factory.mktemp("lane_emu") / "lane_emu.so")
-    subprocess.check_call(["g++", "-O1", "-std=c++17", "-shared", "-fPIC", "-DSB_HOST_EMU", "-Wno-unknown-pragmas", "-I", CSRC, "-o", so, SRC])
+    subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-shared", "-fPIC", "-DSB_HOST_EMU", "-Wno-unknown-pragmas", "-I", CSRC, "-o", so, SRC])
     lib = C.CDLL(so)
     lib.lane_emu_viterbi.argtypes = [C.c_void_p, C.c_uint64, C.c_uint32, C.c_uint32, C.c_int, C.c_uint32, C.c_uint32, C.c_uint32, C.c_void_p, C.c_uint64,
                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_int]
@@ -108,3 +110,68 @@ def test_short_windows(emu, hb):
             g, _ = emu(soft, cr, L, depth, look, hb=hb)
             o = oracle_py.viterbi_blocks(soft, cr, L, depth, look)
             assert (g == o).all(), (cr, depth, look, np.argwhere(g != o)[:4])
+
+# 802.11n soft bytes per OFDM symbol (N_CBPS, two streams) and code rate: MCS 8, 9, 11 (rate 1/2, 52 / 104 / 208 trellis steps per symbol)
+# and 13 (rate 2/3, 416) are not whole 6-step chunks; MCS 10 and 14 (rate 3/4, 156 and 468) are.
+N11N = ((CR_12, 104), (CR_12, 208), (CR_12, 416), (CR_23, 624), (CR_34, 208), (CR_34, 624))
+GROUPS = {CR_12: (2, 1), CR_23: (3, 2), CR_34: (4, 3)}          # soft bytes and trellis steps per puncture group
+RATES = {CR_12: (1, 2), CR_23: (2, 3), CR_34: (3, 4)}
+
+def ragged_11n_blocks(rng, cr, ncbps, nblocks=40):
+    """Code blocks the way k_front11n hands them over: whole symbols of ncbps soft bytes.  Short blocks whose flush point (8 L + 22 steps) lies
+    past their last whole 6-step chunk, at every offset it can take there, alternate with long blocks, so that every warp of every kernel
+    rendering holds both and the short ones run out of whole chunks while their neighbours go on.  Clean code words of varying confidence.
+    Returns soft [nblocks, max nsoft], lens, nsofts and the sent bits."""
+    per, gst = GROUPS[cr]
+    spsym = ncbps // per * gst                                       # trellis steps per symbol
+    shape = lambda L: (lambda S: (S, S // 6 * 6))(-(-(8 * L + 22) // spsym) * spsym)
+    by_off = {}
+    for L in range(1, 500):
+        S, whole = shape(L)
+        if 8 * L + 22 > whole: by_off.setdefault(8 * L + 22 - whole, []).append(L)
+    short = [L for off in sorted(by_off) for L in by_off[off][:4]] or [5, 61, 62, 99]   # rate 3/4: no such length (whole chunks), plain ones
+    lens = []
+    for i in range(nblocks):
+        lens.append(short[(i // 2) % len(short)] if i % 2 == 0 else 200 + 37 * (i % 5))
+    lens = np.array(lens, np.uint32)
+    nsofts = np.array([shape(int(L))[0] // gst * per for L in lens], np.uint32)
+    ns = int(nsofts.max())
+    soft = np.zeros((nblocks, ns), np.uint8); sent = []
+    for i, L in enumerate(lens):
+        S = int(nsofts[i]) // per * gst
+        bits = rng.integers(0, 2, S).astype(np.uint8); bits[8 * int(L) + 16:] = 0
+        A, B = synth.conv_encode(bits)
+        coded = synth.puncture(A, B, RATES[cr])
+        sv = np.where(coded > 0, rng.integers(4, 8, coded.shape), rng.integers(0, 4, coded.shape))
+        soft[i, :len(coded)] = sv; sent.append(bits)
+    return soft, lens, nsofts, sent
+
+def check_ragged(run, cr, ncbps, seed, **kw):
+    """run(soft, cr, Lmax, depth, look, lens=, nsofts=, **kw) -> (bytes, nraw): every block must equal the oracle in full."""
+    soft, lens, nsofts, sent = ragged_11n_blocks(np.random.default_rng(seed), cr, ncbps)
+    g, nraw = run(soft, cr, int(lens.max()), 192, 36, lens=lens, nsofts=nsofts, **kw)
+    for i in range(len(lens)):
+        L = int(lens[i]); n = int(nsofts[i])
+        assert nraw[i] == L + 2, "block %d L=%d nsoft=%d: nraw %d, want %d" % (i, L, n, nraw[i], L + 2)
+        o = oracle_py.viterbi_blocks(soft[i:i + 1, :n], cr, L, 192, 36)[0]
+        assert (g[i, :L + 2] == o).all(), (i, L, np.argwhere(g[i, :L + 2] != o)[:4])
+        assert (np.unpackbits(o, bitorder="little")[:8 * L + 16] == sent[i][:8 * L + 16]).all(), (i, L)
+
+@HB
+@pytest.mark.parametrize("cr, ncbps", N11N)
+def test_ragged_chunks_11n_symbols(emu, hb, cr, ncbps):
+    """A code block that runs out of whole 6-step chunks while a neighbour in its warp still has some must still decode its remaining
+    whole groups and fire its last traceback window (802.11n frames: N_CBPS soft bytes per symbol, flush point in the last partial chunk)."""
+    check_ragged(emu, cr, ncbps, 40 + ncbps + cr, hb=hb)
+
+def test_ragged_chunks_two_blocks(emu):
+    """The smallest case: L = 62 with 10 x 104 soft bytes beside L = 200 with 32 x 104 (rate 1/2, 802.11n window)."""
+    rng = np.random.default_rng(62)
+    soft = rng.integers(0, 8, (2, 32 * 104)).astype(np.uint8)
+    lens = np.array([62, 200], np.uint32); nsofts = np.array([10 * 104, 32 * 104], np.uint32)
+    for hb in (6, 8, 9):
+        g, nraw = emu(soft, CR_12, 200, 192, 36, lens=lens, nsofts=nsofts, hb=hb)
+        for i in range(2):
+            L = int(lens[i])
+            assert nraw[i] == L + 2, "hb %d block %d L=%d: nraw %d, want %d" % (hb, i, L, nraw[i], L + 2)
+            assert (g[i, :L + 2] == oracle_py.viterbi_blocks(soft[i:i + 1, :nsofts[i]], CR_12, L, 192, 36)[0]).all(), (hb, i)
