@@ -263,7 +263,8 @@ struct sb200_handle {
     uint32_t vl_hb = 8;                                // option vl_hist_block: columns per history block of the lane kernel (6 | 8)
     uint32_t vl_flags = 1;                             // option vl_l2_hints: bit 0 ring traffic evict_last, bit 1 soft values evict_first (viterbi_k7_lane.cuh)
     uint32_t vl_pad_smem = 0;                          // experiment knob: the same for the lane kernel (fewer resident warps = a smaller history-ring working set in L2)
-    uint32_t vq_pad_smem = 0;                          // experiment knob: extra dynamic shared memory per Viterbi CTA (lowers occupancy)
+    uint32_t vq_pad_smem = 0;                          // experiment knob: extra dynamic shared memory per Viterbi CTA of the 802.11a receiver (lowers occupancy)
+    struct VrOcc { uint32_t smem = 0, ctas = 0; } vr_occ[2][3];   // k_viterbi_re<CR, LB>: grid of its persistent CTAs, for `smem` bytes of padding
     // viterbi_k7_lane.cuh (one lane per code block, 32 per warp) needs a large batch to fill the machine: it decodes launches of at least
     // lane_min and at most lane_max code blocks, the four-lanes-per-code-block kernel the others.  Options "viterbi_lane_min" / "viterbi_lane_max";
     // SB200_VITERBI=v8 forces it (0 .. 0xFFFFFFFF), v3 forbids it.
@@ -488,51 +489,75 @@ static int slot_table(sb200_handle* h, const uint64_t* frame_off, const uint32_t
     return SB200_OK;
 }
 
-// One launch of the Viterbi for code rate CR: SB200_VITERBI=v2 the per-step-mark quad kernel (dynamic shared memory `smem`); else the lane
+// One launch of the Viterbi for code rate CR: SB200_VITERBI=v2 the per-step-mark quad kernel; else the lane
 // kernel (viterbi_k7_lane.cuh) for launches of lane_min .. lane_max code blocks, in the rendering the options select (8-column history blocks
 // with the deferred walk unless told otherwise); below that the four-lanes-per-code-block kernel (SB200_VITERBI=v4: two lanes, for A/B).
+// `smem`: dynamic shared memory of the quad and the four- / two-lane kernels (padding, the vq_pad_smem knob).
 // vring_need() sizes the lane kernel's history rings for n code blocks first.
 static bool use_lane(const sb200_handle* h, uint32_t n) { return n >= h->lane_min && n <= h->lane_max; }
 static cudaError_t vring_need(sb200_handle* h, uint32_t n) {
     if (use_lane(h, n)) return h->vring.need((size_t)((n + SB_VL_FR - 1) / SB_VL_FR) * SB_VL_NB8D * SB_VL_ENTRY * 16);   // the largest ring of the lane kernel's renderings
     return cudaSuccess;                                // the four- / two-lane kernels keep their ring in shared memory
 }
+// k_viterbi_re<CR, LB> as persistent CTAs: at most as many as the SMs hold at once with `smem` bytes of dynamic shared memory (the
+// occupancy calculator's count, taken once per handle and padding), each taking groups of code blocks from the counter `next`.
+template <int CR, int LB>
+static cudaError_t launch_re(sb200_handle* h, uint32_t n, cudaStream_t s, uint32_t smem, const uint8_t* soft, uint64_t soft_stride, const uint32_t* list,
+                             const uint32_t* cnt, const FrameInfo* info, const VitJob& job, uint8_t* out, uint64_t out_stride, uint32_t raw_off,
+                             uint32_t* nraw, uint32_t* next) {
+    sb200_handle::VrOcc& o = h->vr_occ[LB - 1][CR];
+    if (o.ctas == 0 || o.smem != smem) {
+        if (!h->sms) { const cudaError_t e = cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, h->device); if (e != cudaSuccess) return e; }
+        int per_sm = 0;
+        const cudaError_t e = cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_viterbi_re<CR, LB>, 32, smem);
+        if (e != cudaSuccess) return e;
+        o.ctas = (uint32_t)max(per_sm, 1) * (uint32_t)h->sms; o.smem = smem;
+    }
+    const uint32_t groups = (n + (32u >> LB) - 1) / (32u >> LB);
+    k_viterbi_re<CR, LB><<<min(groups, o.ctas), 32, smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, next);
+    return cudaSuccess;
+}
 template <int CR>
-static void launch_viterbi(sb200_handle* h, uint32_t n, cudaStream_t s, const uint8_t* soft, uint64_t soft_stride, const uint32_t* list, const uint32_t* cnt,
-                           const FrameInfo* info, const VitJob& job, uint8_t* out, uint64_t out_stride, uint32_t* status, uint32_t* crc, uint32_t smem) {
-    if (h->use_v2) { k_viterbi_quad<CR><<<(n + SB_VQ_FR - 1) / SB_VQ_FR, 32 * SB_VQ_WARPS, smem, s>>>(soft, soft_stride, n, info, job, h->T, out, out_stride, status, crc); return; }
-    const unsigned g = (n + SB_VR_FR - 1) / SB_VR_FR, gp = (n + 15) / 16;
+static cudaError_t launch_viterbi(sb200_handle* h, uint32_t n, cudaStream_t s, const uint8_t* soft, uint64_t soft_stride, const uint32_t* list, const uint32_t* cnt,
+                                  const FrameInfo* info, const VitJob& job, uint8_t* out, uint64_t out_stride, uint32_t* status, uint32_t* crc, uint32_t smem,
+                                  uint32_t* next) {
+    if (h->use_v2) { k_viterbi_quad<CR><<<(n + SB_VQ_FR - 1) / SB_VQ_FR, 32 * SB_VQ_WARPS, smem, s>>>(soft, soft_stride, n, info, job, h->T, out, out_stride, status, crc); return cudaSuccess; }
     const uint32_t raw_off = info ? 14u : 0u; uint32_t* const nraw = status;   // frames are decoded 14 bytes into their row, raw blocks at its start
     uint4* const ring = (uint4*)h->vring.p;             // the lane kernel's history rings
     h->last_vit = use_lane(h, n) ? "k_viterbi_lane" : "k_viterbi_re";
     if (use_lane(h, n) && h->vl_hb == 8 && h->vl_defer) k_viterbi_lane<CR, 8, true><<<(n + SB_VL_FR - 1) / SB_VL_FR, 32, h->vl_pad_smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, ring, h->vl_flags);
     else if (use_lane(h, n) && h->vl_hb == 8) k_viterbi_lane<CR, 8><<<(n + SB_VL_FR - 1) / SB_VL_FR, 32, h->vl_pad_smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, ring, h->vl_flags);
     else if (use_lane(h, n))         k_viterbi_lane<CR, 6><<<(n + SB_VL_FR - 1) / SB_VL_FR, 32, h->vl_pad_smem, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw, ring, h->vl_flags);
-    else if (h->use_pair)            k_viterbi_re<CR, 1><<<gp, 32, 0, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw);
-    else                             k_viterbi_re<CR, 2><<<g, 32, 0, s>>>(soft, soft_stride, n, list, cnt, info, job, out, out_stride, raw_off, nraw);
+    else if (h->use_pair)            return launch_re<CR, 1>(h, n, s, smem, soft, soft_stride, list, cnt, info, job, out, out_stride, raw_off, nraw, next);
+    else                             return launch_re<CR, 2>(h, n, s, smem, soft, soft_stride, list, cnt, info, job, out, out_stride, raw_off, nraw, next);
+    return cudaSuccess;
 }
 
 // The Viterbi stage: one launch per code rate of `rates`, in that order.  Frames (`info` set) get work lists (vlist from frame `first`, vcnt
-// block `slot`; the quad kernel needs none) and k_sink11a; raw code blocks (`info` null) neither.  `smem34`: the 802.11a vq_pad_smem knob.
+// block `slot`: the counts, then the group counters of k_viterbi_re's three code rates; the quad kernel needs neither) and k_sink11a; raw
+// code blocks (`info` null) only the counters.  `smem34`: the 802.11a vq_pad_smem knob.
 static int viterbi_stage(sb200_handle* h, uint32_t n, cudaStream_t s, const uint8_t* soft, uint64_t soft_stride, const FrameInfo* info, const VitJob& job,
                          uint8_t* out, uint64_t out_stride, uint32_t* status, uint32_t* crc, const int* rates, uint32_t nrates,
                          uint32_t first = 0, uint32_t slot = 0, uint32_t smem34 = 0) {
-    const uint32_t* list = nullptr; const uint32_t* cnt = nullptr;
+    const uint32_t* list = nullptr; const uint32_t* cnt = nullptr; uint32_t* next = nullptr;
     if (!h->use_v2) {
         CK(vring_need(h, n));
+        CK(h->vcnt.need(32ull * (slot + 1u)));
+        uint32_t* d_cnt = (uint32_t*)h->vcnt.p + 8 * (size_t)slot;
+        CK(cudaMemsetAsync(d_cnt, 0, 32, s));
+        next = d_cnt + 4;
         if (info) {
-            CK(h->vlist.need((first + (size_t)n) * 12ull)); CK(h->vcnt.need(16ull * (slot + 1u)));
-            uint32_t* d_list = (uint32_t*)h->vlist.p + 3 * (size_t)first; uint32_t* d_cnt = (uint32_t*)h->vcnt.p + 4 * (size_t)slot;
-            CK(cudaMemsetAsync(d_cnt, 0, 16, s));
+            CK(h->vlist.need((first + (size_t)n) * 12ull));
+            uint32_t* d_list = (uint32_t*)h->vlist.p + 3 * (size_t)first;
             k_vit_lists<<<(n + 255) / 256, 256, 0, s>>>(info, n, d_cnt, d_list);
             list = d_list; cnt = d_cnt; h->launches += 1;
         }
     }
     for (uint32_t r = 0; r < nrates; r++) {
         const int cr = rates[r];
-        if (cr == CR_34) launch_viterbi<CR_34>(h, n, s, soft, soft_stride, list, cnt, info, job, out, out_stride, status, crc, smem34);
-        else if (cr == CR_12) launch_viterbi<CR_12>(h, n, s, soft, soft_stride, list, cnt, info, job, out, out_stride, status, crc, 0);
-        else launch_viterbi<CR_23>(h, n, s, soft, soft_stride, list, cnt, info, job, out, out_stride, status, crc, 0);
+        if (cr == CR_34) CK(launch_viterbi<CR_34>(h, n, s, soft, soft_stride, list, cnt, info, job, out, out_stride, status, crc, smem34, next + CR_34));
+        else if (cr == CR_12) CK(launch_viterbi<CR_12>(h, n, s, soft, soft_stride, list, cnt, info, job, out, out_stride, status, crc, 0, next + CR_12));
+        else CK(launch_viterbi<CR_23>(h, n, s, soft, soft_stride, list, cnt, info, job, out, out_stride, status, crc, 0, next + CR_23));
     }
     h->launches += nrates;
     if (info && !h->use_v2) { k_sink11a<<<(n + 127) / 128, 128, 0, s>>>(out, out_stride, n, info, h->T, status, crc); h->launches += 1; }
@@ -602,7 +627,7 @@ static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
     const uint32_t want = (no_chunk || rate20) ? 0u : iq_dev ? h->chunk_frames_device : h->chunk_frames;
     const uint32_t chunk = (want == 0 || tapping || nframes <= want || (!iq_dev && !tab_on_host)) ? nframes : want;
     const bool pipelined = chunk < nframes;
-    CK(h->vcnt.need(16ull * ((nframes + chunk - 1) / chunk)));
+    CK(h->vcnt.need(32ull * ((nframes + chunk - 1) / chunk)));
     const bool res_dev_all = is_device_ptr(res), out_dev_all = out_bytes && is_device_ptr(out_bytes);
     sb200_frame_result* d_res_all = res_dev_all ? res : (sb200_frame_result*)h->res.p;
     CK(cudaEventRecord(h->ev0, st));

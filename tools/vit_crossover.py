@@ -9,6 +9,7 @@ import torch
 from sora_b200 import api, synth
 def main():
     dev = torch.device("cuda", 0); eng = api.Engine(0); st = torch.cuda.current_stream()
+    eng.set_option("viterbi_lane_max", 0xFFFFFFFF)       # no upper bound: 65 536 code blocks take the lane kernel too when lane_min allows
     L = 1500; cr = api.CR_34
     nbits = 8 * L + 16 + 6; nbits += (-nbits) % 48
     rng = np.random.default_rng(1); U = 64
