@@ -15,7 +15,7 @@
 //                Reference: freqoffset_11n.hpp:42-279, dsp_math.h:90-247, fft.hpp:110-135, channel_11n.hpp:34-521,
 //                sora_matrix.h:135-150,296-304, PHY_11n.hpp:283-514, demapper11n.hpp:8-171, dsp_demap.h:38-137,
 //                deinterleaver_11n.hpp:6-620, stdbrick.hpp:639-720, pilot_11n.hpp:84-141, viterbicore.h:36-261.
-//   The K=7 Viterbi / descrambler / CRC-32 stage is k_viterbi_quad (viterbi_k7_quad.cuh) with the 11n window 192/36
+//   The K=7 Viterbi / descrambler / CRC-32 stage is the 802.11a one (k_viterbi_re or k_viterbi_lane, then k_sink11a) with the 11n window 192/36
 //   (fb11ndemod_config.hpp:189); the brick's 312-value bursts and zero padding at Flush never reach a decision that is
 //   delivered, because the final traceback fires inside the last real symbol.
 #pragma once

@@ -1,8 +1,8 @@
 // sora_b200 — what the K=7 (133,171) Viterbi kernels share: the frame record handed from kernel to kernel, the branch-metric construction
 // and the history-carrying add-compare-select step (vr_step) with its helpers.  Device functions only — no kernel, no table, no CUDA runtime
-// call — so that tests/cpp/lane_emu.cpp and tests/cpp/re_emu.cpp can compile the one-lane and the four- / two-lane kernels for the HOST (every
+// call — so that tests/cpp/lane_emu.cpp and tests/cpp/re_emu.cpp can compile the one-lane and the four-lane kernels for the HOST (every
 // intrinsic they need is a few lines of C++ in tests/cpp/warp_emu.h) and run the very code the GPU runs against the CPU oracle without a GPU.
-// Arithmetic contract and machine mapping: see viterbi_k7_re.cuh (history-carrying metrics) and viterbi_k7_quad.cuh (in-place trellis).
+// Arithmetic contract and machine mapping: see viterbi_k7_re.cuh (history-carrying metrics, in-place trellis).
 #pragma once
 #include <stdint.h>
 
@@ -82,8 +82,8 @@ struct VrLane {
 //   T <= 1 : mA = mark if this lane holds the odd role else 0, mB = mark - mA;   T = 2..4 : mA = mark;   T = 5 : mA = mark << 16 part, mB = low part.
 // The marks come in as registers so that every constant add is an IMAD.IADD (FMA pipe), not an immediate VIADD (ALU pipe, the busy one).
 // WARP: the whole warp executes the step together (full-mask shuffle).
-// LB = lane bits of the slot address: 2 = four lanes per code block, 8 registers per lane (slot = lane << 4 | reg << 1 | half);
-//                                      1 = two lanes per code block, 16 registers per lane (slot = lane << 5 | reg << 1 | half).
+// LB = lane bits of the slot address: 2 = four lanes per code block, 8 registers per lane (slot = lane << 4 | reg << 1 | half; k_viterbi_re);
+//                                      0 = one lane per code block, 32 registers (slot = reg << 1 | half; k_viterbi_lane).
 // The address bit replaced at phase T is bit 5 - T: a lane bit for T < LB (exchange with lane xor 1 << (LB - 1 - T)), a register bit for
 // LB <= T <= 4 (pair r, r + (1 << (4 - T))), the half for T = 5.
 template <int T, bool WARP, int LB>
@@ -135,7 +135,7 @@ __device__ __forceinline__ void vr_step_rt(uint32_t (&R)[8 << (2 - LB)], const u
     else vr_step<T, WARP, LB>(R, Cbase, L, KC, mark & 0xFFFF0000u, mark & 0x0000FFFFu, qmask);
 }
 
-// branch-metric vector of step s (0..5) of a 6-step chunk held in w[] (vq_bm_*: viterbi_k7_quad.cuh)
+// branch-metric vector of step s (0..5) of a 6-step chunk held in w[] (vq_bm_* above)
 template <int CODE_RATE, int s> __device__ __forceinline__ uint32_t vr_bm(const uint32_t (&w)[3]) {
     if constexpr (CODE_RATE == CR_12) return (s & 1) ? vq_bm_ab<2>(w[s >> 1]) : vq_bm_ab<0>(w[s >> 1]);
     else if constexpr (CODE_RATE == CR_34) return s % 3 == 0 ? vq_bm_ab<0>(w[s / 3]) : s % 3 == 1 ? vq_bm_a<2>(w[s / 3]) : vq_bm_b<3>(w[s / 3]);

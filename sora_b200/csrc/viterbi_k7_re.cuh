@@ -1,4 +1,4 @@
-// sora_b200 — batched K=7 (133,171) soft Viterbi, v3 "history-carrying" kernel for sm_90a.
+// sora_b200 — batched K=7 (133,171) soft Viterbi, four-lane "history-carrying" kernel for sm_90a.
 //
 // Arithmetic contract (bit-exact with kernel/bb/Brick11/src/viterbicore.h:269-556 driven like
 // kernel/bb/Brick11/src/viterbi.hpp:104-237): path metrics are the reference's uint8 values, whose LSB is the survivor mark and whose upper
@@ -6,9 +6,12 @@
 //     new = min_u8( (old[p] + bm) & 0xFE , (old[p+32] + bm') | 1 )   ==   m7' = min(a7, b7) mod 128 with ties to the even candidate,
 //     decision d = (b7 < a7).
 //
-// Machine mapping (the quad / in-place trellis of v2, viterbi_k7_quad.cuh, with different bookkeeping):
+// Machine mapping:
 //   * 4 lanes per code block, 16 metrics per lane, two per register as 16-bit halves; m7 sits in bits 9..15 of its half, so the uint8 wrap is the
-//     half's own carry-out.  Every add is a per-half SIMD add (VIADD.16x2, or the add inside VIADDMNMX.U16x2): nothing crosses halves.
+//     half's own carry-out.  The trellis is updated in place: slot A = lane << 4 | register << 1 | half holds state rol6(A, t mod 6) at time t,
+//     so the butterfly partner of a slot is in the partner lane (two steps of six), the other half of the register (one step) or another
+//     register of the lane (three): only two steps in six exchange metrics between lanes.  Every add is a per-half SIMD add (VIADD.16x2,
+//     or the add inside VIADDMNMX.U16x2): nothing crosses halves.
 //   * The low byte of a half carries the survivor HISTORY of the path that ends in that state: trellis step t gives the odd candidate bit
 //     j = (t - 1) mod 8 (folded into its branch-metric constant) and leaves it clear in the even candidate.  Bits j+1..8 are still zero in both
 //     candidates, so a metric tie is decided by bit j exactly like the reference's LSB mark decides it (even wins), bits below j are never
@@ -26,13 +29,12 @@
 //   * The kernel emits the decoded bytes (SERVICE + PSDU, still scrambled).  Descrambler, CRC-32 and the verdict (scramble.hpp:269-355,
 //     PHY_11a.hpp:609-702) run in k_sink11a, one thread per frame, after it.
 // Instruction rates that shape this (tools/microbench/pipes.cu on an H100 SXM, 400 W limit): VIADDMNMX.U16x2 + IMAD/VIADD issue together at
-// ~0.9 per cycle per sub-partition; VIMNMX + two adds (the v2 ACS) at 0.74; LOP3 and PRMT at 0.5.
+// ~0.9 per cycle per sub-partition; VIMNMX + two adds (a min-based ACS) at 0.74; LOP3 and PRMT at 0.5.
 #pragma once
 #ifndef SB_HOST_EMU
-#include "viterbi_k7_quad.cuh"
-#else        // host emulation (tests/cpp/re_emu.cpp): the decoder and k_viterbi_re only, without the work lists and the frame sink
+#include "rx11a_kernels.cuh"
+#endif       // host emulation (tests/cpp/re_emu.cpp): the decoder and k_viterbi_re only, without the work lists and the frame sink
 #include "viterbi_k7_common.cuh"
-#endif
 #include <type_traits>
 
 namespace sb {
@@ -46,13 +48,12 @@ namespace sb {
 // aligned; absent when kp = 0), then one byte per block, bit 7 = the newest column of the block.  vr_emit turns the row into output bytes.
 // Kept out of line: it runs once per `depth` steps and must not sit in the instruction stream of the step loop.
 #define SB_VR_HB 52                                          // >= (7 + 31 + 256 + 6) / 8 + 2; 13 words: rows of neighbouring lanes fall into different banks
-template <int FR>
 __device__ __noinline__ void vr_traceback(const uint8_t* __restrict__ ring_b, uint8_t* __restrict__ hb, uint32_t e, const uint32_t A0, const uint32_t t, uint32_t todo) {
     uint32_t A = A0, j = 0;
     uint32_t tt = t;                                         // time of the newest column not yet walked
     const uint32_t kp = t & 7u;
     if (kp) {                                                // running block: kp decisions in bits 0..kp-1, one slot-address bit changes per column
-        const uint32_t h = (uint32_t)ring_b[e * (FR * 64) + A];
+        const uint32_t h = (uint32_t)ring_b[e * (SB_VR_FR * 64) + A];
         const uint32_t take = min(kp, todo);
         for (uint32_t c = 0; c < take; c++) {                // column tt - c was produced at phase (tt - c - 1) mod 6: bit 5 - phase is replaced
             const uint32_t b = 5u - (tt - c - 1u) % 6u, d = (h >> (kp - 1u - c)) & 1u;
@@ -62,7 +63,7 @@ __device__ __noinline__ void vr_traceback(const uint8_t* __restrict__ ring_b, ui
         todo -= take; tt -= kp; e = e ? e - 1u : SB_VR_NB - 1u;
     }
     uint32_t ph = tt % 6u;                                   // phase of the block boundary the walk stands on
-    const uint8_t* rp = ring_b + e * (FR * 64);
+    const uint8_t* rp = ring_b + e * (SB_VR_FR * 64);
     while (todo >= 8u) {
         const uint32_t h = (uint32_t)rp[A];
         hb[j++] = (uint8_t)h;
@@ -70,7 +71,7 @@ __device__ __noinline__ void vr_traceback(const uint8_t* __restrict__ ring_b, ui
         const uint32_t G = (r & 0x3Cu) | (r >> 6);           // slot-address bit (i - ph) mod 6 <- column tt - i, the two oldest overriding i = 0, 1
         A = ((G | (G << 6)) >> ph) & 63u;
         todo -= 8u; ph = ph >= 2u ? ph - 2u : ph + 4u;       // (tt - 8) mod 6
-        rp = rp == ring_b ? ring_b + (SB_VR_NB - 1u) * (FR * 64) : rp - FR * 64;
+        rp = rp == ring_b ? ring_b + (SB_VR_NB - 1u) * (SB_VR_FR * 64) : rp - SB_VR_FR * 64;
     }
     if (todo) hb[j++] = rp[A];         // oldest block of the window: only its newest `todo` columns count
     hb[j] = 0; hb[j + 1] = 0;
@@ -92,17 +93,11 @@ __device__ __noinline__ uint32_t vr_best_slot(uint32_t r0, uint32_t r1, uint32_t
     const uint32_t R[8] = {r0, r1, r2, r3, r4, r5, r6, r7};
     return vr_best_core<2>(R, q, tm, tn, QM);
 }
-__device__ __noinline__ uint32_t vr_best_slot16(uint32_t r0, uint32_t r1, uint32_t r2, uint32_t r3, uint32_t r4, uint32_t r5, uint32_t r6, uint32_t r7,
-                                                uint32_t r8, uint32_t r9, uint32_t r10, uint32_t r11, uint32_t r12, uint32_t r13, uint32_t r14, uint32_t r15,
-                                                const uint32_t q, const uint32_t tm, const uint32_t tn, const unsigned QM) {
-    const uint32_t R[16] = {r0, r1, r2, r3, r4, r5, r6, r7, r8, r9, r10, r11, r12, r13, r14, r15};
-    return vr_best_core<1>(R, q, tm, tn, QM);
-}
 
 
-template <int CODE_RATE, int LB>
+template <int CODE_RATE>
 struct VrDecoder {
-    static constexpr int NR = 8 << (2 - LB), NL = 1 << LB, FR = 32 >> LB;                        // registers per lane, lanes per code block, code blocks per warp
+    static constexpr int NR = 8, NL = 4, FR = SB_VR_FR;                                           // registers per lane, lanes per code block, code blocks per warp
     static constexpr uint32_t GROUP = CODE_RATE == CR_12 ? 2u : CODE_RATE == CR_34 ? 4u : 3u;   // soft bytes per puncture group
     static constexpr uint32_t GSTEPS = CODE_RATE == CR_12 ? 1u : CODE_RATE == CR_34 ? 3u : 2u;  // trellis steps per group
     static constexpr uint32_t CHUNK_BYTES = 6u / GSTEPS * GROUP;                                // 12 (R=1/2), 9 (2/3), 8 (3/4) soft bytes per 6 steps
@@ -126,15 +121,12 @@ struct VrDecoder {
                // keep every puncture group inside one word: w0 = b0 b1 b2 -, w1 = b3 b4 b5 -, w2 = b6 b7 b8 -
                a[0] = b[0] | (b[1] << 8) | (b[2] << 16); a[1] = b[3] | (b[4] << 8) | (b[5] << 16); a[2] = b[6] | (b[7] << 8) | (b[8] << 16); }
     }
-    // the history bytes of this lane (low byte of every half: 16 or 32), in slot-address order, into ring entry `e`
+    // the 16 history bytes of this lane (low byte of every half), in slot-address order, into ring entry `e`
     __device__ __forceinline__ void store_hist(const uint32_t e) {
-#pragma unroll
-        for (int i = 0; i < NR / 8; i++) {
-            uint4 w;
-            w.x = __byte_perm(R[8 * i + 0], R[8 * i + 1], 0x6420); w.y = __byte_perm(R[8 * i + 2], R[8 * i + 3], 0x6420);
-            w.z = __byte_perm(R[8 * i + 4], R[8 * i + 5], 0x6420); w.w = __byte_perm(R[8 * i + 6], R[8 * i + 7], 0x6420);
-            ring_q[e * (FR * 4) + i] = w;
-        }
+        uint4 w;
+        w.x = __byte_perm(R[0], R[1], 0x6420); w.y = __byte_perm(R[2], R[3], 0x6420);
+        w.z = __byte_perm(R[4], R[5], 0x6420); w.w = __byte_perm(R[6], R[7], 0x6420);
+        ring_q[e * (FR * 4)] = w;
     }
     __device__ __forceinline__ void clear_hist() {
 #pragma unroll
@@ -144,15 +136,9 @@ struct VrDecoder {
     // viterbi.hpp:177-180 -> viterbicore.h:445-465: subtract (smallest byte & 0xFE) = the smallest m7; `mask` names the lanes that take part
     __device__ __forceinline__ void normalize(const unsigned mask) {
         uint32_t m = __vminu2(__vminu2(__vminu2(R[0], R[1]), __vminu2(R[2], R[3])), __vminu2(__vminu2(R[4], R[5]), __vminu2(R[6], R[7])));
-        if constexpr (NR >= 16) m = __vminu2(m, __vminu2(__vminu2(__vminu2(R[8], R[9]), __vminu2(R[10], R[11])), __vminu2(__vminu2(R[12], R[13]), __vminu2(R[14], R[15]))));
-        if constexpr (NR == 32) {
-            uint32_t m2 = __vminu2(__vminu2(__vminu2(R[16], R[17]), __vminu2(R[18], R[19])), __vminu2(__vminu2(R[20], R[21]), __vminu2(R[22], R[23])));
-            m2 = __vminu2(m2, __vminu2(__vminu2(__vminu2(R[24], R[25]), __vminu2(R[26], R[27])), __vminu2(__vminu2(R[28], R[29]), __vminu2(R[30], R[31]))));
-            m = __vminu2(m, m2);
-        }
         m = min(m & 0xFFFFu, m >> 16) >> 9;             // smallest m7 of this lane
-        if constexpr (LB >= 1) m = min(m, __shfl_xor_sync(mask, m, 1));
-        if constexpr (LB == 2) m = min(m, __shfl_xor_sync(mask, m, 2));
+        m = min(m, __shfl_xor_sync(mask, m, 1));
+        m = min(m, __shfl_xor_sync(mask, m, 2));
         const uint32_t mv = m * 0x02000200u;
 #pragma unroll
         for (int r = 0; r < NR; r++) R[r] -= mv;        // every half >= m << 9: no borrow between halves, histories untouched
@@ -160,7 +146,7 @@ struct VrDecoder {
     // windowed traceback from slot A0 at time t (viterbi.hpp:205-237): one lane of the quad walks the ring (vr_traceback)
     __device__ __forceinline__ void traceback(const uint32_t A0, const uint32_t t, const uint32_t la, const uint32_t nout) {
         __syncwarp(QM);
-        if (q == 0) vr_traceback<FR>(ring_b, hb, wslot, A0, t, la + nout);
+        if (q == 0) vr_traceback(ring_b, hb, wslot, A0, t, la + nout);
         __syncwarp(QM);
         vr_emit(hb, op, out_cap, nraw, nout >> 3, t & 7u, la, (uint32_t)q, (uint32_t)NL);
         nraw += nout >> 3;
@@ -173,9 +159,7 @@ struct VrDecoder {
         if (t >= end) { nout = end - ob - 6u; la = t - end; }
         else { nout = depth; la = look + (t - (ob + depth + look + 6u)) % 8u; }
         if (nout) {                                     // uniform inside the quad
-            uint32_t A0;
-            if constexpr (LB == 2) A0 = vr_best_slot(R[0], R[1], R[2], R[3], R[4], R[5], R[6], R[7], (uint32_t)q, tm, (t - 1u) & 7u, QM);
-            else A0 = vr_best_slot16(R[0], R[1], R[2], R[3], R[4], R[5], R[6], R[7], R[8], R[9], R[10], R[11], R[12], R[13], R[14], R[15], (uint32_t)q, tm, (t - 1u) & 7u, QM);
+            const uint32_t A0 = vr_best_slot(R[0], R[1], R[2], R[3], R[4], R[5], R[6], R[7], (uint32_t)q, tm, (t - 1u) & 7u, QM);
             if (t & 7u) store_hist(wslot);              // mid-block: the partial histories of the running block (a block end has just stored its own)
             traceback(A0, t, la, nout);
             ob += nout;
@@ -190,9 +174,9 @@ struct VrDecoder {
             constexpr int T = S % 6, J = S % 8, I = S / 6;
             const uint32_t cb = vr_bm<CODE_RATE, T>(w[I]);
             const uint32_t KC = kc[vr_ksum<CODE_RATE, T>() == 28u ? 0 : 1];
-            if constexpr (T < LB) vr_step<T, true, LB>(R, cb, LC, KC, mkA[T][I], mkB[T][I], 0xFFFFFFFFu);
-            else if constexpr (T <= 4) vr_step<T, true, LB>(R, cb, LC, KC, mk[J], 0u, 0xFFFFFFFFu);
-            else vr_step<T, true, LB>(R, cb, LC, KC, mkH[I], mkL[I], 0xFFFFFFFFu);
+            if constexpr (T < 2) vr_step<T, true, 2>(R, cb, LC, KC, mkA[T][I], mkB[T][I], 0xFFFFFFFFu);
+            else if constexpr (T <= 4) vr_step<T, true, 2>(R, cb, LC, KC, mk[J], 0u, 0xFFFFFFFFu);
+            else vr_step<T, true, 2>(R, cb, LC, KC, mkH[I], mkL[I], 0xFFFFFFFFu);
             if constexpr ((S + 1) % 8 == 0) {
                 store_hist(wslot); next_slot();
                 if constexpr ((S + 1) % GSTEPS == 0) normalize(0xFFFFFFFFu);
@@ -205,7 +189,7 @@ struct VrDecoder {
     template <int s> __device__ __forceinline__ void slow(const uint32_t (&w)[3], const uint32_t tb, const bool live) {
         if constexpr (s < 6) {
             const uint32_t t = tb + s + 1u;
-            vr_step_rt<s, true, LB>(R, vr_bm<CODE_RATE, s>(w), LC, kc[vr_ksum<CODE_RATE, s>() == 28u ? 0 : 1], 0x00010001u << ((t - 1u) & 7u), 0xFFFFFFFFu);
+            vr_step_rt<s, true, 2>(R, vr_bm<CODE_RATE, s>(w), LC, kc[vr_ksum<CODE_RATE, s>() == 28u ? 0 : 1], 0x00010001u << ((t - 1u) & 7u), 0xFFFFFFFFu);
             const bool blk = (t & 7u) == 0u;            // uniform over the warp
             if (blk) store_hist(wslot);
             if constexpr ((s + 1) % GSTEPS == 0) {
@@ -243,17 +227,17 @@ __global__ void k_vit_lists(const FrameInfo* __restrict__ info, uint32_t nframes
 // groups are counted on the device (cnt), so a launch of a code rate that no frame uses costs the grid, not one CTA per 8 frames.
 // Host emulation: tests/cpp/re_emu_grid.cpp defines SB_EMU_PERSISTENT and the grid intrinsics and runs the loop as the device does;
 // tests/cpp/re_emu.cpp runs one CTA per group without them (`next` null), which the device loop also does when the grid covers every group.
-template <int CODE_RATE, int LB = 2>
+template <int CODE_RATE>
 __global__ void __launch_bounds__(32) k_viterbi_re(const uint8_t* __restrict__ soft, uint64_t soft_stride, uint32_t nframes,
         const uint32_t* __restrict__ list, const uint32_t* __restrict__ cnt, const FrameInfo* __restrict__ info, VitJob job,
         uint8_t* __restrict__ out, uint64_t out_stride, uint32_t raw_off, uint32_t* __restrict__ nraw_out, uint32_t* __restrict__ next = nullptr) {
-    using D = VrDecoder<CODE_RATE, LB>;
-    constexpr int FR = D::FR, NL = D::NL;               // code blocks per warp (8 | 16), lanes per code block (4 | 2)
+    using D = VrDecoder<CODE_RATE>;
+    constexpr int FR = D::FR;
     __shared__ uint4 s_ring[SB_VR_NB][FR][4];          // entry: history bytes of the 64 slots of every code block over 8 columns
     __shared__ uint8_t s_hb[FR][SB_VR_HB];             // traceback scratch: the history bytes a walk passed, per code block
     constexpr unsigned FULL = 0xFFFFFFFFu;
     const uint32_t nvalid = list ? __ldg(cnt + CODE_RATE) : (job.code_rate == (uint32_t)CODE_RATE ? nframes : 0u);
-    const int lane = threadIdx.x & 31, q = lane & (NL - 1), fb = lane >> LB;
+    const int lane = threadIdx.x & 31, q = lane & 3, fb = lane >> 2;
     // a group ends on a full-warp vote after every lane's last shared-memory access of it, so the next group may reuse the ring at once
     for (uint32_t grp = blockIdx.x; (uint64_t)grp * FR < nvalid; ) {
         const uint32_t idx = grp * FR + fb;
@@ -264,21 +248,19 @@ __global__ void __launch_bounds__(32) k_viterbi_re(const uint8_t* __restrict__ s
         d.nsoft = job.nsoft;
         if (valid && info) { const FrameInfo fi = info[f]; L = fi.length; d.nsoft = fi.soft_bytes; }
         if (!valid) d.nsoft = 0;
-        d.q = q; d.QM = (NL == 4 ? 0xFu : NL == 2 ? 0x3u : 0x1u) << (lane & ~(NL - 1));
+        d.q = q; d.QM = 0xFu << (lane & ~3);
         d.depth = job.depth; d.look = job.lookahead;
         d.sp = soft + (size_t)f * soft_stride;
         d.op = out + (size_t)f * out_stride + raw_off;
         d.out_cap = (uint32_t)(out_stride - raw_off < 0xFFFFFFFFull ? out_stride - raw_off : 0xFFFFFFFFull);
     #pragma unroll
         for (int t = 0; t < 6; t++) {
-            const int lc = vq_cls(vq_rol6(q << (6 - LB), t) & 31);     // class contribution of this lane's address bits at phase t
+            const int lc = vq_cls(vq_rol6(q << 4, t) & 31);  // class contribution of this lane's address bits at phase t
             const int K = vr_kcls(t);
             d.LC.sel[t][0] = vq_sel(0 ^ lc, 0 ^ K ^ lc); d.LC.sel[t][1] = vq_sel(1 ^ lc, 1 ^ K ^ lc);
         }
-        if constexpr (LB >= 1) {
-            d.LC.bA[0] = (q >> (LB - 1)) & 1; d.LC.bB[0] = 1u - d.LC.bA[0]; // pair bit at T = 0 is address bit 5 (the top lane bit), at T = 1 (LB = 2) address bit 4
-            d.LC.bA[1] = q & 1;               d.LC.bB[1] = 1u - d.LC.bA[1];
-        } else { d.LC.bA[0] = d.LC.bA[1] = 0u; d.LC.bB[0] = d.LC.bB[1] = 0u; }   // one lane per code block: no lane-pair phase
+        d.LC.bA[0] = (q >> 1) & 1; d.LC.bB[0] = 1u - d.LC.bA[0];  // pair bit at T = 0 is address bit 5 (the top lane bit), at T = 1 address bit 4
+        d.LC.bA[1] = q & 1;        d.LC.bB[1] = 1u - d.LC.bA[1];
         {   // history marks as run-time values (z is always 0, which the compiler cannot know): they must stay register operands
             const uint32_t z = (uint32_t)(soft_stride >> 63);
             d.kc[0] = 0x1C001C00u + z; d.kc[1] = 0x0E000E00u + z;
@@ -298,7 +280,7 @@ __global__ void __launch_bounds__(32) k_viterbi_re(const uint8_t* __restrict__ s
         d.end = L * 8u + 16u + 6u; d.ob = 0; d.nraw = 0; d.wslot = 0; d.done = !valid;
         d.next_tb = min(d.end, d.depth + d.look + 6u);      // first time a traceback can fire (viterbi.hpp:182-203)
         uint4* const ring0 = &s_ring[0][0][0];              // this CTA's ring: [entry][code block][4 x 16 bytes]
-        d.ring_q = ring0 + fb * 4 + q * (4 / NL);     // + entry * (FR * 4): this lane's 16 / 32 / 64 bytes of the code block's 64 (LB = 0: + group * FR)
+        d.ring_q = ring0 + fb * 4 + q;                      // + entry * (FR * 4): this lane's 16 bytes of the code block's 64
         d.ring_b = (const uint8_t*)(ring0 + fb * 4);        // + entry * (FR * 64) + slot
         d.hb = s_hb[fb];
 
@@ -316,9 +298,9 @@ __global__ void __launch_bounds__(32) k_viterbi_re(const uint8_t* __restrict__ s
             uint32_t k = 0;                                 // steps into the chunk at tb
             auto step_rt = [&](const uint32_t Cbase, const uint32_t KC) {
                 const uint32_t mark = 0x00010001u << ((tb + k) & 7u);
-                switch (k) { case 0: vr_step_rt<0, false, LB>(d.R, Cbase, d.LC, KC, mark, d.QM); break; case 1: vr_step_rt<1, false, LB>(d.R, Cbase, d.LC, KC, mark, d.QM); break;
-                             case 2: vr_step_rt<2, false, LB>(d.R, Cbase, d.LC, KC, mark, d.QM); break; case 3: vr_step_rt<3, false, LB>(d.R, Cbase, d.LC, KC, mark, d.QM); break;
-                             case 4: vr_step_rt<4, false, LB>(d.R, Cbase, d.LC, KC, mark, d.QM); break; default: vr_step_rt<5, false, LB>(d.R, Cbase, d.LC, KC, mark, d.QM); }
+                switch (k) { case 0: vr_step_rt<0, false, 2>(d.R, Cbase, d.LC, KC, mark, d.QM); break; case 1: vr_step_rt<1, false, 2>(d.R, Cbase, d.LC, KC, mark, d.QM); break;
+                             case 2: vr_step_rt<2, false, 2>(d.R, Cbase, d.LC, KC, mark, d.QM); break; case 3: vr_step_rt<3, false, 2>(d.R, Cbase, d.LC, KC, mark, d.QM); break;
+                             case 4: vr_step_rt<4, false, 2>(d.R, Cbase, d.LC, KC, mark, d.QM); break; default: vr_step_rt<5, false, 2>(d.R, Cbase, d.LC, KC, mark, d.QM); }
                 k++;
                 if (((tb + k) & 7u) == 0u) d.store_hist(d.wslot);
             };

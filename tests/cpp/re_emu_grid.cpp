@@ -16,19 +16,18 @@ static inline uint32_t __shfl_sync(unsigned mask, uint32_t v, int src) { return 
 // several groups in a row, the ragged last one included.
 extern "C" int re_emu_viterbi_grid(const uint8_t* soft, uint64_t soft_stride, uint32_t nsoft, uint32_t nblocks, int code_rate, uint32_t frame_len,
                                    uint32_t depth, uint32_t lookahead, uint8_t* out, uint64_t out_stride, uint32_t* nraw,
-                                   const uint32_t* lens, const uint32_t* nsofts, int lb, uint32_t ctas) {
-    if (code_rate < 0 || code_rate > 2 || (lb != 1 && lb != 2) || ctas == 0) return -1;
+                                   const uint32_t* lens, const uint32_t* nsofts, uint32_t ctas) {
+    if (code_rate < 0 || code_rate > 2 || ctas == 0) return -1;
     std::vector<sb::FrameInfo> fi;
     if (lens && nsofts) { fi.resize(nblocks); for (uint32_t i = 0; i < nblocks; i++) { fi[i] = sb::FrameInfo{}; fi[i].length = lens[i]; fi[i].soft_bytes = nsofts[i]; fi[i].code_rate = (uint32_t)code_rate; } }
     const sb::FrameInfo* info = fi.empty() ? nullptr : fi.data();
     sb::VitJob job{}; job.code_rate = (uint32_t)code_rate; job.frame_len = frame_len; job.nsoft = nsoft; job.depth = depth; job.lookahead = lookahead; job.raw = 1;
-    const uint32_t fr = 32u >> lb, groups = (nblocks + fr - 1) / fr, grid = std::min(ctas, groups);
+    const uint32_t groups = (nblocks + SB_VR_FR - 1) / SB_VR_FR, grid = std::min(ctas, groups);
     uint32_t next = 0;
     gridDim.x = grid;
     for (uint32_t c = 0; c < grid; c++) warp_emu::run_cta(c, [&] {
-#define SB_EMU_RUN(CR, LB) sb::k_viterbi_re<CR, LB>(soft, soft_stride, nblocks, nullptr, nullptr, info, job, out, out_stride, 0u, nraw, &next)
-        if (lb == 2) { if (code_rate == sb::CR_12) SB_EMU_RUN(sb::CR_12, 2); else if (code_rate == sb::CR_23) SB_EMU_RUN(sb::CR_23, 2); else SB_EMU_RUN(sb::CR_34, 2); }
-        else         { if (code_rate == sb::CR_12) SB_EMU_RUN(sb::CR_12, 1); else if (code_rate == sb::CR_23) SB_EMU_RUN(sb::CR_23, 1); else SB_EMU_RUN(sb::CR_34, 1); }
+#define SB_EMU_RUN(CR) sb::k_viterbi_re<CR>(soft, soft_stride, nblocks, nullptr, nullptr, info, job, out, out_stride, 0u, nraw, &next)
+        if (code_rate == sb::CR_12) SB_EMU_RUN(sb::CR_12); else if (code_rate == sb::CR_23) SB_EMU_RUN(sb::CR_23); else SB_EMU_RUN(sb::CR_34);
     });
     return 0;
 }

@@ -1,6 +1,6 @@
 // Host emulation of one warp for the Viterbi kernels' device source (tests/cpp/lane_emu.cpp, tests/cpp/re_emu.cpp): the CUDA intrinsics
 // they use written out in C++, and a CTA of 32 lanes run as 32 std::threads.  Warp votes, shuffles and __syncwarp are real exchanges
-// between those threads through a std::barrier per lane group (the full warp, a lane quad, a lane pair), so a lane that leaves the
+// between those threads through a std::barrier per lane group (the full warp, a lane quad), so a lane that leaves the
 // lockstep loop on a vote, or a code block whose lanes run a divergent tail while other blocks wait at the next vote, behaves as on the GPU.
 // __shared__ arrays are function statics: one CTA runs at a time, and its 32 threads share them.
 #pragma once
@@ -51,18 +51,16 @@ struct Group {
     explicit Group(int n) : bar(n) {}
 };
 struct Cta {
-    std::unique_ptr<Group> full, quad[8], pair[16];
+    std::unique_ptr<Group> full, quad[8];
     Cta() {
         full = std::make_unique<Group>(32);
         for (auto& g : quad) g = std::make_unique<Group>(4);
-        for (auto& g : pair) g = std::make_unique<Group>(2);
     }
 };
 inline Cta*& cta() { static thread_local Cta* c = nullptr; return c; }
 inline Group* group(unsigned mask, unsigned lane) {
     if (mask == 0xFFFFFFFFu) return cta()->full.get();
     if (mask == 0xFu << (lane & ~3u)) return cta()->quad[lane >> 2].get();
-    if (mask == 0x3u << (lane & ~1u)) return cta()->pair[lane >> 1].get();
     if (mask == 1u << lane) return nullptr;                                     // a lane alone
     std::abort();                                                               // the kernels use no other mask
 }

@@ -1,6 +1,6 @@
-"""GPU parity of every Viterbi kernel (SB200_VITERBI, read when an engine is created) where code blocks of one launch end at different places in
-the trellis, and over the standalone decoder's whole envelope (pytest -m gpu).  Sorted after the per-chain suites: it creates engines under
-different SB200_VITERBI settings, as test_gpu_zz_viterbi_variants.py does.
+"""GPU parity of every Viterbi kernel (forced with the options viterbi_lane_min / viterbi_lane_max) where code blocks of one launch end at
+different places in the trellis, and over the standalone decoder's whole envelope (pytest -m gpu).  Sorted after the per-chain suites, as
+test_gpu_zz_viterbi_variants.py is.
 
   * 802.11n receive with mixed lengths in one call.  A frame's soft values are whole symbols of N_CBPS bytes; at MCS 8, 9, 11 (rate 1/2) and 13
     (rate 2/3) a symbol is not a whole number of 6-step chunks, so a frame can run out of whole chunks before its flush point while a
@@ -10,7 +10,6 @@ different SB200_VITERBI settings, as test_gpu_zz_viterbi_variants.py does.
     a trailing partial group or too few groups, wrap-inducing words, 1 to 37 blocks; staging from and to host and device memory; the
     selection of the kernel by batch size; config #5 (L = 2 500 at rate 3/4) at the batch sizes that select the lane and the four-lane kernel;
     and the arguments it refuses."""
-import os
 import numpy as np, pytest
 import oracle_py
 from sora_b200 import api, synth
@@ -18,25 +17,23 @@ from test_gpu_rx11n import _capture_11n
 
 pytestmark = pytest.mark.gpu
 
-# (SB200_VITERBI, vl_hist_block, vl_defer_walk): v3 four lanes per code block, v8 one lane (6- or 8-column history blocks, walk at the trigger
-# or spread over the step loop), v4 two lanes, v2 the quad kernel
-KERNELS = (("v3", 0, 0), ("v8", 6, 0), ("v8", 8, 0), ("v8", 8, 1), ("v4", 0, 0), ("v2", 0, 0))
-NAME = {"v3": "k_viterbi_re", "v8": "k_viterbi_lane", "v4": "k_viterbi_re", "v2": ""}
+# (kernel, vl_hist_block, vl_defer_walk): four lanes per code block, one lane (6- or 8-column history blocks, walk at the trigger or spread
+# over the step loop)
+KERNELS = (("k_viterbi_re", 0, 0), ("k_viterbi_lane", 6, 0), ("k_viterbi_lane", 8, 0), ("k_viterbi_lane", 8, 1))
 
 class _engine:
-    """An engine created under SB200_VITERBI=v, with the lane kernel's rendering options; the variable is restored on exit."""
+    """An engine that runs kernel v at every batch size, with the lane kernel's rendering options."""
     def __init__(self, v, hb=0, defer=0, mcs_limit=None):
         self.v, self.hb, self.defer, self.mcs_limit = v, hb, defer, mcs_limit
     def __enter__(self):
-        self.old = os.environ.get("SB200_VITERBI"); os.environ["SB200_VITERBI"] = self.v
         self.e = api.Engine(0)
+        if self.v == "k_viterbi_lane": self.e.set_option("viterbi_lane_min", 0); self.e.set_option("viterbi_lane_max", 0xFFFFFFFF)
+        else: self.e.set_option("viterbi_lane_min", 0xFFFFFFFF)
         if self.hb: self.e.set_option("vl_hist_block", self.hb); self.e.set_option("vl_defer_walk", self.defer)
         if self.mcs_limit: self.e.set_option("ht_mcs_limit", self.mcs_limit)
         return self.e
     def __exit__(self, *a):
         self.e.close()
-        if self.old is None: os.environ.pop("SB200_VITERBI", None)
-        else: os.environ["SB200_VITERBI"] = self.old
 
 # ---- 802.11n receive: frames that run out of whole chunks before their flush point, beside longer ones ----
 NDBPS = {8: 52, 9: 104, 10: 156, 11: 208, 12: 312, 13: 416, 14: 468}      # trellis steps per symbol, two streams
@@ -86,7 +83,7 @@ def test_rx11n_mixed_lengths_every_kernel(frames11n, v, hb, defer):
     for mcs, (iq0, iq1, off, ln, ores, oout, caps, orun) in frames11n.items():
         with _engine(v, hb, defer, 15 if mcs >= 11 else None) as e:
             res, out = e.rx11n_batch(iq0, iq1, off, ln)
-            if NAME[v]: assert e.last_viterbi_kernel() == NAME[v]
+            assert e.last_viterbi_kernel() == v
             bad = [(i, int(ores["length"][i]), hex(int(res["status"][i]))) for i in range(len(res)) if res["status"][i] != ores["status"][i]]
             assert not bad, (v, hb, defer, mcs, "frames (slot, length, status) differ from the oracle's FRAME_OK:", bad)
             for k in ("mcs", "length", "crc32", "nsym", "detect_index", "cfo_est", "lsig_length"):

@@ -1,5 +1,5 @@
 // Host-side TDownSample2 gather (sora_b200/csrc/host_gather.cpp) timed alone: T threads over 16 384 slots of 9 824 samples (643 MB read,
-// 322 MB written into a three-chunk staging ring, like the library's pinned buffers).  SB200_GATHER=pf selects the software-prefetch variant.
+// 322 MB written into a three-chunk staging ring, like the library's pinned buffers).
 //   g++ -O2 -std=c++17 -pthread -o host_gather_bench host_gather_bench.cpp ../../sora_b200/csrc/host_gather.cpp && ./host_gather_bench 14
 #include <chrono>
 #include <cstdint>
@@ -30,8 +30,7 @@ int main(int argc, char** argv) {
         const double ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t0).count();
         if (rep && ms < best) best = ms;
     }
-    const char* e = getenv("SB200_GATHER");
-    printf("host gather, %2d threads, %s: %.1f ms per 16384 slots, %.1f GB/s read + %.1f GB/s written (a 65536-slot step: %.1f ms)\n", T, e && e[0] == 'p' ? "prefetchnta" : "no software prefetch",
+    printf("host gather, %2d threads: %.1f ms per 16384 slots, %.1f GB/s read + %.1f GB/s written (a 65536-slot step: %.1f ms)\n", T,
            best, nsrc * 4 / best / 1e6, nsrc * 2 / best / 1e6, best * 4);
     return 0;
 }
