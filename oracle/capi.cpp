@@ -169,6 +169,11 @@ const int16_t* sbo_sts_pattern() { return (const int16_t*)tables().sts_pattern; 
 void sbo_tables(const uint8_t** vit_ma, const uint8_t** vit_mb, const uint8_t** demap4 /*4x256*/) {
     const Tables& T = tables(); *vit_ma = &T.vit_ma[0][0]; *vit_mb = &T.vit_mb[0][0]; *demap4 = T.demap_bpsk;
 }
+// The descrambler of Rx11a::sink_byte / Rx11n::sink_byte on decoded bytes (SERVICE + PSDU): n - 2 PSDU bytes out
+void sbo_descramble(const uint8_t* in, uint32_t n, uint8_t* out) {
+    uint8_t reg = n > 1 ? in[1] >> 1 : 0;
+    for (uint32_t i = 2; i < n; i++) { reg = tables().scramble_lut[reg]; out[i - 2] = in[i] ^ reg; reg >>= 1; }
+}
 uint64_t sbo_resample_44_40(const int16_t* in, uint64_t n_in, int16_t* out) { return resample_44_40((const c16*)in, (size_t)n_in, (c16*)out); }
 
 // ---- 802.11b ----

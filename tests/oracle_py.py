@@ -106,6 +106,12 @@ def viterbi_blocks_n(soft2d, code_rate, frame_len_bytes, depth=256, lookahead=24
                                C.c_uint32(depth), C.c_uint32(lookahead), _p(out), C.c_uint64(stride), _p(n), C.c_int(nthreads))
     return out, n
 
+def descramble(decoded):
+    """The receive chains' descrambler (oracle/rx11a.cpp sink_byte) on Viterbi output (SERVICE + PSDU): the PSDU bytes."""
+    d = np.ascontiguousarray(decoded, dtype=np.uint8); out = np.zeros(max(len(d) - 2, 0), np.uint8)
+    lib().sbo_descramble(_p(d), C.c_uint32(len(d)), _p(out))
+    return out
+
 def fft64(x):
     x = np.ascontiguousarray(x, dtype=np.int16); o = np.zeros((64, 2), np.int16); lib().sbo_fft64(_p(x), _p(o)); return o
 def ifft64(x):
@@ -248,3 +254,34 @@ def ref_fir37(chips):
     x = np.ascontiguousarray(chips, dtype=np.int8).reshape(-1, 2); out = np.zeros_like(x)
     _REF_FIR.ref_fir37(C.c_void_p(x.ctypes.data), C.c_uint(len(x)), C.c_void_p(out.ctypes.data))
     return out
+
+_REF_VIT = None
+REF_VITERBI_INSTS = {0: (48, 256, 24), 1: (312, 192, 36), 2: (48, 24, 24)}   # inst -> (N_INPUT, TRELLIS_DEPTH, TRELLIS_LOOKAHEAD)
+REF_TRELLIS_MAX = 5000 * 8
+def ref_viterbi_available():
+    return os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libviterbi_ref.so"))
+def _ref_vit():
+    global _REF_VIT
+    if _REF_VIT is None:
+        L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libviterbi_ref.so"))
+        L.ref_viterbi_sig11.restype = C.c_uint32; L.ref_viterbi_sig11.argtypes = [C.c_void_p]
+        L.ref_viterbi_block.restype = C.c_size_t
+        L.ref_viterbi_block.argtypes = [C.c_int, C.c_void_p, C.c_size_t, C.c_int, C.c_uint32, C.c_void_p]
+        L.ref_viterbi_debug.argtypes = [C.c_void_p]
+        _REF_VIT = L
+    return _REF_VIT
+def ref_viterbi_sig11(soft48):
+    """oracle/_ref/libviterbi_ref.so: the reference's own Viterbi_sig11 (viterbicore.h) on 48 soft values, >> 6 as T11aViterbiSig does."""
+    s = np.ascontiguousarray(soft48, dtype=np.uint8); assert s.shape == (48,)
+    return int(_ref_vit().ref_viterbi_sig11(s.ctypes.data))
+def ref_viterbi_block(inst, soft, code_rate, frame_len, debug=False):
+    """oracle/_ref/libviterbi_ref.so: the reference's own T11aViterbi<...>::Filter (viterbi.hpp), fresh context, fed len(soft) / N_INPUT
+    bursts.  inst picks the instantiation (REF_VITERBI_INSTS).  Returns the bytes it emitted; with debug=True also (max_min, max_any):
+    the largest unwrapped minimum Normalize subtracted and the largest unwrapped metric of any state at a normalisation (> 255: wrapped)."""
+    s = np.ascontiguousarray(soft, dtype=np.uint8).ravel()
+    out = np.zeros(frame_len + 2 + 64, np.uint8)
+    n = _ref_vit().ref_viterbi_block(inst, s.ctypes.data, len(s), code_rate, frame_len, out.ctypes.data)
+    assert n != C.c_size_t(-1).value, "nsoft must be a multiple of N_INPUT and stay within TRELLIS_MAX trellis columns"
+    if not debug: return out[:n].copy()
+    d = np.zeros(2, np.uint32); _ref_vit().ref_viterbi_debug(d.ctypes.data)
+    return out[:n].copy(), (int(d[0]), int(d[1]))

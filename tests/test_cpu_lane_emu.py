@@ -15,8 +15,8 @@ SRC = os.path.join(ROOT, "tests", "cpp", "lane_emu.cpp"); CSRC = os.path.join(RO
 CR_12, CR_23, CR_34 = 0, 1, 2
 pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="no host compiler")
 
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
+def build_emu(tmp_path_factory):
+    """Compile the emulator into a temporary directory; returns run(soft, cr, L, depth, look, lens=, nsofts=) -> (bytes, nraw)."""
     so = str(tmp_path_factory.mktemp("lane_emu") / "lane_emu.so")
     subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-shared", "-fPIC", "-DSB_HOST_EMU", "-Wno-unknown-pragmas", "-I", CSRC, "-o", so, SRC])
     lib = C.CDLL(so)
@@ -36,6 +36,10 @@ def emu(tmp_path_factory):
         assert rc == 0
         return out[:, :L + 2], nraw
     return run
+
+@pytest.fixture(scope="module")
+def emu(tmp_path_factory):
+    return build_emu(tmp_path_factory)
 
 def _coded(rng, nblocks, L, rate):
     nbits = 8 * L + 16 + 6; nbits += (-nbits) % 48

@@ -13,8 +13,8 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 SRC = os.path.join(ROOT, "tests", "cpp", "re_emu.cpp"); CSRC = os.path.join(ROOT, "sora_b200", "csrc")
 pytestmark = pytest.mark.skipif(shutil.which("g++") is None, reason="no host compiler")
 
-@pytest.fixture(scope="module")
-def emu(tmp_path_factory):
+def build_emu(tmp_path_factory):
+    """Compile the emulator into a temporary directory; returns run(soft, cr, L, depth, look, lens=, nsofts=) -> (bytes, nraw)."""
     so = str(tmp_path_factory.mktemp("re_emu") / "re_emu.so")
     subprocess.check_call(["g++", "-O1", "-std=c++20", "-pthread", "-shared", "-fPIC", "-DSB_HOST_EMU", "-Wno-unknown-pragmas", "-I", CSRC, "-o", so, SRC])
     lib = C.CDLL(so)
@@ -34,6 +34,10 @@ def emu(tmp_path_factory):
         assert rc == 0
         return out[:, :L + 2], nraw
     return run
+
+@pytest.fixture(scope="module")
+def emu(tmp_path_factory):
+    return build_emu(tmp_path_factory)
 
 def test_code_words_clean_and_noisy(emu):
     rng = np.random.default_rng(3)
