@@ -104,10 +104,11 @@ void sbo_rx11a_batch_2t(const int16_t* iq, const uint64_t* off, const uint32_t* 
 }
 
 // Stage taps of the first frame in a buffer.  Buffers sized by the caller: coeffs 64 c16 each;
-// per-symbol arrays max_sym*64 c16; soft max_sym*288 bytes.  Returns number of symbols captured (incl. SIGNAL).
-int sbo_rx11a_taps(const int16_t* iq, uint64_t nsamples, sbo_frame_result* res,
-                   int16_t* freq_coeffs, int16_t* chan_coeffs, int16_t* fft_out, int16_t* equalized, int16_t* tracked,
-                   uint8_t* soft, uint32_t* soft_off, int max_sym) {
+// per-symbol arrays max_sym*64 c16 (fft_in, may be null: what fft64 was handed, fft_out: what it returned); soft max_sym*288 bytes.
+// Returns number of symbols captured (incl. SIGNAL).
+int sbo_rx11a_taps_in(const int16_t* iq, uint64_t nsamples, sbo_frame_result* res,
+                      int16_t* freq_coeffs, int16_t* chan_coeffs, int16_t* fft_out, int16_t* equalized, int16_t* tracked,
+                      uint8_t* soft, uint32_t* soft_off, int max_sym, int16_t* fft_in) {
     Rx11a rx; rx.cca_pwr_threshold = g_cca_thr; rx.taps.enable = true;
     FrameResult r; memset(&r, 0, sizeof r);
     int n = rx.run((const c16*)iq, (size_t)nsamples, &r, nullptr, 0, 1);
@@ -116,6 +117,7 @@ int sbo_rx11a_taps(const int16_t* iq, uint64_t nsamples, sbo_frame_result* res,
     const Taps& t = rx.taps;
     if (t.freq_coeffs.size() == 64) { memcpy(freq_coeffs, t.freq_coeffs.data(), 256); memcpy(chan_coeffs, t.chan_coeffs.data(), 256); }
     int ns = (int)(t.fft_out.size() / 64); if (ns > max_sym) ns = max_sym;
+    if (fft_in) memcpy(fft_in, t.fft_in.data(), (size_t)ns * 256);
     memcpy(fft_out, t.fft_out.data(), (size_t)ns * 256); memcpy(equalized, t.equalized.data(), (size_t)ns * 256);
     memcpy(tracked, t.tracked.data(), (size_t)ns * 256);
     for (int i = 0; i < ns; i++) {
@@ -125,6 +127,12 @@ int sbo_rx11a_taps(const int16_t* iq, uint64_t nsamples, sbo_frame_result* res,
     }
     soft_off[ns] = (uint32_t)(ns < (int)t.soft_off.size() ? t.soft_off[ns] : t.soft.size());
     return ns;
+}
+// the same without the fft_in tap (the entry point's original argument list)
+int sbo_rx11a_taps(const int16_t* iq, uint64_t nsamples, sbo_frame_result* res,
+                   int16_t* freq_coeffs, int16_t* chan_coeffs, int16_t* fft_out, int16_t* equalized, int16_t* tracked,
+                   uint8_t* soft, uint32_t* soft_off, int max_sym) {
+    return sbo_rx11a_taps_in(iq, nsamples, res, freq_coeffs, chan_coeffs, fft_out, equalized, tracked, soft, soft_off, max_sym, nullptr);
 }
 
 // Standalone Viterbi block decode (BASELINE config #5): soft = nsoft coded soft values (0..7) at code_rate,
@@ -160,6 +168,9 @@ uint32_t sbo_viterbi_signal(const uint8_t* soft48) { return viterbi_signal(soft4
 
 void sbo_fft64(const int16_t* in, int16_t* out) { alignas(16) c16 t[64]; memcpy(t, in, 256); alignas(16) c16 o[64]; fft64((v128*)t, (v128*)o); memcpy(out, o, 256); }
 void sbo_ifft64(const int16_t* in, int16_t* out) { alignas(16) c16 t[64]; memcpy(t, in, 256); alignas(16) c16 o[64]; ifft64((v128*)t, (v128*)o); memcpy(out, o, 256); }
+// n vectors of 64 (128) c16 each, back to back
+void sbo_fft64_n(uint64_t n, const int16_t* in, int16_t* out) { for (uint64_t i = 0; i < n; i++) sbo_fft64(in + 128 * i, out + 128 * i); }
+void sbo_ifft64_n(uint64_t n, const int16_t* in, int16_t* out) { for (uint64_t i = 0; i < n; i++) sbo_ifft64(in + 128 * i, out + 128 * i); }
 int16_t sbo_uatan2(int y, int x) { return uatan2(y, x); }
 int16_t sbo_usin(int16_t r) { return usin(r); }
 int16_t sbo_ucos(int16_t r) { return ucos(r); }
@@ -224,10 +235,11 @@ void sbo_rx11n_batch(const int16_t* iq0, const int16_t* iq1, const uint64_t* off
     std::vector<std::thread> th; for (int t = 0; t < nthreads; t++) th.emplace_back(work);
     for (auto& t : th) t.join();
 }
-// stage taps of the first frame: siso [2][64], hinv [4][64], fft_out [2][max_sym][64] (every 64-point FFT in order: 2 L-LTF + symbols),
+// stage taps of the first frame: siso [2][64], hinv [4][64], fft_out [2][max_sym][64] (every 64-point FFT in order: 2 L-LTF + symbols) and
+// fft_in [2][max_sym][64] (may be null: what each of those FFTs was handed),
 // eq [2][max_sym][64] (data symbols), soft (stream-parsed, concatenated), theta per data symbol, sig 9 bytes.  Returns #data symbols.
-int sbo_rx11n_taps(const int16_t* iq0, const int16_t* iq1, uint64_t nsamples, void* res, int16_t* siso, int16_t* hinv, int16_t* fft_out, int16_t* eq,
-                   uint8_t* soft, uint32_t* nsoft, int16_t* theta, uint8_t* sig, int max_sym, int* nfft) {
+int sbo_rx11n_taps_in(const int16_t* iq0, const int16_t* iq1, uint64_t nsamples, void* res, int16_t* siso, int16_t* hinv, int16_t* fft_out, int16_t* eq,
+                      uint8_t* soft, uint32_t* nsoft, int16_t* theta, uint8_t* sig, int max_sym, int* nfft, int16_t* fft_in) {
     Rx11n rx; rx.taps.enable = true;
     FrameResult11n r; memset(&r, 0, sizeof r);
     int n = rx.run((const c16*)iq0, (const c16*)iq1, (size_t)nsamples, &r, nullptr, 0, 1);
@@ -238,6 +250,7 @@ int sbo_rx11n_taps(const int16_t* iq0, const int16_t* iq1, uint64_t nsamples, vo
         if (t.siso[a].size() == 64) memcpy(siso + a * 128, t.siso[a].data(), 256);
         size_t nf = t.fft_out[a].size() / 64; if (nf > (size_t)max_sym) nf = max_sym;
         memcpy(fft_out + (size_t)a * max_sym * 128, t.fft_out[a].data(), nf * 256); *nfft = (int)nf;
+        if (fft_in) memcpy(fft_in + (size_t)a * max_sym * 128, t.fft_in[a].data(), nf * 256);
         size_t ne = t.eq[a].size() / 64; if (ne > (size_t)max_sym) ne = max_sym;
         memcpy(eq + (size_t)a * max_sym * 128, t.eq[a].data(), ne * 256);
     }
@@ -246,6 +259,11 @@ int sbo_rx11n_taps(const int16_t* iq0, const int16_t* iq1, uint64_t nsamples, vo
     size_t nd = t.theta.size(); if (nd > (size_t)max_sym) nd = max_sym;
     memcpy(theta, t.theta.data(), nd * 2); memcpy(sig, t.sig, 9);
     return (int)nd;
+}
+// the same without the fft_in tap (the entry point's original argument list)
+int sbo_rx11n_taps(const int16_t* iq0, const int16_t* iq1, uint64_t nsamples, void* res, int16_t* siso, int16_t* hinv, int16_t* fft_out, int16_t* eq,
+                   uint8_t* soft, uint32_t* nsoft, int16_t* theta, uint8_t* sig, int max_sym, int* nfft) {
+    return sbo_rx11n_taps_in(iq0, iq1, nsamples, res, siso, hinv, fft_out, eq, soft, nsoft, theta, sig, max_sym, nfft, nullptr);
 }
 int16_t sbo_dsp_atan(int x, int y) { return dsp_atan(x, y); }
 void sbo_set_ht_mcs_limit(uint32_t first_refused) { set_ht_mcs_limit(first_refused); }
@@ -267,6 +285,16 @@ uint64_t sbo_tx11a_legacy_modulate(const uint8_t* mpdu, uint32_t len, int append
 }
 uint32_t sbo_tx11a_legacy_nsym(uint32_t psdu_len, uint32_t rate_kbps) { return tx11a_legacy_nsym(psdu_len, rate_kbps); }
 void sbo_ifft128(const int16_t* in, int16_t* out) { alignas(16) c16 t[128]; memcpy(t, in, 512); alignas(16) c16 o[128]; ifft128((v128*)t, (v128*)o); memcpy(out, o, 512); }
+void sbo_ifft128_n(uint64_t n, const int16_t* in, int16_t* out) { for (uint64_t i = 0; i < n; i++) sbo_ifft128(in + 256 * i, out + 256 * i); }
+// Start logging the inputs of every ifft128 on the calling thread (the transmitters run on it); sbo_ifft128_log_end stops, copies up to
+// max of them (128 c16 each) and returns how many there were; the log is kept until the next sbo_ifft128_log_begin.
+static thread_local std::vector<c16> g_ifft128_log;
+void sbo_ifft128_log_begin() { g_ifft128_log.clear(); ifft128_log = &g_ifft128_log; }
+uint64_t sbo_ifft128_log_end(int16_t* out, uint64_t max) {
+    ifft128_log = nullptr; const uint64_t n = g_ifft128_log.size() / 128;
+    if (out && max) memcpy(out, g_ifft128_log.data(), (size_t)(n < max ? n : max) * 512);
+    return n;
+}
 
 // ---- 802.11b transmit ---------------------------------------------------------------------------------------------------
 uint64_t sbo_tx11b_modulate(const uint8_t* payload, uint32_t len, uint32_t rate_kbps, uint32_t init_phase, int8_t* out, uint64_t cap_samples, uint32_t* final_phase) {

@@ -27,10 +27,10 @@ struct FrameResult {
 struct Taps {
     bool enable = false;
     std::vector<c16> freq_coeffs, chan_coeffs;      // 64 each (after LTS)
-    std::vector<c16> fft_out, equalized, tracked;    // 64 per symbol
+    std::vector<c16> fft_in, fft_out, equalized, tracked;    // 64 per symbol (fft_in: what fft64 is handed)
     std::vector<uint8_t> soft;                       // deinterleaved soft bits, N_CBPS per symbol, concatenated
     std::vector<uint32_t> soft_off;                  // offset of each symbol in `soft`
-    void clear() { freq_coeffs.clear(); chan_coeffs.clear(); fft_out.clear(); equalized.clear(); tracked.clear(); soft.clear(); soft_off.clear(); }
+    void clear() { freq_coeffs.clear(); chan_coeffs.clear(); fft_in.clear(); fft_out.clear(); equalized.clear(); tracked.clear(); soft.clear(); soft_off.clear(); }
 };
 
 class Rx11a {

@@ -208,9 +208,11 @@ void Rx11n::on_lltf() {
     }
     for (int ant = 0; ant < 2; ant++) {
         alignas(16) c16 t[64];
-        memcpy(t, x[ant], sizeof t);      fft64((v128*)t, (v128*)F); siso_est64(F, ch1);
+        memcpy(t, x[ant], sizeof t);      if (taps.enable) taps.fft_in[ant].insert(taps.fft_in[ant].end(), t, t + 64);
+        fft64((v128*)t, (v128*)F); siso_est64(F, ch1);
         if (taps.enable) taps.fft_out[ant].insert(taps.fft_out[ant].end(), F, F + 64);
-        memcpy(t, x[ant] + 64, sizeof t); fft64((v128*)t, (v128*)F); siso_est64(F, ch2);
+        memcpy(t, x[ant] + 64, sizeof t); if (taps.enable) taps.fft_in[ant].insert(taps.fft_in[ant].end(), t, t + 64);
+        fft64((v128*)t, (v128*)F); siso_est64(F, ch2);
         if (taps.enable) taps.fft_out[ant].insert(taps.fft_out[ant].end(), F, F + 64);
         for (int i = 0; i < 64; i++) { siso_ch[ant][i].re = (int16_t)(w16(ch1[i].re + ch2[i].re) >> 1); siso_ch[ant][i].im = (int16_t)(w16(ch1[i].im + ch2[i].im) >> 1); }
         if (taps.enable) taps.siso[ant].assign(siso_ch[ant], siso_ch[ant] + 64);
@@ -223,6 +225,7 @@ void Rx11n::on_symbol() {
     alignas(16) c16 Y[2][64];
     for (int ant = 0; ant < 2; ant++) {
         alignas(16) c16 t[64]; memcpy(t, sym_q[ant] + 16, sizeof t);                   // skip_cp = 16
+        if (taps.enable) taps.fft_in[ant].insert(taps.fft_in[ant].end(), t, t + 64);
         fft64((v128*)t, (v128*)Y[ant]);
         if (taps.enable) taps.fft_out[ant].insert(taps.fft_out[ant].end(), Y[ant], Y[ant] + 64);
     }

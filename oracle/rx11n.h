@@ -49,11 +49,11 @@ struct Taps11n {
     bool enable = false;
     std::vector<c16> siso[2];              // 64 each: dot11a_siso_channel_1/2
     std::vector<c16> hinv;                 // [4][64]: inv h11, h12, h21, h22
-    std::vector<c16> fft_out[2], eq[2];    // 64 per symbol per antenna/stream (data symbols only for eq)
+    std::vector<c16> fft_in[2], fft_out[2], eq[2];    // 64 per symbol per antenna/stream (data symbols only for eq; fft_in: what fft64 is handed)
     std::vector<uint8_t> soft;             // stream-parsed soft values per data symbol, concatenated
     std::vector<int16_t> theta;            // vfo_theta_i after each data symbol
     uint8_t sig[9] = {0};
-    void clear() { for (int i = 0; i < 2; i++) { siso[i].clear(); fft_out[i].clear(); eq[i].clear(); } hinv.clear(); soft.clear(); theta.clear(); }
+    void clear() { for (int i = 0; i < 2; i++) { siso[i].clear(); fft_in[i].clear(); fft_out[i].clear(); eq[i].clear(); } hinv.clear(); soft.clear(); theta.clear(); }
 };
 
 class Rx11n {

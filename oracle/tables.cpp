@@ -167,8 +167,10 @@ static inline void ifft8(v128* p) {
     a = _mm_adds_epi16(_mm_xor_si128(a, ODD32), f);
     p[0] = a; p[1] = lo;
 }
+thread_local std::vector<c16>* ifft128_log = nullptr;
 void ifft128(v128* p, v128* out) {
     const Tables& T = tables();
+    if (ifft128_log) ifft128_log->insert(ifft128_log->end(), (const c16*)p, (const c16*)p + 128);
     r4_stage<true>(p, 8, T.tw128[0], T.tw128[1], T.tw128[2]);
     for (int s = 0; s < 4; s++) {
         v128* q = p + 8 * s;

@@ -8,6 +8,7 @@
 //   soft-demap tables     kernel/bb/Brick11/src/demapper.h:56-130 (data, carried run-length coded)
 #pragma once
 #include "ops.h"
+#include <vector>
 
 namespace sbo {
 
@@ -36,5 +37,7 @@ int16_t uatan2(int y, int x);           // kernel/core/inc/intalg.h:96-108
 void fft64(v128* inout /*16 vectors, destroyed*/, v128* out);   // fft_r4dif.h:134-141 FFT<64>
 void ifft64(v128* inout, v128* out);                             // ifft_r4dif.h IFFT<64>
 void ifft128(v128* inout /*32 vectors, destroyed*/, v128* out);  // ifft_r4dif.h:12-160 IFFT<128> = IFFTSSE<128>, 4 x (IFFTSSE<32>, 4 x IFFTSSEEx<8>), 7-bit reversal
+// When set, ifft128 on this thread appends every input it is handed (128 c16 each): tests read back the symbols a transmitter transformed.
+extern thread_local std::vector<c16>* ifft128_log;
 
 } // namespace sbo

@@ -75,8 +75,9 @@ def rx11a_taps(iq, max_sym=600):
     fc = np.zeros((64, 2), np.int16); cc = np.zeros((64, 2), np.int16)
     fo = np.zeros((max_sym, 64, 2), np.int16); eq = np.zeros_like(fo); tr = np.zeros_like(fo)
     soft = np.zeros(max_sym * 288, np.uint8); so = np.zeros(max_sym + 1, np.uint32)
-    ns = lib().sbo_rx11a_taps(_p(iq), C.c_uint64(iq.shape[0]), _p(res), _p(fc), _p(cc), _p(fo), _p(eq), _p(tr), _p(soft), _p(so), C.c_int(max_sym))
-    return dict(res=res[0], freq_coeffs=fc, chan_coeffs=cc, fft_out=fo[:ns], equalized=eq[:ns], tracked=tr[:ns],
+    fi = np.zeros_like(fo)
+    ns = lib().sbo_rx11a_taps_in(_p(iq), C.c_uint64(iq.shape[0]), _p(res), _p(fc), _p(cc), _p(fo), _p(eq), _p(tr), _p(soft), _p(so), C.c_int(max_sym), _p(fi))
+    return dict(res=res[0], freq_coeffs=fc, chan_coeffs=cc, fft_in=fi[:ns], fft_out=fo[:ns], equalized=eq[:ns], tracked=tr[:ns],
                 soft=soft[:so[ns]], soft_off=so[:ns + 1], nsym=ns)
 
 def viterbi_block(soft, code_rate, frame_len_bytes, depth=256, lookahead=24):
@@ -112,10 +113,12 @@ def descramble(decoded):
     lib().sbo_descramble(_p(d), C.c_uint32(len(d)), _p(out))
     return out
 
-def fft64(x):
-    x = np.ascontiguousarray(x, dtype=np.int16); o = np.zeros((64, 2), np.int16); lib().sbo_fft64(_p(x), _p(o)); return o
-def ifft64(x):
-    x = np.ascontiguousarray(x, dtype=np.int16); o = np.zeros((64, 2), np.int16); lib().sbo_ifft64(_p(x), _p(o)); return o
+def _xform(fn, x, N):
+    """x: int16 [..., N, 2], any number of leading axes; one transform per vector, same shape out."""
+    x = np.ascontiguousarray(x, dtype=np.int16); assert x.shape[-2:] == (N, 2), x.shape
+    o = np.zeros_like(x); fn(C.c_uint64(x.size // (2 * N)), _p(x), _p(o)); return o
+def fft64(x): return _xform(lib().sbo_fft64_n, x, 64)
+def ifft64(x): return _xform(lib().sbo_ifft64_n, x, 64)
 def crc32(b):
     b = np.ascontiguousarray(b, dtype=np.uint8); return int(lib().sbo_crc32(_p(b), C.c_uint64(len(b))))
 
@@ -164,11 +167,11 @@ def rx11n_taps(iq0, iq1, max_sym=300):
     iq0 = np.ascontiguousarray(iq0, dtype=np.int16); iq1 = np.ascontiguousarray(iq1, dtype=np.int16)
     res = np.zeros(1, dtype=RES11N_DTYPE)
     siso = np.zeros((2, 64, 2), np.int16); hinv = np.zeros((4, 64, 2), np.int16)
-    fo = np.zeros((2, max_sym, 64, 2), np.int16); eq = np.zeros((2, max_sym, 64, 2), np.int16)
+    fo = np.zeros((2, max_sym, 64, 2), np.int16); eq = np.zeros((2, max_sym, 64, 2), np.int16); fi = np.zeros_like(fo)
     soft = np.zeros(max_sym * 624, np.uint8); nsoft = C.c_uint32(0); theta = np.zeros(max_sym, np.int16); sig = np.zeros(9, np.uint8); nfft = C.c_int(0)
-    nd = lib().sbo_rx11n_taps(_p(iq0), _p(iq1), C.c_uint64(iq0.reshape(-1, 2).shape[0]), _p(res), _p(siso), _p(hinv), _p(fo), _p(eq), _p(soft),
-                              C.byref(nsoft), _p(theta), _p(sig), C.c_int(max_sym), C.byref(nfft))
-    return dict(res=res[0], siso=siso, hinv=hinv, fft_out=fo[:, :nfft.value], eq=eq[:, :nd], soft=soft[:nsoft.value], theta=theta[:nd], sig=sig, ndata=nd)
+    nd = lib().sbo_rx11n_taps_in(_p(iq0), _p(iq1), C.c_uint64(iq0.reshape(-1, 2).shape[0]), _p(res), _p(siso), _p(hinv), _p(fo), _p(eq), _p(soft),
+                              C.byref(nsoft), _p(theta), _p(sig), C.c_int(max_sym), C.byref(nfft), _p(fi))
+    return dict(res=res[0], siso=siso, hinv=hinv, fft_in=fi[:, :nfft.value], fft_out=fo[:, :nfft.value], eq=eq[:, :nd], soft=soft[:nsoft.value], theta=theta[:nd], sig=sig, ndata=nd)
 
 def tables11n():
     sc = np.zeros((65536, 2), np.int16); at = np.zeros(4097, np.int16); dm = np.zeros(256, np.uint8); c8 = np.zeros(256, np.uint8)
@@ -203,8 +206,14 @@ def tx11a_legacy_modulate(body, rate_kbps, append_crc=True):
     assert n == cap, (n, cap)
     return out
 
-def ifft128(x):
-    x = np.ascontiguousarray(x, dtype=np.int16); o = np.zeros((128, 2), np.int16); lib().sbo_ifft128(_p(x), _p(o)); return o
+def ifft128(x): return _xform(lib().sbo_ifft128_n, x, 128)
+def ifft128_inputs(fn, *args, **kw):
+    """Run fn(*args, **kw) (an oracle transmitter) and return (its result, int16 [n, 128, 2]: the input of every ifft128 it made, in order)."""
+    L = lib(); L.sbo_ifft128_log_end.restype = C.c_uint64; L.sbo_ifft128_log_begin()
+    try: r = fn(*args, **kw)
+    finally: n = L.sbo_ifft128_log_end(None, C.c_uint64(0))
+    x = np.zeros((n, 128, 2), np.int16); L.sbo_ifft128_log_end(_p(x), C.c_uint64(n))   # the log stays until the next _begin
+    return r, x
 
 
 # ---- 802.11b transmit (brick modulator restatement) ---------------------------------------------------------------------
@@ -285,3 +294,33 @@ def ref_viterbi_block(inst, soft, code_rate, frame_len, debug=False):
     if not debug: return out[:n].copy()
     d = np.zeros(2, np.uint32); _ref_vit().ref_viterbi_debug(d.ctypes.data)
     return out[:n].copy(), (int(d[0]), int(d[1]))
+
+_REF_FFT = None
+REF_FFT_COUNTERS = ("sat_add", "sat_sub", "pack", "madd")   # the order of ref_fft_debug's counts
+def ref_fft_available():
+    return os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libfft_ref.so"))
+def _ref_fft():
+    global _REF_FFT
+    if _REF_FFT is None:
+        L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libfft_ref.so"))
+        for f in (L.ref_fft64, L.ref_ifft64, L.ref_ifft128): f.argtypes = [C.c_size_t, C.c_void_p, C.c_void_p]; f.restype = None
+        L.ref_fft_debug.argtypes = [C.c_void_p]; L.ref_fft_debug.restype = None
+        _REF_FFT = L
+    return _REF_FFT
+def _ref_xform(fn, x, N):
+    x = np.ascontiguousarray(x, dtype=np.int16); assert x.shape[-2:] == (N, 2), x.shape
+    o = np.zeros_like(x); fn(x.size // (2 * N), x.ctypes.data, o.ctypes.data); return o
+def ref_fft64(x):
+    """oracle/_ref/libfft_ref.so: the reference's own FFTSafe<64> (fft_r4dif.h) on int16 [..., 64, 2], one transform per vector."""
+    return _ref_xform(_ref_fft().ref_fft64, x, 64)
+def ref_ifft64(x):
+    """The reference's own IFFTSafe<64> (ifft_r4dif.h) on int16 [..., 64, 2]."""
+    return _ref_xform(_ref_fft().ref_ifft64, x, 64)
+def ref_ifft128(x):
+    """The reference's own IFFTSafe<128> (ifft_r4dif.h) on int16 [..., 128, 2]."""
+    return _ref_xform(_ref_fft().ref_ifft128, x, 128)
+def ref_fft_debug():
+    """What the tap counted over the last ref_fft64 / ref_ifft64 / ref_ifft128 call of this thread, as {name: lanes} (REF_FFT_COUNTERS):
+    saturated_add / saturated_sub lanes that clipped, pack lanes whose 32-bit value did not fit int16, pmaddwd lanes that wrapped."""
+    d = np.zeros(4, np.uint64); _ref_fft().ref_fft_debug(d.ctypes.data)
+    return dict(zip(REF_FFT_COUNTERS, (int(v) for v in d)))
