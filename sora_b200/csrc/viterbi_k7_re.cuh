@@ -28,8 +28,9 @@
 //     traceback trigger run as one branch-free instruction stream, everything else goes through a 6-step path with the event checks.
 //   * The kernel emits the decoded bytes (SERVICE + PSDU, still scrambled).  Descrambler, CRC-32 and the verdict (scramble.hpp:269-355,
 //     PHY_11a.hpp:609-702) run in k_sink11a, one thread per frame, after it.
-// Instruction rates that shape this (tools/microbench/pipes.cu on an H100 SXM, 400 W limit): VIADDMNMX.U16x2 + IMAD/VIADD issue together at
-// ~0.9 per cycle per sub-partition; VIMNMX + two adds (a min-based ACS) at 0.74; LOP3 and PRMT at 0.5.
+// Instruction rates that shape this (tools/microbench/pipes2.cu on an H100 SXM, DESIGN §4): VIADDMNMX.U16x2, PRMT, LOP3 and IADD3 issue on the
+// ALU pipe, VIADD.16x2, IMAD, IDP.4A and the scalar VIADD on the FMA pipe, each at one warp-instruction per two cycles per sub-partition, and
+// VIADDMNMX takes half an FMA slot as well; so the step constants are built mostly on the ALU pipe (vr_step_pk).
 #pragma once
 #ifndef SB_HOST_EMU
 #include "rx11a_kernels.cuh"
@@ -104,7 +105,7 @@ struct VrDecoder {
     uint32_t R[NR];
     VrLane LC;
     uint32_t kc[2];        // 28 << 8 and 14 << 8 in both halves, as registers
-    uint32_t mk[8], mkA[2][4], mkB[2][4], mkH[4], mkL[4];   // history marks 0x00010001 << j as registers; per lane-pair phase and chunk; T = 5 halves
+    uint32_t mk[8], mkA[2][4], mkB[2][4], mkH[4], mkL[4];   // history marks 0x00010001 << j as registers; per lane-pair phase and chunk; T = 5 (vr_step_pk)
     unsigned QM; int q;
     uint4* ring_q; const uint8_t* ring_b; uint8_t* hb;   // hb: the quad's traceback scratch row (SB_VR_HB bytes of shared memory)
     const uint8_t* sp; uint8_t* op; uint32_t out_cap, nsoft;
@@ -172,11 +173,10 @@ struct VrDecoder {
     template <int S> __device__ __forceinline__ void fast(const uint32_t (&w)[4][3]) {
         if constexpr (S < 24) {
             constexpr int T = S % 6, J = S % 8, I = S / 6;
-            const uint32_t cb = vr_bm<CODE_RATE, T>(w[I]);
-            const uint32_t KC = kc[vr_ksum<CODE_RATE, T>() == 28u ? 0 : 1];
-            if constexpr (T < 2) vr_step<T, true, 2>(R, cb, LC, KC, mkA[T][I], mkB[T][I], 0xFFFFFFFFu);
-            else if constexpr (T <= 4) vr_step<T, true, 2>(R, cb, LC, KC, mk[J], 0u, 0xFFFFFFFFu);
-            else vr_step<T, true, 2>(R, cb, LC, KC, mkH[I], mkL[I], 0xFFFFFFFFu);
+            const uint32_t cb = vr_bm_pk<CODE_RATE, T>(w[I]);
+            if constexpr (T < 2) vr_step_pk<T, true>(R, cb, LC, mkA[T][I], mkB[T][I], 0xFFFFFFFFu);
+            else if constexpr (T <= 4) vr_step_pk<T, true>(R, cb, LC, 0u, mk[J], 0xFFFFFFFFu);
+            else vr_step_pk<T, true>(R, cb, LC, mkH[I], mkL[I], 0xFFFFFFFFu);
             if constexpr ((S + 1) % 8 == 0) {
                 store_hist(wslot); next_slot();
                 if constexpr ((S + 1) % GSTEPS == 0) normalize(0xFFFFFFFFu);
@@ -189,7 +189,7 @@ struct VrDecoder {
     template <int s> __device__ __forceinline__ void slow(const uint32_t (&w)[3], const uint32_t tb, const bool live) {
         if constexpr (s < 6) {
             const uint32_t t = tb + s + 1u;
-            vr_step_rt<s, true, 2>(R, vr_bm<CODE_RATE, s>(w), LC, kc[vr_ksum<CODE_RATE, s>() == 28u ? 0 : 1], 0x00010001u << ((t - 1u) & 7u), 0xFFFFFFFFu);
+            vr_step_rt<s, true, 2>(R, vr_bm_pk<CODE_RATE, s>(w), LC, kc[vr_ksum<CODE_RATE, s>() == 28u ? 0 : 1], 0x00010001u << ((t - 1u) & 7u), 0xFFFFFFFFu);
             const bool blk = (t & 7u) == 0u;            // uniform over the warp
             if (blk) store_hist(wslot);
             if constexpr ((s + 1) % GSTEPS == 0) {
@@ -257,7 +257,8 @@ __global__ void __launch_bounds__(32) k_viterbi_re(const uint8_t* __restrict__ s
         for (int t = 0; t < 6; t++) {
             const int lc = vq_cls(vq_rol6(q << 4, t) & 31);  // class contribution of this lane's address bits at phase t
             const int K = vr_kcls(t);
-            d.LC.sel[t][0] = vq_sel(0 ^ lc, 0 ^ K ^ lc); d.LC.sel[t][1] = vq_sel(1 ^ lc, 1 ^ K ^ lc);
+#pragma unroll
+            for (int c = 0; c < 4; c++) d.LC.sel[t][c] = vq_sel(vr_bmbyte(CODE_RATE, t, c ^ lc), vr_bmbyte(CODE_RATE, t, c ^ K ^ lc));
         }
         d.LC.bA[0] = (q >> 1) & 1; d.LC.bB[0] = 1u - d.LC.bA[0];  // pair bit at T = 0 is address bit 5 (the top lane bit), at T = 1 address bit 4
         d.LC.bA[1] = q & 1;        d.LC.bB[1] = 1u - d.LC.bA[1];
@@ -270,7 +271,7 @@ __global__ void __launch_bounds__(32) k_viterbi_re(const uint8_t* __restrict__ s
             for (int i = 0; i < 4; i++) {                   // chunk i of a 24-step stretch: its steps 0, 1, 5 are steps 6i, 6i+1, 6i+5
                 d.mkA[0][i] = d.LC.bA[0] * d.mk[(6 * i) % 8];     d.mkB[0][i] = d.LC.bB[0] * d.mk[(6 * i) % 8];
                 d.mkA[1][i] = d.LC.bA[1] * d.mk[(6 * i + 1) % 8]; d.mkB[1][i] = d.LC.bB[1] * d.mk[(6 * i + 1) % 8];
-                d.mkH[i] = d.mk[(6 * i + 5) % 8] & 0xFFFF0000u;   d.mkL[i] = d.mk[(6 * i + 5) % 8] & 0x0000FFFFu;
+                d.mkH[i] = d.mk[(6 * i + 5) % 8] & 0xFFFF0000u;   d.mkL[i] = (d.mk[(6 * i + 5) % 8] & 0x0000FFFFu) - d.mkH[i];   // vr_step_pk: Q = P + mkL
             }
         }
         // initial metrics (viterbilut.h:22-32): state 0 -> 0x00, others 0x30; at t=0 state == address; byte value v sits at v << 8
@@ -311,8 +312,8 @@ __global__ void __launch_bounds__(32) k_viterbi_re(const uint8_t* __restrict__ s
                 if (D::GROUP > 3) g |= (uint32_t)__ldg(d.sp + pos + 3) << 24;
                 pos += D::GROUP;
                 step_rt(vq_bm_ab<0>(g), d.kc[0]);
-                if (D::GSTEPS >= 2) { block_end(); step_rt(vq_bm_a<2>(g), d.kc[1]); }
-                if (D::GSTEPS >= 3) { block_end(); step_rt(vq_bm_b<3>(g), d.kc[1]); }
+                if (D::GSTEPS >= 2) { block_end(); step_rt(D::GSTEPS == 3 ? vq_bm_a2b3(g) : vq_bm_a<2>(g), d.kc[1]); }
+                if (D::GSTEPS >= 3) { block_end(); step_rt(vq_bm_a2b3(g), d.kc[1]); }
                 const uint32_t t = tb + k;
                 if ((t & 7u) == 0u) d.normalize(d.QM);
                 d.trigger(t, k == 6 ? 0u : k);
