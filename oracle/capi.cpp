@@ -104,11 +104,12 @@ void sbo_rx11a_batch_2t(const int16_t* iq, const uint64_t* off, const uint32_t* 
 }
 
 // Stage taps of the first frame in a buffer.  Buffers sized by the caller: coeffs 64 c16 each;
-// per-symbol arrays max_sym*64 c16 (fft_in, may be null: what fft64 was handed, fft_out: what it returned); soft max_sym*288 bytes.
+// per-symbol arrays max_sym*64 c16 (fft_in, may be null: what fft64 was handed, fft_out: what it returned); soft max_sym*288 bytes;
+// lts_in (may be null) 144 c16: the block T11aLTS is handed; sym_in (may be null) max_sym*80 c16: the blocks T11aDataSymbol is handed.
 // Returns number of symbols captured (incl. SIGNAL).
-int sbo_rx11a_taps_in(const int16_t* iq, uint64_t nsamples, sbo_frame_result* res,
-                      int16_t* freq_coeffs, int16_t* chan_coeffs, int16_t* fft_out, int16_t* equalized, int16_t* tracked,
-                      uint8_t* soft, uint32_t* soft_off, int max_sym, int16_t* fft_in) {
+int sbo_rx11a_taps_blocks(const int16_t* iq, uint64_t nsamples, sbo_frame_result* res,
+                          int16_t* freq_coeffs, int16_t* chan_coeffs, int16_t* fft_out, int16_t* equalized, int16_t* tracked,
+                          uint8_t* soft, uint32_t* soft_off, int max_sym, int16_t* fft_in, int16_t* lts_in, int16_t* sym_in) {
     Rx11a rx; rx.cca_pwr_threshold = g_cca_thr; rx.taps.enable = true;
     FrameResult r; memset(&r, 0, sizeof r);
     int n = rx.run((const c16*)iq, (size_t)nsamples, &r, nullptr, 0, 1);
@@ -118,6 +119,8 @@ int sbo_rx11a_taps_in(const int16_t* iq, uint64_t nsamples, sbo_frame_result* re
     if (t.freq_coeffs.size() == 64) { memcpy(freq_coeffs, t.freq_coeffs.data(), 256); memcpy(chan_coeffs, t.chan_coeffs.data(), 256); }
     int ns = (int)(t.fft_out.size() / 64); if (ns > max_sym) ns = max_sym;
     if (fft_in) memcpy(fft_in, t.fft_in.data(), (size_t)ns * 256);
+    if (lts_in && t.lts_in.size() == 144) memcpy(lts_in, t.lts_in.data(), 144 * 4);
+    if (sym_in) memcpy(sym_in, t.sym_in.data(), (size_t)ns * 320);
     memcpy(fft_out, t.fft_out.data(), (size_t)ns * 256); memcpy(equalized, t.equalized.data(), (size_t)ns * 256);
     memcpy(tracked, t.tracked.data(), (size_t)ns * 256);
     for (int i = 0; i < ns; i++) {
@@ -127,6 +130,27 @@ int sbo_rx11a_taps_in(const int16_t* iq, uint64_t nsamples, sbo_frame_result* re
     }
     soft_off[ns] = (uint32_t)(ns < (int)t.soft_off.size() ? t.soft_off[ns] : t.soft.size());
     return ns;
+}
+// The carrier-sense trace up to the first frame event: per 20 Msps vector handed to cca_process, 13 int32 after it (cca_state,
+// error_code, DC as 8 int16 lanes, cca_peak_index, cca_pwr_reading, the vector's 20 Msps index).  Returns the number of vectors
+// (at most max_vec); *detect = detect_index of the first detection, or -1.
+uint64_t sbo_rx11a_cs_trace(const int16_t* iq, uint64_t nsamples, int32_t* rec, uint64_t max_vec, int64_t* detect) {
+    Rx11a rx; rx.cca_pwr_threshold = g_cca_thr; rx.taps.enable = true;
+    FrameResult r; memset(&r, 0, sizeof r);
+    int n = rx.run((const c16*)iq, (size_t)nsamples, &r, nullptr, 0, 1);
+    const std::vector<int32_t>& t = rx.taps.cs;
+    size_t m = t.size() / 13; if (m > max_vec) m = max_vec;
+    memcpy(rec, t.data(), m * 13 * sizeof(int32_t));
+    bool det = n > 0 || (!t.empty() && t[t.size() - 13] == 1);
+    *detect = det ? (int64_t)t[t.size() - 1] + 1 : -1;
+    return m;
+}
+// the same without the LTS and symbol-block taps
+int sbo_rx11a_taps_in(const int16_t* iq, uint64_t nsamples, sbo_frame_result* res,
+                      int16_t* freq_coeffs, int16_t* chan_coeffs, int16_t* fft_out, int16_t* equalized, int16_t* tracked,
+                      uint8_t* soft, uint32_t* soft_off, int max_sym, int16_t* fft_in) {
+    return sbo_rx11a_taps_blocks(iq, nsamples, res, freq_coeffs, chan_coeffs, fft_out, equalized, tracked, soft, soft_off, max_sym, fft_in,
+                                 nullptr, nullptr);
 }
 // the same without the fft_in tap (the entry point's original argument list)
 int sbo_rx11a_taps(const int16_t* iq, uint64_t nsamples, sbo_frame_result* res,

@@ -28,9 +28,11 @@ struct Taps {
     bool enable = false;
     std::vector<c16> freq_coeffs, chan_coeffs;      // 64 each (after LTS)
     std::vector<c16> fft_in, fft_out, equalized, tracked;    // 64 per symbol (fft_in: what fft64 is handed)
+    std::vector<c16> lts_in, sym_in;                 // what on_lts (144) and on_symbol (80 per symbol) are handed
+    std::vector<int32_t> cs;                         // per vector cca_process is handed, 13 values after it (see sbo_rx11a_cs_trace)
     std::vector<uint8_t> soft;                       // deinterleaved soft bits, N_CBPS per symbol, concatenated
     std::vector<uint32_t> soft_off;                  // offset of each symbol in `soft`
-    void clear() { freq_coeffs.clear(); chan_coeffs.clear(); fft_in.clear(); fft_out.clear(); equalized.clear(); tracked.clear(); soft.clear(); soft_off.clear(); }
+    void clear() { freq_coeffs.clear(); chan_coeffs.clear(); fft_in.clear(); fft_out.clear(); lts_in.clear(); sym_in.clear(); cs.clear(); equalized.clear(); tracked.clear(); soft.clear(); soft_off.clear(); }
 };
 
 class Rx11a {

@@ -75,10 +75,11 @@ def rx11a_taps(iq, max_sym=600):
     fc = np.zeros((64, 2), np.int16); cc = np.zeros((64, 2), np.int16)
     fo = np.zeros((max_sym, 64, 2), np.int16); eq = np.zeros_like(fo); tr = np.zeros_like(fo)
     soft = np.zeros(max_sym * 288, np.uint8); so = np.zeros(max_sym + 1, np.uint32)
-    fi = np.zeros_like(fo)
-    ns = lib().sbo_rx11a_taps_in(_p(iq), C.c_uint64(iq.shape[0]), _p(res), _p(fc), _p(cc), _p(fo), _p(eq), _p(tr), _p(soft), _p(so), C.c_int(max_sym), _p(fi))
+    fi = np.zeros_like(fo); li = np.zeros((144, 2), np.int16); si = np.zeros((max_sym, 80, 2), np.int16)
+    ns = lib().sbo_rx11a_taps_blocks(_p(iq), C.c_uint64(iq.shape[0]), _p(res), _p(fc), _p(cc), _p(fo), _p(eq), _p(tr), _p(soft), _p(so),
+                                     C.c_int(max_sym), _p(fi), _p(li), _p(si))
     return dict(res=res[0], freq_coeffs=fc, chan_coeffs=cc, fft_in=fi[:ns], fft_out=fo[:ns], equalized=eq[:ns], tracked=tr[:ns],
-                soft=soft[:so[ns]], soft_off=so[:ns + 1], nsym=ns)
+                soft=soft[:so[ns]], soft_off=so[:ns + 1], nsym=ns, lts_in=li, sym_in=si[:ns])
 
 def viterbi_block(soft, code_rate, frame_len_bytes, depth=256, lookahead=24):
     soft = np.ascontiguousarray(soft, dtype=np.uint8)
@@ -324,3 +325,65 @@ def ref_fft_debug():
     saturated_add / saturated_sub lanes that clipped, pack lanes whose 32-bit value did not fit int16, pmaddwd lanes that wrapped."""
     d = np.zeros(4, np.uint64); _ref_fft().ref_fft_debug(d.ctypes.data)
     return dict(zip(REF_FFT_COUNTERS, (int(v) for v in d)))
+
+# ---- oracle/_ref/librx11a_ref.so: the reference's own 802.11a front-end bricks (oracle/build_ref_rx11a.sh) ----
+_REF_RX = None
+REF_RX11A_COUNTERS = ("lts_e0", "lts_pack", "eq_pack", "mul_pack", "demap_clamp", "madd")   # the order of ref_rx11a_debug's counts
+def ref_rx11a_available():
+    return os.path.exists(os.path.join(ROOT, "oracle", "_ref", "librx11a_ref.so"))
+def _ref_rx():
+    global _REF_RX
+    if _REF_RX is None:
+        L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "librx11a_ref.so"))
+        L.ref_rx11a_lts.argtypes = [C.c_void_p] * 4; L.ref_rx11a_lts.restype = None
+        L.ref_rx11a_symbols.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_uint] + [C.c_void_p] * 11; L.ref_rx11a_symbols.restype = C.c_int
+        L.ref_resample_44_40.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p]; L.ref_resample_44_40.restype = C.c_size_t
+        L.ref_rx11a_debug.argtypes = [C.c_void_p]; L.ref_rx11a_debug.restype = None
+        _REF_RX = L
+    return _REF_RX
+def ref_rx11a_lts(lts144):
+    """T11aLTS (channel_11a.hpp) on the 144 samples int16 [144, 2] it is handed, fresh context: (CFO_est, FreqCoeffs, ChannelCoeffs)."""
+    x = np.ascontiguousarray(lts144, np.int16).reshape(144, 2)
+    cfo = np.zeros(1, np.int16); fc = np.zeros((64, 2), np.int16); cc = np.zeros((64, 2), np.int16)
+    _ref_rx().ref_rx11a_lts(_p(x), _p(cfo), _p(fc), _p(cc))
+    return int(cfo[0]), fc, cc
+def ref_rx11a_symbols(lts144, sym80, rate_kbps):
+    """T11aLTS on lts144, then the 80-sample blocks sym80 int16 [n, 80, 2] through the reference's own per-symbol bricks; symbol 0 is
+    SIGNAL.  Returns a dict of every intermediate (see ref_rx11a_symbols in oracle/build_ref_rx11a.sh); soft and demapped are cut to
+    N_CBPS per symbol."""
+    x = np.ascontiguousarray(lts144, np.int16).reshape(144, 2); s = np.ascontiguousarray(sym80, np.int16).reshape(-1, 80, 2); n = len(s)
+    cfo = np.zeros(1, np.int16); fc = np.zeros((64, 2), np.int16); cc = np.zeros((64, 2), np.int16)
+    v = {k: np.zeros((n, 64, 2), np.int16) for k in ("fft_in", "fft_out", "equalized", "phase_comp", "tracked")}
+    dm = np.zeros((n, 288), np.uint8); so = np.zeros((n, 288), np.uint8); st = np.zeros((n, 5), np.int32)
+    rc = _ref_rx().ref_rx11a_symbols(_p(x), n, _p(s), rate_kbps, _p(cfo), _p(fc), _p(cc), _p(v["fft_in"]), _p(v["fft_out"]),
+                                     _p(v["equalized"]), _p(v["phase_comp"]), _p(v["tracked"]), _p(dm), _p(so), _p(st))
+    assert rc == 0, rate_kbps
+    nb = {6000: 1, 9000: 1, 12000: 2, 18000: 2, 24000: 4, 36000: 4, 48000: 6, 54000: 6}[rate_kbps]
+    ncb = [48] + [48 * nb] * (n - 1)
+    v.update(cfo_est=int(cfo[0]), freq_coeffs=fc, chan_coeffs=cc, state=st, ncbps=ncb,
+             demapped=[dm[i, :ncb[i]] for i in range(n)], soft=[so[i, :ncb[i]] for i in range(n)])
+    return v
+def ref_rx11a_debug():
+    """What the tap counted over the last ref_rx11a_lts / ref_rx11a_symbols call of this thread, as {name: lanes} (REF_RX11A_COUNTERS)."""
+    d = np.zeros(6, np.uint64); _ref_rx().ref_rx11a_debug(d.ctypes.data)
+    return dict(zip(REF_RX11A_COUNTERS, (int(v) for v in d)))
+def ref_resample_44_40(iq44):
+    """TDownSample44_40 / Down44to40 (sampling.hpp, 44MTo40M.hpp) over int16 [n, 2] fed in 28-sample blocks: the 40 Msps samples it emits."""
+    x = np.ascontiguousarray(iq44, np.int16).reshape(-1, 2); out = np.zeros_like(x)
+    m = _ref_rx().ref_resample_44_40(_p(x), len(x), _p(out))
+    return out[:m]
+CS_FIELDS = ("cca_state", "error_code", "dc", "cca_peak_index", "cca_pwr_reading", "vec20")   # a carrier-sense record: 13 int32
+def rx11a_cs_trace(iq, max_vec=1 << 20):
+    """The oracle's carrier sense up to the first frame event: (records int32 [n, 13], index of the first vector past the detection or -1)."""
+    iq = np.ascontiguousarray(iq, np.int16); rec = np.zeros((max_vec, 13), np.int32); det = np.zeros(1, np.int64)
+    L = lib(); L.sbo_rx11a_cs_trace.restype = C.c_uint64
+    n = L.sbo_rx11a_cs_trace(_p(iq), C.c_uint64(iq.shape[0]), _p(rec), C.c_uint64(max_vec), _p(det))
+    return rec[:n], int(det[0])
+def ref_rx11a_carrier_sense(iq, cca_pwr_threshold=1000 * 1000, max_vec=1 << 20):
+    """TDownSample2 -> TDCRemoveEx<4> -> TCCA11a -> TDCEstimator of the reference (oracle/build_ref_rx11a.sh) over 40 Msps int16 [n, 2]:
+    the same records as rx11a_cs_trace, and the detection index."""
+    iq = np.ascontiguousarray(iq, np.int16); rec = np.zeros((max_vec, 13), np.int32); det = np.zeros(1, np.int64)
+    L = _ref_rx(); L.ref_rx11a_carrier_sense.restype = C.c_size_t
+    L.ref_rx11a_carrier_sense.argtypes = [C.c_void_p, C.c_size_t, C.c_uint, C.c_void_p, C.c_size_t, C.c_void_p]
+    n = L.ref_rx11a_carrier_sense(_p(iq), len(iq), cca_pwr_threshold, _p(rec), max_vec, _p(det))
+    return rec[:n], int(det[0])
