@@ -334,6 +334,30 @@ uint64_t sbo_tx11n_modulate(const uint8_t* payload, uint32_t len, uint32_t mcs, 
 uint32_t sbo_tx11n_nsym(uint32_t len, uint32_t mcs, uint32_t* signalled) { return tx11n_nsym(len, mcs, signalled); }
 void sbo_tx11n_preamble_tables(int16_t* lstf, int16_t* lltf, int16_t* htstf, int16_t* htltf) { tx11n_preamble_tables((c16*)lstf, (c16*)lltf, (c16*)htstf, (c16*)htltf); }
 
+// ---- the header parsers and the back end on their own ---------------------------------------------------------------------
+// T11aPLCPParser on each of n SIGNAL words, each from a context just Reset: 6 uint32 per word (Rx11a::plcp_parse_only)
+void sbo_plcp11a_parse(const uint32_t* words, uint64_t n, uint32_t* out) {
+    Rx11a* rx = new Rx11a();
+    for (uint64_t i = 0; i < n; i++) rx->plcp_parse_only(words[i], out + 6 * i);
+    delete rx;
+}
+// T11nSigParser on n blocks of 9 bytes in turn, one context: 8 uint32 per block (Rx11n::sig_parse_only); CF_HTRxVector starts at 0
+void sbo_sig11n_parse(const uint8_t* sig9, uint64_t n, uint32_t* out) {
+    Rx11n* rx = new Rx11n();
+    for (uint64_t i = 0; i < n; i++) rx->sig_parse_only(sig9 + 9 * i, out + 8 * i);
+    delete rx;
+}
+// T11aDesc -> TBB11aFrameSink as the 802.11a (chain 0) or the 802.11n (chain 1) receiver runs them, fed n decoded bytes for a frame of
+// frame_length bytes: returns the error code, *crc32 = CF_11aRxVector::crc32, out = the frame buffer's first frame_length bytes
+uint32_t sbo_desc_sink(int chain, const uint8_t* in, uint64_t n, uint16_t frame_length, uint8_t* out, uint32_t* crc32) {
+    uint32_t e;
+    if (chain == 0) { Rx11a* rx = new Rx11a(); e = rx->desc_sink_only(in, (size_t)n, frame_length); *crc32 = rx->back_crc32();
+                      memcpy(out, rx->frame_bytes(), frame_length < 4096 ? frame_length : 4096); delete rx; }
+    else { Rx11n* rx = new Rx11n(); e = rx->desc_sink_only(in, (size_t)n, frame_length); *crc32 = rx->crc32();
+           memcpy(out, rx->frame_bytes(), frame_length < 4096 ? frame_length : 4096); delete rx; }
+    return e;
+}
+
 uint32_t sbo_crc32(const uint8_t* p, uint64_t n) { uint32_t c = 0xFFFFFFFFu; for (uint64_t i = 0; i < n; i++) c = (c >> 8) ^ tables().crc32_lut[p[i] ^ (c & 0xFF)]; return ~c; }
 
 } // extern "C"

@@ -1,0 +1,259 @@
+#!/bin/sh
+# Sourced by the build_ref_*.sh scripts that compile reference bricks from their own headers: `ref_shim DIR` writes the headers those
+# bricks include in place of the reference's framework headers, which only MSVC / the WDK compile.  Each stands for what the reference
+# header gives the bricks, with the line it comes from.  TEST INFRASTRUCTURE ONLY; nothing of the reference is copied here.
+# The shims:
+#   tpltrick.h    Log2, IsPower2, DummyInitializer and static_wrapper (tpltrick.h:95-148; the header itself redeclares template
+#                 parameters as member typedefs, :91-96, which GCC rejects); operator_repeater.h: rep_mul, rep_shift_right, rep_sub,
+#                 rep_memzero, rep_memcpy as the loops operator_repeater.h:42-173, 314 unroll (its rep_saturated_sub names a member
+#                 that does not exist, :182, which GCC rejects even uninstantiated);
+#   const.h       the repo's own sora_b200/brick/brick.hpp (BRICK macros, TFilter / TSink, pin queues) with CTX_VAR_RW / CTX_VAR_RO /
+#                 FACADE_FIELD taking the array extent the reference writes (CTX_VAR_RW(vcs, ChannelCoeffs, [16]), brick.h:426-470), a
+#                 DEFINE_LOCAL_CONTEXT of up to ten facades, FINL / SELECTANY / A16 / MEM_ALIGN (core/inc/const.h:81-86), and
+#                 _dump_symbol / _dump_text as no-ops (brick/inc/bb_debug.h:11-45 only print; with SB_DUMP_TEXT_TAP defined, _dump_text is
+#                 left to the library, whose debug tap counts the messages);
+#   brick.h, sora.h, dspcomm.h, soratime.h, bb/bba.h
+#                 what those headers give the bricks here: brick/inc/dspcomm.h:5-21's includes (vector128.h, fft.h, intalg.h, dspalg.hpp,
+#                 plus operator_repeater.h), SoraStopwatch with a no-op Restart (soratime.h) for CF_TimeStamps, SORA_RADIO_RX_STREAM / FLAG for CF_RxStream,
+#                 COMPLEX32 (complex.h:6), SORA_RX_SIGNAL_UNIT_SIZE 16 / _NUM_PER_DESC 7 (_rx_manager.h:79-81);
+#   vector128.h   vs / vi / vcs / vub (vector128.h:96-138, element access :107-108), SignalBlock (:1643-1648), and each operation as the
+#                 intrinsic or body vector128.h gives it:
+#     shifts      shift_right and >> on vcs (_mm_srai_epi16, :832) and on vi (_mm_srai_epi32, :830)
+#     arithmetic  saturated_add / saturated_sub on vcs (_mm_adds/subs_epi16, :645, :655), xor (:567), and / or, sign (_mm_sign_epi16,
+#                 :535), smin / smax on vcs (_mm_min/max_epi16, :1295, :1318), set_zero (:439)
+#     shuffles    permutate<imm>, permutate_high<imm>, permutate_low<imm> (:688, :683, :677)
+#     complex     conj (:966, XOR), conj0 (:979-989, psignw with 0x8000 on the imaginary halves: -32768 stays -32768), conjre (:952-961,
+#                 psignw), flip (:992-996), mul_j (:1258-1261), pairwise_muladd / muladd (_mm_madd_epi16, :920-921), SquaredNorm
+#                 (:932, muladd(a, a)), hadd on vi (:758, the four lanes summed and duplicated), pack(vi, vi) (:876-883: masked and
+#                 interleaved, it wraps) and pack(vcs&, vi, vi) (:887-890), conj_mul into vi re / im (:1038-1044), mul into vi re / im
+#                 (:1075-1081, conj0 then flip), mul(vcs, vcs) (:1201-1211: >> 15 then the wrapping pack) and the * on vcs it stands
+#                 behind (DEFINE_OPERATOR_OVERLOAD(*, vcs, mul), :1500), mul_shift / conj_mul_shift (:1215-1246)
+#     constants   the vector128_consts masks (:179-284) the FFT names
+#     macros      DSP_INLINE / DSP_INLINE1 (:22-24); __declspec(selectany / align / deprecated)
+ref_shim() {
+mkdir -p "$1/bb"
+cat > "$1/const.h" <<'SHIM'
+#pragma once
+#include "brick.hpp"
+#include <vector>
+#define __int8 char
+#define __int16 short
+#define __int32 int
+#define __int64 long long
+#define __forceinline inline __attribute__((always_inline))
+#define SELECTANY
+#define A16 __attribute__((aligned(16)))
+#define MEM_ALIGN(n) __attribute__((aligned(n)))
+#define UCHAR unsigned char
+#undef CTX_VAR_RW
+#undef CTX_VAR_RO
+#undef FACADE_FIELD
+#undef DEFINE_LOCAL_CONTEXT
+#define CTX_VAR_RW(TYPE, NAME, ...) TYPE (&NAME)__VA_ARGS__;
+#define CTX_VAR_RO(TYPE, NAME, ...) TYPE const (&NAME)__VA_ARGS__;
+#define FACADE_FIELD(TYPE, NAME, ...) private: TYPE __##NAME##__ __VA_ARGS__; public: auto NAME() -> TYPE (&)__VA_ARGS__ { return __##NAME##__; }
+#define SB_VBASES_7(a, b, c, d, e, f, g) SB_VBASES_6(a, b, c, d, e, f), virtual public g
+#define SB_VBASES_8(a, b, c, d, e, f, g, h) SB_VBASES_7(a, b, c, d, e, f, g), virtual public h
+#define SB_VBASES_9(a, b, c, d, e, f, g, h, i) SB_VBASES_8(a, b, c, d, e, f, g, h), virtual public i
+#define SB_VBASES_10(a, b, c, d, e, f, g, h, i, j) SB_VBASES_9(a, b, c, d, e, f, g, h, i), virtual public j
+#define SB_VB_PICK10(_1, _2, _3, _4, _5, _6, _7, _8, _9, _10, NAME, ...) NAME
+#define DEFINE_LOCAL_CONTEXT(TPL_BRICK, ...) struct __LocalContext_##TPL_BRICK : SB_VB_PICK10(__VA_ARGS__, SB_VBASES_10, SB_VBASES_9, \
+    SB_VBASES_8, SB_VBASES_7, SB_VBASES_6, SB_VBASES_5, SB_VBASES_4, SB_VBASES_3, SB_VBASES_2, SB_VBASES_1)(__VA_ARGS__) {};
+template<int N> inline void _dump_symbol(const char*, const COMPLEX16*) {}
+#ifdef SB_DUMP_TEXT_TAP
+void _dump_text(const char* fmt, ...);
+#else
+inline void _dump_text(const char*, ...) {}
+#endif
+SHIM
+printf '#pragma once\n#include "const.h"\n' > "$1/brick.h"
+cat > "$1/tpltrick.h" <<'SHIM'
+#pragma once
+#include "const.h"
+template<int N> struct Log2 { enum { value = Log2<N / 2>::value + 1 }; };
+template<> struct Log2<1> { enum { value = 0 }; };
+template<int N> struct IsPower2 { enum { IsFalse = (N & 1) + IsPower2<N / 2>::IsFalse }; };
+template<> struct IsPower2<1> { enum { IsFalse = 0 }; };
+struct DummyInitializer { void operator()(...) { } };
+template<typename T, typename INITIALIZER = DummyInitializer> class static_wrapper {
+    static T value __attribute__((aligned(16)));
+public:
+    static_wrapper(INITIALIZER init_func = INITIALIZER()) { init_func(value); }
+    operator T&() const { return value; }
+    T& get() const { return value; }
+};
+template<typename T, typename INITIALIZER> T static_wrapper<T, INITIALIZER>::value;
+SHIM
+cat > "$1/operator_repeater.h" <<'SHIM'
+#pragma once
+#include "vector128.h"
+template<size_t N, typename T> inline void rep_mul(T* dst, const T* src0, const T* src1) { for (size_t i = 0; i < N; i++) *dst++ = (*src0++) * (*src1++); }
+template<size_t N, typename T> inline void rep_shift_right(T* dst, const T* src, const int nbits) { for (size_t i = 0; i < N; i++) *dst++ = (*src++) >> nbits; }
+template<size_t N, typename T> inline void rep_sub(T* dst, const T* src, const T& val) { for (size_t i = 0; i < N; i++) *dst++ = sub(*src++, val); }
+template<size_t N, typename T> inline void rep_memzero(T* dst) { for (size_t i = 0; i < N; i++) set_zero(*dst++); }
+template<size_t N, typename T> inline void rep_memcpy(T* dst, const T* src) { for (size_t i = 0; i < N; i++) *dst++ = *src++; }
+SHIM
+cat > "$1/sora.h" <<'SHIM'
+#pragma once
+#include "const.h"
+#include "vector128.h"
+typedef struct SORA_RADIO_RX_STREAM SORA_RADIO_RX_STREAM;
+typedef unsigned char FLAG;
+#define NODEFAULT __builtin_unreachable()
+inline int ceil_div(int x, int mod) { return (x + mod - 1) / mod; }
+SHIM
+cat > "$1/soratime.h" <<'SHIM'
+#pragma once
+struct SoraStopwatch { explicit SoraStopwatch(bool) {} void Restart() {} };
+SHIM
+cat > "$1/dspcomm.h" <<'SHIM'
+#pragma once
+#include "const.h"
+#include "vector128.h"
+#include <fft.h>
+#include <intalg.h>
+#include "operator_repeater.h"
+#include <dspalg.hpp>
+SHIM
+cat > "$1/bb/bba.h" <<'SHIM'
+#pragma once
+#include "../const.h"
+#include "../vector128.h"
+typedef struct _COMPLEX32 { int re, im; } COMPLEX32;
+#define SORA_RX_SIGNAL_UNIT_SIZE 16
+#define SORA_RX_SIGNAL_UNIT_NUM_PER_DESC 7
+#define SORA_RX_SIGNAL_UNIT_COMPLEX16_NUM (SORA_RX_SIGNAL_UNIT_SIZE / sizeof(COMPLEX16))
+SHIM
+cat > "$1/vector128.h" <<'SHIM'
+#pragma once
+#include <smmintrin.h>
+#include <stddef.h>
+#include <string.h>
+#include "const.h"
+#define DSP_INLINE inline __attribute__((always_inline))
+#define DSP_INLINE1 inline
+#define __declspec(x) SB_DECLSPEC_##x
+#define SB_DECLSPEC_selectany
+#define SB_DECLSPEC_deprecated
+#define SB_DECLSPEC_align(n) __attribute__((aligned(n)))
+#define SB_VEC(NAME, TDATA)                                                                                     \
+struct NAME {                                                                                                   \
+    static const size_t size = 16 / sizeof(TDATA);                                                              \
+    typedef TDATA data_type[size] __attribute__((aligned(16)));                                                 \
+    typedef TDATA elem_type;                                                                                    \
+    typedef __m128i raw_type;                                                                                   \
+    NAME() {}                                                                                                   \
+    explicit NAME(__m128i r) : _raw(r) {}                                                                       \
+    template<typename TA> explicit NAME(const TA& a) : _raw((__m128i)a) {}                                      \
+    NAME(const data_type& pa) : _raw(_mm_loadu_si128((const __m128i*)pa)) {}                                    \
+    operator __m128i() const { return _raw; }                                                                   \
+    TDATA& operator[](size_t i) { return ((TDATA*)&_raw)[i]; }                                                  \
+    const TDATA& operator[](size_t i) const { return ((const TDATA*)&_raw)[i]; }                                \
+    __m128i _raw;                                                                                               \
+};
+SB_VEC(vs, short)
+SB_VEC(vi, int)
+SB_VEC(vub, unsigned char)
+SB_VEC(vcs, COMPLEX16)
+struct COMPLEXU32 { unsigned int re, im; };
+SB_VEC(vcui, COMPLEXU32)
+template<typename T> inline T& cast_ref(void* p) { return *reinterpret_cast<T*>(p); }
+template<typename T> inline const T& cast_ref(const void* p) { return *reinterpret_cast<const T*>(p); }
+struct SignalBlock {
+    static const size_t size = 7;
+    vcs _data[size];
+    vcs& operator[](size_t index) { return _data[index]; }
+    const vcs& operator[](size_t index) const { return _data[index]; }
+};
+namespace sbref { extern int phase; void tap_pack(__m128i v, int k); void tap_zero(__m128i v); void tap_clamp(__m128i r, __m128i a);
+                  void tap_madd(__m128i v); }
+class vector128_consts {
+public:
+    template<typename T> static T __0x0000FFFF0000FFFF0000FFFF0000FFFF() { return (T)_mm_set1_epi32(0x0000FFFF); }
+    template<typename T> static T __0xFFFF0000FFFF0000FFFF0000FFFF0000() { return (T)_mm_set1_epi32((int)0xFFFF0000); }
+    template<typename T> static T __0xFFFFFFFF00000000FFFFFFFF00000000() { return (T)_mm_set_epi32(-1, 0, -1, 0); }
+    template<typename T> static T __0xFFFFFFFFFFFFFFFF0000000000000000() { return (T)_mm_set_epi32(-1, -1, 0, 0); }
+    template<typename T> static T __0xFFFF0000FFFF00000000000000000000() { return (T)_mm_set_epi32((int)0xFFFF0000, (int)0xFFFF0000, 0, 0); }
+    template<typename T> static T __0xFFFF0000000000000000000000000000() { return (T)_mm_set_epi32((int)0xFFFF0000, 0, 0, 0); }
+};
+template<typename T> inline void set_zero(T& a) { a = T(_mm_setzero_si128()); }
+inline vcs shift_right(const vcs& a, int n) { return vcs(_mm_srai_epi16(a, n)); }
+inline vi shift_right(const vi& a, int n) { vi r(_mm_srai_epi32(a, n)); if (n == 8) sbref::tap_zero(r); return r; }
+inline vcs operator>>(const vcs& a, int n) { return shift_right(a, n); }
+inline vi operator>>(const vi& a, int n) { return shift_right(a, n); }
+inline vi operator+(const vi& a, const vi& b) { return vi(_mm_add_epi32(a, b)); }
+inline vi& operator*=(vi& a, const vi& b) { a = vi(_mm_mullo_epi32(a, b)); return a; }
+inline vcs saturated_add(const vcs& a, const vcs& b) { return vcs(_mm_adds_epi16(a, b)); }
+inline vcs saturated_sub(const vcs& a, const vcs& b) { return vcs(_mm_subs_epi16(a, b)); }
+inline vcs xor(const vcs& a, const vcs& b) { return vcs(_mm_xor_si128(a, b)); }
+inline vcs sign(const vcs& a, const vcs& b) { return vcs(_mm_sign_epi16(a, b)); }
+inline vcs smin(const vcs& a, const vcs& b) { vcs r(_mm_min_epi16(a, b)); sbref::tap_clamp(r, a); return r; }
+inline vcs smax(const vcs& a, const vcs& b) { vcs r(_mm_max_epi16(a, b)); sbref::tap_clamp(r, a); return r; }
+template<int imm> inline vcs permutate(const vcs& a) { return vcs(_mm_shuffle_epi32(a, imm)); }
+template<int a0, int a1, int a2, int a3> inline vcs permutate(const vcs& a) { return vcs(_mm_shuffle_epi32(a, _MM_SHUFFLE(a3, a2, a1, a0))); }
+inline vcui interleave_low(const vcui& a, const vcui& b) { return vcui(_mm_unpacklo_epi64(a, b)); }
+inline vcs add(const vcs& a, const vcs& b) { return vcs(_mm_add_epi16(a, b)); }
+inline vcs sub(const vcs& a, const vcs& b) { return vcs(_mm_sub_epi16(a, b)); }
+inline vcs hadd(const vcs& a) {
+    __m128i s = _mm_add_epi16(a, _mm_shuffle_epi32(a, 0x4E));
+    return vcs(_mm_add_epi16(s, _mm_shuffle_epi32(s, 0xB1)));
+}
+inline int SquaredNorm(const COMPLEX16& c) { return c.re * c.re + c.im * c.im; }
+template<int imm> inline vcs permutate_high(const vcs& a) { return vcs(_mm_shufflehi_epi16(a, imm)); }
+template<int imm> inline vcs permutate_low(const vcs& a) { return vcs(_mm_shufflelo_epi16(a, imm)); }
+inline vcs conj(const vcs& a) { return xor(a, vector128_consts::__0xFFFF0000FFFF0000FFFF0000FFFF0000<vcs>()); }
+inline vcs conj0(const vcs& a) { return sign(a, vcs(_mm_set1_epi32((int)0x80000001))); }
+inline vcs conjre(const vcs& a) { return sign(a, vcs(_mm_set1_epi32(0x00018000))); }
+inline vcs flip(const vcs& a) { vcs b = permutate_low<0xb1>(a); return permutate_high<0xb1>(b); }
+inline vcs mul_j(const vcs& a) { return xor(flip(a), vector128_consts::__0x0000FFFF0000FFFF0000FFFF0000FFFF<vcs>()); }
+inline vi pairwise_muladd(const vs& a, const vs& b) { __m128i r = _mm_madd_epi16(a, b); sbref::tap_madd(r); return vi(r); }
+inline vi muladd(const vcs& a, const vcs& b) { __m128i r = _mm_madd_epi16(a, b); sbref::tap_madd(r); return vi(r); }
+inline vi SquaredNorm(const vcs& a) { return muladd(a, a); }
+inline vi hadd(const vi& a) {
+    __m128i s = _mm_add_epi32(a, _mm_shuffle_epi32(a, 0x4E));
+    return vi(_mm_add_epi32(s, _mm_shuffle_epi32(s, 0xB1)));
+}
+inline vs pack(const vi& a, const vi& b) {
+    const __m128i m = vector128_consts::__0x0000FFFF0000FFFF0000FFFF0000FFFF<vi>();
+    return vs(_mm_or_si128(_mm_and_si128(a, m), _mm_slli_epi32(_mm_and_si128(b, m), 16)));
+}
+inline void pack(vcs& r, const vi& re, const vi& im) { sbref::tap_pack(re, 0); sbref::tap_pack(im, 0); r = (vcs)pack(re, im); }
+inline void conj_mul(vi& re, vi& im, const vcs& a, const vcs& b) {
+    vcs vs1 = flip(b);
+    vs1 = conjre(vs1);
+    re = pairwise_muladd((vs&)a, (vs&)b);
+    im = pairwise_muladd((vs&)vs1, (vs&)a);
+}
+inline void mul(vi& re, vi& im, const vcs& a, const vcs& b) {
+    vcs vs1 = conj0(b);
+    vcs vs2 = flip(b);
+    re = muladd(a, vs1);
+    im = muladd(a, vs2);
+}
+inline vcs mul(const vcs& a, const vcs& b) {
+    vi re, im;
+    mul(re, im, a, b);
+    re = shift_right(re, 15);
+    im = shift_right(im, 15);
+    sbref::tap_pack(re, 1); sbref::tap_pack(im, 1);
+    return (vcs)pack(re, im);
+}
+inline vcs operator*(const vcs& a, const vcs& b) { return mul(a, b); }
+inline vcs conj_mul_shift(const vcs& a, const vcs& b, int nbits_right) {
+    vcs vcs1 = conjre(a);
+    vcs1 = flip(vcs1);
+    vi vi0 = pairwise_muladd((vs&)a, (vs&)b);
+    vi vi1 = pairwise_muladd((vs&)vcs1, (vs&)b);
+    vi0 = shift_right(vi0, nbits_right);
+    vi1 = shift_right(vi1, nbits_right);
+    return (vcs)pack(vi0, vi1);
+}
+inline vcs mul_shift(const vcs& a, const vcs& b, int nbits_right) {
+    vi vi0 = pairwise_muladd((vs&)a, (vs)conj(b));
+    vi vi1 = pairwise_muladd((vs&)a, (vs)flip(b));
+    vi0 = shift_right(vi0, nbits_right);
+    vi1 = shift_right(vi1, nbits_right);
+    return (vcs)pack(vi0, vi1);
+}
+SHIM
+}

@@ -58,6 +58,12 @@ public:
     uint32_t back_status() const { return error_code; }
     uint32_t back_crc32() const { return frame_crc32; }
     const uint8_t* frame_bytes() const { return frame_buf; }
+    // T11aPLCPParser alone, on a context whose CF_11aRxVector, CF_11RxPLCPSwitch and CF_Error were just Reset (as after every event):
+    // out = plcp_state (1: accepted), error_code, data_rate_kbps, frame_length, total_symbols, code_rate
+    void plcp_parse_only(uint32_t sig, uint32_t out[6]);
+    // T11aDesc -> TBB11aFrameSink alone, both fresh, for a frame of frame_length_ bytes, fed n decoded bytes; returns error_code
+    // (frame_bytes() and back_crc32() hold the rest)
+    uint32_t desc_sink_only(const uint8_t* in, size_t n, uint16_t frame_length_);
 
 private:
     // ---- context facades ----
@@ -89,6 +95,8 @@ private:
     std::vector<uint8_t> vit_out;
 
     void ctx_reset();
+    void rxvector_reset();
+    bool plcp_parse(uint32_t sig);
     void cca_init();
     void dcest_init();
     void on_vec20(v128 v);

@@ -116,10 +116,13 @@ void Rx11n::reset_carrier_sense() {                    // BB11nDemodContext::Res
     error_code = E_SUCCESS; cca_state = 0; symbol_type = SYM_L_LTF;
     sense_count = 0; peak_found = false; peak_count = 0;
 }
-void Rx11n::reset_after_event() {                      // ssrc->Flush(); ctx.Reset(); ssrc->Reset()  (fb11n_demod.cpp:64-70)
-    reset_carrier_sense();
+void Rx11n::rxvector_reset() {
     frame_length = 0; total_symbols = 0; remain_symbols = 0; data_rate_kbps = 6000; code_rate = CR_12; frame_crc32 = 0;   // CF_11aRxVector::Reset()
     lsig_len2 = 0;                                      // the L-SIG length is frame_length before the HT-SIG overwrites it: zero again when L-SIG is refused
+}
+void Rx11n::reset_after_event() {                      // ssrc->Flush(); ctx.Reset(); ssrc->Reset()  (fb11n_demod.cpp:64-70)
+    reset_carrier_sense();
+    rxvector_reset();
     ds_n = 0; lltf_n = sym_n = sig_n = htltf_n = 0;
     vit.max_steps = 5000 * 8; vit.reset(); ob_count = 0; vit_in.clear(); vit_out.assign(256, 0);
     desc_count = 0; desc_reg = 0; byte_count = 0; crc_run = 0xFFFFFFFFu;
@@ -273,6 +276,13 @@ void Rx11n::on_sig3() {                                // T11nSigDemap, T11aDein
     uint32_t lsig = (uint32_t)viterbi_sig_bits(dsoft, 24); memcpy(sig, &lsig, 4);
     uint64_t ht = viterbi_sig_bits(dsoft + 48, 48); memcpy(sig + 3, &ht, 6);
     if (taps.enable) memcpy(taps.sig, sig, 9);
+    if (!parse_sig(sig)) { error_code = E_PLCP_HEADER_FAIL; return; }
+    frame_length = ht_frame_length;
+    symbol_type = SYM_HT_STF;
+}
+
+// T11nSigParser::_parse_plcp and _parse_htsig (PHY_11n.hpp:458-513) on the 9 bytes T11nViterbiSig hands it
+bool Rx11n::parse_sig(const uint8_t* sig) {
     uint32_t u; memcpy(&u, sig, 4); u &= 0xFFFFFF;
     bool ok = !(u & 0xFC0010);
     if (ok) { uint32_t p = (u >> 16) ^ u; p ^= p >> 8; p ^= p >> 4; p ^= p >> 2; p ^= p >> 1; ok = !(p & 1); }
@@ -282,7 +292,9 @@ void Rx11n::on_sig3() {                                // T11nSigDemap, T11aDein
     if (ok) {                                                                               // _parse_htsig
         const uint8_t* ip = sig + 3;
         uint8_t c = crc8_htsig(ip, 4, 2);
-        if (c != (uint8_t)((ip[4] >> 2) | (ip[5] << 6))) { ht_frame_mcs = 0; ht_frame_length = 0; ok = false; }
+        // compared as int, as PHY_11n.hpp:488 compares its UCHAR with an int: a byte 5 above 3 fails the check.  The SIG decoder's >> 6
+        // leaves byte 5 at most 3, so a receiver never gets there; the parser on its own does
+        if (c != ((ip[4] >> 2) | (ip[5] << 6))) { ht_frame_mcs = 0; ht_frame_length = 0; ok = false; }
         else {
             ht_frame_mcs = ip[0] & 0x7F;
             if (ht_frame_mcs < 8 || ht_frame_mcs >= ht_mcs_limit()) ok = false;
@@ -297,9 +309,18 @@ void Rx11n::on_sig3() {                                // T11nSigDemap, T11aDein
             }
         }
     }
-    if (!ok) { error_code = E_PLCP_HEADER_FAIL; return; }
-    frame_length = ht_frame_length;
-    symbol_type = SYM_HT_STF;
+    return ok;
+}
+void Rx11n::sig_parse_only(const uint8_t* sig, uint32_t out[8]) {
+    error_code = E_SUCCESS; rxvector_reset();
+    if (parse_sig(sig)) frame_length = ht_frame_length; else error_code = E_PLCP_HEADER_FAIL;
+    out[0] = error_code == E_SUCCESS; out[1] = error_code; out[2] = data_rate_kbps; out[3] = frame_length; out[4] = total_symbols; out[5] = code_rate;
+    out[6] = ht_frame_mcs; out[7] = ht_frame_length;
+}
+uint32_t Rx11n::desc_sink_only(const uint8_t* in, size_t n, uint16_t frame_length_) {
+    error_code = E_SUCCESS; frame_length = frame_length_; frame_crc32 = 0; desc_count = 0; desc_reg = 0; byte_count = 0; crc_run = 0xFFFFFFFFu;
+    for (size_t i = 0; i < n; i++) sink_byte(in[i]);
+    return error_code;
 }
 
 // ---- HT-LTF: 2x2 channel and its inverse (channel_11n.hpp:331-442, sora_matrix.h:135-150,296-304) ------------------------

@@ -65,6 +65,14 @@ public:
     void reset_carrier_sense();
     int run(const c16* s0, const c16* s1, size_t n, FrameResult11n* res, uint8_t* out, size_t out_stride, int max_frames);
     Taps11n taps;
+    // T11nSigParser alone, after the CF_11aRxVector::Reset and error code clear of every event; CF_HTRxVector carries over from the
+    // call before, as it does between events.  out = accepted, error_code, data_rate_kbps, frame_length, total_symbols, code_rate,
+    // ht_frame_mcs, ht_frame_length
+    void sig_parse_only(const uint8_t* sig, uint32_t out[8]);
+    // T11aDesc -> TBB11aFrameSink alone, both fresh, for a frame of frame_length_ bytes, fed n decoded bytes; returns error_code
+    uint32_t desc_sink_only(const uint8_t* in, size_t n, uint16_t frame_length_);
+    uint32_t crc32() const { return frame_crc32; }
+    const uint8_t* frame_bytes() const { return frame_buf; }
 
 private:
     enum { SYM_L_LTF = 1, SYM_SIG, SYM_HT_STF, SYM_HT_LTF, SYM_DATA };
@@ -100,6 +108,8 @@ private:
     void on_htltf();
     void on_data(const c16 Y[2][64]);
     void viterbi_feed(bool flush);
+    void rxvector_reset();
+    bool parse_sig(const uint8_t* sig);
     void sink_byte(uint8_t b);
 };
 

@@ -476,7 +476,7 @@ __global__ void __launch_bounds__(32 * SB_FRONT11N_WARPS, SB_FRONT11N_MINB) k_fr
 #pragma unroll
             for (int k = 0; k < 2; k++) c = (c & 1) ? (uint8_t)((c >> 1) ^ 0xE0) : (uint8_t)(c >> 1);
             c = (uint8_t)~c;
-            if (c != (uint8_t)((sg[7] >> 2) | (sg[8] << 6))) { mcs = 0; ok = false; }
+            if (c != ((sg[7] >> 2) | (sg[8] << 6))) { mcs = 0; ok = false; }     // as int, as PHY_11n.hpp:488 compares its UCHAR
             else {
                 mcs = sg[3] & 0x7F;
                 if (mcs < 8 || mcs >= N.mcs_limit) ok = false;

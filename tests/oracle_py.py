@@ -387,3 +387,60 @@ def ref_rx11a_carrier_sense(iq, cca_pwr_threshold=1000 * 1000, max_vec=1 << 20):
     L.ref_rx11a_carrier_sense.argtypes = [C.c_void_p, C.c_size_t, C.c_uint, C.c_void_p, C.c_size_t, C.c_void_p]
     n = L.ref_rx11a_carrier_sense(_p(iq), len(iq), cca_pwr_threshold, _p(rec), max_vec, _p(det))
     return rec[:n], int(det[0])
+
+# ---- the header parsers and the descrambler / frame sink alone: the oracle's, and the reference's own (oracle/build_ref_rx11n.sh) ----
+PLCP11A_FIELDS = ("accepted", "error_code", "rate_kbps", "frame_length", "total_symbols", "code_rate")
+SIG11N_FIELDS = PLCP11A_FIELDS + ("ht_mcs", "ht_length")
+def _parse_words(fn, words):
+    w = np.ascontiguousarray(words, np.uint32).reshape(-1); out = np.zeros((len(w), 6), np.uint32)
+    fn(_p(w), C.c_uint64(len(w)), _p(out)); return out
+def _parse_sig9(fn, sig9):
+    s = np.ascontiguousarray(sig9, np.uint8).reshape(-1, 9); out = np.zeros((len(s), 8), np.uint32)
+    fn(_p(s), C.c_uint64(len(s)), _p(out)); return out
+def plcp11a_parse(words):
+    """The oracle's 802.11a SIGNAL parse on each word, from a context just reset: uint32 [n, 6] (PLCP11A_FIELDS)."""
+    return _parse_words(lib().sbo_plcp11a_parse, words)
+def sig11n_parse(sig9):
+    """The oracle's L-SIG + HT-SIG parse on uint8 [n, 9] blocks in turn, one context (the HT fields carry over): uint32 [n, 8] (SIG11N_FIELDS)."""
+    return _parse_sig9(lib().sbo_sig11n_parse, sig9)
+def desc_sink(chain, decoded, frame_length):
+    """The oracle's descrambler and frame sink of the 802.11a (chain 0) or 802.11n (chain 1) receiver, fed the decoded bytes of a frame of
+    frame_length bytes: (error code, CF_11aRxVector::crc32, the frame buffer's first frame_length bytes)."""
+    d = np.ascontiguousarray(decoded, np.uint8); out = np.zeros(frame_length, np.uint8); crc = np.zeros(1, np.uint32)
+    L = lib(); L.sbo_desc_sink.restype = C.c_uint32
+    e = L.sbo_desc_sink(C.c_int(chain), _p(d), C.c_uint64(len(d)), C.c_uint16(frame_length), _p(out), _p(crc))
+    return int(e), int(crc[0]), out
+
+_REF_RX11N = None
+REF_RX11N_COUNTERS = ("lsig_reserved", "lsig_parity", "lsig_rate", "lsig_length", "htsig_crc8", "htsig_mcs", "htsig_length", "accepted",
+                      "fcs_ok", "fcs_fail")   # the order of ref_rx11n_debug's counts
+def ref_rx11n_available():
+    return os.path.exists(os.path.join(ROOT, "oracle", "_ref", "librx11n_ref.so"))
+def _ref_rx11n():
+    global _REF_RX11N
+    if _REF_RX11N is None:
+        L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "librx11n_ref.so"))
+        L.ref_plcp11a_parse.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p]; L.ref_plcp11a_parse.restype = None
+        L.ref_sig11n_parse.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p]; L.ref_sig11n_parse.restype = None
+        L.ref_desc_sink.argtypes = [C.c_void_p, C.c_size_t, C.c_uint16, C.c_void_p, C.c_void_p]; L.ref_desc_sink.restype = C.c_uint32
+        L.ref_rx11n_debug.argtypes = [C.c_void_p]; L.ref_rx11n_debug.restype = None
+        L.ref_rx11n_debug_reset.argtypes = []; L.ref_rx11n_debug_reset.restype = None
+        _REF_RX11N = L
+    return _REF_RX11N
+def ref_plcp11a_parse(words):
+    """T11aPLCPParser (PHY_11a.hpp) on each word, from a context just Reset: uint32 [n, 6] (PLCP11A_FIELDS)."""
+    return _parse_words(_ref_rx11n().ref_plcp11a_parse, words)
+def ref_sig11n_parse(sig9):
+    """T11nSigParser (PHY_11n.hpp) on uint8 [n, 9] blocks in turn, one context: uint32 [n, 8] (SIG11N_FIELDS)."""
+    return _parse_sig9(_ref_rx11n().ref_sig11n_parse, sig9)
+def ref_desc_sink(decoded, frame_length):
+    """T11aDesc -> TBB11aFrameSink (scramble.hpp, PHY_11a.hpp), fresh, fed the decoded bytes: (error code, crc32, frame bytes)."""
+    d = np.ascontiguousarray(decoded, np.uint8); out = np.zeros(max(frame_length, 1), np.uint8); crc = np.zeros(1, np.uint32)
+    e = _ref_rx11n().ref_desc_sink(_p(d), len(d), frame_length, _p(out), _p(crc))
+    return int(e), int(crc[0]), out[:frame_length]
+def ref_rx11n_debug_reset():
+    _ref_rx11n().ref_rx11n_debug_reset()
+def ref_rx11n_debug():
+    """What the tap counted since the last ref_rx11n_debug_reset on this thread, as {name: count} (REF_RX11N_COUNTERS)."""
+    d = np.zeros(10, np.uint64); _ref_rx11n().ref_rx11n_debug(d.ctypes.data)
+    return dict(zip(REF_RX11N_COUNTERS, (int(v) for v in d)))
