@@ -11,6 +11,7 @@
   --config tx11b_legacy  the legacy 802.11b transmitter (BB11BPMDPacketGenSignal: encoder + SSE filter, fused) on the device, 11 Mbps / 1500 B
   --config tx11a_legacy  the legacy 802.11a transmitter (BB11ATxFrameMod) on the device, 54 Mbps / 1500 B, at 40 and at 44 Msps
   --config channelize  the wideband channelizer: four 802.11a channels of a 160 Msps capture, 127 taps, D = 4, device-resident
+  --config combine   the wideband combiner: four 802.11a channel rows at 40 Msps into one 160 Msps capture, 127 taps, U = 4, device-resident
   --config 11n       config #4: 802.11n HT-MF 2x2 RX chain at MCS 8, 9, 10, PSDU 1500 B, 2 x 40 Msps, fixed 2x2 channel
 
 Each prints one JSON line per measurement (same timing rules as bench.py: >= 3 warm-ups, CUDA events on the launch
@@ -460,12 +461,41 @@ def bench_channelize(args):
             "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs of every channel" % m})
     c.close()
 
+def bench_combine(args):
+    """The wideband combiner into a device-resident 160 Msps capture: four 802.11a channel rows at 40 Msps moved to -60 / -20 / +20 / +60 MHz,
+    127 taps, U = 4; as many output samples as --config channelize reads.  Work per output sample: K (2 ceil(ntaps / U) + 4 + 2) integer
+    multiply-adds; HBM traffic 4 B written + 4 K / U B read."""
+    import wideband_inputs as W, combine_model as CM
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    K, U = 4, 4; n_out = args.frames * 9824 * 4; n_in = n_out // U
+    taps = W.lowpass(127, 0.1, gain=U); ch = [(W.phase_inc(f, 160e6), 0, 4096) for f in (-60e6, -20e6, 20e6, 60e6)]
+    x = torch.randint(-8000, 8000, (K, n_in, 2), dtype=torch.int16, device=dev); y = torch.empty((n_out, 2), dtype=torch.int16, device=dev)
+    def step(): eng.combine_raw(x.data_ptr(), n_in, n_in, ch, U, taps, y.data_ptr(), st.cuda_stream)
+    step(); torch.cuda.synchronize()
+    P = 5000; m = U * P - len(taps)                                      # outputs that a prefix of P input samples determines
+    assert (CM.combine(x[:, :P].cpu().numpy(), ch, U, taps)[:m] == y[:m].cpu().numpy()).all(), "combiner output differs from the stated arithmetic"
+    ms = c.timed(step, args.steps)
+    sec = ms * 1e-3
+    hbm = n_out * (4.0 + 4.0 * K / U); macs = n_out * K * (2.0 * -(-len(taps) // U) + 6.0)
+    name, plim, clk = _card(); sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    imad_peak = sms * 64 * clk * 1e6 if clk else None                    # int32 IMAD: 64 per SM per clock on sm_90
+    f_hbm = hbm / sec / 1e9 / peaks(); f_int = (macs / sec / imad_peak) if imad_peak else None
+    c.emit({"metric": "wideband combiner output Msamples/s (COMPLEX16 out, 4 channels, U = 4)", "value": c.world * n_out / sec / 1e6, "unit": "Msamples/s", "ms_per_step": ms, "n_gpus": c.world,
+            "config": {"workload": "4 x 802.11a rows at 40 Msps -> 160 Msps capture, channels at -60/-20/+20/+60 MHz, 127 taps, U = 4, device-resident", "output_samples_per_step_per_gpu": n_out},
+            "hbm": {"achieved": hbm / sec / 1e9, "peak": peaks(), "unit": "GB/s", "frac": f_hbm, "note": "4 B written + 4 K / U B read per output sample"},
+            "int_mad": {"achieved": macs / sec / 1e9, "peak": imad_peak / 1e9 if imad_peak else None, "unit": "G multiply-adds/s", "frac": f_int,
+                        "note": "K (2 ceil(ntaps / U) + 4 + 2) per output sample; peak = SMs x 64 x max SM clock"},
+            "bound": None if f_int is None else ("integer" if f_int > f_hbm else "hbm"),
+            "card": name, "power_limit_w": plim, "max_sm_clock_mhz": clk,
+            "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs" % m})
+    c.close()
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "combine"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "combine": bench_combine}[a.config](a)

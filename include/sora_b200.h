@@ -167,6 +167,28 @@ typedef struct sb200_ddc_channel { uint32_t phase_inc; uint32_t phase0; } sb200_
 int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_in_samples, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t decim,
                      const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride_samples, void* cuda_stream);
 
+/* Wideband combiner, the transmit counterpart of sb200_channelize: K = nchannels rows x_k[0 .. n_in) of COMPLEX16 at the channel rate
+ * (row k at rows + k * row_stride samples) interpolated by U = interp, each moved to its centre frequency, scaled and summed into one
+ * capture y[0 .. U n_in) at the wideband rate; an extension without a reference counterpart.  For channel k = {phase_inc, phase0, gain}
+ * and every output n:
+ *     z_k(i)    = x_k(i / U) if i mod U == 0 and 0 <= i / U < n_in, else 0        zero-stuffing
+ *     u_k(n)    = sat16((sum_j taps[j] * z_k(n + j - c) + 2^14) >> 15)          c = (ntaps - 1) / 2, int32, re and im independently
+ *     phi(n)    = (phase0 + (uint32)n * phase_inc) mod 2^32, (C, S) = NCO[phi >> 20]   the Q14 table of sb200_channelize, n = absolute output index
+ *     v_k(n).re = sat16((u.re * C - u.im * S + 2^13) >> 14)                     u * e^{+j theta}: moves 0 Hz to +f_c
+ *     v_k(n).im = sat16((u.im * C + u.re * S + 2^13) >> 14)
+ *     y(n)      = sat16(sum_k ((v_k(n) * gain_k + 2^11) >> 12))                 gain in Q12 (4096 = unity), int32, re and im independently
+ * The NCO convention is the channelizer's with the opposite sign: a channel sent with (phase_inc, phase0) is recovered by sb200_channelize
+ * with the same pair.  Only the taps j = c - n (mod U) meet a non-zero z, so an interpolation filter may have a DC gain of U (each branch
+ * near unity); the limit that keeps the accumulator from wrapping is per branch.  The tail of the filter past U n_in is cut, as the
+ * channelizer cuts its edges: to keep it, pad the rows with zeros.  rows and out may be host or device pointers (device: 16-byte aligned,
+ * and the call is then asynchronous on the stream); channels and taps are host arrays.  Limits (SB200_E_INVALID, nothing launched):
+ * 1 <= nchannels <= 16, 1 <= interp <= 16, ntaps odd and <= 255, for every residue r mod U the sum of |taps[j]| over j = r (mod U) <= 65535,
+ * gain <= 65535, row_stride >= n_in, a multiple of 4 and <= 2^40, interp * n_in <= 2^40.  One kernel launch; sb200_last_kernel_ms times it.
+ * Input is COMPLEX16 only: COMPLEX8 rows (the 802.11b and legacy transmitters) are widened first, for example x << 7. */
+typedef struct sb200_duc_channel { uint32_t phase_inc; uint32_t phase0; uint32_t gain; } sb200_duc_channel;
+int sb200_combine(sb200_handle* h, const int16_t* rows, uint64_t row_stride_samples, uint64_t n_in_samples, const sb200_duc_channel* channels,
+                  uint32_t nchannels, uint32_t interp, const int16_t* taps, uint32_t ntaps, int16_t* out, void* cuda_stream);
+
 /* Same as sb200_rx11a_batch for captures at `sample_rate_mhz` = 20, 40 or 44.  20: the capture is already at the channel rate (slots counted in
  * 20 Msps samples; sample j stands where TDownSample2 would have put sample 2j of a 40 Msps capture).  44 Msps slots first pass the reference's 11:10 linear
  * resampler (TDownSample44_40 / Down44to40, Brick11/src/sampling.hpp:37-65, 44MTo40M.hpp:63-123; graph

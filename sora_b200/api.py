@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_combine", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -69,11 +69,14 @@ def _payload_table(payloads):
     return flat, offs, lens
 
 def phase_inc(f_hz, fs_hz):
-    """NCO increment of sb200_channelize for a channel centred at f_hz in a capture at fs_hz: round(f / fs * 2^32) mod 2^32 (negative f wraps)."""
+    """NCO increment of sb200_channelize and sb200_combine for a channel centred at f_hz in a capture at fs_hz: round(f / fs * 2^32) mod 2^32 (negative f wraps)."""
     return int(round(f_hz / fs_hz * 2 ** 32)) % 2 ** 32
 
 class DdcChannel(C.Structure):
     _fields_ = [("phase_inc", C.c_uint32), ("phase0", C.c_uint32)]
+
+class DucChannel(C.Structure):
+    _fields_ = [("phase_inc", C.c_uint32), ("phase0", C.c_uint32), ("gain", C.c_uint32)]
 
 _NDBPS_11A = {6000: 24, 9000: 36, 12000: 48, 18000: 72, 24000: 96, 36000: 144, 48000: 192, 54000: 216}   # 802.11a data bits per OFDM symbol
 
@@ -251,6 +254,22 @@ class Engine:
         out = np.zeros((len(channels), stride, 2), np.int16)
         self.channelize_raw(_ptr(iq), len(iq), channels, decim, taps, _ptr(out), stride)
         return out[:, :n_out]
+
+    def combine_raw(self, rows_ptr, row_stride, n_in, channels, interp, taps, out_ptr, stream=0):
+        """Pointer-level sb200_combine: rows_ptr / out_ptr host or device addresses; channels a list of (phase_inc, phase0, gain); taps int16 Q15."""
+        ch = (DucChannel * max(len(channels), 1))(*[DucChannel(int(a) % 2 ** 32, int(b) % 2 ** 32, int(g)) for a, b, g in channels])
+        t = np.ascontiguousarray(taps, dtype=np.int16)
+        self._check(self._lib.sb200_combine(self._h, C.c_void_p(rows_ptr), C.c_uint64(row_stride), C.c_uint64(n_in), C.cast(ch, C.c_void_p), C.c_uint32(len(channels)),
+                                            C.c_uint32(interp), C.c_void_p(_ptr(t)), C.c_uint32(len(t)), C.c_void_p(out_ptr), C.c_void_p(stream)), "sb200_combine")
+
+    def combine(self, rows, channels, interp, taps):
+        """Wideband combiner: int16 [K, n_in, 2] rows and K channels (phase_inc, phase0, gain Q12) -> int16 [interp * n_in, 2], every row
+        interpolated by interp through taps (int16 Q15, odd count <= 255, per-branch sum |t| <= 65535), moved to its centre, scaled and summed."""
+        rows = np.asarray(rows, dtype=np.int16).reshape(len(channels), -1, 2); n_in = rows.shape[1]; stride = (n_in + 3) // 4 * 4
+        x = np.zeros((len(channels), stride, 2), np.int16); x[:, :n_in] = rows
+        out = np.zeros((interp * n_in, 2), np.int16)
+        self.combine_raw(_ptr(x), stride, n_in, channels, interp, taps, _ptr(out))
+        return out
 
     def tx11b_fir37_raw(self, in_ptr, total, off_ptr, len_ptr, nframes, variant, out_ptr, stream=0):
         self._check(self._lib.sb200_tx11b_fir37(self._h, C.c_void_p(in_ptr), C.c_uint64(total), C.c_void_p(off_ptr), C.c_void_p(len_ptr), C.c_uint32(nframes),

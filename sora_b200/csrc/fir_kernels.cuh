@@ -206,4 +206,121 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_channelize(const uint32_t* _
     }
 }
 
+// ---- k_combine: the transmit counterpart (sb200_combine) ------------------------------------------------------------------------------
+// K rows x_k at the channel rate, each zero-stuffed by U, filtered by the taps, moved to +f_k by the NCO (the channelizer's table, the
+// opposite sign), scaled by a Q12 gain and summed into one capture y at U times the rate (include/sora_b200.h states the arithmetic).
+// Output n = U i + r sees only the taps j = j0 + U l, j0 = (c - r) mod U, on the inputs x(i + e_r + l), e_r = (r + j0 - c) / U; so the
+// filter runs on the rows as they are, one branch of taps per phase r, with no zero-stuffed buffer.
+//
+// Mapping: one CTA per tile of TI = 256 J input samples of every row (U TI outputs).  One elected thread starts one bulk copy per row of
+// the tile plus a halo of ceil(c / U) samples (rounded up to 4) on each side, and one of the NCO table when a channel rotates, all on one
+// mbarrier.  For each phase r a thread takes the J input indices tid + 256 j: for one tap the lanes of a warp read consecutive words (no
+// bank conflicts) and the tap is a uniform constant (zero taps skipped).  The K channels of one output are summed in registers; the sums
+// go to a shared output tile that is written to HBM with 16-byte stores.  Each input sample is read from HBM once, each output written once.
+#define SB_CB_SMEM 51200                   // dynamic shared memory budget of k_combine: four CTAs per multiprocessor
+
+struct CbChannels { uint32_t inc[SB_CH_MAXCH], phase0[SB_CH_MAXCH], gain[SB_CH_MAXCH]; uint32_t n; };
+
+// Halo (samples each side) and dynamic shared memory of k_combine for a tile of ti input samples: K windows, the U ti output tile, the
+// NCO table and the mbarrier.
+__host__ __device__ constexpr uint32_t combine_halo(uint32_t ntaps, uint32_t U) { return ((ntaps / 2 + U - 1) / U + 3u) & ~3u; }
+__host__ __device__ constexpr uint32_t combine_smem(uint32_t K, uint32_t U, uint32_t ntaps, uint32_t ti) {
+    return (K * (ti + 2 * combine_halo(ntaps, U)) + U * ti + SB_CH_NCO) * 4u + 16u;
+}
+static_assert(combine_smem(SB_CH_MAXCH, 1, SB_CH_MAXTAPS, SB_FIR_THREADS) <= SB_CB_SMEM && combine_smem(SB_CH_MAXCH, SB_CH_MAXDECIM, SB_CH_MAXTAPS, SB_FIR_THREADS) <= SB_CB_SMEM,
+              "a tile of 256 input samples must fit the budget at every K, U and ntaps (the largest need is at U = 1 and at U = 16)");
+
+// u * e^{+j theta} in Q14 with (C, S) = (cos theta, sin theta) packed as cs16: nco_rotate with the opposite sign
+__device__ __forceinline__ cs16 nco_rotate_up(cs16 u, uint32_t cs) {
+    const cs16 r = unpack(cs);
+    return mk(sat16((u.re * r.re - u.im * r.im + (1 << 13)) >> 14), sat16((u.im * r.re + u.re * r.im + (1 << 13)) >> 14));
+}
+
+// grid tiles, SB_FIR_THREADS threads, combine_smem(K, U, ntaps, 256 J) bytes of dynamic shared memory.  Row k starts at x + k * stride.
+template <int J>
+__global__ void __launch_bounds__(SB_FIR_THREADS) k_combine(const uint32_t* __restrict__ x, uint64_t stride, uint64_t n_in, const uint32_t* __restrict__ nco,
+                                                           CbChannels ch, uint32_t U, ChTaps taps, uint32_t* __restrict__ y) {
+    constexpr uint32_t TI = SB_FIR_THREADS * J;
+    extern __shared__ __align__(16) uint32_t smem[];
+    const uint32_t tid = threadIdx.x, K = ch.n, c = taps.n >> 1, halo = combine_halo(taps.n, U), win = TI + 2 * halo;
+    uint32_t* s_y = smem + K * win; uint32_t* s_nco = s_y + U * TI;
+    unsigned long long* s_bar = (unsigned long long*)(s_nco + SB_CH_NCO);
+    const uint64_t t0 = (uint64_t)blockIdx.x * TI;                      // first input sample of this tile
+    bool rotate = false;                                                // the table is only brought in when a channel needs it
+    for (uint32_t k = 0; k < K; k++) rotate |= ch.inc[k] != 0u || (ch.phase0[k] >> 20) != 0u;
+
+    // Staging: stage_window's steps for K rows on one barrier (window k holds samples [t0 - halo, t0 + TI + halo) of row k, zero outside
+    // [0, n_in)).  halo, TI and stride are multiples of 4, so every copy's source and destination are 16-byte aligned.
+    const uint64_t w0 = t0 >= halo ? t0 - halo : 0ull;
+    const uint64_t w1 = t0 + TI + halo < n_in ? t0 + TI + halo : n_in;
+    const uint32_t dst0 = (uint32_t)(w0 - (t0 - halo)), nw = (uint32_t)(w1 - w0), bulk = nw & ~3u;
+    for (uint32_t i = tid; i < K * win; i += SB_FIR_THREADS) { const uint32_t q = i % win; if (q < dst0 || q >= dst0 + bulk) smem[i] = 0; }
+    if (tid == 0) {
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(s_bar)));
+        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+    }
+    __syncthreads();
+    const uint32_t bytes = K * bulk * 4u + (rotate ? SB_CH_NCO * 4u : 0u);
+    const uint32_t mb = (uint32_t)__cvta_generic_to_shared(s_bar);
+    if (tid == 0 && bytes) {
+        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes) : "memory");
+        if (bulk) for (uint32_t k = 0; k < K; k++)
+            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                         :: "r"((uint32_t)__cvta_generic_to_shared(smem + k * win + dst0)), "l"(x + k * stride + w0), "r"(bulk * 4u), "r"(mb) : "memory");
+        if (rotate) asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                                 :: "r"((uint32_t)__cvta_generic_to_shared(s_nco)), "l"(nco), "r"(SB_CH_NCO * 4u), "r"(mb) : "memory");
+    }
+    if (tid < K * (nw & 3u)) { const uint32_t k = tid / (nw & 3u), q = tid % (nw & 3u); smem[k * win + dst0 + bulk + q] = __ldg(x + k * stride + w0 + bulk + q); }
+    if (bytes) {
+        uint32_t ok = 0;
+        while (!ok) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(ok) : "r"(mb) : "memory");
+    }
+    __syncthreads();
+
+    for (uint32_t r = 0; r < U; r++) {
+        const uint32_t j0 = (c % U + U - r) % U;                        // first tap of phase r's branch
+        const int e = ((int)(r + j0) - (int)c) / (int)U;                // exact: r + j0 - c is a multiple of U
+        const uint32_t* s_r = smem + (int)halo + e + tid;               // window word of input t0 + tid, tap j0
+        int sre[J], sim[J];
+#pragma unroll
+        for (int j = 0; j < J; j++) sre[j] = sim[j] = 0;
+        for (uint32_t k = 0; k < K; k++, s_r += win) {
+            uint32_t accr[J], acci[J];
+#pragma unroll
+            for (int j = 0; j < J; j++) accr[j] = acci[j] = 1u << 14;
+            for (uint32_t jj = j0, l = 0; jj < taps.n; jj += U, l++) {  // one tap at a time over the J inputs: the tap is a uniform constant
+                const int t = taps.t[jj];
+                if (t != 0) {
+#pragma unroll
+                    for (int j = 0; j < J; j++) {
+                        const cs16 v = unpack(s_r[l + SB_FIR_THREADS * j]);
+                        accr[j] += (uint32_t)(t * v.re); acci[j] += (uint32_t)(t * v.im);   // the per-branch tap limit keeps this from wrapping
+                    }
+                }
+            }
+            const uint32_t inc = ch.inc[k], g = ch.gain[k];
+            const bool ident = inc == 0u && (ch.phase0[k] >> 20) == 0u;     // NCO[0] = (2^14, 0): the rotation is the identity
+#pragma unroll
+            for (int j = 0; j < J; j++) {
+                cs16 v = mk(sat16((int)accr[j] >> 15), sat16((int)acci[j] >> 15));
+                if (!ident) {
+                    const uint32_t n = U * (uint32_t)(t0 + tid + SB_FIR_THREADS * j) + r;   // absolute output index mod 2^32
+                    v = nco_rotate_up(v, s_nco[(ch.phase0[k] + n * inc) >> 20]);
+                }
+                sre[j] += (v.re * (int)g + (1 << 11)) >> 12; sim[j] += (v.im * (int)g + (1 << 11)) >> 12;
+            }
+        }
+#pragma unroll
+        for (int j = 0; j < J; j++) s_y[(tid + SB_FIR_THREADS * j) * U + r] = pack(mk(sat16(sre[j]), sat16(sim[j])));
+    }
+    __syncthreads();
+
+    // outputs U t0 .. U t0 + U TI of y[0 .. U n_in): 16-byte stores (U t0 is a multiple of 4), the last 0..3 of the capture by hand
+    const uint64_t n0 = U * t0, n_out = U * n_in, nt = n_out - n0 < (uint64_t)U * TI ? n_out - n0 : (uint64_t)U * TI;
+    const uint32_t n4 = (uint32_t)nt >> 2;
+    uint4* y4 = (uint4*)(y + n0); const uint4* s4 = (const uint4*)s_y;
+    for (uint32_t q = tid; q < n4; q += SB_FIR_THREADS) y4[q] = s4[q];
+    if (tid < ((uint32_t)nt & 3u)) y[n0 + 4 * n4 + tid] = s_y[4 * n4 + tid];
+}
+
 } // namespace sb

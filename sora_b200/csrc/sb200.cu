@@ -269,9 +269,10 @@ struct sb200_handle {
     // lane_min and at most lane_max code blocks, the four-lanes-per-code-block kernel the others.  Options "viterbi_lane_min" / "viterbi_lane_max".
     uint32_t lane_min = SB200_LANE_MIN_DEFAULT, lane_max = SB200_LANE_MAX_DEFAULT;
     const char* last_vit = "";                         // name of the Viterbi kernel the last launch used (sb200_last_viterbi_kernel)
-    DevBuf nco;                                        // channelizer NCO table (fir_kernels.cuh), built on first use
+    DevBuf nco;                                        // NCO table of the channelizer and the combiner (fir_kernels.cuh), built on first use
     uint32_t ch_smem_set = 0;                          // bit J: k_channelize<J> may use SB_CH_SMEM bytes of dynamic shared memory on this device
     int sms = 0;                                       // multiprocessors of the device (channel groups of k_channelize)
+    uint32_t cb_smem_set = 0;                          // bit J: k_combine<J> may use SB_CB_SMEM bytes of dynamic shared memory on this device
     DevBuf vring;
     std::string err;
     int fail(int code, const char* what, cudaError_t e = cudaSuccess) {
@@ -944,6 +945,19 @@ extern "C" int sb200_fir_decimate2(sb200_handle* h, const int16_t* iq, uint64_t 
     return finish_call(h, st, ret, 0, 1);
 }
 
+// The NCO table of sb200_channelize and sb200_combine (fir_kernels.cuh), uploaded on first use:
+// (C, S) = (rint(2^14 cos 2 pi i / 4096), rint(2^14 sin 2 pi i / 4096)), packed like cs16.
+static int upload_nco(sb200_handle* h) {
+    if (h->nco.p) return SB200_OK;
+    std::vector<uint32_t> t(SB_CH_NCO);
+    for (int i = 0; i < SB_CH_NCO; i++) { const double a = 2.0 * M_PI * i / 4096.0; t[i] = pack(mk((int)nearbyint(16384.0 * cos(a)), (int)nearbyint(16384.0 * sin(a)))); }
+    cudaError_t e = h->nco.need(SB_CH_NCO * 4);
+    if (e == cudaSuccess) e = cudaMemcpy(h->nco.p, t.data(), SB_CH_NCO * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();   // landed before a kernel on a non-blocking stream reads it (TableArena::upload)
+    if (e != cudaSuccess) { h->nco.release(); return h->fail(SB200_E_CUDA, "NCO table upload", e); }
+    return SB200_OK;
+}
+
 // Wideband channelizer (fir_kernels.cuh): every channel shifted by its NCO, filtered and decimated by `decim`; channel c in row c of `out`.
 extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t decim,
                                 const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
@@ -963,14 +977,8 @@ extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_i
     const bool in_dev = is_device_ptr(iq), out_dev = is_device_ptr(out);
     if ((in_dev && ((uintptr_t)iq & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device input and output must be 16-byte aligned");
     CallScope call(h, st); CK(call.begin()); call.reads(iq);
-    if (!h->nco.p) {                                   // (C, S) = (rint(2^14 cos 2 pi i / 4096), rint(2^14 sin 2 pi i / 4096)), packed like cs16
-        std::vector<uint32_t> t(SB_CH_NCO);
-        for (int i = 0; i < SB_CH_NCO; i++) { const double a = 2.0 * M_PI * i / 4096.0; t[i] = pack(mk((int)nearbyint(16384.0 * cos(a)), (int)nearbyint(16384.0 * sin(a)))); }
-        cudaError_t e = h->nco.need(SB_CH_NCO * 4);
-        if (e == cudaSuccess) e = cudaMemcpy(h->nco.p, t.data(), SB_CH_NCO * 4, cudaMemcpyHostToDevice);
-        if (e == cudaSuccess) e = cudaDeviceSynchronize();   // landed before a kernel on a non-blocking stream reads it (TableArena::upload)
-        if (e != cudaSuccess) { h->nco.release(); return h->fail(SB200_E_CUDA, "NCO table upload", e); }
-    }
+    const int nrc = upload_nco(h);
+    if (nrc != SB200_OK) return nrc;
     const uint32_t* d_in; uint32_t* d_out = (uint32_t*)out; uint64_t d_stride = out_stride; Returns ret;
     CK(to_device(h->iq, (const uint32_t*)iq, in_dev, n_in * 4ull, st, &d_in, 16));
     if (!out_dev) {                                    // rows n_out (rounded to 4) apart in the workspace, copied into the caller's rows
@@ -981,6 +989,62 @@ extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_i
     ChChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
     for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; }
     const int rc = channelize_launch(h, st, d_in, n_in, ch, decim, T, d_out, d_stride, n_out);
+    return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
+}
+
+// One launch of k_combine<J> (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.
+template <int J>
+static int combine_launch_j(sb200_handle* h, cudaStream_t st, const uint32_t* d_in, uint64_t stride, uint64_t n_in, const CbChannels& ch, uint32_t U,
+                            const ChTaps& T, uint32_t* d_out) {
+    if (!(h->cb_smem_set & (1u << J))) {
+        CK(cudaFuncSetAttribute(k_combine<J>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_CB_SMEM));
+        h->cb_smem_set |= 1u << J;
+    }
+    const uint64_t ti = SB_FIR_THREADS * J;
+    CK(cudaEventRecord(h->ev0, st));
+    k_combine<J><<<(unsigned)((n_in + ti - 1) / ti), SB_FIR_THREADS, combine_smem(ch.n, U, T.n, (uint32_t)ti), st>>>(d_in, stride, n_in, (const uint32_t*)h->nco.p, ch, U, T, d_out);
+    return SB200_OK;
+}
+
+// Wideband combiner (fir_kernels.cuh): every row zero-stuffed by `interp`, filtered, shifted up by its NCO, scaled and summed into `out`.
+// Tiles of 1024, 512 or 256 input samples: the largest whose shared memory fits SB_CB_SMEM (256 always does).
+extern "C" int sb200_combine(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, const sb200_duc_channel* channels, uint32_t nchannels,
+                             uint32_t interp, const int16_t* taps, uint32_t ntaps, int16_t* out, void* cuda_stream) {
+    if (!h) return SB200_E_INVALID;
+    if (!rows || !channels || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
+    if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
+    if (interp < 1 || interp > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "interp must be 1 .. 16");
+    if ((ntaps & 1u) == 0 || ntaps > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 255");
+    for (uint32_t r = 0; r < interp; r++) {           // output n meets only the taps j = c - n (mod interp): one branch per residue
+        uint32_t asum = 0; for (uint32_t i = r; i < ntaps; i += interp) asum += (uint32_t)abs((int)taps[i]);
+        if (asum > 65535u) return h->fail(SB200_E_INVALID, "sum of |taps[j]| over j = r (mod interp) must be at most 65535 for every r (the int32 accumulator must not wrap)");
+    }
+    for (uint32_t i = 0; i < nchannels; i++)
+        if (channels[i].gain > 65535u) return h->fail(SB200_E_INVALID, "gain must be at most 65535");
+    if (row_stride < n_in || (row_stride & 3u) || row_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "row_stride must be at least n_in, at most 2^40 and a multiple of 4");
+    if (n_in > (1ull << 40) / interp) return h->fail(SB200_E_INVALID, "interp * n_in_samples must be at most 2^40");
+    if (n_in == 0) return SB200_OK;
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    CK(cudaSetDevice(h->device));
+    const bool in_dev = is_device_ptr(rows), out_dev = is_device_ptr(out);
+    if ((in_dev && ((uintptr_t)rows & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device rows and output must be 16-byte aligned");
+    CallScope call(h, st); CK(call.begin()); call.reads(rows);
+    const int nrc = upload_nco(h);
+    if (nrc != SB200_OK) return nrc;
+    const uint64_t n_out = interp * n_in;
+    const uint32_t* d_in = (const uint32_t*)rows; uint64_t d_stride = row_stride; uint32_t* d_out; Returns ret;
+    if (!in_dev) {                                     // rows n_in (rounded to 4) apart in the workspace
+        d_stride = (n_in + 3u) & ~3ull; CK(h->iq.need(nchannels * d_stride * 4ull + 16)); d_in = (const uint32_t*)h->iq.p;
+        CK(cudaMemcpy2DAsync(h->iq.p, d_stride * 4ull, rows, row_stride * 4ull, n_in * 4ull, nchannels, cudaMemcpyHostToDevice, st));
+    }
+    CK(ret.bind(h->iq40, (uint32_t*)out, n_out * 4ull, &d_out, 16));
+    ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
+    CbChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
+    for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; ch.gain[i] = channels[i].gain; }
+    int rc;
+    if (combine_smem(nchannels, interp, ntaps, 4 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, T, d_out);
+    else if (combine_smem(nchannels, interp, ntaps, 2 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, T, d_out);
+    else rc = combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, T, d_out);
     return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
 }
 
