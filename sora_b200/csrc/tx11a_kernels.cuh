@@ -126,6 +126,65 @@ __global__ void __launch_bounds__(128) k_tx11a_crc(const uint8_t* __restrict__ p
     crcs[f] = ~c;
 }
 
+// ---- the per-symbol bit path the OFDM modulators share (k_tx11a, k_tx11a_legacy, k_tx11n) ------------------------------------------------
+// even parity of the SIGNAL word into bit 17, folded over the word as the caller built it (a LENGTH of 4096 lands on the parity bit itself)
+__device__ __forceinline__ uint32_t sig_parity(uint32_t w) {
+    uint32_t p = w ^ (w >> 16); p ^= p >> 8; p ^= p >> 4; p ^= p >> 2; p ^= p >> 1;
+    return w | (p & 1u) << 17;
+}
+// data bits of the 802.11a SIGNAL symbol: six zero bits of encoder history, then the 24 bits of the word
+__device__ __forceinline__ void signal_bits(uint8_t* sd, uint32_t sig, int lane) {
+    if (lane < 30) sd[lane] = lane < 6 ? 0 : (uint8_t)((sig >> (lane - 6)) & 1u);
+}
+// scrambled data bits d[j], j in [n0 - 6, n0 + nd), into sd[0 .. nd + 6): byte 0, 1 the SERVICE field, then the payload up to byte
+// body_end, the FCS up to tail_at, the tail and the pad.  The scrambler is read as a 127-periodic sequence from `phase` (the seed's place in
+// it; 255 = the all-zero state, no scrambling); the six tail bits are not scrambled (TAIL_SCRAMBLE: code & 0xC0).  Bits at or past `limit`
+// are zero and not scrambled either (the FlushPort bytes of 802.11n).
+__device__ __forceinline__ void scrambled_bits(uint8_t* sd, uint32_t n0, uint32_t nd, const uint8_t* pl, uint32_t body_end, uint32_t tail_at,
+                                               uint32_t fcs, uint32_t phase, const DevTablesTx& X, int lane, uint32_t limit = 0xFFFFFFFFu) {
+    for (uint32_t i = lane; i < nd + 6u; i += 32) {
+        const int j = (int)n0 - 6 + (int)i;
+        uint32_t bit = 0;
+        if (j >= 0 && (uint32_t)j < limit) {
+            const uint32_t by = (uint32_t)j >> 3, bi = (uint32_t)j & 7u;
+            uint32_t raw = 0;
+            if (by >= 2u && by < body_end) raw = pl[by - 2u]; else if (by >= body_end && by < tail_at) raw = (fcs >> (8u * (by - body_end))) & 0xFFu;
+            const uint32_t scr = phase == 255u ? 0u : __ldg(X.scr_seq + (phase + (uint32_t)j) % 127u);
+            bit = ((raw >> bi) & 1u) ^ scr;
+            if (by == tail_at && bi < 6u) bit = 0;
+        }
+        sd[i] = (uint8_t)bit;
+    }
+}
+// coded bit k of a symbol (puncture pattern of TConvEncode_12/23/34), straight from its data bits; puncture groups never straddle a
+// symbol, so k is local to the symbol
+__device__ __forceinline__ uint32_t coded_bit(const uint8_t* sd, uint32_t cr, uint32_t k) {
+    uint32_t n, isb;
+    if (cr == CR_12) { n = k >> 1; isb = k & 1u; }
+    else if (cr == CR_34) { const uint32_t g = k >> 2, r = k & 3u; n = 3u * g + (r == 3u ? 2u : r >> 1); isb = (r == 1u || r == 3u); }
+    else { const uint32_t g = k / 3u, r = k - 3u * g; n = 2u * g + (r == 2u ? 1u : 0u); isb = r == 1u; }          // rate 2/3: A0 B0 A1 (conv_enc.hpp:102-188)
+    const uint8_t* d = sd + 6 + n;                      // d[0] = x, d[-1] = previous ...; generators 133 (A) and 171 (B) share taps 0, 2, 3, 6
+    return (d[0] ^ d[-2] ^ d[-3] ^ d[-6] ^ (isb ? d[-1] : d[-5])) & 1u;
+}
+// data carrier d (AddPilot order: -(hw + 2) .. -1, then 1 .. hw + 2, pilots skipped) to its slot of the zero-stuffed IFFT<128> input
+// (bins 32..63 move to 96..127); hw = 24 for 802.11a and the 802.11n SIG symbols, 26 for HT data
+__device__ __forceinline__ int carrier_slot(int d, int hw) {
+    int bin = d < hw ? 62 - hw + d : d - hw + 1;
+    if (d < hw) { if (bin >= 43) bin++; if (bin >= 57) bin++; } else { if (bin >= 7) bin++; if (bin >= 21) bin++; }
+    return bin < 32 ? bin : bin + 64;
+}
+// the pilots of carriers -21, -7, 7, 21 into their slots of the zero-stuffed IFFT<128> input
+__device__ __forceinline__ void put_pilots(uint32_t* xs, int m21, int m7, int p7, int p21) {
+    xs[43 + 64] = pack(mk(m21, 0)); xs[57 + 64] = pack(mk(m7, 0)); xs[7] = pack(mk(p7, 0)); xs[21] = pack(mk(p21, 0));
+}
+// T11aAddPilot (pilot.hpp:96-109) at amplitude a: polarity entry 127 for SIGNAL, then 0, 1, ... for the symbols behind it
+__device__ __forceinline__ void pilots11a(uint32_t* xs, const DevTables& T, uint32_t sym, int a) {
+    const int s = __ldg(T.pilot_neg + (sym == 0 ? 127u : (sym - 1u) % 127u)) ? -a : a;
+    put_pilots(xs, s, s, s, -s);
+}
+// time sample behind output sample i (0 .. 159) of a symbol: the last 32 samples go in front as the guard interval
+__device__ __forceinline__ uint32_t gi_sample(uint32_t i) { return i < 32u ? 96u + i : i - 32u; }
+
 #define SB_TX_WARPS 4
 __global__ void __launch_bounds__(32 * SB_TX_WARPS) k_tx11a(const uint8_t* __restrict__ payload, const uint64_t* __restrict__ pay_off, const uint32_t* __restrict__ pay_len,
         const uint8_t* __restrict__ seeds, uint32_t nframes, TxJob job, DevTables T, DevTablesTx X, const uint16_t* __restrict__ inv_deint,
@@ -160,45 +219,18 @@ __global__ void __launch_bounds__(32 * SB_TX_WARPS) k_tx11a(const uint8_t* __res
     const uint32_t nd = sym == 0 ? 24u : job.ndbps, nbpsc = sym == 0 ? 1u : job.nbpsc, cr = sym == 0 ? (uint32_t)CR_12 : job.code_rate;
     const uint32_t n0 = sym == 0 ? 0u : (sym - 1u) * job.ndbps;
     uint8_t* sd = s_d[wib];
-    if (sym == 0) {
-        uint32_t sig = job.rate_code | ((len + 4u) << 5);
-        uint32_t p = sig ^ (sig >> 16); p ^= p >> 8; p ^= p >> 4; p ^= p >> 2; p ^= p >> 1; sig |= (p & 1u) << 17;
-        if (lane < 30) sd[lane] = lane < 6 ? 0 : (uint8_t)((sig >> (lane - 6)) & 1u);
-    } else {
-        const uint8_t* pl = payload + pay_off[f];
-        const uint32_t seed = seeds ? seeds[f] : 0xFFu, phase = __ldg(X.scr_phase + (seed >> 1));
-        const uint32_t crc_at = 2u + len, tail_at = crc_at + 4u;
-        const uint32_t crc = __ldg(crcs + f);          // CF_11aTxVector::crc32, computed by k_tx11a_crc
-        for (uint32_t i = lane; i < nd + 6u; i += 32) {
-            const int j = (int)n0 - 6 + (int)i;
-            uint32_t bit = 0;
-            if (j >= 0) {
-                const uint32_t by = (uint32_t)j >> 3, bi = (uint32_t)j & 7u;
-                uint32_t raw = 0;
-                if (by >= 2u && by < crc_at) raw = pl[by - 2u]; else if (by >= crc_at && by < tail_at) raw = (crc >> (8u * (by - crc_at))) & 0xFFu;
-                const uint32_t scr = phase == 255u ? 0u : __ldg(X.scr_seq + (phase + (uint32_t)j) % 127u);
-                bit = ((raw >> bi) & 1u) ^ scr;
-                if (by == tail_at && bi < 6u) bit = 0;                                    // TAIL_SCRAMBLE: code & 0xC0
-            }
-            sd[i] = (uint8_t)bit;
-        }
+    if (sym == 0) signal_bits(sd, sig_parity(job.rate_code | ((len + 4u) << 5)), lane);
+    else {
+        const uint32_t seed = seeds ? seeds[f] : 0xFFu;
+        // the FCS is CF_11aTxVector::crc32, computed by k_tx11a_crc
+        scrambled_bits(sd, n0, nd, payload + pay_off[f], 2u + len, 6u + len, __ldg(crcs + f), __ldg(X.scr_phase + (seed >> 1)), X, lane);
     }
     __syncwarp();
-    // ---- coded bit k of this symbol (puncture pattern of TConvEncode_12/23/34), straight from the data bits -----------------
-    auto coded = [&](uint32_t k) -> uint32_t {
-        uint32_t n, isb;
-        if (cr == CR_12) { n = k >> 1; isb = k & 1u; }
-        else if (cr == CR_34) { const uint32_t g = k >> 2, r = k & 3u; n = 3u * g + (r == 3u ? 2u : r >> 1); isb = (r == 1u || r == 3u); }
-        else { const uint32_t g = k / 3u, r = k - 3u * g; n = 2u * g + (r == 2u ? 1u : 0u); isb = r == 1u; }
-        const uint8_t* d = sd + 6 + n;                  // d[0] = x, d[-1] = previous ...
-        return isb ? (d[0] ^ d[-1] ^ d[-2] ^ d[-3] ^ d[-6]) & 1u : (d[0] ^ d[-2] ^ d[-3] ^ d[-5] ^ d[-6]) & 1u;
-    };
-    // puncture groups never straddle a symbol at these rates, so coded index k is local to the symbol
     const uint16_t* inv = inv_deint + (nbpsc == 1 ? 0 : nbpsc == 2 ? 48 : nbpsc == 4 ? 144 : 336);     // air position -> coded index
     const int km = nbpsc == 1 ? 10720 : nbpsc == 2 ? (int)(short)(10720 / 1.414) : nbpsc == 4 ? (int)(short)(10720 / 3.162) : (int)(short)(10720 / 6.481);
     auto level = [&](uint32_t p0, uint32_t m) -> int {   // InitQamMapLut (mapper11a.hpp:17-46): first bit is the Gray MSB
         uint32_t bin = 0, acc = 0;
-        for (uint32_t i = 0; i < m; i++) { acc ^= coded(__ldg(inv + p0 + i)); bin = (bin << 1) | acc; }
+        for (uint32_t i = 0; i < m; i++) { acc ^= coded_bit(sd, cr, __ldg(inv + p0 + i)); bin = (bin << 1) | acc; }
         return (2 * (int)bin - ((1 << m) - 1)) * km;
     };
     uint32_t* xs = s_x[wib];
@@ -208,25 +240,18 @@ __global__ void __launch_bounds__(32 * SB_TX_WARPS) k_tx11a(const uint8_t* __res
     for (int w = 0; w < 2; w++) {                       // lanes 0..23 place data carriers d = lane and lane + 24 (T11aAddPilot order: -26..-1, 1..26)
         const int dd = lane + 24 * w;
         if (lane < 24) {
-            int bin = dd < 24 ? 38 + dd : dd - 24 + 1;  // skip the pilot bins
-            if (dd < 24) { if (bin >= 43) bin++; if (bin >= 57) bin++; } else { if (bin >= 7) bin++; if (bin >= 21) bin++; }
             cs16 c;
-            if (nbpsc == 1) c = mk(coded(__ldg(inv + dd)) ? 10720 : -10720, 0);
+            if (nbpsc == 1) c = mk(coded_bit(sd, cr, __ldg(inv + dd)) ? 10720 : -10720, 0);
             else { const uint32_t h = nbpsc >> 1; c = mk(level((uint32_t)dd * nbpsc, h), level((uint32_t)dd * nbpsc + h, h)); }
-            xs[bin < 32 ? bin : bin + 64] = pack(c);    // TIFFTx zero-stuffing: bins 32..63 move to 96..127
+            xs[carrier_slot(dd, 24)] = pack(c);
         }
     }
-    if (lane == 24) {                                   // pilots (pilot.hpp:96-109): index 127 for SIGNAL, then 0, 1, ...
-        const uint32_t pi = sym == 0 ? 127u : (sym - 1u) % 127u;
-        const int s = __ldg(T.pilot_neg + pi) ? -10720 : 10720;
-        xs[7] = pack(mk(s, 0)); xs[21] = pack(mk(-s, 0)); xs[57 + 64] = pack(mk(s, 0)); xs[43 + 64] = pack(mk(s, 0));
-    }
+    if (lane == 24) pilots11a(xs, T, sym, 10720);
     warp_ifft128(xs, X, lane);
     // ---- >> 4, guard interval, window, pack, store (fft.hpp:27-41) ----------------------------------------------------------
     const uint32_t base = job.lead + 640u + 160u * sym;
     for (uint32_t i = lane; i < 160u; i += 32) {
-        const uint32_t t = i < 32u ? 96u + i : i - 32u;
-        cs16 c = sra(unpack(xs[rev7((int)t)]), 4);
+        cs16 c = sra(unpack(xs[rev7((int)gi_sample(i))]), 4);
         if (i < 2u || i >= 158u) c = sra(c, 1);
         put(base + i, c);
     }

@@ -100,39 +100,14 @@ __global__ void __launch_bounds__(32 * SB_TXL_WARPS) k_tx11a_legacy(const uint8_
         const uint32_t nd = sym == 0 ? 24u : job.ndbps, nbpsc = sym == 0 ? 1u : job.nbpsc, cr = sym == 0 ? (uint32_t)CR_12 : job.code_rate;
         const uint32_t n0 = sym == 0 ? 0u : (sym - 1u) * job.ndbps;
         __syncwarp();
-        if (sym == 0) {                                                 // GetSignal (atx.h:78-97): LENGTH 4096 lands on the parity bit
-            uint32_t sg = job.rate_code | (L << 5);
-            uint32_t p = sg ^ (sg >> 16); p ^= p >> 8; p ^= p >> 4; p ^= p >> 2; p ^= p >> 1; sg |= (p & 1u) << 17;
-            if (lane < 30) sd[lane] = lane < 6 ? 0 : (uint8_t)((sg >> (lane - 6)) & 1u);
-        } else {
-            const uint32_t body_end = 2u + len, tail_at = 2u + L;
-            for (uint32_t i = lane; i < nd + 6u; i += 32) {
-                const int j = (int)n0 - 6 + (int)i;
-                uint32_t bit = 0;
-                if (j >= 0) {
-                    const uint32_t by = (uint32_t)j >> 3, bi = (uint32_t)j & 7u;
-                    uint32_t raw = 0;
-                    if (by >= 2u && by < body_end) raw = pl[by - 2u]; else if (by >= body_end && by < tail_at) raw = (crc >> (8u * (by - body_end))) & 0xFFu;
-                    bit = ((raw >> bi) & 1u) ^ __ldg(X.scr_seq + (phase + (uint32_t)j) % 127u);
-                    if (by == tail_at && bi < 6u) bit = 0;                                  // the six tail bits, not scrambled (atx_tpl.h:52)
-                }
-                sd[i] = (uint8_t)bit;
-            }
-        }
+        if (sym == 0) signal_bits(sd, sig_parity(job.rate_code | (L << 5)), lane);        // GetSignal (atx.h:78-97): LENGTH 4096 lands on the parity bit
+        else scrambled_bits(sd, n0, nd, pl, 2u + len, 2u + L, crc, phase, X, lane);          // the six tail bits, not scrambled (atx_tpl.h:52)
         __syncwarp();
-        auto coded = [&](uint32_t k) -> uint32_t {                     // puncturing of the rate-1/2 mother code, straight from the data bits
-            uint32_t n, isb;
-            if (cr == CR_12) { n = k >> 1; isb = k & 1u; }
-            else if (cr == CR_34) { const uint32_t g = k >> 2, r = k & 3u; n = 3u * g + (r == 3u ? 2u : r >> 1); isb = (r == 1u || r == 3u); }
-            else { const uint32_t g = k / 3u, r = k - 3u * g; n = 2u * g + (r == 2u ? 1u : 0u); isb = r == 1u; }
-            const uint8_t* d = sd + 6 + n;
-            return isb ? (d[0] ^ d[-1] ^ d[-2] ^ d[-3] ^ d[-6]) & 1u : (d[0] ^ d[-2] ^ d[-3] ^ d[-5] ^ d[-6]) & 1u;
-        };
         const uint16_t* iv = sym == 0 ? inv_deint : inv;
         const int lev0 = nbpsc == 2 ? 0 : nbpsc == 4 ? 2 : 6;
         auto level = [&](uint32_t p0, uint32_t m) -> int {             // Gray-decoded bin, first bit on air = most significant
             uint32_t bin = 0, acc = 0;
-            for (uint32_t i = 0; i < m; i++) { acc ^= coded(__ldg(iv + p0 + i)); bin = (bin << 1) | acc; }
+            for (uint32_t i = 0; i < m; i++) { acc ^= coded_bit(sd, cr, __ldg(iv + p0 + i)); bin = (bin << 1) | acc; }
             return c_txl_lev[lev0 + bin];
         };
         for (int i = lane; i < 128; i += 32) xs[i] = 0;
@@ -141,19 +116,13 @@ __global__ void __launch_bounds__(32 * SB_TXL_WARPS) k_tx11a_legacy(const uint8_
         for (int h = 0; h < 2; h++) {                                   // AddPilot's carrier order: -26..-1, then 1..26
             const int dd = lane + 24 * h;
             if (lane < 24) {
-                int bin = dd < 24 ? 38 + dd : dd - 24 + 1;
-                if (dd < 24) { if (bin >= 43) bin++; if (bin >= 57) bin++; } else { if (bin >= 7) bin++; if (bin >= 21) bin++; }
                 cs16 c;
-                if (nbpsc == 1) c = mk(coded(__ldg(iv + dd)) ? 10720 : -10720, 0);
+                if (nbpsc == 1) c = mk(coded_bit(sd, cr, __ldg(iv + dd)) ? 10720 : -10720, 0);
                 else { const uint32_t hb = nbpsc >> 1; c = mk(level((uint32_t)dd * nbpsc, hb), level((uint32_t)dd * nbpsc + hb, hb)); }
-                xs[bin < 32 ? bin : bin + 64] = pack(c);                // IFFT64x zero stuffing: bins 32..63 move to 96..127
+                xs[carrier_slot(dd, 24)] = pack(c);
             }
         }
-        if (lane == 24) {
-            const uint32_t pi = sym == 0 ? 127u : (sym - 1u) % 127u;
-            const int s = __ldg(T.pilot_neg + pi) ? -10720 : 10720;
-            xs[7] = pack(mk(s, 0)); xs[21] = pack(mk(-s, 0)); xs[57 + 64] = pack(mk(s, 0)); xs[43 + 64] = pack(mk(s, 0));
-        }
+        if (lane == 24) pilots11a(xs, T, sym, 10720);
         warp_ifft128(xs, X, lane);
     };
     auto raw = [&](int t) { const cs16 v = unpack(xs[rev7(t)]); return mk(sx16(v.re << 2), sx16(v.im << 2)); };   // psllw 2, wraps
@@ -166,7 +135,7 @@ __global__ void __launch_bounds__(32 * SB_TXL_WARPS) k_tx11a_legacy(const uint8_
     for (uint32_t sym = s_first; sym <= s_last; sym++) {
         ifft_symbol(sym);
         for (int i = lane; i < 160; i += 32) {                          // CopyGI + Window
-            cs16 v = raw(i < 32 ? 96 + i : i - 32);
+            cs16 v = raw((int)gi_sample(i));
             if (i < 4) {
                 if (i == 0) v = sra(v, 2); else if (i == 1) v = sra(v, 1); else if (i == 2) v = mk(sx16(v.re - (v.re >> 2)), sx16(v.im - (v.im >> 2)));
                 const cs16 l = i == 0 ? last0 : i == 1 ? last1 : i == 2 ? last2 : mk(0, 0);

@@ -35,22 +35,38 @@ __device__ __forceinline__ unsigned q_of_dqpsk(unsigned i) { return (0x9Cu >> (2
 __device__ __forceinline__ unsigned dqpsk_of_q(unsigned q) { return (0x78u >> (2u * (q & 3u))) & 3u; }      // 0,2,3,1
 __device__ __forceinline__ unsigned q_of_cck11(unsigned i) { return (0xD8u >> (2u * (i & 3u))) & 3u; }      // 0,2,1,3
 
+// PLCP header of a PSDU of `size` bytes (PHY_11b.hpp:82-136, PLCPGetLength in bbb_tx.c:39-65): SIGNAL, SERVICE (length extension in
+// bit 7), LENGTH in microseconds, CRC-16 (CalcCRC16, core/inc/CRC16.h:37-48)
+__device__ __forceinline__ void tx11b_plcp_header(uint8_t (&hdr)[6], uint32_t rate_kbps, uint32_t rate_code, uint32_t size) {
+    uint32_t plen, ext = 0;
+    if (rate_kbps == 1000) plen = size << 3;
+    else if (rate_kbps == 2000) plen = size << 2;
+    else if (rate_kbps == 5500) plen = ((size << 4) - 1u) / 11u + 1u;
+    else { plen = ((size << 3) - 1u) / 11u + 1u; if (plen * 11u - (size << 3) >= 8u) ext = 1; }
+    hdr[0] = (uint8_t)rate_code; hdr[1] = (uint8_t)(ext << 7); hdr[2] = (uint8_t)plen; hdr[3] = (uint8_t)(plen >> 8);
+    unsigned c = 0xFFFFu;
+    for (int i = 0; i < 4; i++) { c ^= hdr[i]; for (int k = 0; k < 8; k++) c = (c & 1u) ? (c >> 1) ^ 0x8408u : c >> 1; }
+    c = ~c & 0xFFFFu; hdr[4] = (uint8_t)c; hdr[5] = (uint8_t)(c >> 8);
+}
+// byte b through the self-synchronising 7-4-1 scrambler (TSc741, gc_ScramblerLUT[b][reg]): o_k = x_k ^ s_k ^ s_(k+3) where the 4-ago tap
+// is still old state (k < 4), then the taps that already see new output bits; reg moves on to the byte's last seven output bits
+__device__ __forceinline__ unsigned tx11b_scramble(unsigned b, unsigned& reg) {
+    const unsigned lo = (b ^ reg ^ (reg >> 3)) & 0xFu;
+    const unsigned mid = ((b >> 4) ^ (reg >> 4) ^ lo) & 0x7u;
+    const unsigned top = ((b >> 7) ^ lo ^ (lo >> 3)) & 1u;
+    const unsigned sb = lo | (mid << 4) | (top << 7);
+    reg = sb >> 1;
+    return sb;
+}
+
 __global__ void __launch_bounds__(128) k_tx11b_code(const uint8_t* __restrict__ payload, const uint64_t* __restrict__ pay_off, const uint32_t* __restrict__ pay_len,
                                                     uint32_t nframes, Tx11bJob job, const uint32_t* __restrict__ crcs, uint16_t* __restrict__ desc, uint32_t* __restrict__ final_phase) {
     const uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= nframes) return;
     const uint8_t* p = payload + pay_off[f]; const uint32_t len = pay_len[f], size = len + 4u;
     uint16_t* d = desc + (size_t)f * job.desc_stride;
-    // PLCP header (PHY_11b.hpp:82-136): SIGNAL, SERVICE (length extension in bit 7), LENGTH in microseconds, CRC-16
-    uint32_t plen, ext = 0;
-    if (job.rate_kbps == 1000) plen = size << 3;
-    else if (job.rate_kbps == 2000) plen = size << 2;
-    else if (job.rate_kbps == 5500) plen = ((size << 4) - 1u) / 11u + 1u;
-    else { plen = ((size << 3) - 1u) / 11u + 1u; if (plen * 11u - (size << 3) >= 8u) ext = 1; }
-    uint8_t hdr[6] = {(uint8_t)job.rate_code, (uint8_t)(ext << 7), (uint8_t)plen, (uint8_t)(plen >> 8), 0, 0};
-    {   unsigned c = 0xFFFFu;                                                           // CalcCRC16 (core/inc/CRC16.h:37-48)
-        for (int i = 0; i < 4; i++) { c ^= hdr[i]; for (int k = 0; k < 8; k++) c = (c & 1u) ? (c >> 1) ^ 0x8408u : c >> 1; }
-        c = ~c & 0xFFFFu; hdr[4] = (uint8_t)c; hdr[5] = (uint8_t)(c >> 8); }
+    uint8_t hdr[6];
+    tx11b_plcp_header(hdr, job.rate_kbps, job.rate_code, size);
     const uint32_t fcs = crcs[f];
     unsigned reg = 0x6C;                                                                // DOT11B_PLCP_LONG_TX_SCRAMBLER_REGISTER
     unsigned ref = job.init_phase & 3u, odd = 0;
@@ -61,12 +77,7 @@ __global__ void __launch_bounds__(128) k_tx11b_code(const uint8_t* __restrict__ 
         else if (i < 24u) b = hdr[i - 18u];
         else if (i < 24u + len) b = p[i - 24u];
         else b = (fcs >> (8u * (i - 24u - len))) & 0xFFu;
-        // TSc741: o_k = x_k ^ s_k ^ s_(k+3) where the 4-ago tap is still old state (k < 4), then the taps that already see new output bits
-        const unsigned lo = (b ^ reg ^ (reg >> 3)) & 0xFu;
-        const unsigned mid = ((b >> 4) ^ (reg >> 4) ^ lo) & 0x7u;
-        const unsigned top = ((b >> 7) ^ lo ^ (lo >> 3)) & 1u;
-        const unsigned sb = lo | (mid << 4) | (top << 7);
-        reg = sb >> 1;
+        const unsigned sb = tx11b_scramble(b, reg);
         unsigned word;
         if (i < 24u || job.rate_kbps == 1000) {                                         // DBPSK: running parity of the bits, from the reference phase
             unsigned c = sb; c ^= c << 1; c ^= c << 2; c ^= c << 4; c &= 0xFFu;

@@ -13,8 +13,7 @@
 //     before p - 9 (instead of +x[2] of group p - 9);
 //   variant 1 (FIR37SSE_INLINE, bbb_fir.c:137-386): the plain filter.
 #pragma once
-#include <cstdint>
-#include <cuda_runtime.h>
+#include "tx11b_kernels.cuh"
 
 namespace sb {
 
@@ -119,15 +118,8 @@ __global__ void __launch_bounds__(128) k_tx11b_legacy_code(const uint8_t* __rest
     const uint8_t* p = payload + pay_off[f];
     const uint32_t len = job.fcs_in_payload ? pay_len[f] - 4u : pay_len[f], size = len + 4u;   // MPDU bytes, PSDU bytes (FCS included)
     uint16_t* d = desc + (size_t)f * job.desc_stride;
-    uint32_t plen, ext = 0;                                                             // PLCPGetLength (bbb_tx.c:39-65), CCK
-    if (job.rate_kbps == 1000) plen = size << 3;
-    else if (job.rate_kbps == 2000) plen = size << 2;
-    else if (job.rate_kbps == 5500) plen = ((size << 4) - 1u) / 11u + 1u;
-    else { plen = ((size << 3) - 1u) / 11u + 1u; if (plen * 11u - (size << 3) >= 8u) ext = 1; }
-    uint8_t hdr[6] = {(uint8_t)job.rate_code, (uint8_t)(ext << 7), (uint8_t)plen, (uint8_t)(plen >> 8), 0, 0};
-    {   unsigned c = 0xFFFFu;                                                           // CalcCRC16 (core/inc/CRC16.h)
-        for (int i = 0; i < 4; i++) { c ^= hdr[i]; for (int k = 0; k < 8; k++) c = (c & 1u) ? (c >> 1) ^ 0x8408u : c >> 1; }
-        c = ~c & 0xFFFFu; hdr[4] = (uint8_t)c; hdr[5] = (uint8_t)(c >> 8); }
+    uint8_t hdr[6];
+    tx11b_plcp_header(hdr, job.rate_kbps, job.rate_code, size);
     const uint32_t fcs = crcs ? crcs[f] : 0u;
     const uint32_t plcp = tx11b_legacy_plcp_bytes(job.short_preamble), nsync = job.short_preamble ? 7u : 16u;
     const uint32_t n_dbpsk = job.short_preamble ? 9u : (job.rate_kbps == 1000 ? plcp + size : plcp);
@@ -142,12 +134,7 @@ __global__ void __launch_bounds__(128) k_tx11b_legacy_code(const uint8_t* __rest
         else if (i < plcp) b = hdr[i - nsync - 2u];
         else if (i < plcp + len || job.fcs_in_payload) b = p[i - plcp];
         else b = (fcs >> (8u * (i - plcp - len))) & 0xFFu;
-        // gc_ScramblerLUT[b][reg]: o_k = x_k ^ s_k ^ s_(k+3), the register reading output bits once they exist
-        const unsigned lo = (b ^ reg ^ (reg >> 3)) & 0xFu;
-        const unsigned mid = ((b >> 4) ^ (reg >> 4) ^ lo) & 0x7u;
-        const unsigned top = ((b >> 7) ^ lo ^ (lo >> 3)) & 1u;
-        const unsigned sb = lo | (mid << 4) | (top << 7);
-        reg = sb >> 1;
+        const unsigned sb = tx11b_scramble(b, reg);
         d[i] = (uint16_t)(sb | (q << 8) | (odd << 10));
         if (i < n_dbpsk) {                                                              // DBPSK: pi per one bit
             unsigned par = sb; par ^= par >> 4; par ^= par >> 2; par ^= par >> 1;

@@ -74,7 +74,7 @@ __global__ void __launch_bounds__(32 * SB_TX11N_WARPS) k_tx11n(const uint8_t* __
     if (sig) {
         // ---- L-SIG (6 Mbps, length that spans the HT part) + HT-SIG (MCS, length, CRC-8): 72 bits, PHY_11n.hpp:244-281 ----------------------
         const uint32_t nsym_all = ns_sig + 5u, lsig_len = (nsym_all * 24u - 16u - 6u) / 8u;
-        uint32_t lsig = 0xBu | (lsig_len << 5); uint32_t p = lsig ^ (lsig >> 16); p ^= p >> 8; p ^= p >> 4; p ^= p >> 2; p ^= p >> 1; lsig |= (p & 1u) << 17;
+        const uint32_t lsig = sig_parity(0xBu | (lsig_len << 5));
         const uint32_t L4 = len + 4u;
         const uint32_t h0 = job.mcs | ((L4 & 0xFFFFu) << 8) | (3u << 24);                           // _b_htsig.h:49-53: mcs, length, smoothing | not sounding
         unsigned c = 0xFF;                                                                          // CalcCRC8 over 4 bytes and 2 tail bits (CRC8.h:28-50)
@@ -91,36 +91,16 @@ __global__ void __launch_bounds__(32 * SB_TX11N_WARPS) k_tx11n(const uint8_t* __
         }
     } else {
         // ---- scrambled data bits d[j], j in [n0 - 6, n0 + N_DBPS): TBB11nSrc through T11aSc, then the FlushPort zero bytes ---------------------
-        const uint32_t n0 = (sym - 3u) * job.ndbps;
-        const uint8_t* pl = payload + pay_off[f];
-        const uint32_t seed = seeds ? seeds[f] : 0xABu, phase = __ldg(X.scr_phase + (seed >> 1));   // fb11nmod_config.hpp:52
-        const uint32_t crc_at = 2u + len, tail_at = crc_at + 4u, src_bits = (ns_sig * job.ndbps + 7u) / 8u * 8u;
-        const uint32_t crc = __ldg(crcs + f);
-        for (uint32_t i = lane; i < job.ndbps + 6u; i += 32) {
-            const int j = (int)n0 - 6 + (int)i;
-            uint32_t bit = 0;
-            if (j >= 0 && (uint32_t)j < src_bits) {
-                const uint32_t by = (uint32_t)j >> 3, bi = (uint32_t)j & 7u;
-                uint32_t raw = 0;
-                if (by >= 2u && by < crc_at) raw = pl[by - 2u]; else if (by >= crc_at && by < tail_at) raw = (crc >> (8u * (by - crc_at))) & 0xFFu;
-                const uint32_t scr = phase == 255u ? 0u : __ldg(X.scr_seq + (phase + (uint32_t)j) % 127u);
-                bit = ((raw >> bi) & 1u) ^ scr;
-                if (by == tail_at && bi < 6u) bit = 0;                                    // TAIL_SCRAMBLE: code & 0xC0
-            }
-            sd[i] = (uint8_t)bit;
-        }
+        const uint32_t seed = seeds ? seeds[f] : 0xABu;                                             // fb11nmod_config.hpp:52
+        scrambled_bits(sd, (sym - 3u) * job.ndbps, job.ndbps, payload + pay_off[f], 2u + len, 6u + len, __ldg(crcs + f), __ldg(X.scr_phase + (seed >> 1)),
+                       X, lane, (ns_sig * job.ndbps + 7u) / 8u * 8u);
     }
     __syncwarp();
     const uint32_t cr = sig ? (uint32_t)CR_12 : job.code_rate;
     const uint32_t cbase = sig ? 0u : (sym - 3u) * 104u * job.nbpsc;                     // index of this symbol's first coded bit in the frame
-    auto coded = [&](uint32_t k) -> uint32_t {           // coded bit k of this symbol (both streams' bits interleaved), as in k_tx11a
+    auto coded = [&](uint32_t k) -> uint32_t {           // coded bit k of this symbol (both streams' bits interleaved)
         if (!sig && cbase + k >= coded_bits) return 0u;  // behind the encoder's last burst: the stream parser's pad bytes
-        uint32_t n, isb;
-        if (cr == CR_12) { n = k >> 1; isb = k & 1u; }
-        else if (cr == CR_34) { const uint32_t g = k >> 2, r = k & 3u; n = 3u * g + (r == 3u ? 2u : r >> 1); isb = (r == 1u || r == 3u); }
-        else { const uint32_t g = k / 3u, r = k - 3u * g; n = 2u * g + (r == 2u ? 1u : 0u); isb = r == 1u; }          // rate 2/3: A0 B0 A1 (conv_enc.hpp:102-188)
-        const uint8_t* d = sd + 6 + n;
-        return isb ? (d[0] ^ d[-1] ^ d[-2] ^ d[-3] ^ d[-6]) & 1u : (d[0] ^ d[-2] ^ d[-3] ^ d[-5] ^ d[-6]) & 1u;
+        return coded_bit(sd, cr, k);
     };
     if (sig) {
         // T11aInterleaveBPSK + TSigMap11n (L-SIG on I, HT-SIG on Q, +-30339) + T11aAddPilot<30339> (index 127, 0, 1)
@@ -128,17 +108,11 @@ __global__ void __launch_bounds__(32 * SB_TX11N_WARPS) k_tx11n(const uint8_t* __
         for (int w = 0; w < 2; w++) {
             const int dd = lane + 24 * w;
             if (lane < 24) {
-                int bin = dd < 24 ? 38 + dd : dd - 24 + 1;
-                if (dd < 24) { if (bin >= 43) bin++; if (bin >= 57) bin++; } else { if (bin >= 7) bin++; if (bin >= 21) bin++; }
                 const int v = coded(__ldg(inv_deint + dd)) ? 30339 : -30339;
-                xs[bin < 32 ? bin : bin + 64] = pack(sym == 0 ? mk(v, 0) : mk(0, v));
+                xs[carrier_slot(dd, 24)] = pack(sym == 0 ? mk(v, 0) : mk(0, v));
             }
         }
-        if (lane == 24) {
-            const uint32_t pi = sym == 0 ? 127u : sym - 1u;
-            const int s = __ldg(T.pilot_neg + pi) ? -30339 : 30339;
-            xs[7] = pack(mk(s, 0)); xs[21] = pack(mk(-s, 0)); xs[57 + 64] = pack(mk(s, 0)); xs[43 + 64] = pack(mk(s, 0));
-        }
+        if (lane == 24) pilots11a(xs, T, sym, 30339);
     } else {
         // stream parser (even coded bits -> stream 1, odd -> stream 2) + T11nInterleave*_S1/_S2 + mapper + T11nAddPilot<iss>
         const uint8_t* inv = N.inv + ((job.nbpsc == 1 ? 0 : 2) + iss) * 104;
@@ -146,8 +120,6 @@ __global__ void __launch_bounds__(32 * SB_TX11N_WARPS) k_tx11n(const uint8_t* __
         for (int w = 0; w < 2; w++) {
             const int dd = lane + 26 * w;               // data carrier 0..51 in T11nAddPilot order: -28..-1 then 1..28
             if (lane < 26) {
-                int bin = dd < 26 ? 36 + dd : dd - 26 + 1;
-                if (dd < 26) { if (bin >= 43) bin++; if (bin >= 57) bin++; } else { if (bin >= 7) bin++; if (bin >= 21) bin++; }
                 cs16 c;
                 if (job.nbpsc == 1) c = mk(coded(2u * __ldg(inv + dd) + iss) ? 30339 : -30339, 0);
                 else if (job.nbpsc == 2) c = mk(coded(2u * __ldg(inv + 2 * dd) + iss) ? 21453 : -21453, coded(2u * __ldg(inv + 2 * dd + 1) + iss) ? 21453 : -21453);
@@ -164,7 +136,7 @@ __global__ void __launch_bounds__(32 * SB_TX11N_WARPS) k_tx11n(const uint8_t* __
                     }
                     c = mk(lv[0], lv[1]);
                 }
-                xs[bin < 32 ? bin : bin + 64] = pack(c);
+                xs[carrier_slot(dd, 26)] = pack(c);
             }
         }
         if (lane == 26) {                               // _b_dot11_pilot.h:7-35: polarity entry (n + 3) % 127, pattern row n & 3
@@ -173,8 +145,7 @@ __global__ void __launch_bounds__(32 * SB_TX11N_WARPS) k_tx11n(const uint8_t* __
             // rows {1,1,-1,-1},{1,-1,-1,1} | {1,-1,-1,1},{-1,-1,1,1} | {-1,-1,1,1},{-1,1,1,-1} | {-1,1,1,-1},{1,1,-1,-1}: bit set = minus, carrier order -21, -7, 7, 21
             const unsigned NEGS = 0xC993366Cu;                  // nibble (row * 2 + stream), low one first: bits 0..3 = the four carriers
             const unsigned nib = (NEGS >> (4u * ((n & 3u) * 2u + iss))) & 0xFu;
-            xs[43 + 64] = pack(mk((nib & 1u) ? -s : s, 0)); xs[57 + 64] = pack(mk((nib & 2u) ? -s : s, 0));
-            xs[7] = pack(mk((nib & 4u) ? -s : s, 0)); xs[21] = pack(mk((nib & 8u) ? -s : s, 0));
+            put_pilots(xs, (nib & 1u) ? -s : s, (nib & 2u) ? -s : s, (nib & 4u) ? -s : s, (nib & 8u) ? -s : s);
         }
     }
     warp_ifft128(xs, X, lane);
@@ -183,13 +154,13 @@ __global__ void __launch_bounds__(32 * SB_TX11N_WARPS) k_tx11n(const uint8_t* __
     const uint32_t base = job.lead + 640u + (sig ? 160u * sym : 480u + 480u + 160u * (sym - 3u));
     if (sig && iss == 0) {                              // one spectrum, two antennas: the first stream's warp writes both
         for (uint32_t i = lane; i < 160u; i += 32) {
-            const uint32_t t = i < 32u ? 96u + i : i - 32u;
+            const uint32_t t = gi_sample(i);
             outs[0][base + i] = xs[rev7((int)t)];
             outs[1][base + i] = xs[rev7((int)((t + 128u - 8u) & 127u))];
         }
     } else if (!sig) {
         for (uint32_t i = lane; i < 160u; i += 32) {
-            const uint32_t t = i < 32u ? 96u + i : i - 32u;
+            const uint32_t t = gi_sample(i);
             outs[iss][base + i] = xs[rev7((int)((t + 128u - shift) & 127u))];
         }
     }
