@@ -4,7 +4,7 @@
 //                state machine, up to the vector where the reference switches to the demod branch.
 //                Reference: samples.hpp:27-49 (TDownSample2), dc.hpp:48-166, cca.hpp:106-441 (TCCA11a),
 //                fb11a_demod.cpp:29-81 (per-28-sample-block error polling, CS-timeout reset).
-//   k_front11a   one warp per slot: LTS (fine CFO, FFT, channel estimate), then per OFDM symbol
+//   k_front11a   one half-warp per slot: LTS (fine CFO, FFT, channel estimate), then per OFDM symbol
 //                CP strip -> freq comp -> FFT64 -> equalise -> phase comp -> pilot track -> soft demap ->
 //                de-interleave; SIGNAL decoded in-warp (K=7 Viterbi, 24 steps) and parsed.  Samples stay packed complex
 //                int16 words from the load through the FFT to the demapper (pk_* in fixed.cuh, bit-exact to the scalar forms);
@@ -227,7 +227,7 @@ __device__ __forceinline__ uint32_t warp_viterbi_signal(const uint8_t* soft, uin
 }
 
 // ------------------------------------------------------------------------------------------------
-// front end: one warp per slot
+// front end: one half-warp per slot
 // ------------------------------------------------------------------------------------------------
 struct FrontTaps {            // optional stage taps (device pointers, nullptr = off); per slot, per symbol, 64 packed c16
     uint32_t* freq_coeffs; uint32_t* chan_coeffs; uint32_t* fft_out; uint32_t* equalized; uint32_t* tracked; uint32_t max_sym;
@@ -242,67 +242,74 @@ __device__ __forceinline__ int data_index(int bin) {   // demapper11a.hpp:22-36 
 __device__ __forceinline__ int data_bin(int d) {       // inverse of data_index, d = 0..47
     return d < 24 ? 38 + d + (d >= 5) + (d >= 18) : d - 23 + (d >= 30) + (d >= 43);
 }
+// Post-FFT role of lane hl of a half-warp: four bins.  Lanes 0-11 own the data-subcarrier pairs (d, d + 3), d = 6 (p / 3) + p % 3 for
+// p = hl (bins 0, 1) and p = hl + 12 (bins 2, 3), in demapper order: at 64-QAM the 802.11a de-interleaver puts coded bit i of d at an even
+// position and bit (2 0 1 5 3 4)[i] of d + 3 right after it, so a pair's soft bits leave as six 16-bit stores.  Lanes 12-15 own one pilot
+// each in bin 0 (43, 57, 7, 21) and three of the twelve zero bins (0, 27..37) in bins 1-3.
+__device__ __forceinline__ int front_pair(int hl, int p) { const int q = hl + 12 * p; return 6 * (q / 3) + q % 3; }
+__device__ __forceinline__ int front_bin(int hl, int i) {
+    if (hl < 12) return data_bin(front_pair(hl, i >> 1) + 3 * (i & 1));
+    const int j = hl - 12, m = 3 * j + i - 1;
+    return i == 0 ? (0x1507392B >> (8 * j)) & 0xFF : m ? 26 + m : 0;
+}
 
 #define SB_FRONT_WARPS 4
+#define SB_FRONT_SLOTS (2 * SB_FRONT_WARPS)   // capture slots per CTA, one per half-warp
 #ifndef SB_FRONT_MINB
-#define SB_FRONT_MINB 5           // resident CTAs per SM the register allocation aims at; front end on the H100 (tools/front_sweep.sh, DESIGN.md §8):
-                                  // 4 -> 2.50 ms (123 registers), 5 -> 2.32 ms (96), 6 -> 2.83 ms (80 registers, 184 B of spill stores)
+#define SB_FRONT_MINB 5           // resident CTAs per SM the register allocation aims at (tools/front_sweep.sh, DESIGN.md §8)
 #endif
-// Two OFDM symbols are transformed at once: lanes 0-15 run the three radix stages of symbol A, lanes 16-31 those of
-// symbol B (16 butterflies per stage = 16 lanes, so every lane is busy); the first stage consumes the freq-compensated
-// time samples straight from registers.  Only the part behind the FFT (phase compensation from the pilot recurrence)
-// is serial across symbols, and there every lane owns two subcarriers.
-// STAGE: how the time samples of the DATA symbols reach the FFT (A/B of the staging experiment, DESIGN.md §4):
+// Each half-warp decodes its own slot, and both run the same instruction stream: lanes 0-15 slot 2 w, lanes 16-31 slot 2 w + 1 of warp w.
+// Per OFDM symbol a half runs the three radix stages of its slot's 64-point FFT (16 butterflies per stage = 16 lanes), the first stage
+// straight from the freq-compensated time samples in registers; behind the FFT each lane owns four bins (front_bin), and the work that
+// does not grow with the bins a lane owns (pilot angle walk, tracker, control) serves both slots at once.  A half whose slot ended, failed
+// its header or held no frame idles in the loop with the other one, so every full-mask shuffle and __syncwarp still sees all 32 lanes.
+// STAGE: how the time samples of the symbols reach the FFT (A/B of the staging experiment, DESIGN.md §4):
 //   0  loaded straight into registers right before the transform (round 1);
-//   1  the next symbol pair's samples are loaded into registers while the current pair is processed (register double buffer);
-//   2  one lane starts a 1-D bulk asynchronous copy (cp.async.bulk, the TMA unit; SASS UBLKCP) of the next pair's span into a shared-memory
-//      double buffer, completion on an mbarrier; the lanes then read their samples from shared memory.
+//   1  the next symbol's samples are loaded into registers while the current one is processed (register double buffer);
+//   2  one lane of each half starts a 1-D bulk asynchronous copy (cp.async.bulk, the TMA unit; SASS UBLKCP) of its slot's next symbol into a
+//      shared-memory double buffer, completion on an mbarrier; the lanes then read their samples from shared memory.
 template <int STAGE>
 __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a(const uint32_t* __restrict__ iq, const uint64_t* __restrict__ off,
         const uint32_t* __restrict__ len, uint32_t nframes, DevTables T, FrameInfo* __restrict__ info,
         uint8_t* __restrict__ soft_out, uint64_t soft_stride, const uint16_t* __restrict__ inv_deint, FrontTaps taps, uint32_t sh, uint32_t lsh) {
     __shared__ uint32_t s_fft[SB_FRONT_WARPS][2][64];
-    __shared__ __align__(16) uint8_t s_soft[SB_FRONT_WARPS][288];
+    __shared__ __align__(16) uint8_t s_soft[SB_FRONT_WARPS][2][288];
     __shared__ uint32_t s_demap[256];                  // per input value: [bpsk/qpsk/first bit | 16-QAM second | 64-QAM second | 64-QAM third] soft bits
     __shared__ uint8_t s_pilot[128];
-    __shared__ uint32_t s_dec[SB_FRONT_WARPS][48];     // SIGNAL decoder's decision ballots
-    __shared__ __align__(16) uint32_t s_stage[STAGE == 2 ? SB_FRONT_WARPS : 1][2][STAGE == 2 ? 328 : 4];   // 2 x (320 words of a symbol pair + alignment slack)
-    __shared__ __align__(8) unsigned long long s_mbar[STAGE == 2 ? SB_FRONT_WARPS : 1][2];
+    __shared__ uint32_t s_dec[SB_FRONT_WARPS][2][48];  // SIGNAL decoder's decision ballots
+    // Per-lane constants of the symbol loop, kept out of the registers: words 0-11 the equaliser factors of the four bins (cfac re, im, nim),
+    // 12-23 the soft-bit positions of the two pairs (see load_positions), 24-27 the signed subcarrier numbers.  A row is 28 words, so
+    // the 16-byte loads of eight consecutive lanes fall on distinct banks.
+    __shared__ __align__(16) int s_lane[SB_FRONT_WARPS][32][28];
+    __shared__ __align__(16) uint32_t s_stage[STAGE == 2 ? SB_FRONT_WARPS : 1][2][2][STAGE == 2 ? 168 : 4];   // per half 2 x (160 words of a symbol + alignment slack)
+    __shared__ __align__(8) unsigned long long s_mbar[STAGE == 2 ? SB_FRONT_WARPS : 1][2][2];
     const unsigned FULL = 0xFFFFFFFFu;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    if (STAGE == 2 && lane == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][0])));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][1])));
+    const int half = lane >> 4, hl = lane & 15;
+    if (STAGE == 2 && hl == 0) {
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][half][0])));
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][half][1])));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = threadIdx.x; i < 256; i += blockDim.x)
         s_demap[i] = (uint32_t)__ldg(T.demap + i) | ((uint32_t)__ldg(T.demap + 256 + i) << 8) | ((uint32_t)__ldg(T.demap + 512 + i) << 16) | ((uint32_t)__ldg(T.demap + 768 + i) << 24);
     for (int i = threadIdx.x; i < 128; i += blockDim.x) s_pilot[i] = __ldg(T.pilot_neg + i);
     __syncthreads();
-    const uint32_t f = blockIdx.x * SB_FRONT_WARPS + wib;
-    if (f >= nframes) return;
-    FrameInfo fi = info[f];
-    if (fi.status != E_SUCCESS) return;
-    uint8_t* sb = s_soft[wib];
-    const uint32_t* x = iq + off[f];
-    const uint32_t nvec = ((len[f] << lsh) / 28u) * 28u / 8u;
+    const uint32_t f = 2u * (blockIdx.x * SB_FRONT_WARPS + (uint32_t)wib) + (uint32_t)half;
+    FrameInfo fi;
+    bool act = f < nframes;                            // this half's slot is still being decoded
+    if (act) { fi = info[f]; act = fi.status == E_SUCCESS; }
+    const uint32_t* x = iq + (act ? off[f] : 0);
+    const uint32_t nvec = act ? ((len[f] << lsh) / 28u) * 28u / 8u : 0u;
     const uint32_t s0 = fi.detect_vec * 4u;            // first 20 Msps sample of the 144-sample LTS block
-    if (fi.detect_vec + 36u > nvec) { if (lane == 0) info[f].status = E_NO_FRAME; return; }
-    const int half = lane >> 4, hl = lane & 15;        // FFT role: which of the two symbols, which butterfly
-    // Post-FFT role: this lane's two bins.  Lanes 0-23 own the data subcarriers d0 = 6 (lane / 3) + lane % 3 and d1 = d0 + 3 (demapper
-    // order): at 64-QAM the 802.11a de-interleaver puts coded bit i of d0 at an even position and bit (2 0 1 5 3 4)[i] of d1 right after
-    // it, so the pair's soft bits leave as six 16-bit stores.  Lanes 24-27 own the pilots (bins 43, 57, 7, 21) in b0, the twelve zero
-    // bins (0, 27..37) fill the rest.
-    const int d0 = lane < 24 ? 6 * (lane / 3) + lane % 3 : -1, d1 = lane < 24 ? d0 + 3 : -1;
-    const int j24 = lane - 24;
-    const int b0 = lane < 24 ? data_bin(d0) : j24 < 4 ? (0x1507392B >> (8 * j24)) & 0xFF : j24 == 4 ? 0 : 22 + j24;
-    const int b1 = lane < 24 ? data_bin(d1) : 30 + j24;
-    const int r0 = bitrev6(b0), r1 = bitrev6(b1);
+    if (act && fi.detect_vec + 36u > nvec) { if (hl == 0) info[f].status = E_NO_FRAME; act = false; }
+    const bool own = act;                              // this half writes its slot's FrameInfo back at the end
+    if (!__any_sync(FULL, act)) return;
     const cfac w64_1 = fac_tw(unpack(__ldg(T.tw64 + hl))), w64_2 = fac_tw(unpack(__ldg(T.tw64 + 16 + hl))), w64_3 = fac_tw(unpack(__ldg(T.tw64 + 32 + hl)));
     const cfac w16_1 = fac_tw(unpack(__ldg(T.tw16 + (hl & 3)))), w16_2 = fac_tw(unpack(__ldg(T.tw16 + 4 + (hl & 3)))), w16_3 = fac_tw(unpack(__ldg(T.tw16 + 8 + (hl & 3))));
+    uint32_t* const xb = s_fft[wib][half];
     // 64-point FFT of four freq-compensated time samples per lane (n = hl + 16 j), this half-warp's buffer; packed words throughout
     auto fft_from_regs = [&](uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-        uint32_t* xb = s_fft[wib][half];
         pk_r4_butterfly(a, b, c, d, w64_1, w64_2, w64_3);                   // FFTSSE<64>, butterfly e = hl
         xb[hl] = a; xb[hl + 16] = b; xb[hl + 32] = c; xb[hl + 48] = d;
         __syncwarp();
@@ -317,27 +324,37 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
         __syncwarp();
     };
     // ---- T11aLTS (channel_11a.hpp:34-230) -----------------------------------------------------------
-    {   // FreqOffsetEstimate<16> (dspalg.hpp:227-243): sum over the 64 samples of (LTS2 * conj(LTS1 >> 1)) >> 5
-        const uint32_t n0 = (uint32_t)lane, n1 = n0 + 32u;
-        cs16 l0 = sra(unpack(__ldg(x + ((s0 + 8u + n0) << sh))), 1), l1 = sra(unpack(__ldg(x + ((s0 + 8u + n1) << sh))), 1);
-        cs16 h0 = unpack(__ldg(x + ((s0 + 72u + n0) << sh))), h1 = unpack(__ldg(x + ((s0 + 72u + n1) << sh)));
-        int re0, im0, re1, im1; cmul_conj32(re0, im0, h0, l0); cmul_conj32(re1, im1, h1, l1);
-        int sr = wadd(re0 >> 5, re1 >> 5), si = wadd(im0 >> 5, im1 >> 5);
-        for (int o = 16; o; o >>= 1) { sr = wadd(sr, __shfl_xor_sync(FULL, sr, o)); si = wadd(si, __shfl_xor_sync(FULL, si, o)); }
+    {   // FreqOffsetEstimate<16> (dspalg.hpp:227-243): sum over the 64 samples of (LTS2 * conj(LTS1 >> 1)) >> 5, wrapping adds in any order
+        int sr = 0, si = 0;
+        if (act) {
+#pragma unroll
+            for (int j = 0; j < 4; j++) {
+                const uint32_t n = (uint32_t)hl + 16u * j;
+                const cs16 l = sra(unpack(__ldg(x + ((s0 + 8u + n) << sh))), 1), h = unpack(__ldg(x + ((s0 + 72u + n) << sh)));
+                int re, im; cmul_conj32(re, im, h, l);
+                sr = wadd(sr, re >> 5); si = wadd(si, im >> 5);
+            }
+        }
+        for (int o = 8; o; o >>= 1) { sr = wadd(sr, __shfl_xor_sync(FULL, sr, o)); si = wadd(si, __shfl_xor_sync(FULL, si, o)); }
         fi.cfo_est = (int)(short)(((uint32_t)d_uatan2(T, si, sr)) / 64u);  // short / size_t (dspalg.hpp:242)
     }
     rfac fcv[4];                                       // FreqCoeffs of this lane's four time samples (dspalg.hpp:201-208)
 #pragma unroll
     for (int j = 0; j < 4; j++) fcv[j] = fac_rotw(d_rotw(T, fi.cfo_est * (hl + 16 * j)));
     auto fcomp = [&](uint32_t w, int j) { return pk_cmul((int)(short)w >> 1, (int)w >> 17, fcv[j]); };   // cmul_q15(sra(w, 1), FreqCoeffs)
-    auto load4 = [&](uint32_t first, uint32_t (&v)[4]) {  // (x >> 1) * FreqCoeffs for samples first + hl + 16 j
+    auto load4 = [&](uint32_t first, uint32_t (&v)[4]) {  // (x >> 1) * FreqCoeffs for samples first + hl + 16 j; zeros in a half that idles
 #pragma unroll
-        for (int j = 0; j < 4; j++) v[j] = fcomp(__ldg(x + ((first + hl + 16u * j) << sh)), j);
+        for (int j = 0; j < 4; j++) v[j] = 0u;
+        if (act) {
+#pragma unroll
+            for (int j = 0; j < 4; j++) v[j] = fcomp(__ldg(x + ((first + hl + 16u * j) << sh)), j);
+        }
     };
-    {   uint32_t v[4]; load4(s0 + 8u, v); fft_from_regs(v[0], v[1], v[2], v[3]); }     // both halves transform LTS1 (same data)
-    cs16 ch0, ch1;
+    {   uint32_t v[4]; load4(s0 + 8u, v); fft_from_regs(v[0], v[1], v[2], v[3]); }     // LTS1
+    int* const tab = s_lane[wib][lane];
+    const int4* const tab4 = (const int4*)tab;
+    int rb[4];                                         // where bin i of this lane sits in the bit-reversed FFT output
     {   // channel_11a.hpp:124-171: H^-1 = (+-1600 conj(Y)) / (|Y|^2 >> 8), C integer division
-        const uint32_t* xb = s_fft[wib][0];
         auto inv = [&](cs16 y, int bin) -> cs16 {
             if (bin >= 28 && bin <= 35) return mk(0, 0);
             int e = wadd(y.re * y.re, y.im * y.im) >> 8;
@@ -345,199 +362,219 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
             int re, im; cmul_conj32(re, im, mk(L, 0), y);
             return e ? mk(sx16(re / e), sx16(im / e)) : mk(0, 0);
         };
-        ch0 = inv(unpack(xb[r0]), b0); ch1 = inv(unpack(xb[r1]), b1);
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            const int b = front_bin(hl, i);
+            rb[i] = bitrev6(b);
+            const cs16 ch = inv(unpack(xb[rb[i]]), b);
+            // bins 28..35 (SSE vectors 7,8) are forced to zero: their channel coefficient is zero, so is everything multiplied by it
+            const cfac eq = fac_mul8(ch);
+            tab[3 * i] = eq.re; tab[3 * i + 1] = eq.im; tab[3 * i + 2] = eq.nim;
+            tab[24 + i] = b < 32 ? b : b - 64;
+            if (taps.freq_coeffs && own) { taps.freq_coeffs[(size_t)f * 64 + b] = d_rotw(T, fi.cfo_est * b); taps.chan_coeffs[(size_t)f * 64 + b] = pack(ch); }
+        }
     }
     __syncwarp();
-    if (taps.freq_coeffs) { taps.freq_coeffs[(size_t)f * 64 + b0] = d_rotw(T, fi.cfo_est * b0); taps.freq_coeffs[(size_t)f * 64 + b1] = d_rotw(T, fi.cfo_est * b1);
-                            taps.chan_coeffs[(size_t)f * 64 + b0] = pack(ch0); taps.chan_coeffs[(size_t)f * 64 + b1] = pack(ch1); }
     // ---- symbols -----------------------------------------------------------------------------------
-    const int k0 = b0 < 32 ? b0 : b0 - 64, k1 = b1 < 32 ? b1 : b1 - 64;   // signed subcarrier numbers of this lane's bins
-    const bool v0 = k0 != 0 && k0 >= -26 && k0 <= 26, v1 = k1 != 0 && k1 >= -26 && k1 <= 26;
-    // bins 28..35 (SSE vectors 7,8) are forced to zero: their channel coefficient is zero, so is everything multiplied by it
-    const cfac eq0 = fac_mul8(ch0), eq1 = fac_mul8(ch1);
-    rfac comp0 = fac_rotw(0x7fffu), comp1 = comp0;
+    rfac comp[4];
+#pragma unroll
+    for (int i = 0; i < 4; i++) comp[i] = fac_rotw(0x7fffu);
     // The tracker's accumulators only ever index the rotation table (mod 2^16) and feed each other by addition, so they wrap mod 2^32
     // instead of being truncated with sx16 at every step: the low 16 bits are the same.
     uint32_t CFO_comp = 0, SFO_comp = 0, CFO_tr = 0, SFO_tr = 0; unsigned symbol_count = 127;
-    int plcp_data = 0; uint32_t remain = 0; uint32_t soft_bytes = 0; int nbpsc = 1;
+    uint32_t remain = 0; uint32_t soft_bytes = 0; int nbpsc = 1;
     uint8_t* sout = soft_out + (size_t)f * soft_stride;
     uint32_t status = E_SUCCESS;
-    // Where this lane's soft bits go after de-interleaving, as byte offsets into s_soft: at 64-QAM pos[i] is the even position of bit i of
-    // d0 (the 16-bit store of the pair); at the other rates the low half of pos[i] is bit i of d0, the high half bit i of d1.
-    uint32_t pos[6];
+    // Where this lane's soft bits go after de-interleaving, as byte offsets into s_soft, words 12 + 6 p + i of the lane's row for pair p: at
+    // 64-QAM bit i of d is at the even position (the 16-bit store of the pair); at the other rates the low half is bit i of d, the high half
+    // bit i of d + 3.
     auto load_positions = [&](int nb) {
         const uint16_t* inv = inv_deint + (nb == 1 ? 0 : nb == 2 ? 48 : nb == 4 ? 144 : 336);
-        const uint32_t base = (uint32_t)wib * 288u;
+        const uint32_t base = (uint32_t)(2 * wib + half) * 288u;
 #pragma unroll
-        for (int i = 0; i < 6; i++) {
-            if (d0 < 0 || i >= nb) pos[i] = 0;
-            else if (nb == 6) pos[i] = base + __ldg(inv + d0 * 6 + i);
-            else pos[i] = (base + __ldg(inv + d0 * nb + i)) | ((base + __ldg(inv + d1 * nb + i)) << 16);
+        for (int p = 0; p < 2; p++) {
+            const int d = front_pair(hl, p);
+#pragma unroll
+            for (int i = 0; i < 6; i++) {
+                uint32_t w = 0;
+                if (hl < 12 && i < nb) w = nb == 6 ? base + __ldg(inv + d * 6 + i) : (base + __ldg(inv + d * nb + i)) | ((base + __ldg(inv + (d + 3) * nb + i)) << 16);
+                tab[12 + 6 * p + i] = (int)w;
+            }
         }
     };
     load_positions(1);
-    uint8_t* const s8 = &s_soft[0][0];
-    // everything behind the FFT for one symbol whose spectrum sits in s_fft[wib][h]; returns false when the frame ended
-    auto post_fft = [&](int h, uint32_t sym) -> bool {
-        const uint32_t* xb = s_fft[wib][h];
-        const uint32_t F0 = xb[r0], F1 = xb[r1];
-        int e0x, e0y, e1x, e1y, c0x, c0y, c1x, c1y;                                    // products as 32-bit sums, value = sum >> 16
-        pk_cmul_xy((int)(short)F0, (int)F0 >> 16, eq0, e0x, e0y);                       // channel_11a.hpp:551-579
-        pk_cmul_xy((int)(short)F1, (int)F1 >> 16, eq1, e1x, e1y);
-        pk_cmul_xy(e0x >> 16, e0y >> 16, comp0, c0x, c0y);                              // freqoffset.hpp:28-30
-        pk_cmul_xy(e1x >> 16, e1y >> 16, comp1, c1x, c1y);
-        const int C0re = c0x >> 16, C0im = c0y >> 16, C1re = c1x >> 16, C1im = c1y >> 16;
-        // pilot.hpp:168-232: one table walk for the whole warp, the pilots sit in C0 of lanes 24-27 (bins 43, 57, 7, 21; bin 21's is sent negated)
-        const bool neg = lane == 27;
-        const int th = turn_pi(d_uatan2(T, neg ? -C0im : C0im, neg ? -C0re : C0re), s_pilot[symbol_count]);
-        const int th1 = __shfl_sync(FULL, th, 24), th2 = __shfl_sync(FULL, th, 25), th3 = __shfl_sync(FULL, th, 26), th4 = __shfl_sync(FULL, th, 27);
+    uint8_t* const s8 = &s_soft[0][0][0];
+    const bool rot123 = hl < 12;                       // bins 1-3 are rotated data subcarriers (bin 0 is data or a pilot: rotated anyway)
+    // everything behind the FFT for symbol `sym` of this half's slot, whose spectrum sits in xb
+    auto post_fft = [&](uint32_t sym) {
+        const int4 q0 = tab4[0], q1 = tab4[1], q2 = tab4[2], kq = tab4[6];
+        const cfac eq[4] = {{q0.x, q0.y, q0.z}, {q0.w, q1.x, q1.y}, {q1.z, q1.w, q2.x}, {q2.y, q2.z, q2.w}};
+        const int k[4] = {kq.x, kq.y, kq.z, kq.w};
+        uint32_t F[4]; int ex[4], ey[4], C[4][2];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            F[i] = xb[rb[i]];
+            int cx, cy;                                                                  // products as 32-bit sums, value = sum >> 16
+            pk_cmul_xy((int)(short)F[i], (int)F[i] >> 16, eq[i], ex[i], ey[i]);          // channel_11a.hpp:551-579
+            pk_cmul_xy(ex[i] >> 16, ey[i] >> 16, comp[i], cx, cy);                       // freqoffset.hpp:28-30
+            C[i][0] = cx >> 16; C[i][1] = cy >> 16;
+        }
+        // pilot.hpp:168-232: one table walk for both slots, the pilots sit in bin 0 of lanes 12-15 of each half (43, 57, 7, 21; 21's is sent negated)
+        const bool neg = hl == 15;
+        const int th = turn_pi(d_uatan2(T, neg ? -C[0][1] : C[0][1], neg ? -C[0][0] : C[0][0]), s_pilot[symbol_count]);
+        const int th1 = __shfl_sync(FULL, th, 12, 16), th2 = __shfl_sync(FULL, th, 13, 16), th3 = __shfl_sync(FULL, th, 14, 16), th4 = __shfl_sync(FULL, th, 15, 16);
         symbol_count++; if (symbol_count >= 127) symbol_count = 0;
         // the angles are int16, so the sum / 4 lies in [-32768, 32767] and each difference / 28 in [-2340, 2340]: the sx16 of both is the identity
         const int avg = (th1 + th2 + th3 + th4) / 4;
         const int del = ((th3 - th1) / 28 + (th4 - th2) / 28) >> 1;
         CFO_tr += (uint32_t)(avg >> 2); SFO_tr += (uint32_t)(del >> 2);
         CFO_comp += (uint32_t)avg + CFO_tr; SFO_comp += (uint32_t)del + SFO_tr;
-        // next symbol's phase compensation; only the rotated bins below use it, every other bin's R is zero whatever its C
-        comp0 = fac_rotw(d_rotw(T, (int)(CFO_comp + (uint32_t)k0 * SFO_comp)));
-        comp1 = fac_rotw(d_rotw(T, (int)(CFO_comp + (uint32_t)k1 * SFO_comp)));
-        // subcarriers -26..-1, 1..26 are rotated, every other bin becomes zero
-        const uint32_t R0 = pk_cmul(C0re, C0im, fac_rotw(v0 ? d_rotw(T, avg + k0 * del) : 0u));
-        const uint32_t R1 = pk_cmul(C1re, C1im, fac_rotw(v1 ? d_rotw(T, avg + k1 * del) : 0u));
-        if (taps.fft_out && sym < taps.max_sym) {
-            size_t o = ((size_t)f * taps.max_sym + sym) * 64;
-            taps.fft_out[o + b0] = F0; taps.fft_out[o + b1] = F1;
-            taps.equalized[o + b0] = __byte_perm((uint32_t)e0x, (uint32_t)e0y, 0x7632); taps.equalized[o + b1] = __byte_perm((uint32_t)e1x, (uint32_t)e1y, 0x7632);
-            taps.tracked[o + b0] = R0; taps.tracked[o + b1] = R1;
+        // subcarriers -26..-1, 1..26 are rotated, every other bin (zero bins 1-3 of lanes 12-15) becomes zero
+        uint32_t R[4];
+#pragma unroll
+        for (int i = 0; i < 4; i++) {
+            // next symbol's phase compensation; only the rotated bins use it, every other bin's R is zero whatever its C
+            comp[i] = fac_rotw(d_rotw(T, (int)(CFO_comp + (uint32_t)k[i] * SFO_comp)));
+            R[i] = pk_cmul(C[i][0], C[i][1], fac_rotw(i == 0 || rot123 ? d_rotw(T, avg + k[i] * del) : 0u));
+        }
+        if (taps.fft_out && act && sym < taps.max_sym) {
+            const size_t o = ((size_t)f * taps.max_sym + sym) * 64;
+#pragma unroll
+            for (int i = 0; i < 4; i++) {
+                const int b = front_bin(hl, i);
+                taps.fft_out[o + b] = F[i]; taps.equalized[o + b] = __byte_perm((uint32_t)ex[i], (uint32_t)ey[i], 0x7632); taps.tracked[o + b] = R[i];
+            }
         }
         // soft demap (demapper.h:141-151 limit + LUTs) scattered through the inverse de-interleaver map
-        const int ncbps = 48 * nbpsc;
-        if (d0 >= 0) {
-            const uint32_t c0 = pk_demap_clamp(R0), c1 = pk_demap_clamp(R1);
-            const uint32_t wr0 = s_demap[(c0 >> 4) & 0xFF], wi0 = s_demap[(c0 >> 20) & 0xFF], wr1 = s_demap[(c1 >> 4) & 0xFF], wi1 = s_demap[(c1 >> 20) & 0xFF];
-            if (nbpsc == 6) {                          // bits 0-2 are bytes 0, 2, 3 of wr, bits 3-5 those of wi; d0's byte low, d1's high
-                auto st16 = [&](uint32_t p, uint32_t v) { *(uint16_t*)(s8 + p) = (uint16_t)v; };
-                st16(pos[0], __byte_perm(wr0, wr1, 0x70)); st16(pos[1], __byte_perm(wr0, wr1, 0x42)); st16(pos[2], __byte_perm(wr0, wr1, 0x63));
-                st16(pos[3], __byte_perm(wi0, wi1, 0x70)); st16(pos[4], __byte_perm(wi0, wi1, 0x42)); st16(pos[5], __byte_perm(wi0, wi1, 0x63));
-            } else {
-                auto st8 = [&](uint32_t p, uint32_t v0w, uint32_t v1w) { s8[p & 0xFFFFu] = (uint8_t)v0w; s8[p >> 16] = (uint8_t)v1w; };
-                if (nbpsc == 1) { st8(pos[0], wr0, wr1); }
-                else if (nbpsc == 2) { st8(pos[0], wr0, wr1); st8(pos[1], wi0, wi1); }
-                else { st8(pos[0], wr0, wr1); st8(pos[1], wr0 >> 8, wr1 >> 8); st8(pos[2], wi0, wi1); st8(pos[3], wi0 >> 8, wi1 >> 8); }
+        if (hl < 12) {
+            const int4 p0 = tab4[3], p1 = tab4[4], p2 = tab4[5];
+            const uint32_t pos[12] = {(uint32_t)p0.x, (uint32_t)p0.y, (uint32_t)p0.z, (uint32_t)p0.w, (uint32_t)p1.x, (uint32_t)p1.y,
+                                      (uint32_t)p1.z, (uint32_t)p1.w, (uint32_t)p2.x, (uint32_t)p2.y, (uint32_t)p2.z, (uint32_t)p2.w};
+#pragma unroll
+            for (int p = 0; p < 2; p++) {
+                const uint32_t c0 = pk_demap_clamp(R[2 * p]), c1 = pk_demap_clamp(R[2 * p + 1]);
+                const uint32_t wr0 = s_demap[(c0 >> 4) & 0xFF], wi0 = s_demap[(c0 >> 20) & 0xFF], wr1 = s_demap[(c1 >> 4) & 0xFF], wi1 = s_demap[(c1 >> 20) & 0xFF];
+                const uint32_t* ps = pos + 6 * p;
+                if (nbpsc == 6) {                      // bits 0-2 are bytes 0, 2, 3 of wr, bits 3-5 those of wi; d's byte low, d + 3's high
+                    auto st16 = [&](uint32_t q, uint32_t v) { *(uint16_t*)(s8 + q) = (uint16_t)v; };
+                    st16(ps[0], __byte_perm(wr0, wr1, 0x70)); st16(ps[1], __byte_perm(wr0, wr1, 0x42)); st16(ps[2], __byte_perm(wr0, wr1, 0x63));
+                    st16(ps[3], __byte_perm(wi0, wi1, 0x70)); st16(ps[4], __byte_perm(wi0, wi1, 0x42)); st16(ps[5], __byte_perm(wi0, wi1, 0x63));
+                } else {
+                    auto st8 = [&](uint32_t q, uint32_t v0w, uint32_t v1w) { s8[q & 0xFFFFu] = (uint8_t)v0w; s8[q >> 16] = (uint8_t)v1w; };
+                    if (nbpsc == 1) { st8(ps[0], wr0, wr1); }
+                    else if (nbpsc == 2) { st8(ps[0], wr0, wr1); st8(ps[1], wi0, wi1); }
+                    else { st8(ps[0], wr0, wr1); st8(ps[1], wr0 >> 8, wr1 >> 8); st8(ps[2], wi0, wi1); st8(ps[3], wi0 >> 8, wi1 >> 8); }
+                }
             }
         }
         __syncwarp();
-        if (!plcp_data) {                              // PHY_11a.hpp:520-604
-            uint32_t sig = warp_viterbi_signal(sb, s_dec[wib], lane) & 0xFFFFFFu;
-            bool ok = !(sig & 0xFC0010u);
-            uint32_t par = (sig >> 16) ^ sig; par ^= par >> 8; par ^= par >> 4; par ^= par >> 2; par ^= par >> 1;
-            ok = ok && !(par & 1);
-            uint32_t rate = 0; int nd = 0, nb = 1, cr = CR_12;
-            switch (sig & 0xF) {                       // ieee80211a_cmn.h:97-157
-                case 0xB: rate = 6000; nd = 24; nb = 1; cr = CR_12; break;   case 0xF: rate = 9000; nd = 36; nb = 1; cr = CR_34; break;
-                case 0xA: rate = 12000; nd = 48; nb = 2; cr = CR_12; break;  case 0xE: rate = 18000; nd = 72; nb = 2; cr = CR_34; break;
-                case 0x9: rate = 24000; nd = 96; nb = 4; cr = CR_12; break;  case 0xD: rate = 36000; nd = 144; nb = 4; cr = CR_34; break;
-                case 0x8: rate = 48000; nd = 192; nb = 6; cr = CR_23; break; case 0xC: rate = 54000; nd = 216; nb = 6; cr = CR_34; break;
-                default: if (ok) fi.rate_kbps = 0; ok = false;    // BB11aParseDataRate() == 0 is stored before the parser gives up
+        if (sym == 0) {                                // PHY_11a.hpp:520-604; both halves' SIGNALs, one after the other on the whole warp
+            uint32_t sig = 0;
+#pragma unroll 1
+            for (int h = 0; h < 2; h++) { const uint32_t s = warp_viterbi_signal(s_soft[wib][h], s_dec[wib][h], lane); if (h == half) sig = s; }
+            sig &= 0xFFFFFFu;
+            if (act) {
+                bool ok = !(sig & 0xFC0010u);
+                uint32_t par = (sig >> 16) ^ sig; par ^= par >> 8; par ^= par >> 4; par ^= par >> 2; par ^= par >> 1;
+                ok = ok && !(par & 1);
+                uint32_t rate = 0; int nd = 0, nb = 1, cr = CR_12;
+                switch (sig & 0xF) {                   // ieee80211a_cmn.h:97-157
+                    case 0xB: rate = 6000; nd = 24; nb = 1; cr = CR_12; break;   case 0xF: rate = 9000; nd = 36; nb = 1; cr = CR_34; break;
+                    case 0xA: rate = 12000; nd = 48; nb = 2; cr = CR_12; break;  case 0xE: rate = 18000; nd = 72; nb = 2; cr = CR_34; break;
+                    case 0x9: rate = 24000; nd = 96; nb = 4; cr = CR_12; break;  case 0xD: rate = 36000; nd = 144; nb = 4; cr = CR_34; break;
+                    case 0x8: rate = 48000; nd = 192; nb = 6; cr = CR_23; break; case 0xC: rate = 54000; nd = 216; nb = 6; cr = CR_34; break;
+                    default: if (ok) fi.rate_kbps = 0; ok = false;    // BB11aParseDataRate() == 0 is stored before the parser gives up
+                }
+                const uint32_t L = (sig >> 5) & 0xFFF;
+                if (ok && rate) { fi.rate_kbps = rate; fi.code_rate = cr; }
+                if (ok) { fi.length = L; ok = L <= 2500; }
+                if (!ok) { status = E_PLCP_HEADER_FAIL; act = false; }
+                else {
+                    fi.nsym_total = (L * 8 + 16 + 6 + nd - 1) / nd + 1;
+                    remain = fi.nsym_total; nbpsc = nb; fi.ncbps = 48 * nb;
+                    load_positions(nb);
+                }
             }
-            uint32_t L = (sig >> 5) & 0xFFF;
-            if (ok && rate) { fi.rate_kbps = rate; fi.code_rate = cr; }
-            if (ok) { fi.length = L; ok = L <= 2500; }
-            if (!ok) { status = E_PLCP_HEADER_FAIL; return false; }
-            fi.nsym_total = (L * 8 + 16 + 6 + nd - 1) / nd + 1;
-            remain = fi.nsym_total; plcp_data = 1; nbpsc = nb; fi.ncbps = 48 * nb;
-            load_positions(nb);
-        } else {                                       // N_CBPS = 48 N_BPSC bytes: 3 N_BPSC 16-byte lines (soft_out and soft_stride are 16-byte aligned)
-            if (lane < 3 * nbpsc) ((uint4*)(sout + soft_bytes))[lane] = ((const uint4*)sb)[lane];
-            soft_bytes += ncbps;
+        } else if (act) {                              // N_CBPS = 48 N_BPSC bytes: 3 N_BPSC 16-byte lines (soft_out and soft_stride are 16-byte aligned)
+            uint4* const dst = (uint4*)(sout + soft_bytes); const uint4* const src = (const uint4*)s_soft[wib][half];
+            if (hl < 3 * nbpsc) dst[hl] = src[hl];
+            if (hl + 16 < 3 * nbpsc) dst[hl + 16] = src[hl + 16];
+            soft_bytes += 48u * nbpsc;
         }
         __syncwarp();
-        remain--;
-        return remain != 0;
+        if (act) { remain--; act = remain != 0; }
     };
-    auto sym_ready = [&](uint32_t sym) { return (s0 + 144u + 80u * sym + 80u) / 4u <= nvec; };   // all 80 samples arrived
-    // SIGNAL symbol alone, then the data symbols two at a time
-    bool more = true;
-    if (!sym_ready(0)) { status = E_NO_FRAME; more = false; }
-    if (more) {
-        uint32_t v[4]; load4(s0 + 144u + 8u, v); fft_from_regs(v[0], v[1], v[2], v[3]);
-        more = post_fft(0, 0);
-    }
-    if (taps.hdr_only && more) {                                          // continuous-capture scout pass: where the frame ends is all the caller wants
-        if (!sym_ready(fi.nsym_total - 1u)) status = E_NO_FRAME;
-        more = false;
-    }
-    // ---- staging of the DATA symbols (see STAGE above) ----
+    auto sym_first = [&](uint32_t sym) { return s0 + 144u + 80u * sym; };                        // first sample of symbol sym (its CP)
+    auto sym_ready = [&](uint32_t sym) { return (sym_first(sym) + 80u) / 4u <= nvec; };         // all 80 samples arrived
+    // ---- staging (see STAGE above) ----
     const uint32_t nsamp20 = nvec * 4u;                                   // 20 Msps samples of the slot that may be read
     uint32_t raw[4] = {0, 0, 0, 0}; uint32_t raw_first = 0xFFFFFFFFu;     // STAGE 1: samples first + hl + 16 j of the prefetched symbol
     auto prefetch_regs = [&](uint32_t first) {                            // whole symbol inside the slot, else nothing
         raw_first = 0xFFFFFFFFu;
-        if (first + 72u <= nsamp20) {
+        if (act && first + 72u <= nsamp20) {
 #pragma unroll
             for (int j = 0; j < 4; j++) raw[j] = __ldg(x + ((first + hl + 16u * j) << sh));
             raw_first = first;
         }
     };
-    uint32_t st_par[2] = {0, 0}; uint32_t st_base[2] = {0, 0}, st_cnt[2] = {0, 0}; uint32_t st_i = 0;   // STAGE 2: parity / first 20 Msps sample / samples per buffer
+    // STAGE 2: parity / first 20 Msps sample / samples per buffer, and which buffers have a copy in flight (bit b)
+    uint32_t st_par[2] = {0, 0}, st_base[2] = {0, 0}, st_cnt[2] = {0, 0}, st_busy = 0;
     auto stage_issue = [&](int b, uint32_t first20, uint32_t n20) {       // samples [first20, first20 + n20) of the slot -> buffer b (word index << sh)
         st_base[b] = first20; st_cnt[b] = 0;
-        if (first20 >= nsamp20) return;
+        if (!act || first20 >= nsamp20) return;
         if (first20 + n20 > nsamp20) n20 = nsamp20 - first20;
-        st_cnt[b] = n20;
-        if (lane == 0) {
+        st_cnt[b] = n20; st_busy |= 1u << b;
+        if (hl == 0) {
             const uint32_t* src = x + (first20 << sh);
             const uintptr_t a0 = (uintptr_t)src & ~(uintptr_t)15, a1 = ((uintptr_t)(src + (n20 << sh)) + 15) & ~(uintptr_t)15;
             const uint32_t bytes = (uint32_t)(a1 - a0);
-            const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][b]), dst = (uint32_t)__cvta_generic_to_shared(&s_stage[wib][b][0]);
+            const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][half][b]), dst = (uint32_t)__cvta_generic_to_shared(&s_stage[wib][half][b][0]);
             asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes) : "memory");
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" :: "r"(dst), "l"(a0), "r"(bytes), "r"(mb) : "memory");
         }
     };
     auto stage_wait = [&](int b) {
-        if (st_cnt[b] == 0) return;
-        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][b]); uint32_t ok = 0;
+        if (!((st_busy >> b) & 1u)) return;
+        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][half][b]); uint32_t ok = 0;
         while (!ok) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }" : "=r"(ok) : "r"(mb), "r"(st_par[b]) : "memory");
-        st_par[b] ^= 1u;
+        st_par[b] ^= 1u; st_busy &= ~(1u << b);
     };
     auto stage_load4 = [&](int b, uint32_t first, uint32_t (&v)[4]) {    // (x >> 1) * FreqCoeffs from buffer b; the buffer starts at the 16-byte line of its first sample
         const uint32_t skew = (uint32_t)(((uintptr_t)(x + (st_base[b] << sh)) & 15u) >> 2);
 #pragma unroll
-        for (int j = 0; j < 4; j++) v[j] = fcomp(s_stage[wib][b][skew + ((first - st_base[b] + hl + 16u * j) << sh)], j);
+        for (int j = 0; j < 4; j++) v[j] = fcomp(s_stage[wib][half][b][skew + ((first - st_base[b] + hl + 16u * j) << sh)], j);
     };
-    if (STAGE == 2 && more) stage_issue(0, s0 + 144u + 80u, 160u);        // symbols 1 and 2
-    if (STAGE == 1 && more) prefetch_regs(s0 + 144u + 80u * (1u + (uint32_t)half) + 8u);
-    for (uint32_t sym = 1; more; sym += 2) {
-        const bool haveA = sym_ready(sym), haveB = remain >= 2 && sym_ready(sym + 1);
-        if (!haveA) { status = E_NO_FRAME; break; }
+    if (STAGE == 2) stage_issue(0, sym_first(0), 80u);
+    if (STAGE == 1) prefetch_regs(sym_first(0) + 8u);
+    // SIGNAL, then the data symbols, one per iteration in each half
+    for (uint32_t sym = 0; ; sym++) {
+        if (act && !sym_ready(sym)) { status = E_NO_FRAME; act = false; }
+        if (!__any_sync(FULL, act)) break;
         {   uint32_t v[4];
-            const uint32_t mine = (half && haveB) ? sym + 1 : sym;          // without a second symbol both halves transform A
-            const uint32_t first = s0 + 144u + 80u * mine + 8u;
+            const uint32_t first = sym_first(sym) + 8u;
             if (STAGE == 2) {
-                const int b = (int)(st_i & 1u);
-                const bool staged = st_base[b] == s0 + 144u + 80u * sym && st_cnt[b] >= (mine - sym + 1u) * 80u;
+                const int b = (int)(sym & 1u);
+                const bool staged = st_base[b] == sym_first(sym) && st_cnt[b] >= 80u;
                 stage_wait(b);
-                if (staged) stage_load4(b, first, v); else load4(first, v);
+                if (act && staged) stage_load4(b, first, v); else load4(first, v);
                 __syncwarp();                                               // every lane has its samples: the other buffer's previous contents are no longer needed either
-                st_i++; stage_issue((int)(st_i & 1u), s0 + 144u + 80u * (sym + 2u), 160u);
+                stage_issue(b ^ 1, sym_first(sym + 1u), 80u);
             } else if (STAGE == 1) {
                 if (raw_first == first) {
 #pragma unroll
                     for (int j = 0; j < 4; j++) v[j] = fcomp(raw[j], j);
                 } else load4(first, v);
-                prefetch_regs(s0 + 144u + 80u * (sym + 2u + (uint32_t)half) + 8u);
+                prefetch_regs(first + 80u);
             } else load4(first, v);
             fft_from_regs(v[0], v[1], v[2], v[3]); }
-        more = post_fft(0, sym);
-        if (!more) break;
-        if (!haveB) {
-            if (remain >= 1 && !sym_ready(sym + 1)) { status = E_NO_FRAME; break; }
-            sym -= 1;                                                       // the next pair starts one symbol later than staged: restage
-            if (STAGE == 2) { stage_wait((int)(st_i & 1u)); __syncwarp(); stage_issue((int)(st_i & 1u), s0 + 144u + 80u * (sym + 2u), 160u); }
-            continue;
+        post_fft(sym);
+        if (sym == 0 && taps.hdr_only && act) {                           // continuous-capture scout pass: where the frame ends is all the caller wants
+            if (!sym_ready(fi.nsym_total - 1u)) status = E_NO_FRAME;
+            act = false;
         }
-        more = post_fft(1, sym + 1);
     }
-    if (STAGE == 2) { stage_wait((int)(st_i & 1u)); __syncwarp(); }        // no copy may be in flight when the CTA's shared memory is released
-    if (lane == 0) { fi.status = status; fi.soft_bytes = soft_bytes; info[f] = fi; }
+    if (STAGE == 2) { stage_wait(0); stage_wait(1); __syncwarp(); }       // no copy may be in flight when the CTA's shared memory is released
+    if (own && hl == 0) { fi.status = status; fi.soft_bytes = soft_bytes; info[f] = fi; }
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -567,7 +567,7 @@ static int launch_chunk(sb200_handle* h, const uint32_t* iq_base, const uint64_t
     if (timed) CK(cudaEventRecord(h->evk[0], sf));
     k_sync11a<<<(n + 127) / 128, 128, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->cca_thr, h->T, d_info, dc_init ? dc_init + f0 : nullptr, sh, lsh);
     if (timed) CK(cudaEventRecord(h->evk[1], sf));
-    {   const dim3 g((n + SB_FRONT_WARPS - 1) / SB_FRONT_WARPS), b(32 * SB_FRONT_WARPS);
+    {   const dim3 g((n + SB_FRONT_SLOTS - 1) / SB_FRONT_SLOTS), b(32 * SB_FRONT_WARPS);
         if (h->front_stage == 2) k_front11a<2><<<g, b, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh);
         else if (h->front_stage == 1) k_front11a<1><<<g, b, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh);
         else k_front11a<0><<<g, b, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh); }
@@ -838,7 +838,7 @@ extern "C" int sb200_rx11a_streams(sb200_handle* h, const int16_t* iq, uint64_t 
         uint32_t k = 0;
         for (; k < ROUND && done_passes + k < max_frames; k++) {
             k_sync11a<<<(n + 127) / 128, 128, 0, st>>>((const uint32_t*)d_iq, (const uint64_t*)h->soff.p, (const uint32_t*)h->slen.p, n, h->cca_thr, h->T, (FrameInfo*)h->info.p, (const int2*)h->dcbuf.p, 1u, 0u);
-            k_front11a<0><<<(n + SB_FRONT_WARPS - 1) / SB_FRONT_WARPS, 32 * SB_FRONT_WARPS, 0, st>>>((const uint32_t*)d_iq, (const uint64_t*)h->soff.p, (const uint32_t*)h->slen.p, n, h->T, (FrameInfo*)h->info.p, nullptr, 0, h->inv_deint, hdr, 1u, 0u);
+            k_front11a<0><<<(n + SB_FRONT_SLOTS - 1) / SB_FRONT_SLOTS, 32 * SB_FRONT_WARPS, 0, st>>>((const uint32_t*)d_iq, (const uint64_t*)h->soff.p, (const uint32_t*)h->slen.p, n, h->T, (FrameInfo*)h->info.p, nullptr, 0, h->inv_deint, hdr, 1u, 0u);
             k_stream_advance<<<(n + 127) / 128, 128, 0, st>>>((const FrameInfo*)h->info.p, n, (uint64_t*)h->soff.p, (uint32_t*)h->slen.p, (int2*)h->dcbuf.p, (uint32_t*)h->spos.p, (uint32_t*)h->snev.p, max_frames, (StreamEvent*)h->sev.p, d_live + k);
             h->launches += 3;
         }
