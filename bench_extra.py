@@ -12,6 +12,8 @@
   --config tx11a_legacy  the legacy 802.11a transmitter (BB11ATxFrameMod) on the device, 54 Mbps / 1500 B, at 40 and at 44 Msps
   --config channelize  the wideband channelizer: four 802.11a channels of a 160 Msps capture, 127 taps, D = 4, device-resident
   --config combine   the wideband combiner: four 802.11a channel rows at 40 Msps into one 160 Msps capture, 127 taps, U = 4, device-resident
+  --config sim       the radio channel simulator: --frames links of config #2's 9 824-sample slots (T = R = 1, L = 16, +20 ppm, a carrier
+                     offset, noise on), and a 2x2 case (T = R = 2, L = 16), device-resident
   --config 11n       config #4: 802.11n HT-MF 2x2 RX chain at MCS 8, 9, 10, PSDU 1500 B, 2 x 40 Msps, fixed 2x2 channel
 
 Each prints one JSON line per measurement (same timing rules as bench.py: >= 3 warm-ups, CUDA events on the launch
@@ -490,12 +492,49 @@ def bench_combine(args):
             "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs" % m})
     c.close()
 
+def bench_sim(args):
+    """The radio channel simulator on device-resident links of config #2's slot length (9 824 samples at 40 Msps): T = R = 1 with 16 taps,
+    and T = R = 2 with 16 taps per pair, every link at +20 ppm with a carrier offset and noise.  Integer work per output sample, from the
+    shapes: 16 T multiply-adds of the interpolation, 4 T L of the taps, 4 of the rotation and the noise's two 64-bit products (counted as
+    8), plus half a Philox4x32-10 block (20 32-bit multiplies); HBM traffic 4 T B read + 4 R B written per output sample and row."""
+    import sim_model as SM
+    from sora_b200 import api
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    name, plim, clk = _card(); sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    imad_peak = sms * 64 * clk * 1e6 if clk else None                    # int32 IMAD: 64 per SM per clock on sm_90
+    for T, R, nl in ((1, 1, args.frames * 2), (2, 2, args.frames // 2)):
+        L = 16; n = 9824; n_out = n
+        x = torch.randint(-8000, 8000, (nl, T, n, 2), dtype=torch.int16, device=dev); y = torch.empty((nl, R, n_out, 2), dtype=torch.int16, device=dev)
+        rng = np.random.default_rng(T)
+        links = api.sim_links([(int(rng.integers(0, 2 ** 32)), api.clock_step(20), api.phase_inc(-20e-6 * 5.2e9, 40e6), int(rng.integers(0, 2 ** 32)), 2000) for _ in range(nl)])
+        taps = rng.integers(-1000, 1000, (nl, R, T, L, 2)).astype(np.int16); taps[:, :, :, 0, 0] = 12000
+        dl = torch.from_numpy(links.view(np.uint8).copy()).to(dev); dt = torch.from_numpy(taps).to(dev)
+        def step(): eng.channel_sim_raw(x.data_ptr(), T * n, n, T, n, dl.data_ptr(), dt.data_ptr(), L, nl, 0x5EED, y.data_ptr(), R * n_out, n_out, R, n_out, st.cuda_stream)
+        step(); torch.cuda.synchronize()
+        pick = [0, nl - 1]
+        want = SM.sim_window(x[pick].cpu().numpy(), links[pick], taps[pick], 0x5EED, 0, 3000, link_ids=pick)
+        assert (y[pick, :, :3000].cpu().numpy() == want).all(), "channel simulator output differs from the stated arithmetic"
+        ms = c.timed(step, args.steps); sec = ms * 1e-3
+        outs = nl * R * n_out
+        work = outs * (16.0 * T + 4.0 * T * L + 4 + 8 + 20 / 2)
+        hbm = nl * n_out * (4.0 * T + 4.0 * R)
+        f_int = (work / sec / imad_peak) if imad_peak else None; f_hbm = hbm / sec / 1e9 / peaks()
+        c.emit({"metric": "channel simulator output Msamples/s (COMPLEX16, T = %d, R = %d, L = %d)" % (T, R, L), "value": c.world * outs / sec / 1e6, "unit": "Msamples/s",
+                "ms_per_step": ms, "n_gpus": c.world,
+                "config": {"workload": "%d links x 9824 samples at 40 Msps, +20 ppm, carrier offset, noise, device-resident" % nl, "output_samples_per_step_per_gpu": outs},
+                "hbm": {"achieved": hbm / sec / 1e9, "peak": peaks(), "unit": "GB/s", "frac": f_hbm, "note": "4 T B read + 4 R B written per output sample of a row"},
+                "int_ops": {"achieved": work / sec / 1e9, "peak": imad_peak / 1e9 if imad_peak else None, "unit": "G integer multiply-adds/s", "frac": f_int,
+                            "note": "16 T + 4 T L + 4 + 8 + 10 per output sample and row; peak = SMs x 64 x max SM clock"},
+                "card": name, "power_limit_w": plim, "max_sm_clock_mhz": clk,
+                "parity": "equal to the numpy model of the stated arithmetic on the first 3000 outputs of the first and last links"})
+    c.close()
+
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "combine"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "combine", "sim"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "combine": bench_combine}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "combine": bench_combine, "sim": bench_sim}[a.config](a)

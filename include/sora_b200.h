@@ -189,6 +189,38 @@ typedef struct sb200_duc_channel { uint32_t phase_inc; uint32_t phase0; uint32_t
 int sb200_combine(sb200_handle* h, const int16_t* rows, uint64_t row_stride_samples, uint64_t n_in_samples, const sb200_duc_channel* channels,
                   uint32_t nchannels, uint32_t interp, const int16_t* taps, uint32_t ntaps, int16_t* out, void* cuda_stream);
 
+/* Radio channel simulator: nlinks independent links, each from T = ntx input rows x_t[0 .. n_in) to R = nrx output rows y_r[0 .. n_out) of
+ * COMPLEX16 through a sampling-clock offset, multipath, a carrier offset and seeded noise, in the manner of GNU Radio's channel_model; an
+ * extension without a reference counterpart.  Row t of link l is at x + l * in_link_stride + t * in_row_stride samples, row r of y at
+ * y + l * out_link_stride + r * out_row_stride.  For link l with record {tau0, step, phase_inc, phase0, noise_q8}, L = ntaps complex Q14
+ * taps g[r][t][j] (taps + ((l R + r) T + t) L * 2: re, im) and every output row r and sample m:
+ *  1. sample clock   tau = tau0 + m * step (uint64, Q32.32 input samples), t' = tau + 2^23, i = t' >> 32, p = (t' >> 24) & 255,
+ *                    s_t(m) = sat16((sum_{k=0..7} H[p][k] * x_t(i - 3 + k) + 2^13) >> 14)      int32, re and im independently,
+ *                    x_t = 0 outside [0, n_in), s_t(m) = 0 for m < 0;
+ *                    H[p][k] = rint(16384 sinc(d) I0(5 sqrt(1 - (d / 4)^2)) / I0(5)), d = k - 3 - p / 256: row 0 is the unit impulse at
+ *                    k = 3, so step = 2^32 with a whole-sample tau0 is a pure delay, bit for bit (Q14, not Q15, for that reason)
+ *  2. multipath      u_r(m) = sat16((sum_t sum_{j<L} g[r][t][j] (x) s_t(m - j) + 2^13) >> 14)     complex product, int32
+ *                    (re = g.re s.re - g.im s.im, im = g.re s.im + g.im s.re)
+ *  3. carrier offset theta = phase0 + m * phase_inc (mod 2^32), (C, S) = NCO[theta >> 20] (the Q14 table of sb200_channelize),
+ *                    v.re = sat16((u.re C - u.im S + 2^13) >> 14), v.im = sat16((u.im C + u.re S + 2^13) >> 14)
+ *  4. noise          (w0, w1, w2, w3) = Philox4x32-10(counter (u32(m >> 1), u32(m >> 33), r, l), key (u32(seed), u32(seed >> 32))),
+ *                    (wa, wb) = (w0, w1) for even m, (w2, w3) for odd m; a = wa | 1, e = clz32(a), mant = u32(a << e) >> 20 in [2048, 4095],
+ *                    Lq = 11629080 e + LNT[mant - 2048], LNT[j] = rint(-ln((2048 + j + 0.5) / 4096) 2^24), Rn = floor(sqrt(2 Lq)) exactly,
+ *                    (Cn, Sn) = NCO[wb >> 20], n.re = (sigma Rn Cn + 2^33) >> 34, n.im = (sigma Rn Sn + 2^33) >> 34 (int64, arithmetic
+ *                    shifts, sigma = noise_q8), y_r(m) = (sat16(v.re + n.re), sat16(v.im + n.im))
+ * Stage 4 is a fixed-point Box-Muller on the NCO table: the noise has a standard deviation of noise_q8 / 256 LSB per real component, and
+ * Rn is at most about 6.7 sigma; noise_q8 = 0 adds none.  Every output is a closed form of (link, r, m): any window of outputs equals the
+ * same slice of the whole.  Limits (SB200_E_INVALID, nothing launched): 1 <= ntx, nrx <= 4, 1 <= ntaps <= 64, step in
+ * [2^32 - 2^24, 2^32 + 2^24], tau0 < 2^62, n_in and n_out <= 2^30, noise_q8 < 2^24, for every link and r the sum over t and j of
+ * |g.re| + |g.im| <= 65535 (the accumulator cannot wrap), the four strides multiples of 4 and below 2^40, and no two output rows overlapping.  Every pointer
+ * may be host or device memory (device x and y 16-byte aligned, device taps 4-byte aligned, device links 8-byte aligned); when links or
+ * taps are on the device their limits are checked there (one small kernel and one read-back).  One simulation launch; sb200_last_kernel_ms
+ * times it.  The two outputs of sb200_tx11n_batch go in as the rows of a link (in_row_stride = the distance between them). */
+typedef struct sb200_link { uint64_t tau0, step; uint32_t phase_inc, phase0, noise_q8, reserved; } sb200_link;
+int sb200_channel_sim(sb200_handle* h, const int16_t* x, uint64_t in_link_stride, uint64_t in_row_stride, uint32_t ntx, uint64_t n_in,
+                      const sb200_link* links, const int16_t* taps, uint32_t ntaps, uint32_t nlinks,
+                      uint64_t seed, int16_t* y, uint64_t out_link_stride, uint64_t out_row_stride, uint32_t nrx, uint64_t n_out, void* cuda_stream);
+
 /* Same as sb200_rx11a_batch for captures at `sample_rate_mhz` = 20, 40 or 44.  20: the capture is already at the channel rate (slots counted in
  * 20 Msps samples; sample j stands where TDownSample2 would have put sample 2j of a 40 Msps capture).  44 Msps slots first pass the reference's 11:10 linear
  * resampler (TDownSample44_40 / Down44to40, Brick11/src/sampling.hpp:37-65, 44MTo40M.hpp:63-123; graph

@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_combine", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_combine", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -77,6 +77,43 @@ class DdcChannel(C.Structure):
 
 class DucChannel(C.Structure):
     _fields_ = [("phase_inc", C.c_uint32), ("phase0", C.c_uint32), ("gain", C.c_uint32)]
+
+class SimLink(C.Structure):
+    """sb200_link: one link of sb200_channel_sim (include/sora_b200.h)."""
+    _fields_ = [("tau0", C.c_uint64), ("step", C.c_uint64), ("phase_inc", C.c_uint32), ("phase0", C.c_uint32), ("noise_q8", C.c_uint32), ("reserved", C.c_uint32)]
+
+LINK_DTYPE = np.dtype([("tau0", "<u8"), ("step", "<u8"), ("phase_inc", "<u4"), ("phase0", "<u4"), ("noise_q8", "<u4"), ("reserved", "<u4")])
+assert LINK_DTYPE.itemsize == C.sizeof(SimLink)
+
+def sim_links(records):
+    """Link records for sb200_channel_sim: a LINK_DTYPE array, or tuples (tau0, step, phase_inc, phase0, noise_q8) -> LINK_DTYPE array.
+    Increments and phases wrap mod 2^32, so a negative phase_inc stands for a negative frequency."""
+    if isinstance(records, np.ndarray) and records.dtype == LINK_DTYPE:
+        return np.ascontiguousarray(records)
+    out = np.zeros(len(records), LINK_DTYPE)
+    for i, (tau0, step, inc, ph, sig) in enumerate(records):
+        out[i] = (int(tau0), int(step), int(inc) % 2 ** 32, int(ph) % 2 ** 32, int(sig), 0)
+    return out
+
+def clock_step(ppm):
+    """Clock step of a link whose receiver's sample clock runs ppm parts per million fast: round(2^32 / (1 + ppm 1e-6)) input samples (Q32.32)
+    per output sample, so the receiver takes (1 + ppm 1e-6) times as many samples of the same signal."""
+    return int(round(2 ** 32 / (1 + ppm * 1e-6)))
+
+def sim_taps(delays, gains, L):
+    """Tapped-delay-line profile (delays in whole samples, complex gains, or 2x2 matrices g[r, t] for a MIMO link) -> Q14 int16 [R, T, L, 2]
+    taps of sb200_channel_sim: g[r][t][d] = rint(16384 gain).  Raises ValueError when a delay is not below L or a row's sum of |re| + |im|
+    exceeds 65535."""
+    g0 = np.asarray(gains[0], np.complex128)
+    R, T = (1, 1) if g0.ndim == 0 else g0.shape
+    h = np.zeros((R, T, L), np.complex128)
+    for d, g in zip(delays, gains):
+        if not 0 <= int(d) < L: raise ValueError(f"delay {d} is not below L = {L}")
+        h[:, :, int(d)] += np.asarray(g, np.complex128).reshape(R, T)
+    q = np.stack([np.rint(h.real * 16384), np.rint(h.imag * 16384)], -1)
+    if np.abs(q).max() > 32767 or (np.abs(q).sum((1, 2, 3)) > 65535).any():
+        raise ValueError("taps out of range: every |g| below 2 and every row's sum of |re| + |im| at most 65535 / 16384")
+    return q.astype(np.int16)
 
 _NDBPS_11A = {6000: 24, 9000: 36, 12000: 48, 18000: 72, 24000: 96, 36000: 144, 48000: 192, 54000: 216}   # 802.11a data bits per OFDM symbol
 
@@ -270,6 +307,27 @@ class Engine:
         out = np.zeros((interp * n_in, 2), np.int16)
         self.combine_raw(_ptr(x), stride, n_in, channels, interp, taps, _ptr(out))
         return out
+
+    def channel_sim_raw(self, x_ptr, in_link_stride, in_row_stride, ntx, n_in, links, taps, ntaps, nlinks, seed, y_ptr, out_link_stride, out_row_stride,
+                        nrx, n_out, stream=0):
+        """Pointer-level sb200_channel_sim: x / y / links / taps each a host or device address (links and taps may also be numpy arrays)."""
+        self._check(self._lib.sb200_channel_sim(self._h, C.c_void_p(x_ptr), C.c_uint64(in_link_stride), C.c_uint64(in_row_stride), C.c_uint32(ntx), C.c_uint64(n_in),
+                                                C.c_void_p(_ptr(links)), C.c_void_p(_ptr(taps)), C.c_uint32(ntaps), C.c_uint32(nlinks), C.c_uint64(seed % 2 ** 64),
+                                                C.c_void_p(y_ptr), C.c_uint64(out_link_stride), C.c_uint64(out_row_stride), C.c_uint32(nrx), C.c_uint64(n_out),
+                                                C.c_void_p(stream)), "sb200_channel_sim")
+
+    def channel_sim(self, x, links, taps, n_out, seed=0):
+        """Radio channel simulator: int16 x [nlinks, T, n_in, 2], link records (sim_links), Q14 taps int16 [nlinks, R, T, L, 2] (or [R, T, L, 2]
+        for every link), n_out -> int16 y [nlinks, R, n_out, 2].  See sb200_channel_sim in include/sora_b200.h for the arithmetic."""
+        x = np.asarray(x, np.int16); nl, T, n_in = x.shape[:3]
+        lk = sim_links(links); assert len(lk) == nl
+        t = np.asarray(taps, np.int16)
+        if t.ndim == 4: t = np.broadcast_to(t, (nl,) + t.shape)
+        t = np.ascontiguousarray(t); R, L = t.shape[1], t.shape[3]; assert t.shape[2] == T
+        si = (n_in + 3) // 4 * 4; xs = np.zeros((nl, T, si, 2), np.int16); xs[:, :, :n_in] = x
+        so = (n_out + 3) // 4 * 4; y = np.zeros((nl, R, so, 2), np.int16)
+        self.channel_sim_raw(_ptr(xs), T * si, si, T, n_in, lk, t, L, nl, seed, _ptr(y), R * so, so, R, n_out)
+        return y[:, :, :n_out]
 
     def tx11b_fir37_raw(self, in_ptr, total, off_ptr, len_ptr, nframes, variant, out_ptr, stream=0):
         self._check(self._lib.sb200_tx11b_fir37(self._h, C.c_void_p(in_ptr), C.c_uint64(total), C.c_void_p(off_ptr), C.c_void_p(len_ptr), C.c_uint32(nframes),

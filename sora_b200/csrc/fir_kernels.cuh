@@ -42,37 +42,43 @@ static_assert(SB_CH_WIN >= SB_FIR_TILE + 2 * SB_CH_MAXHALO + SB_CH_MAXDECIM - 1,
 struct ChTaps { int16_t t[SB_CH_MAXTAPS + 1]; uint32_t n; };
 struct ChChannels { uint32_t inc[SB_CH_MAXCH], phase0[SB_CH_MAXCH]; uint32_t n; };
 
-// k_channelize's staging.  k_fir_decimate2 below keeps a copy of these steps inline with its sizes as constants: keep the two in step.
-// Stages input samples [t0 - halo, t0 + tile + halo) of x[0 .. n_in) into s[0 .. tile + 2 halo), zero outside the buffer, with one bulk
-// copy (plus the 0..3 trailing samples by hand); when `nco` is not null one more bulk copy brings the SB_CH_NCO-word table to s_nco on the
-// same barrier.  halo is a multiple of 4 and t0 of SB_FIR_TILE, so the copy's source and destination are 16-byte aligned.  Every thread
-// of the CTA calls it; it returns after a __syncthreads with the window in place.
-__device__ __forceinline__ void stage_window(const uint32_t* __restrict__ x, uint64_t n_in, uint64_t t0, uint32_t tile, uint32_t halo,
-                                             uint32_t* s, const uint32_t* __restrict__ nco, uint32_t* s_nco, unsigned long long* bar) {
-    const uint32_t tid = threadIdx.x, nthr = blockDim.x, win = tile + 2 * halo;
-    // samples [lo, hi) of the buffer land in s[lo - (t0 - halo) ...]; everything else of the window is zero
-    const uint64_t w0 = t0 >= halo ? t0 - halo : 0ull;
-    const uint64_t w1 = t0 + tile + halo < n_in ? t0 + tile + halo : n_in;
-    const uint32_t dst0 = (uint32_t)(w0 - (t0 - halo));                // halo at the first tile, else 0 (t0 - halo wraps to w0 there)
+// Staging of k_channelize and k_channel_sim (sim_kernels.cuh).  k_fir_decimate2 below keeps a copy of these steps inline with its sizes as
+// constants: keep the two in step.  Stages input samples [lo, lo + win) of each of `rows` rows x + k * xstride (each x[0 .. n_in)) into
+// s + k * sstride, zero outside [0, n_in), with one bulk copy per row (plus the 0..3 trailing samples by hand); when `tab` is not null one
+// more bulk copy brings its tab_words words to s_tab on the same barrier.  lo (which may be negative), xstride and sstride are multiples
+// of 4 and x and s are 16-byte aligned, so every copy's source and destination are 16-byte aligned.  Every thread of the CTA calls it; it
+// returns after a __syncthreads with the windows in place.
+__device__ __forceinline__ void stage_window(const uint32_t* __restrict__ x, uint64_t xstride, uint32_t rows, uint64_t n_in, int64_t lo, uint32_t win,
+                                             uint32_t* s, uint32_t sstride, const uint32_t* __restrict__ tab, uint32_t tab_words, uint32_t* s_tab,
+                                             unsigned long long* bar) {
+    const uint32_t tid = threadIdx.x, nthr = blockDim.x;
+    // samples [w0, w1) of the buffer land in s[w0 - lo ...]; everything else of the window is zero
+    const int64_t hi = lo + (int64_t)win;
+    const uint64_t w0 = lo > 0 ? (uint64_t)lo : 0ull;
+    const uint64_t w1e = hi > 0 ? ((uint64_t)hi < n_in ? (uint64_t)hi : n_in) : 0ull, w1 = w1e > w0 ? w1e : w0;
+    const uint32_t dst0 = (uint32_t)((int64_t)w0 - lo);                // -lo while the window starts before the buffer, else 0
     const uint32_t nw = (uint32_t)(w1 - w0);
     const uint32_t bulk = nw & ~3u;                                     // whole 16-byte units by the copy engine, the last 0..3 samples by hand
-    // zero the parts of the window the copy will not write (buffer edges); done before the copy is started, different words
-    for (uint32_t i = tid; i < win; i += nthr) if (i < dst0 || i >= dst0 + bulk) s[i] = 0;
+    // zero the parts of the windows the copies will not write (buffer edges); done before the copies are started, different words
+    for (uint32_t k = 0; k < rows; k++)
+        for (uint32_t i = tid; i < win; i += nthr) if (i < dst0 || i >= dst0 + bulk) s[k * sstride + i] = 0;
     if (tid == 0) {
         asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(bar)));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     __syncthreads();
-    const uint32_t bytes = bulk * 4u + (nco ? SB_CH_NCO * 4u : 0u);
+    const uint32_t bytes = rows * bulk * 4u + (tab ? tab_words * 4u : 0u);
     if (tid == 0 && bytes) {
         const uint32_t mb = (uint32_t)__cvta_generic_to_shared(bar);
         asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes) : "memory");
-        if (bulk) asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                               :: "r"((uint32_t)__cvta_generic_to_shared(s + dst0)), "l"(x + w0), "r"(bulk * 4u), "r"(mb) : "memory");
-        if (nco) asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                              :: "r"((uint32_t)__cvta_generic_to_shared(s_nco)), "l"(nco), "r"(SB_CH_NCO * 4u), "r"(mb) : "memory");
+        if (bulk) for (uint32_t k = 0; k < rows; k++)
+            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                         :: "r"((uint32_t)__cvta_generic_to_shared(s + k * sstride + dst0)), "l"(x + k * xstride + w0), "r"(bulk * 4u), "r"(mb) : "memory");
+        if (tab) asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+                              :: "r"((uint32_t)__cvta_generic_to_shared(s_tab)), "l"(tab), "r"(tab_words * 4u), "r"(mb) : "memory");
     }
-    if (tid < (nw & 3u)) s[dst0 + bulk + tid] = __ldg(x + w0 + bulk + tid);
+    const uint32_t tail = nw & 3u;
+    if (tid < rows * tail) { const uint32_t k = tid / tail, q = tid % tail; s[k * sstride + dst0 + bulk + q] = __ldg(x + k * xstride + w0 + bulk + q); }
     if (bytes) {
         const uint32_t mb = (uint32_t)__cvta_generic_to_shared(bar); uint32_t ok = 0;
         while (!ok) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(ok) : "r"(mb) : "memory");
@@ -159,7 +165,7 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_channelize(const uint32_t* _
     const uint32_t ch0 = blockIdx.y * chan_per_group, ch1 = min(ch0 + chan_per_group, ch.n);
     bool rotate = false;                                                // the table is only brought in when a channel of the group needs it
     for (uint32_t k = ch0; k < ch1; k++) rotate |= ch.inc[k] != 0u || (ch.phase0[k] >> 20) != 0u;
-    stage_window(x, n_in, t0, SB_FIR_TILE, halo, s_x, rotate ? nco : nullptr, s_nco, s_bar);
+    stage_window(x, 0, 1, n_in, (int64_t)t0 - (int64_t)halo, win, s_x, 0, rotate ? nco : nullptr, SB_CH_NCO, s_nco, s_bar);
     // outputs m0 .. m1 of the tile: D m in [t0, t0 + tile); output m reads window words D m - (t0 - halo) - c + k, k = 0 .. ntaps-1
     const uint64_t m0 = (t0 + D - 1) / D, m1e = (t0 + SB_FIR_TILE + D - 1) / D, m1 = m1e < n_out ? m1e : n_out;
     const uint32_t nm = m1 > m0 ? (uint32_t)(m1 - m0) : 0u;

@@ -11,6 +11,7 @@
 #include "tx11a_legacy_kernels.cuh"
 #include "tx11n_kernels.cuh"
 #include "fir_kernels.cuh"
+#include "sim_kernels.cuh"
 #include <stdlib.h>
 #include <string>
 #include <vector>
@@ -273,6 +274,8 @@ struct sb200_handle {
     uint32_t ch_smem_set = 0;                          // bit J: k_channelize<J> may use SB_CH_SMEM bytes of dynamic shared memory on this device
     int sms = 0;                                       // multiprocessors of the device (channel groups of k_channelize)
     uint32_t cb_smem_set = 0;                          // bit J: k_combine<J> may use SB_CB_SMEM bytes of dynamic shared memory on this device
+    DevBuf simtab, simlink, simtap;                    // channel simulator: its table (sim_kernels.cuh, built on first use), staged links and taps
+    uint32_t sim_smem_set = 0;                         // bit J: k_channel_sim<J> may use its largest dynamic shared memory on this device
     DevBuf vring;
     std::string err;
     int fail(int code, const char* what, cudaError_t e = cudaSuccess) {
@@ -1045,6 +1048,135 @@ extern "C" int sb200_combine(sb200_handle* h, const int16_t* rows, uint64_t row_
     if (combine_smem(nchannels, interp, ntaps, 4 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, T, d_out);
     else if (combine_smem(nchannels, interp, ntaps, 2 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, T, d_out);
     else rc = combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, T, d_out);
+    return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
+}
+
+// The table of sb200_channel_sim (sim_kernels.cuh), uploaded on first use: the NCO of upload_nco, then H (256 rows of 8 Q14 taps, packed in
+// pairs like cs16) and LNT, from the closed forms of include/sora_b200.h.  I0 is its power series (tests/sim_model.py sums the same one).
+static double sim_i0(double x) {
+    double s = 1.0, t = 1.0; const double q = x * x / 4.0;
+    for (int k = 1; k < 32; k++) { t = t * (q / ((double)k * k)); s = s + t; }
+    return s;
+}
+static int upload_simtab(sb200_handle* h) {
+    if (h->simtab.p) return SB200_OK;
+    std::vector<uint32_t> t(SB_SIM_TAB);
+    for (int i = 0; i < SB_CH_NCO; i++) { const double a = 2.0 * M_PI * i / 4096.0; t[i] = pack(mk((int)nearbyint(16384.0 * cos(a)), (int)nearbyint(16384.0 * sin(a)))); }
+    const double i05 = sim_i0(5.0);
+    for (int p = 0; p < 256; p++) {
+        int hv[8];
+        for (int k = 0; k < 8; k++) {
+            const double d = k - 3 - p / 256.0, sinc = d == 0.0 ? 1.0 : sin(M_PI * d) / (M_PI * d);
+            hv[k] = (int)nearbyint(16384.0 * sinc * sim_i0(5.0 * sqrt(1.0 - (d / 4.0) * (d / 4.0))) / i05);
+        }
+        for (int k = 0; k < 4; k++) t[SB_CH_NCO + 4 * p + k] = pack(mk(hv[2 * k], hv[2 * k + 1]));
+    }
+    for (int j = 0; j < SB_SIM_LNT; j++) t[SB_CH_NCO + SB_SIM_H + j] = (uint32_t)nearbyint(-log((2048.0 + j + 0.5) / 4096.0) * 16777216.0);
+    cudaError_t e = h->simtab.need(SB_SIM_TAB * 4);
+    if (e == cudaSuccess) e = cudaMemcpy(h->simtab.p, t.data(), SB_SIM_TAB * 4, cudaMemcpyHostToDevice);
+    if (e == cudaSuccess) e = cudaDeviceSynchronize();   // landed before a kernel on a non-blocking stream reads it (TableArena::upload)
+    if (e != cudaSuccess) { h->simtab.release(); return h->fail(SB200_E_CUDA, "channel simulator table upload", e); }
+    return SB200_OK;
+}
+
+// Rows of length n at l * A + r * B (l < N, r < R) are pairwise disjoint: |dl A + dr B| >= n for every (dl, dr) != 0, |dl| < N, |dr| < R.
+// For each dr > 0 only the dl nearest -dr B / A (clamped) can come closest.
+static bool rows_disjoint(uint64_t A, uint64_t B, uint32_t N, uint32_t R, uint64_t n) {
+    if (N > 1 && A < n) return false;                  // dr = 0, dl = 1
+    for (uint32_t dr = 1; dr < R; dr++) {
+        const double b = (double)dr * (double)B;
+        const long long c = N > 1 ? (long long)floor(-b / (double)A) : 0;
+        for (long long dl = c - 1; dl <= c + 2; dl++) {
+            if (dl <= -(long long)N || dl >= (long long)N) continue;
+            const __int128 v = (__int128)dl * (__int128)A + (__int128)dr * (__int128)B;
+            if ((v < 0 ? -v : v) < (__int128)n) return false;
+        }
+    }
+    return true;
+}
+
+// One launch of k_channel_sim<J> (sim_kernels.cuh), between ev0 and the caller's finish_call.
+template <int J>
+static int sim_launch_j(sb200_handle* h, cudaStream_t st, SimArgs& a) {
+    const uint32_t tm = SB_FIR_THREADS * J;
+    if (!(h->sim_smem_set & (1u << J))) {
+        CK(cudaFuncSetAttribute(k_channel_sim<J>, cudaFuncAttributeMaxDynamicSharedMemorySize, sim_smem(SB_SIM_MAXROWS, SB_SIM_MAXROWS, SB_SIM_MAXTAPS, tm)));
+        h->sim_smem_set |= 1u << J;
+    }
+    a.ntiles = (uint32_t)((a.n_out + tm - 1) / tm);
+    CK(cudaEventRecord(h->ev0, st));
+    k_channel_sim<J><<<(unsigned)((uint64_t)a.ntiles * a.nlinks), SB_FIR_THREADS, sim_smem(a.T, a.R, a.L, tm), st>>>(a);
+    return SB200_OK;
+}
+
+// Radio channel simulator (sim_kernels.cuh): every link's input rows through its clock offset, taps, carrier offset and noise.  Tiles of 2048
+// outputs for T <= 2 and of 1024 for T = 4, which keeps the shared memory at most 68 KB.
+extern "C" int sb200_channel_sim(sb200_handle* h, const int16_t* x, uint64_t in_link_stride, uint64_t in_row_stride, uint32_t ntx, uint64_t n_in,
+                                 const sb200_link* links, const int16_t* taps, uint32_t ntaps, uint32_t nlinks,
+                                 uint64_t seed, int16_t* y, uint64_t out_link_stride, uint64_t out_row_stride, uint32_t nrx, uint64_t n_out, void* cuda_stream) {
+    if (!h) return SB200_E_INVALID;
+    if (!x || !links || !taps || !y) return h->fail(SB200_E_INVALID, "null argument");
+    if (ntx < 1 || ntx > SB_SIM_MAXROWS || nrx < 1 || nrx > SB_SIM_MAXROWS) return h->fail(SB200_E_INVALID, "ntx and nrx must be 1 .. 4");
+    if (ntaps < 1 || ntaps > SB_SIM_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be 1 .. 64");
+    if (n_in > (1ull << 30) || n_out > (1ull << 30)) return h->fail(SB200_E_INVALID, "n_in and n_out must be at most 2^30");
+    if ((in_link_stride | in_row_stride | out_link_stride | out_row_stride) & 3u) return h->fail(SB200_E_INVALID, "strides must be multiples of 4");
+    if ((in_link_stride | in_row_stride | out_link_stride | out_row_stride) >> 40) return h->fail(SB200_E_INVALID, "strides must be below 2^40");
+    if (!rows_disjoint(out_link_stride, out_row_stride, nlinks, nrx, n_out)) return h->fail(SB200_E_INVALID, "output rows overlap");
+    if (nlinks == 0 || n_out == 0) return SB200_OK;
+    const uint32_t T = ntx, R = nrx, L = ntaps;
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    CK(cudaSetDevice(h->device));
+    const bool x_dev = is_device_ptr(x), y_dev = is_device_ptr(y), l_dev = is_device_ptr(links), t_dev = is_device_ptr(taps);
+    if ((x_dev && ((uintptr_t)x & 15u)) || (y_dev && ((uintptr_t)y & 15u))) return h->fail(SB200_E_INVALID, "device x and y must be 16-byte aligned");
+    if ((t_dev && ((uintptr_t)taps & 3u)) || (l_dev && ((uintptr_t)links & 7u))) return h->fail(SB200_E_INVALID, "device taps must be 4-byte and device links 8-byte aligned");
+    const uint64_t ntap_words = (uint64_t)nlinks * R * T * L;
+    if (!l_dev && !t_dev) {                            // host tables: checked here
+        for (uint32_t l = 0; l < nlinks; l++) {
+            const sb200_link& k = links[l];
+            if (k.step < (1ull << 32) - (1ull << 24) || k.step > (1ull << 32) + (1ull << 24)) return h->fail(SB200_E_INVALID, "step must be within 2^32 +- 2^24");
+            if (k.tau0 >= (1ull << 62)) return h->fail(SB200_E_INVALID, "tau0 must be below 2^62");
+            if (k.noise_q8 >= (1u << 24)) return h->fail(SB200_E_INVALID, "noise_q8 must be below 2^24");
+        }
+        for (uint64_t i = 0; i < (uint64_t)nlinks * R; i++) {
+            uint32_t sum = 0; const int16_t* g = taps + i * T * L * 2;
+            for (uint32_t q = 0; q < 2 * T * L; q++) sum += (uint32_t)abs((int)g[q]);
+            if (sum > 65535u) return h->fail(SB200_E_INVALID, "sum of |g.re| + |g.im| over t and j must be at most 65535 for every link and output row");
+        }
+    }
+    CallScope call(h, st); CK(call.begin()); call.reads(x); call.reads(links); call.reads(taps);
+    const sb200_link* d_links; const uint32_t* d_taps;
+    CK(to_device(h->simlink, links, l_dev, nlinks * sizeof(sb200_link), st, &d_links));
+    CK(to_device(h->simtap, (const uint32_t*)taps, t_dev, ntap_words * 4ull, st, &d_taps));
+    if (l_dev || t_dev) {                              // a table on the device: its limits checked there, one 4-byte read-back
+        CK(h->slotchk.need(8));
+        CK(cudaMemsetAsync(h->slotchk.p, 0, 4, st));
+        const uint64_t nt = (uint64_t)nlinks * R;
+        k_sim_check<<<(unsigned)((nt + 255) / 256), 256, 0, st>>>(d_links, (const int16_t*)d_taps, nlinks, R, T, L, (uint32_t*)h->slotchk.p);
+        uint32_t bad = 0;
+        CK(cudaMemcpyAsync(&bad, h->slotchk.p, 4, cudaMemcpyDeviceToHost, st));
+        CK(cudaStreamSynchronize(st));
+        if (bad) return h->fail(SB200_E_INVALID, "a link record or tap sum is out of its limits (step, tau0, noise_q8 or sum of |g| > 65535)");
+    }
+    const int trc = upload_simtab(h);
+    if (trc != SB200_OK) return trc;
+    SimArgs a; memset(&a, 0, sizeof a);
+    a.T = T; a.R = R; a.L = L; a.nlinks = nlinks; a.n_in = n_in; a.n_out = n_out; a.seed = seed;
+    a.links = d_links; a.taps = d_taps; a.tab = (const uint32_t*)h->simtab.p;
+    a.in_link = in_link_stride; a.in_row = in_row_stride; a.out_link = out_link_stride; a.out_row = out_row_stride;
+    if (x_dev) a.x = (const uint32_t*)x;
+    else {                                             // the whole span of the rows, strides kept (rows may share samples: a stride may be 0)
+        const uint64_t span = (uint64_t)(nlinks - 1) * in_link_stride + (uint64_t)(T - 1) * in_row_stride + n_in;
+        CK(to_device(h->iq, (const uint32_t*)x, false, span * 4ull, st, &a.x, 16));
+    }
+    Returns ret;
+    if (y_dev) a.y = (uint32_t*)y;
+    else {                                             // rows n_out (rounded to 4) apart in the workspace, copied into the caller's rows row by row
+        const uint64_t no4 = (n_out + 3) & ~3ull;
+        CK(h->iq40.need((uint64_t)nlinks * R * no4 * 4ull + 16)); a.y = (uint32_t*)h->iq40.p; a.out_row = no4; a.out_link = R * no4;
+        for (uint32_t r = 0; r < R; r++)
+            ret.bind2d(y + 2 * r * out_row_stride, (nlinks > 1 ? out_link_stride : n_out) * 4ull, a.y + r * no4, R * no4 * 4ull, n_out * 4ull, nlinks);
+    }
+    const int rc = T <= 2 ? sim_launch_j<8>(h, st, a) : sim_launch_j<4>(h, st, a);
     return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
 }
 
