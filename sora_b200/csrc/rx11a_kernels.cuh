@@ -4,7 +4,7 @@
 //                state machine, up to the vector where the reference switches to the demod branch.
 //                Reference: samples.hpp:27-49 (TDownSample2), dc.hpp:48-166, cca.hpp:106-441 (TCCA11a),
 //                fb11a_demod.cpp:29-81 (per-28-sample-block error polling, CS-timeout reset).
-//   k_front11a   one half-warp per slot: LTS (fine CFO, FFT, channel estimate), then per OFDM symbol
+//   k_front11a   one quarter-warp per slot: LTS (fine CFO, FFT, channel estimate), then per OFDM symbol
 //                CP strip -> freq comp -> FFT64 -> equalise -> phase comp -> pilot track -> soft demap ->
 //                de-interleave; SIGNAL decoded in-warp (K=7 Viterbi, 24 steps) and parsed.  Samples stay packed complex
 //                int16 words from the load through the FFT to the demapper (pk_* in fixed.cuh, bit-exact to the scalar forms);
@@ -227,7 +227,7 @@ __device__ __forceinline__ uint32_t warp_viterbi_signal(const uint8_t* soft, uin
 }
 
 // ------------------------------------------------------------------------------------------------
-// front end: one half-warp per slot
+// front end: one quarter-warp per slot
 // ------------------------------------------------------------------------------------------------
 struct FrontTaps {            // optional stage taps (device pointers, nullptr = off); per slot, per symbol, 64 packed c16
     uint32_t* freq_coeffs; uint32_t* chan_coeffs; uint32_t* fft_out; uint32_t* equalized; uint32_t* tracked; uint32_t max_sym;
@@ -242,85 +242,101 @@ __device__ __forceinline__ int data_index(int bin) {   // demapper11a.hpp:22-36 
 __device__ __forceinline__ int data_bin(int d) {       // inverse of data_index, d = 0..47
     return d < 24 ? 38 + d + (d >= 5) + (d >= 18) : d - 23 + (d >= 30) + (d >= 43);
 }
-// Post-FFT role of lane hl of a half-warp: four bins.  Lanes 0-11 own the data-subcarrier pairs (d, d + 3), d = 6 (p / 3) + p % 3 for
-// p = hl (bins 0, 1) and p = hl + 12 (bins 2, 3), in demapper order: at 64-QAM the 802.11a de-interleaver puts coded bit i of d at an even
-// position and bit (2 0 1 5 3 4)[i] of d + 3 right after it, so a pair's soft bits leave as six 16-bit stores.  Lanes 12-15 own one pilot
-// each in bin 0 (43, 57, 7, 21) and three of the twelve zero bins (0, 27..37) in bins 1-3.
-__device__ __forceinline__ int front_pair(int hl, int p) { const int q = hl + 12 * p; return 6 * (q / 3) + q % 3; }
-__device__ __forceinline__ int front_bin(int hl, int i) {
-    if (hl < 12) return data_bin(front_pair(hl, i >> 1) + 3 * (i & 1));
-    const int j = hl - 12, m = 3 * j + i - 1;
-    return i == 0 ? (0x1507392B >> (8 * j)) & 0xFF : m ? 26 + m : 0;
+// Post-FFT role of lane ql of a quarter-warp: eight bins.  Bins 0-5 are three data-subcarrier pairs (d, d + 3), d = 6 (q / 3) + q % 3
+// for q = ql + 8 p, p = 0..2 (bins 2 p, 2 p + 1), in demapper order: at 64-QAM the 802.11a de-interleaver puts coded bit i of d at an
+// even position and bit (2 0 1 5 3 4)[i] of d + 3 right after it, so a pair's soft bits leave as six 16-bit stores.  Bin 6 is a pilot in
+// lanes 0-3 (43, 57, 7, 21) and a zero bin in lanes 4-7, bin 7 a zero bin in every lane: of the twelve zero bins z(m) (0, 27..37),
+// lane ql holds z(ql) in bin 7 and, from lane 4 on, z(ql + 4) in bin 6.  Every lane so demaps three pairs and walks one pilot angle
+// (bin 6; lanes 4-7 walk a zero bin's and nobody reads it), and bin 7 needs no work behind the FFT but the stage taps.
+__device__ __forceinline__ int front_pair(int ql, int p) { const int q = ql + 8 * p; return 6 * (q / 3) + q % 3; }
+__device__ __forceinline__ int front_zero(int m) { return m ? 26 + m : 0; }
+__device__ __forceinline__ int front_bin(int ql, int i) {
+    if (i < 6) return data_bin(front_pair(ql, i >> 1) + 3 * (i & 1));
+    if (i == 7) return front_zero(ql);
+    return ql < 4 ? (0x1507392B >> (8 * ql)) & 0xFF : front_zero(ql + 4);
 }
 
 #define SB_FRONT_WARPS 4
-#define SB_FRONT_SLOTS (2 * SB_FRONT_WARPS)   // capture slots per CTA, one per half-warp
+#define SB_FRONT_SLOTS (4 * SB_FRONT_WARPS)   // capture slots per CTA, one per quarter-warp
 #ifndef SB_FRONT_MINB
-#define SB_FRONT_MINB 5           // resident CTAs per SM the register allocation aims at (tools/front_sweep.sh, DESIGN.md §8)
+#define SB_FRONT_MINB 4           // resident CTAs per SM the register allocation aims at (tools/front_sweep.sh, DESIGN.md §8)
 #endif
-// Each half-warp decodes its own slot, and both run the same instruction stream: lanes 0-15 slot 2 w, lanes 16-31 slot 2 w + 1 of warp w.
-// Per OFDM symbol a half runs the three radix stages of its slot's 64-point FFT (16 butterflies per stage = 16 lanes), the first stage
-// straight from the freq-compensated time samples in registers; behind the FFT each lane owns four bins (front_bin), and the work that
-// does not grow with the bins a lane owns (pilot angle walk, tracker, control) serves both slots at once.  A half whose slot ended, failed
-// its header or held no frame idles in the loop with the other one, so every full-mask shuffle and __syncwarp still sees all 32 lanes.
+#define SB_FRONT_FFT_ROW 68       // words per quarter's FFT buffer: the radix-16 stage's loads of the four quarters fall on distinct banks
+#define SB_FRONT_LANE_ROW 52      // words per lane of per-lane constants: 16-byte loads of the eight lanes of a quarter on distinct banks
+#define SB_FRONT_STAGE_WORDS 168  // STAGE 2: words per staging buffer (160 words of a symbol at 40 Msps + alignment slack)
+#define SB_FRONT_STAGE_SMEM (SB_FRONT_WARPS * 4 * 2 * SB_FRONT_STAGE_WORDS * 4)   // STAGE 2's dynamic shared memory per CTA, bytes
+// Each quarter-warp decodes its own slot, and all four run the same instruction stream: lanes 8 s .. 8 s + 7 slot 4 w + s of warp w.
+// Per OFDM symbol a quarter runs the three radix stages of its slot's 64-point FFT (16 butterflies per stage, two per lane), the first
+// stage straight from the freq-compensated time samples in registers; behind the FFT each lane owns eight bins (front_bin), and the work
+// that does not grow with the bins a lane owns (pilot angle walk, tracker, control) serves four slots at once.  A quarter whose slot ended,
+// failed its header or held no frame idles in the loop with the others, so every full-mask shuffle and __syncwarp still sees all 32 lanes.
 // STAGE: how the time samples of the symbols reach the FFT (A/B of the staging experiment, DESIGN.md §4):
-//   0  loaded straight into registers right before the transform (round 1);
-//   1  the next symbol's samples are loaded into registers while the current one is processed (register double buffer);
-//   2  one lane of each half starts a 1-D bulk asynchronous copy (cp.async.bulk, the TMA unit; SASS UBLKCP) of its slot's next symbol into a
-//      shared-memory double buffer, completion on an mbarrier; the lanes then read their samples from shared memory.
+//   0  loaded straight into registers right before the transform;
+//   1  the next symbol's samples are loaded into registers while the current one is processed (register double buffer; the default);
+//   2  one lane of each quarter starts a 1-D bulk asynchronous copy (cp.async.bulk, the TMA unit; SASS UBLKCP) of its slot's next symbol
+//      into a shared-memory double buffer (dynamic shared memory, SB_FRONT_STAGE_SMEM), completion on an mbarrier; the lanes then read
+//      their samples from shared memory.
 template <int STAGE>
 __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a(const uint32_t* __restrict__ iq, const uint64_t* __restrict__ off,
         const uint32_t* __restrict__ len, uint32_t nframes, DevTables T, FrameInfo* __restrict__ info,
         uint8_t* __restrict__ soft_out, uint64_t soft_stride, const uint16_t* __restrict__ inv_deint, FrontTaps taps, uint32_t sh, uint32_t lsh) {
-    __shared__ uint32_t s_fft[SB_FRONT_WARPS][2][64];
-    __shared__ __align__(16) uint8_t s_soft[SB_FRONT_WARPS][2][288];
+    __shared__ __align__(16) uint32_t s_fft[SB_FRONT_WARPS][4][SB_FRONT_FFT_ROW];
+    __shared__ __align__(16) uint8_t s_soft[SB_FRONT_WARPS][4][288];
     __shared__ uint32_t s_demap[256];                  // per input value: [bpsk/qpsk/first bit | 16-QAM second | 64-QAM second | 64-QAM third] soft bits
     __shared__ uint8_t s_pilot[128];
-    __shared__ uint32_t s_dec[SB_FRONT_WARPS][2][48];  // SIGNAL decoder's decision ballots
-    // Per-lane constants of the symbol loop, kept out of the registers: words 0-11 the equaliser factors of the four bins (cfac re, im, nim),
-    // 12-23 the soft-bit positions of the two pairs (see load_positions), 24-27 the signed subcarrier numbers.  A row is 28 words, so
-    // the 16-byte loads of eight consecutive lanes fall on distinct banks.
-    __shared__ __align__(16) int s_lane[SB_FRONT_WARPS][32][28];
-    __shared__ __align__(16) uint32_t s_stage[STAGE == 2 ? SB_FRONT_WARPS : 1][2][2][STAGE == 2 ? 168 : 4];   // per half 2 x (160 words of a symbol + alignment slack)
-    __shared__ __align__(8) unsigned long long s_mbar[STAGE == 2 ? SB_FRONT_WARPS : 1][2][2];
+    __shared__ uint32_t s_dec[SB_FRONT_WARPS][48];     // SIGNAL decoder's decision ballots, one SIGNAL at a time
+    // Per-lane constants of the symbol loop, kept out of the registers: words 0-23 the equaliser factors of the eight bins (cfac re, im,
+    // nim), 24-31 the signed subcarrier numbers, 32-49 the soft-bit positions of the three pairs (see load_positions).
+    __shared__ __align__(16) int s_lane[SB_FRONT_WARPS][32][SB_FRONT_LANE_ROW];
+    extern __shared__ __align__(16) uint32_t s_stage[];   // STAGE 2: [SB_FRONT_WARPS][4 quarters][2 buffers][SB_FRONT_STAGE_WORDS]
+    __shared__ __align__(8) unsigned long long s_mbar[STAGE == 2 ? SB_FRONT_WARPS : 1][4][2];
     const unsigned FULL = 0xFFFFFFFFu;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
-    const int half = lane >> 4, hl = lane & 15;
-    if (STAGE == 2 && hl == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][half][0])));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][half][1])));
+    const int qt = lane >> 3, ql = lane & 7;
+    if (STAGE == 2 && ql == 0) {
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][qt][0])));
+        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][qt][1])));
         asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     }
     for (int i = threadIdx.x; i < 256; i += blockDim.x)
         s_demap[i] = (uint32_t)__ldg(T.demap + i) | ((uint32_t)__ldg(T.demap + 256 + i) << 8) | ((uint32_t)__ldg(T.demap + 512 + i) << 16) | ((uint32_t)__ldg(T.demap + 768 + i) << 24);
     for (int i = threadIdx.x; i < 128; i += blockDim.x) s_pilot[i] = __ldg(T.pilot_neg + i);
     __syncthreads();
-    const uint32_t f = 2u * (blockIdx.x * SB_FRONT_WARPS + (uint32_t)wib) + (uint32_t)half;
+    const uint32_t f = 4u * (blockIdx.x * SB_FRONT_WARPS + (uint32_t)wib) + (uint32_t)qt;
     FrameInfo fi;
-    bool act = f < nframes;                            // this half's slot is still being decoded
+    bool act = f < nframes;                            // this quarter's slot is still being decoded
     if (act) { fi = info[f]; act = fi.status == E_SUCCESS; }
     const uint32_t* x = iq + (act ? off[f] : 0);
     const uint32_t nvec = act ? ((len[f] << lsh) / 28u) * 28u / 8u : 0u;
     const uint32_t s0 = fi.detect_vec * 4u;            // first 20 Msps sample of the 144-sample LTS block
-    if (act && fi.detect_vec + 36u > nvec) { if (hl == 0) info[f].status = E_NO_FRAME; act = false; }
-    const bool own = act;                              // this half writes its slot's FrameInfo back at the end
+    if (act && fi.detect_vec + 36u > nvec) { if (ql == 0) info[f].status = E_NO_FRAME; act = false; }
+    const bool own = act;                              // this quarter writes its slot's FrameInfo back at the end
     if (!__any_sync(FULL, act)) return;
-    const cfac w64_1 = fac_tw(unpack(__ldg(T.tw64 + hl))), w64_2 = fac_tw(unpack(__ldg(T.tw64 + 16 + hl))), w64_3 = fac_tw(unpack(__ldg(T.tw64 + 32 + hl)));
-    const cfac w16_1 = fac_tw(unpack(__ldg(T.tw16 + (hl & 3)))), w16_2 = fac_tw(unpack(__ldg(T.tw16 + 4 + (hl & 3)))), w16_3 = fac_tw(unpack(__ldg(T.tw16 + 8 + (hl & 3))));
-    uint32_t* const xb = s_fft[wib][half];
-    // 64-point FFT of four freq-compensated time samples per lane (n = hl + 16 j), this half-warp's buffer; packed words throughout
-    auto fft_from_regs = [&](uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
-        pk_r4_butterfly(a, b, c, d, w64_1, w64_2, w64_3);                   // FFTSSE<64>, butterfly e = hl
-        xb[hl] = a; xb[hl + 16] = b; xb[hl + 32] = c; xb[hl + 48] = d;
+    // FFTSSE<64> butterflies e = ql (twiddles wa) and e = ql + 8 (wb); FFTSSE<16> butterflies b = ql and b = ql + 8 share twiddle ql & 3
+    const cfac wa1 = fac_tw(unpack(__ldg(T.tw64 + ql))), wa2 = fac_tw(unpack(__ldg(T.tw64 + 16 + ql))), wa3 = fac_tw(unpack(__ldg(T.tw64 + 32 + ql)));
+    const cfac wb1 = fac_tw(unpack(__ldg(T.tw64 + 8 + ql))), wb2 = fac_tw(unpack(__ldg(T.tw64 + 24 + ql))), wb3 = fac_tw(unpack(__ldg(T.tw64 + 40 + ql)));
+    const cfac w16_1 = fac_tw(unpack(__ldg(T.tw16 + (ql & 3)))), w16_2 = fac_tw(unpack(__ldg(T.tw16 + 4 + (ql & 3)))), w16_3 = fac_tw(unpack(__ldg(T.tw16 + 8 + (ql & 3))));
+    uint32_t* const xb = s_fft[wib][qt];
+    // 64-point FFT of eight freq-compensated time samples per lane (v[k] = sample ql + 8 k), this quarter's buffer; packed words throughout
+    auto fft_from_regs = [&](uint32_t (&v)[8]) {
+        pk_r4_butterfly(v[0], v[2], v[4], v[6], wa1, wa2, wa3);            // FFTSSE<64>, butterfly e = ql: samples e, e + 16, e + 32, e + 48
+        pk_r4_butterfly(v[1], v[3], v[5], v[7], wb1, wb2, wb3);            // butterfly e = ql + 8
+#pragma unroll
+        for (int k = 0; k < 8; k++) xb[ql + 8 * k] = v[k];
         __syncwarp();
-        {   const int base = (hl >> 2) * 16 + (hl & 3);                    // 4 x FFTSSE<16>
+        {   const int base = (ql >> 2) * 16 + (ql & 3);                    // 4 x FFTSSE<16>: butterflies b = ql (base) and b = ql + 8 (base + 32)
             uint32_t p = xb[base], q = xb[base + 4], r = xb[base + 8], t = xb[base + 12];
+            uint32_t p2 = xb[base + 32], q2 = xb[base + 36], r2 = xb[base + 40], t2 = xb[base + 44];
             pk_r4_butterfly(p, q, r, t, w16_1, w16_2, w16_3);
-            xb[base] = p; xb[base + 4] = q; xb[base + 8] = r; xb[base + 12] = t; }
+            pk_r4_butterfly(p2, q2, r2, t2, w16_1, w16_2, w16_3);
+            xb[base] = p; xb[base + 4] = q; xb[base + 8] = r; xb[base + 12] = t;
+            xb[base + 32] = p2; xb[base + 36] = q2; xb[base + 40] = r2; xb[base + 44] = t2; }
         __syncwarp();
-        {   uint32_t p = xb[4 * hl], q = xb[4 * hl + 1], r = xb[4 * hl + 2], t = xb[4 * hl + 3];
-            pk_dft4(p, q, r, t);                                            // 16 x FFTSSEEx<4>
-            xb[4 * hl] = p; xb[4 * hl + 1] = q; xb[4 * hl + 2] = r; xb[4 * hl + 3] = t; }
+        {   uint4* const x4 = (uint4*)xb;                                  // 16 x FFTSSEEx<4>: vectors ql and ql + 8, one 16-byte word each
+            uint4 a = x4[ql], b = x4[ql + 8];
+            pk_dft4(a.x, a.y, a.z, a.w);
+            pk_dft4(b.x, b.y, b.z, b.w);
+            x4[ql] = a; x4[ql + 8] = b; }
         __syncwarp();
     };
     // ---- T11aLTS (channel_11a.hpp:34-230) -----------------------------------------------------------
@@ -328,32 +344,32 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
         int sr = 0, si = 0;
         if (act) {
 #pragma unroll
-            for (int j = 0; j < 4; j++) {
-                const uint32_t n = (uint32_t)hl + 16u * j;
+            for (int j = 0; j < 8; j++) {
+                const uint32_t n = (uint32_t)ql + 8u * j;
                 const cs16 l = sra(unpack(__ldg(x + ((s0 + 8u + n) << sh))), 1), h = unpack(__ldg(x + ((s0 + 72u + n) << sh)));
                 int re, im; cmul_conj32(re, im, h, l);
                 sr = wadd(sr, re >> 5); si = wadd(si, im >> 5);
             }
         }
-        for (int o = 8; o; o >>= 1) { sr = wadd(sr, __shfl_xor_sync(FULL, sr, o)); si = wadd(si, __shfl_xor_sync(FULL, si, o)); }
+        for (int o = 4; o; o >>= 1) { sr = wadd(sr, __shfl_xor_sync(FULL, sr, o)); si = wadd(si, __shfl_xor_sync(FULL, si, o)); }
         fi.cfo_est = (int)(short)(((uint32_t)d_uatan2(T, si, sr)) / 64u);  // short / size_t (dspalg.hpp:242)
     }
-    rfac fcv[4];                                       // FreqCoeffs of this lane's four time samples (dspalg.hpp:201-208)
+    rfac fcv[8];                                       // FreqCoeffs of this lane's eight time samples (dspalg.hpp:201-208)
 #pragma unroll
-    for (int j = 0; j < 4; j++) fcv[j] = fac_rotw(d_rotw(T, fi.cfo_est * (hl + 16 * j)));
+    for (int j = 0; j < 8; j++) fcv[j] = fac_rotw(d_rotw(T, fi.cfo_est * (ql + 8 * j)));
     auto fcomp = [&](uint32_t w, int j) { return pk_cmul((int)(short)w >> 1, (int)w >> 17, fcv[j]); };   // cmul_q15(sra(w, 1), FreqCoeffs)
-    auto load4 = [&](uint32_t first, uint32_t (&v)[4]) {  // (x >> 1) * FreqCoeffs for samples first + hl + 16 j; zeros in a half that idles
+    auto load8 = [&](uint32_t first, uint32_t (&v)[8]) {  // (x >> 1) * FreqCoeffs for samples first + ql + 8 j; zeros in a quarter that idles
 #pragma unroll
-        for (int j = 0; j < 4; j++) v[j] = 0u;
+        for (int j = 0; j < 8; j++) v[j] = 0u;
         if (act) {
 #pragma unroll
-            for (int j = 0; j < 4; j++) v[j] = fcomp(__ldg(x + ((first + hl + 16u * j) << sh)), j);
+            for (int j = 0; j < 8; j++) v[j] = fcomp(__ldg(x + ((first + ql + 8u * j) << sh)), j);
         }
     };
-    {   uint32_t v[4]; load4(s0 + 8u, v); fft_from_regs(v[0], v[1], v[2], v[3]); }     // LTS1
+    {   uint32_t v[8]; load8(s0 + 8u, v); fft_from_regs(v); }      // LTS1
     int* const tab = s_lane[wib][lane];
     const int4* const tab4 = (const int4*)tab;
-    int rb[4];                                         // where bin i of this lane sits in the bit-reversed FFT output
+    int rb[8];                                         // where bin i of this lane sits in the bit-reversed FFT output
     {   // channel_11a.hpp:124-171: H^-1 = (+-1600 conj(Y)) / (|Y|^2 >> 8), C integer division
         auto inv = [&](cs16 y, int bin) -> cs16 {
             if (bin >= 28 && bin <= 35) return mk(0, 0);
@@ -363,8 +379,8 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
             return e ? mk(sx16(re / e), sx16(im / e)) : mk(0, 0);
         };
 #pragma unroll
-        for (int i = 0; i < 4; i++) {
-            const int b = front_bin(hl, i);
+        for (int i = 0; i < 8; i++) {
+            const int b = front_bin(ql, i);
             rb[i] = bitrev6(b);
             const cs16 ch = inv(unpack(xb[rb[i]]), b);
             // bins 28..35 (SSE vectors 7,8) are forced to zero: their channel coefficient is zero, so is everything multiplied by it
@@ -376,82 +392,89 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
     }
     __syncwarp();
     // ---- symbols -----------------------------------------------------------------------------------
-    rfac comp[4];
+    rfac comp[7];                                      // bins 0-6; bin 7 is never rotated
 #pragma unroll
-    for (int i = 0; i < 4; i++) comp[i] = fac_rotw(0x7fffu);
+    for (int i = 0; i < 7; i++) comp[i] = fac_rotw(0x7fffu);
     // The tracker's accumulators only ever index the rotation table (mod 2^16) and feed each other by addition, so they wrap mod 2^32
     // instead of being truncated with sx16 at every step: the low 16 bits are the same.
     uint32_t CFO_comp = 0, SFO_comp = 0, CFO_tr = 0, SFO_tr = 0; unsigned symbol_count = 127;
     uint32_t remain = 0; uint32_t soft_bytes = 0; int nbpsc = 1;
     uint8_t* sout = soft_out + (size_t)f * soft_stride;
     uint32_t status = E_SUCCESS;
-    // Where this lane's soft bits go after de-interleaving, as byte offsets into s_soft, words 12 + 6 p + i of the lane's row for pair p: at
+    // Where this lane's soft bits go after de-interleaving, as byte offsets into s_soft, words 32 + 6 p + i of the lane's row for pair p: at
     // 64-QAM bit i of d is at the even position (the 16-bit store of the pair); at the other rates the low half is bit i of d, the high half
     // bit i of d + 3.
     auto load_positions = [&](int nb) {
         const uint16_t* inv = inv_deint + (nb == 1 ? 0 : nb == 2 ? 48 : nb == 4 ? 144 : 336);
-        const uint32_t base = (uint32_t)(2 * wib + half) * 288u;
+        const uint32_t base = (uint32_t)(4 * wib + qt) * 288u;
 #pragma unroll
-        for (int p = 0; p < 2; p++) {
-            const int d = front_pair(hl, p);
+        for (int p = 0; p < 3; p++) {
+            const int d = front_pair(ql, p);
 #pragma unroll
             for (int i = 0; i < 6; i++) {
                 uint32_t w = 0;
-                if (hl < 12 && i < nb) w = nb == 6 ? base + __ldg(inv + d * 6 + i) : (base + __ldg(inv + d * nb + i)) | ((base + __ldg(inv + (d + 3) * nb + i)) << 16);
-                tab[12 + 6 * p + i] = (int)w;
+                if (i < nb) w = nb == 6 ? base + __ldg(inv + d * 6 + i) : (base + __ldg(inv + d * nb + i)) | ((base + __ldg(inv + (d + 3) * nb + i)) << 16);
+                tab[32 + 6 * p + i] = (int)w;
             }
         }
     };
     load_positions(1);
     uint8_t* const s8 = &s_soft[0][0][0];
-    const bool rot123 = hl < 12;                       // bins 1-3 are rotated data subcarriers (bin 0 is data or a pilot: rotated anyway)
-    // everything behind the FFT for symbol `sym` of this half's slot, whose spectrum sits in xb
+    const bool pil = ql < 4;                           // bin 6 is a pilot (rotated) here, a zero bin in lanes 4-7
+    // everything behind the FFT for symbol `sym` of this quarter's slot, whose spectrum sits in xb
     auto post_fft = [&](uint32_t sym) {
-        const int4 q0 = tab4[0], q1 = tab4[1], q2 = tab4[2], kq = tab4[6];
-        const cfac eq[4] = {{q0.x, q0.y, q0.z}, {q0.w, q1.x, q1.y}, {q1.z, q1.w, q2.x}, {q2.y, q2.z, q2.w}};
-        const int k[4] = {kq.x, kq.y, kq.z, kq.w};
-        uint32_t F[4]; int ex[4], ey[4], C[4][2];
+        const int4 q0 = tab4[0], q1 = tab4[1], q2 = tab4[2], q3 = tab4[3], q4 = tab4[4], q5 = tab4[5], k0 = tab4[6], k1 = tab4[7];
+        const cfac eq[7] = {{q0.x, q0.y, q0.z}, {q0.w, q1.x, q1.y}, {q1.z, q1.w, q2.x}, {q2.y, q2.z, q2.w},
+                            {q3.x, q3.y, q3.z}, {q3.w, q4.x, q4.y}, {q4.z, q4.w, q5.x}};
+        const int k[7] = {k0.x, k0.y, k0.z, k0.w, k1.x, k1.y, k1.z};
+        uint32_t F[7]; int ex[7], ey[7], C[7][2];
 #pragma unroll
-        for (int i = 0; i < 4; i++) {
+        for (int i = 0; i < 7; i++) {
             F[i] = xb[rb[i]];
             int cx, cy;                                                                  // products as 32-bit sums, value = sum >> 16
             pk_cmul_xy((int)(short)F[i], (int)F[i] >> 16, eq[i], ex[i], ey[i]);          // channel_11a.hpp:551-579
             pk_cmul_xy(ex[i] >> 16, ey[i] >> 16, comp[i], cx, cy);                       // freqoffset.hpp:28-30
             C[i][0] = cx >> 16; C[i][1] = cy >> 16;
         }
-        // pilot.hpp:168-232: one table walk for both slots, the pilots sit in bin 0 of lanes 12-15 of each half (43, 57, 7, 21; 21's is sent negated)
-        const bool neg = hl == 15;
-        const int th = turn_pi(d_uatan2(T, neg ? -C[0][1] : C[0][1], neg ? -C[0][0] : C[0][0]), s_pilot[symbol_count]);
-        const int th1 = __shfl_sync(FULL, th, 12, 16), th2 = __shfl_sync(FULL, th, 13, 16), th3 = __shfl_sync(FULL, th, 14, 16), th4 = __shfl_sync(FULL, th, 15, 16);
+        // pilot.hpp:168-232: one table walk for four slots, the pilots sit in bin 6 of lanes 0-3 of each quarter (43, 57, 7, 21; 21's is sent negated)
+        const bool neg = ql == 3;
+        const int th = turn_pi(d_uatan2(T, neg ? -C[6][1] : C[6][1], neg ? -C[6][0] : C[6][0]), s_pilot[symbol_count]);
+        const int th1 = __shfl_sync(FULL, th, 0, 8), th2 = __shfl_sync(FULL, th, 1, 8), th3 = __shfl_sync(FULL, th, 2, 8), th4 = __shfl_sync(FULL, th, 3, 8);
         symbol_count++; if (symbol_count >= 127) symbol_count = 0;
         // the angles are int16, so the sum / 4 lies in [-32768, 32767] and each difference / 28 in [-2340, 2340]: the sx16 of both is the identity
         const int avg = (th1 + th2 + th3 + th4) / 4;
         const int del = ((th3 - th1) / 28 + (th4 - th2) / 28) >> 1;
         CFO_tr += (uint32_t)(avg >> 2); SFO_tr += (uint32_t)(del >> 2);
         CFO_comp += (uint32_t)avg + CFO_tr; SFO_comp += (uint32_t)del + SFO_tr;
-        // subcarriers -26..-1, 1..26 are rotated, every other bin (zero bins 1-3 of lanes 12-15) becomes zero
-        uint32_t R[4];
+        // subcarriers -26..-1, 1..26 are rotated, every other bin (bin 6 of lanes 4-7, bin 7) becomes zero
+        uint32_t R[7];
 #pragma unroll
-        for (int i = 0; i < 4; i++) {
+        for (int i = 0; i < 7; i++) {
             // next symbol's phase compensation; only the rotated bins use it, every other bin's R is zero whatever its C
             comp[i] = fac_rotw(d_rotw(T, (int)(CFO_comp + (uint32_t)k[i] * SFO_comp)));
-            R[i] = pk_cmul(C[i][0], C[i][1], fac_rotw(i == 0 || rot123 ? d_rotw(T, avg + k[i] * del) : 0u));
+            R[i] = pk_cmul(C[i][0], C[i][1], fac_rotw(i < 6 || pil ? d_rotw(T, avg + k[i] * del) : 0u));
         }
         if (taps.fft_out && act && sym < taps.max_sym) {
             const size_t o = ((size_t)f * taps.max_sym + sym) * 64;
+            const int4 q5 = tab4[5];
+            const cfac eq7 = {q5.y, q5.z, q5.w};
 #pragma unroll
-            for (int i = 0; i < 4; i++) {
-                const int b = front_bin(hl, i);
-                taps.fft_out[o + b] = F[i]; taps.equalized[o + b] = __byte_perm((uint32_t)ex[i], (uint32_t)ey[i], 0x7632); taps.tracked[o + b] = R[i];
+            for (int i = 0; i < 8; i++) {
+                const int b = front_bin(ql, i);
+                const uint32_t Fi = i < 7 ? F[i] : xb[rb[7]];
+                int exi = i < 7 ? ex[i] : 0, eyi = i < 7 ? ey[i] : 0;
+                if (i == 7) pk_cmul_xy((int)(short)Fi, (int)Fi >> 16, eq7, exi, eyi);
+                taps.fft_out[o + b] = Fi; taps.equalized[o + b] = __byte_perm((uint32_t)exi, (uint32_t)eyi, 0x7632); taps.tracked[o + b] = i < 7 ? R[i] : 0u;
             }
         }
         // soft demap (demapper.h:141-151 limit + LUTs) scattered through the inverse de-interleaver map
-        if (hl < 12) {
-            const int4 p0 = tab4[3], p1 = tab4[4], p2 = tab4[5];
-            const uint32_t pos[12] = {(uint32_t)p0.x, (uint32_t)p0.y, (uint32_t)p0.z, (uint32_t)p0.w, (uint32_t)p1.x, (uint32_t)p1.y,
-                                      (uint32_t)p1.z, (uint32_t)p1.w, (uint32_t)p2.x, (uint32_t)p2.y, (uint32_t)p2.z, (uint32_t)p2.w};
+        {
+            const int4 p0 = tab4[8], p1 = tab4[9], p2 = tab4[10], p3 = tab4[11]; const int2 p4 = *(const int2*)(tab + 48);
+            const uint32_t pos[18] = {(uint32_t)p0.x, (uint32_t)p0.y, (uint32_t)p0.z, (uint32_t)p0.w, (uint32_t)p1.x, (uint32_t)p1.y,
+                                      (uint32_t)p1.z, (uint32_t)p1.w, (uint32_t)p2.x, (uint32_t)p2.y, (uint32_t)p2.z, (uint32_t)p2.w,
+                                      (uint32_t)p3.x, (uint32_t)p3.y, (uint32_t)p3.z, (uint32_t)p3.w, (uint32_t)p4.x, (uint32_t)p4.y};
 #pragma unroll
-            for (int p = 0; p < 2; p++) {
+            for (int p = 0; p < 3; p++) {
                 const uint32_t c0 = pk_demap_clamp(R[2 * p]), c1 = pk_demap_clamp(R[2 * p + 1]);
                 const uint32_t wr0 = s_demap[(c0 >> 4) & 0xFF], wi0 = s_demap[(c0 >> 20) & 0xFF], wr1 = s_demap[(c1 >> 4) & 0xFF], wi1 = s_demap[(c1 >> 20) & 0xFF];
                 const uint32_t* ps = pos + 6 * p;
@@ -468,10 +491,13 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
             }
         }
         __syncwarp();
-        if (sym == 0) {                                // PHY_11a.hpp:520-604; both halves' SIGNALs, one after the other on the whole warp
+        if (sym == 0) {                                // PHY_11a.hpp:520-604; the four quarters' SIGNALs, one after the other on the whole warp
             uint32_t sig = 0;
 #pragma unroll 1
-            for (int h = 0; h < 2; h++) { const uint32_t s = warp_viterbi_signal(s_soft[wib][h], s_dec[wib][h], lane); if (h == half) sig = s; }
+            for (int h = 0; h < 4; h++) {
+                const uint32_t s = warp_viterbi_signal(s_soft[wib][h], s_dec[wib], lane); if (h == qt) sig = s;
+                __syncwarp();                          // every lane's traceback has read s_dec before the next SIGNAL's ballots overwrite it
+            }
             sig &= 0xFFFFFFu;
             if (act) {
                 bool ok = !(sig & 0xFC0010u);
@@ -496,9 +522,11 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
                 }
             }
         } else if (act) {                              // N_CBPS = 48 N_BPSC bytes: 3 N_BPSC 16-byte lines (soft_out and soft_stride are 16-byte aligned)
-            uint4* const dst = (uint4*)(sout + soft_bytes); const uint4* const src = (const uint4*)s_soft[wib][half];
-            if (hl < 3 * nbpsc) dst[hl] = src[hl];
-            if (hl + 16 < 3 * nbpsc) dst[hl + 16] = src[hl + 16];
+            uint4* const dst = (uint4*)(sout + soft_bytes); const uint4* const src = (const uint4*)s_soft[wib][qt];
+            const int lines = 3 * nbpsc;
+            if (ql < lines) dst[ql] = src[ql];
+            if (ql + 8 < lines) dst[ql + 8] = src[ql + 8];
+            if (ql + 16 < lines) dst[ql + 16] = src[ql + 16];
             soft_bytes += 48u * nbpsc;
         }
         __syncwarp();
@@ -508,65 +536,67 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
     auto sym_ready = [&](uint32_t sym) { return (sym_first(sym) + 80u) / 4u <= nvec; };         // all 80 samples arrived
     // ---- staging (see STAGE above) ----
     const uint32_t nsamp20 = nvec * 4u;                                   // 20 Msps samples of the slot that may be read
-    uint32_t raw[4] = {0, 0, 0, 0}; uint32_t raw_first = 0xFFFFFFFFu;     // STAGE 1: samples first + hl + 16 j of the prefetched symbol
+    uint32_t raw[8] = {0, 0, 0, 0, 0, 0, 0, 0}; uint32_t raw_first = 0xFFFFFFFFu;   // STAGE 1: samples first + ql + 8 j of the prefetched symbol
     auto prefetch_regs = [&](uint32_t first) {                            // whole symbol inside the slot, else nothing
         raw_first = 0xFFFFFFFFu;
         if (act && first + 72u <= nsamp20) {
 #pragma unroll
-            for (int j = 0; j < 4; j++) raw[j] = __ldg(x + ((first + hl + 16u * j) << sh));
+            for (int j = 0; j < 8; j++) raw[j] = __ldg(x + ((first + ql + 8u * j) << sh));
             raw_first = first;
         }
     };
     // STAGE 2: parity / first 20 Msps sample / samples per buffer, and which buffers have a copy in flight (bit b)
     uint32_t st_par[2] = {0, 0}, st_base[2] = {0, 0}, st_cnt[2] = {0, 0}, st_busy = 0;
+    uint32_t* const st_buf = s_stage + (4 * wib + qt) * 2 * SB_FRONT_STAGE_WORDS;   // this quarter's two buffers
     auto stage_issue = [&](int b, uint32_t first20, uint32_t n20) {       // samples [first20, first20 + n20) of the slot -> buffer b (word index << sh)
         st_base[b] = first20; st_cnt[b] = 0;
         if (!act || first20 >= nsamp20) return;
         if (first20 + n20 > nsamp20) n20 = nsamp20 - first20;
         st_cnt[b] = n20; st_busy |= 1u << b;
-        if (hl == 0) {
+        if (ql == 0) {
             const uint32_t* src = x + (first20 << sh);
             const uintptr_t a0 = (uintptr_t)src & ~(uintptr_t)15, a1 = ((uintptr_t)(src + (n20 << sh)) + 15) & ~(uintptr_t)15;
             const uint32_t bytes = (uint32_t)(a1 - a0);
-            const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][half][b]), dst = (uint32_t)__cvta_generic_to_shared(&s_stage[wib][half][b][0]);
+            const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][qt][b]), dst = (uint32_t)__cvta_generic_to_shared(st_buf + b * SB_FRONT_STAGE_WORDS);
             asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes) : "memory");
             asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" :: "r"(dst), "l"(a0), "r"(bytes), "r"(mb) : "memory");
         }
     };
     auto stage_wait = [&](int b) {
         if (!((st_busy >> b) & 1u)) return;
-        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][half][b]); uint32_t ok = 0;
+        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][qt][b]); uint32_t ok = 0;
         while (!ok) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }" : "=r"(ok) : "r"(mb), "r"(st_par[b]) : "memory");
         st_par[b] ^= 1u; st_busy &= ~(1u << b);
     };
-    auto stage_load4 = [&](int b, uint32_t first, uint32_t (&v)[4]) {    // (x >> 1) * FreqCoeffs from buffer b; the buffer starts at the 16-byte line of its first sample
+    auto stage_load8 = [&](int b, uint32_t first, uint32_t (&v)[8]) {    // (x >> 1) * FreqCoeffs from buffer b; the buffer starts at the 16-byte line of its first sample
         const uint32_t skew = (uint32_t)(((uintptr_t)(x + (st_base[b] << sh)) & 15u) >> 2);
+        const uint32_t* const buf = st_buf + b * SB_FRONT_STAGE_WORDS;
 #pragma unroll
-        for (int j = 0; j < 4; j++) v[j] = fcomp(s_stage[wib][half][b][skew + ((first - st_base[b] + hl + 16u * j) << sh)], j);
+        for (int j = 0; j < 8; j++) v[j] = fcomp(buf[skew + ((first - st_base[b] + ql + 8u * j) << sh)], j);
     };
     if (STAGE == 2) stage_issue(0, sym_first(0), 80u);
     if (STAGE == 1) prefetch_regs(sym_first(0) + 8u);
-    // SIGNAL, then the data symbols, one per iteration in each half
+    // SIGNAL, then the data symbols, one per iteration in each quarter
     for (uint32_t sym = 0; ; sym++) {
         if (act && !sym_ready(sym)) { status = E_NO_FRAME; act = false; }
         if (!__any_sync(FULL, act)) break;
-        {   uint32_t v[4];
+        {   uint32_t v[8];
             const uint32_t first = sym_first(sym) + 8u;
             if (STAGE == 2) {
                 const int b = (int)(sym & 1u);
                 const bool staged = st_base[b] == sym_first(sym) && st_cnt[b] >= 80u;
                 stage_wait(b);
-                if (act && staged) stage_load4(b, first, v); else load4(first, v);
+                if (act && staged) stage_load8(b, first, v); else load8(first, v);
                 __syncwarp();                                               // every lane has its samples: the other buffer's previous contents are no longer needed either
                 stage_issue(b ^ 1, sym_first(sym + 1u), 80u);
             } else if (STAGE == 1) {
                 if (raw_first == first) {
 #pragma unroll
-                    for (int j = 0; j < 4; j++) v[j] = fcomp(raw[j], j);
-                } else load4(first, v);
+                    for (int j = 0; j < 8; j++) v[j] = fcomp(raw[j], j);
+                } else load8(first, v);
                 prefetch_regs(first + 80u);
-            } else load4(first, v);
-            fft_from_regs(v[0], v[1], v[2], v[3]); }
+            } else load8(first, v);
+            fft_from_regs(v); }
         post_fft(sym);
         if (sym == 0 && taps.hdr_only && act) {                           // continuous-capture scout pass: where the frame ends is all the caller wants
             if (!sym_ready(fi.nsym_total - 1u)) status = E_NO_FRAME;
@@ -574,7 +604,7 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
         }
     }
     if (STAGE == 2) { stage_wait(0); stage_wait(1); __syncwarp(); }       // no copy may be in flight when the CTA's shared memory is released
-    if (own && hl == 0) { fi.status = status; fi.soft_bytes = soft_bytes; info[f] = fi; }
+    if (own && ql == 0) { fi.status = status; fi.soft_bytes = soft_bytes; info[f] = fi; }
 }
 
 // ------------------------------------------------------------------------------------------------

@@ -244,7 +244,8 @@ struct sb200_handle {
     DevTables11n N{}; DevBuf tab11n, iq1;              // 802.11n tables (uploaded on first use) and the second antenna's samples
     std::vector<uint64_t> offh; std::vector<uint32_t> lenh;   // host copy of the slot table (cached for device-resident tables)
     const uint64_t* tab_off = nullptr; const uint32_t* tab_len = nullptr; uint32_t tab_n = 0, tab_max_len = 0; uint64_t tab_total = 0; bool tab_host = false;
-    uint32_t front_stage = 0;                          // option: sample staging of k_front11a (0 direct loads, 1 register double buffer, 2 bulk async copy to shared memory)
+    uint32_t front_stage = 1;                          // option: sample staging of k_front11a (0 direct loads, 1 register double buffer, 2 bulk async copy to shared memory)
+    bool front_smem_set = false;                       // k_front11a<2> may use SB_FRONT_STAGE_SMEM bytes of dynamic shared memory on this device
     uint32_t host_decimate = 0;                        // option: host threads gathering the even samples of host-resident 40 Msps captures (0 = off)
     DecimPool* pool = nullptr; void* hstage[4] = {nullptr, nullptr, nullptr, nullptr}; size_t hstage_cap = 0; cudaEvent_t ev_hfree[4] = {nullptr, nullptr, nullptr, nullptr};
     // host_decimate_mix (default 1 = adaptive): per chunk, the decimating path either gathers on the host threads (half the bytes cross) or,
@@ -571,7 +572,11 @@ static int launch_chunk(sb200_handle* h, const uint32_t* iq_base, const uint64_t
     k_sync11a<<<(n + 127) / 128, 128, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->cca_thr, h->T, d_info, dc_init ? dc_init + f0 : nullptr, sh, lsh);
     if (timed) CK(cudaEventRecord(h->evk[1], sf));
     {   const dim3 g((n + SB_FRONT_SLOTS - 1) / SB_FRONT_SLOTS), b(32 * SB_FRONT_WARPS);
-        if (h->front_stage == 2) k_front11a<2><<<g, b, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh);
+        if (h->front_stage == 2 && !h->front_smem_set) {
+            CK(cudaFuncSetAttribute(k_front11a<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_FRONT_STAGE_SMEM));
+            h->front_smem_set = true;
+        }
+        if (h->front_stage == 2) k_front11a<2><<<g, b, SB_FRONT_STAGE_SMEM, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh);
         else if (h->front_stage == 1) k_front11a<1><<<g, b, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh);
         else k_front11a<0><<<g, b, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh); }
     if (timed) CK(cudaEventRecord(h->evk[2], sf));
