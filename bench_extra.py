@@ -11,6 +11,7 @@
   --config tx11b_legacy  the legacy 802.11b transmitter (BB11BPMDPacketGenSignal: encoder + SSE filter, fused) on the device, 11 Mbps / 1500 B
   --config tx11a_legacy  the legacy 802.11a transmitter (BB11ATxFrameMod) on the device, 54 Mbps / 1500 B, at 40 and at 44 Msps
   --config channelize  the wideband channelizer: four 802.11a channels of a 160 Msps capture, 127 taps, D = 4, device-resident
+  --config channelize_rational  the rational-rate channelizer: three 802.11b channels of a 160 Msps capture to 44 Msps, 1287 taps, U / D = 11 / 40
   --config combine   the wideband combiner: four 802.11a channel rows at 40 Msps into one 160 Msps capture, 127 taps, U = 4, device-resident
   --config sim       the radio channel simulator: --frames links of config #2's 9 824-sample slots (T = R = 1, L = 16, +20 ppm, a carrier
                      offset, noise on), and a 2x2 case (T = R = 2, L = 16), device-resident
@@ -463,6 +464,38 @@ def bench_channelize(args):
             "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs of every channel" % m})
     c.close()
 
+def bench_channelize_rational(args):
+    """The rational-rate channelizer on a device-resident 160 Msps capture the size of --config channelize's: three 802.11b channels at
+    -25 / 0 / +25 MHz brought to 44 Msps (U = 11, D = 40) through 1287 taps (117 per branch).  Work per input sample: K (4 + 2 ntaps / D)
+    integer multiply-adds (each output meets one branch of ntaps / U taps, and there are U / D outputs per input); HBM traffic 4 B read +
+    4 K U / D B written."""
+    import wideband_inputs as W, rational_model as R
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    n = args.frames * 9824 * 4; K, U, D = 3, 11, 40
+    taps = W.lowpass(1287, 12e6 / 1.76e9, gain=11); ch = [(W.phase_inc(f, 160e6), 0) for f in (-25e6, 0.0, 25e6)]
+    n_out = -(-U * n // D); stride = (n_out + 3) // 4 * 4
+    x = torch.randint(-20000, 20000, (n, 2), dtype=torch.int16, device=dev); y = torch.empty((K, stride, 2), dtype=torch.int16, device=dev)
+    def step(): eng.channelize_raw(x.data_ptr(), n, ch, D, taps, y.data_ptr(), stride, st.cuda_stream, interp=U)
+    step(); torch.cuda.synchronize()
+    P = 20000; m = (U * P - len(taps)) // D                              # outputs that a prefix of P samples determines
+    assert (R.channelize_rational(x[:P].cpu().numpy(), ch, U, D, taps)[:, :m] == y[:, :m].cpu().numpy()).all(), "channelizer output differs from the stated arithmetic"
+    ms = c.timed(step, args.steps)
+    sec = ms * 1e-3
+    hbm = n * (4.0 + 4.0 * K * U / D); macs = n * K * (4.0 + 2.0 * len(taps) / D)
+    name, plim, clk = _card(); sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    imad_peak = sms * 64 * clk * 1e6 if clk else None                    # int32 IMAD: 64 per SM per clock on sm_90
+    f_hbm = hbm / sec / 1e9 / peaks(); f_int = (macs / sec / imad_peak) if imad_peak else None
+    c.emit({"metric": "rational channelizer input Msamples/s (COMPLEX16 in, 3 channels, U / D = 11 / 40)", "value": c.world * n / sec / 1e6, "unit": "Msamples/s", "ms_per_step": ms,
+            "n_gpus": c.world,
+            "config": {"workload": "160 Msps capture, 3 x 802.11b channels at -25/0/+25 MHz to 44 Msps, 1287 taps, U = 11, D = 40, device-resident", "samples_per_step_per_gpu": n},
+            "hbm": {"achieved": hbm / sec / 1e9, "peak": peaks(), "unit": "GB/s", "frac": f_hbm, "note": "4 B read + 4 K U / D B written per input sample"},
+            "int_mad": {"achieved": macs / sec / 1e9, "peak": imad_peak / 1e9 if imad_peak else None, "unit": "G multiply-adds/s", "frac": f_int,
+                        "note": "K (4 + 2 ntaps / D) per input sample; peak = SMs x 64 x max SM clock"},
+            "bound": None if f_int is None else ("integer" if f_int > f_hbm else "hbm"),
+            "card": name, "power_limit_w": plim, "sm_clock_max_mhz": clk,
+            "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs of every channel" % m})
+    c.close()
+
 def bench_combine(args):
     """The wideband combiner into a device-resident 160 Msps capture: four 802.11a channel rows at 40 Msps moved to -60 / -20 / +20 / +60 MHz,
     127 taps, U = 4; as many output samples as --config channelize reads.  Work per output sample: K (2 ceil(ntaps / U) + 4 + 2) integer
@@ -531,10 +564,10 @@ def bench_sim(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "combine", "sim"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_rational", "combine", "sim"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "combine": bench_combine, "sim": bench_sim}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_rational": bench_channelize_rational, "combine": bench_combine, "sim": bench_sim}[a.config](a)

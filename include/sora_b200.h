@@ -167,6 +167,24 @@ typedef struct sb200_ddc_channel { uint32_t phase_inc; uint32_t phase0; } sb200_
 int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_in_samples, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t decim,
                      const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride_samples, void* cuda_stream);
 
+/* Rational-rate channelizer: sb200_channelize with the rate changed by U / D (U = interp, D = decim) instead of 1 / D, so that one capture
+ * feeds receivers of rates that no whole-number D reaches from it (802.11b at 44 Msps and OFDM at 40 Msps out of 160 or 176 Msps);
+ * an extension without a reference counterpart.  For channel (phase_inc, phase0), c = (ntaps - 1) / 2 and every output
+ * m in 0 .. n_out = ceil(U n_in / D):
+ *     v(n)  = the Q14 NCO rotation of x(n) by sb200_channelize, with the phase of the absolute INPUT index n
+ *     z(i)  = v(i / U) if i mod U == 0 and 0 <= i / U < n_in, else 0          zero-stuffing
+ *     y[m]  = sat16((sum_k taps[k] * z(D m + k - c) + 2^14) >> 15)             int32 accumulator, re and im independently
+ * Output m stands at input time D m / U: output 0 lines up with input 0.  Only the taps k = c - D m (mod U) meet a non-zero z, so an
+ * interpolation filter has a DC gain of U (each branch near unity) and the accumulator limit is per branch, as in sb200_combine.  With
+ * interp = 1 this is sb200_channelize, bit for bit, with decim up to 64.  Rows, residency, alignment and staging as in sb200_channelize;
+ * the rows go to sb200_rx11a_streams / sb200_rx11b_streams / sb200_rx11n_streams as they are.  Limits (SB200_E_INVALID, nothing launched):
+ * 1 <= interp <= 16, interp <= decim <= 64, gcd(interp, decim) = 1 (rate reduction only), ntaps odd with ceil(ntaps / interp) <= 255, for
+ * every residue r mod interp the sum of |taps[k]| over k = r (mod interp) <= 65535, 1 <= nchannels <= 16, out_stride >= n_out, a multiple
+ * of 4 and <= 2^40, n_in <= 2^40.  One kernel launch; sb200_last_kernel_ms times it. */
+int sb200_channelize_rational(sb200_handle* h, const int16_t* iq, uint64_t n_in_samples, const sb200_ddc_channel* channels, uint32_t nchannels,
+                              uint32_t interp, uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride_samples,
+                              void* cuda_stream);
+
 /* Wideband combiner, the transmit counterpart of sb200_channelize: K = nchannels rows x_k[0 .. n_in) of COMPLEX16 at the channel rate
  * (row k at rows + k * row_stride samples) interpolated by U = interp, each moved to its centre frequency, scaled and summed into one
  * capture y[0 .. U n_in) at the wideband rate; an extension without a reference counterpart.  For channel k = {phase_inc, phase0, gain}

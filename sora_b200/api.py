@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_combine", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_combine", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -276,20 +276,27 @@ class Engine:
         self.fir_decimate2_raw(_ptr(iq), len(iq), _ptr(t) if t is not None else 0, 0 if t is None else len(t), _ptr(out))
         return out
 
-    def channelize_raw(self, in_ptr, n_in, channels, decim, taps, out_ptr, out_stride, stream=0):
-        """Pointer-level sb200_channelize: in_ptr / out_ptr host or device addresses; channels a list of (phase_inc, phase0); taps int16 Q15."""
+    def channelize_raw(self, in_ptr, n_in, channels, decim, taps, out_ptr, out_stride, stream=0, interp=1):
+        """Pointer-level sb200_channelize (interp = 1) or sb200_channelize_rational: in_ptr / out_ptr host or device addresses; channels a
+        list of (phase_inc, phase0); taps int16 Q15."""
         ch = (DdcChannel * max(len(channels), 1))(*[DdcChannel(int(a) % 2 ** 32, int(b) % 2 ** 32) for a, b in channels])
         t = np.ascontiguousarray(taps, dtype=np.int16)
-        self._check(self._lib.sb200_channelize(self._h, C.c_void_p(in_ptr), C.c_uint64(n_in), C.cast(ch, C.c_void_p), C.c_uint32(len(channels)), C.c_uint32(decim),
-                                               C.c_void_p(_ptr(t)), C.c_uint32(len(t)), C.c_void_p(out_ptr), C.c_uint64(out_stride), C.c_void_p(stream)), "sb200_channelize")
+        if interp == 1:
+            self._check(self._lib.sb200_channelize(self._h, C.c_void_p(in_ptr), C.c_uint64(n_in), C.cast(ch, C.c_void_p), C.c_uint32(len(channels)), C.c_uint32(decim),
+                                                   C.c_void_p(_ptr(t)), C.c_uint32(len(t)), C.c_void_p(out_ptr), C.c_uint64(out_stride), C.c_void_p(stream)), "sb200_channelize")
+        else:
+            self._check(self._lib.sb200_channelize_rational(self._h, C.c_void_p(in_ptr), C.c_uint64(n_in), C.cast(ch, C.c_void_p), C.c_uint32(len(channels)),
+                                                            C.c_uint32(interp), C.c_uint32(decim), C.c_void_p(_ptr(t)), C.c_uint32(len(t)), C.c_void_p(out_ptr),
+                                                            C.c_uint64(out_stride), C.c_void_p(stream)), "sb200_channelize_rational")
 
-    def channelize(self, iq, channels, decim, taps):
-        """Wideband channelizer: int16 [n,2] and K channels (phase_inc, phase0) -> int16 [K, ceil(n / decim), 2], channel k shifted to 0 Hz,
-        filtered by taps (int16 Q15, odd count <= 255, sum |t| <= 65535) and decimated."""
+    def channelize(self, iq, channels, decim, taps, interp=1):
+        """Wideband channelizer: int16 [n,2] and K channels (phase_inc, phase0) -> int16 [K, ceil(interp n / decim), 2], channel k shifted
+        to 0 Hz, filtered by taps (int16 Q15, odd count; interp = 1: <= 255 taps, sum |t| <= 65535; else ceil(ntaps / interp) <= 255 and
+        the same limit per branch) and resampled by interp / decim."""
         iq = np.ascontiguousarray(iq, dtype=np.int16).reshape(-1, 2)
-        n_out = -(-len(iq) // decim); stride = (n_out + 3) // 4 * 4
+        n_out = -(-interp * len(iq) // decim); stride = (n_out + 3) // 4 * 4
         out = np.zeros((len(channels), stride, 2), np.int16)
-        self.channelize_raw(_ptr(iq), len(iq), channels, decim, taps, _ptr(out), stride)
+        self.channelize_raw(_ptr(iq), len(iq), channels, decim, taps, _ptr(out), stride, interp=interp)
         return out[:, :n_out]
 
     def combine_raw(self, rows_ptr, row_stride, n_in, channels, interp, taps, out_ptr, stream=0):

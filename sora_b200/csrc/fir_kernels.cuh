@@ -19,7 +19,16 @@
 // outputs of the tile (tid + 256 j), one tap at a time (the tap is a uniform constant; zero taps of a half-band filter are skipped).
 // Work per input sample and channel: 4 multiply-adds of the rotation and 2 ntaps / D of the filter; integer issue bounds it, not HBM
 // (4 B read + 4 K / D B written per input sample).
+//
+// sb200_channelize_rational runs the same kernel at a rational rate U / D: the rotated input is zero-stuffed by U before the filter,
+//     y[m]   = sat16((sum_k taps[k] * z(D m + k - c) + 2^14) >> 15),   z(i) = v(i / U) if U divides i, else 0.
+// Output m = U q + s (phase s) meets only the branch of taps k = r_s + U l, r_s = (c - D s) mod U, on the inputs n = D q + e_s + l,
+// e_s = (D s + r_s - c) / U exactly.  Within one phase consecutive q step the input by D, as at U = 1, so the same polyphase buffer serves
+// every phase without bank conflicts and the tap stays uniform across the warp; the tile's phases run one after another (or side by side
+// on groups of warps when one phase needs fewer warps than the CTA has).  The sb200_channelize case, U = 1, is a compile-time
+// specialisation of the same source (RAT = false): one phase, the taps in ChTaps, and the rotation pass by polyphase column.
 #pragma once
+#include <type_traits>
 #include "fixed.cuh"
 
 namespace sb {
@@ -30,16 +39,21 @@ namespace sb {
 #define SB_CH_MAXTAPS 255                  // sb200_channelize's limit
 #define SB_CH_MAXHALO 128                  // (SB_CH_MAXTAPS - 1) / 2 rounded up to a 16-byte multiple of samples
 #define SB_CH_MAXCH 16
-#define SB_CH_MAXDECIM 16
+#define SB_CH_MAXDECIM 16                  // sb200_channelize's and sb200_combine's limit
+#define SB_CH_MAXINTERP 16                 // sb200_channelize_rational's limits: U <= 16, D <= 64
+#define SB_CH_MAXRDECIM 64
 // Words of one window buffer.  The staged window has win = SB_FIR_TILE + 2 halo words; its polyphase copy spans D phases of
-// P = ceil(win / D) words, D P <= win + D - 1, so a buffer holds the largest window plus SB_CH_MAXDECIM words.
-#define SB_CH_WIN (SB_FIR_TILE + 2 * SB_CH_MAXHALO + SB_CH_MAXDECIM)
+// P = ceil(win / D) words, D P <= win + D - 1, so a buffer holds the largest window plus SB_CH_MAXRDECIM words.
+#define SB_CH_WIN (SB_FIR_TILE + 2 * SB_CH_MAXHALO + SB_CH_MAXRDECIM)
 #define SB_CH_NCO 4096                     // NCO table entries (phi >> 20)
 #define SB_CH_SMEM ((2 * SB_CH_WIN + SB_CH_NCO) * 4 + 16)                  // dynamic shared memory of k_channelize: window, rotated window, table, mbarrier
 static_assert(SB_CH_WIN % 4 == 0, "the NCO table behind the two window buffers must stay 16-byte aligned for the bulk copy");
-static_assert(SB_CH_WIN >= SB_FIR_TILE + 2 * SB_CH_MAXHALO + SB_CH_MAXDECIM - 1, "the polyphase buffer must hold D * ceil(win / D) words");
+static_assert(SB_CH_WIN >= SB_FIR_TILE + 2 * SB_CH_MAXHALO + SB_CH_MAXRDECIM - 1, "the polyphase buffer must hold D * ceil(win / D) words");
 
 struct ChTaps { int16_t t[SB_CH_MAXTAPS + 1]; uint32_t n; };
+// The taps of sb200_channelize_rational by branch: taps[r + U l] at t[r][l].  8 KB of kernel parameters (allowed up to 32 KB since CUDA
+// 12.1 on sm_70 and later), read like ChTaps: one uniform constant-bank load per tap.
+struct RtTaps { int16_t t[SB_CH_MAXINTERP][SB_CH_MAXTAPS + 1]; uint32_t n, u; };
 struct ChChannels { uint32_t inc[SB_CH_MAXCH], phase0[SB_CH_MAXCH]; uint32_t n; };
 
 // Staging of k_channelize and k_channel_sim (sim_kernels.cuh).  k_fir_decimate2 below keeps a copy of these steps inline with its sizes as
@@ -151,62 +165,92 @@ __device__ __forceinline__ uint32_t nco_rotate(uint32_t w, uint32_t cs) {
     return pack(mk(sat16(re >> 14), sat16(im >> 14)));
 }
 
-// grid (tiles, channel groups), SB_FIR_THREADS threads, SB_CH_SMEM bytes of dynamic shared memory.  J = outputs per thread per tile and
-// channel, at least ceil(ceil(SB_FIR_TILE / D) / SB_FIR_THREADS).  Channel c's row starts at y + c * stride.
-template <int J>
+// Halo (samples each side) of a tile for ntaps taps at interpolation U: ceil(c / U) rounded up to a 16-byte multiple of samples, at most
+// SB_CH_MAXHALO while ceil(ntaps / U) <= 255.  k_channelize's tile reads input D m / U - c / U .. D m / U + c / U for its outputs; k_combine
+// (below) reads input i + e_r .. for output U i + r.
+__host__ __device__ constexpr uint32_t combine_halo(uint32_t ntaps, uint32_t U) { return ((ntaps / 2 + U - 1) / U + 3u) & ~3u; }
+
+// grid (tiles, channel groups), SB_FIR_THREADS threads, SB_CH_SMEM bytes of dynamic shared memory.  J = outputs per thread per tile,
+// channel and phase, at least ceil(ceil(SB_FIR_TILE / D) / SB_FIR_THREADS).  Channel c's row starts at y + c * stride.  RAT = false:
+// U = 1 with ChTaps (sb200_channelize); RAT = true: U = taps.u with the branches of RtTaps.
+template <int J, bool RAT>
 __global__ void __launch_bounds__(SB_FIR_THREADS) k_channelize(const uint32_t* __restrict__ x, uint64_t n_in, const uint32_t* __restrict__ nco, ChChannels ch,
-                                                              uint32_t chan_per_group, uint32_t D, ChTaps taps, uint32_t* __restrict__ y, uint64_t stride, uint64_t n_out) {
+                                                              uint32_t chan_per_group, uint32_t D, typename std::conditional<RAT, RtTaps, ChTaps>::type taps,
+                                                              uint32_t* __restrict__ y, uint64_t stride, uint64_t n_out) {
     extern __shared__ __align__(16) uint32_t smem[];
     uint32_t* s_x = smem; uint32_t* s_v = smem + SB_CH_WIN; uint32_t* s_nco = smem + 2 * SB_CH_WIN;
     unsigned long long* s_bar = (unsigned long long*)(smem + 2 * SB_CH_WIN + SB_CH_NCO);
     const uint32_t tid = threadIdx.x;
+    uint32_t U = 1u;
+    if constexpr (RAT) U = taps.u;
     const uint64_t t0 = (uint64_t)blockIdx.x * SB_FIR_TILE;             // first input sample of this tile
-    const uint32_t c = taps.n >> 1, halo = (c + 3u) & ~3u, win = SB_FIR_TILE + 2 * halo;
+    const uint32_t c = taps.n >> 1, halo = combine_halo(taps.n, U), win = SB_FIR_TILE + 2 * halo;
     const uint32_t ch0 = blockIdx.y * chan_per_group, ch1 = min(ch0 + chan_per_group, ch.n);
     bool rotate = false;                                                // the table is only brought in when a channel of the group needs it
     for (uint32_t k = ch0; k < ch1; k++) rotate |= ch.inc[k] != 0u || (ch.phase0[k] >> 20) != 0u;
     stage_window(x, 0, 1, n_in, (int64_t)t0 - (int64_t)halo, win, s_x, 0, rotate ? nco : nullptr, SB_CH_NCO, s_nco, s_bar);
-    // outputs m0 .. m1 of the tile: D m in [t0, t0 + tile); output m reads window words D m - (t0 - halo) - c + k, k = 0 .. ntaps-1
-    const uint64_t m0 = (t0 + D - 1) / D, m1e = (t0 + SB_FIR_TILE + D - 1) / D, m1 = m1e < n_out ? m1e : n_out;
-    const uint32_t nm = m1 > m0 ? (uint32_t)(m1 - m0) : 0u;
-    const uint32_t i0 = (uint32_t)(D * m0 - t0) + halo - c;             // window word of output m0, tap 0
+    // outputs m0 .. m1 of the tile: D m in [U t0, U (t0 + tile)); output m = U q + s reads window words D q + e_s + l - (t0 - halo)
+    const uint64_t m0 = (U * t0 + D - 1) / D, m1e = (U * (t0 + SB_FIR_TILE) + D - 1) / D, m1 = m1e < n_out ? m1e : n_out;
     const uint32_t P = (win + D - 1) / D;                               // words per phase of the polyphase buffer
-    uint32_t off[J];                                                    // word of output j within its phase (0 for outputs past the tile: read, never stored)
-#pragma unroll
-    for (int j = 0; j < J; j++) { const uint32_t q = tid + SB_FIR_THREADS * j; off[j] = q < nm ? q : 0u; }
+    // Phases side by side: at J = 1 one phase's outputs (at most ceil(tile / D)) need W warps, and G = 8 / W groups of W warps take the
+    // phases g, g + G, ...; warps past the last group idle in the filter.  At U = 1 (and J > 1) one group of all warps.
+    const uint32_t W = (RAT && J == 1) ? (((SB_FIR_TILE + D - 1) / D + 31u) >> 5) : SB_FIR_THREADS / 32u;
+    const uint32_t G = (SB_FIR_THREADS / 32u) / W, grp = (tid >> 5) / W, lt = tid - grp * W * 32u;
     for (uint32_t k = ch0; k < ch1; k++) {
         const uint32_t inc = ch.inc[k];
         // window word i = D p + r -> s_v[r P + p]; sample index t0 - halo + i
         uint32_t ph = ch.phase0[k] + (uint32_t)(t0 - halo) * inc;
         const bool ident = inc == 0u && (ch.phase0[k] >> 20) == 0u;     // NCO[0] = (2^14, 0): the rotation is the identity
-        for (uint32_t p = tid; p < P; p += SB_FIR_THREADS) {
-            uint32_t phi = ph + (uint32_t)(D * p) * inc;
-            for (uint32_t r = 0, i = D * p; r < D && i < win; r++, i++, phi += inc) {
+        if constexpr (RAT) {                                            // by window word: P < 256 threads for D > 17
+            const uint32_t sa = SB_FIR_THREADS / D, sb = SB_FIR_THREADS % D;
+            uint32_t p = tid / D, r = tid % D, phi = ph + tid * inc;
+            for (uint32_t i = tid; i < win; i += SB_FIR_THREADS) {
                 const uint32_t w = s_x[i];
                 s_v[r * P + p] = ident ? w : nco_rotate(w, s_nco[phi >> 20]);
+                phi += SB_FIR_THREADS * inc; p += sa; r += sb; if (r >= D) { r -= D; p++; }
+            }
+        } else {
+            for (uint32_t p = tid; p < P; p += SB_FIR_THREADS) {
+                uint32_t phi = ph + (uint32_t)(D * p) * inc;
+                for (uint32_t r = 0, i = D * p; r < D && i < win; r++, i++, phi += inc) {
+                    const uint32_t w = s_x[i];
+                    s_v[r * P + p] = ident ? w : nco_rotate(w, s_nco[phi >> 20]);
+                }
             }
         }
         __syncthreads();
-        uint32_t accr[J], acci[J];
-#pragma unroll
-        for (int j = 0; j < J; j++) accr[j] = acci[j] = 1u << 14;
-        uint32_t r = i0 % D, base = r * P + i0 / D;                     // phase and word of tap 0 for output m0
-        for (uint32_t kk = 0; kk < taps.n; kk++) {                      // one tap at a time over the J outputs: the tap is a uniform constant
-            const int t = taps.t[kk];
-            if (t != 0) {                                               // half-band filters: every other tap
-#pragma unroll
-                for (int j = 0; j < J; j++) {
-                    const cs16 v = unpack(s_v[base + off[j]]);
-                    accr[j] += (uint32_t)(t * v.re); acci[j] += (uint32_t)(t * v.im);   // int32 accumulator, two's-complement wrap
-                }
-            }
-            if (++r == D) { r = 0; base += 1u - (D - 1u) * P; } else base += P;
-        }
         uint32_t* yr = y + (uint64_t)k * stride;
+        for (uint32_t s = grp; s < U; s += G) {
+            // phase s: outputs m = U q + s, q = qa .. qb; branch r_s of the taps (length L), first input e_s past D q
+            const uint64_t qa = (m0 + U - 1 - s) / U, qb = (m1 + U - 1 - s) / U;
+            const uint32_t nq = qb > qa ? (uint32_t)(qb - qa) : 0u;
+            const uint32_t rs = (c % U + U - (D * s) % U) % U, L = rs < taps.n ? (taps.n - 1 - rs) / U + 1 : 0u;
+            const int es = ((int)(D * s + rs) - (int)c) / (int)U;      // exact: D s + r_s - c is a multiple of U
+            const uint32_t i0 = (uint32_t)((int64_t)(D * qa) - (int64_t)t0 + (int64_t)halo + es);   // window word of output qa, tap 0
+            uint32_t off[J];                                            // word of output j within its phase (0 for outputs past the tile: read, never stored)
 #pragma unroll
-        for (int j = 0; j < J; j++) {
-            const uint32_t q = tid + SB_FIR_THREADS * j;
-            if (q < nm) yr[m0 + q] = pack(mk(sat16((int)accr[j] >> 15), sat16((int)acci[j] >> 15)));
+            for (int j = 0; j < J; j++) { const uint32_t q = lt + SB_FIR_THREADS * j; off[j] = q < nq ? q : 0u; }
+            uint32_t accr[J], acci[J];
+#pragma unroll
+            for (int j = 0; j < J; j++) accr[j] = acci[j] = 1u << 14;
+            uint32_t r = i0 % D, base = r * P + i0 / D;                 // phase and word of tap 0 for output qa
+            for (uint32_t l = 0; l < L; l++) {                          // one tap at a time over the J outputs: the tap is a uniform constant
+                int t;
+                if constexpr (RAT) t = taps.t[rs][l]; else t = taps.t[l];
+                if (t != 0) {                                           // half-band filters: every other tap
+#pragma unroll
+                    for (int j = 0; j < J; j++) {
+                        const cs16 v = unpack(s_v[base + off[j]]);
+                        accr[j] += (uint32_t)(t * v.re); acci[j] += (uint32_t)(t * v.im);   // int32 accumulator, two's-complement wrap
+                    }
+                }
+                if (++r == D) { r = 0; base += 1u - (D - 1u) * P; } else base += P;
+            }
+#pragma unroll
+            for (int j = 0; j < J; j++) {
+                const uint32_t q = lt + SB_FIR_THREADS * j;
+                if (q < nq) yr[U * (qa + q) + s] = pack(mk(sat16((int)accr[j] >> 15), sat16((int)acci[j] >> 15)));
+            }
         }
         __syncthreads();                                                // s_v is rewritten by the next channel
     }
@@ -227,9 +271,8 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_channelize(const uint32_t* _
 
 struct CbChannels { uint32_t inc[SB_CH_MAXCH], phase0[SB_CH_MAXCH], gain[SB_CH_MAXCH]; uint32_t n; };
 
-// Halo (samples each side) and dynamic shared memory of k_combine for a tile of ti input samples: K windows, the U ti output tile, the
-// NCO table and the mbarrier.
-__host__ __device__ constexpr uint32_t combine_halo(uint32_t ntaps, uint32_t U) { return ((ntaps / 2 + U - 1) / U + 3u) & ~3u; }
+// Dynamic shared memory of k_combine for a tile of ti input samples: K windows (halo combine_halo above), the U ti output tile, the NCO
+// table and the mbarrier.
 __host__ __device__ constexpr uint32_t combine_smem(uint32_t K, uint32_t U, uint32_t ntaps, uint32_t ti) {
     return (K * (ti + 2 * combine_halo(ntaps, U)) + U * ti + SB_CH_NCO) * 4u + 16u;
 }

@@ -272,7 +272,7 @@ struct sb200_handle {
     uint32_t lane_min = SB200_LANE_MIN_DEFAULT, lane_max = SB200_LANE_MAX_DEFAULT;
     const char* last_vit = "";                         // name of the Viterbi kernel the last launch used (sb200_last_viterbi_kernel)
     DevBuf nco;                                        // NCO table of the channelizer and the combiner (fir_kernels.cuh), built on first use
-    uint32_t ch_smem_set = 0;                          // bit J: k_channelize<J> may use SB_CH_SMEM bytes of dynamic shared memory on this device
+    uint64_t ch_smem_set = 0;                          // bit J (+ 32 for RAT): k_channelize<J, RAT> may use SB_CH_SMEM bytes of dynamic shared memory on this device
     int sms = 0;                                       // multiprocessors of the device (channel groups of k_channelize)
     uint32_t cb_smem_set = 0;                          // bit J: k_combine<J> may use SB_CB_SMEM bytes of dynamic shared memory on this device
     DevBuf simtab, simlink, simtap;                    // channel simulator: its table (sim_kernels.cuh, built on first use), staged links and taps
@@ -901,19 +901,23 @@ extern "C" int sb200_rx11a_stream(sb200_handle* h, const int16_t* iq, uint64_t n
 }
 
 // One launch of k_channelize (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.  Outputs per thread from D;
-// channels split into groups (the input then read once per group) only as far as needed for four CTAs per multiprocessor.
-template <int J>
+// channels split into groups (the input then read once per group) only as far as needed for four CTAs per multiprocessor.  ChTaps
+// launches the U = 1 specialisation, RtTaps the rational one.
+template <int J, class Taps>
 static int channelize_launch_j(sb200_handle* h, cudaStream_t st, dim3 grid, const uint32_t* d_in, uint64_t n_in, const ChChannels& ch, uint32_t cpg,
-                               uint32_t D, const ChTaps& T, uint32_t* d_out, uint64_t stride, uint64_t n_out) {
-    if (!(h->ch_smem_set & (1u << J))) {
-        CK(cudaFuncSetAttribute(k_channelize<J>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_CH_SMEM));
-        h->ch_smem_set |= 1u << J;
+                               uint32_t D, const Taps& T, uint32_t* d_out, uint64_t stride, uint64_t n_out) {
+    constexpr bool RAT = std::is_same<Taps, RtTaps>::value;
+    const uint64_t bit = 1ull << (J + (RAT ? 32 : 0));
+    if (!(h->ch_smem_set & bit)) {
+        CK(cudaFuncSetAttribute(k_channelize<J, RAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_CH_SMEM));
+        h->ch_smem_set |= bit;
     }
     CK(cudaEventRecord(h->ev0, st));
-    k_channelize<J><<<grid, SB_FIR_THREADS, SB_CH_SMEM, st>>>(d_in, n_in, (const uint32_t*)h->nco.p, ch, cpg, D, T, d_out, stride, n_out);
+    k_channelize<J, RAT><<<grid, SB_FIR_THREADS, SB_CH_SMEM, st>>>(d_in, n_in, (const uint32_t*)h->nco.p, ch, cpg, D, T, d_out, stride, n_out);
     return SB200_OK;
 }
-static int channelize_launch(sb200_handle* h, cudaStream_t st, const uint32_t* d_in, uint64_t n_in, const ChChannels& ch, uint32_t D, const ChTaps& T,
+template <class Taps>
+static int channelize_launch(sb200_handle* h, cudaStream_t st, const uint32_t* d_in, uint64_t n_in, const ChChannels& ch, uint32_t D, const Taps& T,
                              uint32_t* d_out, uint64_t stride, uint64_t n_out) {
     if (!h->sms) CK(cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, h->device));
     const uint64_t tiles = (n_in + SB_FIR_TILE - 1) / SB_FIR_TILE;
@@ -921,12 +925,13 @@ static int channelize_launch(sb200_handle* h, cudaStream_t st, const uint32_t* d
     while (groups < ch.n && tiles * groups < 4ull * (uint64_t)h->sms) groups++;
     const uint32_t cpg = (ch.n + groups - 1) / groups; groups = (ch.n + cpg - 1) / cpg;
     const dim3 grid((unsigned)tiles, groups);
-    const uint32_t need = ((SB_FIR_TILE + D - 1) / D + SB_FIR_THREADS - 1) / SB_FIR_THREADS;     // outputs per thread of a tile
+    const uint32_t need = ((SB_FIR_TILE + D - 1) / D + SB_FIR_THREADS - 1) / SB_FIR_THREADS;     // outputs per thread of a tile (and phase)
     if (need <= 1) return channelize_launch_j<1>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
     if (need <= 2) return channelize_launch_j<2>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
     if (need <= 4) return channelize_launch_j<4>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
     if (need <= 8) return channelize_launch_j<8>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
-    return channelize_launch_j<16>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
+    if constexpr (std::is_same<Taps, ChTaps>::value) return channelize_launch_j<16>(h, st, grid, d_in, n_in, ch, cpg, D, T, d_out, stride, n_out);
+    return h->fail(SB200_E_INVALID, "decim must be at least 3 when interp > 1");     // unreachable: D > U >= 2
 }
 
 // 2:1 anti-alias FIR decimator (k_fir_decimate2): channel (0, 0) of the channelizer's arithmetic with D = 2,
@@ -967,18 +972,30 @@ static int upload_nco(sb200_handle* h) {
 }
 
 // Wideband channelizer (fir_kernels.cuh): every channel shifted by its NCO, filtered and decimated by `decim`; channel c in row c of `out`.
-extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t decim,
-                                const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
+// sb200_channelize is the interp = 1 case of sb200_channelize_rational; both share the checks, staging and launch here.
+static int channelize_call(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t interp,
+                           uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream, uint32_t max_decim) {
     if (!h) return SB200_E_INVALID;
     if (!iq || !channels || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
     if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
-    if (decim < 1 || decim > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "decim must be 1 .. 16");
-    if ((ntaps & 1u) == 0 || ntaps > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 255");
-    uint32_t asum = 0; for (uint32_t i = 0; i < ntaps; i++) asum += (uint32_t)abs((int)taps[i]);
-    if (asum > 65535u) return h->fail(SB200_E_INVALID, "sum of |taps| must be at most 65535 (the int32 accumulator must not wrap)");
+    if (max_decim == SB_CH_MAXDECIM) {
+        if (decim < 1 || decim > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "decim must be 1 .. 16");
+        if ((ntaps & 1u) == 0 || ntaps > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 255");
+    } else {
+        if (interp < 1 || interp > SB_CH_MAXINTERP) return h->fail(SB200_E_INVALID, "interp must be 1 .. 16");
+        if (decim < interp || decim > SB_CH_MAXRDECIM) return h->fail(SB200_E_INVALID, "decim must be interp .. 64");
+        uint32_t a = interp, b = decim; while (b) { const uint32_t t = a % b; a = b; b = t; }
+        if (a != 1) return h->fail(SB200_E_INVALID, "interp and decim must be coprime");
+        if ((ntaps & 1u) == 0 || (ntaps + interp - 1) / interp > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and ceil(ntaps / interp) at most 255");
+    }
+    for (uint32_t r = 0; r < interp; r++) {           // output m meets only the taps k = c - D m (mod interp): one branch per residue
+        uint32_t asum = 0; for (uint32_t i = r; i < ntaps; i += interp) asum += (uint32_t)abs((int)taps[i]);
+        if (asum > 65535u) return h->fail(SB200_E_INVALID, interp == 1 ? "sum of |taps| must be at most 65535 (the int32 accumulator must not wrap)"
+                                                                       : "sum of |taps[k]| over k = r (mod interp) must be at most 65535 for every r (the int32 accumulator must not wrap)");
+    }
     if (n_in > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples must be at most 2^40");
-    const uint64_t n_out = (n_in + decim - 1) / decim;
-    if (out_stride < n_out || (out_stride & 3u) || out_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "out_stride must be at least ceil(n_in / decim), at most 2^40 and a multiple of 4");
+    const uint64_t n_out = (interp * n_in + decim - 1) / decim;
+    if (out_stride < n_out || (out_stride & 3u) || out_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "out_stride must be at least ceil(interp n_in / decim), at most 2^40 and a multiple of 4");
     if (n_in == 0) return SB200_OK;
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
@@ -993,11 +1010,27 @@ extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_i
         d_stride = (n_out + 3u) & ~3ull; CK(h->iq40.need(nchannels * d_stride * 4ull)); d_out = (uint32_t*)h->iq40.p;
         ret.bind2d(out, out_stride * 4ull, d_out, d_stride * 4ull, n_out * 4ull, nchannels);
     }
-    ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
     ChChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
     for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; }
-    const int rc = channelize_launch(h, st, d_in, n_in, ch, decim, T, d_out, d_stride, n_out);
+    int rc;
+    if (interp == 1) {
+        ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
+        rc = channelize_launch(h, st, d_in, n_in, ch, decim, T, d_out, d_stride, n_out);
+    } else {                                           // by branch: taps[r + U l] at t[r][l]
+        static_assert(sizeof(RtTaps) + sizeof(ChChannels) + 64 <= 32764, "kernel parameters of k_channelize<J, true>");
+        RtTaps T; memset(&T, 0, sizeof T); T.n = ntaps; T.u = interp; for (uint32_t i = 0; i < ntaps; i++) T.t[i % interp][i / interp] = taps[i];
+        rc = channelize_launch(h, st, d_in, n_in, ch, decim, T, d_out, d_stride, n_out);
+    }
     return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
+}
+extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t decim,
+                                const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
+    return channelize_call(h, iq, n_in, channels, nchannels, 1, decim, taps, ntaps, out, out_stride, cuda_stream, SB_CH_MAXDECIM);
+}
+// Rational-rate channelizer: every channel shifted by its NCO, zero-stuffed by `interp`, filtered and decimated by `decim`.
+extern "C" int sb200_channelize_rational(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels,
+                                         uint32_t interp, uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
+    return channelize_call(h, iq, n_in, channels, nchannels, interp, decim, taps, ntaps, out, out_stride, cuda_stream, SB_CH_MAXRDECIM);
 }
 
 // One launch of k_combine<J> (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.
