@@ -13,6 +13,7 @@
   --config channelize  the wideband channelizer: four 802.11a channels of a 160 Msps capture, 127 taps, D = 4, device-resident
   --config channelize_rational  the rational-rate channelizer: three 802.11b channels of a 160 Msps capture to 44 Msps, 1287 taps, U / D = 11 / 40
   --config combine   the wideband combiner: four 802.11a channel rows at 40 Msps into one 160 Msps capture, 127 taps, U = 4, device-resident
+  --config combine_rational  the rational-rate combiner: three 802.11b rows at 44 Msps into one 160 Msps capture, 1761 taps, U / D = 40 / 11
   --config sim       the radio channel simulator: --frames links of config #2's 9 824-sample slots (T = R = 1, L = 16, +20 ppm, a carrier
                      offset, noise on), and a 2x2 case (T = R = 2, L = 16), device-resident
   --config 11n       config #4: 802.11n HT-MF 2x2 RX chain at MCS 8, 9, 10, PSDU 1500 B, 2 x 40 Msps, fixed 2x2 channel
@@ -525,6 +526,38 @@ def bench_combine(args):
             "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs" % m})
     c.close()
 
+def bench_combine_rational(args):
+    """The rational-rate combiner into a device-resident 160 Msps capture the size of --config combine's: three 802.11b rows at 44 Msps
+    moved to -25 / 0 / +25 MHz, U / D = 40 / 11 through 1761 taps (45 per branch; --ratio U/D picks another pair, with 45 taps per branch
+    of a low-pass at 0.55 of the row's Nyquist).  Work per output sample: K (2 ceil(ntaps / U) + 4 + 2) integer multiply-adds; HBM traffic
+    4 B written + 4 K D / U B read."""
+    import wideband_inputs as W, combine_rational_model as CR
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    U, D = (int(v) for v in args.ratio.split("/")); K = 3; n_out = args.frames * 9824 * 4; n_in = -(-D * n_out // U); stride = (n_in + 3) // 4 * 4
+    taps = W.lowpass(1761, 12e6 / 1.76e9, gain=40) if (U, D) == (40, 11) else W.lowpass(45 * U - 1 + (U % 2), 0.275 / U, gain=U)
+    ch = [(W.phase_inc(f, 160e6), 0, 4096) for f in (-25e6, 0.0, 25e6)]
+    x = torch.randint(-8000, 8000, (K, stride, 2), dtype=torch.int16, device=dev); y = torch.empty((n_out, 2), dtype=torch.int16, device=dev)
+    def step(): eng.combine_raw(x.data_ptr(), stride, n_in, ch, U, taps, y.data_ptr(), st.cuda_stream, decim=D, n_out=n_out)
+    step(); torch.cuda.synchronize()
+    m = 20000                                                            # the first outputs, from the inputs they read
+    assert (CR.combine_rational_window(x[:, :D * m // U + len(taps)].cpu().numpy(), ch, U, D, taps, 0, m) == y[:m].cpu().numpy()).all(), "combiner output differs from the stated arithmetic"
+    ms = c.timed(step, args.steps)
+    sec = ms * 1e-3
+    hbm = n_out * (4.0 + 4.0 * K * D / U); macs = n_out * K * (2.0 * -(-len(taps) // U) + 6.0)
+    name, plim, clk = _card(); sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    imad_peak = sms * 64 * clk * 1e6 if clk else None                    # int32 IMAD: 64 per SM per clock on sm_90
+    f_hbm = hbm / sec / 1e9 / peaks(); f_int = (macs / sec / imad_peak) if imad_peak else None
+    c.emit({"metric": "rational combiner output Msamples/s (COMPLEX16 out, 3 channels, U / D = %d / %d)" % (U, D), "value": c.world * n_out / sec / 1e6, "unit": "Msamples/s", "ms_per_step": ms,
+            "n_gpus": c.world,
+            "config": {"workload": "3 x 802.11b rows at 44 Msps -> 160 Msps capture, channels at -25/0/+25 MHz, %d taps, U = %d, D = %d, device-resident" % (len(taps), U, D), "output_samples_per_step_per_gpu": n_out},
+            "hbm": {"achieved": hbm / sec / 1e9, "peak": peaks(), "unit": "GB/s", "frac": f_hbm, "note": "4 B written + 4 K D / U B read per output sample"},
+            "int_mad": {"achieved": macs / sec / 1e9, "peak": imad_peak / 1e9 if imad_peak else None, "unit": "G multiply-adds/s", "frac": f_int,
+                        "note": "K (2 ceil(ntaps / U) + 4 + 2) per output sample; peak = SMs x 64 x max SM clock"},
+            "bound": None if f_int is None else ("integer" if f_int > f_hbm else "hbm"),
+            "card": name, "power_limit_w": plim, "max_sm_clock_mhz": clk,
+            "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs" % m})
+    c.close()
+
 def bench_sim(args):
     """The radio channel simulator on device-resident links of config #2's slot length (9 824 samples at 40 Msps): T = R = 1 with 16 taps,
     and T = R = 2 with 16 taps per pair, every link at +20 ppm with a carrier offset and noise.  Integer work per output sample, from the
@@ -564,10 +597,12 @@ def bench_sim(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_rational", "combine", "sim"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_rational", "combine", "combine_rational", "sim"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
+    ap.add_argument("--ratio", default="40/11", help="U/D of --config combine_rational; the channel plan stays three rows at -25/0/+25 MHz of 160 Msps, and "
+                    "a pair other than 40/11 takes a generic low-pass of 45 taps per branch at 0.55 of the row's Nyquist")
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_rational": bench_channelize_rational, "combine": bench_combine, "sim": bench_sim}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_rational": bench_channelize_rational, "combine": bench_combine, "combine_rational": bench_combine_rational, "sim": bench_sim}[a.config](a)

@@ -207,6 +207,31 @@ typedef struct sb200_duc_channel { uint32_t phase_inc; uint32_t phase0; uint32_t
 int sb200_combine(sb200_handle* h, const int16_t* rows, uint64_t row_stride_samples, uint64_t n_in_samples, const sb200_duc_channel* channels,
                   uint32_t nchannels, uint32_t interp, const int16_t* taps, uint32_t ntaps, int16_t* out, void* cuda_stream);
 
+/* Rational-rate combiner, the transmit counterpart of sb200_channelize_rational: sb200_combine with the rate changed by U / D (U = interp,
+ * D = decim) instead of U, so that rows of rates that no whole-number U reaches go into one capture (802.11b at 44 Msps into 160 Msps with
+ * (40, 11), OFDM at 40 Msps into 176 Msps with (22, 5)); an extension without a reference counterpart.  For channel k = {phase_inc, phase0,
+ * gain}, c = (ntaps - 1) / 2 and every output n in 0 .. n_out = n_out_samples:
+ *     z_k(i)  = x_k(i / U) if i mod U == 0 and 0 <= i / U < n_in, else 0              zero-stuffing
+ *     u_k(n)  = sat16((sum_j taps[j] * z_k(D n + j - c) + 2^14) >> 15)                int32, re and im independently
+ *     v_k(n)  = u_k(n) rotated UP by NCO[(phase0 + (uint32)n * phase_inc) >> 20]      sb200_combine's rotation, n = absolute output index
+ *     a(n)    = accumulate ? out[n] as it was before the call : 0
+ *     y(n)    = sat16(a(n) + sum_k ((v_k(n) * gain_k + 2^11) >> 12))                  int32, re and im independently
+ * Output n stands at input time D n / U: output 0 lines up with input 0, the channelizer's convention, so a row sent with (U, D, phase_inc,
+ * phase0) comes back from sb200_channelize_rational with (D, U) and the same pair.  Only the taps j = c - D n (mod U) meet a non-zero z,
+ * so the accumulator limit is per branch.  n_out is the caller's choice: outputs past the rows' support are a(n) plus the filter's tails, so
+ * rows need no trailing zeros.  accumulate = 1 adds the call onto out with one saturation per call, so that one capture holds rows of two
+ * rates (two calls into one buffer).  With decim = 1, interp <= 16, ntaps <= 255, n_out = U n_in and accumulate = 0 this is sb200_combine,
+ * bit for bit.  rows and out may be host or device pointers (device: 16-byte aligned, and the call is then asynchronous on the stream; a
+ * host out is uploaded first when accumulate = 1); channels and taps are host arrays.  Limits (SB200_E_INVALID, nothing launched):
+ * 1 <= decim <= 16, decim <= interp <= 64, gcd(interp, decim) = 1 (rate increase only), ntaps odd, <= 4095 and ceil(ntaps / interp) <= 255,
+ * for every residue r mod interp the sum of |taps[j]| over j = r (mod interp) <= 65535, gain <= 65535, 1 <= nchannels <= 16,
+ * row_stride >= n_in, a multiple of 4 and <= 2^40, n_in <= 2^40, n_out <= 2^40, accumulate 0 or 1.  n_out = 0 launches nothing and
+ * n_in = 0 means all-zero rows.  One kernel launch; sb200_last_kernel_ms times it. */
+int sb200_combine_rational(sb200_handle* h, const int16_t* rows, uint64_t row_stride_samples, uint64_t n_in_samples,
+                           const sb200_duc_channel* channels, uint32_t nchannels, uint32_t interp, uint32_t decim,
+                           const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t n_out_samples, uint32_t accumulate,
+                           void* cuda_stream);
+
 /* Radio channel simulator: nlinks independent links, each from T = ntx input rows x_t[0 .. n_in) to R = nrx output rows y_r[0 .. n_out) of
  * COMPLEX16 through a sampling-clock offset, multipath, a carrier offset and seeded noise, in the manner of GNU Radio's channel_model; an
  * extension without a reference counterpart.  Row t of link l is at x + l * in_link_stride + t * in_row_stride samples, row r of y at

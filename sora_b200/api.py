@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_combine", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_combine", "sb200_combine_rational", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -299,20 +299,33 @@ class Engine:
         self.channelize_raw(_ptr(iq), len(iq), channels, decim, taps, _ptr(out), stride, interp=interp)
         return out[:, :n_out]
 
-    def combine_raw(self, rows_ptr, row_stride, n_in, channels, interp, taps, out_ptr, stream=0):
-        """Pointer-level sb200_combine: rows_ptr / out_ptr host or device addresses; channels a list of (phase_inc, phase0, gain); taps int16 Q15."""
+    def combine_raw(self, rows_ptr, row_stride, n_in, channels, interp, taps, out_ptr, stream=0, decim=1, n_out=None, accumulate=False):
+        """Pointer-level sb200_combine (decim = 1, n_out None, accumulate False) or sb200_combine_rational: rows_ptr / out_ptr host or device
+        addresses; channels a list of (phase_inc, phase0, gain); taps int16 Q15; n_out outputs (None: ceil(interp n_in / decim))."""
         ch = (DucChannel * max(len(channels), 1))(*[DucChannel(int(a) % 2 ** 32, int(b) % 2 ** 32, int(g)) for a, b, g in channels])
         t = np.ascontiguousarray(taps, dtype=np.int16)
-        self._check(self._lib.sb200_combine(self._h, C.c_void_p(rows_ptr), C.c_uint64(row_stride), C.c_uint64(n_in), C.cast(ch, C.c_void_p), C.c_uint32(len(channels)),
-                                            C.c_uint32(interp), C.c_void_p(_ptr(t)), C.c_uint32(len(t)), C.c_void_p(out_ptr), C.c_void_p(stream)), "sb200_combine")
+        if decim == 1 and n_out is None and not accumulate:
+            self._check(self._lib.sb200_combine(self._h, C.c_void_p(rows_ptr), C.c_uint64(row_stride), C.c_uint64(n_in), C.cast(ch, C.c_void_p), C.c_uint32(len(channels)),
+                                                C.c_uint32(interp), C.c_void_p(_ptr(t)), C.c_uint32(len(t)), C.c_void_p(out_ptr), C.c_void_p(stream)), "sb200_combine")
+        else:
+            n_out = -(-interp * n_in // decim) if n_out is None else n_out
+            self._check(self._lib.sb200_combine_rational(self._h, C.c_void_p(rows_ptr), C.c_uint64(row_stride), C.c_uint64(n_in), C.cast(ch, C.c_void_p),
+                                                         C.c_uint32(len(channels)), C.c_uint32(interp), C.c_uint32(decim), C.c_void_p(_ptr(t)), C.c_uint32(len(t)),
+                                                         C.c_void_p(out_ptr), C.c_uint64(n_out), C.c_uint32(int(accumulate)), C.c_void_p(stream)), "sb200_combine_rational")
 
-    def combine(self, rows, channels, interp, taps):
-        """Wideband combiner: int16 [K, n_in, 2] rows and K channels (phase_inc, phase0, gain Q12) -> int16 [interp * n_in, 2], every row
-        interpolated by interp through taps (int16 Q15, odd count <= 255, per-branch sum |t| <= 65535), moved to its centre, scaled and summed."""
+    def combine(self, rows, channels, interp, taps, decim=1, n_out=None, accumulate=False, out=None):
+        """Wideband combiner: int16 [K, n_in, 2] rows and K channels (phase_inc, phase0, gain Q12) -> int16 [n_out, 2], every row
+        interpolated by interp through taps (int16 Q15, odd count <= 255, per-branch sum |t| <= 65535), moved to its centre, scaled and summed;
+        n_out = interp * n_in.  With decim, n_out or accumulate it is sb200_combine_rational: the rate changes by interp / decim (ntaps <= 4095
+        with ceil(ntaps / interp) <= 255), n_out defaults to ceil(interp n_in / decim), and accumulate adds the sum onto `out` (int16
+        [n_out, 2], updated in place and returned) with one saturation."""
         rows = np.asarray(rows, dtype=np.int16).reshape(len(channels), -1, 2); n_in = rows.shape[1]; stride = (n_in + 3) // 4 * 4
         x = np.zeros((len(channels), stride, 2), np.int16); x[:, :n_in] = rows
-        out = np.zeros((interp * n_in, 2), np.int16)
-        self.combine_raw(_ptr(x), stride, n_in, channels, interp, taps, _ptr(out))
+        n = -(-interp * n_in // decim) if n_out is None else n_out
+        if out is None: out = np.zeros((n, 2), np.int16)
+        if not (isinstance(out, np.ndarray) and out.dtype == np.int16 and out.shape == (n, 2) and out.flags.c_contiguous and out.flags.writeable):
+            raise ValueError("out must be a writeable C-contiguous int16 numpy array of shape [n_out, 2]")
+        self.combine_raw(_ptr(x), stride, n_in, channels, interp, taps, _ptr(out), decim=decim, n_out=n_out, accumulate=accumulate)
         return out
 
     def channel_sim_raw(self, x_ptr, in_link_stride, in_row_stride, ntx, n_in, links, taps, ntaps, nlinks, seed, y_ptr, out_link_stride, out_row_stride,

@@ -285,23 +285,53 @@ __device__ __forceinline__ cs16 nco_rotate_up(cs16 u, uint32_t cs) {
     return mk(sat16((u.re * r.re - u.im * r.im + (1 << 13)) >> 14), sat16((u.im * r.re + u.re * r.im + (1 << 13)) >> 14));
 }
 
-// grid tiles, SB_FIR_THREADS threads, combine_smem(K, U, ntaps, 256 J) bytes of dynamic shared memory.  Row k starts at x + k * stride.
-template <int J>
+// sb200_combine_rational runs the same kernel at a rational rate U / D (RAT = true): output n = U q + s (phase s) meets only the branch of
+// taps j = r_s + U l, r_s = (c - D s) mod U, on the inputs x(D q + e_s + l), e_s = (D s + r_s - c) / U exactly; at D = 1 this is the
+// mapping above with q = i.  A tile is TQ = 32 W J consecutive q of every phase (U TQ outputs) and reads the inputs D q0 - halo ..
+// D (q0 + TQ) + halo of every row.  The lanes of a warp take consecutive q of one phase, so the tap stays a uniform constant and the lanes
+// read words D apart: free of bank conflicts for odd D (even D is accepted with its gcd(D, 32)-way conflicts, DESIGN.md §8).  Groups of W
+// warps take the phases g, g + G, ... (G = 8 / W) side by side.  The host picks the largest TQ whose shared memory fits SB_CBR_SMEM
+// (four CTAs per multiprocessor), else TQ = 32, which fits SB_CBR_SMEM_MAX (three) at every limit.  With accumulate the output tile is
+// first loaded from HBM with 16-byte loads and each sum adds onto it before its single saturation.
+#define SB_CBR_MAXTAPS 4095                // sb200_combine_rational's limits: U <= 64, D <= 16, ntaps <= 4095
+#define SB_CBR_MAXINTERP 64
+#define SB_CBR_SMEM 57344                  // preferred budget: four CTAs per multiprocessor (4 x (56 + 1) KB of 228 KB)
+#define SB_CBR_SMEM_MAX 75776              // the budget of TQ = 32: three CTAs per multiprocessor (3 x (74 + 1) KB)
+// The taps of sb200_combine_rational by branch: taps[r + U l] at t[r * L + l], L = ceil(ntaps / U), U L <= ntaps + U - 1.  8.3 KB of
+// kernel parameters (allowed up to 32 KB since CUDA 12.1 on sm_70 and later), read like RtTaps: one uniform constant-bank load per tap.
+struct CbrTaps { int16_t t[SB_CBR_MAXTAPS + SB_CBR_MAXINTERP + 1]; uint32_t n, u, L; };
+// Dynamic shared memory of k_combine<J, true> for tq outputs per phase: K windows of D tq + 2 halo words, the U tq output tile, the NCO
+// table and the mbarrier.
+__host__ __device__ constexpr uint32_t combine_smem_r(uint32_t K, uint32_t U, uint32_t D, uint32_t ntaps, uint32_t tq) {
+    return (K * (D * tq + 2 * combine_halo(ntaps, U)) + U * tq + SB_CH_NCO) * 4u + 16u;
+}
+static_assert(combine_smem_r(SB_CH_MAXCH, SB_CBR_MAXINTERP, SB_CH_MAXDECIM, 255 * SB_CBR_MAXINTERP, 32) <= SB_CBR_SMEM_MAX && combine_halo(255 * SB_CBR_MAXINTERP, SB_CBR_MAXINTERP) == SB_CH_MAXHALO,
+              "a tile of 32 outputs per phase must fit SB_CBR_SMEM_MAX at every K, U, D and ntaps (halo <= 128 while ceil(ntaps / U) <= 255)");
+
+// grid (tiles, 1) or, RAT, (gx, gy) with tile = x + gx y; SB_FIR_THREADS threads; combine_smem(K, U, ntaps, 256 J) or, RAT,
+// combine_smem_r(K, U, D, ntaps, 32 W J) bytes of dynamic shared memory.  Row k starts at x + k * stride; outputs y[0 .. n_out).
+// RAT = false: D = W / 8 = 1, ChTaps, n_out = U n_in, no accumulate (sb200_combine); RAT = true: CbrTaps (sb200_combine_rational).
+template <int J, bool RAT>
 __global__ void __launch_bounds__(SB_FIR_THREADS) k_combine(const uint32_t* __restrict__ x, uint64_t stride, uint64_t n_in, const uint32_t* __restrict__ nco,
-                                                           CbChannels ch, uint32_t U, ChTaps taps, uint32_t* __restrict__ y) {
-    constexpr uint32_t TI = SB_FIR_THREADS * J;
+                                                           CbChannels ch, uint32_t U, uint32_t Dr, uint32_t Wr, typename std::conditional<RAT, CbrTaps, ChTaps>::type taps,
+                                                           uint32_t* __restrict__ y, uint64_t n_out, uint32_t accumulate) {
+    const uint32_t D = RAT ? Dr : 1u, W = RAT ? Wr : SB_FIR_THREADS / 32u;
+    const uint32_t TQ = 32u * W * J, G = (SB_FIR_THREADS / 32u) / W;    // outputs per phase of a tile; groups of W warps
     extern __shared__ __align__(16) uint32_t smem[];
-    const uint32_t tid = threadIdx.x, K = ch.n, c = taps.n >> 1, halo = combine_halo(taps.n, U), win = TI + 2 * halo;
-    uint32_t* s_y = smem + K * win; uint32_t* s_nco = s_y + U * TI;
+    const uint32_t tid = threadIdx.x, K = ch.n, c = taps.n >> 1, halo = combine_halo(taps.n, U), win = D * TQ + 2 * halo;
+    uint32_t* s_y = smem + K * win; uint32_t* s_nco = s_y + U * TQ;
     unsigned long long* s_bar = (unsigned long long*)(s_nco + SB_CH_NCO);
-    const uint64_t t0 = (uint64_t)blockIdx.x * TI;                      // first input sample of this tile
+    const uint64_t q0 = (RAT ? (uint64_t)blockIdx.y * gridDim.x + blockIdx.x : (uint64_t)blockIdx.x) * TQ;   // first output of every phase of this tile
+    const uint64_t n0 = U * q0;                                         // first output of this tile
+    if (RAT && n0 >= n_out) return;                                     // the rounded-up grid's last CTAs
+    const uint64_t t0 = D * q0;                                         // input D q0 lines up with output U q0
     bool rotate = false;                                                // the table is only brought in when a channel needs it
     for (uint32_t k = 0; k < K; k++) rotate |= ch.inc[k] != 0u || (ch.phase0[k] >> 20) != 0u;
 
-    // Staging: stage_window's steps for K rows on one barrier (window k holds samples [t0 - halo, t0 + TI + halo) of row k, zero outside
-    // [0, n_in)).  halo, TI and stride are multiples of 4, so every copy's source and destination are 16-byte aligned.
+    // Staging: stage_window's steps for K rows on one barrier (window k holds samples [t0 - halo, t0 + D TQ + halo) of row k, zero outside
+    // [0, n_in)).  halo, D TQ and stride are multiples of 4, so every copy's source and destination are 16-byte aligned.
     const uint64_t w0 = t0 >= halo ? t0 - halo : 0ull;
-    const uint64_t w1 = t0 + TI + halo < n_in ? t0 + TI + halo : n_in;
+    const uint64_t w1e = t0 + D * TQ + halo < n_in ? t0 + D * TQ + halo : n_in, w1 = (RAT && w1e < w0) ? w0 : w1e;   // RAT: tiles past the rows
     const uint32_t dst0 = (uint32_t)(w0 - (t0 - halo)), nw = (uint32_t)(w1 - w0), bulk = nw & ~3u;
     for (uint32_t i = tid; i < K * win; i += SB_FIR_THREADS) { const uint32_t q = i % win; if (q < dst0 || q >= dst0 + bulk) smem[i] = 0; }
     if (tid == 0) {
@@ -320,16 +350,26 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_combine(const uint32_t* __re
                                  :: "r"((uint32_t)__cvta_generic_to_shared(s_nco)), "l"(nco), "r"(SB_CH_NCO * 4u), "r"(mb) : "memory");
     }
     if (tid < K * (nw & 3u)) { const uint32_t k = tid / (nw & 3u), q = tid % (nw & 3u); smem[k * win + dst0 + bulk + q] = __ldg(x + k * stride + w0 + bulk + q); }
+    // outputs n0 .. n0 + nt of y[0 .. n_out); with accumulate they are loaded into the output tile first (16-byte loads: n0 is a multiple of 4)
+    if (RAT && accumulate) {
+        const uint64_t nt = n_out - n0 < (uint64_t)U * TQ ? n_out - n0 : (uint64_t)U * TQ;
+        const uint32_t n4 = (uint32_t)nt >> 2;
+        const uint4* y4 = (const uint4*)(y + n0); uint4* s4 = (uint4*)s_y;
+        for (uint32_t q = tid; q < n4; q += SB_FIR_THREADS) s4[q] = y4[q];
+        if (tid < ((uint32_t)nt & 3u)) s_y[4 * n4 + tid] = y[n0 + 4 * n4 + tid];
+    }
     if (bytes) {
         uint32_t ok = 0;
         while (!ok) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(ok) : "r"(mb) : "memory");
     }
     __syncthreads();
 
-    for (uint32_t r = 0; r < U; r++) {
-        const uint32_t j0 = (c % U + U - r) % U;                        // first tap of phase r's branch
-        const int e = ((int)(r + j0) - (int)c) / (int)U;                // exact: r + j0 - c is a multiple of U
-        const uint32_t* s_r = smem + (int)halo + e + tid;               // window word of input t0 + tid, tap j0
+    // RAT = false: one group, grp = 0 and lt = tid at compile time, so the phase and its taps stay uniform to the compiler (DESIGN.md §8)
+    const uint32_t grp = RAT ? (tid >> 5) / W : 0u, lt = RAT ? tid - grp * W * 32u : tid;
+    for (uint32_t s = grp; s < U; s += G) {                             // warps past the last group (8 % W of them) idle
+        const uint32_t rs = (c % U + U - (D * s) % U) % U;              // first tap of phase s's branch
+        const int e = ((int)(D * s + rs) - (int)c) / (int)U;            // exact: D s + r_s - c is a multiple of U
+        const uint32_t* s_r = smem + (int)halo + e + D * lt;            // window word of input D (q0 + lt) + e_s, tap r_s
         int sre[J], sim[J];
 #pragma unroll
         for (int j = 0; j < J; j++) sre[j] = sim[j] = 0;
@@ -337,13 +377,27 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_combine(const uint32_t* __re
             uint32_t accr[J], acci[J];
 #pragma unroll
             for (int j = 0; j < J; j++) accr[j] = acci[j] = 1u << 14;
-            for (uint32_t jj = j0, l = 0; jj < taps.n; jj += U, l++) {  // one tap at a time over the J inputs: the tap is a uniform constant
-                const int t = taps.t[jj];
-                if (t != 0) {
+            if constexpr (RAT) {
+                const uint32_t L = rs < taps.n ? (taps.n - 1 - rs) / U + 1 : 0u;
+                for (uint32_t l = 0, jb = rs * taps.L; l < L; l++, jb++) {   // one tap at a time over the J outputs: the tap is a uniform constant
+                    const int t = taps.t[jb];
+                    if (t != 0) {
 #pragma unroll
-                    for (int j = 0; j < J; j++) {
-                        const cs16 v = unpack(s_r[l + SB_FIR_THREADS * j]);
-                        accr[j] += (uint32_t)(t * v.re); acci[j] += (uint32_t)(t * v.im);   // the per-branch tap limit keeps this from wrapping
+                        for (int j = 0; j < J; j++) {
+                            const cs16 v = unpack(s_r[l + D * 32u * W * j]);
+                            accr[j] += (uint32_t)(t * v.re); acci[j] += (uint32_t)(t * v.im);   // the per-branch tap limit keeps this from wrapping
+                        }
+                    }
+                }
+            } else {
+                for (uint32_t jj = rs, l = 0; jj < taps.n; jj += U, l++) {  // one tap at a time over the J inputs: the tap is a uniform constant
+                    const int t = taps.t[jj];
+                    if (t != 0) {
+#pragma unroll
+                        for (int j = 0; j < J; j++) {
+                            const cs16 v = unpack(s_r[l + SB_FIR_THREADS * j]);
+                            accr[j] += (uint32_t)(t * v.re); acci[j] += (uint32_t)(t * v.im);   // the per-branch tap limit keeps this from wrapping
+                        }
                     }
                 }
             }
@@ -353,19 +407,23 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_combine(const uint32_t* __re
             for (int j = 0; j < J; j++) {
                 cs16 v = mk(sat16((int)accr[j] >> 15), sat16((int)acci[j] >> 15));
                 if (!ident) {
-                    const uint32_t n = U * (uint32_t)(t0 + tid + SB_FIR_THREADS * j) + r;   // absolute output index mod 2^32
+                    const uint32_t n = U * (uint32_t)(q0 + lt + 32u * W * j) + s;   // absolute output index mod 2^32
                     v = nco_rotate_up(v, s_nco[(ch.phase0[k] + n * inc) >> 20]);
                 }
                 sre[j] += (v.re * (int)g + (1 << 11)) >> 12; sim[j] += (v.im * (int)g + (1 << 11)) >> 12;
             }
         }
 #pragma unroll
-        for (int j = 0; j < J; j++) s_y[(tid + SB_FIR_THREADS * j) * U + r] = pack(mk(sat16(sre[j]), sat16(sim[j])));
+        for (int j = 0; j < J; j++) {
+            uint32_t* o = s_y + (lt + 32u * W * j) * U + s;
+            if (RAT && accumulate) { const cs16 a = unpack(*o); sre[j] += a.re; sim[j] += a.im; }
+            *o = pack(mk(sat16(sre[j]), sat16(sim[j])));
+        }
     }
     __syncthreads();
 
-    // outputs U t0 .. U t0 + U TI of y[0 .. U n_in): 16-byte stores (U t0 is a multiple of 4), the last 0..3 of the capture by hand
-    const uint64_t n0 = U * t0, n_out = U * n_in, nt = n_out - n0 < (uint64_t)U * TI ? n_out - n0 : (uint64_t)U * TI;
+    // the tile's outputs to HBM: 16-byte stores, the last 0..3 of the capture by hand
+    const uint64_t nt = n_out - n0 < (uint64_t)U * TQ ? n_out - n0 : (uint64_t)U * TQ;
     const uint32_t n4 = (uint32_t)nt >> 2;
     uint4* y4 = (uint4*)(y + n0); const uint4* s4 = (const uint4*)s_y;
     for (uint32_t q = tid; q < n4; q += SB_FIR_THREADS) y4[q] = s4[q];

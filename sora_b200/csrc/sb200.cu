@@ -274,7 +274,7 @@ struct sb200_handle {
     DevBuf nco;                                        // NCO table of the channelizer and the combiner (fir_kernels.cuh), built on first use
     uint64_t ch_smem_set = 0;                          // bit J (+ 32 for RAT): k_channelize<J, RAT> may use SB_CH_SMEM bytes of dynamic shared memory on this device
     int sms = 0;                                       // multiprocessors of the device (channel groups of k_channelize)
-    uint32_t cb_smem_set = 0;                          // bit J: k_combine<J> may use SB_CB_SMEM bytes of dynamic shared memory on this device
+    uint32_t cb_smem_set = 0;                          // bit J (+ 16 for RAT): k_combine<J, RAT> may use SB_CB_SMEM (SB_CBR_SMEM_MAX) bytes of dynamic shared memory on this device
     DevBuf simtab, simlink, simtap;                    // channel simulator: its table (sim_kernels.cuh, built on first use), staged links and taps
     uint32_t sim_smem_set = 0;                         // bit J: k_channel_sim<J> may use its largest dynamic shared memory on this device
     DevBuf vring;
@@ -1033,38 +1033,62 @@ extern "C" int sb200_channelize_rational(sb200_handle* h, const int16_t* iq, uin
     return channelize_call(h, iq, n_in, channels, nchannels, interp, decim, taps, ntaps, out, out_stride, cuda_stream, SB_CH_MAXRDECIM);
 }
 
-// One launch of k_combine<J> (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.
-template <int J>
+// One launch of k_combine<J, RAT> (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.  ChTaps launches the
+// sb200_combine specialisation (D = 1, eight warps per phase), CbrTaps the rational one with W warps per phase; tiles of 32 W J outputs per
+// phase, on a grid of (tiles, 1) CTAs or, RAT, (gx, gy) with tile = x + gx y: n_out <= 2^40 and U TQ >= 32 give at most 2^35 tiles,
+// so gy = ceil(tiles / (2^31 - 1)) <= 16 and gx = ceil(tiles / gy) < 2^31 stay within the grid limits.
+template <int J, class Taps>
 static int combine_launch_j(sb200_handle* h, cudaStream_t st, const uint32_t* d_in, uint64_t stride, uint64_t n_in, const CbChannels& ch, uint32_t U,
-                            const ChTaps& T, uint32_t* d_out) {
-    if (!(h->cb_smem_set & (1u << J))) {
-        CK(cudaFuncSetAttribute(k_combine<J>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_CB_SMEM));
-        h->cb_smem_set |= 1u << J;
+                            uint32_t D, uint32_t W, const Taps& T, uint32_t* d_out, uint64_t n_out, uint32_t accumulate) {
+    constexpr bool RAT = std::is_same<Taps, CbrTaps>::value;
+    const uint32_t bit = 1u << (J + (RAT ? 16 : 0));
+    if (!(h->cb_smem_set & bit)) {
+        CK(cudaFuncSetAttribute(k_combine<J, RAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, RAT ? SB_CBR_SMEM_MAX : SB_CB_SMEM));
+        h->cb_smem_set |= bit;
     }
-    const uint64_t ti = SB_FIR_THREADS * J;
+    const uint64_t tq = 32ull * W * J, tiles = (n_out + U * tq - 1) / (U * tq);
+    const uint64_t gy = RAT ? (tiles + 0x7FFFFFFEull) / 0x7FFFFFFFull : 1u, gx = (tiles + gy - 1) / gy;
+    const uint32_t smem = RAT ? combine_smem_r(ch.n, U, D, T.n, (uint32_t)tq) : combine_smem(ch.n, U, T.n, (uint32_t)tq);
     CK(cudaEventRecord(h->ev0, st));
-    k_combine<J><<<(unsigned)((n_in + ti - 1) / ti), SB_FIR_THREADS, combine_smem(ch.n, U, T.n, (uint32_t)ti), st>>>(d_in, stride, n_in, (const uint32_t*)h->nco.p, ch, U, T, d_out);
+    k_combine<J, RAT><<<dim3((unsigned)gx, (unsigned)gy), SB_FIR_THREADS, smem, st>>>(d_in, stride, n_in, (const uint32_t*)h->nco.p, ch, U, D, W, T, d_out, n_out, accumulate);
     return SB200_OK;
 }
 
-// Wideband combiner (fir_kernels.cuh): every row zero-stuffed by `interp`, filtered, shifted up by its NCO, scaled and summed into `out`.
-// Tiles of 1024, 512 or 256 input samples: the largest whose shared memory fits SB_CB_SMEM (256 always does).
-extern "C" int sb200_combine(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, const sb200_duc_channel* channels, uint32_t nchannels,
-                             uint32_t interp, const int16_t* taps, uint32_t ntaps, int16_t* out, void* cuda_stream) {
+// Wideband combiner (fir_kernels.cuh): every row zero-stuffed by `interp`, filtered (and decimated by `decim`), shifted up by its NCO,
+// scaled and summed into `out` (or onto it).  sb200_combine is the decim = 1, n_out = interp n_in case of sb200_combine_rational with its
+// own limits and kernel specialisation; both share the checks, staging and launch here (rational = false: sb200_combine).
+static int combine_call(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, const sb200_duc_channel* channels, uint32_t nchannels,
+                        uint32_t interp, uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t n_out, uint32_t accumulate,
+                        void* cuda_stream, bool rational) {
     if (!h) return SB200_E_INVALID;
     if (!rows || !channels || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
     if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
-    if (interp < 1 || interp > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "interp must be 1 .. 16");
-    if ((ntaps & 1u) == 0 || ntaps > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 255");
-    for (uint32_t r = 0; r < interp; r++) {           // output n meets only the taps j = c - n (mod interp): one branch per residue
+    if (!rational) {
+        if (interp < 1 || interp > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "interp must be 1 .. 16");
+        if ((ntaps & 1u) == 0 || ntaps > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 255");
+    } else {
+        if (decim < 1 || decim > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "decim must be 1 .. 16");
+        if (interp < decim || interp > SB_CBR_MAXINTERP) return h->fail(SB200_E_INVALID, "interp must be decim .. 64");
+        uint32_t a = interp, b = decim; while (b) { const uint32_t t = a % b; a = b; b = t; }
+        if (a != 1) return h->fail(SB200_E_INVALID, "interp and decim must be coprime");
+        if ((ntaps & 1u) == 0 || ntaps > SB_CBR_MAXTAPS || (ntaps + interp - 1) / interp > SB_CH_MAXTAPS)
+            return h->fail(SB200_E_INVALID, "ntaps must be odd, at most 4095 and ceil(ntaps / interp) at most 255");
+        if (accumulate > 1u) return h->fail(SB200_E_INVALID, "accumulate must be 0 or 1");
+    }
+    for (uint32_t r = 0; r < interp; r++) {           // output n meets only the taps j = c - D n (mod interp): one branch per residue
         uint32_t asum = 0; for (uint32_t i = r; i < ntaps; i += interp) asum += (uint32_t)abs((int)taps[i]);
         if (asum > 65535u) return h->fail(SB200_E_INVALID, "sum of |taps[j]| over j = r (mod interp) must be at most 65535 for every r (the int32 accumulator must not wrap)");
     }
     for (uint32_t i = 0; i < nchannels; i++)
         if (channels[i].gain > 65535u) return h->fail(SB200_E_INVALID, "gain must be at most 65535");
     if (row_stride < n_in || (row_stride & 3u) || row_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "row_stride must be at least n_in, at most 2^40 and a multiple of 4");
-    if (n_in > (1ull << 40) / interp) return h->fail(SB200_E_INVALID, "interp * n_in_samples must be at most 2^40");
-    if (n_in == 0) return SB200_OK;
+    if (!rational) {
+        if (n_in > (1ull << 40) / interp) return h->fail(SB200_E_INVALID, "interp * n_in_samples must be at most 2^40");
+        if (n_in == 0) return SB200_OK;
+    } else {
+        if (n_in > (1ull << 40) || n_out > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples and n_out_samples must be at most 2^40");
+        if (n_out == 0) return SB200_OK;
+    }
     cudaStream_t st = (cudaStream_t)cuda_stream;
     CK(cudaSetDevice(h->device));
     const bool in_dev = is_device_ptr(rows), out_dev = is_device_ptr(out);
@@ -1072,21 +1096,47 @@ extern "C" int sb200_combine(sb200_handle* h, const int16_t* rows, uint64_t row_
     CallScope call(h, st); CK(call.begin()); call.reads(rows);
     const int nrc = upload_nco(h);
     if (nrc != SB200_OK) return nrc;
-    const uint64_t n_out = interp * n_in;
     const uint32_t* d_in = (const uint32_t*)rows; uint64_t d_stride = row_stride; uint32_t* d_out; Returns ret;
-    if (!in_dev) {                                     // rows n_in (rounded to 4) apart in the workspace
+    if (!in_dev && n_in) {                             // rows n_in (rounded to 4) apart in the workspace
         d_stride = (n_in + 3u) & ~3ull; CK(h->iq.need(nchannels * d_stride * 4ull + 16)); d_in = (const uint32_t*)h->iq.p;
         CK(cudaMemcpy2DAsync(h->iq.p, d_stride * 4ull, rows, row_stride * 4ull, n_in * 4ull, nchannels, cudaMemcpyHostToDevice, st));
     }
     CK(ret.bind(h->iq40, (uint32_t*)out, n_out * 4ull, &d_out, 16));
-    ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
+    if (accumulate && !out_dev) {                      // the caller's samples go up into the workspace before the launch adds onto them
+        call.reads(out); CK(cudaMemcpyAsync(d_out, out, n_out * 4ull, cudaMemcpyHostToDevice, st));
+    }
     CbChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
     for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; ch.gain[i] = channels[i].gain; }
     int rc;
-    if (combine_smem(nchannels, interp, ntaps, 4 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, T, d_out);
-    else if (combine_smem(nchannels, interp, ntaps, 2 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, T, d_out);
-    else rc = combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, T, d_out);
+    if (!rational) {                                   // tiles of 1024, 512 or 256 input samples: the largest whose shared memory fits SB_CB_SMEM (256 always does)
+        ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
+        if (combine_smem(nchannels, interp, ntaps, 4 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
+        else if (combine_smem(nchannels, interp, ntaps, 2 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
+        else rc = combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
+    } else {                                           // by branch: taps[r + U l] at t[r L + l]
+        static_assert(sizeof(CbrTaps) + sizeof(CbChannels) + 64 <= 32764, "kernel parameters of k_combine<J, true>");
+        CbrTaps T; memset(&T, 0, sizeof T); T.n = ntaps; T.u = interp; T.L = (ntaps + interp - 1) / interp;
+        for (uint32_t i = 0; i < ntaps; i++) T.t[(i % interp) * T.L + i / interp] = taps[i];
+        // 32 W J outputs per phase: the largest of 1024 .. 32 whose shared memory fits SB_CBR_SMEM, else 32 (within SB_CBR_SMEM_MAX)
+        static const uint32_t kj[6] = {4, 2, 1, 1, 1, 1}, kw[6] = {8, 8, 8, 4, 2, 1};
+        int p = 0;
+        while (p < 5 && combine_smem_r(nchannels, interp, decim, ntaps, 32u * kw[p] * kj[p]) > SB_CBR_SMEM) p++;
+        if (kj[p] == 4) rc = combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, decim, kw[p], T, d_out, n_out, accumulate);
+        else if (kj[p] == 2) rc = combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, decim, kw[p], T, d_out, n_out, accumulate);
+        else rc = combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, decim, kw[p], T, d_out, n_out, accumulate);
+    }
     return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
+}
+extern "C" int sb200_combine(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, const sb200_duc_channel* channels, uint32_t nchannels,
+                             uint32_t interp, const int16_t* taps, uint32_t ntaps, int16_t* out, void* cuda_stream) {
+    return combine_call(h, rows, row_stride, n_in, channels, nchannels, interp, 1, taps, ntaps, out, interp * n_in, 0, cuda_stream, false);
+}
+// Rational-rate combiner: every row zero-stuffed by `interp`, filtered, decimated by `decim`, shifted up by its NCO, scaled and summed into
+// n_out outputs, added onto out's samples when `accumulate`.
+extern "C" int sb200_combine_rational(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, const sb200_duc_channel* channels,
+                                      uint32_t nchannels, uint32_t interp, uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out,
+                                      uint64_t n_out, uint32_t accumulate, void* cuda_stream) {
+    return combine_call(h, rows, row_stride, n_in, channels, nchannels, interp, decim, taps, ntaps, out, n_out, accumulate, cuda_stream, true);
 }
 
 // The table of sb200_channel_sim (sim_kernels.cuh), uploaded on first use: the NCO of upload_nco, then H (256 rows of 8 Q14 taps, packed in
