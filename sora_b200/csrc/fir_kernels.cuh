@@ -30,6 +30,7 @@
 #pragma once
 #include <type_traits>
 #include "fixed.cuh"
+#include "bulk_copy.cuh"
 
 namespace sb {
 
@@ -42,6 +43,8 @@ namespace sb {
 #define SB_CH_MAXDECIM 16                  // sb200_channelize's and sb200_combine's limit
 #define SB_CH_MAXINTERP 16                 // sb200_channelize_rational's limits: U <= 16, D <= 64
 #define SB_CH_MAXRDECIM 64
+#define SB_CBR_MAXTAPS 4095                // sb200_combine_rational's limits: U <= 64, D <= 16, ntaps <= 4095
+#define SB_CBR_MAXINTERP 64
 // Words of one window buffer.  The staged window has win = SB_FIR_TILE + 2 halo words; its polyphase copy spans D phases of
 // P = ceil(win / D) words, D P <= win + D - 1, so a buffer holds the largest window plus SB_CH_MAXRDECIM words.
 #define SB_CH_WIN (SB_FIR_TILE + 2 * SB_CH_MAXHALO + SB_CH_MAXRDECIM)
@@ -51,20 +54,23 @@ static_assert(SB_CH_WIN % 4 == 0, "the NCO table behind the two window buffers m
 static_assert(SB_CH_WIN >= SB_FIR_TILE + 2 * SB_CH_MAXHALO + SB_CH_MAXRDECIM - 1, "the polyphase buffer must hold D * ceil(win / D) words");
 
 struct ChTaps { int16_t t[SB_CH_MAXTAPS + 1]; uint32_t n; };
-// The taps of sb200_channelize_rational by branch: taps[r + U l] at t[r][l].  8 KB of kernel parameters (allowed up to 32 KB since CUDA
-// 12.1 on sm_70 and later), read like ChTaps: one uniform constant-bank load per tap.
-struct RtTaps { int16_t t[SB_CH_MAXINTERP][SB_CH_MAXTAPS + 1]; uint32_t n, u; };
+// The taps of the rational-rate kernels (k_channelize<J, true>, k_combine<J, true>) by branch: taps[r + U l] at t[r L + l],
+// L = ceil(ntaps / U), U L <= ntaps + U - 1.  8.3 KB of kernel parameters (allowed up to 32 KB since CUDA 12.1 on sm_70 and later), read
+// like ChTaps: one uniform constant-bank load per tap.
+struct BrTaps { int16_t t[SB_CBR_MAXTAPS + SB_CBR_MAXINTERP + 1]; uint32_t n, u, L; };
+static_assert(SB_CH_MAXINTERP * SB_CH_MAXTAPS <= SB_CBR_MAXTAPS + SB_CBR_MAXINTERP, "BrTaps must hold the channelizer's U L taps as well");
 struct ChChannels { uint32_t inc[SB_CH_MAXCH], phase0[SB_CH_MAXCH]; uint32_t n; };
 
-// Staging of k_channelize and k_channel_sim (sim_kernels.cuh).  k_fir_decimate2 below keeps a copy of these steps inline with its sizes as
-// constants: keep the two in step.  Stages input samples [lo, lo + win) of each of `rows` rows x + k * xstride (each x[0 .. n_in)) into
-// s + k * sstride, zero outside [0, n_in), with one bulk copy per row (plus the 0..3 trailing samples by hand); when `tab` is not null one
-// more bulk copy brings its tab_words words to s_tab on the same barrier.  lo (which may be negative), xstride and sstride are multiples
-// of 4 and x and s are 16-byte aligned, so every copy's source and destination are 16-byte aligned.  Every thread of the CTA calls it; it
-// returns after a __syncthreads with the windows in place.
-__device__ __forceinline__ void stage_window(const uint32_t* __restrict__ x, uint64_t xstride, uint32_t rows, uint64_t n_in, int64_t lo, uint32_t win,
-                                             uint32_t* s, uint32_t sstride, const uint32_t* __restrict__ tab, uint32_t tab_words, uint32_t* s_tab,
-                                             unsigned long long* bar) {
+// Staging of k_channelize, k_combine and k_channel_sim (sim_kernels.cuh).  Stages input samples [lo, lo + win) of each of `rows` rows
+// x + k * xstride (each x[0 .. n_in)) into s + k * sstride, zero outside [0, n_in), with one bulk copy per row (plus the 0..3 trailing
+// samples by hand); when `tab` is not null one more bulk copy brings its tab_words words to s_tab on the same barrier.  lo (which may be
+// negative), xstride and sstride are multiples of 4 and x and s are 16-byte aligned, so every copy's source and destination are 16-byte
+// aligned.  Every thread of the CTA calls both halves: stage_window_issue starts the copies and returns the bytes in flight, which
+// stage_window_wait takes with the barrier's address (smem_addr(bar)); it returns after a __syncthreads with the windows in place.
+// Between the two a kernel may do other work that does not touch the windows (k_combine loads its output tile there).
+__device__ __forceinline__ uint32_t stage_window_issue(const uint32_t* __restrict__ x, uint64_t xstride, uint32_t rows, uint64_t n_in, int64_t lo,
+                                                       uint32_t win, uint32_t* s, uint32_t sstride, const uint32_t* __restrict__ tab,
+                                                       uint32_t tab_words, uint32_t* s_tab, unsigned long long* bar) {
     const uint32_t tid = threadIdx.x, nthr = blockDim.x;
     // samples [w0, w1) of the buffer land in s[w0 - lo ...]; everything else of the window is zero
     const int64_t hi = lo + (int64_t)win;
@@ -76,28 +82,28 @@ __device__ __forceinline__ void stage_window(const uint32_t* __restrict__ x, uin
     // zero the parts of the windows the copies will not write (buffer edges); done before the copies are started, different words
     for (uint32_t k = 0; k < rows; k++)
         for (uint32_t i = tid; i < win; i += nthr) if (i < dst0 || i >= dst0 + bulk) s[k * sstride + i] = 0;
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(bar)));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (tid == 0) mbar_init(smem_addr(bar));
     __syncthreads();
     const uint32_t bytes = rows * bulk * 4u + (tab ? tab_words * 4u : 0u);
     if (tid == 0 && bytes) {
-        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(bar);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes) : "memory");
-        if (bulk) for (uint32_t k = 0; k < rows; k++)
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         :: "r"((uint32_t)__cvta_generic_to_shared(s + k * sstride + dst0)), "l"(x + k * xstride + w0), "r"(bulk * 4u), "r"(mb) : "memory");
-        if (tab) asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                              :: "r"((uint32_t)__cvta_generic_to_shared(s_tab)), "l"(tab), "r"(tab_words * 4u), "r"(mb) : "memory");
+        const uint32_t mb = smem_addr(bar);
+        mbar_expect_tx(mb, bytes);
+        if (bulk) for (uint32_t k = 0; k < rows; k++) bulk_copy_g2s(smem_addr(s + k * sstride + dst0), x + k * xstride + w0, bulk * 4u, mb);
+        if (tab) bulk_copy_g2s(smem_addr(s_tab), tab, tab_words * 4u, mb);
     }
     const uint32_t tail = nw & 3u;
     if (tid < rows * tail) { const uint32_t k = tid / tail, q = tid % tail; s[k * sstride + dst0 + bulk + q] = __ldg(x + k * xstride + w0 + bulk + q); }
-    if (bytes) {
-        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(bar); uint32_t ok = 0;
-        while (!ok) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(ok) : "r"(mb) : "memory");
-    }
+    return bytes;
+}
+__device__ __forceinline__ void stage_window_wait(uint32_t bytes, uint32_t mb) {
+    if (bytes) mbar_wait(mb, 0);
     __syncthreads();
+}
+__device__ __forceinline__ void stage_window(const uint32_t* __restrict__ x, uint64_t xstride, uint32_t rows, uint64_t n_in, int64_t lo, uint32_t win,
+                                             uint32_t* s, uint32_t sstride, const uint32_t* __restrict__ tab, uint32_t tab_words, uint32_t* s_tab,
+                                             unsigned long long* bar) {
+    const uint32_t bytes = stage_window_issue(x, xstride, rows, n_in, lo, win, s, sstride, tab, tab_words, s_tab, bar);
+    stage_window_wait(bytes, smem_addr(bar));
 }
 
 // sb200_fir_decimate2: channel (0, 0), D = 2 of the arithmetic above, ntaps <= 63, on its own kernel.  k_channelize computes the same bits
@@ -112,29 +118,23 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_fir_decimate2(const uint32_t
     __shared__ __align__(8) unsigned long long s_bar;
     const uint64_t t0 = (uint64_t)blockIdx.x * SB_FIR_TILE;             // first input sample of this tile
     const uint32_t tid = threadIdx.x;
-    // A copy of stage_window above (keep the two in step) with its sizes as constants and no NCO table: called through the helper, with
-    // a runtime halo and block size, this kernel ran 5 % slower (DESIGN.md §8).
+    // stage_window's steps for one row with its sizes as constants and no NCO table: called through the helper, with a runtime halo and
+    // block size, this kernel ran 5 % slower (DESIGN.md §8).
     const uint64_t w0 = t0 >= SB_FIR_HALO ? t0 - SB_FIR_HALO : 0ull;
     const uint64_t w1 = t0 + SB_FIR_TILE + SB_FIR_HALO < n_in ? t0 + SB_FIR_TILE + SB_FIR_HALO : n_in;
     const uint32_t dst0 = (uint32_t)(w0 - (t0 - SB_FIR_HALO));
     const uint32_t nw = (uint32_t)(w1 - w0);
     for (uint32_t i = tid; i < SB_FIR_HALO + SB_FIR_TILE + SB_FIR_HALO + 4; i += SB_FIR_THREADS) if (i < dst0 || i >= dst0 + (nw & ~3u)) s_x[i] = 0;
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_bar)));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (tid == 0) mbar_init(smem_addr(&s_bar));
     __syncthreads();
     const uint32_t bulk = nw & ~3u;
     if (tid == 0 && bulk) {
-        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_bar), dst = (uint32_t)__cvta_generic_to_shared(&s_x[dst0]);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bulk * 4u) : "memory");
-        asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" :: "r"(dst), "l"(x + w0), "r"(bulk * 4u), "r"(mb) : "memory");
+        const uint32_t mb = smem_addr(&s_bar);
+        mbar_expect_tx(mb, bulk * 4u);
+        bulk_copy_g2s(smem_addr(&s_x[dst0]), x + w0, bulk * 4u, mb);
     }
     if (tid < (nw & 3u)) s_x[dst0 + bulk + tid] = __ldg(x + w0 + bulk + tid);
-    if (bulk) {
-        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_bar); uint32_t ok = 0;
-        while (!ok) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(ok) : "r"(mb) : "memory");
-    }
+    if (bulk) mbar_wait(smem_addr(&s_bar), 0);
     __syncthreads();
     // thread -> outputs tid + 256 j, j = 0..7 of the tile (lanes two words apart in shared memory: at most a 2-way bank conflict; stores coalesce)
     const int c = (int)(taps.n >> 1);
@@ -172,10 +172,10 @@ __host__ __device__ constexpr uint32_t combine_halo(uint32_t ntaps, uint32_t U) 
 
 // grid (tiles, channel groups), SB_FIR_THREADS threads, SB_CH_SMEM bytes of dynamic shared memory.  J = outputs per thread per tile,
 // channel and phase, at least ceil(ceil(SB_FIR_TILE / D) / SB_FIR_THREADS).  Channel c's row starts at y + c * stride.  RAT = false:
-// U = 1 with ChTaps (sb200_channelize); RAT = true: U = taps.u with the branches of RtTaps.
+// U = 1 with ChTaps (sb200_channelize); RAT = true: U = taps.u with the branches of BrTaps.
 template <int J, bool RAT>
 __global__ void __launch_bounds__(SB_FIR_THREADS) k_channelize(const uint32_t* __restrict__ x, uint64_t n_in, const uint32_t* __restrict__ nco, ChChannels ch,
-                                                              uint32_t chan_per_group, uint32_t D, typename std::conditional<RAT, RtTaps, ChTaps>::type taps,
+                                                              uint32_t chan_per_group, uint32_t D, typename std::conditional<RAT, BrTaps, ChTaps>::type taps,
                                                               uint32_t* __restrict__ y, uint64_t stride, uint64_t n_out) {
     extern __shared__ __align__(16) uint32_t smem[];
     uint32_t* s_x = smem; uint32_t* s_v = smem + SB_CH_WIN; uint32_t* s_nco = smem + 2 * SB_CH_WIN;
@@ -226,6 +226,8 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_channelize(const uint32_t* _
             const uint32_t nq = qb > qa ? (uint32_t)(qb - qa) : 0u;
             const uint32_t rs = (c % U + U - (D * s) % U) % U, L = rs < taps.n ? (taps.n - 1 - rs) / U + 1 : 0u;
             const int es = ((int)(D * s + rs) - (int)c) / (int)U;      // exact: D s + r_s - c is a multiple of U
+            int tb = 0;                                                 // branch r_s in taps.t (int: the unrolled tap loads take immediate offsets)
+            if constexpr (RAT) tb = (int)(rs * taps.L);
             const uint32_t i0 = (uint32_t)((int64_t)(D * qa) - (int64_t)t0 + (int64_t)halo + es);   // window word of output qa, tap 0
             uint32_t off[J];                                            // word of output j within its phase (0 for outputs past the tile: read, never stored)
 #pragma unroll
@@ -235,8 +237,7 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_channelize(const uint32_t* _
             for (int j = 0; j < J; j++) accr[j] = acci[j] = 1u << 14;
             uint32_t r = i0 % D, base = r * P + i0 / D;                 // phase and word of tap 0 for output qa
             for (uint32_t l = 0; l < L; l++) {                          // one tap at a time over the J outputs: the tap is a uniform constant
-                int t;
-                if constexpr (RAT) t = taps.t[rs][l]; else t = taps.t[l];
+                const int t = taps.t[tb + (int)l];
                 if (t != 0) {                                           // half-band filters: every other tap
 #pragma unroll
                     for (int j = 0; j < J; j++) {
@@ -293,13 +294,8 @@ __device__ __forceinline__ cs16 nco_rotate_up(cs16 u, uint32_t cs) {
 // warps take the phases g, g + G, ... (G = 8 / W) side by side.  The host picks the largest TQ whose shared memory fits SB_CBR_SMEM
 // (four CTAs per multiprocessor), else TQ = 32, which fits SB_CBR_SMEM_MAX (three) at every limit.  With accumulate the output tile is
 // first loaded from HBM with 16-byte loads and each sum adds onto it before its single saturation.
-#define SB_CBR_MAXTAPS 4095                // sb200_combine_rational's limits: U <= 64, D <= 16, ntaps <= 4095
-#define SB_CBR_MAXINTERP 64
 #define SB_CBR_SMEM 57344                  // preferred budget: four CTAs per multiprocessor (4 x (56 + 1) KB of 228 KB)
 #define SB_CBR_SMEM_MAX 75776              // the budget of TQ = 32: three CTAs per multiprocessor (3 x (74 + 1) KB)
-// The taps of sb200_combine_rational by branch: taps[r + U l] at t[r * L + l], L = ceil(ntaps / U), U L <= ntaps + U - 1.  8.3 KB of
-// kernel parameters (allowed up to 32 KB since CUDA 12.1 on sm_70 and later), read like RtTaps: one uniform constant-bank load per tap.
-struct CbrTaps { int16_t t[SB_CBR_MAXTAPS + SB_CBR_MAXINTERP + 1]; uint32_t n, u, L; };
 // Dynamic shared memory of k_combine<J, true> for tq outputs per phase: K windows of D tq + 2 halo words, the U tq output tile, the NCO
 // table and the mbarrier.
 __host__ __device__ constexpr uint32_t combine_smem_r(uint32_t K, uint32_t U, uint32_t D, uint32_t ntaps, uint32_t tq) {
@@ -310,10 +306,10 @@ static_assert(combine_smem_r(SB_CH_MAXCH, SB_CBR_MAXINTERP, SB_CH_MAXDECIM, 255 
 
 // grid (tiles, 1) or, RAT, (gx, gy) with tile = x + gx y; SB_FIR_THREADS threads; combine_smem(K, U, ntaps, 256 J) or, RAT,
 // combine_smem_r(K, U, D, ntaps, 32 W J) bytes of dynamic shared memory.  Row k starts at x + k * stride; outputs y[0 .. n_out).
-// RAT = false: D = W / 8 = 1, ChTaps, n_out = U n_in, no accumulate (sb200_combine); RAT = true: CbrTaps (sb200_combine_rational).
+// RAT = false: D = W / 8 = 1, ChTaps, n_out = U n_in, no accumulate (sb200_combine); RAT = true: BrTaps (sb200_combine_rational).
 template <int J, bool RAT>
 __global__ void __launch_bounds__(SB_FIR_THREADS) k_combine(const uint32_t* __restrict__ x, uint64_t stride, uint64_t n_in, const uint32_t* __restrict__ nco,
-                                                           CbChannels ch, uint32_t U, uint32_t Dr, uint32_t Wr, typename std::conditional<RAT, CbrTaps, ChTaps>::type taps,
+                                                           CbChannels ch, uint32_t U, uint32_t Dr, uint32_t Wr, typename std::conditional<RAT, BrTaps, ChTaps>::type taps,
                                                            uint32_t* __restrict__ y, uint64_t n_out, uint32_t accumulate) {
     const uint32_t D = RAT ? Dr : 1u, W = RAT ? Wr : SB_FIR_THREADS / 32u;
     const uint32_t TQ = 32u * W * J, G = (SB_FIR_THREADS / 32u) / W;    // outputs per phase of a tile; groups of W warps
@@ -328,28 +324,8 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_combine(const uint32_t* __re
     bool rotate = false;                                                // the table is only brought in when a channel needs it
     for (uint32_t k = 0; k < K; k++) rotate |= ch.inc[k] != 0u || (ch.phase0[k] >> 20) != 0u;
 
-    // Staging: stage_window's steps for K rows on one barrier (window k holds samples [t0 - halo, t0 + D TQ + halo) of row k, zero outside
-    // [0, n_in)).  halo, D TQ and stride are multiples of 4, so every copy's source and destination are 16-byte aligned.
-    const uint64_t w0 = t0 >= halo ? t0 - halo : 0ull;
-    const uint64_t w1e = t0 + D * TQ + halo < n_in ? t0 + D * TQ + halo : n_in, w1 = (RAT && w1e < w0) ? w0 : w1e;   // RAT: tiles past the rows
-    const uint32_t dst0 = (uint32_t)(w0 - (t0 - halo)), nw = (uint32_t)(w1 - w0), bulk = nw & ~3u;
-    for (uint32_t i = tid; i < K * win; i += SB_FIR_THREADS) { const uint32_t q = i % win; if (q < dst0 || q >= dst0 + bulk) smem[i] = 0; }
-    if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(s_bar)));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
-    __syncthreads();
-    const uint32_t bytes = K * bulk * 4u + (rotate ? SB_CH_NCO * 4u : 0u);
-    const uint32_t mb = (uint32_t)__cvta_generic_to_shared(s_bar);
-    if (tid == 0 && bytes) {
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes) : "memory");
-        if (bulk) for (uint32_t k = 0; k < K; k++)
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         :: "r"((uint32_t)__cvta_generic_to_shared(smem + k * win + dst0)), "l"(x + k * stride + w0), "r"(bulk * 4u), "r"(mb) : "memory");
-        if (rotate) asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                                 :: "r"((uint32_t)__cvta_generic_to_shared(s_nco)), "l"(nco), "r"(SB_CH_NCO * 4u), "r"(mb) : "memory");
-    }
-    if (tid < K * (nw & 3u)) { const uint32_t k = tid / (nw & 3u), q = tid % (nw & 3u); smem[k * win + dst0 + bulk + q] = __ldg(x + k * stride + w0 + bulk + q); }
+    // window k holds samples [t0 - halo, t0 + D TQ + halo) of row k; halo, D TQ and stride are multiples of 4
+    const uint32_t bytes = stage_window_issue(x, stride, K, n_in, (int64_t)t0 - (int64_t)halo, win, smem, win, rotate ? nco : nullptr, SB_CH_NCO, s_nco, s_bar);
     // outputs n0 .. n0 + nt of y[0 .. n_out); with accumulate they are loaded into the output tile first (16-byte loads: n0 is a multiple of 4)
     if (RAT && accumulate) {
         const uint64_t nt = n_out - n0 < (uint64_t)U * TQ ? n_out - n0 : (uint64_t)U * TQ;
@@ -358,11 +334,7 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_combine(const uint32_t* __re
         for (uint32_t q = tid; q < n4; q += SB_FIR_THREADS) s4[q] = y4[q];
         if (tid < ((uint32_t)nt & 3u)) s_y[4 * n4 + tid] = y[n0 + 4 * n4 + tid];
     }
-    if (bytes) {
-        uint32_t ok = 0;
-        while (!ok) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], 0; selp.u32 %0, 1, 0, p; }" : "=r"(ok) : "r"(mb) : "memory");
-    }
-    __syncthreads();
+    stage_window_wait(bytes, smem_addr(s_bar));
 
     // RAT = false: one group, grp = 0 and lt = tid at compile time, so the phase and its taps stay uniform to the compiler (DESIGN.md §8)
     const uint32_t grp = RAT ? (tid >> 5) / W : 0u, lt = RAT ? tid - grp * W * 32u : tid;
@@ -379,8 +351,9 @@ __global__ void __launch_bounds__(SB_FIR_THREADS) k_combine(const uint32_t* __re
             for (int j = 0; j < J; j++) accr[j] = acci[j] = 1u << 14;
             if constexpr (RAT) {
                 const uint32_t L = rs < taps.n ? (taps.n - 1 - rs) / U + 1 : 0u;
-                for (uint32_t l = 0, jb = rs * taps.L; l < L; l++, jb++) {   // one tap at a time over the J outputs: the tap is a uniform constant
-                    const int t = taps.t[jb];
+                const int tb = (int)(rs * taps.L);                      // branch r_s in taps.t (int: the unrolled tap loads take immediate offsets)
+                for (uint32_t l = 0; l < L; l++) {                      // one tap at a time over the J outputs: the tap is a uniform constant
+                    const int t = taps.t[tb + (int)l];
                     if (t != 0) {
 #pragma unroll
                         for (int j = 0; j < J; j++) {

@@ -18,6 +18,7 @@
 #pragma once
 #include "tables.cuh"
 #include "viterbi_k7_common.cuh"
+#include "bulk_copy.cuh"
 
 namespace sb {
 
@@ -293,11 +294,7 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
     const unsigned FULL = 0xFFFFFFFFu;
     const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
     const int qt = lane >> 3, ql = lane & 7;
-    if (STAGE == 2 && ql == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][qt][0])));
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"((uint32_t)__cvta_generic_to_shared(&s_mbar[wib][qt][1])));
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-    }
+    if (STAGE == 2 && ql == 0) mbar_init(smem_addr(&s_mbar[wib][qt][0]), 2);
     for (int i = threadIdx.x; i < 256; i += blockDim.x)
         s_demap[i] = (uint32_t)__ldg(T.demap + i) | ((uint32_t)__ldg(T.demap + 256 + i) << 8) | ((uint32_t)__ldg(T.demap + 512 + i) << 16) | ((uint32_t)__ldg(T.demap + 768 + i) << 24);
     for (int i = threadIdx.x; i < 128; i += blockDim.x) s_pilot[i] = __ldg(T.pilot_neg + i);
@@ -557,15 +554,14 @@ __global__ void __launch_bounds__(32 * SB_FRONT_WARPS, SB_FRONT_MINB) k_front11a
             const uint32_t* src = x + (first20 << sh);
             const uintptr_t a0 = (uintptr_t)src & ~(uintptr_t)15, a1 = ((uintptr_t)(src + (n20 << sh)) + 15) & ~(uintptr_t)15;
             const uint32_t bytes = (uint32_t)(a1 - a0);
-            const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][qt][b]), dst = (uint32_t)__cvta_generic_to_shared(st_buf + b * SB_FRONT_STAGE_WORDS);
-            asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" :: "r"(mb), "r"(bytes) : "memory");
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];" :: "r"(dst), "l"(a0), "r"(bytes), "r"(mb) : "memory");
+            const uint32_t mb = smem_addr(&s_mbar[wib][qt][b]);
+            mbar_expect_tx(mb, bytes);
+            bulk_copy_g2s(smem_addr(st_buf + b * SB_FRONT_STAGE_WORDS), (const void*)a0, bytes, mb);
         }
     };
     auto stage_wait = [&](int b) {
         if (!((st_busy >> b) & 1u)) return;
-        const uint32_t mb = (uint32_t)__cvta_generic_to_shared(&s_mbar[wib][qt][b]); uint32_t ok = 0;
-        while (!ok) asm volatile("{ .reg .pred p; mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2; selp.u32 %0, 1, 0, p; }" : "=r"(ok) : "r"(mb), "r"(st_par[b]) : "memory");
+        mbar_wait(smem_addr(&s_mbar[wib][qt][b]), st_par[b]);
         st_par[b] ^= 1u; st_busy &= ~(1u << b);
     };
     auto stage_load8 = [&](int b, uint32_t first, uint32_t (&v)[8]) {    // (x >> 1) * FreqCoeffs from buffer b; the buffer starts at the 16-byte line of its first sample

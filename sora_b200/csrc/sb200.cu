@@ -902,11 +902,11 @@ extern "C" int sb200_rx11a_stream(sb200_handle* h, const int16_t* iq, uint64_t n
 
 // One launch of k_channelize (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.  Outputs per thread from D;
 // channels split into groups (the input then read once per group) only as far as needed for four CTAs per multiprocessor.  ChTaps
-// launches the U = 1 specialisation, RtTaps the rational one.
+// launches the U = 1 specialisation, BrTaps the rational one.
 template <int J, class Taps>
 static int channelize_launch_j(sb200_handle* h, cudaStream_t st, dim3 grid, const uint32_t* d_in, uint64_t n_in, const ChChannels& ch, uint32_t cpg,
                                uint32_t D, const Taps& T, uint32_t* d_out, uint64_t stride, uint64_t n_out) {
-    constexpr bool RAT = std::is_same<Taps, RtTaps>::value;
+    constexpr bool RAT = std::is_same<Taps, BrTaps>::value;
     const uint64_t bit = 1ull << (J + (RAT ? 32 : 0));
     if (!(h->ch_smem_set & bit)) {
         CK(cudaFuncSetAttribute(k_channelize<J, RAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_CH_SMEM));
@@ -958,12 +958,15 @@ extern "C" int sb200_fir_decimate2(sb200_handle* h, const int16_t* iq, uint64_t 
     return finish_call(h, st, ret, 0, 1);
 }
 
-// The NCO table of sb200_channelize and sb200_combine (fir_kernels.cuh), uploaded on first use:
-// (C, S) = (rint(2^14 cos 2 pi i / 4096), rint(2^14 sin 2 pi i / 4096)), packed like cs16.
+// The Q14 NCO table of fir_kernels.cuh and sim_kernels.cuh, SB_CH_NCO words: (C, S) = (rint(2^14 cos 2 pi i / 4096), rint(2^14 sin 2 pi i / 4096)), packed like cs16.
+static void fill_nco(uint32_t* t) {
+    for (int i = 0; i < SB_CH_NCO; i++) { const double a = 2.0 * M_PI * i / 4096.0; t[i] = pack(mk((int)nearbyint(16384.0 * cos(a)), (int)nearbyint(16384.0 * sin(a)))); }
+}
+// The NCO table of sb200_channelize and sb200_combine, uploaded on first use.
 static int upload_nco(sb200_handle* h) {
     if (h->nco.p) return SB200_OK;
     std::vector<uint32_t> t(SB_CH_NCO);
-    for (int i = 0; i < SB_CH_NCO; i++) { const double a = 2.0 * M_PI * i / 4096.0; t[i] = pack(mk((int)nearbyint(16384.0 * cos(a)), (int)nearbyint(16384.0 * sin(a)))); }
+    fill_nco(t.data());
     cudaError_t e = h->nco.need(SB_CH_NCO * 4);
     if (e == cudaSuccess) e = cudaMemcpy(h->nco.p, t.data(), SB_CH_NCO * 4, cudaMemcpyHostToDevice);
     if (e == cudaSuccess) e = cudaDeviceSynchronize();   // landed before a kernel on a non-blocking stream reads it (TableArena::upload)
@@ -971,28 +974,48 @@ static int upload_nco(sb200_handle* h) {
     return SB200_OK;
 }
 
+// Checks of the channelizer's and the combiner's calls, which pass the messages in their own parameter names.  The rate pair of the
+// rational-rate calls: the smaller factor 1 .. 16, the larger from it to 64, coprime.
+static_assert(SB_CH_MAXINTERP == SB_CH_MAXDECIM && SB_CH_MAXRDECIM == SB_CBR_MAXINTERP, "the rational channelizer and combiner share their rate limits");
+static int check_rate_pair(sb200_handle* h, uint32_t lo, uint32_t hi, const char* lo_msg, const char* hi_msg) {
+    if (lo < 1 || lo > SB_CH_MAXINTERP) return h->fail(SB200_E_INVALID, lo_msg);
+    if (hi < lo || hi > SB_CH_MAXRDECIM) return h->fail(SB200_E_INVALID, hi_msg);
+    uint32_t a = lo, b = hi; while (b) { const uint32_t t = a % b; a = b; b = t; }
+    return a == 1 ? SB200_OK : h->fail(SB200_E_INVALID, "interp and decim must be coprime");
+}
+// The taps: ntaps odd, at most max_ntaps and at most 255 per branch (taps r, r + interp, ...); the |tap| sum of each branch at most 65535,
+// so that the int32 accumulator of an output, which meets one branch, cannot wrap.
+static int check_taps(sb200_handle* h, const int16_t* taps, uint32_t ntaps, uint32_t interp, uint32_t max_ntaps, const char* len_msg, const char* sum_msg) {
+    if ((ntaps & 1u) == 0 || ntaps > max_ntaps || (ntaps + interp - 1) / interp > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, len_msg);
+    for (uint32_t r = 0; r < interp; r++) {
+        uint32_t asum = 0; for (uint32_t i = r; i < ntaps; i += interp) asum += (uint32_t)abs((int)taps[i]);
+        if (asum > 65535u) return h->fail(SB200_E_INVALID, sum_msg);
+    }
+    return SB200_OK;
+}
+// The taps by branch for the rational-rate kernels: taps[r + U l] at t[r L + l].
+static BrTaps branch_taps(const int16_t* taps, uint32_t ntaps, uint32_t U) {
+    static_assert(sizeof(BrTaps) + sizeof(CbChannels) + 64 <= 32764 && sizeof(CbChannels) >= sizeof(ChChannels), "kernel parameters of k_channelize<J, true> and k_combine<J, true>");
+    BrTaps T; memset(&T, 0, sizeof T); T.n = ntaps; T.u = U; T.L = (ntaps + U - 1) / U;
+    for (uint32_t i = 0; i < ntaps; i++) T.t[(i % U) * T.L + i / U] = taps[i];
+    return T;
+}
+
 // Wideband channelizer (fir_kernels.cuh): every channel shifted by its NCO, filtered and decimated by `decim`; channel c in row c of `out`.
-// sb200_channelize is the interp = 1 case of sb200_channelize_rational; both share the checks, staging and launch here.
+// sb200_channelize is the interp = 1 case of sb200_channelize_rational with its own limits; both share the checks, staging and launch
+// here (rational = false: sb200_channelize).
 static int channelize_call(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t interp,
-                           uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream, uint32_t max_decim) {
+                           uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream, bool rational) {
     if (!h) return SB200_E_INVALID;
     if (!iq || !channels || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
     if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
-    if (max_decim == SB_CH_MAXDECIM) {
-        if (decim < 1 || decim > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "decim must be 1 .. 16");
-        if ((ntaps & 1u) == 0 || ntaps > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 255");
-    } else {
-        if (interp < 1 || interp > SB_CH_MAXINTERP) return h->fail(SB200_E_INVALID, "interp must be 1 .. 16");
-        if (decim < interp || decim > SB_CH_MAXRDECIM) return h->fail(SB200_E_INVALID, "decim must be interp .. 64");
-        uint32_t a = interp, b = decim; while (b) { const uint32_t t = a % b; a = b; b = t; }
-        if (a != 1) return h->fail(SB200_E_INVALID, "interp and decim must be coprime");
-        if ((ntaps & 1u) == 0 || (ntaps + interp - 1) / interp > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and ceil(ntaps / interp) at most 255");
-    }
-    for (uint32_t r = 0; r < interp; r++) {           // output m meets only the taps k = c - D m (mod interp): one branch per residue
-        uint32_t asum = 0; for (uint32_t i = r; i < ntaps; i += interp) asum += (uint32_t)abs((int)taps[i]);
-        if (asum > 65535u) return h->fail(SB200_E_INVALID, interp == 1 ? "sum of |taps| must be at most 65535 (the int32 accumulator must not wrap)"
-                                                                       : "sum of |taps[k]| over k = r (mod interp) must be at most 65535 for every r (the int32 accumulator must not wrap)");
-    }
+    if (!rational && (decim < 1 || decim > SB_CH_MAXDECIM)) return h->fail(SB200_E_INVALID, "decim must be 1 .. 16");
+    int rc = rational ? check_rate_pair(h, interp, decim, "interp must be 1 .. 16", "decim must be interp .. 64") : SB200_OK;
+    if (rc == SB200_OK) rc = check_taps(h, taps, ntaps, interp, interp * SB_CH_MAXTAPS,   // no limit on ntaps beyond the branch length
+                                        rational ? "ntaps must be odd and ceil(ntaps / interp) at most 255" : "ntaps must be odd and at most 255",
+                                        interp == 1 ? "sum of |taps| must be at most 65535 (the int32 accumulator must not wrap)"
+                                                    : "sum of |taps[k]| over k = r (mod interp) must be at most 65535 for every r (the int32 accumulator must not wrap)");
+    if (rc != SB200_OK) return rc;
     if (n_in > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples must be at most 2^40");
     const uint64_t n_out = (interp * n_in + decim - 1) / decim;
     if (out_stride < n_out || (out_stride & 3u) || out_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "out_stride must be at least ceil(interp n_in / decim), at most 2^40 and a multiple of 4");
@@ -1012,35 +1035,30 @@ static int channelize_call(sb200_handle* h, const int16_t* iq, uint64_t n_in, co
     }
     ChChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
     for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; }
-    int rc;
     if (interp == 1) {
         ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
         rc = channelize_launch(h, st, d_in, n_in, ch, decim, T, d_out, d_stride, n_out);
-    } else {                                           // by branch: taps[r + U l] at t[r][l]
-        static_assert(sizeof(RtTaps) + sizeof(ChChannels) + 64 <= 32764, "kernel parameters of k_channelize<J, true>");
-        RtTaps T; memset(&T, 0, sizeof T); T.n = ntaps; T.u = interp; for (uint32_t i = 0; i < ntaps; i++) T.t[i % interp][i / interp] = taps[i];
-        rc = channelize_launch(h, st, d_in, n_in, ch, decim, T, d_out, d_stride, n_out);
-    }
+    } else rc = channelize_launch(h, st, d_in, n_in, ch, decim, branch_taps(taps, ntaps, interp), d_out, d_stride, n_out);
     return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
 }
 extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t decim,
                                 const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
-    return channelize_call(h, iq, n_in, channels, nchannels, 1, decim, taps, ntaps, out, out_stride, cuda_stream, SB_CH_MAXDECIM);
+    return channelize_call(h, iq, n_in, channels, nchannels, 1, decim, taps, ntaps, out, out_stride, cuda_stream, false);
 }
 // Rational-rate channelizer: every channel shifted by its NCO, zero-stuffed by `interp`, filtered and decimated by `decim`.
 extern "C" int sb200_channelize_rational(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels,
                                          uint32_t interp, uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
-    return channelize_call(h, iq, n_in, channels, nchannels, interp, decim, taps, ntaps, out, out_stride, cuda_stream, SB_CH_MAXRDECIM);
+    return channelize_call(h, iq, n_in, channels, nchannels, interp, decim, taps, ntaps, out, out_stride, cuda_stream, true);
 }
 
 // One launch of k_combine<J, RAT> (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.  ChTaps launches the
-// sb200_combine specialisation (D = 1, eight warps per phase), CbrTaps the rational one with W warps per phase; tiles of 32 W J outputs per
+// sb200_combine specialisation (D = 1, eight warps per phase), BrTaps the rational one with W warps per phase; tiles of 32 W J outputs per
 // phase, on a grid of (tiles, 1) CTAs or, RAT, (gx, gy) with tile = x + gx y: n_out <= 2^40 and U TQ >= 32 give at most 2^35 tiles,
 // so gy = ceil(tiles / (2^31 - 1)) <= 16 and gx = ceil(tiles / gy) < 2^31 stay within the grid limits.
 template <int J, class Taps>
 static int combine_launch_j(sb200_handle* h, cudaStream_t st, const uint32_t* d_in, uint64_t stride, uint64_t n_in, const CbChannels& ch, uint32_t U,
                             uint32_t D, uint32_t W, const Taps& T, uint32_t* d_out, uint64_t n_out, uint32_t accumulate) {
-    constexpr bool RAT = std::is_same<Taps, CbrTaps>::value;
+    constexpr bool RAT = std::is_same<Taps, BrTaps>::value;
     const uint32_t bit = 1u << (J + (RAT ? 16 : 0));
     if (!(h->cb_smem_set & bit)) {
         CK(cudaFuncSetAttribute(k_combine<J, RAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, RAT ? SB_CBR_SMEM_MAX : SB_CB_SMEM));
@@ -1063,22 +1081,13 @@ static int combine_call(sb200_handle* h, const int16_t* rows, uint64_t row_strid
     if (!h) return SB200_E_INVALID;
     if (!rows || !channels || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
     if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
-    if (!rational) {
-        if (interp < 1 || interp > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "interp must be 1 .. 16");
-        if ((ntaps & 1u) == 0 || ntaps > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 255");
-    } else {
-        if (decim < 1 || decim > SB_CH_MAXDECIM) return h->fail(SB200_E_INVALID, "decim must be 1 .. 16");
-        if (interp < decim || interp > SB_CBR_MAXINTERP) return h->fail(SB200_E_INVALID, "interp must be decim .. 64");
-        uint32_t a = interp, b = decim; while (b) { const uint32_t t = a % b; a = b; b = t; }
-        if (a != 1) return h->fail(SB200_E_INVALID, "interp and decim must be coprime");
-        if ((ntaps & 1u) == 0 || ntaps > SB_CBR_MAXTAPS || (ntaps + interp - 1) / interp > SB_CH_MAXTAPS)
-            return h->fail(SB200_E_INVALID, "ntaps must be odd, at most 4095 and ceil(ntaps / interp) at most 255");
-        if (accumulate > 1u) return h->fail(SB200_E_INVALID, "accumulate must be 0 or 1");
-    }
-    for (uint32_t r = 0; r < interp; r++) {           // output n meets only the taps j = c - D n (mod interp): one branch per residue
-        uint32_t asum = 0; for (uint32_t i = r; i < ntaps; i += interp) asum += (uint32_t)abs((int)taps[i]);
-        if (asum > 65535u) return h->fail(SB200_E_INVALID, "sum of |taps[j]| over j = r (mod interp) must be at most 65535 for every r (the int32 accumulator must not wrap)");
-    }
+    if (!rational && (interp < 1 || interp > SB_CH_MAXDECIM)) return h->fail(SB200_E_INVALID, "interp must be 1 .. 16");
+    int rc = rational ? check_rate_pair(h, decim, interp, "decim must be 1 .. 16", "interp must be decim .. 64") : SB200_OK;
+    if (rc == SB200_OK) rc = check_taps(h, taps, ntaps, interp, rational ? SB_CBR_MAXTAPS : SB_CH_MAXTAPS,
+                                        rational ? "ntaps must be odd, at most 4095 and ceil(ntaps / interp) at most 255" : "ntaps must be odd and at most 255",
+                                        "sum of |taps[j]| over j = r (mod interp) must be at most 65535 for every r (the int32 accumulator must not wrap)");
+    if (rc != SB200_OK) return rc;
+    if (accumulate > 1u) return h->fail(SB200_E_INVALID, "accumulate must be 0 or 1");
     for (uint32_t i = 0; i < nchannels; i++)
         if (channels[i].gain > 65535u) return h->fail(SB200_E_INVALID, "gain must be at most 65535");
     if (row_stride < n_in || (row_stride & 3u) || row_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "row_stride must be at least n_in, at most 2^40 and a multiple of 4");
@@ -1107,16 +1116,13 @@ static int combine_call(sb200_handle* h, const int16_t* rows, uint64_t row_strid
     }
     CbChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
     for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; ch.gain[i] = channels[i].gain; }
-    int rc;
     if (!rational) {                                   // tiles of 1024, 512 or 256 input samples: the largest whose shared memory fits SB_CB_SMEM (256 always does)
         ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
         if (combine_smem(nchannels, interp, ntaps, 4 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
         else if (combine_smem(nchannels, interp, ntaps, 2 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
         else rc = combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
-    } else {                                           // by branch: taps[r + U l] at t[r L + l]
-        static_assert(sizeof(CbrTaps) + sizeof(CbChannels) + 64 <= 32764, "kernel parameters of k_combine<J, true>");
-        CbrTaps T; memset(&T, 0, sizeof T); T.n = ntaps; T.u = interp; T.L = (ntaps + interp - 1) / interp;
-        for (uint32_t i = 0; i < ntaps; i++) T.t[(i % interp) * T.L + i / interp] = taps[i];
+    } else {
+        const BrTaps T = branch_taps(taps, ntaps, interp);
         // 32 W J outputs per phase: the largest of 1024 .. 32 whose shared memory fits SB_CBR_SMEM, else 32 (within SB_CBR_SMEM_MAX)
         static const uint32_t kj[6] = {4, 2, 1, 1, 1, 1}, kw[6] = {8, 8, 8, 4, 2, 1};
         int p = 0;
@@ -1139,7 +1145,7 @@ extern "C" int sb200_combine_rational(sb200_handle* h, const int16_t* rows, uint
     return combine_call(h, rows, row_stride, n_in, channels, nchannels, interp, decim, taps, ntaps, out, n_out, accumulate, cuda_stream, true);
 }
 
-// The table of sb200_channel_sim (sim_kernels.cuh), uploaded on first use: the NCO of upload_nco, then H (256 rows of 8 Q14 taps, packed in
+// The table of sb200_channel_sim (sim_kernels.cuh), uploaded on first use: the NCO of fill_nco, then H (256 rows of 8 Q14 taps, packed in
 // pairs like cs16) and LNT, from the closed forms of include/sora_b200.h.  I0 is its power series (tests/sim_model.py sums the same one).
 static double sim_i0(double x) {
     double s = 1.0, t = 1.0; const double q = x * x / 4.0;
@@ -1149,7 +1155,7 @@ static double sim_i0(double x) {
 static int upload_simtab(sb200_handle* h) {
     if (h->simtab.p) return SB200_OK;
     std::vector<uint32_t> t(SB_SIM_TAB);
-    for (int i = 0; i < SB_CH_NCO; i++) { const double a = 2.0 * M_PI * i / 4096.0; t[i] = pack(mk((int)nearbyint(16384.0 * cos(a)), (int)nearbyint(16384.0 * sin(a)))); }
+    fill_nco(t.data());
     const double i05 = sim_i0(5.0);
     for (int p = 0; p < 256; p++) {
         int hv[8];
