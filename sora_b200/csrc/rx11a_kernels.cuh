@@ -19,6 +19,7 @@
 #include "tables.cuh"
 #include "viterbi_k7_common.cuh"
 #include "bulk_copy.cuh"
+#include "ofdm_bins.cuh"
 
 namespace sb {
 
@@ -68,7 +69,7 @@ __global__ void __launch_bounds__(128) k_sync11a(const uint32_t* __restrict__ iq
                                                   const uint32_t* __restrict__ len, uint32_t nframes, uint32_t cca_thr,
                                                   DevTables T, FrameInfo* __restrict__ info, const int2* __restrict__ dc_init, uint32_t sh, uint32_t lsh) {
     // sh = 1: `iq` is the 40 Msps capture and TDownSample2 (samples.hpp:27-49) is the stride-2 gather below; sh = 0: the caller's samples were
-    // decimated on the way in (host-side gather of the even samples, sb200.cu), off[] then addresses that packed copy; len[] stays in 40 Msps samples
+    // decimated on the way in (host-side gather of the even samples, rx11a.cu), off[] then addresses that packed copy; len[] stays in 40 Msps samples
     uint32_t f = blockIdx.x * blockDim.x + threadIdx.x;
     if (f >= nframes) return;
     const uint32_t* x = iq + off[f];
@@ -182,7 +183,6 @@ __device__ __forceinline__ void warp_fft64(uint32_t* x, const DevTables& T, int 
     }
     __syncwarp();
 }
-__device__ __forceinline__ int bitrev6(int i) { return (int)(__brev((unsigned)i) >> 26); }
 
 // SIGNAL-field Viterbi, one warp: lane l owns the butterfly (l, l+32) -> (2l, 2l+1).  uint8 metrics with the
 // reference's wrap/mark/min/normalise rules (viterbicore.h:36-261).  `soft` = 48 deinterleaved values in shared; `dec` = 48 words of
@@ -235,14 +235,6 @@ struct FrontTaps {            // optional stage taps (device pointers, nullptr =
     uint32_t hdr_only;        // stop after SIGNAL: status = E_SUCCESS (all symbols of the frame lie in the slot) / E_NO_FRAME (they do not) / E_PLCP_HEADER_FAIL
 };
 
-__device__ __forceinline__ int data_index(int bin) {   // demapper11a.hpp:22-36 subcarrier order; -1 for non-data bins
-    if (bin >= 38) { if (bin == 43 || bin == 57) return -1; return bin - 38 - (bin > 43) - (bin > 57); }
-    if (bin >= 1 && bin <= 26) { if (bin == 7 || bin == 21) return -1; return 24 + bin - 1 - (bin > 7) - (bin > 21); }
-    return -1;
-}
-__device__ __forceinline__ int data_bin(int d) {       // inverse of data_index, d = 0..47
-    return d < 24 ? 38 + d + (d >= 5) + (d >= 18) : d - 23 + (d >= 30) + (d >= 43);
-}
 // Post-FFT role of lane ql of a quarter-warp: eight bins.  Bins 0-5 are three data-subcarrier pairs (d, d + 3), d = 6 (q / 3) + q % 3
 // for q = ql + 8 p, p = 0..2 (bins 2 p, 2 p + 1), in demapper order: at 64-QAM the 802.11a de-interleaver puts coded bit i of d at an
 // even position and bit (2 0 1 5 3 4)[i] of d + 3 right after it, so a pair's soft bits leave as six 16-bit stores.  Bin 6 is a pilot in

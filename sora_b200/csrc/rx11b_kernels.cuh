@@ -15,7 +15,8 @@
 //   TDesc741                            kernel/bb/Brick11/src/scramble.hpp:95-162
 //   TBB11bPlcpParser, TBB11bFrameSink   kernel/bb/Brick11/src/PHY_11b.hpp:504-747
 #pragma once
-#include "rx11a_kernels.cuh"
+#include "tables.cuh"
+#include "viterbi_k7_common.cuh"
 
 namespace sb {
 

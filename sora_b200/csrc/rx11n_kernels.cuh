@@ -19,23 +19,12 @@
 //   (fb11ndemod_config.hpp:189); the brick's 312-value bursts and zero padding at Flush never reach a decision that is
 //   delivered, because the final traceback fires inside the last real symbol.
 #pragma once
-#include "rx11a_kernels.cuh"
+#include "tables.cuh"
+#include "viterbi_k7_common.cuh"
+#include "ofdm_bins.cuh"
 
 namespace sb {
 
-struct DevTables11n {
-    const uint32_t* sincos;     // [65536] packed (cos, sin)            dsp_math.h:214-231
-    const int16_t*  atan_lut;   // [4097]                               dsp_math.h:233-247
-    const uint8_t*  demap;      // [256]  BPSK == QPSK table (data)     dsp_demap.h:97-137
-    const uint8_t*  crc8;       // [256]                                core/inc/CRC8.h:16-26
-    const uint8_t*  pos;        // [2 qpsk][2 stream][104] position, in the stream-parsed symbol, of demap output j of stream s
-    const uint8_t*  lltf_pos;   // [64] 1 where the L-LTF carrier is +1  channel_11n.hpp:7-32
-    const uint8_t*  htltf_pos;  // [64] 1 where the HT-LTF carrier is +1 channel_11n.hpp:300-325
-    const uint16_t* pos16;      // [2: 16-QAM, 64-QAM][2 stream][312] the same position map for the 16-QAM / 64-QAM branches (stream parser blocks of 2 / 3)
-    const uint8_t*  demap16;    // [2][256] dsp_demap.h lookup_table_16qam1 / 16qam2 (data)
-    const uint8_t*  demap64;    // [3][288] dsp_demap.h lookup_table_64qam1..3, entry 144 = value 0 (data)
-    uint32_t mcs_limit;         // first MCS index the HT-SIG parser refuses: 11 as the reference ships it (PHY_11n.hpp:497), 15 with the QAM branches enabled
-};
 // FrameInfo::rate_kbps of an event whose HT-SIG was never parsed.  CF_HTRxVector has no Reset() (ieee80211facade.hpp:269-272), so the
 // reference then still holds the previous event's ht_frame_mcs: the stream driver substitutes it, a batch slot (a fresh context) reports 0.
 constexpr uint32_t MCS11N_UNPARSED = 0xFFFFFFFFu;

@@ -13,6 +13,7 @@
 //      and four shuffles hand every lane its words; every lane is active there (no exits before the last store);
 //   4. coalesced 4-byte stores of row r.
 #pragma once
+#include "../../include/sora_b200.h"      // sb200_link
 #include "fir_kernels.cuh"
 
 namespace sb {

@@ -33,6 +33,34 @@ struct DevTables {
     const uint32_t* crc32;       // [256]
 };
 
+struct DevTablesTx {             // 802.11a transmit (tx11a_kernels.cuh)
+    const uint32_t* tw128;     // [3][32] packed c16
+    const uint32_t* tw32;      // [3][8]
+    const uint8_t*  scr_seq;   // [127] scrambler output from the all-ones state
+    const uint8_t*  scr_phase; // [128] phase of state s (7 bits, bit 0 = oldest) in that sequence; 255 for the zero state
+    uint32_t*       preamble;  // [640] packed c16 (before the 16 -> 8 bit pack), filled by k_tx11a_preamble
+};
+
+struct DevTablesTx11n {          // 802.11n transmit (tx11n_kernels.cuh)
+    const uint32_t* pre;       // [2][1120] packed c16: per stream L-STF + L-LTF (640) then HT-STF + HT-LTF x 2 (480), cyclic shifts applied
+    const uint8_t*  inv;       // [2 (BPSK, QPSK)][2 (stream)][104]: air position -> bit index inside the stream's share of the symbol
+    const uint16_t* inv16;     // [2 (16-QAM, 64-QAM)][2 (stream)][312]: the same for the 16-QAM / 64-QAM interleavers
+};
+
+struct DevTables11n {            // 802.11n receive (rx11n_kernels.cuh)
+    const uint32_t* sincos;     // [65536] packed (cos, sin)            dsp_math.h:214-231
+    const int16_t*  atan_lut;   // [4097]                               dsp_math.h:233-247
+    const uint8_t*  demap;      // [256]  BPSK == QPSK table (data)     dsp_demap.h:97-137
+    const uint8_t*  crc8;       // [256]                                core/inc/CRC8.h:16-26
+    const uint8_t*  pos;        // [2 qpsk][2 stream][104] position, in the stream-parsed symbol, of demap output j of stream s
+    const uint8_t*  lltf_pos;   // [64] 1 where the L-LTF carrier is +1  channel_11n.hpp:7-32
+    const uint8_t*  htltf_pos;  // [64] 1 where the HT-LTF carrier is +1 channel_11n.hpp:300-325
+    const uint16_t* pos16;      // [2: 16-QAM, 64-QAM][2 stream][312] the same position map for the 16-QAM / 64-QAM branches (stream parser blocks of 2 / 3)
+    const uint8_t*  demap16;    // [2][256] dsp_demap.h lookup_table_16qam1 / 16qam2 (data)
+    const uint8_t*  demap64;    // [3][288] dsp_demap.h lookup_table_64qam1..3, entry 144 = value 0 (data)
+    uint32_t mcs_limit;         // first MCS index the HT-SIG parser refuses: 11 as the reference ships it (PHY_11n.hpp:497), 15 with the QAM branches enabled
+};
+
 struct HostTables {
     std::vector<int16_t> sin_lut, cos_lut, atan2_lut;
     uint32_t tw64[3][16], tw16[3][4], sts[16][16];

@@ -12,17 +12,10 @@
 //   `demod11 -m` writes) or COMPLEX16 = COMPLEX8 << 8 (what ConvertModFile2DumpFile_8b feeds the receiver), so that a slot can go
 //   straight into sb200_rx11a_batch.
 #pragma once
-#include "rx11a_kernels.cuh"
+#include "tables.cuh"
+#include "viterbi_k7_common.cuh"
 
 namespace sb {
-
-struct DevTablesTx {
-    const uint32_t* tw128;     // [3][32] packed c16
-    const uint32_t* tw32;      // [3][8]
-    const uint8_t*  scr_seq;   // [127] scrambler output from the all-ones state
-    const uint8_t*  scr_phase; // [128] phase of state s (7 bits, bit 0 = oldest) in that sequence; 255 for the zero state
-    uint32_t*       preamble;  // [640] packed c16 (before the 16 -> 8 bit pack), filled by k_tx11a_preamble
-};
 
 // a * conj(w) >> 15 with the reference's negation of a.re (vector128.h:1215-1231 conj_mul_shift)
 __device__ __forceinline__ cs16 conj_tw(cs16 a, cs16 w) {

@@ -15,11 +15,6 @@
 
 namespace sb {
 
-struct DevTablesTx11n {
-    const uint32_t* pre;       // [2][1120] packed c16: per stream L-STF + L-LTF (640) then HT-STF + HT-LTF x 2 (480), cyclic shifts applied
-    const uint8_t*  inv;       // [2 (BPSK, QPSK)][2 (stream)][104]: air position -> bit index inside the stream's share of the symbol
-    const uint16_t* inv16;     // [2 (16-QAM, 64-QAM)][2 (stream)][312]: the same for the 16-QAM / 64-QAM interleavers
-};
 struct Tx11nJob {
     uint32_t mcs, nbpsc, code_rate, ndbps;   // 8..14; N_BPSCS; CR_12 / CR_23 / CR_34; N_DBPS over both streams
     uint32_t enc_in, parse_in;               // input bursts of the encoder and of the stream parser, bytes (conv_enc.hpp, streamparser.hpp)

@@ -33,8 +33,8 @@
 // VIADDMNMX takes half an FMA slot as well; so the step constants are built mostly on the ALU pipe (vr_step_pk).
 #pragma once
 #ifndef SB_HOST_EMU
-#include "rx11a_kernels.cuh"
-#endif       // host emulation (tests/cpp/re_emu.cpp): the decoder and k_viterbi_re only, without the work lists and the frame sink
+#include "tables.cuh"
+#endif       // host emulation (tests/cpp/re_emu.cpp): the decoder and k_viterbi_re only, without the work lists and the frame sink (DevTables)
 #include "viterbi_k7_common.cuh"
 #include <type_traits>
 

@@ -12,8 +12,8 @@ sources must equal the compiled reference byte for byte:
     every rate and MCS, and the STS input of build_sts.
 Device sources on the host (tests/cpp/fft_emu.cpp): the scalar r4_butterfly / dft4 chain of k_front11n and the packed pk_r4_butterfly /
 pk_dft4 chain of k_front11a, both in the kernels' order, and host_ifft64 with the STS table of tables.cuh.  warp_ifft128
-(tx11a_kernels.cuh) is not run here: its header includes the whole 802.11a receive kernel file, which needs most of the CUDA warp
-intrinsics to compile for the host.  tests/test_gpu_fft_reference.py ties it, and the device FFT, to the compiled reference on the GPU."""
+(tx11a_kernels.cuh) is not run here: it runs across the lanes of a warp, which the host build of this file does not emulate.
+tests/test_gpu_fft_reference.py ties it, and the device FFT, to the compiled reference on the GPU."""
 import ctypes as C, os, shutil, subprocess
 import numpy as np, pytest
 import oracle_py, rail_inputs

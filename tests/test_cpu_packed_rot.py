@@ -61,7 +61,7 @@ def test_turn_pi_every_angle(lib):
     _check(got.view(np.uint32), want.view(np.uint32), "turn_pi")
 
 def _deint_inverse(ncbps, nbpsc):
-    """inv[j] = coded-bit position k of received bit j (gen_deint_map of tables.cuh, inverted as sb200.cu uploads it)."""
+    """inv[j] = coded-bit position k of received bit j (gen_deint_map of tables.cuh, inverted as upload_tables in sb200.cu uploads it)."""
     s = max(nbpsc // 2, 1); inv = [0] * ncbps
     for k in range(ncbps):
         i = (ncbps // 16) * (k % 16) + k // 16
