@@ -11,6 +11,8 @@
   --config tx11b_legacy  the legacy 802.11b transmitter (BB11BPMDPacketGenSignal: encoder + SSE filter, fused) on the device, 11 Mbps / 1500 B
   --config tx11a_legacy  the legacy 802.11a transmitter (BB11ATxFrameMod) on the device, 54 Mbps / 1500 B, at 40 and at 44 Msps
   --config channelize  the wideband channelizer: four 802.11a channels of a 160 Msps capture, 127 taps, D = 4, device-resident
+  --config channelize_bank  the filter-bank channelizer: all eight odd-stacked 20 MHz channels of a 160 Msps capture, 255 taps, D = 4,
+                      timed beside sb200_channelize on the same eight channels and taps
   --config channelize_rational  the rational-rate channelizer: three 802.11b channels of a 160 Msps capture to 44 Msps, 1287 taps, U / D = 11 / 40
   --config combine   the wideband combiner: four 802.11a channel rows at 40 Msps into one 160 Msps capture, 127 taps, U = 4, device-resident
   --config combine_rational  the rational-rate combiner: three 802.11b rows at 44 Msps into one 160 Msps capture, 1761 taps, U / D = 40 / 11
@@ -465,6 +467,41 @@ def bench_channelize(args):
             "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs of every channel" % m})
     c.close()
 
+def bench_channelize_bank(args):
+    """The filter-bank channelizer on the device-resident 160 Msps capture of --config channelize: all eight odd-stacked channels
+    (+-10 / +-30 / +-50 / +-70 MHz), 255 taps, D = 4; and, in the same process on the same capture, sb200_channelize on the same eight
+    channels and taps, the way a user would take the band apart without the bank.  Integer work per input sample: bank
+    2 ntaps / D + 4 M^2 / D (branch sums and the direct M-point DFT), channelizer K (4 + 2 ntaps / D)."""
+    import wideband_inputs as W, bank_model as B
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    n = args.frames * 9824 * 4; M, D = 8, 4
+    taps = W.lowpass(255, 10e6 / 160e6); ch = B.phase_incs(M, 1)
+    n_out = -(-n // D); stride = (n_out + 3) // 4 * 4
+    x = torch.randint(-20000, 20000, (n, 2), dtype=torch.int16, device=dev); y = torch.empty((M, stride, 2), dtype=torch.int16, device=dev)
+    P = 20000; m = (P - len(taps)) // D                                  # outputs that a prefix of P samples determines
+    def bank(): eng.channelize_bank_raw(x.data_ptr(), n, M, D, taps, y.data_ptr(), stride, odd=True, stream=st.cuda_stream)
+    def chan(): eng.channelize_raw(x.data_ptr(), n, ch, D, taps, y.data_ptr(), stride, st.cuda_stream)
+    bank(); torch.cuda.synchronize()
+    assert (B.window(x[:P].cpu().numpy(), M, D, 1, taps, 0, m) == y[:, :m].cpu().numpy()).all(), "filter-bank output differs from the stated arithmetic"
+    chan(); torch.cuda.synchronize()
+    assert (W.channelize(x[:P].cpu().numpy(), ch, D, taps)[:, :m] == y[:, :m].cpu().numpy()).all(), "channelizer output differs from the stated arithmetic"
+    ms_bank = c.timed(bank, args.steps); ms_chan = c.timed(chan, args.steps)
+    name, plim, clk = _card(); sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    imad_peak = sms * 64 * clk * 1e6 if clk else None                    # int32 IMAD: 64 per SM per clock on sm_90
+    hbm = n * (4.0 + 4.0 * M / D)
+    for what, ms, work, note in (("filter-bank channelizer (sb200_channelize_bank)", ms_bank, n * (2.0 * len(taps) / D + 4.0 * M * M / D), "2 ntaps / D + 4 M^2 / D per input sample"),
+                                 ("wideband channelizer (sb200_channelize) on the same channels", ms_chan, n * M * (4.0 + 2.0 * len(taps) / D), "K (4 + 2 ntaps / D) per input sample")):
+        sec = ms * 1e-3; f_int = (work / sec / imad_peak) if imad_peak else None
+        c.emit({"metric": "%s input Msamples/s (COMPLEX16 in, 8 odd-stacked channels, 255 taps, D = 4)" % what, "value": c.world * n / sec / 1e6, "unit": "Msamples/s",
+                "ms_per_step": ms, "n_gpus": c.world, "bank_speedup": ms_chan / ms_bank,
+                "config": {"workload": "160 Msps capture, 8 x 20 MHz channels at +-10/30/50/70 MHz, 255 taps, D = 4, device-resident", "samples_per_step_per_gpu": n},
+                "hbm": {"achieved": hbm / sec / 1e9, "peak": peaks(), "unit": "GB/s", "frac": hbm / sec / 1e9 / peaks(), "note": "4 B read + 4 M / D B written per input sample"},
+                "int_mad": {"achieved": work / sec / 1e9, "peak": imad_peak / 1e9 if imad_peak else None, "unit": "G multiply-adds/s", "frac": f_int,
+                            "note": note + "; peak = SMs x 64 x max SM clock"},
+                "card": name, "power_limit_w": plim, "sm_clock_max_mhz": clk,
+                "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs of every channel" % m})
+    c.close()
+
 def bench_channelize_rational(args):
     """The rational-rate channelizer on a device-resident 160 Msps capture the size of --config channelize's: three 802.11b channels at
     -25 / 0 / +25 MHz brought to 44 Msps (U = 11, D = 40) through 1287 taps (117 per branch).  Work per input sample: K (4 + 2 ntaps / D)
@@ -597,7 +634,7 @@ def bench_sim(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_rational", "combine", "combine_rational", "sim"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_bank", "channelize_rational", "combine", "combine_rational", "sim"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
@@ -605,4 +642,4 @@ if __name__ == "__main__":
                     "a pair other than 40/11 takes a generic low-pass of 45 taps per branch at 0.55 of the row's Nyquist")
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_rational": bench_channelize_rational, "combine": bench_combine, "combine_rational": bench_combine_rational, "sim": bench_sim}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_bank": bench_channelize_bank, "channelize_rational": bench_channelize_rational, "combine": bench_combine, "combine_rational": bench_combine_rational, "sim": bench_sim}[a.config](a)

@@ -185,6 +185,24 @@ int sb200_channelize_rational(sb200_handle* h, const int16_t* iq, uint64_t n_in_
                               uint32_t interp, uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride_samples,
                               void* cuda_stream);
 
+/* Polyphase filter-bank channelizer: every channel of a uniform grid of M = nchannels channels, centred at (k + o/2) fs / M for k in
+ * 0 .. M-1 (k >= M/2 wraps to negative frequencies), out of one COMPLEX16 capture x[0 .. n_in) (x = 0 outside it), filtered by one set
+ * of taps and decimated by D = decim, in one pass; an extension without a reference counterpart.  o = odd_stacking: 0 puts channel 0 at
+ * 0 Hz, 1 at fs / 2M.  For channel k, c = (ntaps - 1) / 2 and every output m in 0 .. n_out = ceil(n_in / D):
+ *     n_j       = D m + j - c                                                   absolute input index met by tap j
+ *     (C, S)    = NCO[((2k + o) n_j (2048 / M)) mod 4096]                       the Q14 table of sb200_channelize
+ *     y_k[m].re = sat16((sum_j taps[j] (x.re C + x.im S) + 2^28) >> 29)         int64, one rounding
+ *     y_k[m].im = sat16((sum_j taps[j] (x.im C - x.re S) + 2^28) >> 29)
+ * This is channel k of sb200_channelize with phase_inc = (2k + o) 2^31 / M and phase0 = 0, except that the rotated sample is kept exact
+ * instead of rounded to int16: the two agree within 2 LSB where neither saturates.  The cost grows with ntaps / D + M^2 / D per input
+ * sample, not with M ntaps / D.  Channel k goes to out[k * out_stride .. + n_out) (samples): the rows go to sb200_rx11a_streams /
+ * sb200_rx11b_streams / sb200_rx11n_streams as they are.  iq and out may be host or device pointers (device: 16-byte aligned, and the
+ * call is then asynchronous on the stream); taps is a host array.  Limits (SB200_E_INVALID, nothing launched): nchannels a power of two,
+ * 2 .. 64; decim divides nchannels; odd_stacking 0 or 1; ntaps odd, 1 .. 1023; sum |taps| <= 65535 (every branch sum fits int32);
+ * out_stride >= n_out, a multiple of 4 and <= 2^40; n_in <= 2^40.  One kernel launch; sb200_last_kernel_ms times it. */
+int sb200_channelize_bank(sb200_handle* h, const int16_t* iq, uint64_t n_in_samples, uint32_t nchannels, uint32_t decim, uint32_t odd_stacking,
+                          const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride_samples, void* cuda_stream);
+
 /* Wideband combiner, the transmit counterpart of sb200_channelize: K = nchannels rows x_k[0 .. n_in) of COMPLEX16 at the channel rate
  * (row k at rows + k * row_stride samples) interpolated by U = interp, each moved to its centre frequency, scaled and summed into one
  * capture y[0 .. U n_in) at the wideband rate; an extension without a reference counterpart.  For channel k = {phase_inc, phase0, gain}

@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_combine", "sb200_combine_rational", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_channelize_bank", "sb200_combine", "sb200_combine_rational", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -71,6 +71,12 @@ def _payload_table(payloads):
 def phase_inc(f_hz, fs_hz):
     """NCO increment of sb200_channelize and sb200_combine for a channel centred at f_hz in a capture at fs_hz: round(f / fs * 2^32) mod 2^32 (negative f wraps)."""
     return int(round(f_hz / fs_hz * 2 ** 32)) % 2 ** 32
+
+def bank_centres(nchannels, fs_hz, odd=False):
+    """Centre frequencies (Hz) of sb200_channelize_bank's channels k = 0 .. M-1 in a capture at fs_hz: (k + o/2) fs / M, wrapped to
+    [-fs/2, fs/2) (channels k >= M/2 are the negative frequencies)."""
+    f = (np.arange(nchannels) + 0.5 * bool(odd)) * fs_hz / nchannels
+    return np.where(np.arange(nchannels) >= nchannels // 2, f - fs_hz, f)
 
 class DdcChannel(C.Structure):
     _fields_ = [("phase_inc", C.c_uint32), ("phase0", C.c_uint32)]
@@ -297,6 +303,24 @@ class Engine:
         n_out = -(-interp * len(iq) // decim); stride = (n_out + 3) // 4 * 4
         out = np.zeros((len(channels), stride, 2), np.int16)
         self.channelize_raw(_ptr(iq), len(iq), channels, decim, taps, _ptr(out), stride, interp=interp)
+        return out[:, :n_out]
+
+    def channelize_bank_raw(self, in_ptr, n_in, nchannels, decim, taps, out_ptr, out_stride, odd=False, stream=0):
+        """Pointer-level sb200_channelize_bank: in_ptr / out_ptr host or device addresses, row k of the output at out_ptr + 4 k out_stride
+        bytes; taps int16 Q15."""
+        t = np.ascontiguousarray(taps, dtype=np.int16)
+        self._check(self._lib.sb200_channelize_bank(self._h, C.c_void_p(in_ptr), C.c_uint64(n_in), C.c_uint32(nchannels), C.c_uint32(decim), C.c_uint32(int(bool(odd))),
+                                                    C.c_void_p(_ptr(t)), C.c_uint32(len(t)), C.c_void_p(out_ptr), C.c_uint64(out_stride), C.c_void_p(stream)),
+                    "sb200_channelize_bank")
+
+    def channelize_bank(self, iq, nchannels, decim, taps, odd=False):
+        """Polyphase filter-bank channelizer: int16 [n,2] -> int16 [M, ceil(n / decim), 2], every channel of the uniform grid of M =
+        nchannels (a power of two, 2 .. 64) centred at bank_centres(M, fs, odd), shifted to 0 Hz, filtered by taps (int16 Q15, odd count
+        <= 1023, sum |t| <= 65535) and decimated by decim (a divisor of M)."""
+        iq = np.ascontiguousarray(iq, dtype=np.int16).reshape(-1, 2)
+        n_out = -(-len(iq) // decim); stride = (n_out + 3) // 4 * 4
+        out = np.zeros((nchannels, stride, 2), np.int16)
+        self.channelize_bank_raw(_ptr(iq), len(iq), nchannels, decim, taps, _ptr(out), stride, odd=odd)
         return out[:, :n_out]
 
     def combine_raw(self, rows_ptr, row_stride, n_in, channels, interp, taps, out_ptr, stream=0, decim=1, n_out=None, accumulate=False):

@@ -1,7 +1,8 @@
 // sora_b200 — the wideband filters and the radio channel simulator: sb200_fir_decimate2, the channelizer and the combiner (fir_kernels.cuh),
-// sb200_channel_sim (sim_kernels.cuh).
+// the filter-bank channelizer (bank_kernels.cuh), sb200_channel_sim (sim_kernels.cuh).
 #include "handle.cuh"
 #include "fir_kernels.cuh"
+#include "bank_kernels.cuh"
 #include "sim_kernels.cuh"
 
 // One launch of k_channelize (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.  Outputs per thread from D;
@@ -153,6 +154,56 @@ extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_i
 extern "C" int sb200_channelize_rational(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels,
                                          uint32_t interp, uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
     return channelize_call(h, iq, n_in, channels, nchannels, interp, decim, taps, ntaps, out, out_stride, cuda_stream, true);
+}
+
+// Polyphase filter-bank channelizer (bank_kernels.cuh): all M = nchannels channels of the uniform grid centred at (k + odd / 2) fs / M,
+// filtered and decimated by `decim`, in one launch; channel k in row k of `out`.  Staging and residency as in channelize_call.
+template <int M>
+static void bank_launch(cudaStream_t st, uint64_t tiles, const uint32_t* d_in, uint64_t n_in, const uint32_t* nco, uint32_t D, uint32_t odd,
+                        const BrTaps& T, uint32_t* d_out, uint64_t stride, uint64_t n_out) {
+    k_channelize_bank<M><<<(unsigned)tiles, SB_FIR_THREADS, 0, st>>>(d_in, n_in, nco, D, odd, T, d_out, stride, n_out);
+}
+extern "C" int sb200_channelize_bank(sb200_handle* h, const int16_t* iq, uint64_t n_in, uint32_t nchannels, uint32_t decim, uint32_t odd_stacking,
+                                     const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
+    if (!h) return SB200_E_INVALID;
+    if (!iq || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
+    const uint32_t M = nchannels, D = decim;
+    if (M < 2 || M > SB_BK_MAXCH || (M & (M - 1))) return h->fail(SB200_E_INVALID, "nchannels must be a power of two, 2 .. 64");
+    if (D < 1 || M % D) return h->fail(SB200_E_INVALID, "decim must divide nchannels");
+    if (odd_stacking > 1u) return h->fail(SB200_E_INVALID, "odd_stacking must be 0 or 1");
+    if ((ntaps & 1u) == 0 || ntaps > SB_BK_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 1023");
+    uint32_t asum = 0; for (uint32_t i = 0; i < ntaps; i++) asum += (uint32_t)abs((int)taps[i]);
+    if (asum > 65535u) return h->fail(SB200_E_INVALID, "sum of |taps| must be at most 65535 (every branch sum and butterfly must fit int32)");
+    if (n_in > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples must be at most 2^40");
+    const uint64_t n_out = (n_in + D - 1) / D;
+    if (out_stride < n_out || (out_stride & 3u) || out_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "out_stride must be at least ceil(n_in / decim), at most 2^40 and a multiple of 4");
+    if (n_in == 0) return SB200_OK;
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    CK(cudaSetDevice(h->device));
+    const bool in_dev = is_device_ptr(iq), out_dev = is_device_ptr(out);
+    if ((in_dev && ((uintptr_t)iq & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device input and output must be 16-byte aligned");
+    CallScope call(h, st); CK(call.begin()); call.reads(iq);
+    const int nrc = upload_nco(h);
+    if (nrc != SB200_OK) return nrc;
+    const uint32_t* d_in; uint32_t* d_out = (uint32_t*)out; uint64_t d_stride = out_stride; Returns ret;
+    CK(to_device(h->iq, (const uint32_t*)iq, in_dev, n_in * 4ull, st, &d_in, 16));
+    if (!out_dev) {                                    // rows n_out (rounded to 4) apart in the workspace, copied into the caller's rows
+        d_stride = (n_out + 3u) & ~3ull; CK(h->iq40.need(M * d_stride * 4ull)); d_out = (uint32_t*)h->iq40.p;
+        ret.bind2d(out, out_stride * 4ull, d_out, d_stride * 4ull, n_out * 4ull, M);
+    }
+    const BrTaps T = branch_taps(taps, ntaps, 1);      // the taps in their own order
+    const uint64_t tiles = (n_in + SB_FIR_TILE - 1) / SB_FIR_TILE;
+    const uint32_t* nco = (const uint32_t*)h->nco.p;
+    CK(cudaEventRecord(h->ev0, st));
+    switch (M) {
+        case 2:  bank_launch<2>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
+        case 4:  bank_launch<4>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
+        case 8:  bank_launch<8>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
+        case 16: bank_launch<16>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
+        case 32: bank_launch<32>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
+        default: bank_launch<64>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
+    }
+    return finish_call(h, st, ret, 0, 1);
 }
 
 // One launch of k_combine<J, RAT> (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.  ChTaps launches the
