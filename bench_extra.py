@@ -15,6 +15,8 @@
                       timed beside sb200_channelize on the same eight channels and taps
   --config channelize_rational  the rational-rate channelizer: three 802.11b channels of a 160 Msps capture to 44 Msps, 1287 taps, U / D = 11 / 40
   --config combine   the wideband combiner: four 802.11a channel rows at 40 Msps into one 160 Msps capture, 127 taps, U = 4, device-resident
+  --config combine_bank  the filter-bank combiner: eight odd-stacked 40 Msps rows into one 160 Msps capture, 255 taps, U = 4,
+                      timed beside sb200_combine on the same eight channels and taps
   --config combine_rational  the rational-rate combiner: three 802.11b rows at 44 Msps into one 160 Msps capture, 1761 taps, U / D = 40 / 11
   --config sim       the radio channel simulator: --frames links of config #2's 9 824-sample slots (T = R = 1, L = 16, +20 ppm, a carrier
                      offset, noise on), and a 2x2 case (T = R = 2, L = 16), device-resident
@@ -563,6 +565,39 @@ def bench_combine(args):
             "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs" % m})
     c.close()
 
+def bench_combine_bank(args):
+    """The filter-bank combiner into a device-resident 160 Msps capture of --config combine's size: eight odd-stacked rows at 40 Msps
+    (+-10 / +-30 / +-50 / +-70 MHz), 255 taps, U = 4; and, in the same process on the same rows, sb200_combine on the same eight channels and
+    taps, the way a user would fill the grid without the bank.  Integer work per output sample: bank 2 ntaps / U + 4 M^2 / U (the branch
+    filter and the direct M-point IDFT), combiner K (2 ceil(ntaps / U) + 6)."""
+    import wideband_inputs as W, combine_bank_model as CB
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    M, U = 8, 4; n_out = args.frames * 9824 * 4; n_in = n_out // U
+    taps = W.lowpass(255, 10e6 / 160e6, gain=U); ch = CB.channels(M, 1)
+    x = torch.randint(-8000, 8000, (M, n_in, 2), dtype=torch.int16, device=dev); y = torch.empty((n_out, 2), dtype=torch.int16, device=dev)
+    P = 5000; m = U * P - len(taps)                                      # outputs that a prefix of P input samples determines
+    def bank(): eng.combine_bank_raw(x.data_ptr(), n_in, n_in, M, U, taps, y.data_ptr(), n_out, odd=True, stream=st.cuda_stream)
+    def comb(): eng.combine_raw(x.data_ptr(), n_in, n_in, ch, U, taps, y.data_ptr(), st.cuda_stream)
+    bank(); torch.cuda.synchronize()
+    xp = x[:, :P].cpu().numpy()
+    assert (CB.window(xp, M, U, 1, taps, 0, m) == y[:m].cpu().numpy()).all(), "filter-bank output differs from the stated arithmetic"
+    ms_bank = c.timed(bank, args.steps); ms_comb = c.timed(comb, args.steps)
+    name, plim, clk = _card(); sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    imad_peak = sms * 64 * clk * 1e6 if clk else None                    # int32 IMAD: 64 per SM per clock on sm_90
+    hbm = n_out * (4.0 + 4.0 * M / U)
+    for what, ms, work, note in (("filter-bank combiner (sb200_combine_bank)", ms_bank, n_out * (2.0 * len(taps) / U + 4.0 * M * M / U), "2 ntaps / U + 4 M^2 / U per output sample"),
+                                 ("wideband combiner (sb200_combine) on the same channels", ms_comb, n_out * M * (2.0 * -(-len(taps) // U) + 6.0), "K (2 ceil(ntaps / U) + 6) per output sample")):
+        sec = ms * 1e-3; f_int = (work / sec / imad_peak) if imad_peak else None
+        c.emit({"metric": "%s output Gsamples/s (COMPLEX16 out, 8 odd-stacked channels, 255 taps, U = 4)" % what, "value": c.world * n_out / sec / 1e9, "unit": "Gsamples/s",
+                "ms_per_step": ms, "n_gpus": c.world, "bank_speedup": ms_comb / ms_bank,
+                "config": {"workload": "8 rows at 40 Msps -> 160 Msps capture, channels at +-10/30/50/70 MHz, 255 taps, U = 4, device-resident", "output_samples_per_step_per_gpu": n_out},
+                "hbm": {"achieved": hbm / sec / 1e9, "peak": peaks(), "unit": "GB/s", "frac": hbm / sec / 1e9 / peaks(), "note": "4 B written + 4 M / U B read per output sample"},
+                "int_mad": {"achieved": work / sec / 1e9, "peak": imad_peak / 1e9 if imad_peak else None, "unit": "G multiply-adds/s", "frac": f_int,
+                            "note": note + "; peak = SMs x 64 x max SM clock"},
+                "card": name, "power_limit_w": plim, "sm_clock_max_mhz": clk,
+                "parity": "bank equal to the numpy model of the stated arithmetic on the first %d outputs" % m})
+    c.close()
+
 def bench_combine_rational(args):
     """The rational-rate combiner into a device-resident 160 Msps capture the size of --config combine's: three 802.11b rows at 44 Msps
     moved to -25 / 0 / +25 MHz, U / D = 40 / 11 through 1761 taps (45 per branch; --ratio U/D picks another pair, with 45 taps per branch
@@ -634,7 +669,7 @@ def bench_sim(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_bank", "channelize_rational", "combine", "combine_rational", "sim"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_bank", "channelize_rational", "combine", "combine_bank", "combine_rational", "sim"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
@@ -642,4 +677,4 @@ if __name__ == "__main__":
                     "a pair other than 40/11 takes a generic low-pass of 45 taps per branch at 0.55 of the row's Nyquist")
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_bank": bench_channelize_bank, "channelize_rational": bench_channelize_rational, "combine": bench_combine, "combine_rational": bench_combine_rational, "sim": bench_sim}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_bank": bench_channelize_bank, "channelize_rational": bench_channelize_rational, "combine": bench_combine, "combine_bank": bench_combine_bank, "combine_rational": bench_combine_rational, "sim": bench_sim}[a.config](a)

@@ -203,6 +203,37 @@ int sb200_channelize_rational(sb200_handle* h, const int16_t* iq, uint64_t n_in_
 int sb200_channelize_bank(sb200_handle* h, const int16_t* iq, uint64_t n_in_samples, uint32_t nchannels, uint32_t decim, uint32_t odd_stacking,
                           const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride_samples, void* cuda_stream);
 
+/* Polyphase filter-bank combiner, the transmit counterpart of sb200_channelize_bank: M = nchannels rows x_k[0 .. n_in) of COMPLEX16 (row k
+ * at rows + k * row_stride samples, x_k = 0 outside it) interpolated by U = interp, row k moved to the centre (k + o/2) fs / M of the grid
+ * of sb200_channelize_bank (o = odd_stacking; api.bank_centres gives the centres), and summed into one capture y[0 .. n_out) in one pass;
+ * an extension without a reference counterpart.  With c = (ntaps - 1) / 2, T[i] = NCO[i 2048 / M] (the Q14 table of sb200_channelize) and
+ * sigma(n) = (-1)^(o floor(n / M)), every output n in 0 .. n_out = n_out_samples is, in int64 and exact up to the two roundings:
+ *     W_p(i) = (sum_k x_k(i) T[(2k + o) p mod 2M] + 2^13) >> 14        p = 0 .. M-1; rotating up: re = x.re C - x.im S, im = x.im C + x.re S
+ *     acc(n) = sum_i taps[c + U i - n] W_{n mod M}(i)                   over 0 <= i < n_in, 0 <= c + U i - n < ntaps
+ *     a(n)   = accumulate ? out[n] as it was before the call : 0
+ *     y(n)   = sat16(a(n) + ((sigma(n) acc(n) + 2^14) >> 15))
+ * Channel k is sb200_combine channel {(2k + o) 2^31 / M, 0, 4096} at the same U, rotated by the phase of the absolute output index as
+ * there: for n = M a + p that channel's table entry is NCO[(2k + o) n 2048 / M mod 4096] = sigma(n) T[(2k + o) p mod 2M].  The bank rounds
+ * twice in all where sb200_combine rounds after the filter and after every rotation, so where nothing saturates the two differ by at most
+ * 1.2072 K + 0.5 B / 32768 + 0.5 per component, K the number of non-zero rows and B the largest per-branch sum of |taps|.  Proof: against
+ * the exact value, each of sb200_combine's channels is off by its filter rounding (0.5 per component) carried through the Q14 rotation,
+ * 0.5 (|C| + |S|)_max / 16384 = 0.5 * 23170 / 16384 <= 0.7072, plus the rotation's own 0.5; a zero row adds nothing.  The bank's W is off
+ * by at most 0.5, which the one branch of taps an output meets scales by at most B / 32768 before the final rounding adds 0.5.
+ * A row sent with (M, U, o) comes back from sb200_channelize_bank with (M, D = U, o), aligned at the same index.  With E_p and O_p the
+ * even-k and odd-k halves of the sum, W_p = E_p + O_p and W_{p+M/2} = j^o (E_p - O_p), exact in int64 before the rounding
+ * (NCO[i + 2048] = -NCO[i], NCO[i + 1024] = j NCO[i]): the kernel computes half the products of the direct sum.
+ * Unlike the other wideband calls there is no tap-sum limit: |W| < 2^22 and |acc| < 2^47 at every limit.  There are no per-channel
+ * gains: a Q12 gain on x before the IDFT would need a third rounding or more than int64 range; scale the rows instead.
+ * n_out is the caller's choice: outputs past the rows' support are a(n) plus the filter's tail.  n_out = 0 launches nothing and n_in = 0
+ * means all-zero rows.  rows and out may be host or device pointers (device: 16-byte aligned, and the call is then asynchronous on the
+ * stream; a host out is uploaded first when accumulate = 1); taps is a host array.  Limits (SB200_E_INVALID, nothing launched): nchannels a
+ * power of two, 2 .. 64; interp divides nchannels; odd_stacking 0 or 1; ntaps odd, 1 .. 1023 and ntaps <= 2048 interp / nchannels (that
+ * is, ceil(ntaps / U) M <= 2048); row_stride >= n_in, a multiple of 4 and <= 2^40; n_in <= 2^40; n_out <= 2^40; accumulate 0 or 1.
+ * One kernel launch; sb200_last_kernel_ms times it. */
+int sb200_combine_bank(sb200_handle* h, const int16_t* rows, uint64_t row_stride_samples, uint64_t n_in_samples,
+                       uint32_t nchannels, uint32_t interp, uint32_t odd_stacking, const int16_t* taps, uint32_t ntaps,
+                       int16_t* out, uint64_t n_out_samples, uint32_t accumulate, void* cuda_stream);
+
 /* Wideband combiner, the transmit counterpart of sb200_channelize: K = nchannels rows x_k[0 .. n_in) of COMPLEX16 at the channel rate
  * (row k at rows + k * row_stride samples) interpolated by U = interp, each moved to its centre frequency, scaled and summed into one
  * capture y[0 .. U n_in) at the wideband rate; an extension without a reference counterpart.  For channel k = {phase_inc, phase0, gain}

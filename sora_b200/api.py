@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_channelize_bank", "sb200_combine", "sb200_combine_rational", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_channelize_bank", "sb200_combine", "sb200_combine_rational", "sb200_combine_bank", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -350,6 +350,30 @@ class Engine:
         if not (isinstance(out, np.ndarray) and out.dtype == np.int16 and out.shape == (n, 2) and out.flags.c_contiguous and out.flags.writeable):
             raise ValueError("out must be a writeable C-contiguous int16 numpy array of shape [n_out, 2]")
         self.combine_raw(_ptr(x), stride, n_in, channels, interp, taps, _ptr(out), decim=decim, n_out=n_out, accumulate=accumulate)
+        return out
+
+    def combine_bank_raw(self, rows_ptr, row_stride, n_in, nchannels, interp, taps, out_ptr, n_out, odd=False, accumulate=False, stream=0):
+        """Pointer-level sb200_combine_bank: rows_ptr / out_ptr host or device addresses, row k at rows_ptr + 4 k row_stride bytes; taps
+        int16 Q15; n_out outputs."""
+        t = np.ascontiguousarray(taps, dtype=np.int16)
+        self._check(self._lib.sb200_combine_bank(self._h, C.c_void_p(rows_ptr), C.c_uint64(row_stride), C.c_uint64(n_in), C.c_uint32(nchannels), C.c_uint32(interp),
+                                                 C.c_uint32(int(bool(odd))), C.c_void_p(_ptr(t)), C.c_uint32(len(t)), C.c_void_p(out_ptr), C.c_uint64(n_out),
+                                                 C.c_uint32(int(bool(accumulate))), C.c_void_p(stream)), "sb200_combine_bank")
+
+    def combine_bank(self, rows, interp, taps, odd=False, n_out=None, accumulate=False, out=None):
+        """Polyphase filter-bank combiner: int16 [M, n_in, 2] rows -> int16 [n_out, 2], row k interpolated by interp (a divisor of M, a
+        power of two 2 .. 64) through taps (int16 Q15, odd count <= 1023 and <= 2048 interp / M) and moved to bank_centres(M, fs, odd)[k];
+        n_out defaults to interp * n_in.  accumulate adds the sum onto `out` (int16 [n_out, 2], updated in place and returned) with one
+        saturation."""
+        rows = np.asarray(rows, dtype=np.int16)
+        if rows.ndim != 3 or rows.shape[2] != 2: raise ValueError("rows must be int16 [M, n_in, 2]")
+        M, n_in = rows.shape[:2]; stride = (n_in + 3) // 4 * 4
+        x = np.zeros((M, stride, 2), np.int16); x[:, :n_in] = rows
+        n = interp * n_in if n_out is None else n_out
+        if out is None: out = np.zeros((n, 2), np.int16)
+        if not (isinstance(out, np.ndarray) and out.dtype == np.int16 and out.shape == (n, 2) and out.flags.c_contiguous and out.flags.writeable):
+            raise ValueError("out must be a writeable C-contiguous int16 numpy array of shape [n_out, 2]")
+        self.combine_bank_raw(_ptr(x), stride, n_in, M, interp, taps, _ptr(out), n, odd=odd, accumulate=accumulate)
         return out
 
     def channel_sim_raw(self, x_ptr, in_link_stride, in_row_stride, ntx, n_in, links, taps, ntaps, nlinks, seed, y_ptr, out_link_stride, out_row_stride,

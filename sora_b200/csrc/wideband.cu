@@ -1,5 +1,5 @@
 // sora_b200 — the wideband filters and the radio channel simulator: sb200_fir_decimate2, the channelizer and the combiner (fir_kernels.cuh),
-// the filter-bank channelizer (bank_kernels.cuh), sb200_channel_sim (sim_kernels.cuh).
+// the filter-bank channelizer and combiner (bank_kernels.cuh), sb200_channel_sim (sim_kernels.cuh).
 #include "handle.cuh"
 #include "fir_kernels.cuh"
 #include "bank_kernels.cuh"
@@ -227,6 +227,32 @@ static int combine_launch_j(sb200_handle* h, cudaStream_t st, const uint32_t* d_
     return SB200_OK;
 }
 
+// Residency and staging of the combiners (combine_call, sb200_combine_bank), after their own checks: host rows go up into the workspace
+// n_in (rounded to 4) apart, a host `out` is bound to the workspace (its samples uploaded first when `accumulate`), then
+// launch(st, d_in, d_stride, d_out) launches the kernel between ev0 and finish_call.
+template <class Launch>
+static int combine_run(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, uint32_t nrows, int16_t* out, uint64_t n_out,
+                       uint32_t accumulate, void* cuda_stream, Launch launch) {
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    CK(cudaSetDevice(h->device));
+    const bool in_dev = is_device_ptr(rows), out_dev = is_device_ptr(out);
+    if ((in_dev && ((uintptr_t)rows & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device rows and output must be 16-byte aligned");
+    CallScope call(h, st); CK(call.begin()); call.reads(rows);
+    const int nrc = upload_nco(h);
+    if (nrc != SB200_OK) return nrc;
+    const uint32_t* d_in = (const uint32_t*)rows; uint64_t d_stride = row_stride; uint32_t* d_out; Returns ret;
+    if (!in_dev && n_in) {                             // rows n_in (rounded to 4) apart in the workspace
+        d_stride = (n_in + 3u) & ~3ull; CK(h->iq.need(nrows * d_stride * 4ull + 16)); d_in = (const uint32_t*)h->iq.p;
+        CK(cudaMemcpy2DAsync(h->iq.p, d_stride * 4ull, rows, row_stride * 4ull, n_in * 4ull, nrows, cudaMemcpyHostToDevice, st));
+    }
+    CK(ret.bind(h->iq40, (uint32_t*)out, n_out * 4ull, &d_out, 16));
+    if (accumulate && !out_dev) {                      // the caller's samples go up into the workspace before the launch adds onto them
+        call.reads(out); CK(cudaMemcpyAsync(d_out, out, n_out * 4ull, cudaMemcpyHostToDevice, st));
+    }
+    const int rc = launch(st, d_in, d_stride, d_out);
+    return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
+}
+
 // Wideband combiner (fir_kernels.cuh): every row zero-stuffed by `interp`, filtered (and decimated by `decim`), shifted up by its NCO,
 // scaled and summed into `out` (or onto it).  sb200_combine is the decim = 1, n_out = interp n_in case of sb200_combine_rational with its
 // own limits and kernel specialisation; both share the checks, staging and launch here (rational = false: sb200_combine).
@@ -253,40 +279,25 @@ static int combine_call(sb200_handle* h, const int16_t* rows, uint64_t row_strid
         if (n_in > (1ull << 40) || n_out > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples and n_out_samples must be at most 2^40");
         if (n_out == 0) return SB200_OK;
     }
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    CK(cudaSetDevice(h->device));
-    const bool in_dev = is_device_ptr(rows), out_dev = is_device_ptr(out);
-    if ((in_dev && ((uintptr_t)rows & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device rows and output must be 16-byte aligned");
-    CallScope call(h, st); CK(call.begin()); call.reads(rows);
-    const int nrc = upload_nco(h);
-    if (nrc != SB200_OK) return nrc;
-    const uint32_t* d_in = (const uint32_t*)rows; uint64_t d_stride = row_stride; uint32_t* d_out; Returns ret;
-    if (!in_dev && n_in) {                             // rows n_in (rounded to 4) apart in the workspace
-        d_stride = (n_in + 3u) & ~3ull; CK(h->iq.need(nchannels * d_stride * 4ull + 16)); d_in = (const uint32_t*)h->iq.p;
-        CK(cudaMemcpy2DAsync(h->iq.p, d_stride * 4ull, rows, row_stride * 4ull, n_in * 4ull, nchannels, cudaMemcpyHostToDevice, st));
-    }
-    CK(ret.bind(h->iq40, (uint32_t*)out, n_out * 4ull, &d_out, 16));
-    if (accumulate && !out_dev) {                      // the caller's samples go up into the workspace before the launch adds onto them
-        call.reads(out); CK(cudaMemcpyAsync(d_out, out, n_out * 4ull, cudaMemcpyHostToDevice, st));
-    }
-    CbChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
-    for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; ch.gain[i] = channels[i].gain; }
-    if (!rational) {                                   // tiles of 1024, 512 or 256 input samples: the largest whose shared memory fits SB_CB_SMEM (256 always does)
-        ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
-        if (combine_smem(nchannels, interp, ntaps, 4 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
-        else if (combine_smem(nchannels, interp, ntaps, 2 * SB_FIR_THREADS) <= SB_CB_SMEM) rc = combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
-        else rc = combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
-    } else {
+    return combine_run(h, rows, row_stride, n_in, nchannels, out, n_out, accumulate, cuda_stream,
+                       [&](cudaStream_t st, const uint32_t* d_in, uint64_t d_stride, uint32_t* d_out) {
+        CbChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
+        for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; ch.gain[i] = channels[i].gain; }
+        if (!rational) {                               // tiles of 1024, 512 or 256 input samples: the largest whose shared memory fits SB_CB_SMEM (256 always does)
+            ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
+            if (combine_smem(nchannels, interp, ntaps, 4 * SB_FIR_THREADS) <= SB_CB_SMEM) return combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
+            if (combine_smem(nchannels, interp, ntaps, 2 * SB_FIR_THREADS) <= SB_CB_SMEM) return combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
+            return combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, 1, 8, T, d_out, n_out, 0);
+        }
         const BrTaps T = branch_taps(taps, ntaps, interp);
         // 32 W J outputs per phase: the largest of 1024 .. 32 whose shared memory fits SB_CBR_SMEM, else 32 (within SB_CBR_SMEM_MAX)
         static const uint32_t kj[6] = {4, 2, 1, 1, 1, 1}, kw[6] = {8, 8, 8, 4, 2, 1};
         int p = 0;
         while (p < 5 && combine_smem_r(nchannels, interp, decim, ntaps, 32u * kw[p] * kj[p]) > SB_CBR_SMEM) p++;
-        if (kj[p] == 4) rc = combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, decim, kw[p], T, d_out, n_out, accumulate);
-        else if (kj[p] == 2) rc = combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, decim, kw[p], T, d_out, n_out, accumulate);
-        else rc = combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, decim, kw[p], T, d_out, n_out, accumulate);
-    }
-    return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
+        if (kj[p] == 4) return combine_launch_j<4>(h, st, d_in, d_stride, n_in, ch, interp, decim, kw[p], T, d_out, n_out, accumulate);
+        if (kj[p] == 2) return combine_launch_j<2>(h, st, d_in, d_stride, n_in, ch, interp, decim, kw[p], T, d_out, n_out, accumulate);
+        return combine_launch_j<1>(h, st, d_in, d_stride, n_in, ch, interp, decim, kw[p], T, d_out, n_out, accumulate);
+    });
 }
 extern "C" int sb200_combine(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, const sb200_duc_channel* channels, uint32_t nchannels,
                              uint32_t interp, const int16_t* taps, uint32_t ntaps, int16_t* out, void* cuda_stream) {
@@ -298,6 +309,48 @@ extern "C" int sb200_combine_rational(sb200_handle* h, const int16_t* rows, uint
                                       uint32_t nchannels, uint32_t interp, uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out,
                                       uint64_t n_out, uint32_t accumulate, void* cuda_stream) {
     return combine_call(h, rows, row_stride, n_in, channels, nchannels, interp, decim, taps, ntaps, out, n_out, accumulate, cuda_stream, true);
+}
+
+// Polyphase filter-bank combiner (bank_kernels.cuh): the M = nchannels rows onto the uniform grid centred at (k + odd / 2) fs / M,
+// interpolated by `interp`, summed into n_out outputs (added onto out's samples when `accumulate`) in one launch.  Residency and staging
+// as in combine_call; tiles of U 1024 / M outputs on a grid of (gx, gy) as combine_launch_j's: n_out <= 2^40 gives at most 2^36 tiles.
+template <int M>
+static void combine_bank_launch(cudaStream_t st, uint64_t n_out, const uint32_t* d_in, uint64_t stride, uint64_t n_in, const uint32_t* nco, uint32_t U,
+                                uint32_t odd, const BrTaps& T, uint32_t* d_out, uint32_t accumulate) {
+    const uint64_t to = U * (SB_CBK_SPAN / M), tiles = (n_out + to - 1) / to;
+    const uint64_t gy = (tiles + 0x7FFFFFFEull) / 0x7FFFFFFFull, gx = (tiles + gy - 1) / gy;
+    k_combine_bank<M><<<dim3((unsigned)gx, (unsigned)gy), SB_FIR_THREADS, 0, st>>>(d_in, stride, n_in, nco, U, odd, T, d_out, n_out, accumulate);
+}
+extern "C" int sb200_combine_bank(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, uint32_t nchannels, uint32_t interp,
+                                  uint32_t odd_stacking, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t n_out, uint32_t accumulate,
+                                  void* cuda_stream) {
+    if (!h) return SB200_E_INVALID;
+    if (!rows || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
+    const uint32_t M = nchannels, U = interp;
+    if (M < 2 || M > SB_BK_MAXCH || (M & (M - 1))) return h->fail(SB200_E_INVALID, "nchannels must be a power of two, 2 .. 64");
+    if (U < 1 || M % U) return h->fail(SB200_E_INVALID, "interp must divide nchannels");
+    if (odd_stacking > 1u) return h->fail(SB200_E_INVALID, "odd_stacking must be 0 or 1");
+    if ((ntaps & 1u) == 0 || ntaps > SB_BK_MAXTAPS || ntaps > 2 * SB_CBK_SPAN / M * U)
+        return h->fail(SB200_E_INVALID, "ntaps must be odd, at most 1023 and at most 2048 interp / nchannels");
+    if (accumulate > 1u) return h->fail(SB200_E_INVALID, "accumulate must be 0 or 1");
+    if (row_stride < n_in || (row_stride & 3u) || row_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "row_stride must be at least n_in, at most 2^40 and a multiple of 4");
+    if (n_in > (1ull << 40) || n_out > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples and n_out_samples must be at most 2^40");
+    if (n_out == 0) return SB200_OK;
+    return combine_run(h, rows, row_stride, n_in, M, out, n_out, accumulate, cuda_stream,
+                       [&](cudaStream_t st, const uint32_t* d_in, uint64_t d_stride, uint32_t* d_out) {
+        const BrTaps T = branch_taps(taps, ntaps, 1);  // the taps in their own order
+        const uint32_t* nco = (const uint32_t*)h->nco.p;
+        CK(cudaEventRecord(h->ev0, st));
+        switch (M) {
+            case 2:  combine_bank_launch<2>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
+            case 4:  combine_bank_launch<4>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
+            case 8:  combine_bank_launch<8>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
+            case 16: combine_bank_launch<16>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
+            case 32: combine_bank_launch<32>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
+            default: combine_bank_launch<64>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
+        }
+        return SB200_OK;
+    });
 }
 
 // The table of sb200_channel_sim (sim_kernels.cuh), uploaded on first use: the NCO of fill_nco, then H (256 rows of 8 Q14 taps, packed in
