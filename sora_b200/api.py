@@ -135,6 +135,20 @@ def _ptr(a):
         return a.data_ptr()
     raise TypeError(type(a))
 
+def _rows4(k, n, rows=None):
+    """k zeroed int16 rows of n samples, a stride of n rounded up to 4 apart, with `rows` ([k, n, 2]) copied in -> (int16 [k, stride, 2], stride)."""
+    stride = (n + 3) // 4 * 4
+    x = np.zeros((k, stride, 2), np.int16)
+    if rows is not None: x[:, :n] = rows
+    return x, stride
+
+def _out_samples(out, n):
+    """The output of a combiner: zeros when out is None, else out itself once checked to be a writeable C-contiguous int16 [n, 2] array."""
+    if out is None: return np.zeros((n, 2), np.int16)
+    if not (isinstance(out, np.ndarray) and out.dtype == np.int16 and out.shape == (n, 2) and out.flags.c_contiguous and out.flags.writeable):
+        raise ValueError("out must be a writeable C-contiguous int16 numpy array of shape [n_out, 2]")
+    return out
+
 class Engine:
     """One sb200 handle = one GPU context (BB11aDemodContext analogue: fb11ademod_config.hpp:20-123)."""
     def __init__(self, device=0, cca_pwr_threshold=0):
@@ -300,8 +314,7 @@ class Engine:
         to 0 Hz, filtered by taps (int16 Q15, odd count; interp = 1: <= 255 taps, sum |t| <= 65535; else ceil(ntaps / interp) <= 255 and
         the same limit per branch) and resampled by interp / decim."""
         iq = np.ascontiguousarray(iq, dtype=np.int16).reshape(-1, 2)
-        n_out = -(-interp * len(iq) // decim); stride = (n_out + 3) // 4 * 4
-        out = np.zeros((len(channels), stride, 2), np.int16)
+        n_out = -(-interp * len(iq) // decim); out, stride = _rows4(len(channels), n_out)
         self.channelize_raw(_ptr(iq), len(iq), channels, decim, taps, _ptr(out), stride, interp=interp)
         return out[:, :n_out]
 
@@ -318,8 +331,7 @@ class Engine:
         nchannels (a power of two, 2 .. 64) centred at bank_centres(M, fs, odd), shifted to 0 Hz, filtered by taps (int16 Q15, odd count
         <= 1023, sum |t| <= 65535) and decimated by decim (a divisor of M)."""
         iq = np.ascontiguousarray(iq, dtype=np.int16).reshape(-1, 2)
-        n_out = -(-len(iq) // decim); stride = (n_out + 3) // 4 * 4
-        out = np.zeros((nchannels, stride, 2), np.int16)
+        n_out = -(-len(iq) // decim); out, stride = _rows4(nchannels, n_out)
         self.channelize_bank_raw(_ptr(iq), len(iq), nchannels, decim, taps, _ptr(out), stride, odd=odd)
         return out[:, :n_out]
 
@@ -343,12 +355,8 @@ class Engine:
         n_out = interp * n_in.  With decim, n_out or accumulate it is sb200_combine_rational: the rate changes by interp / decim (ntaps <= 4095
         with ceil(ntaps / interp) <= 255), n_out defaults to ceil(interp n_in / decim), and accumulate adds the sum onto `out` (int16
         [n_out, 2], updated in place and returned) with one saturation."""
-        rows = np.asarray(rows, dtype=np.int16).reshape(len(channels), -1, 2); n_in = rows.shape[1]; stride = (n_in + 3) // 4 * 4
-        x = np.zeros((len(channels), stride, 2), np.int16); x[:, :n_in] = rows
-        n = -(-interp * n_in // decim) if n_out is None else n_out
-        if out is None: out = np.zeros((n, 2), np.int16)
-        if not (isinstance(out, np.ndarray) and out.dtype == np.int16 and out.shape == (n, 2) and out.flags.c_contiguous and out.flags.writeable):
-            raise ValueError("out must be a writeable C-contiguous int16 numpy array of shape [n_out, 2]")
+        rows = np.asarray(rows, dtype=np.int16).reshape(len(channels), -1, 2); n_in = rows.shape[1]; x, stride = _rows4(len(channels), n_in, rows)
+        out = _out_samples(out, -(-interp * n_in // decim) if n_out is None else n_out)
         self.combine_raw(_ptr(x), stride, n_in, channels, interp, taps, _ptr(out), decim=decim, n_out=n_out, accumulate=accumulate)
         return out
 
@@ -367,13 +375,9 @@ class Engine:
         saturation."""
         rows = np.asarray(rows, dtype=np.int16)
         if rows.ndim != 3 or rows.shape[2] != 2: raise ValueError("rows must be int16 [M, n_in, 2]")
-        M, n_in = rows.shape[:2]; stride = (n_in + 3) // 4 * 4
-        x = np.zeros((M, stride, 2), np.int16); x[:, :n_in] = rows
-        n = interp * n_in if n_out is None else n_out
-        if out is None: out = np.zeros((n, 2), np.int16)
-        if not (isinstance(out, np.ndarray) and out.dtype == np.int16 and out.shape == (n, 2) and out.flags.c_contiguous and out.flags.writeable):
-            raise ValueError("out must be a writeable C-contiguous int16 numpy array of shape [n_out, 2]")
-        self.combine_bank_raw(_ptr(x), stride, n_in, M, interp, taps, _ptr(out), n, odd=odd, accumulate=accumulate)
+        M, n_in = rows.shape[:2]; x, stride = _rows4(M, n_in, rows)
+        out = _out_samples(out, interp * n_in if n_out is None else n_out)
+        self.combine_bank_raw(_ptr(x), stride, n_in, M, interp, taps, _ptr(out), len(out), odd=odd, accumulate=accumulate)
         return out
 
     def channel_sim_raw(self, x_ptr, in_link_stride, in_row_stride, ntx, n_in, links, taps, ntaps, nlinks, seed, y_ptr, out_link_stride, out_row_stride,

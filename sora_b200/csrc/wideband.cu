@@ -5,6 +5,15 @@
 #include "bank_kernels.cuh"
 #include "sim_kernels.cuh"
 
+// Lets `kernel` use `bytes` of dynamic shared memory on this device, once per handle: bit `bit` of `set` records that it has.
+template <class Mask, class Kernel>
+static cudaError_t smem_once(Mask& set, uint64_t bit, Kernel kernel, int bytes) {
+    if (set & bit) return cudaSuccess;
+    const cudaError_t e = cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+    if (e == cudaSuccess) set |= (Mask)bit;
+    return e;
+}
+
 // One launch of k_channelize (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.  Outputs per thread from D;
 // channels split into groups (the input then read once per group) only as far as needed for four CTAs per multiprocessor.  ChTaps
 // launches the U = 1 specialisation, BrTaps the rational one.
@@ -12,11 +21,7 @@ template <int J, class Taps>
 static int channelize_launch_j(sb200_handle* h, cudaStream_t st, dim3 grid, const uint32_t* d_in, uint64_t n_in, const ChChannels& ch, uint32_t cpg,
                                uint32_t D, const Taps& T, uint32_t* d_out, uint64_t stride, uint64_t n_out) {
     constexpr bool RAT = std::is_same<Taps, BrTaps>::value;
-    const uint64_t bit = 1ull << (J + (RAT ? 32 : 0));
-    if (!(h->ch_smem_set & bit)) {
-        CK(cudaFuncSetAttribute(k_channelize<J, RAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_CH_SMEM));
-        h->ch_smem_set |= bit;
-    }
+    CK(smem_once(h->ch_smem_set, 1ull << (J + (RAT ? 32 : 0)), k_channelize<J, RAT>, SB_CH_SMEM));
     CK(cudaEventRecord(h->ev0, st));
     k_channelize<J, RAT><<<grid, SB_FIR_THREADS, SB_CH_SMEM, st>>>(d_in, n_in, (const uint32_t*)h->nco.p, ch, cpg, D, T, d_out, stride, n_out);
     return SB200_OK;
@@ -67,19 +72,16 @@ extern "C" int sb200_fir_decimate2(sb200_handle* h, const int16_t* iq, uint64_t 
 static void fill_nco(uint32_t* t) {
     for (int i = 0; i < SB_CH_NCO; i++) { const double a = 2.0 * M_PI * i / 4096.0; t[i] = pack(mk((int)nearbyint(16384.0 * cos(a)), (int)nearbyint(16384.0 * sin(a)))); }
 }
-// The NCO table of sb200_channelize and sb200_combine, uploaded on first use.
+// The NCO table of the channelizers and the combiners, uploaded on first use.
 static int upload_nco(sb200_handle* h) {
     if (h->nco.p) return SB200_OK;
     std::vector<uint32_t> t(SB_CH_NCO);
     fill_nco(t.data());
-    cudaError_t e = h->nco.need(SB_CH_NCO * 4);
-    if (e == cudaSuccess) e = cudaMemcpy(h->nco.p, t.data(), SB_CH_NCO * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();   // landed before a kernel on a non-blocking stream reads it (TableArena::upload)
-    if (e != cudaSuccess) { h->nco.release(); return h->fail(SB200_E_CUDA, "NCO table upload", e); }
-    return SB200_OK;
+    TableArena ar; ar.add(t.data(), SB_CH_NCO * 4);
+    return ar.upload(h, h->nco, "cudaMalloc NCO table", "NCO table upload");
 }
 
-// Checks of the channelizer's and the combiner's calls, which pass the messages in their own parameter names.  The rate pair of the
+// Checks of the channelizers' and the combiners' calls, which pass the messages in their own parameter names.  The rate pair of the
 // rational-rate calls: the smaller factor 1 .. 16, the larger from it to 64, coprime.
 static_assert(SB_CH_MAXINTERP == SB_CH_MAXDECIM && SB_CH_MAXRDECIM == SB_CBR_MAXINTERP, "the rational channelizer and combiner share their rate limits");
 static int check_rate_pair(sb200_handle* h, uint32_t lo, uint32_t hi, const char* lo_msg, const char* hi_msg) {
@@ -88,14 +90,29 @@ static int check_rate_pair(sb200_handle* h, uint32_t lo, uint32_t hi, const char
     uint32_t a = lo, b = hi; while (b) { const uint32_t t = a % b; a = b; b = t; }
     return a == 1 ? SB200_OK : h->fail(SB200_E_INVALID, "interp and decim must be coprime");
 }
-// The taps: ntaps odd, at most max_ntaps and at most 255 per branch (taps r, r + interp, ...); the |tap| sum of each branch at most 65535,
-// so that the int32 accumulator of an output, which meets one branch, cannot wrap.
-static int check_taps(sb200_handle* h, const int16_t* taps, uint32_t ntaps, uint32_t interp, uint32_t max_ntaps, const char* len_msg, const char* sum_msg) {
-    if ((ntaps & 1u) == 0 || ntaps > max_ntaps || (ntaps + interp - 1) / interp > SB_CH_MAXTAPS) return h->fail(SB200_E_INVALID, len_msg);
+// The |tap| sum of each branch (taps r, r + interp, ...) at most 65535, so that the int32 sums over one branch cannot wrap.
+static int check_tap_sums(sb200_handle* h, const int16_t* taps, uint32_t ntaps, uint32_t interp) {
     for (uint32_t r = 0; r < interp; r++) {
         uint32_t asum = 0; for (uint32_t i = r; i < ntaps; i += interp) asum += (uint32_t)abs((int)taps[i]);
-        if (asum > 65535u) return h->fail(SB200_E_INVALID, sum_msg);
+        if (asum > 65535u)
+            return h->fail(SB200_E_INVALID, interp == 1 ? "sum of |taps| must be at most 65535 (int32 sums must not wrap)"
+                                                        : "sum of |taps[k]| over k = r (mod interp) must be at most 65535 for every r (int32 sums must not wrap)");
     }
+    return SB200_OK;
+}
+// The lengths of a channelizer: n_in at most 2^40, rows of n_out = ceil(interp n_in / decim) samples out_stride apart, out_stride at most
+// 2^40 and a multiple of 4.
+static int check_out_rows(sb200_handle* h, uint64_t n_in, uint32_t interp, uint32_t decim, uint64_t out_stride, uint64_t* n_out) {
+    if (n_in > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples must be at most 2^40");
+    *n_out = (interp * n_in + decim - 1) / decim;
+    if (out_stride < *n_out || (out_stride & 3u) || out_stride > (1ull << 40))
+        return h->fail(SB200_E_INVALID, "out_stride must be at least ceil(interp n_in / decim), at most 2^40 and a multiple of 4");
+    return SB200_OK;
+}
+// The lengths of a combiner: rows row_stride apart, row_stride at least n_in, at most 2^40 and a multiple of 4; n_in and n_out at most 2^40.
+static int check_in_rows(sb200_handle* h, uint64_t row_stride, uint64_t n_in, uint64_t n_out) {
+    if (row_stride < n_in || (row_stride & 3u) || row_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "row_stride must be at least n_in, at most 2^40 and a multiple of 4");
+    if (n_in > (1ull << 40) || n_out > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples and n_out_samples (interp n_in_samples) must be at most 2^40");
     return SB200_OK;
 }
 // The taps by branch for the rational-rate kernels: taps[r + U l] at t[r L + l].
@@ -104,6 +121,42 @@ static BrTaps branch_taps(const int16_t* taps, uint32_t ntaps, uint32_t U) {
     BrTaps T; memset(&T, 0, sizeof T); T.n = ntaps; T.u = U; T.L = (ntaps + U - 1) / U;
     for (uint32_t i = 0; i < ntaps; i++) T.t[(i % U) * T.L + i / U] = taps[i];
     return T;
+}
+// f(std::integral_constant<int, M>()) for a bank size M of 2 .. 64 (a power of two, checked by the caller): the kernels of bank_kernels.cuh
+// take M as a template parameter.
+template <class F>
+static void with_bank_size(uint32_t M, F f) {
+    switch (M) {
+        case 2:  f(std::integral_constant<int, 2>()); break;
+        case 4:  f(std::integral_constant<int, 4>()); break;
+        case 8:  f(std::integral_constant<int, 8>()); break;
+        case 16: f(std::integral_constant<int, 16>()); break;
+        case 32: f(std::integral_constant<int, 32>()); break;
+        default: f(std::integral_constant<int, 64>()); break;
+    }
+}
+
+// Residency and staging of the channelizers (channelize_call, sb200_channelize_bank), after their own checks: a host capture goes up into
+// the workspace, a host `out` is bound to the workspace with rows n_out (rounded to 4) apart, copied into the caller's rows at the end;
+// then launch(st, d_in, d_out, d_stride) launches the kernel between ev0 and finish_call.
+template <class Launch>
+static int channelize_run(sb200_handle* h, const int16_t* iq, uint64_t n_in, uint32_t nrows, int16_t* out, uint64_t out_stride, uint64_t n_out,
+                          void* cuda_stream, Launch launch) {
+    cudaStream_t st = (cudaStream_t)cuda_stream;
+    CK(cudaSetDevice(h->device));
+    const bool in_dev = is_device_ptr(iq), out_dev = is_device_ptr(out);
+    if ((in_dev && ((uintptr_t)iq & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device input and output must be 16-byte aligned");
+    CallScope call(h, st); CK(call.begin()); call.reads(iq);
+    const int nrc = upload_nco(h);
+    if (nrc != SB200_OK) return nrc;
+    const uint32_t* d_in; uint32_t* d_out = (uint32_t*)out; uint64_t d_stride = out_stride; Returns ret;
+    CK(to_device(h->iq, (const uint32_t*)iq, in_dev, n_in * 4ull, st, &d_in, 16));
+    if (!out_dev) {
+        d_stride = (n_out + 3u) & ~3ull; CK(h->iq40.need(nrows * d_stride * 4ull)); d_out = (uint32_t*)h->iq40.p;
+        ret.bind2d(out, out_stride * 4ull, d_out, d_stride * 4ull, n_out * 4ull, nrows);
+    }
+    const int rc = launch(st, d_in, d_out, d_stride);
+    return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
 }
 
 // Wideband channelizer (fir_kernels.cuh): every channel shifted by its NCO, filtered and decimated by `decim`; channel c in row c of `out`.
@@ -116,35 +169,19 @@ static int channelize_call(sb200_handle* h, const int16_t* iq, uint64_t n_in, co
     if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
     if (!rational && (decim < 1 || decim > SB_CH_MAXDECIM)) return h->fail(SB200_E_INVALID, "decim must be 1 .. 16");
     int rc = rational ? check_rate_pair(h, interp, decim, "interp must be 1 .. 16", "decim must be interp .. 64") : SB200_OK;
-    if (rc == SB200_OK) rc = check_taps(h, taps, ntaps, interp, interp * SB_CH_MAXTAPS,   // no limit on ntaps beyond the branch length
-                                        rational ? "ntaps must be odd and ceil(ntaps / interp) at most 255" : "ntaps must be odd and at most 255",
-                                        interp == 1 ? "sum of |taps| must be at most 65535 (the int32 accumulator must not wrap)"
-                                                    : "sum of |taps[k]| over k = r (mod interp) must be at most 65535 for every r (the int32 accumulator must not wrap)");
     if (rc != SB200_OK) return rc;
-    if (n_in > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples must be at most 2^40");
-    const uint64_t n_out = (interp * n_in + decim - 1) / decim;
-    if (out_stride < n_out || (out_stride & 3u) || out_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "out_stride must be at least ceil(interp n_in / decim), at most 2^40 and a multiple of 4");
+    if ((ntaps & 1u) == 0 || ntaps > interp * SB_CH_MAXTAPS)       // no limit on ntaps beyond the branch length
+        return h->fail(SB200_E_INVALID, rational ? "ntaps must be odd and ceil(ntaps / interp) at most 255" : "ntaps must be odd and at most 255");
+    uint64_t n_out;
+    if ((rc = check_tap_sums(h, taps, ntaps, interp)) != SB200_OK || (rc = check_out_rows(h, n_in, interp, decim, out_stride, &n_out)) != SB200_OK) return rc;
     if (n_in == 0) return SB200_OK;
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    CK(cudaSetDevice(h->device));
-    const bool in_dev = is_device_ptr(iq), out_dev = is_device_ptr(out);
-    if ((in_dev && ((uintptr_t)iq & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device input and output must be 16-byte aligned");
-    CallScope call(h, st); CK(call.begin()); call.reads(iq);
-    const int nrc = upload_nco(h);
-    if (nrc != SB200_OK) return nrc;
-    const uint32_t* d_in; uint32_t* d_out = (uint32_t*)out; uint64_t d_stride = out_stride; Returns ret;
-    CK(to_device(h->iq, (const uint32_t*)iq, in_dev, n_in * 4ull, st, &d_in, 16));
-    if (!out_dev) {                                    // rows n_out (rounded to 4) apart in the workspace, copied into the caller's rows
-        d_stride = (n_out + 3u) & ~3ull; CK(h->iq40.need(nchannels * d_stride * 4ull)); d_out = (uint32_t*)h->iq40.p;
-        ret.bind2d(out, out_stride * 4ull, d_out, d_stride * 4ull, n_out * 4ull, nchannels);
-    }
-    ChChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
-    for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; }
-    if (interp == 1) {
+    return channelize_run(h, iq, n_in, nchannels, out, out_stride, n_out, cuda_stream, [&](cudaStream_t st, const uint32_t* d_in, uint32_t* d_out, uint64_t d_stride) {
+        ChChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
+        for (uint32_t i = 0; i < nchannels; i++) { ch.inc[i] = channels[i].phase_inc; ch.phase0[i] = channels[i].phase0; }
+        if (interp > 1) return channelize_launch(h, st, d_in, n_in, ch, decim, branch_taps(taps, ntaps, interp), d_out, d_stride, n_out);
         ChTaps T; memset(&T, 0, sizeof T); T.n = ntaps; for (uint32_t i = 0; i < ntaps; i++) T.t[i] = taps[i];
-        rc = channelize_launch(h, st, d_in, n_in, ch, decim, T, d_out, d_stride, n_out);
-    } else rc = channelize_launch(h, st, d_in, n_in, ch, decim, branch_taps(taps, ntaps, interp), d_out, d_stride, n_out);
-    return rc != SB200_OK ? rc : finish_call(h, st, ret, 0, 1);
+        return channelize_launch(h, st, d_in, n_in, ch, decim, T, d_out, d_stride, n_out);
+    });
 }
 extern "C" int sb200_channelize(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels, uint32_t decim,
                                 const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
@@ -157,12 +194,7 @@ extern "C" int sb200_channelize_rational(sb200_handle* h, const int16_t* iq, uin
 }
 
 // Polyphase filter-bank channelizer (bank_kernels.cuh): all M = nchannels channels of the uniform grid centred at (k + odd / 2) fs / M,
-// filtered and decimated by `decim`, in one launch; channel k in row k of `out`.  Staging and residency as in channelize_call.
-template <int M>
-static void bank_launch(cudaStream_t st, uint64_t tiles, const uint32_t* d_in, uint64_t n_in, const uint32_t* nco, uint32_t D, uint32_t odd,
-                        const BrTaps& T, uint32_t* d_out, uint64_t stride, uint64_t n_out) {
-    k_channelize_bank<M><<<(unsigned)tiles, SB_FIR_THREADS, 0, st>>>(d_in, n_in, nco, D, odd, T, d_out, stride, n_out);
-}
+// filtered and decimated by `decim`, in one launch; channel k in row k of `out`.
 extern "C" int sb200_channelize_bank(sb200_handle* h, const int16_t* iq, uint64_t n_in, uint32_t nchannels, uint32_t decim, uint32_t odd_stacking,
                                      const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride, void* cuda_stream) {
     if (!h) return SB200_E_INVALID;
@@ -172,58 +204,40 @@ extern "C" int sb200_channelize_bank(sb200_handle* h, const int16_t* iq, uint64_
     if (D < 1 || M % D) return h->fail(SB200_E_INVALID, "decim must divide nchannels");
     if (odd_stacking > 1u) return h->fail(SB200_E_INVALID, "odd_stacking must be 0 or 1");
     if ((ntaps & 1u) == 0 || ntaps > SB_BK_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be odd and at most 1023");
-    uint32_t asum = 0; for (uint32_t i = 0; i < ntaps; i++) asum += (uint32_t)abs((int)taps[i]);
-    if (asum > 65535u) return h->fail(SB200_E_INVALID, "sum of |taps| must be at most 65535 (every branch sum and butterfly must fit int32)");
-    if (n_in > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples must be at most 2^40");
-    const uint64_t n_out = (n_in + D - 1) / D;
-    if (out_stride < n_out || (out_stride & 3u) || out_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "out_stride must be at least ceil(n_in / decim), at most 2^40 and a multiple of 4");
+    uint64_t n_out; int rc;
+    if ((rc = check_tap_sums(h, taps, ntaps, 1)) != SB200_OK || (rc = check_out_rows(h, n_in, 1, D, out_stride, &n_out)) != SB200_OK) return rc;
     if (n_in == 0) return SB200_OK;
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    CK(cudaSetDevice(h->device));
-    const bool in_dev = is_device_ptr(iq), out_dev = is_device_ptr(out);
-    if ((in_dev && ((uintptr_t)iq & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device input and output must be 16-byte aligned");
-    CallScope call(h, st); CK(call.begin()); call.reads(iq);
-    const int nrc = upload_nco(h);
-    if (nrc != SB200_OK) return nrc;
-    const uint32_t* d_in; uint32_t* d_out = (uint32_t*)out; uint64_t d_stride = out_stride; Returns ret;
-    CK(to_device(h->iq, (const uint32_t*)iq, in_dev, n_in * 4ull, st, &d_in, 16));
-    if (!out_dev) {                                    // rows n_out (rounded to 4) apart in the workspace, copied into the caller's rows
-        d_stride = (n_out + 3u) & ~3ull; CK(h->iq40.need(M * d_stride * 4ull)); d_out = (uint32_t*)h->iq40.p;
-        ret.bind2d(out, out_stride * 4ull, d_out, d_stride * 4ull, n_out * 4ull, M);
-    }
-    const BrTaps T = branch_taps(taps, ntaps, 1);      // the taps in their own order
-    const uint64_t tiles = (n_in + SB_FIR_TILE - 1) / SB_FIR_TILE;
-    const uint32_t* nco = (const uint32_t*)h->nco.p;
-    CK(cudaEventRecord(h->ev0, st));
-    switch (M) {
-        case 2:  bank_launch<2>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
-        case 4:  bank_launch<4>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
-        case 8:  bank_launch<8>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
-        case 16: bank_launch<16>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
-        case 32: bank_launch<32>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
-        default: bank_launch<64>(st, tiles, d_in, n_in, nco, D, odd_stacking, T, d_out, d_stride, n_out); break;
-    }
-    return finish_call(h, st, ret, 0, 1);
+    return channelize_run(h, iq, n_in, M, out, out_stride, n_out, cuda_stream, [&](cudaStream_t st, const uint32_t* d_in, uint32_t* d_out, uint64_t d_stride) {
+        const BrTaps T = branch_taps(taps, ntaps, 1);  // the taps in their own order
+        CK(cudaEventRecord(h->ev0, st));
+        with_bank_size(M, [&](auto m) {
+            k_channelize_bank<decltype(m)::value><<<(unsigned)((n_in + SB_FIR_TILE - 1) / SB_FIR_TILE), SB_FIR_THREADS, 0, st>>>(
+                d_in, n_in, (const uint32_t*)h->nco.p, D, odd_stacking, T, d_out, d_stride, n_out);
+        });
+        return SB200_OK;
+    });
+}
+
+// The grid of k_combine<J, true> and k_combine_bank<M>, which take tile x + gx y of `tiles`.  A tile holds at least 16 outputs (32 W J
+// per phase of k_combine, U 1024 / M of the bank), so n_out <= 2^40 gives at most 2^36 tiles: gy = ceil(tiles / (2^31 - 1)) <= 33 and
+// gx = ceil(tiles / gy) < 2^31 stay within the grid limits.
+static dim3 tile_grid(uint64_t tiles) {
+    const uint64_t gy = (tiles + 0x7FFFFFFEull) / 0x7FFFFFFFull, gx = (tiles + gy - 1) / gy;
+    return dim3((unsigned)gx, (unsigned)gy);
 }
 
 // One launch of k_combine<J, RAT> (fir_kernels.cuh) over device buffers, between ev0 and the caller's finish_call.  ChTaps launches the
-// sb200_combine specialisation (D = 1, eight warps per phase), BrTaps the rational one with W warps per phase; tiles of 32 W J outputs per
-// phase, on a grid of (tiles, 1) CTAs or, RAT, (gx, gy) with tile = x + gx y: n_out <= 2^40 and U TQ >= 32 give at most 2^35 tiles,
-// so gy = ceil(tiles / (2^31 - 1)) <= 16 and gx = ceil(tiles / gy) < 2^31 stay within the grid limits.
+// sb200_combine specialisation (D = 1, eight warps per phase, tile = x), BrTaps the rational one with W warps per phase on tile_grid;
+// tiles of 32 W J outputs per phase.
 template <int J, class Taps>
 static int combine_launch_j(sb200_handle* h, cudaStream_t st, const uint32_t* d_in, uint64_t stride, uint64_t n_in, const CbChannels& ch, uint32_t U,
                             uint32_t D, uint32_t W, const Taps& T, uint32_t* d_out, uint64_t n_out, uint32_t accumulate) {
     constexpr bool RAT = std::is_same<Taps, BrTaps>::value;
-    const uint32_t bit = 1u << (J + (RAT ? 16 : 0));
-    if (!(h->cb_smem_set & bit)) {
-        CK(cudaFuncSetAttribute(k_combine<J, RAT>, cudaFuncAttributeMaxDynamicSharedMemorySize, RAT ? SB_CBR_SMEM_MAX : SB_CB_SMEM));
-        h->cb_smem_set |= bit;
-    }
+    CK(smem_once(h->cb_smem_set, 1u << (J + (RAT ? 16 : 0)), k_combine<J, RAT>, RAT ? SB_CBR_SMEM_MAX : SB_CB_SMEM));
     const uint64_t tq = 32ull * W * J, tiles = (n_out + U * tq - 1) / (U * tq);
-    const uint64_t gy = RAT ? (tiles + 0x7FFFFFFEull) / 0x7FFFFFFFull : 1u, gx = (tiles + gy - 1) / gy;
     const uint32_t smem = RAT ? combine_smem_r(ch.n, U, D, T.n, (uint32_t)tq) : combine_smem(ch.n, U, T.n, (uint32_t)tq);
     CK(cudaEventRecord(h->ev0, st));
-    k_combine<J, RAT><<<dim3((unsigned)gx, (unsigned)gy), SB_FIR_THREADS, smem, st>>>(d_in, stride, n_in, (const uint32_t*)h->nco.p, ch, U, D, W, T, d_out, n_out, accumulate);
+    k_combine<J, RAT><<<RAT ? tile_grid(tiles) : dim3((unsigned)tiles), SB_FIR_THREADS, smem, st>>>(d_in, stride, n_in, (const uint32_t*)h->nco.p, ch, U, D, W, T, d_out, n_out, accumulate);
     return SB200_OK;
 }
 
@@ -264,21 +278,15 @@ static int combine_call(sb200_handle* h, const int16_t* rows, uint64_t row_strid
     if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
     if (!rational && (interp < 1 || interp > SB_CH_MAXDECIM)) return h->fail(SB200_E_INVALID, "interp must be 1 .. 16");
     int rc = rational ? check_rate_pair(h, decim, interp, "decim must be 1 .. 16", "interp must be decim .. 64") : SB200_OK;
-    if (rc == SB200_OK) rc = check_taps(h, taps, ntaps, interp, rational ? SB_CBR_MAXTAPS : SB_CH_MAXTAPS,
-                                        rational ? "ntaps must be odd, at most 4095 and ceil(ntaps / interp) at most 255" : "ntaps must be odd and at most 255",
-                                        "sum of |taps[j]| over j = r (mod interp) must be at most 65535 for every r (the int32 accumulator must not wrap)");
     if (rc != SB200_OK) return rc;
+    if ((ntaps & 1u) == 0 || ntaps > (rational ? SB_CBR_MAXTAPS : SB_CH_MAXTAPS) || (ntaps + interp - 1) / interp > SB_CH_MAXTAPS)
+        return h->fail(SB200_E_INVALID, rational ? "ntaps must be odd, at most 4095 and ceil(ntaps / interp) at most 255" : "ntaps must be odd and at most 255");
+    if ((rc = check_tap_sums(h, taps, ntaps, interp)) != SB200_OK) return rc;
     if (accumulate > 1u) return h->fail(SB200_E_INVALID, "accumulate must be 0 or 1");
     for (uint32_t i = 0; i < nchannels; i++)
         if (channels[i].gain > 65535u) return h->fail(SB200_E_INVALID, "gain must be at most 65535");
-    if (row_stride < n_in || (row_stride & 3u) || row_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "row_stride must be at least n_in, at most 2^40 and a multiple of 4");
-    if (!rational) {
-        if (n_in > (1ull << 40) / interp) return h->fail(SB200_E_INVALID, "interp * n_in_samples must be at most 2^40");
-        if (n_in == 0) return SB200_OK;
-    } else {
-        if (n_in > (1ull << 40) || n_out > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples and n_out_samples must be at most 2^40");
-        if (n_out == 0) return SB200_OK;
-    }
+    if ((rc = check_in_rows(h, row_stride, n_in, n_out)) != SB200_OK) return rc;
+    if (n_out == 0) return SB200_OK;
     return combine_run(h, rows, row_stride, n_in, nchannels, out, n_out, accumulate, cuda_stream,
                        [&](cudaStream_t st, const uint32_t* d_in, uint64_t d_stride, uint32_t* d_out) {
         CbChannels ch; memset(&ch, 0, sizeof ch); ch.n = nchannels;
@@ -312,15 +320,8 @@ extern "C" int sb200_combine_rational(sb200_handle* h, const int16_t* rows, uint
 }
 
 // Polyphase filter-bank combiner (bank_kernels.cuh): the M = nchannels rows onto the uniform grid centred at (k + odd / 2) fs / M,
-// interpolated by `interp`, summed into n_out outputs (added onto out's samples when `accumulate`) in one launch.  Residency and staging
-// as in combine_call; tiles of U 1024 / M outputs on a grid of (gx, gy) as combine_launch_j's: n_out <= 2^40 gives at most 2^36 tiles.
-template <int M>
-static void combine_bank_launch(cudaStream_t st, uint64_t n_out, const uint32_t* d_in, uint64_t stride, uint64_t n_in, const uint32_t* nco, uint32_t U,
-                                uint32_t odd, const BrTaps& T, uint32_t* d_out, uint32_t accumulate) {
-    const uint64_t to = U * (SB_CBK_SPAN / M), tiles = (n_out + to - 1) / to;
-    const uint64_t gy = (tiles + 0x7FFFFFFEull) / 0x7FFFFFFFull, gx = (tiles + gy - 1) / gy;
-    k_combine_bank<M><<<dim3((unsigned)gx, (unsigned)gy), SB_FIR_THREADS, 0, st>>>(d_in, stride, n_in, nco, U, odd, T, d_out, n_out, accumulate);
-}
+// interpolated by `interp`, summed into n_out outputs (added onto out's samples when `accumulate`) in one launch, on tile_grid's grid of
+// tiles of U 1024 / M outputs.
 extern "C" int sb200_combine_bank(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, uint32_t nchannels, uint32_t interp,
                                   uint32_t odd_stacking, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t n_out, uint32_t accumulate,
                                   void* cuda_stream) {
@@ -333,22 +334,18 @@ extern "C" int sb200_combine_bank(sb200_handle* h, const int16_t* rows, uint64_t
     if ((ntaps & 1u) == 0 || ntaps > SB_BK_MAXTAPS || ntaps > 2 * SB_CBK_SPAN / M * U)
         return h->fail(SB200_E_INVALID, "ntaps must be odd, at most 1023 and at most 2048 interp / nchannels");
     if (accumulate > 1u) return h->fail(SB200_E_INVALID, "accumulate must be 0 or 1");
-    if (row_stride < n_in || (row_stride & 3u) || row_stride > (1ull << 40)) return h->fail(SB200_E_INVALID, "row_stride must be at least n_in, at most 2^40 and a multiple of 4");
-    if (n_in > (1ull << 40) || n_out > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples and n_out_samples must be at most 2^40");
+    const int rc = check_in_rows(h, row_stride, n_in, n_out);
+    if (rc != SB200_OK) return rc;
     if (n_out == 0) return SB200_OK;
     return combine_run(h, rows, row_stride, n_in, M, out, n_out, accumulate, cuda_stream,
                        [&](cudaStream_t st, const uint32_t* d_in, uint64_t d_stride, uint32_t* d_out) {
         const BrTaps T = branch_taps(taps, ntaps, 1);  // the taps in their own order
-        const uint32_t* nco = (const uint32_t*)h->nco.p;
+        const uint64_t to = U * (SB_CBK_SPAN / M), tiles = (n_out + to - 1) / to;
         CK(cudaEventRecord(h->ev0, st));
-        switch (M) {
-            case 2:  combine_bank_launch<2>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
-            case 4:  combine_bank_launch<4>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
-            case 8:  combine_bank_launch<8>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
-            case 16: combine_bank_launch<16>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
-            case 32: combine_bank_launch<32>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
-            default: combine_bank_launch<64>(st, n_out, d_in, d_stride, n_in, nco, U, odd_stacking, T, d_out, accumulate); break;
-        }
+        with_bank_size(M, [&](auto m) {
+            k_combine_bank<decltype(m)::value><<<tile_grid(tiles), SB_FIR_THREADS, 0, st>>>(d_in, d_stride, n_in, (const uint32_t*)h->nco.p, U, odd_stacking, T,
+                                                                                           d_out, n_out, accumulate);
+        });
         return SB200_OK;
     });
 }
@@ -374,11 +371,8 @@ static int upload_simtab(sb200_handle* h) {
         for (int k = 0; k < 4; k++) t[SB_CH_NCO + 4 * p + k] = pack(mk(hv[2 * k], hv[2 * k + 1]));
     }
     for (int j = 0; j < SB_SIM_LNT; j++) t[SB_CH_NCO + SB_SIM_H + j] = (uint32_t)nearbyint(-log((2048.0 + j + 0.5) / 4096.0) * 16777216.0);
-    cudaError_t e = h->simtab.need(SB_SIM_TAB * 4);
-    if (e == cudaSuccess) e = cudaMemcpy(h->simtab.p, t.data(), SB_SIM_TAB * 4, cudaMemcpyHostToDevice);
-    if (e == cudaSuccess) e = cudaDeviceSynchronize();   // landed before a kernel on a non-blocking stream reads it (TableArena::upload)
-    if (e != cudaSuccess) { h->simtab.release(); return h->fail(SB200_E_CUDA, "channel simulator table upload", e); }
-    return SB200_OK;
+    TableArena ar; ar.add(t.data(), SB_SIM_TAB * 4);
+    return ar.upload(h, h->simtab, "cudaMalloc channel simulator table", "channel simulator table upload");
 }
 
 // Rows of length n at l * A + r * B (l < N, r < R) are pairwise disjoint: |dl A + dr B| >= n for every (dl, dr) != 0, |dl| < N, |dr| < R.
@@ -401,10 +395,7 @@ static bool rows_disjoint(uint64_t A, uint64_t B, uint32_t N, uint32_t R, uint64
 template <int J>
 static int sim_launch_j(sb200_handle* h, cudaStream_t st, SimArgs& a) {
     const uint32_t tm = SB_FIR_THREADS * J;
-    if (!(h->sim_smem_set & (1u << J))) {
-        CK(cudaFuncSetAttribute(k_channel_sim<J>, cudaFuncAttributeMaxDynamicSharedMemorySize, sim_smem(SB_SIM_MAXROWS, SB_SIM_MAXROWS, SB_SIM_MAXTAPS, tm)));
-        h->sim_smem_set |= 1u << J;
-    }
+    CK(smem_once(h->sim_smem_set, 1u << J, k_channel_sim<J>, sim_smem(SB_SIM_MAXROWS, SB_SIM_MAXROWS, SB_SIM_MAXTAPS, tm)));
     a.ntiles = (uint32_t)((a.n_out + tm - 1) / tm);
     CK(cudaEventRecord(h->ev0, st));
     k_channel_sim<J><<<(unsigned)((uint64_t)a.ntiles * a.nlinks), SB_FIR_THREADS, sim_smem(a.T, a.R, a.L, tm), st>>>(a);

@@ -5,11 +5,12 @@ device-resident, against the CPU oracle decoding the numpy-channelized streams."
 import ctypes as C
 import numpy as np, pytest
 import torch
-import oracle_py
 import wideband_inputs as W
+import wideband_device as WD
 from sora_b200 import api
 from test_gpu_abi_residency import _matrix, _each, _fill
-from test_cpu_channelize import (CCA_WIDE, TAPS_11A, TAPS_11B, _full_scale, channels_11a, channels_11b, channels_11n, decode_11a)
+from test_cpu_channelize import CCA_WIDE, TAPS_11A, TAPS_11B, _full_scale, channels_11a, channels_11b, channels_11n
+from wideband_device import GROUP_CH, DDC_INCS as INCS, ddc_channels as _channels, ddc_taps as _taps, sms as _sms
 
 pytestmark = pytest.mark.gpu
 V, U32, U64 = C.c_void_p, C.c_uint32, C.c_uint64
@@ -18,19 +19,6 @@ TILE = 4096
 @pytest.fixture(scope="module")
 def eng():
     return api.Engine(0)
-
-def _taps(n, seed, total=40000):
-    """n random Q15 taps, sum |t| = total (rounded down), the centre one largest."""
-    rng = np.random.default_rng(seed)
-    t = rng.integers(-1000, 1000, n).astype(np.float64); t[n // 2] = 5000.0
-    t = np.trunc(t * total / np.abs(t).sum())
-    return t.astype(np.int16)
-
-INCS = [0, 2 ** 30, 2 ** 31, W.phase_inc(-20e6, 160e6), W.phase_inc(-60e6, 160e6), W.phase_inc(25e6, 176e6), 0x9E3779B9, 3 * 2 ** 30]
-
-def _channels(k, seed):
-    rng = np.random.default_rng(seed)
-    return [(INCS[i % len(INCS)], int(rng.integers(0, 2 ** 32)) if i % 3 else 0) for i in range(k)]
 
 def _same(eng, x, ch, d, taps):
     got = eng.channelize(x, ch, d, taps); want = W.channelize(x, ch, d, taps)
@@ -65,18 +53,7 @@ def test_tap_sum_at_the_limit(eng):
     _same(eng, x, [(0, 0), (2 ** 30, 0), (2 ** 31, 0)], 2, t)
 
 
-# ---- long captures: several channels per CTA ----------------------------------------------------------------------------------------
-# The launch splits the channels into groups only until there are four CTAs per multiprocessor, so a capture of at least 4 x SMs tiles runs
-# every channel of the call in one CTA (the staged tile, the rotated buffer and the NCO table reused from channel to channel), and one of
-# G tiles with 4 x SMs / G < K splits them into groups of several.  Identity and rotating channels are mixed within a group, and most
-# increments are multiples of 2^29 (the channel plan of a 160 Msps capture), whose phases hit NCO[0] on every eighth sample.
-GROUP_CH = [(0, 0), (2 ** 29, 0), (W.phase_inc(-60e6, 160e6), 0), (2 ** 30, 0xDEADBEEF), (0, 0x000FFFFF), (2 ** 31, 0), (0x9E3779B9, 12345),
-            (3 * 2 ** 29, 1 << 29), (0, 1 << 20), (W.phase_inc(20e6, 160e6), 7), (W.phase_inc(-20e6, 160e6), 0), (0, 0), (5 * 2 ** 29, 0),
-            (W.phase_inc(25e6, 176e6), 0x80000000), (7 * 2 ** 29, 99), (2 ** 32 - 2 ** 30, 0)]
-
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
+# ---- long captures: several channels per CTA (GROUP_CH) -----------------------------------------------------------------------------
 def _long_case(eng, tiles, k, d, taps, seed):
     """A full-scale capture of `tiles` tiles plus 777 samples, channelized on the device; its first, middle and last outputs against
     the model (channelize_window)."""
@@ -148,68 +125,31 @@ def test_invalid_arguments_are_rejected(eng):
 # ---- end to end, device-resident ----------------------------------------------------------------------------------------------------
 def _dev_channelize(eng, x, fcs, fs, taps):
     """The capture on the device, channelized into device rows; returns (device rows [K, stride, 2], stride, n_out)."""
-    d_in = torch.from_numpy(np.ascontiguousarray(x)).cuda(); n = len(x); n_out = -(-n // 4); stride = (n_out + 3) // 4 * 4 + 64
-    d_out = torch.zeros((len(fcs), stride, 2), dtype=torch.int16, device="cuda")
+    d_in = torch.from_numpy(np.ascontiguousarray(x)).cuda(); n = len(x); n_out = -(-n // 4)
+    d_out = WD.dev_rows(len(fcs), n_out, 64); stride = d_out.shape[1]
     eng.channelize_raw(d_in.data_ptr(), n, [(W.phase_inc(f, fs), 0) for f in fcs], 4, taps, d_out.data_ptr(), stride)
     return d_out, stride, n_out
 
-def _tables(K, stride, n_out):
-    return np.arange(K, dtype=np.uint64) * stride, np.full(K, n_out, np.uint32)
-
 def test_wideband_11a_on_the_device():
-    iq, fcs, _ = W.capture_11a(); rows, _ = channels_11a(); K = len(fcs); M = 16; OUT = 4096
+    iq, fcs, _ = W.capture_11a(); rows, _ = channels_11a(); K = len(fcs)
     e = api.Engine(0, cca_pwr_threshold=CCA_WIDE)
     try:
         d, stride, n_out = _dev_channelize(e, iq, fcs, W.FS_11A_WIDE, TAPS_11A)
         assert (d[:, :n_out].cpu().numpy() == rows).all()
-        off, ln = _tables(K, stride, n_out)
-        res = np.zeros((K, M), api.RESULT_DTYPE); out = np.zeros((K, M, OUT), np.uint8); sidx = np.zeros((K, M), np.uint32); cnt = np.zeros(K, np.uint32)
-        e._check(e._lib.sb200_rx11a_streams(e._h, V(d.data_ptr()), U64(K * stride), V(off.ctypes.data), V(ln.ctypes.data), U32(K), U32(M), V(out.ctypes.data), U32(OUT),
-                                            V(res.ctypes.data), V(sidx.ctypes.data), V(cnt.ctypes.data), V(0)), "sb200_rx11a_streams")
+        got = WD.rx11a(e, d, stride, n_out, K)
     finally:
         e.close()
-    for c, (o, ob) in enumerate(decode_11a(rows)):
-        assert cnt[c] == len(o) and len(o) >= 3, (c, cnt[c], o)
-        r = res[c, :cnt[c]]
-        for k in ("status", "rate_kbps", "length", "crc32", "nsym", "cfo_est"): assert (r[k] == o[k]).all(), (c, k)
-        assert (sidx[c, :cnt[c]] == o["sample_index"]).all(), c
-        seg = np.diff(np.concatenate([[0], o["sample_index"].astype(np.int64)]))       # the oracle counts 20 Msps vectors from the capture's start
-        assert (r["detect_index"] + np.concatenate([[0], np.cumsum(4 * (seg // 8))[:-1]]) == o["detect_index"]).all(), c
-        for i in range(len(o)):
-            L = int(o["length"][i]); assert (out[c, i, :L] == ob[i, :L]).all(), (c, i)
+    for c, (o, _) in enumerate(WD.equal_11a(rows, got)): assert len(o) >= 3, (c, o)
 
 def test_wideband_11b_on_the_device(eng):
-    iq, fcs, _ = W.capture_11b(); rows, _ = channels_11b(); K = len(fcs); M = 16; OUT = 4096
+    iq, fcs, _ = W.capture_11b(); rows, _ = channels_11b(); K = len(fcs)
     d, stride, n_out = _dev_channelize(eng, iq, fcs, W.FS_11B_WIDE, TAPS_11B)
     assert (d[:, :n_out].cpu().numpy() == rows).all()
-    off, ln = _tables(K, stride, n_out)
-    res = np.zeros((K, M), api.RESULT11B_DTYPE); out = np.zeros((K, M, OUT), np.uint8); cnt = np.zeros(K, np.uint32)
-    eng._check(eng._lib.sb200_rx11b_streams(eng._h, V(d.data_ptr()), U64(K * stride), V(off.ctypes.data), V(ln.ctypes.data), U32(K), U32(M), V(out.ctypes.data), U32(OUT),
-                                            V(res.ctypes.data), V(cnt.ctypes.data), V(0)), "sb200_rx11b_streams")
-    for c in range(K):
-        o, ob = oracle_py.rx11b_run(rows[c], max_frames=M, out_stride=OUT)
-        assert cnt[c] == len(o) and len(o) >= 2, (c, cnt[c], o)
-        r = res[c, :cnt[c]]
-        for k in ("status", "rate_kbps", "length", "crc32", "sample_index", "detect_vec"): assert (r[k] == o[k]).all(), (c, k)
-        for i in range(len(o)):
-            L = int(o["length"][i]) - 1; assert (out[c, i, :L] == ob[i, :L]).all(), (c, i)
+    for c, (o, _) in enumerate(WD.equal_11b(rows, WD.rx11b(eng, d, stride, n_out, K))): assert len(o) >= 2, (c, o)
 
 def test_wideband_11n_on_the_device(eng):
-    (a0, a1), fcs, _ = W.capture_11n(); r0, r1, _ = channels_11n(); K = len(fcs); M = 16; OUT = 1536
+    (a0, a1), fcs, _ = W.capture_11n(); r0, r1, _ = channels_11n(); K = len(fcs)
     d0, stride, n_out = _dev_channelize(eng, a0, fcs, W.FS_11A_WIDE, TAPS_11A)
     d1, _, _ = _dev_channelize(eng, a1, fcs, W.FS_11A_WIDE, TAPS_11A)
     assert (d0[:, :n_out].cpu().numpy() == r0).all() and (d1[:, :n_out].cpu().numpy() == r1).all()
-    off, ln = _tables(K, stride, n_out)
-    res = np.zeros((K, M), api.RESULT11N_DTYPE); out = np.zeros((K, M, OUT), np.uint8); sidx = np.zeros((K, M), np.uint32); cnt = np.zeros(K, np.uint32)
-    eng._check(eng._lib.sb200_rx11n_streams(eng._h, V(d0.data_ptr()), V(d1.data_ptr()), U64(K * stride), V(off.ctypes.data), V(ln.ctypes.data), U32(K), U32(M),
-                                            V(out.ctypes.data), U32(OUT), V(res.ctypes.data), V(sidx.ctypes.data), V(cnt.ctypes.data), V(0)), "sb200_rx11n_streams")
-    for c in range(K):
-        o, ob = oracle_py.rx11n_run(r0[c], r1[c], max_frames=M, out_stride=OUT)
-        assert cnt[c] == len(o) and len(o) >= 2, (c, cnt[c], o)
-        vec_base = 0; prev = 0
-        for k in range(len(o)):
-            for f in ("status", "mcs", "length", "crc32", "nsym", "cfo_est", "lsig_length"): assert res[c, k][f] == o[k][f], (c, k, f)
-            assert sidx[c, k] == o[k]["sample_index"], (c, k)
-            assert vec_base + res[c, k]["detect_index"] == o[k]["detect_index"], (c, k)
-            vec_base += 4 * ((int(sidx[c, k]) - prev) // 8); prev = int(sidx[c, k])
-            L = int(o[k]["length"]); assert (out[c, k, :L] == ob[k, :L]).all(), (c, k)
+    for c, (o, _) in enumerate(WD.equal_11n(r0, r1, WD.rx11n(eng, d0, d1, stride, n_out, K))): assert len(o) >= 2, (c, o)

@@ -7,11 +7,13 @@ import numpy as np, pytest
 import torch
 import oracle_py
 import wideband_inputs as W
+import wideband_device as WD
 import bank_model as B
 from sora_b200 import api
 from test_gpu_abi_residency import _matrix, _each, _fill
-from test_cpu_channelize import CCA_WIDE, _full_scale, decode_11a
+from test_cpu_channelize import CCA_WIDE, _full_scale
 from test_cpu_channelize_bank import GRID, bank_rows_11a, bank_rows_11n, bank_rows_octet
+from wideband_device import ddc_taps as _taps
 
 pytestmark = pytest.mark.gpu
 V, U32, U64 = C.c_void_p, C.c_uint32, C.c_uint64
@@ -20,12 +22,6 @@ TILE = 4096
 @pytest.fixture(scope="module")
 def eng():
     return api.Engine(0)
-
-def _taps(n, seed, total=40000):
-    """n random Q15 taps, sum |t| = total (rounded down), the centre one largest."""
-    rng = np.random.default_rng(seed)
-    t = rng.integers(-1000, 1000, n).astype(np.float64); t[n // 2] = 5000.0
-    return np.trunc(t * total / np.abs(t).sum()).astype(np.int16)
 
 def _same(eng, x, M, D, odd, taps):
     got = eng.channelize_bank(x, M, D, taps, odd=odd); want = B.bank(x, M, D, odd, taps)
@@ -62,13 +58,10 @@ def test_tap_sum_at_the_limit(eng, M):
     for odd in (0, 1):
         _same(eng, x, M, min(M, 4), odd, t)
 
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
 @pytest.mark.parametrize("M,D,ntaps", [(8, 4, 255), (64, 64, 1023), (2, 1, 63)])
 def test_long_capture(eng, M, D, ntaps):
     """A capture of 4 x SMs tiles plus 777 samples, device-resident; its first, middle and last outputs against the model's windows."""
-    n = 4 * _sms() * TILE + 777; x = _full_scale(n, M + ntaps); taps = _taps(ntaps, M)
+    n = 4 * WD.sms() * TILE + 777; x = _full_scale(n, M + ntaps); taps = _taps(ntaps, M)
     n_out = -(-n // D); stride = (n_out + 3) // 4 * 4
     d_in = torch.from_numpy(x).cuda(); d_out = torch.zeros((M, stride, 2), dtype=torch.int16, device="cuda")
     for odd in (0, 1):
@@ -146,13 +139,10 @@ def test_against_the_device_channelizer(eng, M):
 # ---- end to end, device-resident ----------------------------------------------------------------------------------------------------
 def _dev_bank(eng, x, odd):
     """The capture on the device, taken apart by the M = 8, D = 4 bank into device rows; returns (rows [8, stride, 2], stride, n_out)."""
-    d_in = torch.from_numpy(np.ascontiguousarray(x)).cuda(); n = len(x); n_out = -(-n // 4); stride = (n_out + 3) // 4 * 4 + 64
-    d_out = torch.zeros((8, stride, 2), dtype=torch.int16, device="cuda")
+    d_in = torch.from_numpy(np.ascontiguousarray(x)).cuda(); n = len(x); n_out = -(-n // 4)
+    d_out = WD.dev_rows(8, n_out, 64); stride = d_out.shape[1]
     eng.channelize_bank_raw(d_in.data_ptr(), n, 8, 4, B.TAPS_BANK, d_out.data_ptr(), stride, odd=odd)
     return d_out, stride, n_out
-
-def _tables(K, stride, n_out):
-    return np.arange(K, dtype=np.uint64) * stride, np.full(K, n_out, np.uint32)
 
 @pytest.mark.parametrize("case", ["even", "odd"])
 def test_bank_11a_on_the_device(case):
@@ -160,44 +150,20 @@ def test_bank_11a_on_the_device(case):
     equal to the oracle decoding the model's rows, on every field, event position and delivered byte."""
     iq, fcs, _ = W.capture_11a() if case == "even" else B.capture_11a_octet()
     rows, want = bank_rows_11a() if case == "even" else bank_rows_octet()
-    K = 8; M = 16; OUT = 4096
     e = api.Engine(0, cca_pwr_threshold=CCA_WIDE)
     try:
         d, stride, n_out = _dev_bank(e, iq, case == "odd")
         assert (d[:, :n_out].cpu().numpy() == rows).all()
-        off, ln = _tables(K, stride, n_out)
-        res = np.zeros((K, M), api.RESULT_DTYPE); out = np.zeros((K, M, OUT), np.uint8); sidx = np.zeros((K, M), np.uint32); cnt = np.zeros(K, np.uint32)
-        e._check(e._lib.sb200_rx11a_streams(e._h, V(d.data_ptr()), U64(K * stride), V(off.ctypes.data), V(ln.ctypes.data), U32(K), U32(M), V(out.ctypes.data), U32(OUT),
-                                            V(res.ctypes.data), V(sidx.ctypes.data), V(cnt.ctypes.data), V(0)), "sb200_rx11a_streams")
+        got = WD.rx11a(e, d, stride, n_out, 8)
     finally:
         e.close()
-    for c, (o, ob) in enumerate(decode_11a(rows)):
-        assert cnt[c] == len(o), (c, cnt[c], o)
+    for c, (o, _) in enumerate(WD.equal_11a(rows, got)):
         assert sum((o["status"] == oracle_py.E_FRAME_OK)) == len(want.get(c, [])), c
-        r = res[c, :cnt[c]]
-        for k in ("status", "rate_kbps", "length", "crc32", "nsym", "cfo_est"): assert (r[k] == o[k]).all(), (c, k)
-        assert (sidx[c, :cnt[c]] == o["sample_index"]).all(), c
-        seg = np.diff(np.concatenate([[0], o["sample_index"].astype(np.int64)]))       # the oracle counts 20 Msps vectors from the capture's start
-        assert (r["detect_index"] + np.concatenate([[0], np.cumsum(4 * (seg // 8))[:-1]]).astype(np.int64) == o["detect_index"]).all(), c
-        for i in range(len(o)):
-            L = int(o["length"][i]); assert (out[c, i, :L] == ob[i, :L]).all(), (c, i)
 
 def test_bank_11n_on_the_device(eng):
-    (a0, a1), fcs, _ = W.capture_11n(); r0, r1, want = bank_rows_11n(); K = 8; M = 16; OUT = 1536
+    (a0, a1), fcs, _ = W.capture_11n(); r0, r1, want = bank_rows_11n()
     d0, stride, n_out = _dev_bank(eng, a0, False)
     d1, _, _ = _dev_bank(eng, a1, False)
     assert (d0[:, :n_out].cpu().numpy() == r0).all() and (d1[:, :n_out].cpu().numpy() == r1).all()
-    off, ln = _tables(K, stride, n_out)
-    res = np.zeros((K, M), api.RESULT11N_DTYPE); out = np.zeros((K, M, OUT), np.uint8); sidx = np.zeros((K, M), np.uint32); cnt = np.zeros(K, np.uint32)
-    eng._check(eng._lib.sb200_rx11n_streams(eng._h, V(d0.data_ptr()), V(d1.data_ptr()), U64(K * stride), V(off.ctypes.data), V(ln.ctypes.data), U32(K), U32(M),
-                                            V(out.ctypes.data), U32(OUT), V(res.ctypes.data), V(sidx.ctypes.data), V(cnt.ctypes.data), V(0)), "sb200_rx11n_streams")
-    for c in range(K):
-        o, ob = oracle_py.rx11n_run(r0[c], r1[c], max_frames=M, out_stride=OUT)
-        assert cnt[c] == len(o) and sum(o["status"] == oracle_py.E_FRAME_OK) == len(want.get(c, [])), (c, cnt[c], o)
-        vec_base = 0; prev = 0
-        for k in range(len(o)):
-            for f in ("status", "mcs", "length", "crc32", "nsym", "cfo_est", "lsig_length"): assert res[c, k][f] == o[k][f], (c, k, f)
-            assert sidx[c, k] == o[k]["sample_index"], (c, k)
-            assert vec_base + res[c, k]["detect_index"] == o[k]["detect_index"], (c, k)
-            vec_base += 4 * ((int(sidx[c, k]) - prev) // 8); prev = int(sidx[c, k])
-            L = int(o[k]["length"]); assert (out[c, k, :L] == ob[k, :L]).all(), (c, k)
+    for c, (o, _) in enumerate(WD.equal_11n(r0, r1, WD.rx11n(eng, d0, d1, stride, n_out, 8))):
+        assert sum(o["status"] == oracle_py.E_FRAME_OK) == len(want.get(c, [])), (c, o)

@@ -6,14 +6,14 @@ import ctypes as C
 from math import gcd
 import numpy as np, pytest
 import torch
-import oracle_py
 import wideband_inputs as W
+import wideband_device as WD
 import rational_model as R
 from sora_b200 import api
 from test_gpu_abi_residency import _matrix, _each, _fill
-from test_cpu_channelize import CCA_WIDE, _full_scale, decode_11a
+from test_cpu_channelize import CCA_WIDE, _full_scale
 from test_cpu_channelize_rational import PLANS, TAPS_160_44, rows_24ghz
-from test_gpu_channelize import GROUP_CH, INCS, _channels, _sms, _taps
+from wideband_device import GROUP_CH, DDC_INCS as INCS, ddc_channels as _channels, ddc_taps as _taps, sms as _sms
 
 pytestmark = pytest.mark.gpu
 V, U32, U64 = C.c_void_p, C.c_uint32, C.c_uint64
@@ -177,44 +177,26 @@ def test_invalid_arguments_are_rejected(eng):
 def test_24ghz_on_the_device(fs):
     """capture_24ghz on the device -> device channelizer (802.11b rows at 44 Msps, the OFDM row at 40 Msps) -> sb200_rx11b_streams and
     sb200_rx11a_streams, against the oracle on the model's rows: every field, event position and delivered byte; every PSDU delivered."""
-    iq, rows, ps = rows_24ghz(fs); (ub, db), tb, (ua, da), ta = PLANS[fs]; M = 16; OUT = 4096
+    iq, rows, ps = rows_24ghz(fs); (ub, db), tb, (ua, da), ta = PLANS[fs]
     e = api.Engine(0); ea = api.Engine(0, cca_pwr_threshold=CCA_WIDE)           # the OFDM receiver with the wideband carrier-sense threshold
     try:
         d_in = torch.from_numpy(np.ascontiguousarray(iq)).cuda(); n = len(iq)
         b_ch = [c for c, k in enumerate(R.KIND_24) if k == "11b"]; a_ch = [c for c, k in enumerate(R.KIND_24) if k == "ofdm"]
         def dev_rows(chans, u, d, t):
-            n_out = -(-u * n // d); stride = (n_out + 3) // 4 * 4 + 64
-            out = torch.zeros((len(chans), stride, 2), dtype=torch.int16, device="cuda")
+            n_out = -(-u * n // d); out = WD.dev_rows(len(chans), n_out, 64); stride = out.shape[1]
             e.channelize_raw(d_in.data_ptr(), n, [(W.phase_inc(R.CH_24[c], fs), 0) for c in chans], d, t, out.data_ptr(), stride, interp=u)
             return out, stride, n_out
         db_, sb, nb = dev_rows(b_ch, ub, db, tb); da_, sa, na = dev_rows(a_ch, ua, da, ta)
         for i, c in enumerate(b_ch): assert (db_[i, :nb].cpu().numpy() == rows[c]).all(), c
         for i, c in enumerate(a_ch): assert (da_[i, :na].cpu().numpy() == rows[c]).all(), c
-        Kb, Ka = len(b_ch), len(a_ch)
-        off = np.arange(Kb, dtype=np.uint64) * sb; ln = np.full(Kb, nb, np.uint32)
-        rb = np.zeros((Kb, M), api.RESULT11B_DTYPE); ob = np.zeros((Kb, M, OUT), np.uint8); cb = np.zeros(Kb, np.uint32)
-        e._check(e._lib.sb200_rx11b_streams(e._h, V(db_.data_ptr()), U64(Kb * sb), V(off.ctypes.data), V(ln.ctypes.data), U32(Kb), U32(M), V(ob.ctypes.data), U32(OUT),
-                                            V(rb.ctypes.data), V(cb.ctypes.data), V(0)), "sb200_rx11b_streams")
-        off = np.arange(Ka, dtype=np.uint64) * sa; ln = np.full(Ka, na, np.uint32)
-        ra = np.zeros((Ka, M), api.RESULT_DTYPE); oa = np.zeros((Ka, M, OUT), np.uint8); sidx = np.zeros((Ka, M), np.uint32); ca = np.zeros(Ka, np.uint32)
-        ea._check(ea._lib.sb200_rx11a_streams(ea._h, V(da_.data_ptr()), U64(Ka * sa), V(off.ctypes.data), V(ln.ctypes.data), U32(Ka), U32(M), V(oa.ctypes.data), U32(OUT),
-                                              V(ra.ctypes.data), V(sidx.ctypes.data), V(ca.ctypes.data), V(0)), "sb200_rx11a_streams")
+        got_b = WD.rx11b(e, db_, sb, nb, len(b_ch)); got_a = WD.rx11a(ea, da_, sa, na, len(a_ch))
     finally:
         e.close(); ea.close()
-    for i, c in enumerate(b_ch):
-        o, obo = oracle_py.rx11b_run(rows[c], max_frames=M, out_stride=OUT)
-        assert cb[i] == len(o) == len(ps[c]), (c, cb[i], len(o))
-        r = rb[i, :cb[i]]
-        for k in ("status", "rate_kbps", "length", "crc32", "sample_index", "detect_vec"): assert (r[k] == o[k]).all(), (c, k)
+    for i, (c, (o, _)) in enumerate(zip(b_ch, WD.equal_11b([rows[c] for c in b_ch], got_b))):
+        assert len(o) == len(ps[c]), (c, len(o))
         for j in range(len(o)):
-            L = int(o["length"][j]) - 1; assert (ob[i, j, :L] == obo[j, :L]).all() and bytes(ob[i, j, :L]) == bytes(ps[c][j][:-1]), (c, j)
-    for i, c in enumerate(a_ch):
-        (o, obo), = decode_11a([rows[c]])
-        assert ca[i] == len(o) == len(ps[c]), (c, ca[i], len(o))
-        r = ra[i, :ca[i]]
-        for k in ("status", "rate_kbps", "length", "crc32", "nsym", "cfo_est"): assert (r[k] == o[k]).all(), (c, k)
-        assert (sidx[i, :ca[i]] == o["sample_index"]).all(), c
-        seg = np.diff(np.concatenate([[0], o["sample_index"].astype(np.int64)]))
-        assert (r["detect_index"] + np.concatenate([[0], np.cumsum(4 * (seg // 8))[:-1]]) == o["detect_index"]).all(), c
+            L = int(o["length"][j]) - 1; assert bytes(got_b[1][i, j, :L]) == bytes(ps[c][j][:-1]), (c, j)
+    for i, (c, (o, _)) in enumerate(zip(a_ch, WD.equal_11a([rows[c] for c in a_ch], got_a))):
+        assert len(o) == len(ps[c]), (c, len(o))
         for j in range(len(o)):
-            L = int(o["length"][j]); assert (oa[i, j, :L] == obo[j, :L]).all() and bytes(oa[i, j, :L]) == bytes(ps[c][j]), (c, j)
+            L = int(o["length"][j]); assert bytes(got_a[1][i, j, :L]) == bytes(ps[c][j]), (c, j)

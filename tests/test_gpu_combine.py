@@ -7,11 +7,13 @@ import numpy as np, pytest
 import torch
 import oracle_py
 import wideband_inputs as W
+import wideband_device as WD
 import combine_model as CM
 from sora_b200 import api
 from test_gpu_abi_residency import _matrix, _each, _fill
-from test_cpu_channelize import CCA_WIDE, TAPS_11A, TAPS_11B, _full_scale, decode_11a
+from test_cpu_channelize import CCA_WIDE, TAPS_11A, TAPS_11B
 from test_cpu_combine import TAPS_UP, TAPS_UP_11B, GAIN_11A, frames_11a, frames_11b, frames_11n, wide_11a, wide_11b, wide_11n
+from wideband_device import GAINS, DUC_INCS as INCS, duc_channels as _channels, duc_rows as _rows, duc_taps as _taps, sms as _sms
 
 pytestmark = pytest.mark.gpu
 V, U32, U64 = C.c_void_p, C.c_uint32, C.c_uint64
@@ -26,23 +28,6 @@ def _tile(K, U, ntaps):
     for ti in (1024, 512):
         if (K * (ti + 2 * halo) + U * ti + 4096) * 4 + 16 <= 51200: return ti
     return 256
-
-def _taps(n, U, seed, total=50000):
-    """n random Q15 taps, the centre one largest, every branch j = r (mod U) with sum |t| <= total."""
-    rng = np.random.default_rng(seed)
-    t = rng.integers(-1000, 1000, n).astype(np.float64); t[n // 2] = 5000.0
-    worst = max(np.abs(t[r::U]).sum() for r in range(min(U, n)))
-    return np.trunc(t * min(total / worst, 32767 / 5000)).astype(np.int16)
-
-INCS = [0, 2 ** 30, 2 ** 31, 3 * 2 ** 30, W.phase_inc(-20e6, 160e6), W.phase_inc(-60e6, 160e6), W.phase_inc(25e6, 176e6), 0x9E3779B9]
-GAINS = [4096, 0, 65535, 4096, 1, 30000, 4096, 8191]
-
-def _channels(k, seed):
-    rng = np.random.default_rng(seed)
-    return [(INCS[i % len(INCS)], int(rng.integers(0, 2 ** 32)) if i % 3 else 0, GAINS[(i + seed) % len(GAINS)]) for i in range(k)]
-
-def _rows(k, n, seed):
-    return np.stack([_full_scale(n, seed + 1000 * i) for i in range(k)])
 
 def _same(eng, rows, ch, u, taps):
     got = eng.combine(rows, ch, u, taps); want = CM.combine(rows, ch, u, taps)
@@ -81,9 +66,6 @@ def test_the_limits_at_once(eng):
 
 
 # ---- long captures --------------------------------------------------------------------------------------------------------------------
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
 @pytest.mark.parametrize("K,U,ntaps", [(4, 4, 127), (16, 16, 255), (7, 1, 255), (16, 3, 101), (2, 15, 253)])
 def test_long_captures(eng, K, U, ntaps):
     """At least 4 x SMs tiles plus 777 samples, on the device; the first, middle and last outputs against combine_window."""
@@ -160,121 +142,57 @@ def test_invalid_arguments_are_rejected(eng):
 
 
 # ---- end to end, device-resident: transmitter -> combiner -> channelizer -> stream receivers -------------------------------------------
-def _ceil4(n):
-    return (n + 3) // 4 * 4
-
-def _dev_rows(K, n):
-    return torch.zeros((K, _ceil4(n), 2), dtype=torch.int16, device="cuda")
-
-def _tx11a(eng, mpdu, rate, seed):
-    """One frame of k_tx11a into device memory -> int8 [ns, 2] device tensor."""
-    flat, offs, lens = api._payload_table([mpdu]); sd = np.array([seed], np.uint8); ns = np.zeros(1, np.uint32)
-    stride = 640 + 160 * (2 + -(-(len(mpdu) + 7) * 8 // api._NDBPS_11A[rate]) + 1) + 32
-    out = torch.zeros((1, stride, 2), dtype=torch.int8, device="cuda")
-    eng.tx11a_raw(api._ptr(flat), flat.size, api._ptr(offs), api._ptr(lens), api._ptr(sd), 1, rate, 0, 8, out.data_ptr(), stride, api._ptr(ns))
-    return out[0, :int(ns[0])]
-
-def _tx11b(eng, mpdu, rate):
-    flat, offs, lens = api._payload_table([mpdu]); ns = np.zeros(1, np.uint32)
-    cpb = {1000: 88, 2000: 44, 5500: 16, 11000: 8}[rate]; stride = ((24 * 88 + (len(mpdu) + 4) * cpb + 5) * 4 + 15) // 8 * 8
-    out = torch.zeros((1, stride, 2), dtype=torch.int8, device="cuda")
-    eng.tx11b_raw(api._ptr(flat), flat.size, api._ptr(offs), api._ptr(lens), 1, rate, 0, 0, 8, out.data_ptr(), stride, api._ptr(ns))
-    return out[0, :int(ns[0])]
-
-def _tx11n(eng, mpdu, mcs, seed):
-    flat, offs, lens = api._payload_table([mpdu]); sd = np.array([seed], np.uint8); ns = np.zeros(1, np.uint32)
-    stride = 1600 + 160 * (-(-((len(mpdu) + 4) * 8 + 22) // {8: 52, 9: 104, 10: 156}[mcs]) + 1)
-    o0 = torch.zeros((1, stride, 2), dtype=torch.int16, device="cuda"); o1 = torch.zeros_like(o0)
-    eng.tx11n_raw(api._ptr(flat), flat.size, api._ptr(offs), api._ptr(lens), api._ptr(sd), 1, mcs, 0, o0.data_ptr(), o1.data_ptr(), stride, api._ptr(ns))
-    return o0[0, :int(ns[0])], o1[0, :int(ns[0])]
-
 def _dev_chain(eng, rows, n, ch, taps_up, taps_down):
     """rows (device [K, stride, 2]) -> combined on the device (interp 4) -> channelized (decim 4) into device rows; returns (y, rows, stride)."""
     K = len(ch); y = torch.zeros((4 * n, 2), dtype=torch.int16, device="cuda")
     eng.combine_raw(rows.data_ptr(), rows.shape[1], n, ch, 4, taps_up, y.data_ptr())
-    stride = _ceil4(n) + 64; back = torch.zeros((K, stride, 2), dtype=torch.int16, device="cuda")
+    back = WD.dev_rows(K, n, 64); stride = back.shape[1]
     eng.channelize_raw(y.data_ptr(), 4 * n, [(a, b) for a, b, _ in ch], 4, taps_down, back.data_ptr(), stride)
     return y, back, stride
 
-def _tables(K, stride, n):
-    return np.arange(K, dtype=np.uint64) * stride, np.full(K, n, np.uint32)
-
 def test_round_trip_11a_on_the_device():
-    rows_h, mpdus, plan = frames_11a(); K, n = rows_h.shape[:2]; M = 16; OUT = 4096
+    rows_h, mpdus, plan = frames_11a(); K, n = rows_h.shape[:2]
     y_h, back_h, _ = wide_11a()
     ch = [(W.phase_inc(f, W.FS_11A_WIDE), 0, g) for f, g in zip(W.CH_11A, GAIN_11A)]
     e = api.Engine(0, cca_pwr_threshold=CCA_WIDE)
     try:
-        rows = _dev_rows(K, n)
+        rows = WD.dev_rows(K, n)
         for c, pl in enumerate(plan):
             for (t, rate, seed), m in zip(pl, mpdus[c]):
-                f = _tx11a(e, m, rate, seed); rows[c, t:t + len(f)] = f.to(torch.int16) * 20
+                f = WD.tx11a(e, m, rate, seed); rows[c, t:t + len(f)] = f.to(torch.int16) * 20
         assert (rows[:, :n].cpu().numpy() == rows_h).all()
         y, back, stride = _dev_chain(e, rows, n, ch, TAPS_UP, TAPS_11A)
         assert (y.cpu().numpy() == y_h).all() and (back[:, :n].cpu().numpy() == back_h).all()
-        off, ln = _tables(K, stride, n)
-        res = np.zeros((K, M), api.RESULT_DTYPE); out = np.zeros((K, M, OUT), np.uint8); sidx = np.zeros((K, M), np.uint32); cnt = np.zeros(K, np.uint32)
-        e._check(e._lib.sb200_rx11a_streams(e._h, V(back.data_ptr()), U64(K * stride), V(off.ctypes.data), V(ln.ctypes.data), U32(K), U32(M), V(out.ctypes.data), U32(OUT),
-                                            V(res.ctypes.data), V(sidx.ctypes.data), V(cnt.ctypes.data), V(0)), "sb200_rx11a_streams")
+        got = WD.rx11a(e, back, stride, n, K)
     finally:
         e.close()
-    for c, (o, ob) in enumerate(decode_11a(back_h)):
-        assert cnt[c] == len(o) == 3 and (o["status"] == oracle_py.E_FRAME_OK).all(), (c, cnt[c], o)
-        r = res[c, :cnt[c]]
-        for k in ("status", "rate_kbps", "length", "crc32", "nsym", "cfo_est"): assert (r[k] == o[k]).all(), (c, k)
-        assert (sidx[c, :cnt[c]] == o["sample_index"]).all(), c
-        seg = np.diff(np.concatenate([[0], o["sample_index"].astype(np.int64)]))       # the oracle counts 20 Msps vectors from the capture's start
-        assert (r["detect_index"] + np.concatenate([[0], np.cumsum(4 * (seg // 8))[:-1]]) == o["detect_index"]).all(), c
-        for i in range(len(o)):
-            L = int(o["length"][i]); assert (out[c, i, :L] == ob[i, :L]).all(), (c, i)
+    for c, (o, _) in enumerate(WD.equal_11a(back_h, got)):
+        assert len(o) == 3 and (o["status"] == oracle_py.E_FRAME_OK).all(), (c, o)
 
 def test_round_trip_11b_on_the_device(eng):
-    rows_h, mpdus, plan = frames_11b(); K, n = rows_h.shape[:2]; M = 16; OUT = 4096
+    rows_h, mpdus, plan = frames_11b(); K, n = rows_h.shape[:2]
     y_h, back_h, _ = wide_11b()
     ch = [(W.phase_inc(f, W.FS_11B_WIDE), 0, 4096) for f in W.CH_11B]
-    rows = _dev_rows(K, n)
+    rows = WD.dev_rows(K, n)
     for c, pl in enumerate(plan):
         for (t, rate), m in zip(pl, mpdus[c]):
-            f = _tx11b(eng, m, rate); rows[c, t:t + len(f)] = f.to(torch.int16) * 64
+            f = WD.tx11b(eng, m, rate); rows[c, t:t + len(f)] = f.to(torch.int16) * 64
     assert (rows[:, :n].cpu().numpy() == rows_h).all()
     y, back, stride = _dev_chain(eng, rows, n, ch, TAPS_UP_11B, TAPS_11B)
     assert (y.cpu().numpy() == y_h).all() and (back[:, :n].cpu().numpy() == back_h).all()
-    off, ln = _tables(K, stride, n)
-    res = np.zeros((K, M), api.RESULT11B_DTYPE); out = np.zeros((K, M, OUT), np.uint8); cnt = np.zeros(K, np.uint32)
-    eng._check(eng._lib.sb200_rx11b_streams(eng._h, V(back.data_ptr()), U64(K * stride), V(off.ctypes.data), V(ln.ctypes.data), U32(K), U32(M), V(out.ctypes.data), U32(OUT),
-                                            V(res.ctypes.data), V(cnt.ctypes.data), V(0)), "sb200_rx11b_streams")
-    for c in range(K):
-        o, ob = oracle_py.rx11b_run(back_h[c], max_frames=M, out_stride=OUT)
-        assert cnt[c] == len(o) == 2, (c, cnt[c], o)
-        r = res[c, :cnt[c]]
-        for k in ("status", "rate_kbps", "length", "crc32", "sample_index", "detect_vec"): assert (r[k] == o[k]).all(), (c, k)
-        for i in range(len(o)):
-            L = int(o["length"][i]) - 1; assert (out[c, i, :L] == ob[i, :L]).all(), (c, i)
+    for c, (o, _) in enumerate(WD.equal_11b(back_h, WD.rx11b(eng, back, stride, n, K))): assert len(o) == 2, (c, o)
 
 def test_round_trip_11n_on_the_device(eng):
-    r0_h, r1_h, mpdus, plan = frames_11n(); K, n = r0_h.shape[:2]; M = 16; OUT = 1536
+    r0_h, r1_h, mpdus, plan = frames_11n(); K, n = r0_h.shape[:2]
     (y0_h, y1_h), (b0_h, b1_h), _ = wide_11n()
     ch = [(W.phase_inc(f, W.FS_11A_WIDE), 0, 4096) for f in W.CH_11N]
-    r0, r1 = _dev_rows(K, n), _dev_rows(K, n)
+    r0, r1 = WD.dev_rows(K, n), WD.dev_rows(K, n)
     for c, pl in enumerate(plan):
         for (t, seed), m in zip(pl, mpdus[c]):
-            a, b = _tx11n(eng, m, 9, seed); r0[c, t:t + len(a)] = a; r1[c, t:t + len(b)] = b
+            a, b = WD.tx11n(eng, m, 9, seed); r0[c, t:t + len(a)] = a; r1[c, t:t + len(b)] = b
     assert (r0[:, :n].cpu().numpy() == r0_h).all() and (r1[:, :n].cpu().numpy() == r1_h).all()
     y0, d0, stride = _dev_chain(eng, r0, n, ch, TAPS_UP, TAPS_11A)
     y1, d1, _ = _dev_chain(eng, r1, n, ch, TAPS_UP, TAPS_11A)
     assert (y0.cpu().numpy() == y0_h).all() and (y1.cpu().numpy() == y1_h).all()
     assert (d0[:, :n].cpu().numpy() == b0_h).all() and (d1[:, :n].cpu().numpy() == b1_h).all()
-    off, ln = _tables(K, stride, n)
-    res = np.zeros((K, M), api.RESULT11N_DTYPE); out = np.zeros((K, M, OUT), np.uint8); sidx = np.zeros((K, M), np.uint32); cnt = np.zeros(K, np.uint32)
-    eng._check(eng._lib.sb200_rx11n_streams(eng._h, V(d0.data_ptr()), V(d1.data_ptr()), U64(K * stride), V(off.ctypes.data), V(ln.ctypes.data), U32(K), U32(M),
-                                            V(out.ctypes.data), U32(OUT), V(res.ctypes.data), V(sidx.ctypes.data), V(cnt.ctypes.data), V(0)), "sb200_rx11n_streams")
-    for c in range(K):
-        o, ob = oracle_py.rx11n_run(b0_h[c], b1_h[c], max_frames=M, out_stride=OUT)
-        assert cnt[c] == len(o) == 2, (c, cnt[c], o)
-        vec_base = 0; prev = 0
-        for k in range(len(o)):
-            for f in ("status", "mcs", "length", "crc32", "nsym", "cfo_est", "lsig_length"): assert res[c, k][f] == o[k][f], (c, k, f)
-            assert sidx[c, k] == o[k]["sample_index"], (c, k)
-            assert vec_base + res[c, k]["detect_index"] == o[k]["detect_index"], (c, k)
-            vec_base += 4 * ((int(sidx[c, k]) - prev) // 8); prev = int(sidx[c, k])
-            L = int(o[k]["length"]); assert (out[c, k, :L] == ob[k, :L]).all(), (c, k)
+    for c, (o, _) in enumerate(WD.equal_11n(b0_h, b1_h, WD.rx11n(eng, d0, d1, stride, n, K))): assert len(o) == 2, (c, o)

@@ -7,14 +7,14 @@ import numpy as np, pytest
 import torch
 import oracle_py
 import wideband_inputs as W
+import wideband_device as WD
 import bank_model as B
 import combine_bank_model as CB
 import combine_rational_model as CR
 import rational_model as R
 from sora_b200 import api
 from test_gpu_abi_residency import _matrix, _each, _fill
-from test_gpu_combine import _tx11a, _tx11b
-from test_cpu_channelize import CCA_WIDE, decode_11a
+from test_cpu_channelize import CCA_WIDE
 from test_cpu_combine import _psdus
 from test_cpu_combine_bank import GRID, TAPS_TX, combine_taps, OFDM_ROWS, F_11B, GAIN_11B, FRAMES_11B, max_taps, frames_octet, frames_11b_row, mixed_capture
 from test_cpu_channelize_rational import TAPS_160_44
@@ -97,13 +97,10 @@ def test_accumulate(eng):
         eng.combine_bank_raw(d_in.data_ptr(), 900, 900, 16, U, taps, d_out.data_ptr(), n, odd=True, accumulate=True)
         assert (d_out.cpu().numpy() == CB.window(x, 16, U, 1, taps, 0, n, acc)).all()
 
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
 @pytest.mark.parametrize("M,U,ntaps", [(8, 4, 255), (64, 64, 1023), (2, 1, 63), (64, 1, 31)])
 def test_long_capture(eng, M, U, ntaps):
     """4 x SMs tiles plus 777 outputs, device-resident; the first, middle and last outputs against the model's windows."""
-    n_out = 4 * _sms() * _tile(M, U) + 777; n = -(-n_out // U); stride = (n + 3) // 4 * 4
+    n_out = 4 * WD.sms() * _tile(M, U) + 777; n = -(-n_out // U); stride = (n + 3) // 4 * 4
     x = np.zeros((M, stride, 2), np.int16); x[:, :n] = _rows(M, n, M + ntaps); taps = _taps(ntaps, M)
     d_in = torch.from_numpy(x).cuda(); d_out = torch.zeros((n_out, 2), dtype=torch.int16, device="cuda")
     for odd in (0, 1):
@@ -194,31 +191,19 @@ def test_against_the_device_combiner(eng, M):
 
 
 # ---- end to end, device-resident ----------------------------------------------------------------------------------------------------
-def _rx11a(e, d, stride, n_out, K):
-    M = 16; OUT = 4096
-    off = np.arange(K, dtype=np.uint64) * stride; ln = np.full(K, n_out, np.uint32)
-    res = np.zeros((K, M), api.RESULT_DTYPE); out = np.zeros((K, M, OUT), np.uint8); sidx = np.zeros((K, M), np.uint32); cnt = np.zeros(K, np.uint32)
-    e._check(e._lib.sb200_rx11a_streams(e._h, V(d.data_ptr()), U64(K * stride), V(off.ctypes.data), V(ln.ctypes.data), U32(K), U32(M), V(out.ctypes.data), U32(OUT),
-                                        V(res.ctypes.data), V(sidx.ctypes.data), V(cnt.ctypes.data), V(0)), "sb200_rx11a_streams")
-    return res, out, sidx, cnt
-
-def _equal_to_the_oracle_11a(rows, res, out, sidx, cnt, want):
-    for c, (o, ob) in enumerate(decode_11a(rows)):
-        assert cnt[c] == len(o) and sum(o["status"] == oracle_py.E_FRAME_OK) == len(want[c]), (c, cnt[c], o)
-        r = res[c, :cnt[c]]
-        for k in ("status", "rate_kbps", "length", "crc32", "nsym", "cfo_est"): assert (r[k] == o[k]).all(), (c, k)
-        assert (sidx[c, :cnt[c]] == o["sample_index"]).all(), c
-        seg = np.diff(np.concatenate([[0], o["sample_index"].astype(np.int64)]))
-        assert (r["detect_index"] + np.concatenate([[0], np.cumsum(4 * (seg // 8))[:-1]]).astype(np.int64) == o["detect_index"]).all(), c
+def _equal_to_the_oracle_11a(rows, got, want):
+    """The receiver equal to the oracle on the model chain's rows, and every PSDU of want[c] delivered on row c."""
+    res, out, _, cnt = got
+    for c, (o, _) in enumerate(WD.equal_11a(rows, got)):
+        assert sum(o["status"] == oracle_py.E_FRAME_OK) == len(want[c]), (c, cnt[c], o)
         for i in range(len(o)):
-            L = int(o["length"][i]); assert (out[c, i, :L] == ob[i, :L]).all() and bytes(out[c, i, :L]) == want[c][i], (c, i)
+            L = int(o["length"][i]); assert bytes(out[c, i, :L]) == want[c][i], (c, i)
 
 def _dev_rows_11a(e, rows_h, plan, mpdus):
     """k_tx11a frames (x 20) in device rows at the oracle rows' positions; checked against them -> (device [8, stride, 2], stride)."""
-    n = rows_h.shape[1]; stride = (n + 3) // 4 * 4
-    d = torch.zeros((8, stride, 2), dtype=torch.int16, device="cuda")
+    n = rows_h.shape[1]; d = WD.dev_rows(8, n); stride = d.shape[1]
     for c, (t, rate, seed) in plan.items():
-        f = _tx11a(e, mpdus[c][0], rate, seed); d[c, t:t + len(f)] = f.to(torch.int16) * 20
+        f = WD.tx11a(e, mpdus[c][0], rate, seed); d[c, t:t + len(f)] = f.to(torch.int16) * 20
     assert (d[:, :n].cpu().numpy() == rows_h).all()
     return d, stride
 
@@ -233,13 +218,13 @@ def test_octet_round_trip_on_the_device():
         y = torch.zeros((4 * n, 2), dtype=torch.int16, device="cuda")
         e.combine_bank_raw(d.data_ptr(), stride, n, 8, 4, TAPS_TX, y.data_ptr(), 4 * n, odd=True)
         assert (y.cpu().numpy() == y_h).all()
-        rs = (n + 3) // 4 * 4 + 64; rows = torch.zeros((8, rs, 2), dtype=torch.int16, device="cuda")
+        rows = WD.dev_rows(8, n, 64); rs = rows.shape[1]
         e.channelize_bank_raw(y.data_ptr(), 4 * n, 8, 4, B.TAPS_BANK, rows.data_ptr(), rs, odd=True)
         assert (rows[:, :n].cpu().numpy() == back_h).all()
-        res, out, sidx, cnt = _rx11a(e, rows, rs, n, 8)
+        got = WD.rx11a(e, rows, rs, n, 8)
     finally:
         e.close()
-    _equal_to_the_oracle_11a(back_h, res, out, sidx, cnt, {c: _psdus(mpdus[c]) for c in range(8)})
+    _equal_to_the_oracle_11a(back_h, got, [_psdus(mpdus[c]) for c in range(8)])
 
 def test_mixed_capture_on_the_device():
     """OFDM rows on four bank channels by sb200_combine_bank, then an 802.11b row over two empty channels added by
@@ -255,30 +240,25 @@ def test_mixed_capture_on_the_device():
         y = torch.zeros((n_out, 2), dtype=torch.int16, device="cuda")
         e.combine_bank_raw(d.data_ptr(), stride, n, 8, 4, TAPS_TX, y.data_ptr(), n_out, odd=True)
         assert (y.cpu().numpy() == first_h).all()
-        nb = len(rb_h); sb = (nb + 3) // 4 * 4; rb = torch.zeros((1, sb, 2), dtype=torch.int16, device="cuda"); t = 500
+        nb = len(rb_h); rb = WD.dev_rows(1, nb); sb = rb.shape[1]; t = 500
         for (rate, _), m in zip(FRAMES_11B, mb):
-            f = _tx11b(e, m, rate); rb[0, t:t + len(f)] = f.to(torch.int16) << 6; t += len(f) + 900
+            f = WD.tx11b(e, m, rate); rb[0, t:t + len(f)] = f.to(torch.int16) << 6; t += len(f) + 900
         assert (rb[0, :nb].cpu().numpy() == rb_h).all()
         e.combine_raw(rb.data_ptr(), sb, nb, [(W.phase_inc(F_11B, 160e6), 0, GAIN_11B)], 40, TAPS_44_160, y.data_ptr(), decim=11, n_out=n_out, accumulate=True)
         assert (y.cpu().numpy() == y_h).all()
-        no = n_out // 4; rs = (no + 3) // 4 * 4 + 64; rows = torch.zeros((8, rs, 2), dtype=torch.int16, device="cuda")
+        no = n_out // 4; rows = WD.dev_rows(8, no, 64); rs = rows.shape[1]
         e.channelize_bank_raw(y.data_ptr(), n_out, 8, 4, B.TAPS_BANK, rows.data_ptr(), rs, odd=True)
         assert (rows[:, :no].cpu().numpy() == back_h).all()
         ofdm = torch.stack([rows[c] for c in OFDM_ROWS]).contiguous()
-        res, out, sidx, cnt = _rx11a(e, ofdm, rs, no, len(OFDM_ROWS))
-        nbo = len(row_b_h); sbo = (nbo + 3) // 4 * 4; row_b = torch.zeros((1, sbo, 2), dtype=torch.int16, device="cuda")
+        got_a = WD.rx11a(e, ofdm, rs, no, len(OFDM_ROWS))
+        nbo = len(row_b_h); row_b = WD.dev_rows(1, nbo); sbo = row_b.shape[1]
         e.channelize_raw(y.data_ptr(), n_out, [(W.phase_inc(F_11B, 160e6), 0)], 40, TAPS_160_44, row_b.data_ptr(), sbo, interp=11)
         assert (row_b[0, :nbo].cpu().numpy() == row_b_h).all()
-        M = 16; OUT = 4096; off = np.zeros(1, np.uint64); ln = np.full(1, nbo, np.uint32)
-        r11b = np.zeros((1, M), api.RESULT11B_DTYPE); o11b = np.zeros((1, M, OUT), np.uint8); c11b = np.zeros(1, np.uint32)
-        e._check(e._lib.sb200_rx11b_streams(e._h, V(row_b.data_ptr()), U64(sbo), V(off.ctypes.data), V(ln.ctypes.data), U32(1), U32(M), V(o11b.ctypes.data), U32(OUT),
-                                            V(r11b.ctypes.data), V(c11b.ctypes.data), V(0)), "sb200_rx11b_streams")
+        got_b = WD.rx11b(e, row_b, sbo, nbo, 1)
     finally:
         e.close()
-    _equal_to_the_oracle_11a(back_h[list(OFDM_ROWS)], res, out, sidx, cnt, [_psdus(mpdus[c]) for c in OFDM_ROWS])
-    ps = _psdus(mb); o, obo = oracle_py.rx11b_run(row_b_h, max_frames=16, out_stride=4096)
-    assert c11b[0] == len(o) == len(ps), (c11b[0], len(o))
-    r = r11b[0, :c11b[0]]
-    for k in ("status", "rate_kbps", "length", "crc32", "sample_index", "detect_vec"): assert (r[k] == o[k]).all(), k
+    _equal_to_the_oracle_11a(back_h[list(OFDM_ROWS)], got_a, [_psdus(mpdus[c]) for c in OFDM_ROWS])
+    ps = _psdus(mb); (o, _), = WD.equal_11b([row_b_h], got_b)
+    assert len(o) == len(ps), len(o)
     for j in range(len(o)):
-        L = int(o["length"][j]) - 1; assert (o11b[0, j, :L] == obo[j, :L]).all() and bytes(o11b[0, j, :L]) == ps[j][:-1], j
+        L = int(o["length"][j]) - 1; assert bytes(got_b[1][0, j, :L]) == ps[j][:-1], j

@@ -8,17 +8,17 @@ import ctypes as C
 from math import gcd
 import numpy as np, pytest
 import torch
-import oracle_py
 import wideband_inputs as W
+import wideband_device as WD
 import combine_rational_model as CR
 import rational_model as R
 from sora_b200 import api
 from test_gpu_abi_residency import _matrix, _each, _fill
-from test_cpu_channelize import CCA_WIDE, _full_scale, decode_11a
+from test_cpu_channelize import CCA_WIDE
 from test_cpu_channelize_rational import PLANS
 from test_cpu_combine_rational import TX_PLANS, GAIN_A, GAIN_B, TAPS_44_160, TAPS_40_176, SIM_LINK_24, SIM_TAPS_24, SIM_SEED_24, frames_24ghz, capture_of, through_the_air
 from test_cpu_combine import _psdus
-from test_gpu_combine import INCS, GAINS, _channels, _rows, _taps, _tx11a, _tx11b
+from wideband_device import GAINS, DUC_INCS as INCS, duc_channels as _channels, duc_rows as _rows, duc_taps as _taps, sms as _sms
 
 pytestmark = pytest.mark.gpu
 V, U32, U64 = C.c_void_p, C.c_uint32, C.c_uint64
@@ -117,9 +117,6 @@ def test_shared_memory_corners(eng):
 
 
 # ---- long captures --------------------------------------------------------------------------------------------------------------------
-def _sms():
-    return torch.cuda.get_device_properties(0).multi_processor_count
-
 @pytest.mark.parametrize("K,U,D,ntaps", [(3, 40, 11, 1761), (1, 22, 5, 1321), (16, 17, 16, 255), (2, 64, 1, 4095)])
 def test_long_captures(eng, K, U, D, ntaps):
     """At least 4 x SMs tiles plus 777 samples, on the device; the first, middle and last outputs against combine_rational_window."""
@@ -231,16 +228,16 @@ def test_24ghz_transmit_on_the_device(fs):
     channelizers -> sb200_rx11b_streams and sb200_rx11a_streams.  The capture, before and after the channel, equals the model chain on the
     oracle transmitters' output; the receivers equal the oracle on every field, event position and delivered byte; every PSDU delivered."""
     rows_h, mpdus, plan = frames_24ghz(); clean_h, _ = capture_of(fs, rows_h); y_h = through_the_air(clean_h)
-    (ub, db), tb, (ua, da), ta = TX_PLANS[fs]; (rub, rdb), rtb, (rua, rda), rta = PLANS[fs]; M = 16; OUT = 4096
+    (ub, db), tb, (ua, da), ta = TX_PLANS[fs]; (rub, rdb), rtb, (rua, rda), rta = PLANS[fs]
     e = api.Engine(0); ea = api.Engine(0, cca_pwr_threshold=CCA_WIDE)
     try:
         n_b = max(len(rows_h[0]), len(rows_h[2])); sb_in = (n_b + 3) // 4 * 4; n_a = len(rows_h[1]); sa_in = (n_a + 3) // 4 * 4
         rb = torch.zeros((2, sb_in, 2), dtype=torch.int16, device="cuda"); ra_ = torch.zeros((1, sa_in, 2), dtype=torch.int16, device="cuda")
         for i, c in enumerate((0, 2)):
             for (t, rate, _), m in zip(plan[c], mpdus[c]):
-                f = _tx11b(e, m, rate); rb[i, t:t + len(f)] = f.to(torch.int16) << 6
+                f = WD.tx11b(e, m, rate); rb[i, t:t + len(f)] = f.to(torch.int16) << 6
         for (t, rate, seed), m in zip(plan[1], mpdus[1]):
-            f = _tx11a(e, m, rate, seed); ra_[0, t:t + len(f)] = f.to(torch.int16) * 20
+            f = WD.tx11a(e, m, rate, seed); ra_[0, t:t + len(f)] = f.to(torch.int16) * 20
         assert (rb[0, :len(rows_h[0])].cpu().numpy() == rows_h[0]).all() and (rb[1, :len(rows_h[2])].cpu().numpy() == rows_h[2]).all()
         assert (ra_[0, :n_a].cpu().numpy() == rows_h[1]).all()
         n = len(y_h); tx = torch.zeros((n, 2), dtype=torch.int16, device="cuda"); y = torch.zeros_like(tx)     # n is a multiple of 4
@@ -250,8 +247,7 @@ def test_24ghz_transmit_on_the_device(fs):
         e.channel_sim_raw(tx.data_ptr(), n, n, 1, n, api.sim_links([SIM_LINK_24]), SIM_TAPS_24, 1, 1, SIM_SEED_24, y.data_ptr(), n, n, 1, n)
         assert (y.cpu().numpy() == y_h).all()
         def dev_rows(chans, u, d, t):
-            n_out = -(-u * n // d); stride = (n_out + 3) // 4 * 4 + 64
-            out = torch.zeros((len(chans), stride, 2), dtype=torch.int16, device="cuda")
+            n_out = -(-u * n // d); out = WD.dev_rows(len(chans), n_out, 64); stride = out.shape[1]
             e.channelize_raw(y.data_ptr(), n, [(W.phase_inc(R.CH_24[c], fs), 0) for c in chans], d, t, out.data_ptr(), stride, interp=u)
             return out, stride, n_out
         b_ch, a_ch = [0, 2], [1]
@@ -259,30 +255,14 @@ def test_24ghz_transmit_on_the_device(fs):
         back = {c: R.channelize_rational(y_h, [(W.phase_inc(R.CH_24[c], fs), 0)], *((rub, rdb, rtb) if c != 1 else (rua, rda, rta)))[0] for c in range(3)}
         for i, c in enumerate(b_ch): assert (db_[i, :nb].cpu().numpy() == back[c]).all(), c
         assert (da_[0, :na].cpu().numpy() == back[1]).all()
-        Kb, Ka = 2, 1
-        off = np.arange(Kb, dtype=np.uint64) * sb; ln = np.full(Kb, nb, np.uint32)
-        rb_ = np.zeros((Kb, M), api.RESULT11B_DTYPE); ob = np.zeros((Kb, M, OUT), np.uint8); cb = np.zeros(Kb, np.uint32)
-        e._check(e._lib.sb200_rx11b_streams(e._h, V(db_.data_ptr()), U64(Kb * sb), V(off.ctypes.data), V(ln.ctypes.data), U32(Kb), U32(M), V(ob.ctypes.data), U32(OUT),
-                                            V(rb_.ctypes.data), V(cb.ctypes.data), V(0)), "sb200_rx11b_streams")
-        off = np.zeros(1, np.uint64); ln = np.full(1, na, np.uint32)
-        ra = np.zeros((Ka, M), api.RESULT_DTYPE); oa = np.zeros((Ka, M, OUT), np.uint8); sidx = np.zeros((Ka, M), np.uint32); ca = np.zeros(Ka, np.uint32)
-        ea._check(ea._lib.sb200_rx11a_streams(ea._h, V(da_.data_ptr()), U64(sa), V(off.ctypes.data), V(ln.ctypes.data), U32(Ka), U32(M), V(oa.ctypes.data), U32(OUT),
-                                              V(ra.ctypes.data), V(sidx.ctypes.data), V(ca.ctypes.data), V(0)), "sb200_rx11a_streams")
+        got_b = WD.rx11b(e, db_, sb, nb, len(b_ch)); got_a = WD.rx11a(ea, da_, sa, na, len(a_ch))
     finally:
         e.close(); ea.close()
-    for i, c in enumerate(b_ch):
-        ps = _psdus(mpdus[c]); o, obo = oracle_py.rx11b_run(back[c], max_frames=M, out_stride=OUT)
-        assert cb[i] == len(o) == len(ps), (c, cb[i], len(o))
-        r = rb_[i, :cb[i]]
-        for k in ("status", "rate_kbps", "length", "crc32", "sample_index", "detect_vec"): assert (r[k] == o[k]).all(), (c, k)
+    for i, (c, (o, _)) in enumerate(zip(b_ch, WD.equal_11b([back[c] for c in b_ch], got_b))):
+        ps = _psdus(mpdus[c]); assert len(o) == len(ps), (c, len(o))
         for j in range(len(o)):
-            L = int(o["length"][j]) - 1; assert (ob[i, j, :L] == obo[j, :L]).all() and bytes(ob[i, j, :L]) == ps[j][:-1], (c, j)
-    ps = _psdus(mpdus[1]); (o, obo), = decode_11a([back[1]])
-    assert ca[0] == len(o) == len(ps), (ca[0], len(o))
-    r = ra[0, :ca[0]]
-    for k in ("status", "rate_kbps", "length", "crc32", "nsym", "cfo_est"): assert (r[k] == o[k]).all(), k
-    assert (sidx[0, :ca[0]] == o["sample_index"]).all()
-    seg = np.diff(np.concatenate([[0], o["sample_index"].astype(np.int64)]))
-    assert (r["detect_index"] + np.concatenate([[0], np.cumsum(4 * (seg // 8))[:-1]]) == o["detect_index"]).all()
+            L = int(o["length"][j]) - 1; assert bytes(got_b[1][i, j, :L]) == ps[j][:-1], (c, j)
+    (o, _), = WD.equal_11a([back[1]], got_a); ps = _psdus(mpdus[1])
+    assert len(o) == len(ps), len(o)
     for j in range(len(o)):
-        L = int(o["length"][j]); assert (oa[0, j, :L] == obo[j, :L]).all() and bytes(oa[0, j, :L]) == ps[j], j
+        L = int(o["length"][j]); assert bytes(got_a[1][0, j, :L]) == ps[j], j
