@@ -122,6 +122,8 @@ def sim_taps(delays, gains, L):
     return q.astype(np.int16)
 
 _NDBPS_11A = {6000: 24, 9000: 36, 12000: 48, 18000: 72, 24000: 96, 36000: 144, 48000: 192, 54000: 216}   # 802.11a data bits per OFDM symbol
+_NDBPS_11N = {8: 52, 9: 104, 10: 156}                   # 802.11n data bits per OFDM symbol over both streams, MCS 8 .. 10
+_CHIPS_11B = {1000: 88, 2000: 44, 5500: 16, 11000: 8}   # 802.11b chips per PSDU byte
 
 def _ptr(a):
     """numpy array -> host pointer; torch tensor / int -> raw (device or pinned) pointer."""
@@ -234,13 +236,16 @@ class Engine:
                                                 C.c_uint32(nframes), C.c_uint32(rate_kbps), C.c_uint32(lead), C.c_uint32(bits), C.c_void_p(out_ptr), C.c_uint64(out_stride),
                                                 C.c_void_p(ns_ptr), C.c_void_p(stream)), "sb200_tx11a_batch")
 
+    @staticmethod
+    def tx11a_out_stride(length, rate_kbps, lead=0):
+        """Default out_stride of tx11a_batch for MPDUs of up to `length` bytes (FCS not included): lead, the preamble, SIGNAL and the data
+        symbols with two to spare, and 32 samples more.  KeyError for a rate that is not an 802.11a rate."""
+        return lead + 640 + 160 * (2 + -(-(length + 7) * 8 // _NDBPS_11A[rate_kbps]) + 1) + 32
+
     def tx11a_batch(self, payloads, rate_kbps, seeds=None, lead=0, sample_bits=8, out_stride=None):
         """payloads: list of uint8 arrays (MPDUs without FCS) -> (samples [F, out_stride, 2] int8 or int16, nsamples [F])."""
         flat, offs, lens = _payload_table(payloads)
-        from math import ceil
-        if out_stride is None:
-            nd = _NDBPS_11A[rate_kbps]
-            out_stride = lead + 640 + 160 * (2 + ceil((int(lens.max()) + 7) * 8 / nd) + 1) + 32
+        if out_stride is None: out_stride = self.tx11a_out_stride(int(lens.max()), rate_kbps, lead)
         out = np.zeros((len(lens), out_stride, 2), np.int8 if sample_bits == 8 else np.int16); ns = np.zeros(len(lens), np.uint32)
         sd = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.uint8)
         self.tx11a_raw(_ptr(flat), flat.size, _ptr(offs), _ptr(lens), 0 if sd is None else _ptr(sd), len(lens), rate_kbps, lead, sample_bits, _ptr(out), out_stride, _ptr(ns))
@@ -251,12 +256,16 @@ class Engine:
                                                 C.c_uint32(mcs), C.c_uint32(lead), C.c_void_p(out0_ptr), C.c_void_p(out1_ptr), C.c_uint64(out_stride), C.c_void_p(ns_ptr),
                                                 C.c_void_p(stream)), "sb200_tx11n_batch")
 
+    @staticmethod
+    def tx11n_out_stride(length, mcs, lead=0):
+        """Default out_stride of tx11n_batch for MPDUs of up to `length` bytes (FCS not included): lead, the preamble and SIG symbols, and the
+        data symbols with one to spare.  MCS 11 .. 14 are sized as MCS 8, which needs the most symbols."""
+        return lead + 1600 + 160 * (-(-((length + 4) * 8 + 22) // _NDBPS_11N.get(mcs, 52)) + 1)
+
     def tx11n_batch(self, payloads, mcs, seeds=None, lead=0, out_stride=None):
         """payloads: list of uint8 arrays (MPDUs without FCS) -> (stream 0 [F, out_stride, 2] int16, stream 1, nsamples [F]) at 40 Msps."""
         flat, offs, lens = _payload_table(payloads)
-        if out_stride is None:
-            nd = {8: 52, 9: 104, 10: 156}.get(mcs, 52)
-            out_stride = lead + 1600 + 160 * (-(-((int(lens.max()) + 4) * 8 + 22) // nd) + 1)
+        if out_stride is None: out_stride = self.tx11n_out_stride(int(lens.max()), mcs, lead)
         o0 = np.zeros((len(lens), out_stride, 2), np.int16); o1 = np.zeros_like(o0); ns = np.zeros(len(lens), np.uint32)
         sd = None if seeds is None else np.ascontiguousarray(seeds, dtype=np.uint8)
         self.tx11n_raw(_ptr(flat), flat.size, _ptr(offs), _ptr(lens), 0 if sd is None else _ptr(sd), len(lens), mcs, lead, _ptr(o0), _ptr(o1), out_stride, _ptr(ns))
@@ -267,12 +276,16 @@ class Engine:
                                                 C.c_uint32(rate_kbps), C.c_uint32(init_phase), C.c_uint32(lead), C.c_uint32(bits), C.c_void_p(out_ptr),
                                                 C.c_uint64(out_stride), C.c_void_p(ns_ptr), C.c_void_p(fp_ptr), C.c_void_p(stream)), "sb200_tx11b_batch")
 
+    @staticmethod
+    def tx11b_out_stride(length, rate_kbps, lead=0):
+        """Default out_stride of tx11b_batch for MPDUs of up to `length` bytes (FCS not included): lead and four samples per chip of the PLCP
+        and the PSDU and five more, rounded up to 8.  An unknown rate is the library's error to report."""
+        return (lead + (24 * 88 + (length + 4) * _CHIPS_11B.get(rate_kbps, 8) + 5) * 4 + 15) // 8 * 8
+
     def tx11b_batch(self, payloads, rate_kbps, init_phase=0, lead=0, sample_bits=8, out_stride=None, return_phase=False):
         """payloads: list of uint8 arrays (MPDUs without FCS) -> (samples [F, out_stride, 2] int8 or int16 at 44 Msps, nsamples [F])."""
         flat, offs, lens = _payload_table(payloads)
-        if out_stride is None:
-            cpb = {1000: 88, 2000: 44, 5500: 16, 11000: 8}.get(rate_kbps, 8)      # an unknown rate is the library's error to report
-            out_stride = (lead + (24 * 88 + (int(lens.max()) + 4) * cpb + 5) * 4 + 15) // 8 * 8
+        if out_stride is None: out_stride = self.tx11b_out_stride(int(lens.max()), rate_kbps, lead)
         out = np.zeros((len(lens), out_stride, 2), np.int8 if sample_bits == 8 else np.int16); ns = np.zeros(len(lens), np.uint32)
         fp = np.zeros(len(lens), np.uint32)
         self.tx11b_raw(_ptr(flat), flat.size, _ptr(offs), _ptr(lens), len(lens), rate_kbps, init_phase, lead, sample_bits, _ptr(out), out_stride, _ptr(ns), 0, _ptr(fp))
@@ -422,14 +435,18 @@ class Engine:
                                                        C.c_uint32(rate_kbps), C.c_uint32(short_preamble), C.c_uint32(flags), C.c_uint32(filt), C.c_void_p(out_ptr),
                                                        C.c_uint64(out_stride), C.c_void_p(ns_ptr), C.c_void_p(stream)), "sb200_tx11b_legacy_batch")
 
+    @staticmethod
+    def tx11b_legacy_nsamples(psdu_len, rate_kbps, short_preamble=False):
+        """Samples BB11BPMDBufferTx4X* writes for a PSDU of psdu_len bytes (FCS included): four per chip and TX_FIR_DEPTH zeros, rounded up
+        to 128.  The short preamble sends no data chips at 1 Mbps."""
+        cpb = 0 if short_preamble and rate_kbps == 1000 else _CHIPS_11B.get(rate_kbps, 8)     # an unknown rate is the library's error to report
+        return (4 * ((1056 if short_preamble else 2112) + psdu_len * cpb) + 37 + 127) // 128 * 128
+
     def tx11b_legacy_batch(self, payloads, rate_kbps, short_preamble=False, filter=1, fcs_in_payload=False, out_stride=None):
         """The legacy 802.11b transmitter (BB11BPMDBufferTx4X* and, filter 1 / 2, the SSE / ASM 37-tap filter).  payloads: list of uint8 arrays,
         MPDUs without FCS (or with it, fcs_in_payload=True) -> (COMPLEX8 samples int8 [F, out_stride, 2] at 44 Msps, nsamples [F])."""
         flat, offs, lens = _payload_table(payloads)
-        if out_stride is None:
-            size = int(lens.max()) + (0 if fcs_in_payload else 4)
-            cpb = {1000: 0 if short_preamble else 88, 2000: 44, 5500: 16, 11000: 8}.get(rate_kbps, 8)     # an unknown rate is the library's error to report
-            out_stride = (4 * ((1056 if short_preamble else 2112) + size * cpb) + 37 + 127) // 128 * 128
+        if out_stride is None: out_stride = self.tx11b_legacy_nsamples(int(lens.max()) + (0 if fcs_in_payload else 4), rate_kbps, short_preamble)
         out = np.zeros((len(lens), out_stride, 2), np.int8); ns = np.zeros(len(lens), np.uint32)
         self.tx11b_legacy_raw(_ptr(flat), flat.size, _ptr(offs), _ptr(lens), len(lens), rate_kbps, int(bool(short_preamble)),
                               self.TX11B_LEGACY_FCS_IN_PAYLOAD if fcs_in_payload else 0, filter, _ptr(out), out_stride, _ptr(ns))

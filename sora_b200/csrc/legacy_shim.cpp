@@ -6,9 +6,11 @@
 // and move the stream's scan pointer exactly as far as the samples they consumed.
 #include "../../include/sora_b200_legacy.h"
 #include "../../include/sora_b200.h"
+#include "tx_frames.cuh"
 #include <cstdlib>
 #include <cstring>
 #include <vector>
+using sb::Rate11a; using sb::kRates11a; using sb::Rate11b; using sb::kRates11b; using sb::find_rate;
 
 namespace {
 struct Event { sb200_frame_result r; uint32_t end_sample; uint32_t start_sample; std::vector<uint8_t> bytes; };
@@ -182,7 +184,7 @@ extern "C" HRESULT BB11BRx(PBB11B_RX_CONTEXT c, PSORA_RADIO_RX_STREAM s) {
     if (s->__pScanPt >= s->__pEndPt) { s->__pScanPt = s->__pStartPt; E->base = nullptr; }
     BB11B_COMMON& B = c->BB11bCommon;
     B.b_length = e.r.length; B.b_isLongPreamble = 1; B.b_crc32 = e.r.crc32;
-    B.b_dataRate = e.r.rate_kbps == 1000 ? 0x0A : e.r.rate_kbps == 2000 ? 0x14 : e.r.rate_kbps == 5500 ? 0x37 : e.r.rate_kbps == 11000 ? 0x6E : 0;
+    const Rate11b* r = find_rate(kRates11b, e.r.rate_kbps); B.b_dataRate = r ? (UCHAR)r->code : 0;
     switch (e.r.status) {
         case SB200_FRAME_OK: case SB200_FRAME_CRC32_FAIL:
             if (!B.b_outputPt || e.bytes.size() > B.b_maxOutputSize) { B.b_errFrame++; return BB11B_E_DATA; }
@@ -222,14 +224,9 @@ extern "C" HRESULT BB11BPMDSpreadFIR4ASM(const SORA_COMPLEX8* s, uint32_t n, SOR
 
 // ---- the legacy 802.11b transmitter (bbb.h:204-240, bbb_tx.c) over sb200_tx11b_legacy_batch ---------------------------------------------
 namespace {
-uint32_t kbps_of_code(UCHAR c) { return c == 0x0A ? 1000u : c == 0x14 ? 2000u : c == 0x37 ? 5500u : c == 0x6E ? 11000u : 0u; }
-// the samples BB11BPMDBufferTx4X* writes for a PSDU of `size` bytes (FCS included): 4 per chip, TX_FIR_DEPTH zeros rounded up to 128
-uint32_t legacy_nsamples(uint32_t size, UCHAR pre, uint32_t kbps) {
-    const uint32_t cpb = kbps == 1000 ? (pre ? 0u : 88u) : kbps == 2000 ? 44u : kbps == 5500 ? 16u : 8u;
-    return (4u * ((pre ? 1056u : 2112u) + size * cpb) + 37u + 127u) & ~127u;
-}
-// the scrambler's side effect on the caller's bytes: the stream runs over the PLCP frame first (bbb_tx.c:537-538, :669-670)
-void scramble_in_place(const DOT11B_PLCP_TXVECTOR* v, uint32_t kbps, uint32_t size, const std::vector<uint8_t*>& bytes) {
+// the scrambler's side effect on the caller's bytes: the stream runs over the PLCP frame first (bbb_tx.c:537-538, :669-670); v's rate is valid
+void scramble_in_place(const DOT11B_PLCP_TXVECTOR* v, uint32_t size, const std::vector<uint8_t*>& bytes) {
+    const uint32_t kbps = find_rate(kRates11b, v->DateRate, &Rate11b::code)->kbps;
     uint32_t plen, ext = 0;                                                                 // PLCPGetLength (bbb_tx.c:39-65), CCK
     if (kbps == 1000) plen = size << 3; else if (kbps == 2000) plen = size << 2;
     else if (kbps == 5500) plen = ((size << 4) - 1u) / 11u + 1u;
@@ -248,15 +245,15 @@ void scramble_in_place(const DOT11B_PLCP_TXVECTOR* v, uint32_t kbps, uint32_t si
 }
 // encode psdu (FCS included) with the filter selected (0 encoder output, 1 SSE filter) into dst; n = samples written
 HRESULT legacy_tx(const DOT11B_PLCP_TXVECTOR* v, const std::vector<uint8_t>& psdu, uint32_t filter, void* dst, uint32_t* n) {
-    const uint32_t kbps = kbps_of_code(v->DateRate);
-    if (!kbps || v->PreambleType > 1 || v->ModSelect != 0 || psdu.size() < 4 || psdu.size() > 4095) return SORA_E_FAIL;
-    const uint32_t ns = legacy_nsamples((uint32_t)psdu.size(), v->PreambleType, kbps);
+    const Rate11b* R = find_rate(kRates11b, v->DateRate, &Rate11b::code);
+    if (!R || v->PreambleType > 1 || v->ModSelect != 0 || psdu.size() < 4 || psdu.size() > 4095) return SORA_E_FAIL;
+    const uint32_t ns = sb::tx11b_legacy_nsamples((uint32_t)psdu.size(), v->PreambleType, sb::tx11b_legacy_data_chips(*R, v->PreambleType));
     void* buf = nullptr;
     if (posix_memalign(&buf, 16, (size_t)ns * 2) != 0) return SORA_E_FAIL;
     const uint64_t off = 0; const uint32_t len = (uint32_t)psdu.size(); uint32_t got = 0;
     int rc;
     {   std::lock_guard<std::mutex> lk(g_fir_mu);
-        rc = fir_engine() ? sb200_tx11b_legacy_batch(g_fir_engine, psdu.data(), len, &off, &len, 1, kbps, v->PreambleType, SB200_TX11B_LEGACY_FCS_IN_PAYLOAD, filter,
+        rc = fir_engine() ? sb200_tx11b_legacy_batch(g_fir_engine, psdu.data(), len, &off, &len, 1, R->kbps, v->PreambleType, SB200_TX11B_LEGACY_FCS_IN_PAYLOAD, filter,
                                                      (int8_t*)buf, ns, &got, nullptr) : SB200_E_NODEVICE; }
     if (rc == SB200_OK && got == ns) memcpy(dst, buf, (size_t)ns * 2);
     free(buf);
@@ -272,7 +269,7 @@ HRESULT buffer_tx(PDOT11B_PLCP_TXVECTOR v, PUCHAR data, unsigned int dataLength,
     const HRESULT r = legacy_tx(&w, psdu, 0, out, &ns);
     if (r != SORA_S_OK) return r;
     std::vector<uint8_t*> bytes; for (unsigned int i = 0; i < dataLength + 4u; i++) bytes.push_back(data + i);
-    scramble_in_place(&w, kbps_of_code(w.DateRate), dataLength + 4u, bytes);
+    scramble_in_place(&w, dataLength + 4u, bytes);
     *n = ns;
     return SORA_S_OK;
 }
@@ -293,7 +290,7 @@ HRESULT packet_tx(PDOT11B_PLCP_TXVECTOR v, PPACKET_BASE p, PUCHAR out, ULONG* n,
     HRESULT r = legacy_tx(v, psdu, 0, out, &ns);
     if (r == SORA_S_OK && filtered) r = legacy_tx(v, psdu, 1, filtered, &ns);
     if (r != SORA_S_OK) return r;
-    scramble_in_place(v, kbps_of_code(v->DateRate), (uint32_t)psdu.size(), where);
+    scramble_in_place(v, (uint32_t)psdu.size(), where);
     if (n) *n = ns;
     if (nfiltered) *nfiltered = ns;
     return SORA_S_OK;
@@ -327,18 +324,12 @@ extern "C" HRESULT BB11BPMDPacketGenSignal(PPACKET_BASE p, PDOT11B_PLCP_TXVECTOR
 // ---- the legacy 802.11a transmitter (bba.h:201-247, atx_fe.c) over sb200_tx11a_legacy_batch ------------------------------------------------
 namespace {
 std::mutex g_pre_mu; bool g_pre_set = false; int16_t g_pre[1280];
-uint32_t kbps_of_11a(unsigned int c) {
-    switch (c) { case 0xB: return 6000; case 0xF: return 9000; case 0xA: return 12000; case 0xE: return 18000;
-                 case 0x9: return 24000; case 0xD: return 36000; case 0x8: return 48000; case 0xC: return 54000; default: return 0; }
-}
-uint32_t nsamples_11a(uint32_t size, uint32_t kbps, unsigned int sr) {   // GetSignalBytes (atx_tpl.h:69-83) / 2, rounded up to 128 bytes
-    const uint32_t ndbps = kbps / 250u, nsym = (22u + 8u * size + ndbps - 1u) / ndbps;
-    return ((sr == 44 ? 176u : 160u) * (5u + nsym) + 8u + 63u) & ~63u;
-}
-// modulate psdu (FCS included) into dst, which holds at least cap_bytes; *n = padded samples
-bool tx11a(const std::vector<uint8_t>& psdu, uint32_t kbps, unsigned int sr, void* dst, size_t cap_bytes, uint32_t* n) {
-    if (!kbps || (sr != 40 && sr != 44) || psdu.size() < 4 || psdu.size() > 4096 || !dst) return false;
-    const uint32_t ns = nsamples_11a((uint32_t)psdu.size(), kbps, sr);
+// GetSignalBytes (atx_tpl.h:69-83) / 2 of a PSDU of `size` bytes, rounded up to 128 bytes
+uint32_t nsamples_11a(uint32_t size, const Rate11a& r, unsigned int sr) { return sb::tx11a_legacy_padded(sb::tx11a_legacy_nsym(size, r.ndbps), sr == 44); }
+// modulate psdu (FCS included) at rate r into dst, which holds at least cap_bytes; *n = padded samples
+bool tx11a(const std::vector<uint8_t>& psdu, const Rate11a* r, unsigned int sr, void* dst, size_t cap_bytes, uint32_t* n) {
+    if (!r || (sr != 40 && sr != 44) || psdu.size() < 4 || psdu.size() > 4096 || !dst) return false;
+    const uint32_t ns = nsamples_11a((uint32_t)psdu.size(), *r, sr);
     if ((size_t)ns * 2 > cap_bytes) return false;
     void* buf = nullptr;
     if (posix_memalign(&buf, 16, (size_t)ns * 2) != 0) return false;
@@ -349,7 +340,7 @@ bool tx11a(const std::vector<uint8_t>& psdu, uint32_t kbps, unsigned int sr, voi
     const uint64_t off = 0; const uint32_t len = (uint32_t)psdu.size(); uint32_t got = 0;
     int rc;
     {   std::lock_guard<std::mutex> lk(g_fir_mu);
-        rc = fir_engine() ? sb200_tx11a_legacy_batch(g_fir_engine, psdu.data(), len, &off, &len, 1, kbps, sr, SB200_TX11A_LEGACY_FCS_IN_PAYLOAD, pre,
+        rc = fir_engine() ? sb200_tx11a_legacy_batch(g_fir_engine, psdu.data(), len, &off, &len, 1, r->kbps, sr, SB200_TX11A_LEGACY_FCS_IN_PAYLOAD, pre,
                                                      (int8_t*)buf, ns, &got, nullptr) : SB200_E_NODEVICE; }
     const bool ok = rc == SB200_OK && got == ns;
     if (ok) memcpy(dst, buf, (size_t)ns * 2);
@@ -371,14 +362,14 @@ extern "C" void BB11ATxContextInit(PBB11A_TX_VECTOR info, unsigned int SampleRat
 extern "C" HRESULT BB11ATxFrameMod(PBB11A_TX_VECTOR info, PPACKET_BASE p) {
     if (!info || !p) return SORA_E_FAIL;
     if (p->PacketSize + 4u > 4096u) return SORA_E_FAIL;                                    // atx_fe.c:23
-    const uint32_t kbps = kbps_of_11a(info->ti_uiDataRate);
-    if (!kbps) return SORA_E_FAIL;                                                          // atx_fe.c:59-62
+    const Rate11a* r = find_rate(kRates11a, info->ti_uiDataRate, &Rate11a::code);
+    if (!r) return SORA_E_FAIL;                                                             // atx_fe.c:59-62
     std::vector<uint8_t> psdu; std::vector<uint8_t*> where;
     if (!packet_bytes(p, psdu, where)) return SORA_E_FAIL;                                  // MDL chain + Reserved1 (atx_tpl.h:24-46)
     PTXSAMPLE sb = nullptr; ULONG sb_size = 0;
     SoraPacketGetTxSampleBuffer(p, &sb, &sb_size);
     uint32_t n = 0;
-    if (!tx11a(psdu, kbps, info->SampleRate, sb, sb_size, &n)) return SORA_E_FAIL;
+    if (!tx11a(psdu, r, info->SampleRate, sb, sb_size, &n)) return SORA_E_FAIL;
     SoraPacketSetSignalLength(p, n * (ULONG)sizeof(TXSAMPLE));
     return SORA_S_OK;
 }
@@ -392,6 +383,7 @@ extern "C" ULONG BB11AModulateACK(unsigned int SampleRate, const PMAC_ADDRESS ra
     for (int i = 0; i < 4; i++) ack.push_back((uint8_t)(c >> (8 * i)));
     // BB11ATxBufferMod6M: 6 Mbps whatever ti_uiDataRate says (the reference sets DOT11A_RATE_24M and never reads it there)
     uint32_t n = 0;
-    if (!tx11a(ack, 6000, SampleRate, out, (size_t)nsamples_11a(14, 6000, SampleRate) * 2, &n)) return 0;
+    const Rate11a* r = find_rate(kRates11a, 6000);
+    if (!tx11a(ack, r, SampleRate, out, (size_t)nsamples_11a(14, *r, SampleRate) * 2, &n)) return 0;
     return n * (ULONG)sizeof(TXSAMPLE);
 }

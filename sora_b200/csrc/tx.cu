@@ -1,10 +1,12 @@
 // sora_b200 — the transmitters: 802.11a, 802.11b, 802.11n and the legacy 802.11a / 802.11b ones, and the legacy 802.11b transmit filter.
 #include "handle.cuh"
+#include "tx_frames.cuh"
 #include "tx11a_kernels.cuh"
 #include "tx11b_kernels.cuh"
 #include "tx11b_legacy_kernels.cuh"
 #include "tx11a_legacy_kernels.cuh"
 #include "tx11n_kernels.cuh"
+#include <type_traits>
 
 // ---- 802.11a transmit (SURVEY.md §8(f) rank 2) -------------------------------------------------------------------------------
 static int upload_tables_tx(sb200_handle* h) {
@@ -39,76 +41,102 @@ static int upload_tables_tx(sb200_handle* h) {
     return SB200_OK;
 }
 
-// 802.11a rates: SIGNAL rate code, coded bits per subcarrier, code rate, data bits per symbol (ieee80211a_cmn.h:66-157; bba.h:179-186, atx.h:20-57)
-struct Rate11a { uint32_t kbps, code, nbpsc, cr, ndbps; };
-static const Rate11a kRates11a[8] = {{6000, 0xB, 1, CR_12, 24}, {9000, 0xF, 1, CR_34, 36}, {12000, 0xA, 2, CR_12, 48}, {18000, 0xE, 2, CR_34, 72},
-    {24000, 0x9, 4, CR_12, 96}, {36000, 0xD, 4, CR_34, 144}, {48000, 0x8, 6, CR_23, 192}, {54000, 0xC, 6, CR_34, 216}};
-// 802.11b rates: SIGNAL rate code, chips per PSDU byte (bb/bbb.h:47-50, DataRate.h:40-43)
-struct Rate11b { uint32_t kbps, code, chips_per_byte; };
-static const Rate11b kRates11b[4] = {{1000, 0x0A, 88}, {2000, 0x14, 44}, {5500, 0x37, 16}, {11000, 0x6E, 8}};
-template <class R, size_t N> static const R* find_rate(const R (&rates)[N], uint32_t kbps) {
-    for (const R& r : rates) if (r.kbps == kbps) return &r;
-    return nullptr;
+// ---- what the batch transmitters share ----------------------------------------------------------------------------------------------
+// The argument checks before a transmitter looks at its rate: no null handle or pointer among `p`; then, after the chain's own checks,
+// check_out(): the sample format (8 | 16) and, where `aligned_out` is given, 16-byte aligned output rows a multiple of 8 samples apart.
+template <class... P> static int check_null(sb200_handle* h, const P*... p) {
+    if (!h) return SB200_E_INVALID;
+    return (p && ...) ? SB200_OK : h->fail(SB200_E_INVALID, "null argument");
 }
-
-// The FCS of every payload (k_tx11a_crc) into the crc workspace, for the transmitters that append it
-static int crc_pass(sb200_handle* h, cudaStream_t st, const uint8_t* d_pay, const uint64_t* d_off, const uint32_t* d_len, uint32_t nframes, const uint32_t** d_crc) {
-    CK(h->crc.need(nframes * 4ull));
-    k_tx11a_crc<<<(nframes + 127) / 128, 128, 0, st>>>(d_pay, d_off, d_len, nframes, h->T, (uint32_t*)h->crc.p);
-    *d_crc = (const uint32_t*)h->crc.p; h->launches += 1;
+static int check_out(sb200_handle* h, uint32_t sample_bits, const void* aligned_out, uint64_t out_stride_samples) {
+    if (sample_bits != 8 && sample_bits != 16) return h->fail(SB200_E_INVALID, "sample_bits must be 8 (COMPLEX8) or 16 (COMPLEX16 = COMPLEX8 << 8)");
+    if (aligned_out && (out_stride_samples % 8u || ((uintptr_t)aligned_out & 15u))) return h->fail(SB200_E_INVALID, "out must be 16-byte aligned and out_stride_samples a multiple of 8");
     return SB200_OK;
 }
+
+// f(std::integral_constant<int, i>()) for a runtime i of 0 .. N - 1 (checked by the caller): the transmit kernels take their rate, output
+// alignment, filter or variant as a template parameter.
+template <int N, class F> static void with_index(uint32_t i, F f) {
+    if constexpr (N > 1) { if (i == N - 1) return f(std::integral_constant<int, N - 1>()); with_index<N - 1>(i, f); }
+    else f(std::integral_constant<int, 0>());
+}
+
+// One call of a batch transmitter after its argument checks, in this order: begin() sets the device and opens the call (the payload and
+// `in` are read on the stream); load() reads the frame table with the chain's own per-slot check (FrameTable::load); stage() places the
+// payload and its off / len tables on the device; bind() binds `out` and nsamples; start() sizes the remaining workspaces, records ev0 and,
+// for the chains that append the FCS, runs k_tx11a_crc into the crc workspace (d_crc, else null); finish() ends the call with the chain's
+// own launches.  No workspace grows between ev0 and ev1.
+struct TxCall {
+    sb200_handle* h; cudaStream_t st; cudaError_t dev; CallScope scope; FrameTable ft; Returns ret;
+    const uint8_t* d_pay = nullptr; const uint64_t* d_off = nullptr; const uint32_t* d_len = nullptr; uint32_t* d_ns = nullptr; const uint32_t* d_crc = nullptr;
+    TxCall(sb200_handle* h_, void* stream, const uint64_t* off, const uint32_t* len, uint32_t n)
+        : h(h_), st((cudaStream_t)stream), dev(cudaSetDevice(h_->device)), scope(h_, st), ft(off, len, n) {}
+    int begin(const void* payload, const void* in = nullptr) {
+        if (dev != cudaSuccess) return h->fail(SB200_E_CUDA, "cudaSetDevice(h->device)", dev);
+        CK(scope.begin()); scope.reads(payload); scope.reads(in);
+        return SB200_OK;
+    }
+    template <class Slot> int load(uint64_t total, Slot slot) { return ft.load(h, st, total, slot); }
+    cudaError_t stage(const uint8_t* payload, uint64_t total, size_t slack = 0) {
+        const cudaError_t e = to_device(h->txpay, payload, is_device_ptr(payload), total, st, &d_pay, slack);
+        return e != cudaSuccess ? e : ft.upload(h->txoff, h->txlen, st, &d_off, &d_len);
+    }
+    template <class T> cudaError_t bind(T* out, size_t out_bytes, T** d_out, uint32_t* nsamples) {
+        const cudaError_t e = ret.bind(h->txout, out, out_bytes, d_out);
+        return e != cudaSuccess ? e : ret.bind(h->txns, nsamples, ft.n * 4ull, &d_ns);
+    }
+    cudaError_t start(bool fcs, size_t desc_bytes = 0) {
+        cudaError_t e = fcs ? h->crc.need(ft.n * 4ull) : cudaSuccess;
+        if (e == cudaSuccess && desc_bytes) e = h->txdesc.need(desc_bytes);
+        if (e == cudaSuccess) e = cudaEventRecord(h->ev0, st);
+        if (e != cudaSuccess || !fcs) return e;
+        k_tx11a_crc<<<(ft.n + 127) / 128, 128, 0, st>>>(d_pay, d_off, d_len, ft.n, h->T, (uint32_t*)h->crc.p);
+        d_crc = (const uint32_t*)h->crc.p; h->launches += 1;
+        return cudaSuccess;
+    }
+    int finish(uint64_t launches) { return finish_call(h, st, ret, 0, launches); }
+};
 
 extern "C" int sb200_tx11a_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_total, const uint64_t* pay_off, const uint32_t* pay_len, const uint8_t* seeds,
                                  uint32_t nframes, uint32_t rate_kbps, uint32_t lead_samples, uint32_t sample_bits, void* out, uint64_t out_stride_samples,
                                  uint32_t* nsamples, void* cuda_stream) {
-    if (!h || !payload || !pay_off || !pay_len || !out) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
-    if (sample_bits != 8 && sample_bits != 16) return h->fail(SB200_E_INVALID, "sample_bits must be 8 (COMPLEX8) or 16 (COMPLEX16 = COMPLEX8 << 8)");
-    if (nframes == 0) return SB200_OK;
+    int rc = check_null(h, payload, pay_off, pay_len, out);
+    if (rc == SB200_OK) rc = check_out(h, sample_bits, nullptr, 0);
+    if (rc != SB200_OK || nframes == 0) return rc;
     const Rate11a* R = find_rate(kRates11a, rate_kbps);
     if (!R) return h->fail(SB200_E_INVALID, "rate_kbps is not an 802.11a rate");
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    CK(cudaSetDevice(h->device));
-    CallScope call(h, st); CK(call.begin()); call.reads(payload); call.reads(seeds);
-    int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
-    // frame table on the host (sizes the grid and checks the slots)
-    FrameTable ft(pay_off, pay_len, nframes);
-    TxJob job{}; job.rate_code = R->code; job.nbpsc = R->nbpsc; job.code_rate = R->cr; job.ndbps = R->ndbps; job.ndbps_pad = rate_kbps == 9000 ? 72 : R->ndbps;
+    TxJob job{}; job.rate_code = R->code; job.nbpsc = R->nbpsc; job.code_rate = R->cr; job.ndbps = R->ndbps; job.ndbps_pad = R->ndbps_pad;
     job.lead = lead_samples; job.fmt16 = sample_bits == 16;
+    TxCall c(h, cuda_stream, pay_off, pay_len, nframes);
     uint32_t max_nsym = 0;
-    rc = ft.load(h, st, payload_total, [&](uint32_t i, bool inside) {
-        if (ft.lenh[i] > 4091u || !inside) return h->fail(SB200_E_INVALID, "payload slot out of range (LENGTH is 12 bits incl. FCS)");
-        const uint32_t ns = tx11a_nsym(ft.lenh[i], job.ndbps, job.ndbps_pad);
-        if ((uint64_t)lead_samples + 640u + 160ull * (1u + ns) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
+    if ((rc = c.begin(payload, seeds)) != SB200_OK || (rc = upload_tables_tx(h)) != SB200_OK) return rc;
+    rc = c.load(payload_total, [&](uint32_t i, bool inside) {
+        if (c.ft.lenh[i] > 4091u || !inside) return h->fail(SB200_E_INVALID, "payload slot out of range (LENGTH is 12 bits incl. FCS)");
+        const uint32_t ns = tx11a_nsym(c.ft.lenh[i], job.ndbps, job.ndbps_pad);
+        if (lead_samples + tx11a_samples(ns) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
         if (ns > max_nsym) max_nsym = ns;
         return SB200_OK;
     });
     if (rc != SB200_OK) return rc;
     job.max_sym = 1u + max_nsym;
-    const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len; const uint8_t* d_seed = nullptr;
-    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay));
-    CK(ft.upload(h->txoff, h->txlen, st, &d_off, &d_len));
-    if (seeds) CK(to_device(h->txseed, seeds, is_device_ptr(seeds), nframes, st, &d_seed));
-    const size_t bps = sample_bits == 16 ? 4 : 2, out_bytes = (size_t)nframes * out_stride_samples * bps;
-    Returns ret; void* d_out; uint32_t* d_ns;
-    CK(ret.bind(h->txout, out, out_bytes, &d_out));
-    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
+    const uint8_t* d_seed = nullptr; void* d_out;
+    CK(c.stage(payload, payload_total));
+    if (seeds) CK(to_device(h->txseed, seeds, is_device_ptr(seeds), nframes, c.st, &d_seed));
+    CK(c.bind(out, (size_t)nframes * out_stride_samples * (sample_bits / 4u), &d_out, nsamples));
     const unsigned helpers = 8;                          // warps per frame for the preamble and the zero fill
-    dim3 grid(nframes, (job.max_sym + helpers + SB_TX_WARPS - 1) / SB_TX_WARPS);
-    CK(cudaEventRecord(h->ev0, st));
-    const uint32_t* d_crc; rc = crc_pass(h, st, d_pay, d_off, d_len, nframes, &d_crc); if (rc != SB200_OK) return rc;
-    k_tx11a<<<grid, 32 * SB_TX_WARPS, 0, st>>>(d_pay, d_off, d_len, d_seed, nframes, job, h->T, h->X, h->inv_deint, d_crc, d_out, out_stride_samples, d_ns);
-    return finish_call(h, st, ret, 0, 1);
+    const dim3 grid(nframes, (job.max_sym + helpers + SB_TX_WARPS - 1) / SB_TX_WARPS);
+    CK(c.start(true));
+    k_tx11a<<<grid, 32 * SB_TX_WARPS, 0, c.st>>>(c.d_pay, c.d_off, c.d_len, d_seed, nframes, job, h->T, h->X, h->inv_deint, c.d_crc, d_out, out_stride_samples, c.d_ns);
+    return c.finish(1);
 }
 
 // 802.11b transmit (tx11b_kernels.cuh)
 extern "C" int sb200_tx11b_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_total, const uint64_t* pay_off, const uint32_t* pay_len,
                                  uint32_t nframes, uint32_t rate_kbps, uint32_t init_phase, uint32_t lead_samples, uint32_t sample_bits, void* out,
                                  uint64_t out_stride_samples, uint32_t* nsamples, uint32_t* final_phase, void* cuda_stream) {
-    if (!h || !payload || !pay_off || !pay_len || !out) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
-    if (sample_bits != 8 && sample_bits != 16) return h->fail(SB200_E_INVALID, "sample_bits must be 8 (COMPLEX8) or 16 (COMPLEX16 = COMPLEX8 << 8)");
-    if (out_stride_samples % 8u || ((uintptr_t)out & 15u)) return h->fail(SB200_E_INVALID, "out must be 16-byte aligned and out_stride_samples a multiple of 8");
-    if (nframes == 0) return SB200_OK;
+    int rc = check_null(h, payload, pay_off, pay_len, out);
+    if (rc == SB200_OK) rc = check_out(h, sample_bits, out, out_stride_samples);
+    if (rc != SB200_OK || nframes == 0) return rc;
     Tx11bJob job{};
     job.rate_kbps = rate_kbps; job.lead = lead_samples; job.fmt16 = sample_bits == 16; job.init_phase = init_phase & 3u;
     const Rate11b* R = find_rate(kRates11b, rate_kbps);
@@ -121,13 +149,11 @@ extern "C" int sb200_tx11b_batch(sb200_handle* h, const uint8_t* payload, uint64
     }
     {   const int H[20] = SB_TX11B_TAPS;                                                    // the aligned kernel's compile-time copy
         for (int k = 0; k < 20; k++) if (job.taps[k] != H[k]) return h->fail(SB200_E_INVALID, "shaper taps differ from the compiled constants"); }
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    CK(cudaSetDevice(h->device));
-    CallScope call(h, st); CK(call.begin()); call.reads(payload);
-    FrameTable ft(pay_off, pay_len, nframes);
+    TxCall c(h, cuda_stream, pay_off, pay_len, nframes);
     uint32_t max_len = 0;
-    int rc = ft.load(h, st, payload_total, [&](uint32_t i, bool inside) {
-        const uint32_t len = ft.lenh[i];
+    if ((rc = c.begin(payload)) != SB200_OK) return rc;
+    rc = c.load(payload_total, [&](uint32_t i, bool inside) {
+        const uint32_t len = c.ft.lenh[i];
         if (len > 4091u || !inside) return h->fail(SB200_E_INVALID, "payload slot out of range (frame_length 1..4095 incl. FCS)");
         if ((uint64_t)lead_samples + tx11b_nsamples(tx11b_nchips(len, job.chips_per_byte)) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
         if (len > max_len) max_len = len;
@@ -135,63 +161,50 @@ extern "C" int sb200_tx11b_batch(sb200_handle* h, const uint8_t* payload, uint64
     });
     if (rc != SB200_OK) return rc;
     job.desc_stride = (24u + max_len + 4u + 7u) & ~7u;
-    const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len;
-    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay));
-    CK(ft.upload(h->txoff, h->txlen, st, &d_off, &d_len));
-    const size_t bps = sample_bits == 16 ? 4 : 2, out_bytes = (size_t)nframes * out_stride_samples * bps;
-    Returns ret; void* d_out; uint32_t* d_ns; uint32_t* d_fp;
-    CK(ret.bind(h->txout, out, out_bytes, &d_out));
-    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
-    CK(ret.bind(h->txseed, final_phase, nframes * 4ull, &d_fp));
-    CK(h->crc.need(nframes * 4ull)); CK(h->txdesc.need((size_t)nframes * job.desc_stride * 2ull));   // sized before ev0: crc_pass then finds it large enough
+    void* d_out; uint32_t* d_fp;
+    CK(c.stage(payload, payload_total));
+    CK(c.bind(out, (size_t)nframes * out_stride_samples * (sample_bits / 4u), &d_out, nsamples));
+    CK(c.ret.bind(h->txseed, final_phase, nframes * 4ull, &d_fp));
     const uint64_t per_cta = (uint64_t)SB_TX11B_THREADS * SB_TX11B_SPT, ny = (out_stride_samples + per_cta - 1) / per_cta;
     if (ny > 65535u || (uint64_t)lead_samples + out_stride_samples >= (1ull << 27)) return h->fail(SB200_E_INVALID, "out_stride_samples too large");
-    CK(cudaEventRecord(h->ev0, st));
-    const uint32_t* d_crc; rc = crc_pass(h, st, d_pay, d_off, d_len, nframes, &d_crc); if (rc != SB200_OK) return rc;
-    k_tx11b_code<<<(nframes + 127) / 128, 128, 0, st>>>(d_pay, d_off, d_len, nframes, job, d_crc, (uint16_t*)h->txdesc.p, d_fp);
-    {   const dim3 grid(nframes, (unsigned)ny); const uint16_t* dd = (const uint16_t*)h->txdesc.p; const bool al = lead_samples % 4u == 0;
-#define SB_TX11B_LAUNCH(R) do { if (al) k_tx11b_shape<true, R><<<grid, SB_TX11B_THREADS, 0, st>>>(d_len, job, dd, d_out, out_stride_samples, d_ns); \
-                                else k_tx11b_shape<false, R><<<grid, SB_TX11B_THREADS, 0, st>>>(d_len, job, dd, d_out, out_stride_samples, d_ns); } while (0)
-        switch (rate_kbps) { case 1000: SB_TX11B_LAUNCH(1000); break; case 2000: SB_TX11B_LAUNCH(2000); break; case 5500: SB_TX11B_LAUNCH(5500); break; default: SB_TX11B_LAUNCH(11000); break; }
-#undef SB_TX11B_LAUNCH
-    }
-    return finish_call(h, st, ret, 0, 2);
+    CK(c.start(true, (size_t)nframes * job.desc_stride * 2ull));
+    const uint16_t* dd = (const uint16_t*)h->txdesc.p; const dim3 grid(nframes, (unsigned)ny);
+    k_tx11b_code<<<(nframes + 127) / 128, 128, 0, c.st>>>(c.d_pay, c.d_off, c.d_len, nframes, job, c.d_crc, (uint16_t*)h->txdesc.p, d_fp);
+    with_index<4>((uint32_t)(R - kRates11b), [&](auto r) { with_index<2>(lead_samples % 4u == 0, [&](auto al) {
+        k_tx11b_shape<decltype(al)::value == 1, kRates11b[decltype(r)::value].kbps><<<grid, SB_TX11B_THREADS, 0, c.st>>>(c.d_len, job, dd, d_out, out_stride_samples, c.d_ns);
+    }); });
+    return c.finish(2);
 }
 
 // Legacy 802.11b transmit filter (tx11b_legacy_kernels.cuh): BB11BPMDSpreadFIR4SSE (variant 0) / BB11BPMDSpreadFIR4ASM (variant 1), batched.
 extern "C" int sb200_tx11b_fir37(sb200_handle* h, const int8_t* chips, uint64_t chips_total, const uint64_t* frame_off, const uint32_t* frame_len,
                                  uint32_t nframes, uint32_t variant, int8_t* out, void* cuda_stream) {
-    if (!h || !chips || !frame_off || !frame_len || !out) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
-    if (variant > 1) return h->fail(SB200_E_INVALID, "variant must be 0 (BB11BPMDSpreadFIR4SSE) or 1 (BB11BPMDSpreadFIR4ASM)");
-    if (nframes == 0) return SB200_OK;
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    CK(cudaSetDevice(h->device));
-    CallScope call(h, st); CK(call.begin()); call.reads(chips);
-    FrameTable ft(frame_off, frame_len, nframes);
-    const bool in_dev = is_device_ptr(chips), out_dev = is_device_ptr(out);
+    int rc = check_null(h, chips, frame_off, frame_len, out);
+    if (rc == SB200_OK && variant > 1) rc = h->fail(SB200_E_INVALID, "variant must be 0 (BB11BPMDSpreadFIR4SSE) or 1 (BB11BPMDSpreadFIR4ASM)");
+    if (rc != SB200_OK || nframes == 0) return rc;
+    TxCall c(h, cuda_stream, frame_off, frame_len, nframes);
     uint32_t max_len = 0;
-    const int rc = ft.load(h, st, chips_total, [&](uint32_t i, bool inside) {
-        if ((ft.lenh[i] & 7u) || (ft.offh[i] & 7u)) return h->fail(SB200_E_INVALID, "frame_off and frame_len must be multiples of 8 samples (the reference fails on uiInputSize & 7 and needs 16-byte aligned buffers)");
+    if ((rc = c.begin(chips)) != SB200_OK) return rc;
+    const bool in_dev = is_device_ptr(chips), out_dev = is_device_ptr(out);
+    rc = c.load(chips_total, [&](uint32_t i, bool inside) {
+        if ((c.ft.lenh[i] & 7u) || (c.ft.offh[i] & 7u)) return h->fail(SB200_E_INVALID, "frame_off and frame_len must be multiples of 8 samples (the reference fails on uiInputSize & 7 and needs 16-byte aligned buffers)");
         if (!inside) return h->fail(SB200_E_INVALID, "frame exceeds chips_total");
-        if (ft.lenh[i] > max_len) max_len = ft.lenh[i];
+        if (c.ft.lenh[i] > max_len) max_len = c.ft.lenh[i];
         return SB200_OK;
     });
     if (rc != SB200_OK) return rc;
     if ((in_dev && ((uintptr_t)chips & 15u)) || (out_dev && ((uintptr_t)out & 15u))) return h->fail(SB200_E_INVALID, "device buffers must be 16-byte aligned");
-    const int8_t* d_in; int8_t* d_out = out; const uint64_t* d_off; const uint32_t* d_len;
-    CK(to_device(h->txpay, chips, in_dev, chips_total * 2ull, st, &d_in, 16));
+    const int8_t* d_in; int8_t* d_out = out;
+    CK(to_device(h->txpay, chips, in_dev, chips_total * 2ull, c.st, &d_in, 16));
     if (!out_dev) { CK(h->txout.need(chips_total * 2ull + 16)); d_out = (int8_t*)h->txout.p; }
-    CK(ft.upload(h->txoff, h->txlen, st, &d_off, &d_len));
+    CK(c.ft.upload(h->txoff, h->txlen, c.st, &c.d_off, &c.d_len));
     const uint64_t groups = (uint64_t)(max_len >> 3) * 2u; uint64_t ny = (groups + SB_FIR37_THREADS - 1) / SB_FIR37_THREADS; if (ny > 4096) ny = 4096; if (ny == 0) ny = 1;
-    CK(cudaEventRecord(h->ev0, st));
-    const dim3 grid(nframes, (unsigned)ny);
-    if (variant == 0) k_fir37_legacy<0><<<grid, SB_FIR37_THREADS, 0, st>>>(d_in, d_off, d_len, nframes, d_out);
-    else k_fir37_legacy<1><<<grid, SB_FIR37_THREADS, 0, st>>>(d_in, d_off, d_len, nframes, d_out);
-    Returns none;                                       // only the frames' own ranges are defined: copied back one by one below (they may be sparse in the buffer)
-    const int frc = finish_call(h, st, none, 0, 1);
+    CK(c.start(false));
+    with_index<2>(variant, [&](auto v) { k_fir37_legacy<decltype(v)::value><<<dim3(nframes, (unsigned)ny), SB_FIR37_THREADS, 0, c.st>>>(d_in, c.d_off, c.d_len, nframes, d_out); });
+    const int frc = c.finish(1);                        // nothing bound: only the frames' own ranges are defined, copied back one by one below (they may be sparse in the buffer)
     if (frc != SB200_OK || out_dev) return frc;
-    for (uint32_t i = 0; i < nframes; i++) if (ft.lenh[i]) CK(cudaMemcpyAsync(out + 2ull * ft.offh[i], d_out + 2ull * ft.offh[i], 2ull * ft.lenh[i], cudaMemcpyDeviceToHost, st));
-    CK(cudaStreamSynchronize(st));
+    for (uint32_t i = 0; i < nframes; i++) if (c.ft.lenh[i]) CK(cudaMemcpyAsync(out + 2ull * c.ft.offh[i], d_out + 2ull * c.ft.offh[i], 2ull * c.ft.lenh[i], cudaMemcpyDeviceToHost, c.st));
+    CK(cudaStreamSynchronize(c.st));
     return SB200_OK;
 }
 
@@ -199,25 +212,23 @@ extern "C" int sb200_tx11b_fir37(sb200_handle* h, const int8_t* chips, uint64_t 
 extern "C" int sb200_tx11b_legacy_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_total, const uint64_t* pay_off, const uint32_t* pay_len,
                                         uint32_t nframes, uint32_t rate_kbps, uint32_t short_preamble, uint32_t flags, uint32_t filter, int8_t* out,
                                         uint64_t out_stride_samples, uint32_t* nsamples, void* cuda_stream) {
-    if (!h || !payload || !pay_off || !pay_len || !out) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
+    int rc = check_null(h, payload, pay_off, pay_len, out);
+    if (rc != SB200_OK) return rc;
     if (flags & SB200_TX11B_LEGACY_PBCC) return h->fail(SB200_E_INVALID, "PBCC is not supported: the reference only lengthens PLCPGetLength for it and still sends CCK");
     if (flags & ~SB200_TX11B_LEGACY_FCS_IN_PAYLOAD) return h->fail(SB200_E_INVALID, "unknown flags");
     if (filter > 2) return h->fail(SB200_E_INVALID, "filter must be 0 (encoder output), 1 (BB11BPMDSpreadFIR4SSE) or 2 (BB11BPMDSpreadFIR4ASM)");
     if (short_preamble > 1) return h->fail(SB200_E_INVALID, "short_preamble must be 0 or 1");
-    if (out_stride_samples % 8u || ((uintptr_t)out & 15u)) return h->fail(SB200_E_INVALID, "out must be 16-byte aligned and out_stride_samples a multiple of 8");
-    if (nframes == 0) return SB200_OK;
+    if ((rc = check_out(h, 8, out, out_stride_samples)) != SB200_OK || nframes == 0) return rc;
     Tx11bLegacyJob job{};
     job.rate_kbps = rate_kbps; job.short_preamble = short_preamble; job.fcs_in_payload = (flags & SB200_TX11B_LEGACY_FCS_IN_PAYLOAD) ? 1u : 0u; job.filter = filter;
     const Rate11b* R = find_rate(kRates11b, rate_kbps);
     if (!R) return h->fail(SB200_E_INVALID, "rate_kbps is not an 802.11b rate");
-    job.rate_code = R->code; job.data_chips_per_byte = short_preamble && rate_kbps == 1000 ? 0u : R->chips_per_byte;   // the short preamble's 1 Mbps case sends no data chips
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    CK(cudaSetDevice(h->device));
-    CallScope call(h, st); CK(call.begin()); call.reads(payload);
-    FrameTable ft(pay_off, pay_len, nframes);
+    job.rate_code = R->code; job.data_chips_per_byte = tx11b_legacy_data_chips(*R, short_preamble);
+    TxCall c(h, cuda_stream, pay_off, pay_len, nframes);
     uint32_t max_size = 0;
-    int rc = ft.load(h, st, payload_total, [&](uint32_t i, bool inside) {
-        const uint32_t len = ft.lenh[i], size = job.fcs_in_payload ? len : len + 4u;    // PSDU bytes, FCS included
+    if ((rc = c.begin(payload)) != SB200_OK) return rc;
+    rc = c.load(payload_total, [&](uint32_t i, bool inside) {
+        const uint32_t len = c.ft.lenh[i], size = job.fcs_in_payload ? len : len + 4u;    // PSDU bytes, FCS included
         if (job.fcs_in_payload && len < 4u) return h->fail(SB200_E_INVALID, "with SB200_TX11B_LEGACY_FCS_IN_PAYLOAD every payload carries its 4 FCS bytes");
         if (len > 4095u || size > 4095u || !inside) return h->fail(SB200_E_INVALID, "payload slot out of range (PSDU 4 .. 4095 bytes incl. FCS)");
         if (tx11b_legacy_nsamples(size, short_preamble, job.data_chips_per_byte) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
@@ -226,50 +237,39 @@ extern "C" int sb200_tx11b_legacy_batch(sb200_handle* h, const uint8_t* payload,
     });
     if (rc != SB200_OK) return rc;
     job.desc_stride = (24u + max_size + 7u) & ~7u;
-    const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len;
-    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay));
-    CK(ft.upload(h->txoff, h->txlen, st, &d_off, &d_len));
-    const size_t out_bytes = (size_t)nframes * out_stride_samples * 2;
-    Returns ret; int8_t* d_out; uint32_t* d_ns;
-    CK(ret.bind(h->txout, out, out_bytes, &d_out));
-    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
-    CK(h->txdesc.need((size_t)nframes * job.desc_stride * 2ull));
+    int8_t* d_out;
+    CK(c.stage(payload, payload_total));
+    CK(c.bind(out, (size_t)nframes * out_stride_samples * 2, &d_out, nsamples));
     const uint64_t per_cta = SB_TX11B_LEGACY_THREADS * 8, ny = (out_stride_samples + per_cta - 1) / per_cta;
     if (ny > 65535u) return h->fail(SB200_E_INVALID, "out_stride_samples too large");
-    CK(cudaEventRecord(h->ev0, st));
-    const uint32_t* d_crc = nullptr;
-    if (!job.fcs_in_payload) { rc = crc_pass(h, st, d_pay, d_off, d_len, nframes, &d_crc); if (rc != SB200_OK) return rc; }
-    k_tx11b_legacy_code<<<(nframes + 127) / 128, 128, 0, st>>>(d_pay, d_off, d_len, nframes, job, d_crc, (uint16_t*)h->txdesc.p);
-    const dim3 grid(nframes, (unsigned)ny); const uint16_t* dd = (const uint16_t*)h->txdesc.p;
-    if (filter == 0) k_tx11b_legacy_spread<0><<<grid, SB_TX11B_LEGACY_THREADS, 0, st>>>(d_len, job, dd, d_out, out_stride_samples, d_ns);
-    else if (filter == 1) k_tx11b_legacy_spread<1><<<grid, SB_TX11B_LEGACY_THREADS, 0, st>>>(d_len, job, dd, d_out, out_stride_samples, d_ns);
-    else k_tx11b_legacy_spread<2><<<grid, SB_TX11B_LEGACY_THREADS, 0, st>>>(d_len, job, dd, d_out, out_stride_samples, d_ns);
-    return finish_call(h, st, ret, 0, 2);
+    CK(c.start(!job.fcs_in_payload, (size_t)nframes * job.desc_stride * 2ull));
+    const uint16_t* dd = (const uint16_t*)h->txdesc.p;
+    k_tx11b_legacy_code<<<(nframes + 127) / 128, 128, 0, c.st>>>(c.d_pay, c.d_off, c.d_len, nframes, job, c.d_crc, (uint16_t*)h->txdesc.p);
+    with_index<3>(filter, [&](auto f) {
+        k_tx11b_legacy_spread<decltype(f)::value><<<dim3(nframes, (unsigned)ny), SB_TX11B_LEGACY_THREADS, 0, c.st>>>(c.d_len, job, dd, d_out, out_stride_samples, c.d_ns);
+    });
+    return c.finish(2);
 }
 
 // Legacy 802.11a transmitter (tx11a_legacy_kernels.cuh): BB11ATxFrameMod / BB11ATxBufferMod6M at SampleRate 40 or 44.
 extern "C" int sb200_tx11a_legacy_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_total, const uint64_t* pay_off, const uint32_t* pay_len,
                                         uint32_t nframes, uint32_t rate_kbps, uint32_t sample_rate_mhz, uint32_t flags, const int16_t* preamble, int8_t* out,
                                         uint64_t out_stride_samples, uint32_t* nsamples, void* cuda_stream) {
-    if (!h || !payload || !pay_off || !pay_len || !out || !preamble) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
+    int rc = check_null(h, payload, pay_off, pay_len, out, preamble);
+    if (rc != SB200_OK) return rc;
     if (flags & ~SB200_TX11A_LEGACY_FCS_IN_PAYLOAD) return h->fail(SB200_E_INVALID, "unknown flags");
     if (sample_rate_mhz != 40 && sample_rate_mhz != 44) return h->fail(SB200_E_INVALID, "sample_rate_mhz must be 40 or 44");
-    if (out_stride_samples % 8u || ((uintptr_t)out & 15u)) return h->fail(SB200_E_INVALID, "out must be 16-byte aligned and out_stride_samples a multiple of 8");
-    if (nframes == 0) return SB200_OK;
+    if ((rc = check_out(h, 8, out, out_stride_samples)) != SB200_OK || nframes == 0) return rc;
     const Rate11a* R = find_rate(kRates11a, rate_kbps);
     if (!R) return h->fail(SB200_E_INVALID, "rate_kbps is not an 802.11a rate");
     Tx11aLegacyJob job{};
     job.rate_code = R->code; job.nbpsc = R->nbpsc; job.code_rate = R->cr; job.ndbps = R->ndbps;
     job.sr44 = sample_rate_mhz == 44; job.fcs_in_payload = (flags & SB200_TX11A_LEGACY_FCS_IN_PAYLOAD) ? 1u : 0u;
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    CK(cudaSetDevice(h->device));
-    CallScope call(h, st); CK(call.begin()); call.reads(payload); call.reads(preamble);
-    int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
-    FrameTable ft(pay_off, pay_len, nframes);
-    const bool pre_dev = is_device_ptr(preamble);
+    TxCall c(h, cuda_stream, pay_off, pay_len, nframes);
     uint32_t max_nsym = 0;
-    rc = ft.load(h, st, payload_total, [&](uint32_t i, bool inside) {
-        const uint32_t len = ft.lenh[i], size = job.fcs_in_payload ? len : len + 4u;    // PSDU bytes, FCS included
+    if ((rc = c.begin(payload, preamble)) != SB200_OK || (rc = upload_tables_tx(h)) != SB200_OK) return rc;
+    rc = c.load(payload_total, [&](uint32_t i, bool inside) {
+        const uint32_t len = c.ft.lenh[i], size = job.fcs_in_payload ? len : len + 4u;    // PSDU bytes, FCS included
         if (job.fcs_in_payload && len < 4u) return h->fail(SB200_E_INVALID, "with SB200_TX11A_LEGACY_FCS_IN_PAYLOAD every payload carries its 4 FCS bytes");
         if (len > 4096u || size > 4096u || !inside) return h->fail(SB200_E_INVALID, "payload slot out of range (MPDU + FCS at most 4096 bytes)");
         const uint32_t ns = tx11a_legacy_nsym(size, job.ndbps);
@@ -279,23 +279,17 @@ extern "C" int sb200_tx11a_legacy_batch(sb200_handle* h, const uint8_t* payload,
     });
     if (rc != SB200_OK) return rc;
     job.runs = (1u + max_nsym + SB_TXL_RUN - 1u) / SB_TXL_RUN;
-    const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len; const uint32_t* d_pre;
-    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay, 1));
-    CK(ft.upload(h->txoff, h->txlen, st, &d_off, &d_len));
+    const uint32_t* d_pre; int8_t* d_out; const bool pre_dev = is_device_ptr(preamble);
+    CK(c.stage(payload, payload_total, 1));
     if (pre_dev && ((uintptr_t)preamble & 3u) == 0) d_pre = (const uint32_t*)preamble;
-    else { CK(h->txpre.need(640 * 4)); CK(cudaMemcpyAsync(h->txpre.p, preamble, 640 * 4, pre_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, st)); d_pre = (const uint32_t*)h->txpre.p; }
-    const size_t out_bytes = (size_t)nframes * out_stride_samples * 2;
-    Returns ret; int8_t* d_out; uint32_t* d_ns;
-    CK(ret.bind(h->txout, out, out_bytes, &d_out));
-    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
+    else { CK(h->txpre.need(640 * 4)); CK(cudaMemcpyAsync(h->txpre.p, preamble, 640 * 4, pre_dev ? cudaMemcpyDeviceToDevice : cudaMemcpyHostToDevice, c.st)); d_pre = (const uint32_t*)h->txpre.p; }
+    CK(c.bind(out, (size_t)nframes * out_stride_samples * 2, &d_out, nsamples));
     const unsigned helpers = 4;                          // warps per frame for the preamble and the zero fill
     const uint64_t ny = (job.runs + helpers + SB_TXL_WARPS - 1) / SB_TXL_WARPS;
     if (ny > 65535u) return h->fail(SB200_E_INVALID, "too many symbols per frame");
-    CK(cudaEventRecord(h->ev0, st));
-    const uint32_t* d_crc = nullptr;
-    if (!job.fcs_in_payload) { rc = crc_pass(h, st, d_pay, d_off, d_len, nframes, &d_crc); if (rc != SB200_OK) return rc; }
-    k_tx11a_legacy<<<dim3(nframes, (unsigned)ny), 32 * SB_TXL_WARPS, 0, st>>>(d_pay, d_off, d_len, nframes, job, h->T, h->X, h->inv_deint, d_crc, d_pre, d_out, out_stride_samples, d_ns);
-    return finish_call(h, st, ret, 0, 1);
+    CK(c.start(!job.fcs_in_payload));
+    k_tx11a_legacy<<<dim3(nframes, (unsigned)ny), 32 * SB_TXL_WARPS, 0, c.st>>>(c.d_pay, c.d_off, c.d_len, nframes, job, h->T, h->X, h->inv_deint, c.d_crc, d_pre, d_out, out_stride_samples, c.d_ns);
+    return c.finish(1);
 }
 
 // 802.11n transmit (tx11n_kernels.cuh)
@@ -363,49 +357,32 @@ static int upload_tables_tx11n(sb200_handle* h) {
 extern "C" int sb200_tx11n_batch(sb200_handle* h, const uint8_t* payload, uint64_t payload_total, const uint64_t* pay_off, const uint32_t* pay_len, const uint8_t* seeds,
                                  uint32_t nframes, uint32_t mcs, uint32_t lead_samples, int16_t* out0, int16_t* out1, uint64_t out_stride_samples,
                                  uint32_t* nsamples, void* cuda_stream) {
-    if (!h || !payload || !pay_off || !pay_len || !out0 || !out1) return h ? h->fail(SB200_E_INVALID, "null argument") : SB200_E_INVALID;
-    if (nframes == 0) return SB200_OK;
-    Tx11nJob job{}; job.mcs = mcs; job.lead = lead_samples;
-    switch (mcs) {                                      // ieee80211const.h:35-55; the range the receiver accepts (PHY_11n.hpp:496-501)
-        case 8:  job.nbpsc = 1; job.code_rate = CR_12; job.ndbps = 52;  job.enc_in = 1; job.parse_in = 13; break;
-        case 9:  job.nbpsc = 2; job.code_rate = CR_12; job.ndbps = 104; job.enc_in = 1; job.parse_in = 26; break;
-        case 10: job.nbpsc = 2; job.code_rate = CR_34; job.ndbps = 156; job.enc_in = 3; job.parse_in = 26; break;
-        case 11: job.nbpsc = 4; job.code_rate = CR_12; job.ndbps = 208; job.enc_in = 1; job.parse_in = 52; break;      // the 16-QAM / 64-QAM branches of the modulator graph
-        case 12: job.nbpsc = 4; job.code_rate = CR_34; job.ndbps = 312; job.enc_in = 3; job.parse_in = 52; break;      // (fb11nmod_config.hpp:133-155: enc11 .. enc14)
-        case 13: job.nbpsc = 6; job.code_rate = CR_23; job.ndbps = 416; job.enc_in = 2; job.parse_in = 78; break;
-        case 14: job.nbpsc = 6; job.code_rate = CR_34; job.ndbps = 468; job.enc_in = 3; job.parse_in = 78; break;
-        default: return h->fail(SB200_E_INVALID, "mcs must be 8 .. 14");
-    }
-    cudaStream_t st = (cudaStream_t)cuda_stream;
-    CK(cudaSetDevice(h->device));
-    CallScope call(h, st); CK(call.begin()); call.reads(payload); call.reads(seeds);
-    int rc = upload_tables_tx(h); if (rc != SB200_OK) return rc;
-    rc = upload_tables_tx11n(h); if (rc != SB200_OK) return rc;
-    FrameTable ft(pay_off, pay_len, nframes);
-    if (is_device_ptr(out0) != is_device_ptr(out1)) return h->fail(SB200_E_INVALID, "both output buffers must live on the same side");
+    int rc = check_null(h, payload, pay_off, pay_len, out0, out1);
+    if (rc != SB200_OK || nframes == 0) return rc;
+    const Mcs11n* M = find_rate(kMcs11n, mcs, &Mcs11n::mcs);
+    if (!M) return h->fail(SB200_E_INVALID, "mcs must be 8 .. 14");
+    Tx11nJob job = tx11n_job(*M, lead_samples);
+    TxCall c(h, cuda_stream, pay_off, pay_len, nframes);
     uint32_t max_nsym = 0;
-    rc = ft.load(h, st, payload_total, [&](uint32_t i, bool inside) {
-        if (ft.lenh[i] > 4091u || !inside) return h->fail(SB200_E_INVALID, "payload slot out of range");
-        const uint32_t ns = tx11n_nsym_emitted(ft.lenh[i], job, nullptr, nullptr);
-        if ((uint64_t)lead_samples + 1600u + 160ull * ns > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
+    if ((rc = c.begin(payload, seeds)) != SB200_OK || (rc = upload_tables_tx(h)) != SB200_OK || (rc = upload_tables_tx11n(h)) != SB200_OK) return rc;
+    if (is_device_ptr(out0) != is_device_ptr(out1)) return h->fail(SB200_E_INVALID, "both output buffers must live on the same side");
+    rc = c.load(payload_total, [&](uint32_t i, bool inside) {
+        if (c.ft.lenh[i] > 4091u || !inside) return h->fail(SB200_E_INVALID, "payload slot out of range");
+        const uint32_t ns = tx11n_nsym_emitted(c.ft.lenh[i], job, nullptr, nullptr);
+        if (lead_samples + tx11n_samples(ns) > out_stride_samples) return h->fail(SB200_E_INVALID, "out_stride_samples too small for the frame");
         if (ns > max_nsym) max_nsym = ns;
         return SB200_OK;
     });
     if (rc != SB200_OK) return rc;
     job.max_sym = 3u + max_nsym;
-    const uint8_t* d_pay; const uint64_t* d_off; const uint32_t* d_len; const uint8_t* d_seed = nullptr;
-    CK(to_device(h->txpay, payload, is_device_ptr(payload), payload_total, st, &d_pay));
-    CK(ft.upload(h->txoff, h->txlen, st, &d_off, &d_len));
-    if (seeds) CK(to_device(h->txseed, seeds, is_device_ptr(seeds), nframes, st, &d_seed));
-    const size_t out_bytes = (size_t)nframes * out_stride_samples * 4;
-    Returns ret; int16_t* d_o0; int16_t* d_o1; uint32_t* d_ns;
-    CK(ret.bind(h->txout, out0, out_bytes, &d_o0));
-    CK(ret.bind(h->txout1, out1, out_bytes, &d_o1));
-    CK(ret.bind(h->txns, nsamples, nframes * 4ull, &d_ns));
+    const uint8_t* d_seed = nullptr; int16_t* d_o0; int16_t* d_o1; const size_t out_bytes = (size_t)nframes * out_stride_samples * 4;
+    CK(c.stage(payload, payload_total));
+    if (seeds) CK(to_device(h->txseed, seeds, is_device_ptr(seeds), nframes, c.st, &d_seed));
+    CK(c.bind(out0, out_bytes, &d_o0, nsamples));
+    CK(c.ret.bind(h->txout1, out1, out_bytes, &d_o1));
     const unsigned helpers = 8;
-    dim3 grid(nframes, (2u * job.max_sym + helpers + SB_TX11N_WARPS - 1) / SB_TX11N_WARPS);
-    CK(cudaEventRecord(h->ev0, st));
-    const uint32_t* d_crc; rc = crc_pass(h, st, d_pay, d_off, d_len, nframes, &d_crc); if (rc != SB200_OK) return rc;
-    k_tx11n<<<grid, 32 * SB_TX11N_WARPS, 0, st>>>(d_pay, d_off, d_len, d_seed, nframes, job, h->T, h->X, h->XN, h->inv_deint, d_crc, (uint32_t*)d_o0, (uint32_t*)d_o1, out_stride_samples, d_ns);
-    return finish_call(h, st, ret, 0, 1);
+    const dim3 grid(nframes, (2u * job.max_sym + helpers + SB_TX11N_WARPS - 1) / SB_TX11N_WARPS);
+    CK(c.start(true));
+    k_tx11n<<<grid, 32 * SB_TX11N_WARPS, 0, c.st>>>(c.d_pay, c.d_off, c.d_len, d_seed, nframes, job, h->T, h->X, h->XN, h->inv_deint, c.d_crc, (uint32_t*)d_o0, (uint32_t*)d_o1, out_stride_samples, c.d_ns);
+    return c.finish(1);
 }

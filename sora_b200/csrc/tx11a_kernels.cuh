@@ -14,6 +14,7 @@
 #pragma once
 #include "tables.cuh"
 #include "viterbi_k7_common.cuh"
+#include "tx_frames.cuh"
 
 namespace sb {
 
@@ -103,10 +104,6 @@ struct TxJob {
     uint32_t lead, fmt16;                           // zero samples in front of the preamble; 0 = COMPLEX8 out, 1 = COMPLEX16 (<< 8)
     uint32_t max_sym;                               // symbols per frame the grid covers (SIGNAL included)
 };
-__host__ __device__ inline uint32_t tx11a_nsym(uint32_t len, uint32_t ndbps, uint32_t ndbps_pad) {   // TBB11aSrc::GetPadingByte
-    const uint32_t bits = (2u + len + 4u + 1u) * 8u, padded = (bits + ndbps_pad - 1u) / ndbps_pad * ndbps_pad;
-    return (bits + ((padded - bits + 7u) / 8u) * 8u) / ndbps;
-}
 
 // CRC-32 of every MPDU (what fb11amod_config.hpp:40 stores in CF_11aTxVector::crc32): one thread per frame
 __global__ void __launch_bounds__(128) k_tx11a_crc(const uint8_t* __restrict__ payload, const uint64_t* __restrict__ pay_off, const uint32_t* __restrict__ pay_len,

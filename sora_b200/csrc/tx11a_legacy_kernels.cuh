@@ -20,6 +20,7 @@
 //   Upsample40MTo44M_3, then four zeros), zeros to the end of the slot.  Every store is 16 bytes (eight COMPLEX8 samples).
 #pragma once
 #include "tx11a_kernels.cuh"
+#include "tx_frames.cuh"
 
 namespace sb {
 
@@ -29,10 +30,6 @@ struct Tx11aLegacyJob {
     uint32_t fcs_in_payload;                        // 1: the payload's last four bytes are the FCS; 0: CRC-32 appended
     uint32_t runs;                                  // symbol warps per frame (the rest of the frame's warps are helpers)
 };
-__host__ __device__ inline uint32_t tx11a_legacy_nsym(uint32_t psdu_len, uint32_t ndbps) { return (22u + 8u * psdu_len + ndbps - 1u) / ndbps; }
-// GetSignalBytes / 2 (atx_tpl.h:69-83) and its RCB padding to 128 bytes (_tx_manager2.h:29-38)
-__host__ __device__ inline uint32_t tx11a_legacy_signal(uint32_t nsym, uint32_t sr44) { return (sr44 ? 176u : 160u) * (5u + nsym) + 8u; }
-__host__ __device__ inline uint32_t tx11a_legacy_padded(uint32_t nsym, uint32_t sr44) { return (tx11a_legacy_signal(nsym, sr44) + 63u) & ~63u; }
 
 #define SB_TXL_WARPS 4
 #ifndef SB_TXL_RUN

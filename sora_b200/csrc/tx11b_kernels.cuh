@@ -14,6 +14,7 @@
 //                  Reference: barkerspread.hpp:48-65,160-188; cck.hpp:797-828,893-918; pulse.hpp:260-379; stdbrick.hpp:413-445,278-330.
 #pragma once
 #include "tx11a_kernels.cuh"
+#include "tx_frames.cuh"
 
 namespace sb {
 
@@ -25,8 +26,6 @@ struct Tx11bJob {
     uint32_t desc_stride;                // descriptors per frame row
     short taps[20];                      // h(8) .. h(-11), pulse.hpp:279-305 (built on the host from the reference's formula)
 };
-__host__ __device__ inline uint32_t tx11b_nchips(uint32_t len, uint32_t chips_per_byte) { return 24u * 88u + (len + 4u) * chips_per_byte; }
-__host__ __device__ inline uint32_t tx11b_nsamples(uint32_t nchips) { return ((nchips + 5u) * 4u + 7u) / 8u * 8u; }   // + 5 flush vectors, bursts of 8
 
 // quarter turns of the reference's two phase alphabets and the way back
 //   DQPSKEncode[]  = {1, -j, +j, -1} (cck.hpp:766)      -> 0, 3, 1, 2

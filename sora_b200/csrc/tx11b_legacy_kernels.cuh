@@ -14,6 +14,7 @@
 //   variant 1 (FIR37SSE_INLINE, bbb_fir.c:137-386): the plain filter.
 #pragma once
 #include "tx11b_kernels.cuh"
+#include "tx_frames.cuh"
 
 namespace sb {
 
@@ -104,12 +105,6 @@ struct Tx11bLegacyJob {
     uint32_t filter;                     // 0 encoder output, 1 BB11BPMDSpreadFIR4SSE, 2 BB11BPMDSpreadFIR4ASM
     uint32_t desc_stride;                // descriptors per frame row
 };
-__host__ __device__ inline uint32_t tx11b_legacy_plcp_bytes(uint32_t short_preamble) { return short_preamble ? 15u : 24u; }
-__host__ __device__ inline uint32_t tx11b_legacy_header_chips(uint32_t short_preamble) { return short_preamble ? 9u * 88u + 6u * 44u : 24u * 88u; }
-__host__ __device__ inline uint32_t tx11b_legacy_nsamples(uint32_t psdu_len, uint32_t short_preamble, uint32_t data_chips_per_byte) {
-    const uint32_t n = 4u * (tx11b_legacy_header_chips(short_preamble) + psdu_len * data_chips_per_byte);
-    return (n + 37u + 127u) & ~127u;                                                   // TX_FIR_DEPTH zeros, rounded up to a multiple of 128
-}
 
 __global__ void __launch_bounds__(128) k_tx11b_legacy_code(const uint8_t* __restrict__ payload, const uint64_t* __restrict__ pay_off,
         const uint32_t* __restrict__ pay_len, uint32_t nframes, Tx11bLegacyJob job, const uint32_t* __restrict__ crcs, uint16_t* __restrict__ desc) {

@@ -12,23 +12,9 @@
 //             fft.hpp:62-101; csd.hpp:38-51; gi.hpp:32-41; preamble11n.hpp:9-80.
 #pragma once
 #include "tx11a_kernels.cuh"
+#include "tx_frames.cuh"
 
 namespace sb {
-
-struct Tx11nJob {
-    uint32_t mcs, nbpsc, code_rate, ndbps;   // 8..14; N_BPSCS; CR_12 / CR_23 / CR_34; N_DBPS over both streams
-    uint32_t enc_in, parse_in;               // input bursts of the encoder and of the stream parser, bytes (conv_enc.hpp, streamparser.hpp)
-    uint32_t lead, max_sym;                  // zero samples in front; symbols per frame the grid covers (3 SIG + data)
-};
-__host__ __device__ inline uint32_t tx11n_nsym_signalled(uint32_t len, uint32_t ndbps) { return ((len + 4u) * 8u + 16u + 6u + ndbps - 1u) / ndbps; }   // ht_symbol_count
-// data symbols the graph emits: the Flush padding (FlushPort: encoder burst, then stream-parser burst) can add one
-__host__ __device__ inline uint32_t tx11n_nsym_emitted(uint32_t len, const Tx11nJob& j, uint32_t* enc_bits, uint32_t* coded_bits) {
-    const uint32_t ns = tx11n_nsym_signalled(len, j.ndbps);
-    uint32_t bytes = (ns * j.ndbps + 7u) / 8u; bytes = (bytes + j.enc_in - 1u) / j.enc_in * j.enc_in;
-    const uint32_t cbytes = j.code_rate == CR_12 ? 2u * bytes : j.code_rate == CR_34 ? bytes / 3u * 4u : bytes / 2u * 3u;
-    if (enc_bits) *enc_bits = bytes * 8u; if (coded_bits) *coded_bits = cbytes * 8u;
-    return (cbytes + j.parse_in - 1u) / j.parse_in;
-}
 
 #define SB_TX11N_WARPS 4
 __global__ void __launch_bounds__(32 * SB_TX11N_WARPS) k_tx11n(const uint8_t* __restrict__ payload, const uint64_t* __restrict__ pay_off, const uint32_t* __restrict__ pay_len,

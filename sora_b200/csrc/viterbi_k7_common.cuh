@@ -5,6 +5,7 @@
 // Arithmetic contract and machine mapping: see viterbi_k7_re.cuh (history-carrying metrics, in-place trellis).
 #pragma once
 #include <stdint.h>
+#include "tx_frames.cuh"                     // CR_12 / CR_23 / CR_34
 
 namespace sb {
 
@@ -12,7 +13,6 @@ enum : uint32_t {
     E_SUCCESS = 0, E_FRAME_OK = 1, E_FAILED = 0x8000FFFFu, E_PLCP_HEADER_FAIL = 0x80000005u,
     E_CRC32_FAIL = 0x80000006u, E_CS_TIMEOUT = 0x80000007u, E_NO_FRAME = 0x8000F001u,
 };
-enum { CR_12 = 0, CR_23 = 1, CR_34 = 2 };
 
 struct FrameInfo {            // per-slot state handed from kernel to kernel (device memory)
     uint32_t status;          // E_SUCCESS while decoding proceeds, else terminal code

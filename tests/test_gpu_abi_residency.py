@@ -168,14 +168,14 @@ def _payloads(lens, seed):
 
 def test_tx11a_batch(eng):
     pay, off, ln = _payloads([40, 300, 77], 0xAB80); F = 3
-    stride = 20 + 640 + 160 * (2 + -(-(300 + 7) * 8 // 144)) + 32
+    stride = api.Engine.tx11a_out_stride(300, 36000, lead=20)
     args = dict(pay=pay, off=off, len=ln, seeds=np.array([0x11, 0x5A, 0x7F], np.uint8), out=_fill(F * stride * 4), ns=_fill(F * 4))
     call = lambda p: eng.tx11a_raw(p["pay"], pay.size, p["off"], p["len"], p["seeds"], F, 36000, 20, 16, p["out"], stride, p["ns"])
     _matrix(call, args, _each(*args))
 
 def test_tx11b_batch(eng):
     pay, off, ln = _payloads([30, 64], 0xAB90); F = 2
-    stride = ((24 * 88 + (64 + 4) * 16 + 5) * 4 + 15) // 8 * 8
+    stride = api.Engine.tx11b_out_stride(64, 5500)
     args = dict(pay=pay, off=off, len=ln, out=_fill(F * stride * 2), ns=_fill(F * 4), fp=_fill(F * 4))
     call = lambda p: eng.tx11b_raw(p["pay"], pay.size, p["off"], p["len"], F, 5500, 1, 0, 8, p["out"], stride, p["ns"], 0, p["fp"])
     _matrix(call, args, _each(*args))
@@ -195,7 +195,7 @@ def test_tx11b_fir37(eng):
 
 def test_tx11b_legacy_batch(eng):
     pay, off, ln = _payloads([20, 50], 0xABB0); F = 2
-    stride = (4 * (1056 + 54 * 16) + 37 + 127) // 128 * 128
+    stride = api.Engine.tx11b_legacy_nsamples(54, 5500, short_preamble=True)
     args = dict(pay=pay, off=off, len=ln, out=_fill(F * stride * 2), ns=_fill(F * 4))
     call = lambda p: eng.tx11b_legacy_raw(p["pay"], pay.size, p["off"], p["len"], F, 5500, 1, 0, 1, p["out"], stride, p["ns"])
     _matrix(call, args, _each(*args))
@@ -212,7 +212,7 @@ def test_tx11a_legacy_batch(eng):
 
 def test_tx11n_batch(eng):
     pay, off, ln = _payloads([50, 120], 0xABD0); F = 2
-    stride = 10 + 1600 + 160 * (-(-((120 + 4) * 8 + 22) // 104) + 1)
+    stride = api.Engine.tx11n_out_stride(120, 9, lead=10)
     args = dict(pay=pay, off=off, len=ln, seeds=np.array([0x33, 0x44], np.uint8), out0=_fill(F * stride * 4), out1=_fill(F * stride * 4), ns=_fill(F * 4))
     call = lambda p: eng.tx11n_raw(p["pay"], pay.size, p["off"], p["len"], p["seeds"], F, 9, 10, p["out0"], p["out1"], stride, p["ns"])
     _matrix(call, args, _each("pay", "off", "len", "seeds") + [("out0", "out1"), ("ns",)])

@@ -42,8 +42,7 @@ def test_loopback_tx_to_rx_on_device(eng):
         pay = rng.integers(0, 256, (F, L)).astype(np.uint8)
         d_pay = torch.from_numpy(pay.reshape(-1)).cuda()
         d_off = torch.arange(F, dtype=torch.int64, device="cuda") * L; d_len = torch.full((F,), L, dtype=torch.int32, device="cuda")
-        nd = synth.RATES[rate][3]; nsym = -(-(L + 7) * 8 // nd) + 1
-        slot = (400 + 640 + 160 * (1 + nsym) + 400 + 27) // 28 * 28
+        slot = (api.Engine.tx11a_out_stride(L, rate, lead=400) + 400 + 27) // 28 * 28   # the default slot and 400 samples of silence
         d_iq = torch.zeros((F, slot, 2), dtype=torch.int16, device="cuda"); d_ns = torch.zeros(F, dtype=torch.int32, device="cuda")
         eng.tx11a_raw(d_pay.data_ptr(), F * L, d_off.data_ptr(), d_len.data_ptr(), 0, F, rate, 400, 16, d_iq.data_ptr(), slot, d_ns.data_ptr(), torch.cuda.current_stream().cuda_stream)
         s_off = torch.arange(F, dtype=torch.int64, device="cuda") * slot; s_len = torch.full((F,), slot, dtype=torch.int32, device="cuda")

@@ -50,8 +50,7 @@ def test_loopback_tx_to_rx_on_device(eng, rate, L, F):
     pay = rng.integers(0, 256, (F, L)).astype(np.uint8)
     d_pay = torch.from_numpy(pay.reshape(-1)).cuda()
     d_off = torch.arange(F, dtype=torch.int64, device="cuda") * L; d_len = torch.full((F,), L, dtype=torch.int32, device="cuda")
-    cpb = {1000: 88, 2000: 44, 5500: 16, 11000: 8}[rate]
-    slot = (304 + (24 * 88 + (L + 4) * cpb + 5) * 4 + 600 + 55) // 56 * 56
+    slot = (api.Engine.tx11b_out_stride(L, rate, lead=304) + 600 + 55) // 56 * 56
     d_iq = torch.empty((F, slot, 2), dtype=torch.int16, device="cuda"); d_ns = torch.zeros(F, dtype=torch.int32, device="cuda")
     st = torch.cuda.current_stream().cuda_stream
     eng.tx11b_raw(d_pay.data_ptr(), F * L, d_off.data_ptr(), d_len.data_ptr(), F, rate, 0, 304, 16, d_iq.data_ptr(), slot, d_ns.data_ptr(), st)

@@ -62,8 +62,7 @@ def test_loopback_tx_to_rx_on_device(eng, mcs, L, F):
     pay = rng.integers(0, 256, (F, L)).astype(np.uint8)
     d_pay = torch.from_numpy(pay.reshape(-1)).cuda()
     d_off = torch.arange(F, dtype=torch.int64, device="cuda") * L; d_len = torch.full((F,), L, dtype=torch.int32, device="cuda")
-    nd = {8: 52, 9: 104, 10: 156}[mcs]; nsym = -(-((L + 4) * 8 + 22) // nd) + 1
-    slot = (400 + 1600 + 160 * nsym + 300 + 27) // 28 * 28
+    slot = (api.Engine.tx11n_out_stride(L, mcs, lead=400) + 300 + 27) // 28 * 28
     d0 = torch.empty((F, slot, 2), dtype=torch.int16, device="cuda"); d1 = torch.empty_like(d0); st = torch.cuda.current_stream().cuda_stream
     eng.tx11n_raw(d_pay.data_ptr(), F * L, d_off.data_ptr(), d_len.data_ptr(), 0, F, mcs, 400, d0.data_ptr(), d1.data_ptr(), slot, 0, st)
     s_off = torch.arange(F, dtype=torch.int64, device="cuda") * slot; s_len = torch.full((F,), slot, dtype=torch.int32, device="cuda")

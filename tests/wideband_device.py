@@ -71,21 +71,21 @@ def tables(K, stride, n):
 def tx11a(eng, mpdu, rate, seed):
     """One frame of k_tx11a into device memory -> int8 [ns, 2] device tensor."""
     flat, offs, lens = api._payload_table([mpdu]); sd = np.array([seed], np.uint8); ns = np.zeros(1, np.uint32)
-    stride = 640 + 160 * (2 + -(-(len(mpdu) + 7) * 8 // api._NDBPS_11A[rate]) + 1) + 32
+    stride = api.Engine.tx11a_out_stride(len(mpdu), rate)
     out = torch.zeros((1, stride, 2), dtype=torch.int8, device="cuda")
     eng.tx11a_raw(api._ptr(flat), flat.size, api._ptr(offs), api._ptr(lens), api._ptr(sd), 1, rate, 0, 8, out.data_ptr(), stride, api._ptr(ns))
     return out[0, :int(ns[0])]
 
 def tx11b(eng, mpdu, rate):
     flat, offs, lens = api._payload_table([mpdu]); ns = np.zeros(1, np.uint32)
-    cpb = {1000: 88, 2000: 44, 5500: 16, 11000: 8}[rate]; stride = ((24 * 88 + (len(mpdu) + 4) * cpb + 5) * 4 + 15) // 8 * 8
+    stride = api.Engine.tx11b_out_stride(len(mpdu), rate)
     out = torch.zeros((1, stride, 2), dtype=torch.int8, device="cuda")
     eng.tx11b_raw(api._ptr(flat), flat.size, api._ptr(offs), api._ptr(lens), 1, rate, 0, 0, 8, out.data_ptr(), stride, api._ptr(ns))
     return out[0, :int(ns[0])]
 
 def tx11n(eng, mpdu, mcs, seed):
     flat, offs, lens = api._payload_table([mpdu]); sd = np.array([seed], np.uint8); ns = np.zeros(1, np.uint32)
-    stride = 1600 + 160 * (-(-((len(mpdu) + 4) * 8 + 22) // {8: 52, 9: 104, 10: 156}[mcs]) + 1)
+    stride = api.Engine.tx11n_out_stride(len(mpdu), mcs)
     o0 = torch.zeros((1, stride, 2), dtype=torch.int16, device="cuda"); o1 = torch.zeros_like(o0)
     eng.tx11n_raw(api._ptr(flat), flat.size, api._ptr(offs), api._ptr(lens), api._ptr(sd), 1, mcs, 0, o0.data_ptr(), o1.data_ptr(), stride, api._ptr(ns))
     return o0[0, :int(ns[0])], o1[0, :int(ns[0])]
