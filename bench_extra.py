@@ -14,6 +14,8 @@
   --config channelize_bank  the filter-bank channelizer: all eight odd-stacked 20 MHz channels of a 160 Msps capture, 255 taps, D = 4,
                       timed beside sb200_channelize on the same eight channels and taps
   --config channelize_rational  the rational-rate channelizer: three 802.11b channels of a 160 Msps capture to 44 Msps, 1287 taps, U / D = 11 / 40
+  --config channelize_arbitrary  the arbitrary-rate channelizer: --config channelize_rational's capture to 44 Msps through a 64-tap table,
+                      timed beside sb200_channelize_rational; and a 122.88 Msps capture of the 2.4 GHz band to 44 and 40 Msps
   --config combine   the wideband combiner: four 802.11a channel rows at 40 Msps into one 160 Msps capture, 127 taps, U = 4, device-resident
   --config combine_bank  the filter-bank combiner: eight odd-stacked 40 Msps rows into one 160 Msps capture, 255 taps, U = 4,
                       timed beside sb200_combine on the same eight channels and taps
@@ -536,6 +538,63 @@ def bench_channelize_rational(args):
             "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs of every channel" % m})
     c.close()
 
+def bench_channelize_arbitrary(args):
+    """The arbitrary-rate channelizer on device-resident captures the size of --config channelize's, 64-tap tables.
+    1. --config channelize_rational's workload: three 802.11b channels at -25 / 0 / +25 MHz of 160 Msps to 44 Msps (step 160 / 44), timed in
+       the same process beside sb200_channelize_rational (U / D = 11 / 40, 1287 taps) on the same capture.  The two use different filters:
+       a data point, not a like-for-like comparison.
+    2. A 122.88 Msps capture of the 2.4 GHz band, which no other call brings to the receivers' rates: 802.11b at -25 and +25 MHz to 44 Msps
+       and OFDM at 0 Hz to 40 Msps, two calls per step.
+    Integer work per output: 2 ntaps multiply-adds per component pair, plus 4 per input sample and rotating channel (the rotation)."""
+    import wideband_inputs as W, rational_model as R, arbitrary_model as A
+    from sora_b200 import api
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    n = args.frames * 9824 * 4; P = 20000
+    x = torch.randint(-20000, 20000, (n, 2), dtype=torch.int16, device=dev); xp = x[:P].cpu().numpy()
+    name, plim, clk = _card(); sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    imad_peak = sms * 64 * clk * 1e6 if clk else None                    # int32 IMAD: 64 per SM per clock on sm_90
+    def calls(fs, plan):
+        """plan: [(centres, fs_out, passband, stop band)] -> (step function, [(channels, step, taps, n_out)], output buffers)"""
+        out = []
+        for fcs, fo, fp, fsb in plan:
+            ch = [(W.phase_inc(f, fs), 0) for f in fcs]; step = api.arbitrary_step(fs, fo); taps = api.arbitrary_taps(fs, fo, 64, fp, fsb)
+            n_out = A.n_inside(n, 0, step); y = torch.empty((len(ch), (n_out + 3) // 4 * 4, 2), dtype=torch.int16, device=dev)
+            out.append((ch, step, taps, n_out, y))
+        def step_fn():
+            for ch, step, taps, n_out, y in out: eng.channelize_arbitrary_raw(x.data_ptr(), n, ch, 0, step, taps, y.data_ptr(), y.shape[1], n_out, stream=st.cuda_stream)
+        step_fn(); torch.cuda.synchronize()
+        for ch, step, taps, n_out, y in out:
+            m = ((P - 64) << 32) // step                                 # outputs that a prefix of P samples determines
+            assert (A.channelize_arbitrary(xp, ch, 0, step, taps, m) == y[:, :m].cpu().numpy()).all(), "arbitrary-rate output differs from the stated arithmetic"
+        return step_fn, out
+    def emit(what, ms, out, workload, extra):
+        sec = ms * 1e-3; work = sum(len(ch) * (n_o * 2.0 * taps.shape[1] + 4.0 * n * any(a or b >> 20 for a, b in ch)) for ch, _, taps, n_o, _ in out)
+        f_int = (work / sec / imad_peak) if imad_peak else None
+        c.emit(dict({"metric": "%s input Msamples/s (COMPLEX16 in)" % what, "value": c.world * n / sec / 1e6, "unit": "Msamples/s", "ms_per_step": ms, "n_gpus": c.world,
+                     "config": {"workload": workload, "samples_per_step_per_gpu": n},
+                     "int_mad": {"achieved": work / sec / 1e9, "peak": imad_peak / 1e9 if imad_peak else None, "unit": "G multiply-adds/s", "frac": f_int,
+                                 "note": "2 ntaps per output and channel + 4 per input sample and rotating channel; peak = SMs x 64 x max SM clock"},
+                     "card": name, "power_limit_w": plim, "sm_clock_max_mhz": clk,
+                     "parity": "equal to the numpy model of the stated arithmetic on the outputs a %d-sample prefix determines" % P}, **extra))
+    arb160, out160 = calls(160e6, [((-25e6, 0.0, 25e6), 44e6, 9e6, 17e6)])
+    U, D = 11, 40; rtaps = W.lowpass(1287, 12e6 / 1.76e9, gain=11); rch = out160[0][0]
+    n_r = -(-U * n // D); yr = torch.empty((3, (n_r + 3) // 4 * 4, 2), dtype=torch.int16, device=dev)
+    def rat(): eng.channelize_raw(x.data_ptr(), n, rch, D, rtaps, yr.data_ptr(), yr.shape[1], st.cuda_stream, interp=U)
+    rat(); torch.cuda.synchronize()
+    m = (U * P - len(rtaps)) // D
+    assert (R.channelize_rational(xp, rch, U, D, rtaps)[:, :m] == yr[:, :m].cpu().numpy()).all(), "channelizer output differs from the stated arithmetic"
+    ms_arb = c.timed(arb160, args.steps); ms_rat = c.timed(rat, args.steps)
+    emit("arbitrary-rate channelizer (sb200_channelize_arbitrary), 160 -> 44 Msps", ms_arb, out160,
+         "160 Msps capture, 3 x 802.11b channels at -25/0/+25 MHz to 44 Msps, 64-tap table, step 160 / 44, device-resident",
+         {"rational_ms_per_step": ms_rat, "rational_msamples_per_s": c.world * n / (ms_rat * 1e-3) / 1e6,
+          "rational_note": "sb200_channelize_rational on the same capture and channels: U / D = 11 / 40, 1287 taps (a different filter)"})
+    del out160, yr
+    arb122, out122 = calls(122.88e6, [((-25e6, 25e6), 44e6, 9e6, 17e6), ((0.0,), 40e6, 8.3e6, 17e6)])
+    ms = c.timed(arb122, args.steps)
+    emit("arbitrary-rate channelizer (sb200_channelize_arbitrary), 122.88 -> 44 and 40 Msps", ms, out122,
+         "122.88 Msps capture of the 2.4 GHz band: 802.11b at -25/+25 MHz to 44 Msps and OFDM at 0 Hz to 40 Msps (two calls), 64-tap tables, device-resident", {})
+    c.close()
+
 def bench_combine(args):
     """The wideband combiner into a device-resident 160 Msps capture: four 802.11a channel rows at 40 Msps moved to -60 / -20 / +20 / +60 MHz,
     127 taps, U = 4; as many output samples as --config channelize reads.  Work per output sample: K (2 ceil(ntaps / U) + 4 + 2) integer
@@ -669,7 +728,7 @@ def bench_sim(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_bank", "channelize_rational", "combine", "combine_bank", "combine_rational", "sim"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_bank", "channelize_rational", "channelize_arbitrary", "combine", "combine_bank", "combine_rational", "sim"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
@@ -677,4 +736,4 @@ if __name__ == "__main__":
                     "a pair other than 40/11 takes a generic low-pass of 45 taps per branch at 0.55 of the row's Nyquist")
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_bank": bench_channelize_bank, "channelize_rational": bench_channelize_rational, "combine": bench_combine, "combine_bank": bench_combine_bank, "combine_rational": bench_combine_rational, "sim": bench_sim}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_bank": bench_channelize_bank, "channelize_rational": bench_channelize_rational, "channelize_arbitrary": bench_channelize_arbitrary, "combine": bench_combine, "combine_bank": bench_combine_bank, "combine_rational": bench_combine_rational, "sim": bench_sim}[a.config](a)

@@ -185,6 +185,30 @@ int sb200_channelize_rational(sb200_handle* h, const int16_t* iq, uint64_t n_in_
                               uint32_t interp, uint32_t decim, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride_samples,
                               void* cuda_stream);
 
+/* Arbitrary-rate channelizer: sb200_channelize with the rate changed by any factor between x16 and /4, so that captures at rates derived
+ * from 30.72 MHz (30.72, 61.44, 122.88 Msps) reach the receivers at 40 and 44 Msps; an extension without a reference counterpart.  For
+ * channel (phase_inc, phase0), c = floor((ntaps - 1) / 2) and every output m in 0 .. n_out = n_out_samples:
+ *     v(n)    = the Q14 NCO rotation of x(n) by sb200_channelize, at the phase of the absolute INPUT index n   (x = 0 outside [0, n_in))
+ *     t_m     = tau0 + m * step                                  exact, uint64 (Q32.32 input samples); the limits keep it below 2^63
+ *     t'      = t_m + 2^23,  i = t' >> 32,  p = (t' >> 24) & 255
+ *     y[m]    = sat16((sum_{k < ntaps} H[p][k] * v(i - c + k) + 2^13) >> 14)     int32, re and im independently
+ *     H[p][k] = taps[p * ntaps + k]                               256 rows of ntaps Q14 taps; row p is the fractional delay p / 256
+ * Output m stands at input time t_m / 2^32, rounded to 1/256 of an input sample.  The table is Q14, not the channelizers' Q15, as in
+ * sb200_channel_sim, so that a unit impulse is representable: with step = 2^32, tau0 = d 2^32, phase_inc = phase0 = 0 and row 0 the unit
+ * impulse at k = c, y[m] = x[m + d] bit for bit; with ntaps = 8 and sb200_channel_sim's H this is that call's stage 1.  A capture at fs_in
+ * to fs_out takes step = round(2^32 fs_in / fs_out) (api.arbitrary_step) and a low-pass table cut by the lower of the two rates
+ * (api.arbitrary_taps).  There is one (tau0, step) and one table per call: rows of two rates (802.11b at 44 Msps beside OFDM at 40 Msps)
+ * take two calls, as with sb200_channelize_rational.  n_out is the caller's choice; outputs past the input read zeros.  Larger decimations
+ * go through sb200_channelize or sb200_channelize_bank with a whole decim first (245.76 -> 122.88 Msps, then this call).  Channel c goes
+ * to out[c * out_stride .. + n_out) (samples): the rows go to sb200_rx11a_streams / sb200_rx11b_streams / sb200_rx11n_streams as they are.
+ * iq and out may be host or device pointers (device: 16-byte aligned, and the call is then asynchronous on the stream); channels and taps
+ * are host arrays.  Limits (SB200_E_INVALID, nothing launched): 1 <= nchannels <= 16, 1 <= ntaps <= 64, 2^28 <= step <= 2^34,
+ * tau0 + (n_out - 1) step < 2^63, for every row p sum_k |H[p][k]| <= 65535 (the accumulator cannot wrap), n_in <= 2^40, out_stride >=
+ * n_out, a multiple of 4 and <= 2^40.  n_out = 0 launches nothing.  One kernel launch; sb200_last_kernel_ms times it. */
+int sb200_channelize_arbitrary(sb200_handle* h, const int16_t* iq, uint64_t n_in_samples, const sb200_ddc_channel* channels, uint32_t nchannels,
+                               uint64_t tau0, uint64_t step, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride_samples,
+                               uint64_t n_out_samples, void* cuda_stream);
+
 /* Polyphase filter-bank channelizer: every channel of a uniform grid of M = nchannels channels, centred at (k + o/2) fs / M for k in
  * 0 .. M-1 (k >= M/2 wraps to negative frequencies), out of one COMPLEX16 capture x[0 .. n_in) (x = 0 outside it), filtered by one set
  * of taps and decimated by D = decim, in one pass; an extension without a reference counterpart.  o = odd_stacking: 0 puts channel 0 at

@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_channelize_bank", "sb200_combine", "sb200_combine_rational", "sb200_combine_bank", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_channelize_bank", "sb200_channelize_arbitrary", "sb200_combine", "sb200_combine_rational", "sb200_combine_bank", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -77,6 +77,37 @@ def bank_centres(nchannels, fs_hz, odd=False):
     [-fs/2, fs/2) (channels k >= M/2 are the negative frequencies)."""
     f = (np.arange(nchannels) + 0.5 * bool(odd)) * fs_hz / nchannels
     return np.where(np.arange(nchannels) >= nchannels // 2, f - fs_hz, f)
+
+def arbitrary_step(fs_in, fs_out):
+    """Input samples per output of sb200_channelize_arbitrary for a capture at fs_in brought to fs_out: round(2^32 fs_in / fs_out) (Q32.32)."""
+    return int(round(2 ** 32 * fs_in / fs_out))
+
+def _kaiser_beta(atten_db):
+    """Kaiser's window parameter for a stop-band attenuation of atten_db."""
+    if atten_db > 50: return 0.1102 * (atten_db - 8.7)
+    if atten_db > 21: return 0.5842 * (atten_db - 21) ** 0.4 + 0.07886 * (atten_db - 21)
+    return 0.0
+
+def arbitrary_taps(fs_in, fs_out, ntaps, passband_hz, stopband_hz=None, beta=None):
+    """The 256 x ntaps Q14 table H of sb200_channelize_arbitrary for a capture at fs_in brought to fs_out: a low-pass Kaiser-windowed sinc
+    cut halfway between passband_hz and stopband_hz, row p evaluated at d = k - c - p / 256 (c = (ntaps - 1) // 2), where the output at
+    input time i + p / 256 meets input i - c + k.  stopband_hz defaults to min(fs_in, fs_out) - passband_hz, the lowest frequency that
+    the rate change folds (decimation) or images (interpolation) into the passband; beta defaults to the Kaiser value for the attenuation
+    that ntaps buys over that transition band.  Every row is scaled to a DC gain of exactly 16384 (unity), so the gain does not depend on
+    the phase.  -> int16 [256, ntaps].  Raises ValueError when the band edges do not fit the rates or a row's sum |H| exceeds 65535."""
+    f_lo = min(fs_in, fs_out)
+    stopband_hz = f_lo - passband_hz if stopband_hz is None else stopband_hz
+    if not 0 < passband_hz < stopband_hz <= f_lo: raise ValueError("need 0 < passband_hz < stopband_hz <= min(fs_in, fs_out)")
+    if not 1 <= ntaps <= 64: raise ValueError("ntaps must be 1 .. 64")
+    if beta is None: beta = _kaiser_beta(2.285 * 2 * np.pi * (stopband_hz - passband_hz) / fs_in * max(ntaps - 1, 1) + 8)
+    fc = 0.5 * (passband_hz + stopband_hz) / fs_in                       # cycles per input sample
+    c = (ntaps - 1) // 2; half = ntaps / 2.0
+    d = np.arange(ntaps)[None, :] - c - (np.arange(256) / 256.0)[:, None]
+    h = 2 * fc * np.sinc(2 * fc * d) * np.i0(beta * np.sqrt(np.clip(1 - (d / half) ** 2, 0, 1))) / np.i0(beta)
+    q = np.rint(h / h.sum(1, keepdims=True) * 16384).astype(np.int64)
+    q[np.arange(256), np.argmax(np.abs(q), 1)] += 16384 - q.sum(1)       # exact unity DC gain on every row
+    if np.abs(q).max() > 32767 or (np.abs(q).sum(1) > 65535).any(): raise ValueError("a row of the table exceeds sum |H| <= 65535")
+    return q.astype(np.int16)
 
 class DdcChannel(C.Structure):
     _fields_ = [("phase_inc", C.c_uint32), ("phase0", C.c_uint32)]
@@ -346,6 +377,26 @@ class Engine:
         iq = np.ascontiguousarray(iq, dtype=np.int16).reshape(-1, 2)
         n_out = -(-len(iq) // decim); out, stride = _rows4(nchannels, n_out)
         self.channelize_bank_raw(_ptr(iq), len(iq), nchannels, decim, taps, _ptr(out), stride, odd=odd)
+        return out[:, :n_out]
+
+    def channelize_arbitrary_raw(self, in_ptr, n_in, channels, tau0, step, taps, out_ptr, out_stride, n_out, stream=0):
+        """Pointer-level sb200_channelize_arbitrary: in_ptr / out_ptr host or device addresses, row k of the output at out_ptr + 4 k out_stride
+        bytes; channels a list of (phase_inc, phase0); taps int16 Q14 [256, ntaps]."""
+        ch = (DdcChannel * max(len(channels), 1))(*[DdcChannel(int(a) % 2 ** 32, int(b) % 2 ** 32) for a, b in channels])
+        t = np.ascontiguousarray(taps, dtype=np.int16)
+        if t.ndim != 2 or t.shape[0] != 256: raise ValueError("taps must be int16 [256, ntaps]")
+        self._check(self._lib.sb200_channelize_arbitrary(self._h, C.c_void_p(in_ptr), C.c_uint64(n_in), C.cast(ch, C.c_void_p), C.c_uint32(len(channels)),
+                                                         C.c_uint64(tau0), C.c_uint64(step), C.c_void_p(_ptr(t)), C.c_uint32(t.shape[1]), C.c_void_p(out_ptr),
+                                                         C.c_uint64(out_stride), C.c_uint64(n_out), C.c_void_p(stream)), "sb200_channelize_arbitrary")
+
+    def channelize_arbitrary(self, iq, channels, step, taps, tau0=0, n_out=None):
+        """Arbitrary-rate channelizer: int16 [n,2] and K channels (phase_inc, phase0) -> int16 [K, n_out, 2], channel k shifted to 0 Hz and
+        resampled at input times (tau0 + m step) / 2^32 through the 256-phase Q14 table taps (int16 [256, ntaps], arbitrary_taps);
+        step = arbitrary_step(fs_in, fs_out).  n_out defaults to the outputs whose time lies inside the input, tau0 + m step < n 2^32."""
+        iq = np.ascontiguousarray(iq, dtype=np.int16).reshape(-1, 2)
+        if n_out is None: n_out = max(0, -(-((len(iq) << 32) - tau0) // step))
+        out, stride = _rows4(len(channels), n_out)
+        self.channelize_arbitrary_raw(_ptr(iq), len(iq), channels, tau0, step, taps, _ptr(out), stride, n_out)
         return out[:, :n_out]
 
     def combine_raw(self, rows_ptr, row_stride, n_in, channels, interp, taps, out_ptr, stream=0, decim=1, n_out=None, accumulate=False):

@@ -1,8 +1,10 @@
 // sora_b200 — the wideband filters and the radio channel simulator: sb200_fir_decimate2, the channelizer and the combiner (fir_kernels.cuh),
-// the filter-bank channelizer and combiner (bank_kernels.cuh), sb200_channel_sim (sim_kernels.cuh).
+// the filter-bank channelizer and combiner (bank_kernels.cuh), the arbitrary-rate channelizer (arb_kernels.cuh), sb200_channel_sim
+// (sim_kernels.cuh).
 #include "handle.cuh"
 #include "fir_kernels.cuh"
 #include "bank_kernels.cuh"
+#include "arb_kernels.cuh"
 #include "sim_kernels.cuh"
 
 // Lets `kernel` use `bytes` of dynamic shared memory on this device, once per handle: bit `bit` of `set` records that it has.
@@ -214,6 +216,56 @@ extern "C" int sb200_channelize_bank(sb200_handle* h, const int16_t* iq, uint64_
             k_channelize_bank<decltype(m)::value><<<(unsigned)((n_in + SB_FIR_TILE - 1) / SB_FIR_TILE), SB_FIR_THREADS, 0, st>>>(
                 d_in, n_in, (const uint32_t*)h->nco.p, D, odd_stacking, T, d_out, d_stride, n_out);
         });
+        return SB200_OK;
+    });
+}
+
+// Arbitrary-rate channelizer (arb_kernels.cuh): every channel shifted by its NCO and resampled at input times (tau0 + m step) / 2^32
+// through the 256-phase table H; channel c in row c of `out`.  The table goes up per call behind the NCO (one device-to-device copy), so
+// that one bulk copy per CTA brings both in.  Channels split into groups as in channelize_launch.
+extern "C" int sb200_channelize_arbitrary(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels,
+                                          uint64_t tau0, uint64_t step, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride,
+                                          uint64_t n_out, void* cuda_stream) {
+    if (!h) return SB200_E_INVALID;
+    if (!iq || !channels || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
+    if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
+    if (ntaps < 1 || ntaps > SB_ARB_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be 1 .. 64");
+    if (step < SB_ARB_MINSTEP || step > SB_ARB_MAXSTEP) return h->fail(SB200_E_INVALID, "step must be within 2^28 .. 2^34");
+    if (n_out && (tau0 >> 63 || (n_out - 1) > ((1ull << 63) - 1 - tau0) / step)) return h->fail(SB200_E_INVALID, "tau0 + (n_out - 1) step must be below 2^63");
+    for (uint32_t p = 0; p < SB_ARB_ROWS; p++) {
+        const int rc = check_tap_sums(h, taps + (uint64_t)p * ntaps, ntaps, 1);     // every row of H
+        if (rc != SB200_OK) return rc;
+    }
+    if (n_in > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples must be at most 2^40");
+    if (out_stride < n_out || (out_stride & 3u) || out_stride > (1ull << 40))
+        return h->fail(SB200_E_INVALID, "out_stride must be at least n_out, at most 2^40 and a multiple of 4");
+    if (n_out == 0) return SB200_OK;
+    return channelize_run(h, iq, n_in, nchannels, out, out_stride, n_out, cuda_stream, [&](cudaStream_t st, const uint32_t* d_in, uint32_t* d_out, uint64_t d_stride) {
+        ArbArgs a; memset(&a, 0, sizeof a);
+        a.ch.n = nchannels;
+        bool rot = false;
+        for (uint32_t i = 0; i < nchannels; i++) {
+            a.ch.inc[i] = channels[i].phase_inc; a.ch.phase0[i] = channels[i].phase0;
+            rot |= channels[i].phase_inc != 0u || (channels[i].phase0 >> 20) != 0u;
+        }
+        a.rs = arb_row_words(ntaps);
+        std::vector<uint32_t> H((size_t)SB_ARB_ROWS * a.rs, 0u);      // row p: taps 2q (low half) and 2q + 1 (high half) in word q
+        for (uint32_t p = 0; p < SB_ARB_ROWS; p++)
+            for (uint32_t k = 0; k < ntaps; k++) H[p * a.rs + k / 2] |= (uint32_t)(uint16_t)taps[(uint64_t)p * ntaps + k] << (16 * (k & 1));
+        CK(h->arbtab.need((SB_CH_NCO + H.size()) * 4));
+        CK(cudaMemcpyAsync(h->arbtab.p, h->nco.p, SB_CH_NCO * 4, cudaMemcpyDeviceToDevice, st));
+        CK(cudaMemcpyAsync((uint32_t*)h->arbtab.p + SB_CH_NCO, H.data(), H.size() * 4, cudaMemcpyHostToDevice, st));
+        a.x = d_in; a.n_in = n_in; a.tab = (const uint32_t*)h->arbtab.p;
+        a.tau0 = tau0; a.step = step; a.ntaps = ntaps; a.win = arb_win(step, ntaps); a.nco_words = rot ? SB_CH_NCO : 0u;
+        a.y = d_out; a.stride = d_stride; a.n_out = n_out;
+        if (!h->sms) CK(cudaDeviceGetAttribute(&h->sms, cudaDevAttrMultiProcessorCount, h->device));
+        const uint64_t tiles = (n_out + SB_ARB_TM - 1) / SB_ARB_TM;
+        uint32_t groups = 1;
+        while (groups < nchannels && tiles * groups < 4ull * (uint64_t)h->sms) groups++;
+        a.chan_per_group = (nchannels + groups - 1) / groups; groups = (nchannels + a.chan_per_group - 1) / a.chan_per_group;
+        CK(smem_once(h->arb_smem_set, 1u, k_channelize_arbitrary, SB_ARB_SMEM_MAX));
+        CK(cudaEventRecord(h->ev0, st));
+        k_channelize_arbitrary<<<dim3((unsigned)tiles, groups), SB_FIR_THREADS, arb_smem(step, ntaps, rot), st>>>(a);
         return SB200_OK;
     });
 }
