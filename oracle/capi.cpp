@@ -234,6 +234,31 @@ void sbo_rx11b_batch(const int16_t* iq, const uint64_t* off, const uint32_t* len
     std::vector<std::thread> th; for (int t = 0; t < nthreads; t++) th.emplace_back(work);
     for (auto& t : th) t.join();
 }
+// the CCK decoders the chain runs, on n symbols (CCK-11: 8 chips, is_even from 0) / bytes (CCK-5.5: 16 chips) in turn; last2 in / out
+void sbo_cck11_decode_n(const int16_t* chips, uint64_t n, int16_t* last2, uint8_t* out) {
+    c16 l{last2[0], last2[1]}; int even = 0;
+    for (uint64_t i = 0; i < n; i++) out[i] = cck11_decode((const c16*)chips + 8 * i, l, even);
+    last2[0] = l.re; last2[1] = l.im;
+}
+void sbo_cck5_decode_n(const int16_t* chips, uint64_t n, int16_t* last2, uint8_t* out) {
+    c16 l{last2[0], last2[1]};
+    for (uint64_t i = 0; i < n; i++) out[i] = cck5_decode((const c16*)chips + 16 * i, l);
+    last2[0] = l.re; last2[1] = l.im;
+}
+// the Barker branches the chain runs: despread on n blocks of 11 chips; DBPSK / DQPSK on n bytes of 8 / 4 symbols in turn, last2 in / out
+void sbo_despread_n(const int16_t* chips, uint64_t n, int16_t* out) {
+    for (uint64_t i = 0; i < n; i++) { c16 s = barker_despread((const c16*)chips + 11 * i); out[2 * i] = s.re; out[2 * i + 1] = s.im; }
+}
+void sbo_dbpsk_demap_n(const int16_t* sym, uint64_t n, int16_t* last2, uint8_t* out) {
+    c16 l{last2[0], last2[1]};
+    for (uint64_t i = 0; i < n; i++) out[i] = dbpsk_demap((const c16*)sym + 8 * i, l);
+    last2[0] = l.re; last2[1] = l.im;
+}
+void sbo_dqpsk_demap_n(const int16_t* sym, uint64_t n, int16_t* last2, uint8_t* out) {
+    c16 l{last2[0], last2[1]};
+    for (uint64_t i = 0; i < n; i++) out[i] = dqpsk_demap((const c16*)sym + 4 * i, l);
+    last2[0] = l.re; last2[1] = l.im;
+}
 uint8_t sbo_cck11_decode(const int16_t* chips8, int16_t* last2, int* even) { c16 l{last2[0], last2[1]}; uint8_t b = cck11_decode((const c16*)chips8, l, *even); last2[0] = l.re; last2[1] = l.im; return b; }
 
 // ---- 802.11n 2x2 -----------------------------------------------------------------------------------------------------

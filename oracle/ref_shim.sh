@@ -30,6 +30,18 @@
 #                 behind (DEFINE_OPERATOR_OVERLOAD(*, vcs, mul), :1500), mul_shift / conj_mul_shift (:1215-1246)
 #     constants   the vector128_consts masks (:179-284) the FFT names
 #     macros      DSP_INLINE / DSP_INLINE1 (:22-24); __declspec(selectany / align / deprecated)
+#     802.11b     vcb and vci (:136, :140; COMPLEX32 is complex.h:6), shift_right / >> on vci (_mm_srai_epi32, :833),
+#                 shift_element_left / shift_element_right (_mm_slli_si128 / _mm_srli_si128, :855-864: template arguments in the
+#                 order barkerspread.hpp:294, :376 write them), insert<ndx> on vcs (_mm_insert_epi32, :1466), load (:1352)
+#   complex_ext.h the COMPLEX16 operators + and - (short results, complex_ext.h:94, :107), >> (:115) and norm2 (:134-138); += and -= of
+#                 a COMPLEX16 into a COMPLEX32 (:89-103);
+#   operator_repeater.h, further: rep_sqrnorm (:195-211, SquaredNorm per vector) and rep_sum (:214-230, += on vi);
+#   windef.h, soratypes.h   the Windows integer names the 802.11b headers use (USHORT, PUSHORT, BOOLEAN, BYTE / WORD / DWORD, ...)
+#                 and soratypes.h:22-33's typedefs (its `ulong` is the compiler's `unsigned long`: a build that wants MSVC's 32-bit
+#                 width defines the name itself);
+#   demux.h       TDemux with up to five outputs (kernel/brick/inc/demux.h:13-152: AddRef of every output, Reset and Flush of every
+#                 output, an empty Process), DEFINE_OPORTS (brick.h:204-240), FlushPort(N) (brick.h:461), DummyBrick (brick.h:477-490),
+#                 and the TDEMUX2/4/5 macro sets (demux.h:154-266).
 ref_shim() {
 mkdir -p "$1/bb"
 cat > "$1/const.h" <<'SHIM'
@@ -45,6 +57,7 @@ cat > "$1/const.h" <<'SHIM'
 #define A16 __attribute__((aligned(16)))
 #define MEM_ALIGN(n) __attribute__((aligned(n)))
 #define UCHAR unsigned char
+#define A32 __attribute__((aligned(32)))
 #undef CTX_VAR_RW
 #undef CTX_VAR_RO
 #undef FACADE_FIELD
@@ -92,15 +105,120 @@ template<size_t N, typename T> inline void rep_shift_right(T* dst, const T* src,
 template<size_t N, typename T> inline void rep_sub(T* dst, const T* src, const T& val) { for (size_t i = 0; i < N; i++) *dst++ = sub(*src++, val); }
 template<size_t N, typename T> inline void rep_memzero(T* dst) { for (size_t i = 0; i < N; i++) set_zero(*dst++); }
 template<size_t N, typename T> inline void rep_memcpy(T* dst, const T* src) { for (size_t i = 0; i < N; i++) *dst++ = *src++; }
+template<size_t N> inline void rep_sqrnorm(vi* dst, const vcs* src) { for (size_t i = 0; i < N; i++) *dst++ = SquaredNorm(*src++); }
+template<size_t N, typename T> inline void rep_sum(T& result, const T* src) { for (size_t i = 0; i < N; i++) result += *src++; }
 SHIM
 cat > "$1/sora.h" <<'SHIM'
 #pragma once
 #include "const.h"
 #include "vector128.h"
+#include "complex_ext.h"
 typedef struct SORA_RADIO_RX_STREAM SORA_RADIO_RX_STREAM;
 typedef unsigned char FLAG;
 #define NODEFAULT __builtin_unreachable()
 inline int ceil_div(int x, int mod) { return (x + mod - 1) / mod; }
+SHIM
+cat > "$1/complex_ext.h" <<'SHIM'
+#pragma once
+#include "const.h"
+inline COMPLEX16 operator+(const COMPLEX16& a, const COMPLEX16& b) { COMPLEX16 r; r.re = (short)(a.re + b.re); r.im = (short)(a.im + b.im); return r; }
+inline COMPLEX16 operator-(const COMPLEX16& a, const COMPLEX16& b) { COMPLEX16 r; r.re = (short)(a.re - b.re); r.im = (short)(a.im - b.im); return r; }
+inline COMPLEX16 operator>>(const COMPLEX16& a, int n) { COMPLEX16 r; r.re = (short)(a.re >> n); r.im = (short)(a.im >> n); return r; }
+inline int norm2(const COMPLEX16& a) { return a.re * a.re + a.im * a.im; }
+inline COMPLEX32& operator+=(COMPLEX32& a, const COMPLEX16& b) { a.re += b.re; a.im += b.im; return a; }
+inline COMPLEX32& operator-=(COMPLEX32& a, const COMPLEX16& b) { a.re -= b.re; a.im -= b.im; return a; }
+SHIM
+cat > "$1/windef.h" <<'SHIM'
+#pragma once
+typedef unsigned char BYTE, BOOLEAN, *PUCHAR;
+typedef unsigned short WORD, USHORT, *PUSHORT;
+typedef unsigned int DWORD, UINT, *PUINT;
+#ifndef TRUE
+#define TRUE 1
+#define FALSE 0
+#endif
+#define IN
+#define OUT
+SHIM
+cat > "$1/soratypes.h" <<'SHIM'
+#pragma once
+#include <emmintrin.h>
+#include "windef.h"
+#include "const.h"
+typedef int s_int32; typedef unsigned int s_uint32; typedef short s_int16; typedef unsigned short s_uint16;
+typedef COMPLEX16 SAMPLE, *PSAMPLE;
+SHIM
+cat > "$1/demux.h" <<'SHIM'
+#pragma once
+#include "const.h"
+#include <type_traits>
+class DummyBrick : public IReferenceCounting, public IControlPoint {
+public:
+    typedef ::iport_traits<void, 1> iport_traits;
+    void Reset() override {}
+    void Flush() override {}
+    template<class T_IPIN> bool Process(T_IPIN& pin) { pin.clear(); return true; }
+};
+inline DummyBrick DummyBrickInstance;
+#define NON_DUMMYBRICK(INDEX) (!std::is_same<T_NEXT##INDEX, DummyBrick>::value)
+template<class T_CTX, class T_NEXT0 = DummyBrick, class T_NEXT1 = DummyBrick, class T_NEXT2 = DummyBrick, class T_NEXT3 = DummyBrick,
+         class T_NEXT4 = DummyBrick>
+class TDemux : public TBrick<T_CTX>, public IReferenceCounting, public IControlPoint {
+protected:
+    T_NEXT0* __next_0; T_NEXT1* __next_1; T_NEXT2* __next_2; T_NEXT3* __next_3; T_NEXT4* __next_4;
+    T_NEXT0* Next0() { return __next_0; } T_NEXT1* Next1() { return __next_1; } T_NEXT2* Next2() { return __next_2; }
+    T_NEXT3* Next3() { return __next_3; } T_NEXT4* Next4() { return __next_4; }
+public:
+    typedef TDemux TDemuxBase;
+    TDemux(T_CTX& ctx, T_NEXT0* n0 = NULL, T_NEXT1* n1 = NULL, T_NEXT2* n2 = &DummyBrickInstance, T_NEXT3* n3 = &DummyBrickInstance,
+           T_NEXT4* n4 = &DummyBrickInstance) : TBrick<T_CTX>(ctx), __next_0(n0), __next_1(n1), __next_2(n2), __next_3(n3), __next_4(n4) {
+        if (NON_DUMMYBRICK(0)) AddRef(Next0()); if (NON_DUMMYBRICK(1)) AddRef(Next1()); if (NON_DUMMYBRICK(2)) AddRef(Next2());
+        if (NON_DUMMYBRICK(3)) AddRef(Next3()); if (NON_DUMMYBRICK(4)) AddRef(Next4());
+    }
+    ~TDemux() {
+        if (NON_DUMMYBRICK(0)) IReferenceCounting::Release(Next0()); if (NON_DUMMYBRICK(1)) IReferenceCounting::Release(Next1());
+        if (NON_DUMMYBRICK(2)) IReferenceCounting::Release(Next2()); if (NON_DUMMYBRICK(3)) IReferenceCounting::Release(Next3());
+        if (NON_DUMMYBRICK(4)) IReferenceCounting::Release(Next4());
+    }
+    void Reset() {
+        if (NON_DUMMYBRICK(0)) Next0()->Reset(); if (NON_DUMMYBRICK(1)) Next1()->Reset(); if (NON_DUMMYBRICK(2)) Next2()->Reset();
+        if (NON_DUMMYBRICK(3)) Next3()->Reset(); if (NON_DUMMYBRICK(4)) Next4()->Reset();
+    }
+    void Flush() {
+        if (NON_DUMMYBRICK(0)) Next0()->Flush(); if (NON_DUMMYBRICK(1)) Next1()->Flush(); if (NON_DUMMYBRICK(2)) Next2()->Flush();
+        if (NON_DUMMYBRICK(3)) Next3()->Flush(); if (NON_DUMMYBRICK(4)) Next4()->Flush();
+    }
+    template<class T_IPIN> bool Process(T_IPIN&) { return true; }
+};
+#undef FlushPort
+#define FlushPort(N) do { if (opin##N().pad()) this->Next##N()->Process(opin##N()); this->Next##N()->Flush(); } while (false)
+#define DEFINE_OPORTS(INDEX, TYPE, BURST)                                                                                      \
+    typedef ::oport_traits<TYPE, BURST, 1> oport_traits##INDEX;                                                                \
+    typedef typename DeducedPinQueue<oport_traits##INDEX, typename T_NEXT##INDEX::iport_traits>::type opin_type##INDEX;          \
+    opin_type##INDEX __opin##INDEX##_;                                                                                           \
+    opin_type##INDEX& opin##INDEX() { return __opin##INDEX##_; }
+#define TDEMUX2_ARGS class T_CTX, class T_NEXT0, class T_NEXT1
+#define TDEMUX2_PARAMS T_CTX, T_NEXT0, T_NEXT1
+#define STD_DEMUX2_CONSTRUCTOR(name) name(T_CTX& ctx, T_NEXT0* n0, T_NEXT1* n1) : TDemux<TDEMUX2_PARAMS>(ctx, n0, n1)
+#define STD_TDEMUX2_RESET() FINL void Reset() { this->TDemuxBase::Reset(); opin0().clear(); opin1().clear(); __ResetSelf(); } FINL void __ResetSelf()
+#define TDEMUX4_ARGS class T_CTX, class T_NEXT0, class T_NEXT1, class T_NEXT2, class T_NEXT3
+#define TDEMUX4_PARAMS T_CTX, T_NEXT0, T_NEXT1, T_NEXT2, T_NEXT3
+#define STD_DEMUX4_CONSTRUCTOR(name) name(T_CTX& ctx, T_NEXT0* n0, T_NEXT1* n1, T_NEXT2* n2, T_NEXT3* n3) : TDemux<TDEMUX4_PARAMS>(ctx, n0, n1, n2, n3)
+#define STD_TDEMUX4_RESET() FINL void Reset() { this->TDemuxBase::Reset(); opin0().clear(); opin1().clear(); opin2().clear(); opin3().clear(); __ResetSelf(); } \
+    FINL void __ResetSelf()
+#define TDEMUX5_ARGS class T_CTX, class T_NEXT0, class T_NEXT1, class T_NEXT2, class T_NEXT3, class T_NEXT4
+#define TDEMUX5_PARAMS T_CTX, T_NEXT0, T_NEXT1, T_NEXT2, T_NEXT3, T_NEXT4
+#define STD_DEMUX5_CONSTRUCTOR(name) name(T_CTX& ctx, T_NEXT0* n0, T_NEXT1* n1, T_NEXT2* n2, T_NEXT3* n3, T_NEXT4* n4) \
+    : TDemux<TDEMUX5_PARAMS>(ctx, n0, n1, n2, n3, n4)
+#define STD_TDEMUX5_RESET() FINL void Reset() { this->TDemuxBase::Reset(); opin0().clear(); opin1().clear(); opin2().clear(); opin3().clear(); \
+    opin4().clear(); __ResetSelf(); } FINL void __ResetSelf()
+#define CREATE_BRICK_DEMUX2(NAME, TPL, CTX, N0, N1) \
+    typedef TPL<std::remove_reference<decltype(CTX)>::type, std::remove_reference<decltype(*N0)>::type, std::remove_reference<decltype(*N1)>::type> __C_##NAME; \
+    __C_##NAME* NAME = new __C_##NAME(CTX, N0, N1);
+#define CREATE_BRICK_DEMUX5(NAME, TPL, CTX, N0, N1, N2, N3, N4) \
+    typedef TPL<std::remove_reference<decltype(CTX)>::type, std::remove_reference<decltype(*N0)>::type, std::remove_reference<decltype(*N1)>::type, \
+                std::remove_reference<decltype(*N2)>::type, std::remove_reference<decltype(*N3)>::type, std::remove_reference<decltype(*N4)>::type> __C_##NAME; \
+    __C_##NAME* NAME = new __C_##NAME(CTX, N0, N1, N2, N3, N4);
 SHIM
 cat > "$1/soratime.h" <<'SHIM'
 #pragma once
@@ -119,7 +237,6 @@ cat > "$1/bb/bba.h" <<'SHIM'
 #pragma once
 #include "../const.h"
 #include "../vector128.h"
-typedef struct _COMPLEX32 { int re, im; } COMPLEX32;
 #define SORA_RX_SIGNAL_UNIT_SIZE 16
 #define SORA_RX_SIGNAL_UNIT_NUM_PER_DESC 7
 #define SORA_RX_SIGNAL_UNIT_COMPLEX16_NUM (SORA_RX_SIGNAL_UNIT_SIZE / sizeof(COMPLEX16))
@@ -155,6 +272,9 @@ SB_VEC(vs, short)
 SB_VEC(vi, int)
 SB_VEC(vub, unsigned char)
 SB_VEC(vcs, COMPLEX16)
+typedef struct _COMPLEX32 { int re, im; } COMPLEX32;
+SB_VEC(vci, COMPLEX32)
+SB_VEC(vcb, COMPLEX8)
 struct COMPLEXU32 { unsigned int re, im; };
 SB_VEC(vcui, COMPLEXU32)
 template<typename T> inline T& cast_ref(void* p) { return *reinterpret_cast<T*>(p); }
@@ -182,6 +302,13 @@ inline vi shift_right(const vi& a, int n) { vi r(_mm_srai_epi32(a, n)); if (n ==
 inline vcs operator>>(const vcs& a, int n) { return shift_right(a, n); }
 inline vi operator>>(const vi& a, int n) { return shift_right(a, n); }
 inline vi operator+(const vi& a, const vi& b) { return vi(_mm_add_epi32(a, b)); }
+inline vi& operator+=(vi& a, const vi& b) { a = a + b; return a; }
+inline vci shift_right(const vci& a, int n) { return vci(_mm_srai_epi32(a, n)); }
+inline vci operator>>(const vci& a, int n) { return shift_right(a, n); }
+template<typename T, int n> inline T shift_element_left(const T& a) { return T(_mm_slli_si128(a, n * sizeof(typename T::elem_type))); }
+template<typename T, int n> inline T shift_element_right(const T& a) { return T(_mm_srli_si128(a, n * sizeof(typename T::elem_type))); }
+template<int ndx> inline vcs insert(const vcs& a, COMPLEX16 b) { unsigned int w; memcpy(&w, &b, 4); return vcs(_mm_insert_epi32(a, (int)w, ndx)); }
+template<typename T> inline void load(T& r, const void* p) { r = T(_mm_loadu_si128((const __m128i*)p)); }
 inline vi& operator*=(vi& a, const vi& b) { a = vi(_mm_mullo_epi32(a, b)); return a; }
 inline vcs saturated_add(const vcs& a, const vcs& b) { return vcs(_mm_adds_epi16(a, b)); }
 inline vcs saturated_sub(const vcs& a, const vcs& b) { return vcs(_mm_subs_epi16(a, b)); }

@@ -110,11 +110,18 @@ static Pick cck11_module(int32_t a1r, int32_t a1i, int32_t a2r, int32_t a2i, int
     else               { if (mx[3] > p.max) { p.max = mx[3]; p.val = vl[3]; } }
     return p;
 }
-static inline void dqpsk_bits(uint8_t& r, int pos, c16 ref, c16 s) {       // barkerspread.hpp:430-437
-    // int C: after a CCK symbol `ref` is a raw chip, and full-scale chips wrap the sums
+static inline void dqpsk_bits(uint8_t& r, int pos, c16 ref, c16 s) {       // TDQPSKDemap::demap_dqpsk_bits (barkerspread.hpp:432-439)
+    // MSVC's 32-bit long: re + im and re - im wrap when both products are near 2^30 (the despread symbols of the chain stay below that)
     int32_t re = wadd(ref.re * s.re, ref.im * s.im), im = wsub(ref.re * s.im, ref.im * s.re);
     r |= (uint8_t)(((uint32_t)wadd(re, im) >> 31) << pos);
     r |= (uint8_t)(((uint32_t)wsub(re, im) >> 31) << (pos + 1));
+}
+static inline void cck_dqpsk_bits(uint8_t& r, int pos, c16 ref, c16 s) {   // the free demap_dqpsk_bits the CCK decoders call (soradsp.h:190-199)
+    // it halves re and im before the sums (:194-195), so re + im and re - im never wrap; re itself wraps to INT_MIN when both products
+    // are 2^30 (a raw chip of -32768, -32768 against its like: after a CCK symbol `ref` is a raw chip)
+    int32_t re = wadd(ref.re * s.re, ref.im * s.im) >> 1, im = wsub(ref.re * s.im, ref.im * s.re) >> 1;
+    r |= (uint8_t)(((uint32_t)(re + im) >> 31) << pos);
+    r |= (uint8_t)(((uint32_t)(re - im) >> 31) << (pos + 1));
 }
 uint8_t cck11_decode(const c16* P, c16& last, int& even) {                  // cck.hpp:262-769 CCK11_DECODER
     int32_t p[8][2]; for (int i = 0; i < 8; i++) { p[i][0] = P[i].re; p[i][1] = P[i].im; }
@@ -135,7 +142,7 @@ uint8_t cck11_decode(const c16* P, c16& last, int& even) {                  // c
     }
 #undef R
 #undef I
-    dqpsk_bits(out, 0, last, P[7]);
+    cck_dqpsk_bits(out, 0, last, P[7]);
     out ^= (uint8_t)((even << 1) | even);
     even ^= 1;
     last = P[7];
@@ -161,9 +168,39 @@ static void cck5_half(uint8_t& out, const c16* P, c16& last, bool hi) {
     if (l1 > 0) { max1 = l1; v1 = 0; } else { max1 = wneg(l1); v1 = b3; }
     if (l2 > 0) { max2 = l2; v2 = b2; } else { max2 = wneg(l2); v2 = (uint8_t)(b2 | b3); }
     const uint8_t pick = max1 > max2 ? v1 : v2;
-    if (!hi) { out = pick; dqpsk_bits(out, 0, last, P[7]); }
-    else { out |= pick; dqpsk_bits(out, 4, last, P[7]); out ^= 0x30; }
+    if (!hi) { out = pick; cck_dqpsk_bits(out, 0, last, P[7]); }
+    else { out |= pick; cck_dqpsk_bits(out, 4, last, P[7]); out ^= 0x30; }
     last = P[7];
+}
+uint8_t cck5_decode(const c16* P, c16& last) {                             // TCCK5P5Decoder (cck.hpp:26-45): two half bytes per 16 chips
+    uint8_t b = 0; cck5_half(b, P, last, false); cck5_half(b, P + 8, last, true);
+    return b;
+}
+
+// ---- the Barker branches: TBB11bDespread, TDBPSKDemap, TDQPSKDemap ----
+c16 barker_despread(const c16* q) {                                         // QuickBarkerDespread (barkerspread.hpp:276-304), 11 chips
+    int sr = 0, si = 0;
+    static const int sgn[11] = {1, -1, 1, 1, -1, 1, 1, 1, -1, -1, -1};
+    for (int i = 0; i < 11; i++) {
+        int16_t re, im;
+        if (i == 1 || i == 4) { re = w16(w16(-q[i].re) >> 4); im = w16(w16(-q[i].im) >> 4); }                   // negate, then >> 4
+        else if (sgn[i] < 0) { re = w16(-(q[i].re >> 4)); im = w16(-(q[i].im >> 4)); }                          // >> 4, then subtract
+        else { re = w16(q[i].re >> 4); im = w16(q[i].im >> 4); }
+        sr += re; si += im;
+    }
+    return c16{w16(sr), w16(si)};                                           // the hadd of int16 lanes wraps
+}
+uint8_t dbpsk_demap(const c16* sym, c16& last) {                            // TDBPSKDemap::DemapDBPSK (barkerspread.hpp:353-371), 8 symbols
+    uint8_t r = 0; c16 ref = last;
+    for (int i = 0; i < 8; i++) { r |= (uint8_t)(((uint32_t)wadd(ref.re * sym[i].re, ref.im * sym[i].im) >> 31) << i); ref = sym[i]; }
+    last = sym[7];
+    return r;
+}
+uint8_t dqpsk_demap(const c16* sym, c16& last) {                            // TDQPSKDemap::DemapDQPSK (barkerspread.hpp:441-450), 4 symbols
+    uint8_t r = 0; c16 ref = last;
+    for (int i = 0; i < 4; i++) { dqpsk_bits(r, 2 * i, ref, sym[i]); ref = sym[i]; }
+    last = sym[3];
+    return r;
 }
 
 // ---- byte path: TDesc741 -> TBB11bPlcpSwitch -> parser | frame sink ----
@@ -211,16 +248,7 @@ void Rx11b::on_chip(c16 s) {
         dsp_q[dsp_n++] = s;
         if (dsp_n < 11) return;
         dsp_n = 0;
-        int sr = 0, si = 0;
-        static const int sgn[11] = {1, -1, 1, 1, -1, 1, 1, 1, -1, -1, -1};
-        for (int i = 0; i < 11; i++) {
-            int16_t re, im;
-            if (i == 1 || i == 4) { re = w16(w16(-dsp_q[i].re) >> 4); im = w16(w16(-dsp_q[i].im) >> 4); }       // negate, then >> 4
-            else if (sgn[i] < 0) { re = w16(-(dsp_q[i].re >> 4)); im = w16(-(dsp_q[i].im >> 4)); }              // >> 4, then subtract
-            else { re = w16(dsp_q[i].re >> 4); im = w16(dsp_q[i].im >> 4); }
-            sr += re; si += im;
-        }
-        c16 sym{w16(sr), w16(si)};
+        const c16 sym = barker_despread(dsp_q);
         if (rate_state == 0) {                                              // TSFDSync (sfd_sync.hpp:12-133)
             unsigned bit = (uint32_t)(last_symbol.re * sym.re + last_symbol.im * sym.im) >> 31;
             last_symbol = sym;
@@ -239,19 +267,17 @@ void Rx11b::on_chip(c16 s) {
         }
         sym_q[sym_n++] = sym;
         if (rate_state == 1 && sym_n == 8) {                                // TDBPSKDemap (barkerspread.hpp:314-390)
-            uint8_t r = 0; c16 ref = last_symbol;
-            for (int i = 0; i < 8; i++) { r |= (uint8_t)(((uint32_t)(ref.re * sym_q[i].re + ref.im * sym_q[i].im) >> 31) << i); ref = sym_q[i]; }
-            last_symbol = sym_q[7]; sym_n = 0; on_byte(r);
+            const uint8_t r = dbpsk_demap(sym_q, last_symbol);
+            sym_n = 0; on_byte(r);
         } else if (rate_state == 2 && sym_n == 4) {                         // TDQPSKDemap (barkerspread.hpp:398-451)
-            uint8_t r = 0; c16 ref = last_symbol;
-            for (int i = 0; i < 4; i++) { dqpsk_bits(r, 2 * i, ref, sym_q[i]); ref = sym_q[i]; }
-            last_symbol = sym_q[3]; sym_n = 0; on_byte(r);
+            const uint8_t r = dqpsk_demap(sym_q, last_symbol);
+            sym_n = 0; on_byte(r);
         }
         return;
     }
     cck_q[cck_n++] = s;
     if (rate_state == 3 && cck_n == 16) {                                   // TCCK5P5Decoder (cck.hpp:11-69)
-        uint8_t b = 0; cck5_half(b, cck_q, last_symbol, false); cck5_half(b, cck_q + 8, last_symbol, true);
+        uint8_t b = cck5_decode(cck_q, last_symbol);
         cck_n = 0; on_byte(b);
     } else if (rate_state == 4 && cck_n == 8) {                             // TCCK11Decoder (cck.hpp:210-260)
         uint8_t b = cck11_decode(cck_q, last_symbol, cck_even);

@@ -9,6 +9,10 @@ enum : uint32_t { E_SFD_FAIL = 0x80000004u, E_SFD_TIMEOUT = 0x80000008u, E_SYNC_
 struct FrameResult11b { uint32_t status, rate_kbps, length, crc32, sample_index, detect_vec; };
 
 uint8_t cck11_decode(const c16* P, c16& last, int& even);
+uint8_t cck5_decode(const c16* P, c16& last);
+c16 barker_despread(const c16* chips11);
+uint8_t dbpsk_demap(const c16* sym8, c16& last);
+uint8_t dqpsk_demap(const c16* sym4, c16& last);
 
 class Rx11b {
 public:

@@ -58,9 +58,15 @@ __device__ __forceinline__ CckPick cck11_module(int a1r, int a1i, int a2r, int a
     else               { if (mx[3] > p.mx) { p.mx = mx[3]; p.val = vl[3]; } }
     return p;
 }
-__device__ __forceinline__ unsigned dqpsk_bits(S16 ref, S16 s) {              // barkerspread.hpp:430-437; bit0 | bit1<<1
-    const int re = wadd(ref.re * s.re, ref.im * s.im), im = wsub(ref.re * s.im, ref.im * s.re);     // after a CCK symbol `ref` is a raw chip: wraps at full scale
+__device__ __forceinline__ unsigned dqpsk_bits(S16 ref, S16 s) {              // TDQPSKDemap (barkerspread.hpp:432-439); bit0 | bit1<<1
+    const int re = wadd(ref.re * s.re, ref.im * s.im), im = wsub(ref.re * s.im, ref.im * s.re);     // MSVC's 32-bit long: the sums wrap
     return ((unsigned)wadd(re, im) >> 31) | (((unsigned)wsub(re, im) >> 31) << 1);
+}
+__device__ __forceinline__ unsigned cck_dqpsk_bits(S16 ref, S16 s) {          // the demap_dqpsk_bits the CCK decoders call (soradsp.h:190-199)
+    // re and im are halved before the sums (:194-195), so re + im never wraps; re wraps to INT_MIN when both products are 2^30 (after a
+    // CCK symbol `ref` is a raw chip)
+    const int re = wadd(ref.re * s.re, ref.im * s.im) >> 1, im = wsub(ref.re * s.im, ref.im * s.re) >> 1;
+    return ((unsigned)(re + im) >> 31) | (((unsigned)(re - im) >> 31) << 1);
 }
 
 struct Rx11bState {
@@ -218,7 +224,7 @@ __global__ void __launch_bounds__(64) k_rx11b(const uint32_t* __restrict__ iq, c
                 CckPick m3 = cck11_module(R[1] - R[0], I[1] - I[0], -(R[2] + R[3]), -(I[2] + I[3]), R[5] - R[4], I[5] - I[4], R[6] + R[7], I[6] + I[7]);
                 m3.val |= 0x04u; o = m2.mx > m3.mx ? m2.val : m3.val;
             }
-            o |= dqpsk_bits(s.last_symbol, q7);
+            o |= cck_dqpsk_bits(s.last_symbol, q7);
             o ^= (unsigned)((s.cck_even << 1) | s.cck_even);
             s.cck_even ^= 1; s.last_symbol = q7;
             on_byte(o & 0xFFu);
@@ -245,7 +251,7 @@ __global__ void __launch_bounds__(64) k_rx11b(const uint32_t* __restrict__ iq, c
             if (l1 > 0) { max1 = l1; v1 = 0; } else { max1 = wneg(l1); v1 = b3; }
             if (l2 > 0) { max2 = l2; v2 = b2; } else { max2 = wneg(l2); v2 = b2 | b3; }
             b |= max1 > max2 ? v1 : v2;
-            b |= dqpsk_bits(s.last_symbol, q7) << (4 * hb);
+            b |= cck_dqpsk_bits(s.last_symbol, q7) << (4 * hb);
             if (hb) b ^= 0x30u;
             s.last_symbol = q7;
         }

@@ -444,3 +444,94 @@ def ref_rx11n_debug():
     """What the tap counted since the last ref_rx11n_debug_reset on this thread, as {name: count} (REF_RX11N_COUNTERS)."""
     d = np.zeros(10, np.uint64); _ref_rx11n().ref_rx11n_debug(d.ctypes.data)
     return dict(zip(REF_RX11N_COUNTERS, (int(v) for v in d)))
+
+# ---- the reference's own 802.11b receiver bricks and graph (oracle/build_ref_rx11b.sh) ----
+_REF_RX11B = None
+REF_RX11B_COUNTERS = ("cck_int_min", "cck_tie", "dqpsk_re_wrap", "dqpsk_sum_wrap", "sfd_found", "sfd_fail", "sfd_timeout", "sync_timeout",
+                      "plcp_crc16", "plcp_unknown_rate", "plcp_short_length", "fcs_ok", "fcs_fail", "cs_timeout")   # ref_rx11b_debug's order
+def ref_rx11b_available():
+    return os.path.exists(os.path.join(ROOT, "oracle", "_ref", "librx11b_ref.so"))
+def _ref_rx11b():
+    global _REF_RX11B
+    if _REF_RX11B is None:
+        L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "librx11b_ref.so"))
+        for f in ("ref_cck11_decode", "ref_cck5_decode", "ref_dqpsk_demap", "ref_dbpsk_demap"):
+            getattr(L, f).argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p]; getattr(L, f).restype = None
+        L.ref_despread.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p]; L.ref_despread.restype = None
+        L.ref_plcp11b_parse.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p]; L.ref_plcp11b_parse.restype = None
+        L.ref_desc_sink.argtypes = [C.c_void_p, C.c_size_t, C.c_uint8, C.c_uint16, C.c_void_p, C.c_void_p]; L.ref_desc_sink.restype = C.c_uint32
+        L.ref_rx11b_run.argtypes = [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_size_t, C.c_int]; L.ref_rx11b_run.restype = C.c_int
+        L.ref_rx11b_debug.argtypes = [C.c_void_p]; L.ref_rx11b_debug.restype = None
+        L.ref_rx11b_debug_reset.argtypes = []; L.ref_rx11b_debug_reset.restype = None
+        _REF_RX11B = L
+    return _REF_RX11B
+def _ref_decode(fn, x, per, last):
+    x = np.ascontiguousarray(x, np.int16).reshape(-1, per, 2); out = np.zeros(len(x), np.uint8)
+    l = np.ascontiguousarray(last, np.int16).reshape(2); lo = np.zeros(2, np.int16)
+    getattr(_ref_rx11b(), fn)(_p(x), len(x), _p(l), _p(out), _p(lo)); return out, lo
+def ref_cck11_decode(chips, last=(0, 0)):
+    """TCCK11Decoder (cck.hpp), one instance, on int16 [n, 8, 2] symbols: (bytes [n], last_symbol after)."""
+    return _ref_decode("ref_cck11_decode", chips, 8, last)
+def ref_cck5_decode(chips, last=(0, 0)):
+    """TCCK5P5Decoder (cck.hpp) on int16 [n, 16, 2]: (bytes [n], last_symbol after)."""
+    return _ref_decode("ref_cck5_decode", chips, 16, last)
+def ref_dqpsk_demap(sym, last=(0, 0)):
+    """TDQPSKDemap (barkerspread.hpp) on int16 [n, 4, 2] symbols: (bytes [n], last_symbol after)."""
+    return _ref_decode("ref_dqpsk_demap", sym, 4, last)
+def ref_dbpsk_demap(sym, last=(0, 0)):
+    """TDBPSKDemap (barkerspread.hpp) on int16 [n, 8, 2] symbols: (bytes [n], last_symbol after)."""
+    return _ref_decode("ref_dbpsk_demap", sym, 8, last)
+def ref_despread(chips):
+    """TBB11bDespread (barkerspread.hpp) on int16 [n, 11, 2] chips: int16 [n, 2] symbols."""
+    x = np.ascontiguousarray(chips, np.int16).reshape(-1, 11, 2); out = np.zeros((len(x), 2), np.int16)
+    _ref_rx11b().ref_despread(_p(x), len(x), _p(out)); return out
+PLCP11B_FIELDS = ("error_code", "plcp_state", "rxrate_state", "rate_kbps", "frame_length")
+def ref_plcp11b_parse(hdr6, prev=(0, 0, 0)):
+    """TBB11bPlcpParser (PHY_11b.hpp) on uint8 [n, 6] headers in turn through one context (CF_11bRxVector and CF_11bRxMRSel carry over
+    from `prev` = (rxrate_state, rate_kbps, frame_length)): uint32 [n, 5] (PLCP11B_FIELDS)."""
+    h = np.ascontiguousarray(hdr6, np.uint8).reshape(-1, 6); out = np.zeros((len(h), 5), np.uint32); pv = np.asarray(prev, np.uint32)
+    _ref_rx11b().ref_plcp11b_parse(_p(h), len(h), _p(pv), _p(out)); return out
+def ref_desc_sink11b(scrambled, seed, frame_length):
+    """TDesc741 -> TBB11bFrameSink (scramble.hpp, PHY_11b.hpp), fresh, byte_reg = seed: (error code, crc32 low 24 bits, frame bytes)."""
+    d = np.ascontiguousarray(scrambled, np.uint8); out = np.zeros(max(frame_length, 1), np.uint8); crc = np.zeros(1, np.uint32)
+    e = _ref_rx11b().ref_desc_sink(_p(d), len(d), seed, frame_length, _p(out), _p(crc))
+    return int(e), int(crc[0]), out[:frame_length]
+def ref_rx11b_run(iq, max_frames=8, out_stride=4096):
+    """CreateDemodGraph driven as MAC11b_Receive drives it, on one 44 Msps capture: (RES11B_DTYPE events, bytes [ne, out_stride])."""
+    iq = np.ascontiguousarray(iq, np.int16).reshape(-1, 2)
+    res = np.zeros(max_frames, dtype=RES11B_DTYPE); out = np.zeros((max_frames, out_stride), np.uint8)
+    n = _ref_rx11b().ref_rx11b_run(_p(iq), iq.shape[0], _p(res), _p(out), out_stride, max_frames)
+    return res[:n], out[:n]
+def ref_rx11b_batch(iq, off, length, out_stride=4096):
+    """ref_rx11b_run on each slot, first event only, shaped like rx11b_batch (a slot without an event reports E_NO_FRAME)."""
+    iq = np.ascontiguousarray(iq, np.int16).reshape(-1, 2)
+    res = np.zeros(len(off), dtype=RES11B_DTYPE); out = np.zeros((len(off), out_stride), np.uint8); res["status"] = E_NO_FRAME
+    for i, (o, n) in enumerate(zip(off, length)):
+        r, b = ref_rx11b_run(iq[int(o):int(o) + int(n)], 1, out_stride)
+        if len(r): res[i] = r[0]; out[i] = b[0]
+    return res, out
+def ref_rx11b_debug_reset():
+    _ref_rx11b().ref_rx11b_debug_reset()
+def ref_rx11b_debug():
+    """What the tap counted since the last ref_rx11b_debug_reset on this thread, as {name: count} (REF_RX11B_COUNTERS)."""
+    d = np.zeros(len(REF_RX11B_COUNTERS), np.uint64); _ref_rx11b().ref_rx11b_debug(d.ctypes.data)
+    return dict(zip(REF_RX11B_COUNTERS, (int(v) for v in d)))
+def _cck_n(fn, x, per, last):
+    x = np.ascontiguousarray(x, np.int16).reshape(-1, per, 2); out = np.zeros(len(x), np.uint8); l = np.array(last, np.int16).reshape(2).copy()
+    fn(_p(x), C.c_uint64(len(x)), _p(l), _p(out)); return out, l
+def cck11_decode_n(chips, last=(0, 0)):
+    """The oracle's CCK-11 decoder on int16 [n, 8, 2] symbols in turn (is_even from 0): (bytes [n], last_symbol after)."""
+    return _cck_n(lib().sbo_cck11_decode_n, chips, 8, last)
+def dbpsk_demap_n(sym, last=(0, 0)):
+    """The oracle's DBPSK demapper on int16 [n, 8, 2] symbols in turn: (bytes [n], last_symbol after)."""
+    return _cck_n(lib().sbo_dbpsk_demap_n, sym, 8, last)
+def dqpsk_demap_n(sym, last=(0, 0)):
+    """The oracle's DQPSK demapper on int16 [n, 4, 2] symbols in turn: (bytes [n], last_symbol after)."""
+    return _cck_n(lib().sbo_dqpsk_demap_n, sym, 4, last)
+def despread_n(chips):
+    """The oracle's Barker despreader on int16 [n, 11, 2] chips: int16 [n, 2] symbols."""
+    x = np.ascontiguousarray(chips, np.int16).reshape(-1, 11, 2); out = np.zeros((len(x), 2), np.int16)
+    lib().sbo_despread_n(_p(x), C.c_uint64(len(x)), _p(out)); return out
+def cck5_decode_n(chips, last=(0, 0)):
+    """The oracle's CCK-5.5 decoder on int16 [n, 16, 2] bytes in turn: (bytes [n], last_symbol after)."""
+    return _cck_n(lib().sbo_cck5_decode_n, chips, 16, last)

@@ -158,3 +158,14 @@ if __name__ == "__main__":
         import oracle_py
         oracle_py.use_library(sys.argv[1])
     _run_oracle()
+
+def cck_rail_frames_11b(rate_kbps, n=4, seed=0):
+    """802.11b frames at 5.5 or 11 Mbps whose 64-byte PSDU is replaced by random rectangular chips on the int16 rails (32767 / -32768,
+    four samples per chip).  The lead is 200 samples, so the energy detector fires on the first preamble vector and the DC estimate stays
+    exactly 0: the CCK decoders see the rails themselves.  There the phase decision on the last chip (soradsp.h:190-199) halves re and im
+    before re + im; without the halving re + im wraps and the delivered bytes change.  Returns int16 [n, slot, 2]."""
+    iq, _ = synth.make_frames_11b(n, psdu_len=64, rate_kbps=rate_kbps, snr_db=None, gain=1.0, seed0=0x2A11 + rate_kbps + seed, lead=200)
+    p0 = 200 + 192 * 44; nchip = 64 * (8 if rate_kbps == 11000 else 16)
+    chips = np.where(np.random.default_rng(seed + rate_kbps).random((n, nchip, 2)) < 0.5, -32768, 32767).astype(np.int16)
+    iq[:, p0:p0 + 4 * nchip] = np.repeat(chips, 4, axis=1)
+    return iq

@@ -35,8 +35,12 @@ def test_all_rates(eng, rate):
         iq, ps = synth.make_frames_11b(5, psdu_len=96, rate_kbps=rate, snr_db=snr, gain=gain, seed0=rate + 7)
         F, slot, _ = iq.shape
         res, out = _cmp(eng, iq.reshape(-1, 2), np.arange(F, dtype=np.uint64) * slot, np.full(F, slot, np.uint32))
-        if snr in (None, 40) and not (rate == 11000 and snr is None):
-            assert (res["status"] == 1).all() and (out[:, :95] == ps[:, :95]).all()
+        if snr in (None, 40):
+            # frame 2 of the clean 11 Mbps frames at gain 1.0 (peak 32512) fails its FCS in the reference's own chain too
+            # (test_gpu_rx11b_reference.py::test_full_scale_11m_equals_the_reference); every other frame must decode
+            ok = np.ones(F, bool)
+            if rate == 11000 and snr is None: ok[2] = False
+            assert (res["status"][ok] == 1).all() and (out[ok, :95] == ps[ok, :95]).all()
 
 def test_edges(eng):
     rng = np.random.default_rng(4)
