@@ -329,6 +329,24 @@ uint64_t sbo_tx11a_modulate(const uint8_t* payload, uint32_t len, uint32_t rate_
     return tx11a_modulate(payload, len, rate_kbps, seed, out, (size_t)cap_samples, tail_zeros);
 }
 uint32_t sbo_tx11a_nsym(uint32_t len, uint32_t rate_kbps) { return tx11a_nsym(len, rate_kbps); }
+// the 802.11a transmit stages on their own (tx11a.h); bits one per byte
+void sbo_tx11a_scramble_n(const uint8_t* in, const uint8_t* ctrl, uint64_t n, uint8_t seed, uint8_t* out) { uint8_t reg = seed; tx11a_scramble(in, ctrl, (size_t)n, reg, out); }
+uint64_t sbo_tx11a_encode_bits(const uint8_t* in, uint64_t n, int cr, uint8_t* out) {
+    std::vector<uint8_t> b(in, in + n), c; tx11a_encode_bits(b, cr, c); memcpy(out, c.data(), c.size()); return c.size();
+}
+void sbo_tx11a_interleave_n(const uint8_t* coded, uint64_t nsym, int nbpsc, uint8_t* air) {
+    for (uint64_t s = 0; s < nsym; s++) tx11a_interleave(coded + 48 * nbpsc * s, nbpsc, air + 48 * nbpsc * s);
+}
+void sbo_tx11a_map_n(const uint8_t* air, uint64_t nsym, int nbpsc, int16_t* d48) {
+    for (uint64_t s = 0; s < nsym; s++) tx11a_map(air + 48 * nbpsc * s, nbpsc, (c16*)d48 + 48 * s);
+}
+void sbo_tx11a_add_pilot_n(const int16_t* d48, uint64_t nsym, int16_t* f64) {          // pilot index 127 first, as after T11aAddPilot::Reset
+    unsigned pi = 127; for (uint64_t s = 0; s < nsym; s++) tx11a_add_pilot((const c16*)d48 + 48 * s, pi, (c16*)f64 + 64 * s);
+}
+void sbo_tx11a_ifftx_n(const int16_t* f64, uint64_t nsym, int16_t* out160) {
+    for (uint64_t s = 0; s < nsym; s++) tx11a_ifftx((const c16*)f64 + 64 * s, (c16*)out160 + 160 * s);
+}
+void sbo_tx11a_pack8_n(const int16_t* in, uint64_t n, int8_t* out) { tx11a_pack8((const c16*)in, (size_t)n, out); }
 uint64_t sbo_tx11a_legacy_modulate(const uint8_t* mpdu, uint32_t len, int append_crc, uint32_t rate_kbps, const int16_t* preamble640, int8_t* out, uint64_t cap_samples) {
     return tx11a_legacy_modulate(mpdu, len, append_crc, rate_kbps, (const c16*)preamble640, out, (size_t)cap_samples);
 }

@@ -3,9 +3,9 @@
 # bricks include in place of the reference's framework headers, which only MSVC / the WDK compile.  Each stands for what the reference
 # header gives the bricks, with the line it comes from.  TEST INFRASTRUCTURE ONLY; nothing of the reference is copied here.
 # The shims:
-#   tpltrick.h    Log2, IsPower2, DummyInitializer and static_wrapper (tpltrick.h:95-148; the header itself redeclares template
+#   tpltrick.h    intpow, ceiling_div (tpltrick.h:23-31), Log2, IsPower2, DummyInitializer and static_wrapper (tpltrick.h:95-148; the header itself redeclares template
 #                 parameters as member typedefs, :91-96, which GCC rejects); operator_repeater.h: rep_mul, rep_shift_right, rep_sub,
-#                 rep_memzero, rep_memcpy as the loops operator_repeater.h:42-173, 314 unroll (its rep_saturated_sub names a member
+#                 rep_memzero, rep_memcpy, rep_or as the loops operator_repeater.h:42-173, 314 unroll (its rep_saturated_sub names a member
 #                 that does not exist, :182, which GCC rejects even uninstantiated);
 #   const.h       the repo's own sora_b200/brick/brick.hpp (BRICK macros, TFilter / TSink, pin queues) with CTX_VAR_RW / CTX_VAR_RO /
 #                 FACADE_FIELD taking the array extent the reference writes (CTX_VAR_RW(vcs, ChannelCoeffs, [16]), brick.h:426-470), a
@@ -39,9 +39,10 @@
 #   windef.h, soratypes.h   the Windows integer names the 802.11b headers use (USHORT, PUSHORT, BOOLEAN, BYTE / WORD / DWORD, ...)
 #                 and soratypes.h:22-33's typedefs (its `ulong` is the compiler's `unsigned long`: a build that wants MSVC's 32-bit
 #                 width defines the name itself);
-#   demux.h       TDemux with up to five outputs (kernel/brick/inc/demux.h:13-152: AddRef of every output, Reset and Flush of every
+#   demux.h       TDemux with up to eight outputs (kernel/brick/inc/demux.h:13-152: AddRef of every output, Reset and Flush of every
 #                 output, an empty Process), DEFINE_OPORTS (brick.h:204-240), FlushPort(N) (brick.h:461), DummyBrick (brick.h:477-490),
-#                 and the TDEMUX2/4/5 macro sets (demux.h:154-266).
+#                 and the TDEMUX2/4/5/8 macro sets (demux.h:154-266, :343-382);
+#   vector128.h, further: vb and saturated_pack(vs, vs) (_mm_packs_epi16, vector128.h:870), whose lanes feed sbref::tap_spack.
 ref_shim() {
 mkdir -p "$1/bb"
 cat > "$1/const.h" <<'SHIM'
@@ -87,6 +88,9 @@ template<int N> struct Log2 { enum { value = Log2<N / 2>::value + 1 }; };
 template<> struct Log2<1> { enum { value = 0 }; };
 template<int N> struct IsPower2 { enum { IsFalse = (N & 1) + IsPower2<N / 2>::IsFalse }; };
 template<> struct IsPower2<1> { enum { IsFalse = 0 }; };
+template<int x, unsigned int p> struct intpow { enum { value = x * intpow<x, p - 1>::value }; };
+template<int x> struct intpow<x, 0> { enum { value = 1 }; };
+template<int x, int y> struct ceiling_div { enum { value = (x + y - 1) / y }; };
 struct DummyInitializer { void operator()(...) { } };
 template<typename T, typename INITIALIZER = DummyInitializer> class static_wrapper {
     static T value __attribute__((aligned(16)));
@@ -105,6 +109,7 @@ template<size_t N, typename T> inline void rep_shift_right(T* dst, const T* src,
 template<size_t N, typename T> inline void rep_sub(T* dst, const T* src, const T& val) { for (size_t i = 0; i < N; i++) *dst++ = sub(*src++, val); }
 template<size_t N, typename T> inline void rep_memzero(T* dst) { for (size_t i = 0; i < N; i++) set_zero(*dst++); }
 template<size_t N, typename T> inline void rep_memcpy(T* dst, const T* src) { for (size_t i = 0; i < N; i++) *dst++ = *src++; }
+template<size_t N, typename T> inline void rep_or(T* dst, const T* src0, const T* src1) { for (size_t i = 0; i < N; i++) *dst++ = (*src0++) | (*src1++); }
 template<size_t N> inline void rep_sqrnorm(vi* dst, const vcs* src) { for (size_t i = 0; i < N; i++) *dst++ = SquaredNorm(*src++); }
 template<size_t N, typename T> inline void rep_sum(T& result, const T* src) { for (size_t i = 0; i < N; i++) result += *src++; }
 SHIM
@@ -162,31 +167,39 @@ public:
 inline DummyBrick DummyBrickInstance;
 #define NON_DUMMYBRICK(INDEX) (!std::is_same<T_NEXT##INDEX, DummyBrick>::value)
 template<class T_CTX, class T_NEXT0 = DummyBrick, class T_NEXT1 = DummyBrick, class T_NEXT2 = DummyBrick, class T_NEXT3 = DummyBrick,
-         class T_NEXT4 = DummyBrick>
+         class T_NEXT4 = DummyBrick, class T_NEXT5 = DummyBrick, class T_NEXT6 = DummyBrick, class T_NEXT7 = DummyBrick>
 class TDemux : public TBrick<T_CTX>, public IReferenceCounting, public IControlPoint {
 protected:
-    T_NEXT0* __next_0; T_NEXT1* __next_1; T_NEXT2* __next_2; T_NEXT3* __next_3; T_NEXT4* __next_4;
+    T_NEXT0* __next_0; T_NEXT1* __next_1; T_NEXT2* __next_2; T_NEXT3* __next_3; T_NEXT4* __next_4; T_NEXT5* __next_5; T_NEXT6* __next_6;
+    T_NEXT7* __next_7;
     T_NEXT0* Next0() { return __next_0; } T_NEXT1* Next1() { return __next_1; } T_NEXT2* Next2() { return __next_2; }
-    T_NEXT3* Next3() { return __next_3; } T_NEXT4* Next4() { return __next_4; }
+    T_NEXT3* Next3() { return __next_3; } T_NEXT4* Next4() { return __next_4; } T_NEXT5* Next5() { return __next_5; }
+    T_NEXT6* Next6() { return __next_6; } T_NEXT7* Next7() { return __next_7; }
 public:
     typedef TDemux TDemuxBase;
     TDemux(T_CTX& ctx, T_NEXT0* n0 = NULL, T_NEXT1* n1 = NULL, T_NEXT2* n2 = &DummyBrickInstance, T_NEXT3* n3 = &DummyBrickInstance,
-           T_NEXT4* n4 = &DummyBrickInstance) : TBrick<T_CTX>(ctx), __next_0(n0), __next_1(n1), __next_2(n2), __next_3(n3), __next_4(n4) {
+           T_NEXT4* n4 = &DummyBrickInstance, T_NEXT5* n5 = &DummyBrickInstance, T_NEXT6* n6 = &DummyBrickInstance,
+           T_NEXT7* n7 = &DummyBrickInstance)
+        : TBrick<T_CTX>(ctx), __next_0(n0), __next_1(n1), __next_2(n2), __next_3(n3), __next_4(n4), __next_5(n5), __next_6(n6), __next_7(n7) {
         if (NON_DUMMYBRICK(0)) AddRef(Next0()); if (NON_DUMMYBRICK(1)) AddRef(Next1()); if (NON_DUMMYBRICK(2)) AddRef(Next2());
-        if (NON_DUMMYBRICK(3)) AddRef(Next3()); if (NON_DUMMYBRICK(4)) AddRef(Next4());
+        if (NON_DUMMYBRICK(3)) AddRef(Next3()); if (NON_DUMMYBRICK(4)) AddRef(Next4()); if (NON_DUMMYBRICK(5)) AddRef(Next5());
+        if (NON_DUMMYBRICK(6)) AddRef(Next6()); if (NON_DUMMYBRICK(7)) AddRef(Next7());
     }
     ~TDemux() {
         if (NON_DUMMYBRICK(0)) IReferenceCounting::Release(Next0()); if (NON_DUMMYBRICK(1)) IReferenceCounting::Release(Next1());
         if (NON_DUMMYBRICK(2)) IReferenceCounting::Release(Next2()); if (NON_DUMMYBRICK(3)) IReferenceCounting::Release(Next3());
-        if (NON_DUMMYBRICK(4)) IReferenceCounting::Release(Next4());
+        if (NON_DUMMYBRICK(4)) IReferenceCounting::Release(Next4()); if (NON_DUMMYBRICK(5)) IReferenceCounting::Release(Next5());
+        if (NON_DUMMYBRICK(6)) IReferenceCounting::Release(Next6()); if (NON_DUMMYBRICK(7)) IReferenceCounting::Release(Next7());
     }
     void Reset() {
         if (NON_DUMMYBRICK(0)) Next0()->Reset(); if (NON_DUMMYBRICK(1)) Next1()->Reset(); if (NON_DUMMYBRICK(2)) Next2()->Reset();
-        if (NON_DUMMYBRICK(3)) Next3()->Reset(); if (NON_DUMMYBRICK(4)) Next4()->Reset();
+        if (NON_DUMMYBRICK(3)) Next3()->Reset(); if (NON_DUMMYBRICK(4)) Next4()->Reset(); if (NON_DUMMYBRICK(5)) Next5()->Reset();
+        if (NON_DUMMYBRICK(6)) Next6()->Reset(); if (NON_DUMMYBRICK(7)) Next7()->Reset();
     }
     void Flush() {
         if (NON_DUMMYBRICK(0)) Next0()->Flush(); if (NON_DUMMYBRICK(1)) Next1()->Flush(); if (NON_DUMMYBRICK(2)) Next2()->Flush();
-        if (NON_DUMMYBRICK(3)) Next3()->Flush(); if (NON_DUMMYBRICK(4)) Next4()->Flush();
+        if (NON_DUMMYBRICK(3)) Next3()->Flush(); if (NON_DUMMYBRICK(4)) Next4()->Flush(); if (NON_DUMMYBRICK(5)) Next5()->Flush();
+        if (NON_DUMMYBRICK(6)) Next6()->Flush(); if (NON_DUMMYBRICK(7)) Next7()->Flush();
     }
     template<class T_IPIN> bool Process(T_IPIN&) { return true; }
 };
@@ -212,6 +225,12 @@ public:
     : TDemux<TDEMUX5_PARAMS>(ctx, n0, n1, n2, n3, n4)
 #define STD_TDEMUX5_RESET() FINL void Reset() { this->TDemuxBase::Reset(); opin0().clear(); opin1().clear(); opin2().clear(); opin3().clear(); \
     opin4().clear(); __ResetSelf(); } FINL void __ResetSelf()
+#define TDEMUX8_ARGS class T_CTX, class T_NEXT0, class T_NEXT1, class T_NEXT2, class T_NEXT3, class T_NEXT4, class T_NEXT5, class T_NEXT6, class T_NEXT7
+#define TDEMUX8_PARAMS T_CTX, T_NEXT0, T_NEXT1, T_NEXT2, T_NEXT3, T_NEXT4, T_NEXT5, T_NEXT6, T_NEXT7
+#define STD_DEMUX8_CONSTRUCTOR(name) name(T_CTX& ctx, T_NEXT0* n0, T_NEXT1* n1, T_NEXT2* n2, T_NEXT3* n3, T_NEXT4* n4, T_NEXT5* n5, T_NEXT6* n6, \
+                                          T_NEXT7* n7) : TDemux<TDEMUX8_PARAMS>(ctx, n0, n1, n2, n3, n4, n5, n6, n7)
+#define STD_TDEMUX8_RESET() FINL void Reset() { this->TDemuxBase::Reset(); opin0().clear(); opin1().clear(); opin2().clear(); opin3().clear(); \
+    opin4().clear(); opin5().clear(); opin6().clear(); opin7().clear(); __ResetSelf(); } FINL void __ResetSelf()
 #define CREATE_BRICK_DEMUX2(NAME, TPL, CTX, N0, N1) \
     typedef TPL<std::remove_reference<decltype(CTX)>::type, std::remove_reference<decltype(*N0)>::type, std::remove_reference<decltype(*N1)>::type> __C_##NAME; \
     __C_##NAME* NAME = new __C_##NAME(CTX, N0, N1);
@@ -219,6 +238,11 @@ public:
     typedef TPL<std::remove_reference<decltype(CTX)>::type, std::remove_reference<decltype(*N0)>::type, std::remove_reference<decltype(*N1)>::type, \
                 std::remove_reference<decltype(*N2)>::type, std::remove_reference<decltype(*N3)>::type, std::remove_reference<decltype(*N4)>::type> __C_##NAME; \
     __C_##NAME* NAME = new __C_##NAME(CTX, N0, N1, N2, N3, N4);
+#define CREATE_BRICK_DEMUX8(NAME, TPL, CTX, N0, N1, N2, N3, N4, N5, N6, N7) \
+    typedef TPL<std::remove_reference<decltype(CTX)>::type, std::remove_reference<decltype(*N0)>::type, std::remove_reference<decltype(*N1)>::type, \
+                std::remove_reference<decltype(*N2)>::type, std::remove_reference<decltype(*N3)>::type, std::remove_reference<decltype(*N4)>::type, \
+                std::remove_reference<decltype(*N5)>::type, std::remove_reference<decltype(*N6)>::type, std::remove_reference<decltype(*N7)>::type> __C_##NAME; \
+    __C_##NAME* NAME = new __C_##NAME(CTX, N0, N1, N2, N3, N4, N5, N6, N7);
 SHIM
 cat > "$1/soratime.h" <<'SHIM'
 #pragma once
@@ -275,6 +299,7 @@ SB_VEC(vcs, COMPLEX16)
 typedef struct _COMPLEX32 { int re, im; } COMPLEX32;
 SB_VEC(vci, COMPLEX32)
 SB_VEC(vcb, COMPLEX8)
+SB_VEC(vb, signed char)
 struct COMPLEXU32 { unsigned int re, im; };
 SB_VEC(vcui, COMPLEXU32)
 template<typename T> inline T& cast_ref(void* p) { return *reinterpret_cast<T*>(p); }
@@ -286,7 +311,7 @@ struct SignalBlock {
     const vcs& operator[](size_t index) const { return _data[index]; }
 };
 namespace sbref { extern int phase; void tap_pack(__m128i v, int k); void tap_zero(__m128i v); void tap_clamp(__m128i r, __m128i a);
-                  void tap_madd(__m128i v); }
+                  void tap_madd(__m128i v); void tap_spack(__m128i a, __m128i b); }
 class vector128_consts {
 public:
     template<typename T> static T __0x0000FFFF0000FFFF0000FFFF0000FFFF() { return (T)_mm_set1_epi32(0x0000FFFF); }
@@ -344,6 +369,7 @@ inline vs pack(const vi& a, const vi& b) {
     const __m128i m = vector128_consts::__0x0000FFFF0000FFFF0000FFFF0000FFFF<vi>();
     return vs(_mm_or_si128(_mm_and_si128(a, m), _mm_slli_epi32(_mm_and_si128(b, m), 16)));
 }
+inline vb saturated_pack(const vs& a, const vs& b) { sbref::tap_spack(a, b); return vb(_mm_packs_epi16(a, b)); }
 inline void pack(vcs& r, const vi& re, const vi& im) { sbref::tap_pack(re, 0); sbref::tap_pack(im, 0); r = (vcs)pack(re, im); }
 inline void conj_mul(vi& re, vi& im, const vcs& a, const vcs& b) {
     vcs vs1 = flip(b);

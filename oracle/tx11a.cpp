@@ -17,7 +17,7 @@ static const RateInfo RATES[8] = {{6000, 0xB, 1, CR_12, 24}, {9000, 0xF, 1, CR_3
 static const RateInfo* rate_info(uint32_t kbps) { for (auto& r : RATES) if (r.kbps == kbps) return &r; return nullptr; }
 
 // IFFTx of one 64-carrier symbol: zero-stuffed IFFT<128>, >> 4, 32-sample GI, window (fft.hpp:9-60)
-static void ifftx(const c16* f64, c16* out160) {
+void tx11a_ifftx(const c16* f64, c16* out160) {
     alignas(16) c16 t[128], o[128];
     memset(t, 0, sizeof t); memcpy(t, f64, 32 * sizeof(c16)); memcpy(t + 96, f64 + 32, 32 * sizeof(c16));
     ifft128((v128*)t, (v128*)o);
@@ -26,6 +26,7 @@ static void ifftx(const c16* f64, c16* out160) {
     for (int i : {0, 1, 158, 159}) { out160[i].re >>= 1; out160[i].im >>= 1; }
 }
 static inline int8_t pack8(int16_t v) { return (int8_t)(v > 127 ? 127 : v < -128 ? -128 : v); }   // TPackSample16to8: packsswb (stdbrick.hpp:413-445)
+void tx11a_pack8(const c16* in, size_t n, int8_t* out) { for (size_t i = 0; i < n; i++) { out[2 * i] = pack8(in[i].re); out[2 * i + 1] = pack8(in[i].im); } }
 
 void tx11a_preamble16(c16* lut) {
     alignas(16) c16 t[128], o[128];
@@ -56,36 +57,67 @@ uint32_t tx11a_nsym(uint32_t len, uint32_t rate_kbps) {
     return (bits + ((padded - bits + 7u) / 8u) * 8u) / ri->ndbps;
 }
 
-// one OFDM symbol worth of coded bits -> 160 samples (interleave.hpp:16-96, mapper11a.hpp:13-298, pilot.hpp:31-118, fft.hpp:9-60)
-static void symbol_out(const uint8_t* coded /*ncbps bits, one per byte*/, int nbpsc, unsigned& pilot_index, int8_t* out) {
+// T11Interleave (interleave.hpp:16-96): coded bit k of the symbol goes on air at deint[k]; one bit per byte both sides
+void tx11a_interleave(const uint8_t* coded, int nbpsc, uint8_t* air) {
     const Tables& T = tables();
-    const int ncbps = 48 * nbpsc;
-    const uint16_t* dm = nbpsc == 1 ? T.deint48 : nbpsc == 2 ? T.deint96 : nbpsc == 4 ? T.deint192 : T.deint288;   // deint[k] = position on air of coded bit k
-    uint8_t air[288];
-    for (int k = 0; k < ncbps; k++) air[dm[k]] = coded[k];
-    alignas(16) c16 f[64]; memset(f, 0, sizeof f);
+    const uint16_t* dm = nbpsc == 1 ? T.deint48 : nbpsc == 2 ? T.deint96 : nbpsc == 4 ? T.deint192 : T.deint288;
+    for (int k = 0; k < 48 * nbpsc; k++) air[dm[k]] = coded[k];
+}
+
+// TMap11a* (mapper11a.hpp:13-298): 48 * nbpsc air bits -> 48 points.  Levels are (2b - (2^m - 1)) * kmod with the Gray code read first bit
+// most significant (InitQamMapLut: bit-reverse, Gray -> binary)
+void tx11a_map(const uint8_t* air, int nbpsc, c16* d48) {
     const int16_t km = kmod_of(nbpsc); const int h = nbpsc / 2;
-    auto level = [&](const uint8_t* b, int m) -> int16_t {                                   // InitQamMapLut: bit-reverse, Gray -> binary, 2b - (2^m - 1)
+    auto level = [&](const uint8_t* b, int m) -> int16_t {
         int g = 0; for (int i = 0; i < m; i++) g = (g << 1) | b[i];
         int bin = 0, acc = 0; for (int i = m - 1; i >= 0; i--) { acc ^= (g >> i) & 1; bin = (bin << 1) | acc; }
         return (int16_t)((2 * bin - ((1 << m) - 1)) * km);
     };
+    for (int d = 0; d < 48; d++) {
+        const uint8_t* b = air + d * nbpsc;
+        if (nbpsc == 1) { d48[d].re = b[0] ? BPSK_MOD : (int16_t)-BPSK_MOD; d48[d].im = 0; }
+        else { d48[d].re = level(b, h); d48[d].im = level(b + h, h); }
+    }
+}
+
+// T11aAddPilot<> (pilot.hpp:10-119): data on carriers 38..63 then 1..26 around the pilots, pilots by PilotSgn[pilot_index], then the index
+// advances (wrapping 127 -> 0 past 126); DC and the guard carriers stay 0
+void tx11a_add_pilot(const c16* d48, unsigned& pilot_index, c16* f64) {
+    memset(f64, 0, 64 * sizeof(c16));
     int d = 0;
     for (int pass = 0; pass < 2; pass++)
         for (int i = pass ? 1 : 38; i <= (pass ? 26 : 63); i++) {
             if (i == 43 || i == 57 || i == 7 || i == 21) continue;
-            const uint8_t* b = air + d * nbpsc; d++;
-            if (nbpsc == 1) { f[i].re = b[0] ? BPSK_MOD : (int16_t)-BPSK_MOD; f[i].im = 0; }
-            else { f[i].re = level(b, h); f[i].im = level(b + h, h); }
+            f64[i] = d48[d++];
         }
     static const uint8_t* neg = nullptr; static uint8_t negtab[128];
     if (!neg) { unsigned st = 0x7F; uint8_t seq[127]; for (int i = 0; i < 127; i++) { unsigned o = ((st >> 6) ^ (st >> 3)) & 1; st = ((st << 1) | o) & 0x7F; seq[i] = (uint8_t)o; }
                 for (int i = 0; i < 127; i++) negtab[i] = seq[(i + 1) % 127]; negtab[127] = 0; neg = negtab; }   // PilotSgn (pilot.hpp:10-28): [i] = p_{i+1}, [127] = SIGNAL
     const int s = neg[pilot_index] ? -1 : 1;
-    f[7].re = (int16_t)(s * BPSK_MOD); f[21].re = (int16_t)(-s * BPSK_MOD); f[57].re = (int16_t)(s * BPSK_MOD); f[43].re = (int16_t)(s * BPSK_MOD);
+    f64[7].re = (int16_t)(s * BPSK_MOD); f64[21].re = (int16_t)(-s * BPSK_MOD); f64[57].re = (int16_t)(s * BPSK_MOD); f64[43].re = (int16_t)(s * BPSK_MOD);
     pilot_index++; if (pilot_index >= 127) pilot_index = 0;
-    c16 td[160]; ifftx(f, td);
-    for (int i = 0; i < 160; i++) { out[2 * i] = pack8(td[i].re); out[2 * i + 1] = pack8(td[i].im); }
+}
+
+// one OFDM symbol worth of coded bits -> 160 samples: the stages above, TIFFTx, TPackSample16to8
+static void symbol_out(const uint8_t* coded /*ncbps bits, one per byte*/, int nbpsc, unsigned& pilot_index, int8_t* out) {
+    uint8_t air[288]; c16 d[48], f[64], td[160];
+    tx11a_interleave(coded, nbpsc, air);
+    tx11a_map(air, nbpsc, d);
+    tx11a_add_pilot(d, pilot_index, f);
+    tx11a_ifftx(f, td);
+    tx11a_pack8(td, 160, out);
+}
+
+// T11aSc (scramble.hpp:170-262): per byte, ctrl 0 passes it (NO_SCRAMBLE), 1 steps the register and XORs (DO_SCRAMBLE), anything else
+// steps, XORs and keeps the top two bits (TAIL_SCRAMBLE: the six tail bits leave the encoder as zeros)
+void tx11a_scramble(const uint8_t* in, const uint8_t* ctrl, size_t n, uint8_t& reg, uint8_t* out) {
+    const Tables& T = tables();
+    for (size_t i = 0; i < n; i++) {
+        if (ctrl[i] == 0) { out[i] = in[i]; continue; }
+        reg = T.scramble_lut[reg >> 1];
+        out[i] = (uint8_t)(in[i] ^ reg);
+        if (ctrl[i] != 1) out[i] &= 0xC0;
+    }
 }
 
 // rate-1/2 mother code, bits LSB first, then puncturing (conv_enc.hpp:5-280): returns coded bits, one per byte
@@ -112,7 +144,7 @@ size_t tx11a_modulate(const uint8_t* payload, uint32_t len, uint32_t rate_kbps, 
     if (total > cap) return 0;
     // preamble through the 16 -> 8 bit pack
     c16 pre[640]; tx11a_preamble16(pre);
-    for (int i = 0; i < 640; i++) { out[2 * i] = pack8(pre[i].re); out[2 * i + 1] = pack8(pre[i].im); }
+    tx11a_pack8(pre, 640, out);
     unsigned pilot_index = 127;
     // SIGNAL: rate code, reserved, LENGTH (incl. FCS), even parity, 6 tail bits; never scrambled, always 6 Mbps (ieee80211a_cmn.h B11aGetPLCPSignal)
     {
@@ -127,13 +159,9 @@ size_t tx11a_modulate(const uint8_t* payload, uint32_t len, uint32_t rate_kbps, 
     const uint32_t nbytes = nsym * ri->ndbps / 8u;
     std::vector<uint8_t> data(nbytes, 0);
     memcpy(data.data() + 2, payload, len); memcpy(data.data() + 2 + len, &crc, 4);
+    std::vector<uint8_t> ctrl(nbytes, 1); ctrl[2 + len + 4] = 2;                // TBB11aSrc: DO_SCRAMBLE, TAIL_SCRAMBLE on the tail byte
     uint8_t reg = sc_seed;
-    const uint32_t tail_at = 2 + len + 4;
-    for (uint32_t i = 0; i < nbytes; i++) {
-        reg = T.scramble_lut[reg >> 1];
-        data[i] = (uint8_t)(data[i] ^ reg);
-        if (i == tail_at) data[i] &= 0xC0;
-    }
+    tx11a_scramble(data.data(), ctrl.data(), nbytes, reg, data.data());
     std::vector<uint8_t> coded; tx11a_encode_bits(data, ri->cr, coded);
     const int ncbps = 48 * ri->nbpsc;
     for (uint32_t s = 0; s < nsym; s++) symbol_out(coded.data() + (size_t)s * ncbps, ri->nbpsc, pilot_index, out + 2 * (640 + 160 * (size_t)(1 + s)));

@@ -6,7 +6,8 @@
 // PARITY UNPINNED: the reference holds no output vector of this graph (the *.mf.bin captures under kernel/HWTest come from another
 // shaping filter: 18 leading zeros and a 1,0,-2,0,4 ramp that neither this graph's 20-tap shaper nor the legacy 37-tap FIR produces).
 // What is checked: the stage tables rebuilt from the reference's formulas, and a round trip through the receive oracle, which IS
-// pinned by those captures.
+// pinned by those captures.  Not yet compared with the graph's own compiled bricks (oracle/build_ref_mod.sh compiles the 802.11a
+// modulator only).
 #pragma once
 #include <stdint.h>
 #include <stddef.h>

@@ -5,7 +5,8 @@
 // Purpose: the reference ships no 802.11n vector at all (SURVEY.md §8c), so the receive oracle (rx11n.cpp) cannot be pinned; this
 // restates the OTHER half of the reference's 11n code, so that the two independently restated halves can be played against each other
 // (tests/test_cpu_oracle_tx11n.py).  PARITY UNPINNED like the receive side; the four preamble tables are regenerated from their
-// defining formula and compared with the reference's literal tables when the reference tree is present.
+// defining formula and compared with the reference's literal tables when the reference tree is present.  Not yet compared with the
+// graphs' own compiled bricks (oracle/build_ref_mod.sh compiles the 802.11a modulator only).
 #pragma once
 #include "tables.h"
 #include <stddef.h>

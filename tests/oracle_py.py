@@ -196,6 +196,35 @@ def tx11a_modulate(payload, rate_kbps, seed=0xFF, tail_zeros=32):
     assert n == cap, (n, cap)
     return out
 
+def tx11a_scramble(data, ctrl, seed):
+    """The oracle's T11aSc: uint8 [n] under the per-byte scramble_ctrl ctrl (0 none, 1 scramble, 2 tail), register from seed."""
+    d = np.ascontiguousarray(data, np.uint8); c = np.ascontiguousarray(np.broadcast_to(ctrl, d.shape), np.uint8); out = np.zeros_like(d)
+    lib().sbo_tx11a_scramble_n(_p(d), _p(c), C.c_uint64(len(d)), C.c_uint8(seed), _p(out)); return out
+def tx11a_encode_bits(data, cr):
+    """The oracle's convolutional encoder and puncturing (cr 0 = 1/2, 1 = 2/3, 2 = 3/4) from state 0: coded bits, one per byte."""
+    d = np.ascontiguousarray(data, np.uint8); out = np.zeros(16 * len(d) + 8, np.uint8); L = lib(); L.sbo_tx11a_encode_bits.restype = C.c_uint64
+    m = L.sbo_tx11a_encode_bits(_p(d), C.c_uint64(len(d)), C.c_int(cr), _p(out)); return out[:m]
+def tx11a_interleave(bits, nbpsc):
+    """The oracle's 802.11a interleaver on bits [nsym, 48 nbpsc] (one per byte): the on-air bits."""
+    b = np.ascontiguousarray(bits, np.uint8).reshape(-1, 48 * nbpsc); out = np.zeros_like(b)
+    lib().sbo_tx11a_interleave_n(_p(b), C.c_uint64(len(b)), C.c_int(nbpsc), _p(out)); return out
+def tx11a_map(bits, nbpsc):
+    """The oracle's 802.11a mapper on on-air bits [nsym, 48 nbpsc]: int16 [nsym, 48, 2]."""
+    b = np.ascontiguousarray(bits, np.uint8).reshape(-1, 48 * nbpsc); out = np.zeros((len(b), 48, 2), np.int16)
+    lib().sbo_tx11a_map_n(_p(b), C.c_uint64(len(b)), C.c_int(nbpsc), _p(out)); return out
+def tx11a_add_pilot(data48):
+    """The oracle's pilot inserter on int16 [nsym, 48, 2] (pilot index 127 first): int16 [nsym, 64, 2]."""
+    d = np.ascontiguousarray(data48, np.int16).reshape(-1, 48, 2); out = np.zeros((len(d), 64, 2), np.int16)
+    lib().sbo_tx11a_add_pilot_n(_p(d), C.c_uint64(len(d)), _p(out)); return out
+def tx11a_ifftx(spec64):
+    """The oracle's TIFFTx on int16 [nsym, 64, 2]: int16 [nsym, 160, 2]."""
+    d = np.ascontiguousarray(spec64, np.int16).reshape(-1, 64, 2); out = np.zeros((len(d), 160, 2), np.int16)
+    lib().sbo_tx11a_ifftx_n(_p(d), C.c_uint64(len(d)), _p(out)); return out
+def tx11a_pack8(x):
+    """The oracle's TPackSample16to8 on int16 [n, 2]: int8 [n, 2]."""
+    d = np.ascontiguousarray(x, np.int16).reshape(-1, 2); out = np.zeros(d.shape, np.int8)
+    lib().sbo_tx11a_pack8_n(_p(d), C.c_uint64(len(d)), _p(out)); return out
+
 def tx11a_legacy_modulate(body, rate_kbps, append_crc=True):
     """The reference's LEGACY transmitter (BB11ATxFrameMod; oracle/tx11a_legacy.cpp).  Returns int8 [n, 2]: 640 + 160 (1 + nsym) + 8 samples at 40 Msps."""
     body = np.ascontiguousarray(body, dtype=np.uint8); L = lib(); L.sbo_tx11a_legacy_modulate.restype = C.c_uint64
@@ -535,3 +564,72 @@ def despread_n(chips):
 def cck5_decode_n(chips, last=(0, 0)):
     """The oracle's CCK-5.5 decoder on int16 [n, 16, 2] bytes in turn: (bytes [n], last_symbol after)."""
     return _cck_n(lib().sbo_cck5_decode_n, chips, 16, last)
+
+
+# ---- oracle/_ref/libmod_ref.so: the reference's own 802.11a brick modulator (oracle/build_ref_mod.sh) ----
+_REF_MOD = None
+REF_MOD_COUNTERS = ("pack_saturated", "pad_9m_pair", "nsym_over_standard")
+def ref_mod_available():
+    return os.path.exists(os.path.join(ROOT, "oracle", "_ref", "libmod_ref.so"))
+def _ref_mod():
+    global _REF_MOD
+    if _REF_MOD is None:
+        L = C.CDLL(os.path.join(ROOT, "oracle", "_ref", "libmod_ref.so"))
+        L.ref_mod11a_frame.argtypes = [C.c_void_p, C.c_uint32, C.c_uint32, C.c_uint8, C.c_void_p, C.c_size_t]; L.ref_mod11a_frame.restype = C.c_int64
+        L.ref_mod11a_scramble.argtypes = [C.c_void_p, C.c_void_p, C.c_size_t, C.c_uint8, C.c_void_p]; L.ref_mod11a_scramble.restype = None
+        L.ref_mod11a_encode.argtypes = [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]; L.ref_mod11a_encode.restype = C.c_size_t
+        L.ref_mod11a_interleave.argtypes = [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]; L.ref_mod11a_interleave.restype = None
+        L.ref_mod11a_map.argtypes = [C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]; L.ref_mod11a_map.restype = C.c_size_t
+        for f in ("ref_mod11a_add_pilot", "ref_mod11a_ifftx", "ref_pack16to8"):
+            getattr(L, f).argtypes = [C.c_void_p, C.c_size_t, C.c_void_p]; getattr(L, f).restype = None
+        L.ref_mod_debug.argtypes = [C.c_void_p]; L.ref_mod_debug.restype = None
+        L.ref_mod_debug_reset.argtypes = []; L.ref_mod_debug_reset.restype = None
+        _REF_MOD = L
+    return _REF_MOD
+def ref_mod11a_frame(payload, rate_kbps, seed=0xFF):
+    """CreatePreamble11a_40M then CreateModGraph11a_40M, driven as Test11A_FB_Mod drives them, with sc_seed = seed: int8 [n, 2] at 40 Msps
+    (what TModSink wrote: preamble, SIGNAL and DATA, no trailing zeros)."""
+    p = np.ascontiguousarray(payload, np.uint8)
+    # room for the preamble, SIGNAL, the standard's N_SYM and two symbols more: the reference pads to at most a 9 Mbps symbol pair and
+    # counts the tail as a whole byte, one symbol each at most.  The library sizes its own buffer the same way and reports how many
+    # samples it wrote, so a graph that wrote more would fail the assert below rather than be cut short.
+    std_nsym = -(-(16 + 8 * (len(p) + 4) + 6) // (rate_kbps // 250))
+    cap = 640 + 160 * (1 + std_nsym + 2); out = np.zeros((cap, 2), np.int8)
+    n = _ref_mod().ref_mod11a_frame(_p(p), len(p), rate_kbps, seed, _p(out), cap)
+    assert 0 < n <= cap, (n, cap)
+    return out[:n]
+def ref_mod11a_scramble(data, ctrl, seed):
+    """T11aSc, fresh, sc_seed = seed, on uint8 [n] with the scramble_ctrl ctrl[i] (0 none, 1 scramble, 2 tail) in force for byte i."""
+    d = np.ascontiguousarray(data, np.uint8); c = np.ascontiguousarray(np.broadcast_to(ctrl, d.shape), np.uint8); out = np.zeros_like(d)
+    _ref_mod().ref_mod11a_scramble(_p(d), _p(c), len(d), seed, _p(out))
+    return out
+def ref_mod11a_encode(cr, data):
+    """TConvEncode_12 (cr 0), _23 (1), _34 (2), fresh, on uint8 [n] (whole input bursts of 1, 2, 3 bytes): the coded bytes."""
+    d = np.ascontiguousarray(data, np.uint8); out = np.zeros(2 * len(d) + 8, np.uint8)
+    m = _ref_mod().ref_mod11a_encode(cr, _p(d), len(d), _p(out)); return out[:m]
+def ref_mod11a_interleave(nbpsc, data):
+    """T11aInterleave{BPSK,QPSK,QAM16,QAM64} on uint8 [nsym, 6 * nbpsc] (coded bits packed LSB first)."""
+    d = np.ascontiguousarray(data, np.uint8).reshape(-1, 6 * nbpsc); out = np.zeros_like(d)
+    _ref_mod().ref_mod11a_interleave(nbpsc, _p(d), len(d), _p(out)); return out
+def ref_mod11a_map(nbpsc, data):
+    """TMap11a{BPSK,QPSK,QAM16,QAM64}<> on uint8 input bursts (1 byte; 3 bytes at QAM64): int16 [m, 2] constellation points."""
+    d = np.ascontiguousarray(data, np.uint8); per = 3 if nbpsc == 6 else 1; out = np.zeros((8 * len(d), 2), np.int16)
+    m = _ref_mod().ref_mod11a_map(nbpsc, _p(d), len(d) // per, _p(out)); return out[:m]
+def ref_mod11a_add_pilot(data48):
+    """T11aAddPilot<>, fresh (pilot index 127 first), on int16 [nsym, 48, 2]: int16 [nsym, 64, 2]."""
+    d = np.ascontiguousarray(data48, np.int16).reshape(-1, 48, 2); out = np.zeros((len(d), 64, 2), np.int16)
+    _ref_mod().ref_mod11a_add_pilot(_p(d), len(d), _p(out)); return out
+def ref_mod11a_ifftx(spec64):
+    """TIFFTx on int16 [nsym, 64, 2] spectra: int16 [nsym, 160, 2] (32-sample GI, windowed)."""
+    d = np.ascontiguousarray(spec64, np.int16).reshape(-1, 64, 2); out = np.zeros((len(d), 160, 2), np.int16)
+    _ref_mod().ref_mod11a_ifftx(_p(d), len(d), _p(out)); return out
+def ref_pack16to8(x):
+    """TPackSample16to8 on int16 [8 n, 2]: int8 [8 n, 2]."""
+    d = np.ascontiguousarray(x, np.int16).reshape(-1, 8, 2); out = np.zeros((len(d) * 8, 2), np.int8)
+    _ref_mod().ref_pack16to8(_p(d), len(d), _p(out)); return out
+def ref_mod_debug_reset():
+    _ref_mod().ref_mod_debug_reset()
+def ref_mod_debug():
+    """What the tap counted since the last ref_mod_debug_reset on this thread, as {name: count} (REF_MOD_COUNTERS)."""
+    d = np.zeros(len(REF_MOD_COUNTERS), np.uint64); _ref_mod().ref_mod_debug(d.ctypes.data)
+    return dict(zip(REF_MOD_COUNTERS, (int(v) for v in d)))
