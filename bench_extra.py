@@ -20,6 +20,8 @@
   --config combine_bank  the filter-bank combiner: eight odd-stacked 40 Msps rows into one 160 Msps capture, 255 taps, U = 4,
                       timed beside sb200_combine on the same eight channels and taps
   --config combine_rational  the rational-rate combiner: three 802.11b rows at 44 Msps into one 160 Msps capture, 1761 taps, U / D = 40 / 11
+  --config combine_arbitrary  the arbitrary-rate combiner: --config combine_rational's rows into 160 Msps through a 64-tap table, timed
+                      beside sb200_combine_rational; and the 2.4 GHz band into a 122.88 Msps capture from 44 and 40 Msps
   --config sim       the radio channel simulator: --frames links of config #2's 9 824-sample slots (T = R = 1, L = 16, +20 ppm, a carrier
                      offset, noise on), and a 2x2 case (T = R = 2, L = 16), device-resident
   --config 11n       config #4: 802.11n HT-MF 2x2 RX chain at MCS 8, 9, 10, PSDU 1500 B, 2 x 40 Msps, fixed 2x2 channel
@@ -689,6 +691,71 @@ def bench_combine_rational(args):
             "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs" % m})
     c.close()
 
+def bench_combine_arbitrary(args):
+    """The arbitrary-rate combiner into device-resident captures of --config combine's size, 64-tap tables (api.arbitrary_taps):
+    1. Three 802.11b rows at 44 Msps moved to -25 / 0 / +25 MHz of a 160 Msps capture (step 44 / 160), timed in the same process beside
+       sb200_combine_rational (U / D = 40 / 11, 1761 taps) on the same rows.  The two use different filters: a data point, not a
+       like-for-like comparison.
+    2. The 2.4 GHz band at 122.88 Msps, which no other call reaches from the transmitters' rates: 802.11b rows at -25 and +25 MHz from
+       44 Msps, then the OFDM row at 0 Hz from 40 Msps added onto them, two calls per step.
+    Work per output sample and row: 2 ntaps integer multiply-adds of the filter + 4 of the rotation + 2 of the gain; HBM traffic 4 B written
+    (plus 4 B read with accumulate) per output sample + 4 B read per row sample."""
+    import wideband_inputs as W, combine_arbitrary_model as CA, combine_rational_model as CR, arbitrary_model as A
+    from sora_b200 import api
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    n_out = args.frames * 9824 * 4; P = 20000
+    name, plim, clk = _card(); sms = torch.cuda.get_device_properties(dev).multi_processor_count
+    imad_peak = sms * 64 * clk * 1e6 if clk else None                    # int32 IMAD: 64 per SM per clock on sm_90
+    def calls(fs, plan):
+        """plan: [(centres, row rate, passband)], one call each, the later ones added onto the earlier -> (step function, [(channels, step,
+        taps, rows, n_in)], output)"""
+        y = torch.empty((n_out, 2), dtype=torch.int16, device=dev); out = []
+        for fcs, fr, fp in plan:
+            ch = [(W.phase_inc(f, fs), 0, 4096) for f in fcs]; step = api.arbitrary_step(fr, fs); taps = api.arbitrary_taps(fr, fs, 64, fp)
+            n_in = (n_out * step >> 32) + 64; n_in += (-n_in) % 4
+            out.append((ch, step, taps, torch.randint(-8000, 8000, (len(ch), n_in, 2), dtype=torch.int16, device=dev), n_in))
+        def step_fn():
+            for i, (ch, step, taps, x, n_in) in enumerate(out):
+                eng.combine_arbitrary_raw(x.data_ptr(), n_in, n_in, ch, 0, step, taps, y.data_ptr(), n_out, accumulate=i > 0, stream=st.cuda_stream)
+        step_fn(); torch.cuda.synchronize()
+        m = min(((P - 64) << 32) // step for _, step, _, _, _ in out)    # outputs that a prefix of P row samples determines
+        want = None
+        for ch, step, taps, x, _ in out: want = CA.combine_arbitrary_window(x[:, :P].cpu().numpy(), ch, 0, step, taps, 0, m, want)
+        assert (want == y[:m].cpu().numpy()).all(), "arbitrary-rate combiner output differs from the stated arithmetic"
+        return step_fn, out, m
+    def emit(what, ms, out, m, workload, extra):
+        sec = ms * 1e-3
+        work = n_out * sum(len(ch) * (2.0 * taps.shape[1] + 6.0) for ch, _, taps, _, _ in out)
+        hbm = n_out * 4.0 * (2 * len(out) - 1) + sum(4.0 * len(ch) * n_in for ch, _, _, _, n_in in out)
+        f_hbm = hbm / sec / 1e9 / peaks(); f_int = (work / sec / imad_peak) if imad_peak else None
+        c.emit(dict({"metric": "%s output Msamples/s (COMPLEX16 out)" % what, "value": c.world * n_out / sec / 1e6, "unit": "Msamples/s", "ms_per_step": ms, "n_gpus": c.world,
+                     "config": {"workload": workload, "output_samples_per_step_per_gpu": n_out},
+                     "hbm": {"achieved": hbm / sec / 1e9, "peak": peaks(), "unit": "GB/s", "frac": f_hbm,
+                             "note": "per call 4 B written (+ 4 B read with accumulate) per output sample + 4 B read per row sample"},
+                     "int_mad": {"achieved": work / sec / 1e9, "peak": imad_peak / 1e9 if imad_peak else None, "unit": "G multiply-adds/s", "frac": f_int,
+                                 "note": "K (2 ntaps + 6) per output sample and call; peak = SMs x 64 x max SM clock"},
+                     "bound": None if f_int is None else ("integer" if f_int > f_hbm else "hbm"),
+                     "card": name, "power_limit_w": plim, "max_sm_clock_mhz": clk,
+                     "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs" % m}, **extra))
+    arb160, out160, m160 = calls(160e6, [((-25e6, 0.0, 25e6), 44e6, 9e6)])
+    U, D = 40, 11; rtaps = W.lowpass(1761, 12e6 / 1.76e9, gain=40); ch, _, _, x, n_in = out160[0]
+    n_r = -(-D * n_out // U); yr = torch.empty((n_out, 2), dtype=torch.int16, device=dev)
+    def rat(): eng.combine_raw(x.data_ptr(), n_in, n_r, ch, U, rtaps, yr.data_ptr(), st.cuda_stream, decim=D, n_out=n_out)
+    rat(); torch.cuda.synchronize()
+    mr = 20000
+    assert (CR.combine_rational_window(x[:, :D * mr // U + len(rtaps)].cpu().numpy(), ch, U, D, rtaps, 0, mr) == yr[:mr].cpu().numpy()).all(), "combiner output differs from the stated arithmetic"
+    ms_arb = c.timed(arb160, args.steps); ms_rat = c.timed(rat, args.steps)
+    emit("arbitrary-rate combiner (sb200_combine_arbitrary), 44 -> 160 Msps", ms_arb, out160, m160,
+         "3 x 802.11b rows at 44 Msps -> 160 Msps capture, channels at -25/0/+25 MHz, 64-tap table, step 44 / 160, device-resident",
+         {"rational_ms_per_step": ms_rat, "rational_msamples_per_s": c.world * n_out / (ms_rat * 1e-3) / 1e6,
+          "rational_note": "sb200_combine_rational on the same rows and channels: U / D = 40 / 11, 1761 taps (a different filter)"})
+    del out160, yr, x
+    arb122, out122, m122 = calls(122.88e6, [((-25e6, 25e6), 44e6, 9e6), ((0.0,), 40e6, 8.3e6)])
+    ms = c.timed(arb122, args.steps)
+    emit("arbitrary-rate combiner (sb200_combine_arbitrary), 44 and 40 -> 122.88 Msps", ms, out122, m122,
+         "122.88 Msps capture of the 2.4 GHz band: 802.11b rows at -25/+25 MHz from 44 Msps, then OFDM at 0 Hz from 40 Msps added onto them (two calls), 64-tap tables, device-resident", {})
+    c.close()
+
 def bench_sim(args):
     """The radio channel simulator on device-resident links of config #2's slot length (9 824 samples at 40 Msps): T = R = 1 with 16 taps,
     and T = R = 2 with 16 taps per pair, every link at +20 ppm with a carrier offset and noise.  Integer work per output sample, from the
@@ -728,7 +795,7 @@ def bench_sim(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_bank", "channelize_rational", "channelize_arbitrary", "combine", "combine_bank", "combine_rational", "sim"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_bank", "channelize_rational", "channelize_arbitrary", "combine", "combine_bank", "combine_rational", "combine_arbitrary", "sim"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
@@ -736,4 +803,4 @@ if __name__ == "__main__":
                     "a pair other than 40/11 takes a generic low-pass of 45 taps per branch at 0.55 of the row's Nyquist")
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_bank": bench_channelize_bank, "channelize_rational": bench_channelize_rational, "channelize_arbitrary": bench_channelize_arbitrary, "combine": bench_combine, "combine_bank": bench_combine_bank, "combine_rational": bench_combine_rational, "sim": bench_sim}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_bank": bench_channelize_bank, "channelize_rational": bench_channelize_rational, "channelize_arbitrary": bench_channelize_arbitrary, "combine": bench_combine, "combine_bank": bench_combine_bank, "combine_rational": bench_combine_rational, "combine_arbitrary": bench_combine_arbitrary, "sim": bench_sim}[a.config](a)

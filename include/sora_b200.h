@@ -305,6 +305,39 @@ int sb200_combine_rational(sb200_handle* h, const int16_t* rows, uint64_t row_st
                            const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t n_out_samples, uint32_t accumulate,
                            void* cuda_stream);
 
+/* Arbitrary-rate combiner, the transmit counterpart of sb200_channelize_arbitrary: sb200_combine_rational with the rate changed by any
+ * factor between x16 and /4, so that rows at 40 and 44 Msps go into captures at rates derived from 30.72 MHz (30.72, 61.44, 122.88 Msps;
+ * 44 -> 122.88 Msps is U / D = 768 / 275); an extension without a reference counterpart.  K = nchannels rows x_k[0 .. n_in) of COMPLEX16,
+ * row k at rows + k * row_stride samples, x_k = 0 outside [0, n_in).  For channel k = {phase_inc, phase0, gain}, c = floor((ntaps - 1) / 2)
+ * and every output n in 0 .. n_out = n_out_samples:
+ *     t_n     = tau0 + n * step                                 exact, uint64 (Q32.32 row samples); the limits keep it below 2^63
+ *     t'      = t_n + 2^23,  i = t' >> 32,  p = (t' >> 24) & 255
+ *     u_k(n)  = sat16((sum_{j < ntaps} H[p][j] * x_k(i - c + j) + 2^13) >> 14)      int32, re and im independently
+ *     v_k(n)  = u_k(n) rotated UP by NCO[(phase0 + (uint32)n * phase_inc) >> 20]   sb200_combine's rotation, n = absolute output index
+ *     a(n)    = accumulate ? out[n] as it was before the call : 0
+ *     y(n)    = sat16(a(n) + sum_k ((v_k(n) * gain_k + 2^11) >> 12))               int32, re and im independently
+ *     H[p][j] = taps[p * ntaps + j]                              256 rows of ntaps Q14 taps; row p is the fractional delay p / 256
+ * Stage u is sb200_channelize_arbitrary's resampler with the same table; stages v and y are sb200_combine_rational's rotation, gain, sum
+ * and accumulate.  Rows at fs_rows into a capture at fs_capture take step = round(2^32 fs_rows / fs_capture) (api.arbitrary_step) and the
+ * table api.arbitrary_taps(fs_rows, fs_capture, ntaps, passband), whose default stop band puts the cut at the rows' Nyquist rate, which
+ * removes the images.  There is one (tau0, step) and one table per call: rows of two rates (802.11b at 44 Msps beside OFDM at 40 Msps) take
+ * two calls into one buffer, the second with accumulate = 1, as with sb200_combine_rational.  Pins:
+ *   - with one row, channel {0, 0, 4096} and accumulate = 0 the call is sb200_channelize_arbitrary's channel (0, 0) with the same tau0,
+ *     step, table and n_out, bit for bit: NCO[0] = (16384, 0), and the rotation and the Q12 gain of 4096 are then exact identities (so with
+ *     sb200_channel_sim's H and 8 taps it is also that call's stage 1);
+ *   - with row 0 the unit impulse at j = c, step = 2^32 and tau0 = d 2^32 it is a pure shift, y[n] = x[n + d];
+ *   - a row sent with (phase_inc, phase0), tau0 = 0 and step s comes back from sb200_channelize_arbitrary with the same pair and step
+ *     ~ 2^64 / s; not bit for bit (two filters, two roundings), but the receivers decode it.
+ * rows and out may be host, page-locked or device pointers (device: 16-byte aligned, and the call is then asynchronous on the stream; a
+ * host out is uploaded first when accumulate = 1); channels and taps are host arrays.  Limits (SB200_E_INVALID, nothing launched):
+ * 1 <= nchannels <= 16, 1 <= ntaps <= 64, 2^28 <= step <= 2^34, tau0 + (n_out - 1) step < 2^63, for every row p sum_j |H[p][j]| <= 65535
+ * (the accumulator cannot wrap), gain <= 65535, row_stride >= n_in, a multiple of 4 and <= 2^40, n_in <= 2^40, n_out <= 2^40, accumulate
+ * 0 or 1.  n_out = 0 launches nothing and n_in = 0 means all-zero rows.  One kernel launch; sb200_last_kernel_ms times it. */
+int sb200_combine_arbitrary(sb200_handle* h, const int16_t* rows, uint64_t row_stride_samples, uint64_t n_in_samples,
+                            const sb200_duc_channel* channels, uint32_t nchannels, uint64_t tau0, uint64_t step,
+                            const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t n_out_samples,
+                            uint32_t accumulate, void* cuda_stream);
+
 /* Radio channel simulator: nlinks independent links, each from T = ntx input rows x_t[0 .. n_in) to R = nrx output rows y_r[0 .. n_out) of
  * COMPLEX16 through a sampling-clock offset, multipath, a carrier offset and seeded noise, in the manner of GNU Radio's channel_model; an
  * extension without a reference counterpart.  Row t of link l is at x + l * in_link_stride + t * in_row_stride samples, row r of y at

@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_channelize_bank", "sb200_channelize_arbitrary", "sb200_combine", "sb200_combine_rational", "sb200_combine_bank", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_channelize_bank", "sb200_channelize_arbitrary", "sb200_combine", "sb200_combine_rational", "sb200_combine_bank", "sb200_combine_arbitrary", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -79,7 +79,8 @@ def bank_centres(nchannels, fs_hz, odd=False):
     return np.where(np.arange(nchannels) >= nchannels // 2, f - fs_hz, f)
 
 def arbitrary_step(fs_in, fs_out):
-    """Input samples per output of sb200_channelize_arbitrary for a capture at fs_in brought to fs_out: round(2^32 fs_in / fs_out) (Q32.32)."""
+    """Input samples per output of sb200_channelize_arbitrary for a capture at fs_in brought to fs_out, and of sb200_combine_arbitrary for
+    rows at fs_in put into a capture at fs_out: round(2^32 fs_in / fs_out) (Q32.32)."""
     return int(round(2 ** 32 * fs_in / fs_out))
 
 def _kaiser_beta(atten_db):
@@ -89,7 +90,8 @@ def _kaiser_beta(atten_db):
     return 0.0
 
 def arbitrary_taps(fs_in, fs_out, ntaps, passband_hz, stopband_hz=None, beta=None):
-    """The 256 x ntaps Q14 table H of sb200_channelize_arbitrary for a capture at fs_in brought to fs_out: a low-pass Kaiser-windowed sinc
+    """The 256 x ntaps Q14 table H of sb200_channelize_arbitrary for a capture at fs_in brought to fs_out, and of sb200_combine_arbitrary
+    for rows at fs_in put into a capture at fs_out (there the default stop band puts the cut at the rows' Nyquist rate): a low-pass Kaiser-windowed sinc
     cut halfway between passband_hz and stopband_hz, row p evaluated at d = k - c - p / 256 (c = (ntaps - 1) // 2), where the output at
     input time i + p / 256 meets input i - c + k.  stopband_hz defaults to min(fs_in, fs_out) - passband_hz, the lowest frequency that
     the rate change folds (decimation) or images (interpolation) into the passband; beta defaults to the Kaiser value for the attenuation
@@ -442,6 +444,29 @@ class Engine:
         M, n_in = rows.shape[:2]; x, stride = _rows4(M, n_in, rows)
         out = _out_samples(out, interp * n_in if n_out is None else n_out)
         self.combine_bank_raw(_ptr(x), stride, n_in, M, interp, taps, _ptr(out), len(out), odd=odd, accumulate=accumulate)
+        return out
+
+    def combine_arbitrary_raw(self, rows_ptr, row_stride, n_in, channels, tau0, step, taps, out_ptr, n_out, accumulate=False, stream=0):
+        """Pointer-level sb200_combine_arbitrary: rows_ptr / out_ptr host or device addresses, row k at rows_ptr + 4 k row_stride bytes;
+        channels a list of (phase_inc, phase0, gain); taps int16 Q14 [256, ntaps]; n_out outputs."""
+        ch = (DucChannel * max(len(channels), 1))(*[DucChannel(int(a) % 2 ** 32, int(b) % 2 ** 32, int(g)) for a, b, g in channels])
+        t = np.ascontiguousarray(taps, dtype=np.int16)
+        if t.ndim != 2 or t.shape[0] != 256: raise ValueError("taps must be int16 [256, ntaps]")
+        self._check(self._lib.sb200_combine_arbitrary(self._h, C.c_void_p(rows_ptr), C.c_uint64(row_stride), C.c_uint64(n_in), C.cast(ch, C.c_void_p),
+                                                      C.c_uint32(len(channels)), C.c_uint64(tau0), C.c_uint64(step), C.c_void_p(_ptr(t)), C.c_uint32(t.shape[1]),
+                                                      C.c_void_p(out_ptr), C.c_uint64(n_out), C.c_uint32(int(bool(accumulate))), C.c_void_p(stream)),
+                    "sb200_combine_arbitrary")
+
+    def combine_arbitrary(self, rows, channels, step, taps, tau0=0, n_out=None, accumulate=False, out=None):
+        """Arbitrary-rate combiner: int16 [K, n_in, 2] rows and K channels (phase_inc, phase0, gain Q12) -> int16 [n_out, 2], every row
+        resampled at row times (tau0 + n step) / 2^32 through the 256-phase Q14 table taps (int16 [256, ntaps], arbitrary_taps), moved to
+        its centre, scaled and summed; step = arbitrary_step(fs_rows, fs_capture).  n_out defaults to the outputs whose time lies inside
+        the rows, tau0 + n step < n_in 2^32.  accumulate adds the sum onto `out` (int16 [n_out, 2], updated in place and returned) with one
+        saturation."""
+        rows = np.asarray(rows, dtype=np.int16).reshape(len(channels), -1, 2); n_in = rows.shape[1]; x, stride = _rows4(len(channels), n_in, rows)
+        if n_out is None: n_out = max(0, -(-((n_in << 32) - tau0) // step))
+        out = _out_samples(out, n_out)
+        self.combine_arbitrary_raw(_ptr(x), stride, n_in, channels, tau0, step, taps, _ptr(out), n_out, accumulate=accumulate)
         return out
 
     def channel_sim_raw(self, x_ptr, in_link_stride, in_row_stride, ntx, n_in, links, taps, ntaps, nlinks, seed, y_ptr, out_link_stride, out_row_stride,

@@ -167,8 +167,8 @@ struct sb200_handle {
     uint32_t cb_smem_set = 0;                          // bit J (+ 16 for RAT): k_combine<J, RAT> may use SB_CB_SMEM (SB_CBR_SMEM_MAX) bytes of dynamic shared memory on this device
     DevBuf simtab, simlink, simtap;                    // channel simulator: its table (sim_kernels.cuh, built on first use), staged links and taps
     uint32_t sim_smem_set = 0;                         // bit J: k_channel_sim<J> may use its largest dynamic shared memory on this device
-    DevBuf arbtab;                                     // sb200_channelize_arbitrary: the NCO table and the call's H, staged per call (arb_kernels.cuh)
-    uint32_t arb_smem_set = 0;                         // bit 0: k_channelize_arbitrary may use SB_ARB_SMEM_MAX bytes of dynamic shared memory on this device
+    DevBuf arbtab;                                     // sb200_channelize_arbitrary and sb200_combine_arbitrary: the NCO table and the call's H, staged per call (arb_kernels.cuh)
+    uint32_t arb_smem_set = 0;                         // bit 0: k_channelize_arbitrary may use SB_ARB_SMEM_MAX bytes of dynamic shared memory on this device; bit J: k_combine_arbitrary<J> its budget
     DevBuf vring;
     std::string err;
     int fail(int code, const char* what, cudaError_t e = cudaSuccess) {

@@ -1,6 +1,6 @@
 // sora_b200 — the wideband filters and the radio channel simulator: sb200_fir_decimate2, the channelizer and the combiner (fir_kernels.cuh),
-// the filter-bank channelizer and combiner (bank_kernels.cuh), the arbitrary-rate channelizer (arb_kernels.cuh), sb200_channel_sim
-// (sim_kernels.cuh).
+// the filter-bank channelizer and combiner (bank_kernels.cuh), the arbitrary-rate channelizer and combiner (arb_kernels.cuh),
+// sb200_channel_sim (sim_kernels.cuh).
 #include "handle.cuh"
 #include "fir_kernels.cuh"
 #include "bank_kernels.cuh"
@@ -220,9 +220,34 @@ extern "C" int sb200_channelize_bank(sb200_handle* h, const int16_t* iq, uint64_
     });
 }
 
+// The checks of both arbitrary-rate calls on their resampler: the step range, t_(n_out - 1) = tau0 + (n_out - 1) step below 2^63, and
+// the |tap| sum of every row of H.
+static int check_arbitrary(sb200_handle* h, uint64_t tau0, uint64_t step, const int16_t* taps, uint32_t ntaps, uint64_t n_out) {
+    if (step < SB_ARB_MINSTEP || step > SB_ARB_MAXSTEP) return h->fail(SB200_E_INVALID, "step must be within 2^28 .. 2^34");
+    if (n_out && (tau0 >> 63 || (n_out - 1) > ((1ull << 63) - 1 - tau0) / step)) return h->fail(SB200_E_INVALID, "tau0 + (n_out - 1) step must be below 2^63");
+    for (uint32_t p = 0; p < SB_ARB_ROWS; p++) {
+        const int rc = check_tap_sums(h, taps + (uint64_t)p * ntaps, ntaps, 1);     // every row of H
+        if (rc != SB200_OK) return rc;
+    }
+    return SB200_OK;
+}
+// The table of both arbitrary-rate kernels, staged per call into h->arbtab on `st`: the NCO (one device-to-device copy), then H packed in
+// tap pairs, row p at word p * arb_row_words(ntaps) with taps 2q (low half) and 2q + 1 (high half) in word q, so that one bulk copy per
+// CTA brings both in.  Calls on one handle run in order (CallScope), so a call never rewrites the table under another's kernel.
+static int upload_arbtab(sb200_handle* h, cudaStream_t st, const int16_t* taps, uint32_t ntaps) {
+    const uint32_t rs = arb_row_words(ntaps);
+    std::vector<uint32_t> H((size_t)SB_ARB_ROWS * rs, 0u);
+    for (uint32_t p = 0; p < SB_ARB_ROWS; p++)
+        for (uint32_t k = 0; k < ntaps; k++) H[p * rs + k / 2] |= (uint32_t)(uint16_t)taps[(uint64_t)p * ntaps + k] << (16 * (k & 1));
+    CK(h->arbtab.need((SB_CH_NCO + H.size()) * 4));
+    CK(cudaMemcpyAsync(h->arbtab.p, h->nco.p, SB_CH_NCO * 4, cudaMemcpyDeviceToDevice, st));
+    CK(cudaMemcpyAsync((uint32_t*)h->arbtab.p + SB_CH_NCO, H.data(), H.size() * 4, cudaMemcpyHostToDevice, st));
+    return SB200_OK;
+}
+
 // Arbitrary-rate channelizer (arb_kernels.cuh): every channel shifted by its NCO and resampled at input times (tau0 + m step) / 2^32
-// through the 256-phase table H; channel c in row c of `out`.  The table goes up per call behind the NCO (one device-to-device copy), so
-// that one bulk copy per CTA brings both in.  Channels split into groups as in channelize_launch.
+// through the 256-phase table H; channel c in row c of `out`.  The table goes up per call (upload_arbtab).  Channels split into groups as
+// in channelize_launch.
 extern "C" int sb200_channelize_arbitrary(sb200_handle* h, const int16_t* iq, uint64_t n_in, const sb200_ddc_channel* channels, uint32_t nchannels,
                                           uint64_t tau0, uint64_t step, const int16_t* taps, uint32_t ntaps, int16_t* out, uint64_t out_stride,
                                           uint64_t n_out, void* cuda_stream) {
@@ -230,12 +255,8 @@ extern "C" int sb200_channelize_arbitrary(sb200_handle* h, const int16_t* iq, ui
     if (!iq || !channels || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
     if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
     if (ntaps < 1 || ntaps > SB_ARB_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be 1 .. 64");
-    if (step < SB_ARB_MINSTEP || step > SB_ARB_MAXSTEP) return h->fail(SB200_E_INVALID, "step must be within 2^28 .. 2^34");
-    if (n_out && (tau0 >> 63 || (n_out - 1) > ((1ull << 63) - 1 - tau0) / step)) return h->fail(SB200_E_INVALID, "tau0 + (n_out - 1) step must be below 2^63");
-    for (uint32_t p = 0; p < SB_ARB_ROWS; p++) {
-        const int rc = check_tap_sums(h, taps + (uint64_t)p * ntaps, ntaps, 1);     // every row of H
-        if (rc != SB200_OK) return rc;
-    }
+    const int crc = check_arbitrary(h, tau0, step, taps, ntaps, n_out);
+    if (crc != SB200_OK) return crc;
     if (n_in > (1ull << 40)) return h->fail(SB200_E_INVALID, "n_in_samples must be at most 2^40");
     if (out_stride < n_out || (out_stride & 3u) || out_stride > (1ull << 40))
         return h->fail(SB200_E_INVALID, "out_stride must be at least n_out, at most 2^40 and a multiple of 4");
@@ -249,12 +270,8 @@ extern "C" int sb200_channelize_arbitrary(sb200_handle* h, const int16_t* iq, ui
             rot |= channels[i].phase_inc != 0u || (channels[i].phase0 >> 20) != 0u;
         }
         a.rs = arb_row_words(ntaps);
-        std::vector<uint32_t> H((size_t)SB_ARB_ROWS * a.rs, 0u);      // row p: taps 2q (low half) and 2q + 1 (high half) in word q
-        for (uint32_t p = 0; p < SB_ARB_ROWS; p++)
-            for (uint32_t k = 0; k < ntaps; k++) H[p * a.rs + k / 2] |= (uint32_t)(uint16_t)taps[(uint64_t)p * ntaps + k] << (16 * (k & 1));
-        CK(h->arbtab.need((SB_CH_NCO + H.size()) * 4));
-        CK(cudaMemcpyAsync(h->arbtab.p, h->nco.p, SB_CH_NCO * 4, cudaMemcpyDeviceToDevice, st));
-        CK(cudaMemcpyAsync((uint32_t*)h->arbtab.p + SB_CH_NCO, H.data(), H.size() * 4, cudaMemcpyHostToDevice, st));
+        const int trc = upload_arbtab(h, st, taps, ntaps);
+        if (trc != SB200_OK) return trc;
         a.x = d_in; a.n_in = n_in; a.tab = (const uint32_t*)h->arbtab.p;
         a.tau0 = tau0; a.step = step; a.ntaps = ntaps; a.win = arb_win(step, ntaps); a.nco_words = rot ? SB_CH_NCO : 0u;
         a.y = d_out; a.stride = d_stride; a.n_out = n_out;
@@ -270,8 +287,9 @@ extern "C" int sb200_channelize_arbitrary(sb200_handle* h, const int16_t* iq, ui
     });
 }
 
-// The grid of k_combine<J, true> and k_combine_bank<M>, which take tile x + gx y of `tiles`.  A tile holds at least 16 outputs (32 W J
-// per phase of k_combine, U 1024 / M of the bank), so n_out <= 2^40 gives at most 2^36 tiles: gy = ceil(tiles / (2^31 - 1)) <= 33 and
+// The grid of k_combine<J, true>, k_combine_bank<M> and k_combine_arbitrary<J>, which take tile x + gx y of `tiles`.  A tile holds at
+// least 16 outputs (32 W J per phase of k_combine, U 1024 / M of the bank, 256 J of the arbitrary-rate combiner), so n_out <= 2^40 gives
+// at most 2^36 tiles: gy = ceil(tiles / (2^31 - 1)) <= 33 and
 // gx = ceil(tiles / gy) < 2^31 stay within the grid limits.
 static dim3 tile_grid(uint64_t tiles) {
     const uint64_t gy = (tiles + 0x7FFFFFFEull) / 0x7FFFFFFFull, gx = (tiles + gy - 1) / gy;
@@ -399,6 +417,56 @@ extern "C" int sb200_combine_bank(sb200_handle* h, const int16_t* rows, uint64_t
                                                                                            d_out, n_out, accumulate);
         });
         return SB200_OK;
+    });
+}
+
+// One launch of k_combine_arbitrary<J> (arb_kernels.cuh) on tile_grid's grid of tiles of 256 J outputs, between ev0 and the caller's
+// finish_call.  Bit J of arb_smem_set (bit 0 is k_channelize_arbitrary's).
+template <int J>
+static int combine_arbitrary_launch_j(sb200_handle* h, cudaStream_t st, ArbCbArgs& a) {
+    constexpr uint32_t TM = SB_FIR_THREADS * J;
+    CK(smem_once(h->arb_smem_set, 1u << J, k_combine_arbitrary<J>, J == 1 ? SB_ARB_CB_SMEM_MAX : SB_CBR_SMEM));
+    a.win = arb_win(a.step, a.ntaps, TM);
+    CK(cudaEventRecord(h->ev0, st));
+    k_combine_arbitrary<J><<<tile_grid((a.n_out + TM - 1) / TM), SB_FIR_THREADS, arb_combine_smem(a.ch.n, a.step, a.ntaps, a.nco_words != 0, TM), st>>>(a);
+    return SB200_OK;
+}
+
+// Arbitrary-rate combiner (arb_kernels.cuh): every row resampled at row times (tau0 + n step) / 2^32 through the 256-phase table H, shifted
+// up by its NCO, scaled and summed into n_out outputs (added onto out's samples when `accumulate`) in one launch.  Tiles of 1024, 512 or 256
+// outputs: the largest whose shared memory fits SB_CBR_SMEM (256 fits SB_ARB_CB_SMEM_MAX at every limit).  The table goes up per call
+// (upload_arbtab), residency and staging are combine_run's.
+extern "C" int sb200_combine_arbitrary(sb200_handle* h, const int16_t* rows, uint64_t row_stride, uint64_t n_in, const sb200_duc_channel* channels,
+                                       uint32_t nchannels, uint64_t tau0, uint64_t step, const int16_t* taps, uint32_t ntaps, int16_t* out,
+                                       uint64_t n_out, uint32_t accumulate, void* cuda_stream) {
+    if (!h) return SB200_E_INVALID;
+    if (!rows || !channels || !taps || !out) return h->fail(SB200_E_INVALID, "null argument");
+    if (nchannels < 1 || nchannels > SB_CH_MAXCH) return h->fail(SB200_E_INVALID, "nchannels must be 1 .. 16");
+    if (ntaps < 1 || ntaps > SB_ARB_MAXTAPS) return h->fail(SB200_E_INVALID, "ntaps must be 1 .. 64");
+    int rc = check_arbitrary(h, tau0, step, taps, ntaps, n_out);
+    if (rc != SB200_OK) return rc;
+    if (accumulate > 1u) return h->fail(SB200_E_INVALID, "accumulate must be 0 or 1");
+    for (uint32_t i = 0; i < nchannels; i++)
+        if (channels[i].gain > 65535u) return h->fail(SB200_E_INVALID, "gain must be at most 65535");
+    if ((rc = check_in_rows(h, row_stride, n_in, n_out)) != SB200_OK) return rc;
+    if (n_out == 0) return SB200_OK;
+    return combine_run(h, rows, row_stride, n_in, nchannels, out, n_out, accumulate, cuda_stream,
+                       [&](cudaStream_t st, const uint32_t* d_in, uint64_t d_stride, uint32_t* d_out) {
+        ArbCbArgs a; memset(&a, 0, sizeof a);
+        a.ch.n = nchannels;
+        bool rot = false;
+        for (uint32_t i = 0; i < nchannels; i++) {
+            a.ch.inc[i] = channels[i].phase_inc; a.ch.phase0[i] = channels[i].phase0; a.ch.gain[i] = channels[i].gain;
+            rot |= channels[i].phase_inc != 0u || (channels[i].phase0 >> 20) != 0u;
+        }
+        const int trc = upload_arbtab(h, st, taps, ntaps);
+        if (trc != SB200_OK) return trc;
+        a.x = d_in; a.stride = d_stride; a.n_in = n_in; a.tab = (const uint32_t*)h->arbtab.p;
+        a.tau0 = tau0; a.step = step; a.ntaps = ntaps; a.rs = arb_row_words(ntaps); a.nco_words = rot ? SB_CH_NCO : 0u;
+        a.y = d_out; a.n_out = n_out; a.accumulate = accumulate;
+        if (arb_combine_smem(nchannels, step, ntaps, rot, 4 * SB_FIR_THREADS) <= SB_CBR_SMEM) return combine_arbitrary_launch_j<4>(h, st, a);
+        if (arb_combine_smem(nchannels, step, ntaps, rot, 2 * SB_FIR_THREADS) <= SB_CBR_SMEM) return combine_arbitrary_launch_j<2>(h, st, a);
+        return combine_arbitrary_launch_j<1>(h, st, a);
     });
 }
 
