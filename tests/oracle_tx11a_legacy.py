@@ -6,6 +6,9 @@
 - `up160_numpy` / `up3_numpy` are a second, scalar reading of the same code: every output is at most two rounded Q15 products of
   neighbouring inputs, summed with a 16-bit wrap.
 - `ref_up160` / `ref_up3` drive the reference's own upsampler body where oracle/build_ref_tx11a44.sh could compile it (oracle/_ref).
+- `ref_modulate`, `ref_frame_mod_raw`, `ref_ack` drive the reference's own BB11ATxFrameMod / BB11AModulateACK as a whole, where
+  oracle/build_ref_tx11a_legacy.sh could compile them (oracle/_ref/libtx11a_legacy_ref.so), with `ref_preamble`, `ref_set_pad` and the
+  debug tap `ref_debug`.
 """
 import ctypes as C, os, subprocess, zlib
 import numpy as np
@@ -145,3 +148,93 @@ def ref_up160(x160, in_place_tail=True, behind=None):
 def ref_up3(x4):
     x = np.ascontiguousarray(x4, dtype=np.int16); o = np.zeros((4, 2), np.int16)
     _ref().ref_upsample44_3(oracle_py._p(x), oracle_py._p(o)); return o
+
+
+# ---- the reference's own transmitter, compiled from atx_*.c by oracle/build_ref_tx11a_legacy.sh -------------------------------------------
+REF_TX_SO = os.path.join(ROOT, "oracle", "_ref", "libtx11a_legacy_ref.so")
+REF_TX_COUNTERS = ("window_sat", "window_wrap", "pack_sat", "ifft_shl_loss", "ifft_sat")    # the order of ref_tx11a_legacy_debug's counts
+
+
+class MDL(C.Structure):
+    pass
+MDL._fields_ = [("Next", C.POINTER(MDL)), ("StartVa", C.c_void_p), ("ByteOffset", C.c_uint32), ("ByteCount", C.c_uint32)]
+
+
+def ref_tx_available():
+    return os.path.exists(REF_TX_SO)
+
+
+_REFTX = None
+def _reftx():
+    global _REFTX
+    if _REFTX is None:
+        L = C.CDLL(REF_TX_SO)
+        L.ref_tx11a_legacy_ctx_new.restype = C.c_void_p
+        L.ref_tx11a_legacy_ctx_free.argtypes = [C.c_void_p]
+        L.ref_tx11a_legacy_frame_mod.argtypes = [C.c_void_p, C.c_uint, C.c_uint, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32, C.POINTER(C.c_uint32)]
+        L.ref_tx11a_legacy_frame_mod.restype = C.c_int32
+        L.ref_tx11a_legacy_ack.argtypes = [C.c_uint, C.c_void_p, C.c_void_p]; L.ref_tx11a_legacy_ack.restype = C.c_uint32
+        for f in (L.ref_tx11a_legacy_preamble, L.ref_tx11a_legacy_set_pad, L.ref_tx11a_legacy_debug): f.argtypes = [C.c_void_p]; f.restype = None
+        _REFTX = L
+    return _REFTX
+
+
+class RefContext:
+    """One BB11A_TX_VECTOR of the compiled transmitter, kept across frames (as BB11ATxContextInit leaves it when made)."""
+    def __init__(self): self.p = _reftx().ref_tx11a_legacy_ctx_new()
+    def __del__(self):
+        if getattr(self, "p", None): _reftx().ref_tx11a_legacy_ctx_free(self.p); self.p = None
+
+
+def ref_frame_mod_raw(parts, fcs, rate_code, sample_rate, ctx=None, offsets=None, out=None):
+    """BB11ATxFrameMod compiled from the reference: the MPDU in MDLs over `parts` (uint8 arrays; StartVa + ByteOffset = the part's first byte,
+    ByteOffset = offsets[i]), FCS = Reserved1.  out: uint8 buffer the transmitter writes (default: 0x55 bytes enough for LENGTH 4096).
+    Returns (HRESULT, out, SignalLength in bytes)."""
+    parts = [np.ascontiguousarray(p, dtype=np.uint8) for p in parts]
+    offsets = offsets or [0] * len(parts)
+    mdls = [MDL(None, C.c_void_p(p.ctypes.data - o if p.size else 0x1000), o, p.size) for p, o in zip(parts, offsets)]
+    for a, b in zip(mdls, mdls[1:]): a.Next = C.pointer(b)
+    if out is None: out = np.full(4 * padded_samples(4096, 6000, 44), 0x55, np.uint8)
+    sl = C.c_uint32(0)
+    hr = _reftx().ref_tx11a_legacy_frame_mod(ctx.p if ctx else None, rate_code, sample_rate, C.addressof(mdls[0]) if mdls else None,
+                                             C.c_uint32(fcs), out.ctypes.data, out.size, C.byref(sl))
+    return hr, out, sl.value
+
+
+def ref_modulate(psdu, rate_kbps, sample_rate=40, ctx=None):
+    """The compiled transmitter on MPDU + FCS (its last 4 bytes, sent as Reserved1): int8 [SignalLength / 2, 2], what `modulate(..,
+    append_crc=False)` returns."""
+    psdu = np.ascontiguousarray(psdu, dtype=np.uint8); assert psdu.size >= 4
+    hr, out, sl = ref_frame_mod_raw([psdu[:-4]], int.from_bytes(bytes(psdu[-4:]), "little"), CODE[rate_kbps], sample_rate, ctx)
+    assert hr == 0 and sl % 128 == 0, (hr, sl)
+    assert (out[sl:] == 0x55).all()
+    return out[:sl].view(np.int8).reshape(-1, 2)
+
+
+def ref_ack(ra, sample_rate):
+    """BB11AModulateACK compiled from the reference: (return value, uint8 buffer it wrote, pre-filled 0x55)."""
+    buf = np.full(2 * padded_samples(14, 6000, 44) + 256, 0x55, np.uint8)
+    off = (-buf.ctypes.data) % 16                                       # Copy_NT streams: 16-byte aligned
+    r = np.ascontiguousarray(ra, dtype=np.uint8)
+    n = _reftx().ref_tx11a_legacy_ack(sample_rate, r.ctypes.data, buf[off:].ctypes.data)
+    return n, buf[off:off + 2 * padded_samples(14, 6000, 44) + 128]
+
+
+def ref_preamble():
+    """The compiled PREAMBLE40_11A_LUT (lutst/preamble40_11a.c), int16 [640, 2]."""
+    o = np.zeros((640, 2), np.int16); _reftx().ref_tx11a_legacy_preamble(o.ctypes.data); return o
+
+
+def ref_set_pad(pad):
+    """The 8 samples the compiled transmitter reads behind PREAMBLE40_11A_LUT (int16 [8, 2]; zeros unless set)."""
+    p = np.ascontiguousarray(pad, dtype=np.int16); assert p.shape == (8, 2); _reftx().ref_tx11a_legacy_set_pad(p.ctypes.data)
+
+
+def ref_debug_reset():
+    _reftx().ref_tx11a_legacy_debug_reset()
+
+
+def ref_debug():
+    """The tap's lane counts since ref_debug_reset, as {name: lanes} (REF_TX_COUNTERS)."""
+    d = np.zeros(5, np.uint64); _reftx().ref_tx11a_legacy_debug(d.ctypes.data)
+    return dict(zip(REF_TX_COUNTERS, (int(x) for x in d)))

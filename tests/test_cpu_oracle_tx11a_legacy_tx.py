@@ -30,6 +30,16 @@ def test_40msps_reproduces_ofdm_bin_and_the_table_vectors():
         assert (O.modulate(body, kbps, 40)[:len(want)] == want).all(), kbps
 
 
+def test_44msps_reproduces_the_compiled_transmitter_vectors():
+    """tests/golden/legacy_tx44/: one frame per rate that the reference's own BB11ATxFrameMod, compiled from atx_*.c, made at 44 Msps
+    (make_legacy_tx44_vectors.py); the .bin is the MPDU + FCS as sent.  Padding included, sample for sample."""
+    for kbps in O.RATES:
+        psdu = np.fromfile(os.path.join(GOLD, "legacy_tx44", f"legacy_tx44_{kbps}.bin"), np.uint8)
+        want = np.fromfile(os.path.join(GOLD, "legacy_tx44", f"legacy_tx44_{kbps}.i8"), np.int8).reshape(-1, 2)
+        got = O.modulate(psdu, kbps, 44, append_crc=False)
+        assert got.shape == want.shape and (got == want).all(), kbps
+
+
 def _chunks():
     rng = np.random.default_rng(5)
     yield rng.integers(-32768, 32768, (164, 2)).astype(np.int16)                  # full range
