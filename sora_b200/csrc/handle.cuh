@@ -1,5 +1,5 @@
 // sora_b200 — what the host files of the C ABI (include/sora_b200.h) share: the handle, its device workspaces, the staging of a call's
-// arguments and results, and the bookkeeping of a call.  Private to the library: every .cu file here includes it.
+// arguments and results, and the bookkeeping of a call; what only the 802.11a pipeline uses is HostPipe's (rx11a.cu).  Private to the library.
 #pragma once
 #include "../../include/sora_b200.h"
 #include "tables.cuh"
@@ -104,8 +104,10 @@ struct Returns {
 
 using namespace sb;
 
-struct DecimPool;                                      // rx11a.cu: the host threads of option host_decimate
-void free_decim_pool(DecimPool* pool);                 // deletes the pool once its threads have joined
+struct HostPipe;                                       // rx11a.cu: the chunked pipeline of the 802.11a batch receiver
+int host_pipe_create(HostPipe** out);                 // SB200_E_CUDA without its streams or events; *out is set even then, for host_pipe_destroy
+void host_pipe_destroy(HostPipe* p);                  // joins the host threads, then frees the pinned slabs
+void host_pipe_forget_gather_cost(HostPipe* p);       // option host_decimate_mix: the next call measures the host gather anew
 
 #define SB200_LANE_MIN_DEFAULT 16384u                 // the lane kernel for launches of 16 384 .. 49 152 code blocks, the four-lane kernel outside
 #define SB200_LANE_MAX_DEFAULT 49152u                 // (tools/vit_crossover.py on an H100 SXM at 400 W: lane/four-lane time 1.46 at 8 192, 0.96 at 16 384, 0.85-0.93 up to 49 152, 1.03 at 65 536)
@@ -124,10 +126,8 @@ struct sb200_handle {
     uint64_t launches = 0;
     uint32_t chunk_frames_device = 0;
     uint32_t chunk_frames = 4096;                      // slots per pipeline chunk (0 = one chunk, everything on the caller's stream)
-    cudaStream_t s_copy = nullptr, s_front = nullptr;
-    cudaEvent_t ev_start = nullptr, ev_h2d[2] = {nullptr, nullptr}, ev_front[2] = {nullptr, nullptr};
+    HostPipe* pipe = nullptr;                          // streams, events, pinned slabs and host threads of the chunked 802.11a calls (rx11a.cu)
     DevBuf stage[2], iq40, off40, len40, dcbuf;
-    double gather_ms = 0.0;                            // host_decimate: time the host threads spent gathering during the last call (SB200_TRACE prints it)
     uint32_t ht_mcs_limit = 11;                        // first MCS the 802.11n HT-SIG parser refuses (PHY_11n.hpp:497); option "ht_mcs_limit"
     DevBuf soff, slen, spos, snev, sev;                // continuous-capture scout: current slot of every capture, position, event count, event list
     DevTablesTx X{}; DevBuf tabtx, txpay, txoff, txlen, txseed, txout, txns, txdesc, cca11n, ccaidx, tabtx11n, txout1, txpre; DevTablesTx11n XN{};   // 802.11a transmit tables (built on first use) and staging
@@ -137,18 +137,8 @@ struct sb200_handle {
     uint32_t front_stage = 1;                          // option: sample staging of k_front11a (0 direct loads, 1 register double buffer, 2 bulk async copy to shared memory)
     bool front_smem_set = false;                       // k_front11a<2> may use SB_FRONT_STAGE_SMEM bytes of dynamic shared memory on this device
     uint32_t host_decimate = 0;                        // option: host threads gathering the even samples of host-resident 40 Msps captures (0 = off)
-    DecimPool* pool = nullptr; void* hstage[4] = {nullptr, nullptr, nullptr, nullptr}; size_t hstage_cap = 0; cudaEvent_t ev_hfree[4] = {nullptr, nullptr, nullptr, nullptr};
-    // host_decimate_mix (default 1 = adaptive): per chunk, the decimating path either gathers on the host threads (half the bytes cross) or,
-    // when the copies already queued would run out before a gather could finish, sends the chunk as it is — the link and the host cores are
-    // two resources and the call keeps both busy.  0 = every chunk gathered; 2 = alternate (tests).
-    uint32_t host_mix = 1;
-    bool hstage_wc = false, hstage_is_wc = false;      // option host_stage_wc: pinned staging buffers of the decimating path allocated write-combined
-    std::vector<cudaEvent_t> ev_link; std::vector<uint64_t> link_bytes;     // one timed event per chunk copy of the current call, and its size
-    double link_bpms = 50e6;                           // estimate of the link rate, bytes per ms (largest rate seen between two consecutive copy ends)
-    double gather_ms_per_sample = 0.0;                 // running estimate of the host gather cost per 40 Msps sample (0 = not measured yet)
-    uint64_t last_h2d_bytes = 0, last_gathered_chunks = 0, last_chunks = 0;
-    std::vector<uint64_t> chunk_lo, chunk_hi; std::vector<int8_t> chunk_buf;   // per chunk of the current call: span in the capture, pinned buffer of a gathered chunk
-    DevBuf doff; std::vector<uint64_t> doffh;
+    uint32_t host_mix = 1;                             // option host_decimate_mix: which chunks the pipeline gathers (0 all, 1 adaptive, 2 the odd ones)
+    bool hstage_wc = false;                            // option host_stage_wc: pinned staging buffers of the decimating path allocated write-combined
     bool tab_immutable = false;                        // option slot_table_immutable: device-resident slot tables may be cached by address
     DevBuf slotchk;
     bool vl_defer = true;                              // option vl_defer_walk: the traceback spread over the step loop, one look-up per chunk (8-column blocks only)

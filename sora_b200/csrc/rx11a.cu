@@ -1,5 +1,5 @@
-// sora_b200 — 802.11a receive (rx11a_kernels.cuh): the batch pipeline (chunked over three streams for host-resident captures, with the
-// host threads of option host_decimate), the continuous-capture scout and the 44 Msps and stage-tap entry points.
+// sora_b200 — 802.11a receive (rx11a_kernels.cuh): the batch receiver, with HostPipe, the handle's pipeline of large calls (three streams,
+// the pinned slabs and host threads of option host_decimate), the continuous-capture scout and the 44 Msps and stage-tap entry points.
 #include "handle.cuh"
 #include "rx11a_kernels.cuh"
 #include <stdio.h>
@@ -57,13 +57,11 @@ __global__ void k_stream_advance(const FrameInfo* __restrict__ info, uint32_t n,
 
 } // namespace
 
-// ---- host-side TDownSample2 for host-resident captures ---------------------------------------------------------------------------------
-// The 802.11a graph keeps samples 0 and 2 of every 4 (samples.hpp:27-49): half of a 40 Msps capture is dropped on arrival.  With the option
-// "host_decimate" = T > 0 the chunked host-IQ path gathers the even samples of every slot of a chunk into pinned staging memory with T host
-// threads and sends only those over PCIe (half the bytes); the kernels then read the packed copy with stride 1 (sh = 0).  Results are
-// identical: the same samples reach the same arithmetic.
+// ---- the chunked pipeline of the batch receiver ----------------------------------------------------------------------------------------
+// The 802.11a graph keeps samples 0 and 2 of every 4 (samples.hpp:27-49).  With option "host_decimate" = T > 0, T host threads gather the
+// even samples of every slot of a host-resident chunk into pinned memory and only those cross PCIe (half the bytes); the kernels read the
+// packed copy with stride 1 (sh = 0), so the same samples reach the same arithmetic.
 namespace sb { void gather_even(const uint32_t* src, uint32_t n2, uint32_t* dst); }      // host_gather.cpp: dst[j] = src[2 j], streaming stores, SSE2 / AVX-512 chosen at run time
-static inline void decimate_slot(const uint32_t* src, uint32_t n2, uint32_t* dst) { sb::gather_even(src, n2, dst); }
 struct DecimPool {
     // n worker threads; submit() hands them one chunk and returns, wait() blocks until it is gathered: the caller queues the previous chunk's
     // copies and kernels in between, so the host cores never wait for the launch path (and the launch path never waits for them).
@@ -71,19 +69,15 @@ struct DecimPool {
     std::vector<std::thread> th; std::mutex m; std::condition_variable cv, cv_done;
     Job job{}; uint64_t gen = 0; int pending = 0; bool stop = false; int n = 0;
     std::chrono::steady_clock::time_point t_submit; double last_ms = 0.0;   // wall time from submit() to the last worker's end
-    static void part(const Job& j, int w, int n) {
-        const uint64_t cnt = j.f1 - j.f0; const uint32_t a = j.f0 + (uint32_t)(cnt * w / n), b = j.f0 + (uint32_t)(cnt * (w + 1) / n);
-        for (uint32_t f = a; f < b; f++) decimate_slot(j.iq + j.off[f], (j.len[f] + 1u) / 2u, j.dst + (j.doff[f] - j.doff[j.f0]));
-        _mm_sfence();                                   // streaming stores visible before the copy is queued
-    }
-    void start(int nthreads) {
-        shutdown(); n = nthreads < 1 ? 1 : nthreads; stop = false;
+    explicit DecimPool(int nthreads) : n(nthreads < 1 ? 1 : nthreads) {
         for (int w = 0; w < n; w++) th.emplace_back([this, w]() {
             uint64_t seen = 0;
             for (;;) {
                 Job j;
                 { std::unique_lock<std::mutex> l(m); cv.wait(l, [&] { return stop || gen != seen; }); if (stop) return; seen = gen; j = job; }
-                part(j, w, n);
+                const uint64_t cnt = j.f1 - j.f0; const uint32_t a = j.f0 + (uint32_t)(cnt * w / n), b = j.f0 + (uint32_t)(cnt * (w + 1) / n);   // this worker's slots
+                for (uint32_t f = a; f < b; f++) sb::gather_even(j.iq + j.off[f], (j.len[f] + 1u) / 2u, j.dst + (j.doff[f] - j.doff[j.f0]));
+                _mm_sfence();                           // streaming stores visible before the copy is queued
                 { std::lock_guard<std::mutex> l(m);
                   if (--pending == 0) { last_ms = std::chrono::duration<double, std::milli>(std::chrono::steady_clock::now() - t_submit).count(); cv_done.notify_all(); } }
             }
@@ -93,52 +87,233 @@ struct DecimPool {
         { std::lock_guard<std::mutex> l(m); job = j; gen++; pending = n; t_submit = std::chrono::steady_clock::now(); }
         cv.notify_all();
     }
-    double wait() { std::unique_lock<std::mutex> l(m); cv_done.wait(l, [&] { return pending == 0; }); return last_ms; }
-    void shutdown() {
+    double wait() { std::unique_lock<std::mutex> l(m); cv_done.wait(l, [&] { return pending == 0; }); return last_ms; }   // at once when nothing is in flight
+    ~DecimPool() {
         { std::lock_guard<std::mutex> l(m); stop = true; }
         cv.notify_all();
         for (auto& t : th) t.join();
-        th.clear(); n = 0;
     }
-    ~DecimPool() { shutdown(); }
 };
-void free_decim_pool(DecimPool* pool) { delete pool; }
 
-// Launch the decode kernels for frames [f0, f1) of a call.  `iq_base + off[f]` must address slot f.
-// sync + front end go to `sf`, the Viterbi launches to `sv` (sv waits for `front_done` when the streams differ).
-static int launch_chunk(sb200_handle* h, const uint32_t* iq_base, const uint64_t* d_off, const uint32_t* d_len, uint32_t f0, uint32_t f1,
-                        uint64_t soft_stride, uint64_t row, cudaStream_t sf, cudaStream_t sv, cudaEvent_t front_done, FrontTaps taps, bool timed, const int2* dc_init = nullptr, uint32_t chunk_idx = 0, uint32_t sh = 1, uint32_t lsh = 0) {
+// One call of the batch receiver as rx11a_run has laid it out (d_res: where k_pack_results writes the results, `res` itself when res_dev).
+struct Batch {
+    const int16_t* iq; bool iq_dev; const uint64_t* d_off; const uint32_t* d_len; uint32_t nframes; uint64_t soft_stride, row; FrontTaps taps;
+    cudaStream_t st; uint8_t* out_bytes; uint32_t out_stride; bool out_dev; sb200_frame_result* res; sb200_frame_result* d_res; bool res_dev;
+};
+// Where a launch finds the samples of slot f: from word base + off[f] on, every (1 << sh)-th word (sh = 1: a 40 Msps capture; 0: samples at
+// 20 Msps), len[f] of them counted at 40 Msps (lsh = 0) or at 20 Msps (lsh = 1).  The DC estimate of slot f starts from dc[f] (null: zero).
+struct Samples { const uint32_t* base; const uint64_t* off; uint32_t sh, lsh; const int2* dc; };
+
+// Launch the decode kernels for slots [f0, f1) of `bt`, chunk `part` of the call, with their samples where `x` says: sync + front end on
+// `sf`, the Viterbi on `sv` (sv waits for `front_done` when the streams differ); `timed` records evk[0..3].
+static int launch_chunk(sb200_handle* h, const Batch& bt, const Samples& x, uint32_t f0, uint32_t f1, uint32_t part, cudaStream_t sf, cudaStream_t sv, cudaEvent_t front_done, bool timed) {
     const uint32_t n = f1 - f0;
     FrameInfo* d_info = (FrameInfo*)h->info.p + f0;
-    uint8_t* d_soft = (uint8_t*)h->soft.p + (size_t)f0 * soft_stride;
-    uint8_t* d_out = (uint8_t*)h->out.p + (size_t)f0 * row;
+    uint8_t* d_soft = (uint8_t*)h->soft.p + (size_t)f0 * bt.soft_stride;
+    uint8_t* d_out = (uint8_t*)h->out.p + (size_t)f0 * bt.row;
     uint32_t* d_status = (uint32_t*)h->status.p + f0; uint32_t* d_crc = (uint32_t*)h->crc.p + f0;
     if (timed) CK(cudaEventRecord(h->evk[0], sf));
-    k_sync11a<<<(n + 127) / 128, 128, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->cca_thr, h->T, d_info, dc_init ? dc_init + f0 : nullptr, sh, lsh);
+    k_sync11a<<<(n + 127) / 128, 128, 0, sf>>>(x.base, x.off + f0, bt.d_len + f0, n, h->cca_thr, h->T, d_info, x.dc ? x.dc + f0 : nullptr, x.sh, x.lsh);
     if (timed) CK(cudaEventRecord(h->evk[1], sf));
     {   const dim3 g((n + SB_FRONT_SLOTS - 1) / SB_FRONT_SLOTS), b(32 * SB_FRONT_WARPS);
         if (h->front_stage == 2 && !h->front_smem_set) {
             CK(cudaFuncSetAttribute(k_front11a<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, SB_FRONT_STAGE_SMEM));
             h->front_smem_set = true;
         }
-        if (h->front_stage == 2) k_front11a<2><<<g, b, SB_FRONT_STAGE_SMEM, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh);
-        else if (h->front_stage == 1) k_front11a<1><<<g, b, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh);
-        else k_front11a<0><<<g, b, 0, sf>>>(iq_base, d_off + f0, d_len + f0, n, h->T, d_info, d_soft, soft_stride, h->inv_deint, taps, sh, lsh); }
+        const auto front = h->front_stage == 2 ? k_front11a<2> : h->front_stage == 1 ? k_front11a<1> : k_front11a<0>;
+        front<<<g, b, h->front_stage == 2 ? SB_FRONT_STAGE_SMEM : 0, sf>>>(x.base, x.off + f0, bt.d_len + f0, n, h->T, d_info, d_soft, bt.soft_stride, h->inv_deint, bt.taps, x.sh, x.lsh); }
     if (timed) CK(cudaEventRecord(h->evk[2], sf));
     if (sv != sf) { CK(cudaEventRecord(front_done, sf)); CK(cudaStreamWaitEvent(sv, front_done, 0)); }
     h->launches += 2;
     VitJob job{}; job.depth = 256; job.lookahead = 24; job.raw = 0;
     static const int rates[3] = {CR_34, CR_12, CR_23};
-    const int rc = viterbi_stage(h, n, sv, d_soft, soft_stride, d_info, job, d_out, row, d_status, d_crc, rates, 3, f0, chunk_idx, h->vq_pad_smem);
+    const int rc = viterbi_stage(h, n, sv, d_soft, bt.soft_stride, d_info, job, d_out, bt.row, d_status, d_crc, rates, 3, f0, part, h->vq_pad_smem);
     if (rc != SB200_OK) return rc;
     if (timed) CK(cudaEventRecord(h->evk[3], sv));
     return SB200_OK;
 }
 
-// shared body of sb200_rx11a_batch / sb200_rx11a_taps.
-// Large calls are cut into chunks of h->chunk_frames slots and pipelined over three streams: host->device copy of chunk
-// k+1 (copy stream) | carrier sense + OFDM front end of chunk k+1 (front stream) | Viterbi of chunk k (caller's stream).
-// The front end is latency bound and the Viterbi integer-issue bound, so they overlap well on the same SMs.
+// The pipeline of large calls, one per handle: host->device copy of chunk k+1 (s_copy) | carrier sense + OFDM front end of chunk k+1
+// (s_front) | Viterbi of chunk k (the caller's stream); the front end is latency bound and the Viterbi integer-issue bound, so they overlap
+// well on the same SMs.  A host-resident chunk reaches one of two device buffers as its span of the capture or, with host_decimate, as the
+// even samples of its slots, which the host threads gather into one of four pinned slabs while earlier chunks are in flight.  Mix 0 of
+// host_decimate_mix gathers every chunk, 2 the odd ones, 1 (default) those whose gather would not outlast the copies already queued on the
+// link, so that the link and the host cores are both kept busy.  Device-resident captures take the same loop without the copies.
+struct HostPipe {
+    cudaStream_t s_copy = nullptr, s_front = nullptr;
+    cudaEvent_t ev_start = nullptr, ev_h2d[2] = {nullptr, nullptr}, ev_front[2] = {nullptr, nullptr};
+    DecimPool* pool = nullptr;                         // the host threads, started by the first call that gathers
+    void* hstage[4] = {nullptr, nullptr, nullptr, nullptr}; size_t hstage_cap = 0; cudaEvent_t ev_hfree[4] = {nullptr, nullptr, nullptr, nullptr};
+    bool hstage_is_wc = false;                         // the pinned slabs were allocated write-combined (option host_stage_wc)
+    std::vector<cudaEvent_t> ev_link; std::vector<uint64_t> link_bytes;     // one timed event per chunk copy of the current call, and its size
+    double link_bpms = 50e6;                           // estimate of the link rate, bytes per ms (largest rate seen between two consecutive copy ends)
+    double gather_ms_per_sample = 0.0;                 // running estimate of the host gather cost per 40 Msps sample (0 = not measured yet)
+    std::vector<uint64_t> chunk_lo, chunk_hi; std::vector<int8_t> chunk_buf;   // per chunk of the current call: span in the capture, pinned slab of a gathered chunk
+    DevBuf doff; std::vector<uint64_t> doffh;          // offset of every slot in the gathered copy of the call, on the device and on the host
+    uint64_t last_h2d_bytes = 0, last_gathered_chunks = 0, last_chunks = 0;   // the last host-IQ call (sb200_last_transfer)
+    ~HostPipe() {
+        delete pool;                                    // the host threads have joined before the slabs they write go
+        for (int i = 0; i < 4; i++) { if (hstage[i]) cudaFreeHost(hstage[i]); if (ev_hfree[i]) cudaEventDestroy(ev_hfree[i]); }
+        for (cudaEvent_t e : ev_link) cudaEventDestroy(e);
+        for (cudaEvent_t e : {ev_start, ev_h2d[0], ev_h2d[1], ev_front[0], ev_front[1]}) if (e) cudaEventDestroy(e);
+        for (cudaStream_t s : {s_copy, s_front}) if (s) cudaStreamDestroy(s);
+    }
+    int run(sb200_handle* h, const Batch& bt, uint32_t chunk);
+};
+
+int host_pipe_create(HostPipe** out) {
+    HostPipe* p = *out = new (std::nothrow) HostPipe();
+    if (!p) return SB200_E_NOMEM;
+    for (cudaStream_t* s : {&p->s_copy, &p->s_front}) if (cudaStreamCreateWithFlags(s, cudaStreamNonBlocking) != cudaSuccess) return SB200_E_CUDA;
+    for (cudaEvent_t* e : {&p->ev_start, &p->ev_h2d[0], &p->ev_h2d[1], &p->ev_front[0], &p->ev_front[1], &p->ev_hfree[0], &p->ev_hfree[1], &p->ev_hfree[2], &p->ev_hfree[3]})
+        if (cudaEventCreateWithFlags(e, cudaEventDisableTiming) != cudaSuccess) return SB200_E_CUDA;
+    return SB200_OK;
+}
+void host_pipe_destroy(HostPipe* p) { delete p; }
+void host_pipe_forget_gather_cost(HostPipe* p) { p->gather_ms_per_sample = 0.0; }
+extern "C" int sb200_last_transfer(const sb200_handle* h, uint64_t* h2d_bytes, uint32_t* chunks, uint32_t* chunks_gathered) {
+    if (!h) return SB200_E_INVALID;
+    if (h2d_bytes) *h2d_bytes = h->pipe->last_h2d_bytes;
+    if (chunks) *chunks = (uint32_t)h->pipe->last_chunks;
+    if (chunks_gathered) *chunks_gathered = (uint32_t)h->pipe->last_gathered_chunks;
+    return SB200_OK;
+}
+
+// One call in chunks of `chunk` slots.  Host IQ is sized first: the span [lo, hi) of every chunk that may travel as it is, the slot offsets
+// in the gathered copy, and the staging for the largest chunk.
+int HostPipe::run(sb200_handle* h, const Batch& bt, uint32_t chunk) {
+    const std::vector<uint64_t>& offh = h->offh; const std::vector<uint32_t>& lenh = h->lenh;
+    const uint32_t nframes = bt.nframes, nchunks = (nframes + chunk - 1) / chunk;
+    const bool host = !bt.iq_dev, dec = host && h->host_decimate > 0;
+    const uint32_t mix = dec ? h->host_mix : 0u;
+    const bool out_host = bt.out_bytes && bt.out_stride && !bt.out_dev;     // the bytes go back chunk by chunk
+    const size_t w = bt.out_stride < bt.row ? bt.out_stride : bt.row;
+    if (host) {
+        if (dec) {
+            doffh.resize((size_t)nframes + 1); doffh[0] = 0;
+            for (uint32_t i = 0; i < nframes; i++) doffh[i + 1] = doffh[i] + (lenh[i] + 1u) / 2u;
+        }
+        chunk_lo.assign(nchunks, 0); chunk_hi.assign(nchunks, 0); chunk_buf.assign(nchunks, -1);     // -1: sent as it is
+        uint64_t stage_samples = 0, hstage_samples = 0;
+        for (uint32_t c = 0, f0 = 0; c < nchunks; c++, f0 += chunk) {
+            const uint32_t f1 = f0 + chunk < nframes ? f0 + chunk : nframes;
+            if (dec && doffh[f1] - doffh[f0] > hstage_samples) hstage_samples = doffh[f1] - doffh[f0];
+            if (dec && !mix) continue;                  // every chunk is gathered
+            uint64_t lo = ~0ull, hi = 0;
+            for (uint32_t i = f0; i < f1; i++) { if (offh[i] < lo) lo = offh[i]; if (offh[i] + lenh[i] > hi) hi = offh[i] + lenh[i]; }
+            chunk_lo[c] = lo; chunk_hi[c] = hi;
+            if (hi - lo > stage_samples) stage_samples = hi - lo;
+        }
+        if (hstage_samples > stage_samples) stage_samples = hstage_samples;
+        CK(h->stage[0].need(stage_samples * 4ull + 16)); CK(h->stage[1].need(stage_samples * 4ull + 16));
+        if (dec) {
+            if (!pool || pool->n != (int)h->host_decimate) { delete pool; pool = new (std::nothrow) DecimPool((int)h->host_decimate); if (!pool) return h->fail(SB200_E_NOMEM, "host thread pool"); }
+            if (hstage_cap < hstage_samples * 4ull || h->hstage_wc != hstage_is_wc) {
+                hstage_cap = 0;
+                for (int i = 0; i < 4; i++) { CK(cudaEventSynchronize(ev_hfree[i])); if (hstage[i]) cudaFreeHost(hstage[i]); hstage[i] = nullptr; }   // no copy out of a slab still queued
+                const size_t want_b = hstage_samples * 4ull + hstage_samples / 2 + 256;
+                // the staging buffers are written once by the host threads (streaming stores) and read only by the copy engine: write-combined
+                // memory (option host_stage_wc) is not snooped on its way over PCIe
+                for (int i = 0; i < 4; i++) CK(cudaHostAlloc(&hstage[i], want_b, h->hstage_wc ? cudaHostAllocWriteCombined : cudaHostAllocDefault));
+                hstage_cap = want_b; hstage_is_wc = h->hstage_wc;
+            }
+            CK(doff.need(nframes * 8ull)); CK(cudaMemcpyAsync(doff.p, doffh.data(), nframes * 8ull, cudaMemcpyHostToDevice, bt.st));
+        }
+        while (ev_link.size() < nchunks) { cudaEvent_t e; CK(cudaEventCreate(&e)); ev_link.push_back(e); }
+        link_bytes.assign(nchunks, 0);
+    }
+    CK(cudaEventRecord(ev_start, bt.st));
+    CK(cudaStreamWaitEvent(s_copy, ev_start, 0)); CK(cudaStreamWaitEvent(s_front, ev_start, 0));
+    uint32_t k = 0, gsub = 0, link_head = 0;          // chunk index, chunks handed to the host threads, first chunk whose copy may still be on the wire
+    uint64_t h2d_bytes = 0;
+    double gather_ms = 0.0;                            // time the host threads spent gathering (SB200_TRACE prints it)
+    struct InFlight { DecimPool* p; ~InFlight() { if (p) p->wait(); } } inflight{pool};   // no return while the host threads still read the caller's capture
+    // Decide how chunk c travels and, if it is to be gathered, hand it to the host threads now: the caller then queues the previous
+    // chunk's copies and kernels while they work.  `ahead` = bytes of the chunk that is about to be queued in front of it.
+    auto plan = [&](const uint32_t c, const uint64_t ahead) -> int {
+        const uint32_t f0 = c * chunk, f1 = f0 + chunk < nframes ? f0 + chunk : nframes;
+        bool gather = dec;
+        if (dec && mix == 2u) gather = (c & 1u) != 0u;
+        else if (dec && mix) {
+            // bytes still queued on the link: copies whose end event has not fired.  Two consecutive ends also give the link rate.
+            uint64_t pend = ahead;
+            for (uint32_t i = link_head; i + 1 < c; i++) {              // chunks 0 .. c-2 are queued; c-1 is `ahead`
+                const cudaError_t q = cudaEventQuery(ev_link[i]);
+                if (q == cudaSuccess) {
+                    if (i == link_head) {
+                        float ms = 0.f;
+                        if (i > 0 && cudaEventElapsedTime(&ms, ev_link[i - 1], ev_link[i]) == cudaSuccess && ms > 0.f) {
+                            const double r = (double)link_bytes[i] / ms;
+                            link_bpms = r > link_bpms ? r : 0.95 * link_bpms + 0.05 * r;   // a gap before the copy only lowers r
+                        }
+                        link_head++;
+                    }
+                } else if (q == cudaErrorNotReady) { (void)cudaGetLastError(); pend += link_bytes[i]; }
+                else return h->fail(SB200_E_CUDA, "cudaEventQuery", q);
+            }
+            const double pend_ms = (double)pend / link_bpms;
+            const double gather_est = gather_ms_per_sample * (double)(chunk_hi[c] - chunk_lo[c]);
+            // a gather whose copy would reach the link after it has run dry costs link time: send the chunk as it is instead.
+            // Not measured yet: the first chunk goes as it is (the link is idle anyway), the second is gathered and gives the estimate
+            gather = gather_ms_per_sample > 0.0 ? pend_ms >= gather_est : c != 0u;
+        }
+        if (!gather) return SB200_OK;
+        const int hb = (int)(gsub % 4u);
+        // pinned buffer hb is free once its last copy has crossed the link: the gathered chunk four back, or one of an earlier call that
+        // returned with its copies still queued (an event never recorded counts as complete)
+        CK(cudaEventSynchronize(ev_hfree[hb]));
+        pool->submit(DecimPool::Job{(const uint32_t*)bt.iq, offh.data(), lenh.data(), doffh.data(), f0, f1, (uint32_t*)hstage[hb]});
+        chunk_buf[c] = (int8_t)hb; gsub++;
+        return SB200_OK;
+    };
+    if (host) { const int rc = plan(0, 0); if (rc != SB200_OK) return rc; }
+    for (uint32_t f0 = 0; f0 < nframes; f0 += chunk, k++) {
+        const uint32_t f1 = f0 + chunk < nframes ? f0 + chunk : nframes; const int b = k & 1;
+        Samples x{(const uint32_t*)bt.iq, bt.d_off, 1u, 0u, nullptr};
+        if (host) {
+            const bool gathered = chunk_buf[k] >= 0;
+            if (gathered) {                              // the host threads finish this chunk; its cost per sample feeds the next decisions
+                const double gms = pool->wait();
+                gather_ms += gms;
+                const double per = gms / (double)(2u * (doffh[f1] - doffh[f0]) + 1u);
+                gather_ms_per_sample = gather_ms_per_sample > 0.0 ? 0.75 * gather_ms_per_sample + 0.25 * per : per;
+            }
+            link_bytes[k] = gathered ? (doffh[f1] - doffh[f0]) * 4ull : (chunk_hi[k] - chunk_lo[k]) * 4ull;
+            if (k + 1 < nchunks) { const int rc = plan(k + 1, link_bytes[k]); if (rc != SB200_OK) return rc; }
+            if (k >= 2) CK(cudaStreamWaitEvent(s_copy, ev_front[b], 0));            // device buffer b is free once chunk k-2's front end has read it
+            if (gathered) {
+                CK(cudaMemcpyAsync(h->stage[b].p, hstage[chunk_buf[k]], link_bytes[k], cudaMemcpyHostToDevice, s_copy));
+                CK(cudaEventRecord(ev_hfree[chunk_buf[k]], s_copy));
+                x = Samples{(const uint32_t*)h->stage[b].p - doffh[f0], (const uint64_t*)doff.p, 0u, 0u, nullptr};
+            } else {
+                CK(cudaMemcpyAsync(h->stage[b].p, (const uint32_t*)bt.iq + chunk_lo[k], link_bytes[k], cudaMemcpyHostToDevice, s_copy));
+                x.base = (const uint32_t*)h->stage[b].p - chunk_lo[k];
+            }
+            h2d_bytes += link_bytes[k];
+            CK(cudaEventRecord(ev_link[k], s_copy));
+            CK(cudaEventRecord(ev_h2d[b], s_copy));
+            CK(cudaStreamWaitEvent(s_front, ev_h2d[b], 0));
+        }
+        int rc = launch_chunk(h, bt, x, f0, f1, k, s_front, bt.st, ev_front[b], false);
+        if (rc != SB200_OK) return rc;
+        // results of this chunk go back while the next chunks are still coming in (PCIe is full duplex): only the last chunk's
+        // device-to-host copy is left exposed at the end of the call
+        const uint32_t n = f1 - f0;
+        k_pack_results<<<(n + 255) / 256, 256, 0, bt.st>>>((const FrameInfo*)h->info.p + f0, (const uint32_t*)h->status.p + f0, (const uint32_t*)h->crc.p + f0, n, bt.d_res + f0);
+        if (out_host) CK(cudaMemcpy2DAsync(bt.out_bytes + (size_t)f0 * bt.out_stride, bt.out_stride, (const uint8_t*)h->out.p + (size_t)f0 * bt.row, bt.row, w, n, cudaMemcpyDeviceToHost, bt.st));
+        if (!bt.res_dev) CK(cudaMemcpyAsync(bt.res + f0, bt.d_res + f0, n * sizeof(sb200_frame_result), cudaMemcpyDeviceToHost, bt.st));
+    }
+    if (host) { last_h2d_bytes = h2d_bytes; last_gathered_chunks = gsub; last_chunks = k; }
+    if (dec && getenv("SB200_TRACE")) fprintf(stderr, "[sb200] rx11a host_decimate: %u chunks (%u gathered, %u sent as they are), host gather %.2f ms in total (%u threads), link estimate %.1f GB/s, %.1f MB copied\n", k, gsub, k - gsub, gather_ms, h->host_decimate, link_bpms / 1e6, h2d_bytes / 1e6);
+    Returns ret;                                        // what goes to the host was already queued chunk by chunk
+    if (bt.out_bytes && bt.out_stride && bt.out_dev) ret.bind2d(bt.out_bytes, bt.out_stride, h->out.p, bt.row, w, nframes);
+    const int rc = finish_call(h, bt.st, ret, 0, k);     // k launches of k_pack_results
+    if (rc == SB200_OK && (out_host || !bt.res_dev)) CK(cudaStreamSynchronize(bt.st));
+    return rc;
+}
+
+// shared body of sb200_rx11a_batch / sb200_rx11a_taps: the checks, the slot table and the workspaces, then one pass on the caller's stream
+// or, for a large call, the handle's pipeline.
 static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, const uint64_t* frame_off, const uint32_t* frame_len,
                      uint32_t nframes, uint8_t* out_bytes, uint32_t out_stride, sb200_frame_result* res, cudaStream_t st,
                      FrontTaps taps, uint8_t* soft_host, uint64_t soft_host_stride, const int2* dc_init = nullptr, bool no_chunk = false, bool rate20 = false) {
@@ -148,14 +323,11 @@ static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
     CallScope call(h, st); CK(call.begin()); call.reads(iq);
     // slot table: checked on every call (slot_table, sb200.cu); the chunked host-IQ path also needs it on the host
     const bool iq_dev = is_device_ptr(iq);
-    std::vector<uint64_t>& offh = h->offh; std::vector<uint32_t>& lenh = h->lenh;
     const uint64_t* d_off; const uint32_t* d_len; uint32_t max_len = 0; bool tab_on_host = false;
-    {
-        const bool may_chunk = !no_chunk && !rate20 && !iq_dev && h->chunk_frames != 0 && nframes > h->chunk_frames;
-        int rc = slot_table(h, frame_off, frame_len, nframes, iq_total, may_chunk, st, &d_off, &d_len, &max_len, &tab_on_host);
-        if (rc != SB200_OK) return rc;
-        if (rate20) { if (max_len > 0x7FFFFFFFu) return h->fail(SB200_E_INVALID, "slot too long"); max_len <<= 1; }   // slots counted in 20 Msps samples
-    }
+    const bool may_chunk = !no_chunk && !rate20 && !iq_dev && h->chunk_frames != 0 && nframes > h->chunk_frames;
+    int rc = slot_table(h, frame_off, frame_len, nframes, iq_total, may_chunk, st, &d_off, &d_len, &max_len, &tab_on_host);
+    if (rc != SB200_OK) return rc;
+    if (rate20) { if (max_len > 0x7FFFFFFFu) return h->fail(SB200_E_INVALID, "slot too long"); max_len <<= 1; }   // slots counted in 20 Msps samples
     // workspaces
     const uint64_t max_sym = (max_len / 2u) / 80u + 1u;
     const uint64_t soft_stride = ((max_sym * 288ull) + 15ull) & ~15ull;
@@ -170,173 +342,24 @@ static int rx11a_run(sb200_handle* h, const int16_t* iq, uint64_t iq_total, cons
     // the PCIe copy of chunk k+1 hides behind the kernels of chunk k.  chunk_frames_device lets a caller force it anyway.
     const uint32_t want = (no_chunk || rate20) ? 0u : iq_dev ? h->chunk_frames_device : h->chunk_frames;
     const uint32_t chunk = (want == 0 || tapping || nframes <= want || (!iq_dev && !tab_on_host)) ? nframes : want;
-    const bool pipelined = chunk < nframes;
     CK(h->vcnt.need(32ull * ((nframes + chunk - 1) / chunk)));
-    const bool res_dev_all = is_device_ptr(res), out_dev_all = out_bytes && is_device_ptr(out_bytes);
-    sb200_frame_result* d_res_all = res_dev_all ? res : (sb200_frame_result*)h->res.p;
+    const bool res_dev = is_device_ptr(res);
+    const Batch bt{iq, iq_dev, d_off, d_len, nframes, soft_stride, row, taps, st, out_bytes, out_stride, out_bytes && is_device_ptr(out_bytes),
+                   res, res_dev ? res : (sb200_frame_result*)h->res.p, res_dev};
     CK(cudaEventRecord(h->ev0, st));
-    if (!pipelined) {
-        const uint32_t* d_iq;
-        CK(to_device(h->iq, (const uint32_t*)iq, iq_dev, iq_total * 4ull, st, &d_iq));
-        if (!iq_dev) { h->last_h2d_bytes = iq_total * 4ull; h->last_gathered_chunks = 0; h->last_chunks = 1; }
-        int rc = launch_chunk(h, d_iq, d_off, d_len, 0, nframes, soft_stride, row, st, st, nullptr, taps, true, dc_init, 0, rate20 ? 0u : 1u, rate20 ? 1u : 0u);
-        if (rc != SB200_OK) return rc;
-    } else {
-        // host IQ: per-chunk sample range [lo, hi) staged through two device buffers; with host_decimate only the even samples of every slot
-        // travel, gathered by the host threads into one of four pinned buffers while earlier chunks are on the wire / in the kernels
-        const bool dec = !iq_dev && h->host_decimate > 0;
-        const uint32_t mix = dec ? h->host_mix : 0u;
-        const uint64_t* d_off_dec = nullptr; std::vector<uint64_t>& doffh = h->doffh;
-        uint64_t stage_samples = 0, hstage_samples = 0;
-        const uint32_t nchunks = (nframes + chunk - 1) / chunk;
-        if (!iq_dev) {
-            if (dec) {
-                doffh.resize((size_t)nframes + 1); doffh[0] = 0;
-                for (uint32_t i = 0; i < nframes; i++) doffh[i + 1] = doffh[i] + (lenh[i] + 1u) / 2u;
-            }
-            for (uint32_t f0 = 0; f0 < nframes; f0 += chunk) {
-                const uint32_t f1 = f0 + chunk < nframes ? f0 + chunk : nframes;
-                if (dec) { const uint64_t n = doffh[f1] - doffh[f0]; if (n > hstage_samples) hstage_samples = n; if (n > stage_samples) stage_samples = n; }
-                if (!dec || mix) {
-                    uint64_t lo = ~0ull, hi = 0;
-                    for (uint32_t i = f0; i < f1; i++) { if (offh[i] < lo) lo = offh[i]; if (offh[i] + lenh[i] > hi) hi = offh[i] + lenh[i]; }
-                    if (hi - lo > stage_samples) stage_samples = hi - lo;
-                }
-            }
-            CK(h->stage[0].need(stage_samples * 4ull + 16)); CK(h->stage[1].need(stage_samples * 4ull + 16));
-            if (dec) {
-                if (!h->pool || h->pool->n != (int)h->host_decimate) { delete h->pool; h->pool = new (std::nothrow) DecimPool(); if (!h->pool) return h->fail(SB200_E_NOMEM, "host thread pool"); h->pool->start((int)h->host_decimate); }
-                if (h->hstage_cap < hstage_samples * 4ull || h->hstage_wc != h->hstage_is_wc) {
-                    for (int i = 0; i < 4; i++) if (h->ev_hfree[i]) CK(cudaEventSynchronize(h->ev_hfree[i]));     // no copy out of a buffer still queued
-                    for (int i = 0; i < 4; i++) { if (h->hstage[i]) cudaFreeHost(h->hstage[i]); h->hstage[i] = nullptr; }
-                    h->hstage_cap = 0;
-                    const size_t want_b = hstage_samples * 4ull + hstage_samples / 2 + 256;
-                    // the staging buffers are written once by the host threads (streaming stores) and read only by the copy engine: write-combined
-                    // memory (option host_stage_wc) is not snooped on its way over PCIe
-                    for (int i = 0; i < 4; i++) CK(cudaHostAlloc(&h->hstage[i], want_b, h->hstage_wc ? cudaHostAllocWriteCombined : cudaHostAllocDefault));
-                    h->hstage_cap = want_b; h->hstage_is_wc = h->hstage_wc;
-                }
-                for (int i = 0; i < 4; i++) if (!h->ev_hfree[i]) CK(cudaEventCreateWithFlags(&h->ev_hfree[i], cudaEventDisableTiming));
-                CK(h->doff.need(nframes * 8ull)); CK(cudaMemcpyAsync(h->doff.p, doffh.data(), nframes * 8ull, cudaMemcpyHostToDevice, st));
-                d_off_dec = (const uint64_t*)h->doff.p;
-            }
-            while (h->ev_link.size() < nchunks) { cudaEvent_t e; CK(cudaEventCreate(&e)); h->ev_link.push_back(e); }
-            h->link_bytes.assign(nchunks, 0);
-        }
-        CK(cudaEventRecord(h->ev_start, st));
-        CK(cudaStreamWaitEvent(h->s_copy, h->ev_start, 0)); CK(cudaStreamWaitEvent(h->s_front, h->ev_start, 0));
-        uint32_t k = 0, gk = 0, gsub = 0, link_head = 0;  // chunk index, gathered chunks queued on the link / handed to the host threads, first chunk whose copy may still be on the wire
-        uint64_t h2d_bytes = 0;
-        std::vector<uint64_t>& clo = h->chunk_lo; std::vector<uint64_t>& chi = h->chunk_hi; std::vector<int8_t>& cbuf = h->chunk_buf;
-        if (!iq_dev) {
-            h->gather_ms = 0.0;
-            clo.assign(nchunks, 0); chi.assign(nchunks, 0); cbuf.assign(nchunks, -1);          // span of every chunk in the capture; pinned buffer of a gathered chunk (-1: sent as it is)
-            if (!dec || mix) for (uint32_t c = 0; c < nchunks; c++) {
-                const uint32_t f0 = c * chunk, f1 = f0 + chunk < nframes ? f0 + chunk : nframes; uint64_t lo = ~0ull, hi = 0;
-                for (uint32_t i = f0; i < f1; i++) { if (offh[i] < lo) lo = offh[i]; if (offh[i] + lenh[i] > hi) hi = offh[i] + lenh[i]; }
-                clo[c] = lo; chi[c] = hi;
-            }
-        }
-        struct InFlight { DecimPool* p = nullptr; bool on = false; ~InFlight() { if (p && on) p->wait(); } } inflight;   // no return while the host threads still read the caller's capture
-        inflight.p = h->pool;
-        // Decide how chunk c travels and, if it is to be gathered, hand it to the host threads now: the caller then queues the previous
-        // chunk's copies and kernels while they work.  `ahead` = bytes of the chunk that is about to be queued in front of it.
-        auto plan = [&](const uint32_t c, const uint64_t ahead) -> int {
-            const uint32_t f0 = c * chunk, f1 = f0 + chunk < nframes ? f0 + chunk : nframes;
-            bool gather = dec;
-            if (dec && mix == 2u) gather = (c & 1u) != 0u;
-            else if (dec && mix) {
-                // bytes still queued on the link: copies whose end event has not fired.  Two consecutive ends also give the link rate.
-                uint64_t pend = ahead;
-                for (uint32_t i = link_head; i + 1 < c; i++) {              // chunks 0 .. c-2 are queued; c-1 is `ahead`
-                    const cudaError_t q = cudaEventQuery(h->ev_link[i]);
-                    if (q == cudaSuccess) {
-                        if (i == link_head) {
-                            float ms = 0.f;
-                            if (i > 0 && cudaEventElapsedTime(&ms, h->ev_link[i - 1], h->ev_link[i]) == cudaSuccess && ms > 0.f) {
-                                const double r = (double)h->link_bytes[i] / ms;
-                                h->link_bpms = r > h->link_bpms ? r : 0.95 * h->link_bpms + 0.05 * r;   // a gap before the copy only lowers r
-                            }
-                            link_head++;
-                        }
-                    } else if (q == cudaErrorNotReady) { (void)cudaGetLastError(); pend += h->link_bytes[i]; }
-                    else return h->fail(SB200_E_CUDA, "cudaEventQuery", q);
-                }
-                const double pend_ms = (double)pend / h->link_bpms;
-                const double gather_est = h->gather_ms_per_sample * (double)(chi[c] - clo[c]);
-                // a gather whose copy would reach the link after it has run dry costs link time: send the chunk as it is instead.
-                // Not measured yet: the first chunk goes as it is (the link is idle anyway), the second is gathered and gives the estimate
-                gather = h->gather_ms_per_sample > 0.0 ? pend_ms >= gather_est : c != 0u;
-            }
-            if (!gather) return SB200_OK;
-            const int hb = (int)(gsub % 4u);
-            // pinned buffer hb is free once its last copy has crossed the link: the gathered chunk four back, or one of an earlier call that
-            // returned with its copies still queued (an event never recorded counts as complete)
-            CK(cudaEventSynchronize(h->ev_hfree[hb]));
-            DecimPool::Job j{(const uint32_t*)iq, offh.data(), lenh.data(), doffh.data(), f0, f1, (uint32_t*)h->hstage[hb]};
-            h->pool->submit(j); inflight.on = true;
-            cbuf[c] = (int8_t)hb; gsub++;
-            return SB200_OK;
-        };
-        if (!iq_dev) { const int rc = plan(0, 0); if (rc != SB200_OK) return rc; }
-        for (uint32_t f0 = 0; f0 < nframes; f0 += chunk, k++) {
-            const uint32_t f1 = f0 + chunk < nframes ? f0 + chunk : nframes; const int b = k & 1;
-            const uint32_t* base = (const uint32_t*)iq;
-            const uint64_t* d_off_k = d_off; uint32_t sh_k = 1u;
-            if (!iq_dev) {
-                const bool gathered = cbuf[k] >= 0;
-                if (gathered) {                              // the host threads finish this chunk; its cost per sample feeds the next decisions
-                    const double gms = h->pool->wait(); inflight.on = false;
-                    h->gather_ms += gms;
-                    const double per = gms / (double)(2u * (doffh[f1] - doffh[f0]) + 1u);
-                    h->gather_ms_per_sample = h->gather_ms_per_sample > 0.0 ? 0.75 * h->gather_ms_per_sample + 0.25 * per : per;
-                }
-                h->link_bytes[k] = gathered ? (doffh[f1] - doffh[f0]) * 4ull : (chi[k] - clo[k]) * 4ull;
-                if (k + 1 < nchunks) { const int rc = plan(k + 1, h->link_bytes[k]); if (rc != SB200_OK) return rc; }
-                if (k >= 2) CK(cudaStreamWaitEvent(h->s_copy, h->ev_front[b], 0));            // device buffer b is free once chunk k-2's front end has read it
-                if (gathered) {
-                    CK(cudaMemcpyAsync(h->stage[b].p, h->hstage[cbuf[k]], h->link_bytes[k], cudaMemcpyHostToDevice, h->s_copy));
-                    CK(cudaEventRecord(h->ev_hfree[cbuf[k]], h->s_copy));
-                    base = (const uint32_t*)h->stage[b].p - doffh[f0]; d_off_k = d_off_dec; sh_k = 0u; gk++;
-                } else {
-                    CK(cudaMemcpyAsync(h->stage[b].p, (const uint32_t*)iq + clo[k], h->link_bytes[k], cudaMemcpyHostToDevice, h->s_copy));
-                    base = (const uint32_t*)h->stage[b].p - clo[k];
-                }
-                h2d_bytes += h->link_bytes[k];
-                CK(cudaEventRecord(h->ev_link[k], h->s_copy));
-                CK(cudaEventRecord(h->ev_h2d[b], h->s_copy));
-                CK(cudaStreamWaitEvent(h->s_front, h->ev_h2d[b], 0));
-            }
-            int rc = launch_chunk(h, base, d_off_k, d_len, f0, f1, soft_stride, row, h->s_front, st, h->ev_front[b], taps, false, nullptr, k, sh_k);
-            if (rc != SB200_OK) return rc;
-            // results of this chunk go back while the next chunks are still coming in (PCIe is full duplex): only the last chunk's
-            // device-to-host copy is left exposed at the end of the call
-            const uint32_t n = f1 - f0;
-            k_pack_results<<<(n + 255) / 256, 256, 0, st>>>((const FrameInfo*)h->info.p + f0, (const uint32_t*)h->status.p + f0, (const uint32_t*)h->crc.p + f0, n, d_res_all + f0);
-            h->launches += 1;
-            if (out_bytes && out_stride && !out_dev_all) {
-                const size_t w = out_stride < row ? out_stride : row;
-                CK(cudaMemcpy2DAsync(out_bytes + (size_t)f0 * out_stride, out_stride, (const uint8_t*)h->out.p + (size_t)f0 * row, row, w, n, cudaMemcpyDeviceToHost, st));
-            }
-            if (!res_dev_all) CK(cudaMemcpyAsync(res + f0, d_res_all + f0, n * sizeof(sb200_frame_result), cudaMemcpyDeviceToHost, st));
-        }
-        if (!iq_dev) { h->last_h2d_bytes = h2d_bytes; h->last_gathered_chunks = gk; h->last_chunks = k; }
-        if (dec && getenv("SB200_TRACE")) fprintf(stderr, "[sb200] rx11a host_decimate: %u chunks (%u gathered, %u sent as they are), host gather %.2f ms in total (%u threads), link estimate %.1f GB/s, %.1f MB copied\n", k, gk, k - gk, h->gather_ms, h->host_decimate, h->link_bpms / 1e6, h2d_bytes / 1e6);
-        Returns none;                                   // everything that goes to the host was already queued per chunk
-        const int rc = finish_call(h, st, none, 0, 0);
-        if (rc != SB200_OK) return rc;
-        if (out_bytes && out_stride && out_dev_all) { const size_t w = out_stride < row ? out_stride : row; CK(cudaMemcpy2DAsync(out_bytes, out_stride, h->out.p, row, w, nframes, cudaMemcpyDeviceToDevice, st)); }
-        if ((out_bytes && out_stride && !out_dev_all) || !res_dev_all) CK(cudaStreamSynchronize(st));
-        return SB200_OK;
-    }
-    k_pack_results<<<(nframes + 255) / 256, 256, 0, st>>>((const FrameInfo*)h->info.p, (const uint32_t*)h->status.p, (const uint32_t*)h->crc.p, nframes, d_res_all);
-    h->launches += 1;
+    if (chunk < nframes) return h->pipe->run(h, bt, chunk);
+    const uint32_t* d_iq;
+    CK(to_device(h->iq, (const uint32_t*)iq, iq_dev, iq_total * 4ull, st, &d_iq));
+    if (!iq_dev) { h->pipe->last_h2d_bytes = iq_total * 4ull; h->pipe->last_gathered_chunks = 0; h->pipe->last_chunks = 1; }
+    rc = launch_chunk(h, bt, Samples{d_iq, d_off, rate20 ? 0u : 1u, rate20 ? 1u : 0u, dc_init}, 0, nframes, 0, st, st, nullptr, true);
+    if (rc != SB200_OK) return rc;
+    k_pack_results<<<(nframes + 255) / 256, 256, 0, st>>>((const FrameInfo*)h->info.p, (const uint32_t*)h->status.p, (const uint32_t*)h->crc.p, nframes, bt.d_res);
     CK(cudaEventRecord(h->evk[4], st));
     Returns ret;
     if (out_bytes && out_stride) ret.bind2d(out_bytes, out_stride, h->out.p, row, out_stride < row ? out_stride : row, nframes);
-    if (!res_dev_all) ret.copy(res, d_res_all, nframes * sizeof(sb200_frame_result));
+    if (!res_dev) ret.copy(res, bt.d_res, nframes * sizeof(sb200_frame_result));
     if (soft_host) ret.bind2d(soft_host, soft_host_stride, h->soft.p, soft_stride, soft_host_stride < soft_stride ? soft_host_stride : soft_stride, nframes);
-    return finish_call(h, st, ret, 4, 0);
+    return finish_call(h, st, ret, 4, 1);
 }
 
 // Many continuous captures at once.  Every pass decodes the next frame of every capture that still has samples (one slot per

@@ -58,9 +58,8 @@ extern "C" int sb200_create(int device, const sb200_cfg* cfg, sb200_handle** out
     int rc = upload_tables(h);
     if (rc == SB200_OK && (cudaEventCreate(&h->ev0) != cudaSuccess || cudaEventCreate(&h->ev1) != cudaSuccess)) rc = SB200_E_CUDA;
     for (int i = 0; i < 5 && rc == SB200_OK; i++) if (cudaEventCreate(&h->evk[i]) != cudaSuccess) rc = SB200_E_CUDA;
-    if (rc == SB200_OK && (cudaStreamCreateWithFlags(&h->s_copy, cudaStreamNonBlocking) != cudaSuccess || cudaStreamCreateWithFlags(&h->s_front, cudaStreamNonBlocking) != cudaSuccess)) rc = SB200_E_CUDA;
-    if (rc == SB200_OK && (cudaEventCreateWithFlags(&h->ev_start, cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&h->ev_done, cudaEventDisableTiming) != cudaSuccess)) rc = SB200_E_CUDA;
-    for (int i = 0; i < 2 && rc == SB200_OK; i++) if (cudaEventCreateWithFlags(&h->ev_h2d[i], cudaEventDisableTiming) != cudaSuccess || cudaEventCreateWithFlags(&h->ev_front[i], cudaEventDisableTiming) != cudaSuccess) rc = SB200_E_CUDA;
+    if (rc == SB200_OK && cudaEventCreateWithFlags(&h->ev_done, cudaEventDisableTiming) != cudaSuccess) rc = SB200_E_CUDA;
+    if (rc == SB200_OK) rc = host_pipe_create(&h->pipe);
     if (rc != SB200_OK) { sb200_destroy(h); return rc; }
     *out = h;
     return SB200_OK;
@@ -72,25 +71,13 @@ extern "C" void sb200_destroy(sb200_handle* h) {
     if (h->ev0) cudaEventDestroy(h->ev0);
     if (h->ev1) cudaEventDestroy(h->ev1);
     for (int i = 0; i < 5; i++) if (h->evk[i]) cudaEventDestroy(h->evk[i]);
-    if (h->ev_start) cudaEventDestroy(h->ev_start);
     if (h->ev_done) cudaEventDestroy(h->ev_done);
-    for (int i = 0; i < 2; i++) { if (h->ev_h2d[i]) cudaEventDestroy(h->ev_h2d[i]); if (h->ev_front[i]) cudaEventDestroy(h->ev_front[i]); }
-    for (cudaEvent_t e : h->ev_link) cudaEventDestroy(e);
-    free_decim_pool(h->pool); for (int i = 0; i < 4; i++) { if (h->hstage[i]) cudaFreeHost(h->hstage[i]); if (h->ev_hfree[i]) cudaEventDestroy(h->ev_hfree[i]); }
-    if (h->s_copy) cudaStreamDestroy(h->s_copy);
-    if (h->s_front) cudaStreamDestroy(h->s_front);
+    host_pipe_destroy(h->pipe);
     delete h;
 }
 extern "C" const char* sb200_last_error(const sb200_handle* h) { return h ? h->err.c_str() : "null handle"; }
 extern "C" uint64_t sb200_launch_count(const sb200_handle* h) { return h ? h->launches : 0; }
 extern "C" const char* sb200_last_viterbi_kernel(const sb200_handle* h) { return h ? h->last_vit : ""; }
-extern "C" int sb200_last_transfer(const sb200_handle* h, uint64_t* h2d_bytes, uint32_t* chunks, uint32_t* chunks_gathered) {
-    if (!h) return SB200_E_INVALID;
-    if (h2d_bytes) *h2d_bytes = h->last_h2d_bytes;
-    if (chunks) *chunks = (uint32_t)h->last_chunks;
-    if (chunks_gathered) *chunks_gathered = (uint32_t)h->last_gathered_chunks;
-    return SB200_OK;
-}
 extern "C" float sb200_last_kernel_ms(sb200_handle* h) {
     if (!h || !h->timed) return -1.f;
     float ms = -1.f;
@@ -239,7 +226,7 @@ extern "C" int sb200_set_option(sb200_handle* h, const char* name, uint64_t valu
     if (!strcmp(name, "viterbi_lane_min")) { h->lane_min = value > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)value; return SB200_OK; }
     if (!strcmp(name, "viterbi_lane_max")) { h->lane_max = value > 0xFFFFFFFFull ? 0xFFFFFFFFu : (uint32_t)value; return SB200_OK; }
     if (!strcmp(name, "host_stage_wc")) { h->hstage_wc = value != 0; return SB200_OK; }
-    if (!strcmp(name, "host_decimate_mix")) { if (value > 2) return h->fail(SB200_E_INVALID, "host_decimate_mix: 0, 1 or 2"); h->host_mix = (uint32_t)value; h->gather_ms_per_sample = 0.0; return SB200_OK; }
+    if (!strcmp(name, "host_decimate_mix")) { if (value > 2) return h->fail(SB200_E_INVALID, "host_decimate_mix: 0, 1 or 2"); h->host_mix = (uint32_t)value; host_pipe_forget_gather_cost(h->pipe); return SB200_OK; }
     if (!strcmp(name, "slot_table_immutable")) { h->tab_immutable = value != 0; h->tab_off = nullptr; return SB200_OK; }
     if (!strcmp(name, "ht_mcs_limit")) { if (value < 9 || value > 15) return h->fail(SB200_E_INVALID, "ht_mcs_limit is the first 802.11n MCS index refused: 9 .. 15 (11 = the reference's parser, 15 = MCS 8..14)"); h->ht_mcs_limit = (uint32_t)value; return SB200_OK; }
     return h->fail(SB200_E_INVALID, "unknown option");
