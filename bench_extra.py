@@ -22,6 +22,8 @@
   --config combine_rational  the rational-rate combiner: three 802.11b rows at 44 Msps into one 160 Msps capture, 1761 taps, U / D = 40 / 11
   --config combine_arbitrary  the arbitrary-rate combiner: --config combine_rational's rows into 160 Msps through a 64-tap table, timed
                       beside sb200_combine_rational; and the 2.4 GHz band into a 122.88 Msps capture from 44 and 40 Msps
+  --config spectrum  the spectrum meter: --config channelize's 160 Msps capture, FFT<1024> every 1024 samples, Hann, 64 frames per group,
+                     device-resident; also the power meter on the same capture (blocks of 4096)
   --config sim       the radio channel simulator: --frames links of config #2's 9 824-sample slots (T = R = 1, L = 16, +20 ppm, a carrier
                      offset, noise on), and a 2x2 case (T = R = 2, L = 16), device-resident
   --config 11n       config #4: 802.11n HT-MF 2x2 RX chain at MCS 8, 9, 10, PSDU 1500 B, 2 x 40 Msps, fixed 2x2 channel
@@ -473,6 +475,37 @@ def bench_channelize(args):
             "parity": "equal to the numpy model of the stated arithmetic on the first %d outputs of every channel" % m})
     c.close()
 
+def bench_spectrum(args):
+    """The spectrum meter on the device-resident 160 Msps capture of --config channelize: FFT<1024> every 1024 samples, Hann window, sums of
+    64 frames (a 0.41 ms display line per group).  HBM traffic: 4 B read per input sample + 8 N B per group written.  Then, in the same
+    process on the same capture, the power meter over blocks of 4096 (4 B read per sample)."""
+    import numpy as np
+    sys.path.insert(0, os.path.join(os.path.dirname(os.path.abspath(__file__)), "tests"))
+    import spectrum_model as SM
+    c = Ctx(); torch = c.torch; eng, dev, st = c.eng, c.dev, c.st
+    n = args.frames * 9824 * 4; N, hop, avg = 1024, 1024, 64
+    from sora_b200 import api
+    w = api.spectrum_window(N, "hann"); ng = api.spectrum_frames(n, N, hop) // avg
+    x = torch.randint(-20000, 20000, (n, 2), dtype=torch.int16, device=dev); y = torch.empty((ng, N), dtype=torch.int64, device=dev)
+    pb = 4096; yp = torch.empty((n // pb,), dtype=torch.int32, device=dev)
+    def step(): eng.spectrum_raw(x.data_ptr(), n, 1, n, N, hop, avg, w, y.data_ptr(), st.cuda_stream)
+    def pstep(): eng.power_meter_raw(x.data_ptr(), n, 1, n, pb, yp.data_ptr(), st.cuda_stream)
+    step(); pstep(); torch.cuda.synchronize()
+    G = 4; xs = x[:G * avg * N].cpu().numpy()
+    assert (SM.spectrum(xs, N, hop, avg, w)[0] == y[:G].cpu().numpy()).all(), "spectrum differs from the model of the stated arithmetic"
+    assert (SM.power_meter(xs, pb)[0] == yp[:G * avg * N // pb].cpu().numpy().view(np.uint32)).all(), "power meter differs from the model"
+    ms = c.timed(step, args.steps); pms = c.timed(pstep, args.steps)
+    hbm = n * 4.0 + ng * N * 8.0; phbm = n * 4.0 + (n // pb) * 4.0
+    name, plim, clk = _card()
+    c.emit({"metric": "spectrum meter input Msamples/s (COMPLEX16 in, FFT<1024>, Hann, avg 64)", "value": c.world * n / (ms * 1e-3) / 1e6, "unit": "Msamples/s",
+            "ms_per_step": ms, "n_gpus": c.world,
+            "config": {"workload": "160 Msps capture, N = 1024, hop 1024, Hann, avg 64, device-resident", "samples_per_step_per_gpu": n, "groups": ng},
+            "hbm": {"achieved": hbm / (ms * 1e-3) / 1e9, "peak": peaks(), "unit": "GB/s", "frac": hbm / (ms * 1e-3) / 1e9 / peaks(), "note": "4 B read per input sample + 8 N B per group"},
+            "power_meter": {"block_len": pb, "ms_per_step": pms, "Msamples_per_s": n / (pms * 1e-3) / 1e6, "hbm_GBps": phbm / (pms * 1e-3) / 1e9},
+            "card": name, "power_limit_w": plim, "max_sm_clock_mhz": clk,
+            "parity": "equal to tests/spectrum_model.py on the first %d groups and their power-meter blocks" % G})
+    c.close()
+
 def bench_channelize_bank(args):
     """The filter-bank channelizer on the device-resident 160 Msps capture of --config channelize: all eight odd-stacked channels
     (+-10 / +-30 / +-50 / +-70 MHz), 255 taps, D = 4; and, in the same process on the same capture, sb200_channelize on the same eight
@@ -795,7 +828,7 @@ def bench_sim(args):
 
 if __name__ == "__main__":
     ap = argparse.ArgumentParser()
-    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_bank", "channelize_rational", "channelize_arbitrary", "combine", "combine_bank", "combine_rational", "combine_arbitrary", "sim"], required=True)
+    ap.add_argument("--config", choices=["viterbi", "11b", "11n", "tx11a", "tx11b", "tx11n", "fir", "fir37", "tx11b_legacy", "tx11a_legacy", "channelize", "channelize_bank", "channelize_rational", "channelize_arbitrary", "combine", "combine_bank", "combine_rational", "combine_arbitrary", "spectrum", "sim"], required=True)
     ap.add_argument("--steps", type=int, default=5)
     ap.add_argument("--blocks", type=int, default=0, help="Viterbi code blocks per GPU (0 = BASELINE config #5: 1e9 coded bits in total over all GPUs)")
     ap.add_argument("--frames", type=int, default=32768)
@@ -803,4 +836,4 @@ if __name__ == "__main__":
                     "a pair other than 40/11 takes a generic low-pass of 45 taps per branch at 0.55 of the row's Nyquist")
     ap.add_argument("--mcs", default="8,9,10", help="802.11n MCS list for --config 11n (11..14 enable the engine option ht_mcs_limit = 15)")
     a = ap.parse_args()
-    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_bank": bench_channelize_bank, "channelize_rational": bench_channelize_rational, "channelize_arbitrary": bench_channelize_arbitrary, "combine": bench_combine, "combine_bank": bench_combine_bank, "combine_rational": bench_combine_rational, "combine_arbitrary": bench_combine_arbitrary, "sim": bench_sim}[a.config](a)
+    {"viterbi": bench_viterbi, "11b": bench_11b, "11n": bench_11n, "tx11a": bench_tx11a, "tx11b": bench_tx11b, "tx11n": bench_tx11n, "fir": bench_fir, "fir37": bench_fir37, "tx11b_legacy": bench_tx11b_legacy, "tx11a_legacy": bench_tx11a_legacy, "channelize": bench_channelize, "channelize_bank": bench_channelize_bank, "channelize_rational": bench_channelize_rational, "channelize_arbitrary": bench_channelize_arbitrary, "combine": bench_combine, "combine_bank": bench_combine_bank, "combine_rational": bench_combine_rational, "combine_arbitrary": bench_combine_arbitrary, "spectrum": bench_spectrum, "sim": bench_sim}[a.config](a)

@@ -370,6 +370,41 @@ int sb200_channel_sim(sb200_handle* h, const int16_t* x, uint64_t in_link_stride
                       const sb200_link* links, const int16_t* taps, uint32_t ntaps, uint32_t nlinks,
                       uint64_t seed, int16_t* y, uint64_t out_link_stride, uint64_t out_row_stride, uint32_t nrx, uint64_t n_out, void* cuda_stream);
 
+/* Spectrum meter: TSpecMeter<N> of the reference spectrum analyser (kernel/sdl/inc/sdlmeasure.hpp:66-121; kernel/sdl/exe/speanalyzer/
+ * specanalyzer.cpp feeds it through THanningWin<16>), with overlap, a window and averaging.  nrows rows of COMPLEX16, row r at
+ * iq + r * row_stride samples: a capture (nrows = 1) or the rows a channelizer wrote.  With N = fft_len, frame f of a row covers samples
+ * [f hop, f hop + N), nframes = n_in >= N ? (n_in - N) / hop + 1 : 0 (no partial frame is formed, as the pin queue would form none).  Per frame:
+ *     x'[n] = window ? (x[n] * w[n] + 2^14) >> 15 : x[n]            re and im independently, w Q15 in [0, 32767]
+ *     X     = FFT<N>(x')                                             exactly FFTSSEEx<N> and the bit-reversed read-out of FFT<N>
+ *             (core/inc/fft_r4dif.h:11-141): radix-4 stages FFTSSE<N'> with the input >> 2, saturating adds and subtracts, mul_j, mul_shift
+ *             by the twiddle (pmaddwd, >> 15, the wrapping pack; twiddles (trunc(32767 cos(2 pi j M / N')), trunc(-32767 sin(2 pi j M / N'))),
+ *             M = 1, 2, 3), down to FFTSSEEx<4> (input >> 2) or FFTSSEEx<8> (input >> 3) with their XOR (one's-complement) negations
+ *     P[k]  = re^2 + im^2                                            wrapping int32 (SquaredNorm = pmaddwd(x, x): -32768 twice is INT32_MIN)
+ *     P[0]  = 0
+ *     out[(r * ngroups + g) * N + k] = sum of P_f[k] over f in [g avg, (g + 1) avg)    int64, ngroups = nframes / avg
+ * Bins are in natural FFT order, as TSpecMeter emits them: bin k is at +k fs / N (k < N / 2) or (k - N) fs / N.  Trailing frames that do
+ * not fill a group are not used.  With window = NULL, hop = N and avg = 1 every output row is TSpecMeter<N>'s output row bit for bit.
+ * hop gives overlapped (Welch) frames, the window keeps a strong channel's leakage off a weak neighbour, and avg keeps the output small (at
+ * avg = 1 it is twice the size of the capture).  iq and out may be host, page-locked or device pointers (device: 16-byte aligned, and the
+ * call is then asynchronous on the stream); window is a host array.  Limits (SB200_E_INVALID, nothing launched): fft_len a power of two,
+ * 4 .. 32768; 1 <= hop <= 2^32; 1 <= avg <= 2^31; 1 <= nrows <= 64; row_stride >= n_in, a multiple of 4 and <= 2^40; n_in <= 2^40; window
+ * entries in [0, 32767].  ngroups = 0 launches nothing.  One kernel launch; sb200_last_kernel_ms times it. */
+int sb200_spectrum(sb200_handle* h, const int16_t* iq, uint64_t row_stride_samples, uint32_t nrows, uint64_t n_in_samples,
+                   uint32_t fft_len, uint64_t hop_samples, uint32_t avg, const int16_t* window, int64_t* out, void* cuda_stream);
+
+/* Power meter: TPowerMeter<N> of the reference spectrum analyser (sdlmeasure.hpp:9-63) over consecutive blocks of N = block_len samples of
+ * each row (rows as in sb200_spectrum): out[r * (n_in / N) + b] for block b = samples [b N, b N + N); a partial last block is not used.  As
+ * the reference computes it:
+ *     per 4-sample vector i < N / 4:   s = hadd(SquaredNorm(x[4i .. 4i + 3]))     wrapping int32, both steps
+ *                                      avg += (uint)((size_t)s / N)              s converted to 64 bits: a wrapped negative s divides as 2^64 + s
+ *     per tail sample (N % 4 != 0):    avg += (uint)((size_t)(re^2 + im^2) / N)   the same, one sample at a time
+ * with avg a uint (it wraps).  The speanalyzer graph puts TDCRemoveEx<4> (brick/inc/dc.hpp:45-85) before the meter; it subtracts
+ * CF_VecDC::direct_current, which no TDCEstimator in that graph ever updates, so it stays at its reset value and the brick changes nothing:
+ * this call leaves it out.  Pointers as in sb200_spectrum.  Limits (SB200_E_INVALID, nothing launched): 1 <= block_len <= 65536 and the row
+ * limits of sb200_spectrum.  n_in < block_len launches nothing.  One kernel launch; sb200_last_kernel_ms times it. */
+int sb200_power_meter(sb200_handle* h, const int16_t* iq, uint64_t row_stride_samples, uint32_t nrows, uint64_t n_in_samples,
+                      uint32_t block_len, uint32_t* out, void* cuda_stream);
+
 /* Same as sb200_rx11a_batch for captures at `sample_rate_mhz` = 20, 40 or 44.  20: the capture is already at the channel rate (slots counted in
  * 20 Msps samples; sample j stands where TDownSample2 would have put sample 2j of a 40 Msps capture).  44 Msps slots first pass the reference's 11:10 linear
  * resampler (TDownSample44_40 / Down44to40, Brick11/src/sampling.hpp:37-65, 44MTo40M.hpp:63-123; graph

@@ -23,7 +23,7 @@ RESULT11N_DTYPE = np.dtype([("status", "<u4"), ("mcs", "<u4"), ("length", "<u4")
 
 EXPORTS = ["sb200_create", "sb200_destroy", "sb200_last_error", "sb200_launch_count", "sb200_last_kernel_ms",
            "sb200_last_kernel_times", "sb200_set_option", "sb200_rx11a_batch", "sb200_rx11a_batch_ex", "sb200_rx11a_stream", "sb200_rx11a_streams", "sb200_rx11b_batch", "sb200_viterbi_k7", "sb200_rx11a_taps",
-           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_channelize_bank", "sb200_channelize_arbitrary", "sb200_combine", "sb200_combine_rational", "sb200_combine_bank", "sb200_combine_arbitrary", "sb200_channel_sim", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
+           "sb200_rx11n_batch", "sb200_rx11n_taps", "sb200_rxblocks_unpack", "sb200_tx11a_batch", "sb200_tx11b_batch", "sb200_rx11b_streams", "sb200_rx11n_streams", "sb200_tx11n_batch", "sb200_rxblocks_desc", "sb200_fir_decimate2", "sb200_channelize", "sb200_channelize_rational", "sb200_channelize_bank", "sb200_channelize_arbitrary", "sb200_combine", "sb200_combine_rational", "sb200_combine_bank", "sb200_combine_arbitrary", "sb200_channel_sim", "sb200_spectrum", "sb200_power_meter", "sb200_tx11b_fir37", "sb200_tx11b_legacy_batch", "sb200_tx11a_legacy_batch", "sb200_host_alloc", "sb200_host_free", "sb200_last_transfer", "sb200_last_viterbi_kernel"]
 
 class Sb200Error(RuntimeError):
     pass
@@ -153,6 +153,27 @@ def sim_taps(delays, gains, L):
     if np.abs(q).max() > 32767 or (np.abs(q).sum((1, 2, 3)) > 65535).any():
         raise ValueError("taps out of range: every |g| below 2 and every row's sum of |re| + |im| at most 65535 / 16384")
     return q.astype(np.int16)
+
+def spectrum_window(N, kind="hann"):
+    """Q15 window of N taps for Engine.spectrum: rint(32767 w[n]) of the periodic (DFT-even) window, n = 0 .. N - 1.
+    kind "hann":            w[n] = 0.5 - 0.5 cos(2 pi n / N)
+    kind "blackman-harris": w[n] = 0.35875 - 0.48829 cos(2 pi n / N) + 0.14128 cos(4 pi n / N) - 0.01168 cos(6 pi n / N)  (4 terms)"""
+    a = 2 * np.pi * np.arange(N) / N
+    if kind == "hann": w = 0.5 - 0.5 * np.cos(a)
+    elif kind in ("blackman-harris", "blackmanharris"): w = 0.35875 - 0.48829 * np.cos(a) + 0.14128 * np.cos(2 * a) - 0.01168 * np.cos(3 * a)
+    else: raise ValueError("kind must be 'hann' or 'blackman-harris'")
+    return np.clip(np.rint(32767 * w), 0, 32767).astype(np.int16)
+
+def spectrum_frames(n_in, N, hop=None):
+    """Frames of sb200_spectrum in a row of n_in samples: frame f covers [f hop, f hop + N); (n_in - N) // hop + 1 if n_in >= N, else 0."""
+    hop = N if hop is None else hop
+    return (n_in - N) // hop + 1 if n_in >= N else 0
+
+def fftshift_bins(spec, fs_hz=1.0):
+    """Display order of a spectrum (bins in natural FFT order along the last axis, bin k at k fs / N for k < N / 2 and (k - N) fs / N
+    above): (the bins in centred order, from -fs / 2 up, and their frequencies in Hz)."""
+    spec = np.asarray(spec); N = spec.shape[-1]
+    return np.fft.fftshift(spec, axes=-1), np.fft.fftshift(np.fft.fftfreq(N, 1.0 / fs_hz))
 
 _NDBPS_11A = {6000: 24, 9000: 36, 12000: 48, 18000: 72, 24000: 96, 36000: 144, 48000: 192, 54000: 216}   # 802.11a data bits per OFDM symbol
 _NDBPS_11N = {8: 52, 9: 104, 10: 156}                   # 802.11n data bits per OFDM symbol over both streams, MCS 8 .. 10
@@ -489,6 +510,44 @@ class Engine:
         so = (n_out + 3) // 4 * 4; y = np.zeros((nl, R, so, 2), np.int16)
         self.channel_sim_raw(_ptr(xs), T * si, si, T, n_in, lk, t, L, nl, seed, _ptr(y), R * so, so, R, n_out)
         return y[:, :, :n_out]
+
+    def spectrum_raw(self, in_ptr, row_stride, nrows, n_in, fft_len, hop, avg, window, out_ptr, stream=0):
+        """Pointer-level sb200_spectrum: in_ptr / out_ptr host or device addresses, row r at in_ptr + 4 r row_stride bytes; window None or
+        int16 Q15 [fft_len] (host); out int64 [nrows, ngroups, fft_len]."""
+        w = None if window is None else np.ascontiguousarray(window, dtype=np.int16)
+        self._check(self._lib.sb200_spectrum(self._h, C.c_void_p(in_ptr), C.c_uint64(row_stride), C.c_uint32(nrows), C.c_uint64(n_in), C.c_uint32(fft_len),
+                                             C.c_uint64(hop), C.c_uint32(avg), C.c_void_p(_ptr(w)), C.c_void_p(out_ptr), C.c_void_p(stream)), "sb200_spectrum")
+
+    def spectrum(self, iq_rows, fft_len, hop=None, avg=1, window=None):
+        """Spectrum meter (TSpecMeter<N> of the reference spectrum analyser, generalised): int16 [n_in, 2] or [R, n_in, 2] -> int64
+        [R, ngroups, N].  Frames of N = fft_len samples every hop (default N) samples, windowed by `window` (None, int16 Q15 [N], or a
+        spectrum_window kind such as "hann"), through FFT<N>; |X[k]|^2 per bin in natural FFT order (bin k at k fs / N, see fftshift_bins),
+        bin 0 cleared, summed over groups of avg frames; ngroups = spectrum_frames(n_in, N, hop) // avg."""
+        x = np.asarray(iq_rows, dtype=np.int16)
+        if x.ndim == 2: x = x[None]
+        if x.ndim != 3 or x.shape[2] != 2: raise ValueError("iq_rows must be int16 [n_in, 2] or [R, n_in, 2]")
+        R, n_in = x.shape[:2]; xs, stride = _rows4(R, n_in, x)
+        hop = fft_len if hop is None else hop
+        if isinstance(window, str): window = spectrum_window(fft_len, window)
+        out = np.zeros((R, spectrum_frames(n_in, fft_len, hop) // avg, fft_len), np.int64)
+        self.spectrum_raw(_ptr(xs), stride, R, n_in, fft_len, hop, avg, window, _ptr(out))
+        return out
+
+    def power_meter_raw(self, in_ptr, row_stride, nrows, n_in, block_len, out_ptr, stream=0):
+        """Pointer-level sb200_power_meter: in_ptr / out_ptr host or device addresses; out uint32 [nrows, n_in // block_len]."""
+        self._check(self._lib.sb200_power_meter(self._h, C.c_void_p(in_ptr), C.c_uint64(row_stride), C.c_uint32(nrows), C.c_uint64(n_in),
+                                                C.c_uint32(block_len), C.c_void_p(out_ptr), C.c_void_p(stream)), "sb200_power_meter")
+
+    def power_meter(self, iq_rows, block_len):
+        """Power meter (TPowerMeter<N> of the reference spectrum analyser): int16 [n_in, 2] or [R, n_in, 2] -> uint32 [R, n_in // N], the
+        mean |x|^2 of each block of N = block_len samples with the reference's per-vector division order (include/sora_b200.h)."""
+        x = np.asarray(iq_rows, dtype=np.int16)
+        if x.ndim == 2: x = x[None]
+        if x.ndim != 3 or x.shape[2] != 2: raise ValueError("iq_rows must be int16 [n_in, 2] or [R, n_in, 2]")
+        R, n_in = x.shape[:2]; xs, stride = _rows4(R, n_in, x)
+        out = np.zeros((R, n_in // block_len), np.uint32)
+        self.power_meter_raw(_ptr(xs), stride, R, n_in, block_len, _ptr(out))
+        return out
 
     def tx11b_fir37_raw(self, in_ptr, total, off_ptr, len_ptr, nframes, variant, out_ptr, stream=0):
         self._check(self._lib.sb200_tx11b_fir37(self._h, C.c_void_p(in_ptr), C.c_uint64(total), C.c_void_p(off_ptr), C.c_void_p(len_ptr), C.c_uint32(nframes),

@@ -159,6 +159,8 @@ struct sb200_handle {
     uint32_t sim_smem_set = 0;                         // bit J: k_channel_sim<J> may use its largest dynamic shared memory on this device
     DevBuf arbtab;                                     // sb200_channelize_arbitrary and sb200_combine_arbitrary: the NCO table and the call's H, staged per call (arb_kernels.cuh)
     uint32_t arb_smem_set = 0;                         // bit 0: k_channelize_arbitrary may use SB_ARB_SMEM_MAX bytes of dynamic shared memory on this device; bit J: k_combine_arbitrary<J> its budget
+    DevBuf sptab, spwin;                               // sb200_spectrum: the twiddles of every stage size (built on first use) and the call's window
+    uint32_t sp_smem_set = 0;                          // bit log2 N: k_spectrum<N> may use its dynamic shared memory on this device
     DevBuf vring;
     std::string err;
     int fail(int code, const char* what, cudaError_t e = cudaSuccess) {
